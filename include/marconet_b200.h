@@ -323,6 +323,34 @@ int mn_preprocess_lq_u8(const uint8_t* img, int h, int w, int cn, double fx, dou
 int mn_postprocess_sr_u8(const float* sr, long long stride_n, long long stride_c, long long stride_h, long long stride_w,
                          uint8_t* out, int B, int C, int H, int W, void* stream);
 
+/* Text lines wider than the canvas (and batches of lines of any width): test_sr.py:98-111 applied to many crops in one launch.
+ * Each crop is an image of its own: `img` points at row 0, first column of the crop inside a larger uint8 [.][.][cn] image whose
+ * rows are `row_pitch` bytes apart; the crop is h x w pixels and the cubic taps replicate ITS border, never reading outside it
+ * (= cv2.resize(img[:, a:b], (0,0), fx, fy, INTER_CUBIC), what a user who crops by hand gets).  dh = round_half_even(h*fy),
+ * dw = round_half_even(w*fx) <= out_w.  crops: DEVICE array of n records (the caller validates them before copying them over).
+ * lq: [n][cn][out_h][out_w] fp32, crop i bit-identical to mn_preprocess_lq_u8 on a contiguous copy of crop i. */
+typedef struct {
+    const uint8_t* img;
+    int64_t row_pitch;          /* bytes between rows of the source image */
+    int h, w, cn;
+    double fx, fy;
+    int dh, dw;
+} mn_lq_crop;
+int mn_preprocess_lq_u8_batched(const mn_lq_crop* crops, int n, int cn, float* lq, int out_h, int out_w, void* stream);
+
+/* test_sr.py:198-201 (the bytes of mn_postprocess_sr_u8, channel flip included) for column ranges of several SR lines, written
+ * into several destination images in one launch -- the stitch of a line restored crop by crop:
+ *   dst[y*dst_pitch + x*C + (C-1-c)] = u8(sr[line, c, y, src_x0 + x]),   y < H, x < width, src_x0 + width <= W.
+ * sr is addressed through element strides (the channels_last view TSPSRNet returns is read in place).  pieces: DEVICE array of
+ * n_pieces records (validated by the caller); max_width >= every piece's width. */
+typedef struct {
+    int32_t line, src_x0, width;
+    uint8_t* dst;               /* row 0, first column of the piece inside its image */
+    int64_t dst_pitch;          /* bytes between rows of the destination image */
+} mn_sr_piece;
+int mn_postprocess_sr_u8_pieces(const float* sr, long long stride_n, long long stride_c, long long stride_h, long long stride_w,
+                                int C, int H, int W, const mn_sr_piece* pieces, int n_pieces, int max_width, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -46,6 +46,15 @@ class Window(Structure):
     _fields_ = [("line", c_int32), ("x1", c_int32), ("x2", c_int32), ("y1", c_int32)]
 
 
+class LqCrop(Structure):
+    _fields_ = [("img", c_void_p), ("row_pitch", c_int64), ("h", c_int), ("w", c_int), ("cn", c_int), ("fx", c_double), ("fy", c_double),
+                ("dh", c_int), ("dw", c_int)]
+
+
+class SrPiece(Structure):
+    _fields_ = [("line", c_int32), ("src_x0", c_int32), ("width", c_int32), ("dst", c_void_p), ("dst_pitch", c_int64)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -86,6 +95,9 @@ SYMBOLS = {
                                      c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_longlong, c_void_p]),
     "mn_preprocess_lq_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_double, c_double, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "mn_postprocess_sr_u8": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "mn_preprocess_lq_u8_batched": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "mn_postprocess_sr_u8_pieces": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_int, c_int, c_int, c_void_p, c_int, c_int,
+                                            c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

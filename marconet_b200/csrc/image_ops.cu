@@ -32,11 +32,12 @@ __device__ __forceinline__ CubicTaps cubic_taps(int d, double scale) {
     return r;
 }
 
-__global__ void preprocess_lq_kernel(const uint8_t* __restrict__ img, int h, int w, int cn, double scale_x, double scale_y,
-                                     int dh, int dw, float* __restrict__ lq, uint8_t* __restrict__ lq_u8, int out_h, int out_w) {
-    mn_pdl_prologue();
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= out_h * out_w * cn) return;
+// One canvas element (idx over [out_h][out_w][cn]) of test_sr.py:98-111 for an 8-bit image whose rows start `row_pitch` bytes
+// apart.  The cubic taps replicate the border of [0, h) x [0, w): a crop passed as (pointer to its first column, the source
+// image's pitch, its own width) is resized as an isolated image, exactly what cv2.resize(img[:, a:b], ...) computes.
+__device__ __forceinline__ void preprocess_lq_element(const uint8_t* __restrict__ img, long long row_pitch, int h, int w, int cn,
+                                                      double scale_x, double scale_y, int dh, int dw, int idx,
+                                                      float* __restrict__ lq, uint8_t* __restrict__ lq_u8, int out_h, int out_w) {
     const int c = idx % cn;
     const int dx = (idx / cn) % out_w;
     const int dy = idx / (cn * out_w);
@@ -51,7 +52,7 @@ __global__ void preprocess_lq_kernel(const uint8_t* __restrict__ img, int h, int
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const int xx = min(max(tx.ofs - 1 + j, 0), w - 1);
-                acc += (int)img[((size_t)yy * w + xx) * cn + c] * tx.t[j];
+                acc += (int)img[(size_t)yy * row_pitch + (size_t)xx * cn + c] * tx.t[j];
             }
             S[r] = acc;
         }
@@ -74,6 +75,32 @@ __global__ void preprocess_lq_kernel(const uint8_t* __restrict__ img, int h, int
     lq[((size_t)c * out_h + dy) * out_w + dx] = t;
 }
 
+__global__ void preprocess_lq_kernel(const uint8_t* __restrict__ img, int h, int w, int cn, double scale_x, double scale_y,
+                                     int dh, int dw, float* __restrict__ lq, uint8_t* __restrict__ lq_u8, int out_h, int out_w) {
+    mn_pdl_prologue();
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= out_h * out_w * cn) return;
+    preprocess_lq_element(img, (long long)w * cn, h, w, cn, scale_x, scale_y, dh, dw, idx, lq, lq_u8, out_h, out_w);
+}
+
+// blockIdx.y = crop; every crop fills its own [cn][out_h][out_w] canvas of lq.
+__global__ void preprocess_lq_crops_kernel(const mn_lq_crop* __restrict__ crops, int cn, float* __restrict__ lq, int out_h, int out_w) {
+    mn_pdl_prologue();
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= out_h * out_w * cn) return;
+    const mn_lq_crop k = crops[blockIdx.y];
+    preprocess_lq_element(k.img, k.row_pitch, k.h, k.w, cn, __ddiv_rn(1.0, k.fx), __ddiv_rn(1.0, k.fy), k.dh, k.dw, idx,
+                          lq + (size_t)blockIdx.y * cn * out_h * out_w, nullptr, out_h, out_w);
+}
+
+// test_sr.py:198-201 + cv2.imwrite's rounding for one value
+__device__ __forceinline__ uint8_t sr_to_u8(float x) {
+    float v = __fadd_rn(__fmul_rn(x, 0.5f), 0.5f);
+    v = fminf(fmaxf(v, 0.f), 1.f);
+    const int q = __float2int_rn(__fmul_rn(v, 255.f));
+    return (uint8_t)min(max(q, 0), 255);
+}
+
 __global__ void postprocess_sr_kernel(const float* __restrict__ sr, long long sn, long long sc, long long sh, long long sw,
                                       uint8_t* __restrict__ out, int B, int C, int H, int W) {
     mn_pdl_prologue();
@@ -82,12 +109,21 @@ __global__ void postprocess_sr_kernel(const float* __restrict__ sr, long long sn
     const int x = (int)(idx % W), y = (int)((idx / W) % H), b = (int)(idx / ((long long)W * H));
     const float* p = sr + b * sn + y * sh + x * sw;
     uint8_t* o = out + idx * C;
-    for (int c = 0; c < C; ++c) {
-        float v = __fadd_rn(__fmul_rn(p[c * sc], 0.5f), 0.5f);
-        v = fminf(fmaxf(v, 0.f), 1.f);
-        const int q = __float2int_rn(__fmul_rn(v, 255.f));
-        o[C - 1 - c] = (uint8_t)min(max(q, 0), 255);          // .flip(2): channel c lands in byte C-1-c
-    }
+    for (int c = 0; c < C; ++c) o[C - 1 - c] = sr_to_u8(p[c * sc]);          // .flip(2): channel c lands in byte C-1-c
+}
+
+// blockIdx.y = piece; threads cover [H][max_width] pixels, those at x >= the piece's width exit.
+__global__ void postprocess_sr_pieces_kernel(const float* __restrict__ sr, long long sn, long long sc, long long sh, long long sw,
+                                             int C, int H, const mn_sr_piece* __restrict__ pieces, int max_width) {
+    mn_pdl_prologue();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)H * max_width) return;
+    const mn_sr_piece pc = pieces[blockIdx.y];
+    const int x = (int)(idx % max_width), y = (int)(idx / max_width);
+    if (x >= pc.width) return;
+    const float* p = sr + pc.line * sn + y * sh + (long long)(pc.src_x0 + x) * sw;
+    uint8_t* o = pc.dst + y * pc.dst_pitch + (long long)x * C;
+    for (int c = 0; c < C; ++c) o[C - 1 - c] = sr_to_u8(p[c * sc]);
 }
 
 }  // namespace
@@ -111,6 +147,27 @@ extern "C" int mn_postprocess_sr_u8(const float* sr, long long stride_n, long lo
     const long long total = (long long)B * H * W;
     MN_CUDA_CHECK((mn_launch(postprocess_sr_kernel, dim3((unsigned)mn_cdiv64(total, 256)), dim3(256), 0, (cudaStream_t)stream, sr, stride_n, stride_c,
                              stride_h, stride_w, out, B, C, H, W)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_preprocess_lq_u8_batched(const mn_lq_crop* crops, int n, int cn, float* lq, int out_h, int out_w, void* stream) {
+    MN_REQUIRE(crops && lq && n > 0 && n <= 65535 && cn > 0 && cn <= 4 && out_h > 0 && out_w > 0, "mn_preprocess_lq_u8_batched: bad args");
+    MN_REQUIRE((long long)out_h * out_w * cn < (1ll << 31), "mn_preprocess_lq_u8_batched: canvas too large");
+    const int total = out_h * out_w * cn;
+    MN_CUDA_CHECK((mn_launch(preprocess_lq_crops_kernel, dim3(mn_cdiv(total, 128), n), dim3(128), 0, (cudaStream_t)stream, crops, cn,
+                             lq, out_h, out_w)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_postprocess_sr_u8_pieces(const float* sr, long long stride_n, long long stride_c, long long stride_h, long long stride_w,
+                                           int C, int H, int W, const mn_sr_piece* pieces, int n_pieces, int max_width, void* stream) {
+    MN_REQUIRE(sr && pieces && C > 0 && C <= 4 && H > 0 && W > 0 && n_pieces > 0 && n_pieces <= 65535 && max_width > 0 && max_width <= W,
+               "mn_postprocess_sr_u8_pieces: bad args");
+    const long long total = (long long)H * max_width;
+    MN_CUDA_CHECK((mn_launch(postprocess_sr_pieces_kernel, dim3((unsigned)mn_cdiv64(total, 256), n_pieces), dim3(256), 0, (cudaStream_t)stream,
+                             sr, stride_n, stride_c, stride_h, stride_w, C, H, pieces, max_width)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -852,3 +852,83 @@ def postprocess_sr(sr):
     _lib.check(_lib.load().mn_postprocess_sr_u8(_ptr(sr), sn, sc, sh, sw, _ptr(out), b, c, h, w, _stream()), "mn_postprocess_sr_u8")
     LAUNCHES += 1
     return out
+
+
+def _table(ctype, records, device):
+    """Host-built array of C records -> device byte tensor (the kernels read their descriptors from device memory)."""
+    import numpy as np
+    arr = (ctype * len(records))(*records)
+    return torch.from_numpy(np.frombuffer(bytes(arr), dtype=np.uint8).copy()).to(device)
+
+
+def preprocess_lq_crops(crops, out_h=32, out_w=512):
+    """test_sr.py:98-111 for many crops in one launch (mn_preprocess_lq_u8_batched).  crops: list of (img, x0, x1), img a uint8
+    [h, w, cn] CUDA tensor with dense pixels (stride(1) == cn, stride(2) == 1, any row stride) read in place, [x0, x1) the crop's
+    source columns.  Each crop is resized as an image of its own (its border is replicated): crop i of the result is
+    bit-identical to ``preprocess_lq(img[:, x0:x1].contiguous())``.  Returns (lq fp32 [n, cn, out_h, out_w], resized widths)."""
+    global LAUNCHES
+    if not crops:
+        raise ValueError("preprocess_lq_crops: no crops")
+    cn = None
+    recs, widths = [], []
+    for i, (img, x0, x1) in enumerate(crops):
+        if not isinstance(img, torch.Tensor) or not img.is_cuda:
+            raise RuntimeError("marconet_b200: img must be a CUDA tensor (there is no CPU path)")
+        if img.device.index != torch.cuda.current_device():
+            raise RuntimeError(f"preprocess_lq_crops: crop {i} lives on {img.device}, the current device is cuda:{torch.cuda.current_device()}")
+        if img.dtype != torch.uint8 or img.dim() != 3 or img.stride(2) != 1 or img.stride(1) != img.shape[2] or img.stride(0) < img.shape[1] * img.shape[2]:
+            raise RuntimeError(f"preprocess_lq_crops: crop {i}: expects a uint8 [h, w, c] image with dense pixels")
+        h, w, c = img.shape
+        if cn is None:
+            cn = c
+        if c != cn or not 1 <= c <= 4:
+            raise RuntimeError(f"preprocess_lq_crops: crop {i} has {c} channels, expected {cn} (1 to 4)")
+        x0, x1 = int(x0), int(x1)
+        if not 0 <= x0 < x1 <= w:
+            raise ValueError(f"preprocess_lq_crops: crop {i}: columns [{x0}, {x1}) are not a non-empty range of the {w}-wide image")
+        fx = fy = out_h / h
+        dh, dw = round_half_even(h * fy), round_half_even((x1 - x0) * fx)
+        if dw > out_w or dh > out_h or dw < 1 or dh < 1:
+            raise ValueError(f"crop {i}: LQ size {dh}x{dw} does not fit the {out_h}x{out_w} canvas: crop the line into shorter segments "
+                             f"(test_sr.py:107-109)")
+        recs.append(_lib.LqCrop(img.data_ptr() + x0 * cn, img.stride(0), h, x1 - x0, cn, fx, fy, dh, dw))
+        widths.append(dw)
+    dev = crops[0][0].device
+    table = _table(_lib.LqCrop, recs, dev)
+    lq = torch.empty((len(recs), cn, out_h, out_w), dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().mn_preprocess_lq_u8_batched(_ptr(table), len(recs), cn, _ptr(lq), out_h, out_w, _stream()),
+               "mn_preprocess_lq_u8_batched")
+    LAUNCHES += 1
+    return lq, widths
+
+
+def postprocess_sr_pieces(sr, pieces):
+    """test_sr.py:198-201 for column ranges of several SR lines into several images, one launch (mn_postprocess_sr_u8_pieces).
+    sr: fp32 [B, C, H, W] (any strides: the channels_last view TSPSRNet returns is read in place).  pieces: list of
+    (line, src_x0, dst), dst a uint8 CUDA view [H, width, C] with dense pixels (typically ``out[:, x0:x0 + width]`` of an image):
+    dst receives columns [src_x0, src_x0 + width) of line ``line`` as ``postprocess_sr`` bytes."""
+    global LAUNCHES
+    _require_cuda(sr, "sr")
+    if sr.dim() != 4:
+        raise RuntimeError("postprocess_sr_pieces: expects an fp32 [B, C, H, W] tensor")
+    if not pieces:
+        raise ValueError("postprocess_sr_pieces: no pieces")
+    b, c, h, w = sr.shape
+    recs, mx = [], 0
+    for i, (line, x0, dst) in enumerate(pieces):
+        line, x0 = int(line), int(x0)
+        if not isinstance(dst, torch.Tensor) or dst.device != sr.device or dst.dtype != torch.uint8 or dst.dim() != 3:
+            raise RuntimeError(f"postprocess_sr_pieces: piece {i}: dst must be a uint8 [H, width, C] tensor on {sr.device}")
+        if dst.shape[0] != h or dst.shape[2] != c or dst.stride(2) != 1 or dst.stride(1) != c or dst.shape[1] < 1:
+            raise RuntimeError(f"postprocess_sr_pieces: piece {i}: dst {tuple(dst.shape)} (strides {dst.stride()}) is not a dense "
+                               f"[{h}, width, {c}] view")
+        width = dst.shape[1]
+        if not (0 <= line < b and 0 <= x0 and x0 + width <= w):
+            raise ValueError(f"postprocess_sr_pieces: piece {i}: line {line}, columns [{x0}, {x0 + width}) outside the [{b}, {w}] SR output")
+        recs.append(_lib.SrPiece(line, x0, width, dst.data_ptr(), dst.stride(0)))
+        mx = max(mx, width)
+    table = _table(_lib.SrPiece, recs, sr.device)
+    sn, sc, sh, sw = sr.stride()
+    _lib.check(_lib.load().mn_postprocess_sr_u8_pieces(_ptr(sr), sn, sc, sh, sw, c, h, w, _ptr(table), len(recs), mx, _stream()),
+               "mn_postprocess_sr_u8_pieces")
+    LAUNCHES += 1

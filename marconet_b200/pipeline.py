@@ -6,6 +6,9 @@ boxes converted from the encoder's (left, right) pairs to (centre, half-width) e
 (Train/tspgan/models/tspgan_model.py:331-337).  Integer outputs (labels) are computed on the host, bit-exactly like the
 reference; everything numeric runs through the module API (and therefore through the CUDA kernels).
 """
+import threading
+from typing import NamedTuple
+
 import torch
 
 ALPHABET_SIZE = 6735          # classes [0, 6735) are characters, 6735 is the CTC blank (utils/alphabets.py, test_w.py:38)
@@ -119,6 +122,274 @@ def restore_image(encoder, tspgan, sr, img_u8, labels, boxes):
     show_w = ops.round_half_even(img.shape[1] * (128 / h))    # ShowLQ = cv2.resize(img, fx=128/h, ...) (test_sr.py:98)
     sr_u8 = ops.postprocess_sr(out)[0, :, :show_w]            # ShowSR = sr[:, :ShowLQ.shape[1]] (test_sr.py:201)
     return dict(sr_u8=sr_u8, sr=out, lq=lq, lq_width=lq_w, prior=img_prior, locs=locs)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Lines of any width, many images per call.  test_sr.py restores one image per call and skips lines wider than the 32x512 LQ
+# canvas (:107-110, "crop it into shorter segments").  Here every image is cut between characters into crops that fit the canvas,
+# every crop of every image becomes one line of a batch, and each crop's core columns are written back into its image.  Each crop
+# is exactly what the script computes on a hand-made crop (the resize sees the crop alone; its characters, boxes shifted).
+# ---------------------------------------------------------------------------------------------------------------------
+class Segment(NamedTuple):
+    """One crop of a text-line image, in integer source columns: ``core`` [c_k, c_k+1) is the part of the line it restores,
+    ``crop`` [a_k, b_k) what it reads (the core plus context on both sides), ``chars`` [i0, i1) the characters it owns and
+    ``boxes`` their detector boxes shifted by -a_k."""
+    core: tuple
+    crop: tuple
+    chars: tuple
+    boxes: list
+
+
+def plan_segments(h, w, boxes, canvas=512, context=16, labels=None, name="image"):
+    """Cut an h x w text-line image with detector boxes [x1, y1, x2, y2] (source pixels, reading order) into Segments whose
+    crops fit the 32 x ``canvas`` LQ canvas.
+
+    An image that fits (round_half_even(w*32/h) <= canvas) is one segment: crop = core = the whole image.  Otherwise cuts
+    0 = c_0 < ... < c_S = w never fall strictly inside a character span [floor(x1), ceil(x2)) (overlapping spans stay together);
+    a crop is its core plus m = ceil(context*h/32) columns of context per side, clipped to the image, with (b-a)*32/h <= canvas-0.5.
+    Greedy: each segment takes as many characters as fit and cuts in the middle of the gap that follows them; where the middle
+    does not fit, or would leave the next character unable to fit its own segment, the cut moves to the nearest gap column that
+    does.  A gap wider than the canvas yields segments without characters.  Characters belong to the segment whose core holds
+    their span (zero-width boxes: their centre).
+    Raises ValueError naming ``name`` and the character: a label count that differs from the box count, a box outside the image,
+    box centres that decrease, a character (or run of overlapping characters) wider than the canvas with its context."""
+    import math
+    from .ops import round_half_even
+    h, w, n = int(h), int(w), len(boxes)
+    if h < 1 or w < 1:
+        raise ValueError(f"{name}: empty image ({h}x{w})")
+    if labels is not None and len(labels) != n:
+        raise ValueError(f"{name}: {len(labels)} labels for {n} boxes")
+    spans, centres = [], []
+    for i, box in enumerate(boxes):
+        x1, _, x2, _ = [float(v) for v in box]
+        if not 0 <= x1 <= x2 <= w:
+            raise ValueError(f"{name}, character {i}: box {[float(v) for v in box]} is outside the image (columns [0, {w}])")
+        c = (x1 + x2) / 2.0
+        if centres and c < centres[-1]:
+            raise ValueError(f"{name}, character {i}: box centre {c} lies left of character {i - 1}'s ({centres[-1]}); "
+                             f"boxes must be in reading order")
+        spans.append((math.floor(x1), math.ceil(x2)))
+        centres.append(c)
+    if round_half_even(w * (32 / h)) <= canvas:
+        return [Segment((0, w), (0, w), (0, n), [list(b) for b in boxes])]
+    m = -(-context * h // 32)
+    maxw = (2 * canvas - 1) * h // 64                    # widest crop: cols * 32 / h <= canvas - 0.5
+    if maxw <= 2 * m:
+        raise ValueError(f"{name}: {context} pixels of context leave no room in a {canvas}-pixel canvas")
+
+    def crop_cols(lo, hi):                               # width of the crop around core [lo, hi)
+        return min(w, hi + m) - max(0, lo - m)
+
+    clusters = []                                        # [start, end, first char, last char] of runs of overlapping spans
+    for i in sorted(range(n), key=lambda i: spans[i]):
+        s, e = spans[i]
+        if e <= s:
+            continue
+        if clusters and s < clusters[-1][1]:
+            cl = clusters[-1]
+            cl[1], cl[2], cl[3] = max(cl[1], e), min(cl[2], i), max(cl[3], i)
+        else:
+            clusters.append([s, e, i, i])
+    for s, e, i0, i1 in clusters:
+        if crop_cols(s, e) > maxw:
+            who = f"character {i0}" if i0 == i1 else f"characters {i0} to {i1} (overlapping boxes)"
+            raise ValueError(f"{name}, {who}: columns [{s}, {e}) with {m} columns of context per side are wider than the "
+                             f"{canvas}-pixel LQ canvas at height {h}; a single character cannot be split")
+    # gaps between clusters: closed ranges of columns where a cut may fall, and the cluster that follows each
+    gaps = []
+    lo = 0
+    for s, e, _, _ in clusters:
+        gaps.append((lo, s, e))
+        lo = e
+    gaps.append((lo, w, None))
+    cuts = [0]
+    while cuts[-1] < w:
+        c = cuts[-1]
+        a = max(0, c - m)
+        if w - a <= maxw:
+            cuts.append(w)
+            break
+        cmax = a + maxw - m                              # furthest cut whose crop fits
+        L, R, nxt_end = [g for g in gaps if g[0] <= cmax and g[1] > c][-1]
+        need = L
+        if nxt_end is not None:                          # the segment that starts at the cut must reach the next cluster's end
+            need = max(L, min(w, nxt_end + m) - maxw + m)
+        cuts.append(min(max((L + R) // 2, need, L, c + 1), R, cmax))
+    import bisect
+    owner = [min(len(cuts) - 2, bisect.bisect_right(cuts, ctr) - 1) for ctr in centres]
+    segs = []
+    for k in range(len(cuts) - 1):
+        i0 = bisect.bisect_left(owner, k)
+        i1 = bisect.bisect_right(owner, k)
+        a, b = max(0, cuts[k] - m), min(w, cuts[k + 1] + m)
+        segs.append(Segment((cuts[k], cuts[k + 1]), (a, b), (i0, i1), [[bx[0] - a, bx[1], bx[2] - a, bx[3]] for bx in boxes[i0:i1]]))
+    return segs
+
+
+def stitch_pieces(h, w, segments, sr_width=2048):
+    """Where each segment's SR columns land: (output width, [(segment index, out_x0, src_x0, width)]).  Output column x of an
+    h x w image lies at source column x*h/128 (ShowLQ's scale, test_sr.py:99): segment k fills [r(c_k), r(c_k+1)) from its own SR
+    output shifted left by r(a_k), r(x) = round_half_even(x*128/h).  A single-segment image is restore_image's
+    ``sr[:, :round_half_even(w*128/h)]``, clamped to the SR width as that slice is."""
+    from .ops import round_half_even
+
+    def r(x):
+        return round_half_even(x * (128 / h))
+    if len(segments) == 1:
+        width = min(r(w), sr_width)
+        return width, [(0, 0, 0, width)]
+    out = []
+    for k, s in enumerate(segments):
+        o0, o1 = r(s.core[0]), r(s.core[1])
+        if o1 > o0:
+            out.append((k, o0, o0 - r(s.crop[0]), o1 - o0))
+    return r(w), out
+
+
+_TLS = threading.local()
+
+
+def _staging(nbytes, device):
+    """Per-thread, per-device pinned host buffer for the host->device copy of a batch's images, reused once its last copy (the
+    event, recorded after it) has finished."""
+    stages = _TLS.__dict__.setdefault("stages", {})
+    st = stages.get(device.index)
+    if st is None or st[0].numel() < nbytes:
+        st = (torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8, pin_memory=True), torch.cuda.Event())
+        stages[device.index] = st
+    else:
+        st[1].synchronize()
+    return st
+
+
+def _as_image(img, i):
+    if not isinstance(img, torch.Tensor):
+        import numpy as np
+        img = torch.from_numpy(np.ascontiguousarray(img))
+    if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3 or img.shape[0] < 1 or img.shape[1] < 1:
+        raise ValueError(f"image {i}: expected a uint8 [h, w, 3] image, got {img.dtype} {tuple(img.shape)}")
+    return img
+
+
+@torch.no_grad()
+def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, context=16, skip_invalid=False, to_host=False):
+    """Text-line images of any sizes end to end, batched: the flow of restore_image for every image, each cut into crops that
+    fit the 32x512 LQ canvas (plan_segments) and every crop of every image run as one line of a batch of at most ``max_lines``.
+
+    images: uint8 [h_i, w_i, 3] numpy arrays or CPU / CUDA tensors; labels / boxes: one list per image, as restore_image takes.
+    Every image is planned and validated before any launch (a label outside the generator's classes raises IndexError, as the
+    module would); with ``skip_invalid`` a bad image's entry becomes dict(error=...) and the others still run.  Per batch: one
+    host->device copy of the batch's host images through pinned memory, one crop kernel (mn_preprocess_lq_u8_batched), the
+    encoder, one TSPGAN call for all characters (each crop's characters take that crop's style w, as on a hand-made crop),
+    TSPSRNet, a synchronisation and ops.poll_range (the batch re-runs, at most 3 times, when a layer was re-routed for fp16
+    range), then one stitch kernel (mn_postprocess_sr_u8_pieces) into the images' outputs.
+    Returns one dict per image: sr_u8 (uint8 [128, W_i, 3], W_i = round_half_even(w_i*128/h_i), on the device, or numpy through
+    one pinned device->host copy with ``to_host``) and segments (the plan).  A single-segment image gives restore_image's bytes."""
+    from . import ops
+    n = len(images)
+    if not (len(labels) == len(boxes) == n):
+        raise ValueError(f"{n} images, {len(labels)} label lists, {len(boxes)} box lists")
+    if max_lines < 1:
+        raise ValueError("max_lines must be >= 1")
+    dev = next(encoder.parameters()).device
+    n_cls = tspgan.TextGenerator.input_text.TextEmbeddings.shape[0]
+    results, imgs, labs, plans = [None] * n, [None] * n, [None] * n, [None] * n
+    for i in range(n):
+        try:
+            img = _as_image(images[i], i)
+            lab = [int(v) for v in torch.as_tensor(labels[i], dtype=torch.long).reshape(-1).tolist()]
+            if not lab:
+                raise ValueError(f"image {i}: no character labels (test_sr.py:168-170 skips such images)")
+            segs = plan_segments(img.shape[0], img.shape[1], boxes[i], labels=lab, context=context, name=f"image {i}")
+            bad = [j for j, v in enumerate(lab) if not 0 <= v < n_cls]
+            if bad:
+                raise IndexError(f"image {i}, character {bad[0]}: label {lab[bad[0]]} outside [0, {n_cls}) "
+                                 f"(reference: empty embedding slice, networks.py:211)")
+        except (ValueError, IndexError) as e:
+            if not skip_invalid:
+                raise
+            results[i] = dict(error=f"{type(e).__name__}: {e}")
+            continue
+        imgs[i], labs[i], plans[i] = img, lab, segs
+    valid = [i for i in range(n) if plans[i] is not None]
+    if not valid:
+        return results
+    with torch.cuda.device(dev):
+        layout, total = {}, 0
+        for i in valid:
+            width, pieces = stitch_pieces(imgs[i].shape[0], imgs[i].shape[1], plans[i])
+            layout[i] = (total, width, pieces)
+            total += 128 * width * 3
+        flat = torch.empty(total, dtype=torch.uint8, device=dev)
+        outs = {i: flat[o:o + 128 * wd * 3].view(128, wd, 3) for i, (o, wd, _) in layout.items()}
+        lines = [(i, k) for i in valid for k in range(len(plans[i]))]
+        for b0 in range(0, len(lines), max_lines):
+            batch = lines[b0:b0 + max_lines]
+            dimg = {}
+            host = []
+            for i in dict.fromkeys(i for i, _ in batch):
+                t = imgs[i]
+                if not t.is_cuda:
+                    host.append(i)
+                    continue
+                t = t.to(dev)
+                if t.stride(2) != 1 or t.stride(1) != 3:
+                    t = t.contiguous()
+                dimg[i] = t
+            if host:
+                nbytes = sum(imgs[i].numel() for i in host)
+                stage, ev = _staging(nbytes, dev)
+                o = 0
+                for i in host:
+                    stage[o:o + imgs[i].numel()].view(imgs[i].shape).copy_(imgs[i])
+                    o += imgs[i].numel()
+                dbuf = stage[:nbytes].to(dev, non_blocking=True)
+                ev.record()
+                o = 0
+                for i in host:
+                    dimg[i] = dbuf[o:o + imgs[i].numel()].view(imgs[i].shape)
+                    o += imgs[i].numel()
+            segs = [plans[i][k] for i, k in batch]
+            lq, _ = ops.preprocess_lq_crops([(dimg[i], s.crop[0], s.crop[1]) for (i, _), s in zip(batch, segs)])
+            counts = [s.chars[1] - s.chars[0] for s in segs]
+            lab_all = torch.tensor([v for (i, _), s in zip(batch, segs) for v in labs[i][s.chars[0]:s.chars[1]]],
+                                   dtype=torch.long).reshape(-1, 1)
+            locs = torch.zeros(len(batch), 2 * max(1, max(counts)), dtype=torch.float32)
+            for b, ((i, _), s) in enumerate(zip(batch, segs)):
+                if counts[b]:
+                    locs[b, :2 * counts[b]] = boxes_to_locs(s.boxes, imgs[i].shape[0], lq.shape[-1])[0]
+            for attempt in range(4):
+                _, _, w = encoder(lq)
+                p64, p32 = [], []
+                if lab_all.shape[0] > 0:
+                    styles = torch.cat([w[b:b + 1].expand(c, -1) for b, c in enumerate(counts) if c > 0], dim=0)
+                    _, f64, f32_ = tspgan(styles=styles, labels=lab_all, noise=None)
+                    o = 0
+                    for c in counts:
+                        p64.append(f64[o:o + c]); p32.append(f32_[o:o + c]); o += c
+                else:
+                    p64 = [torch.zeros(0, 256, 64, 64, device=dev) for _ in counts]
+                    p32 = [torch.zeros(0, 512, 32, 32, device=dev) for _ in counts]
+                out = sr(lq, p64, p32, locs)
+                torch.cuda.synchronize(dev)
+                if not ops.poll_range(dev) or attempt == 3:
+                    break
+            pieces = []
+            for b, (i, k) in enumerate(batch):
+                for kk, x0, src, wd in layout[i][2]:
+                    if kk == k:
+                        pieces.append((b, src, outs[i][:, x0:x0 + wd]))
+            if pieces:
+                ops.postprocess_sr_pieces(out, pieces)
+        if to_host:
+            pinned = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+            pinned.copy_(flat, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+            outs = {i: pinned[o:o + 128 * wd * 3].view(128, wd, 3).numpy() for i, (o, wd, _) in layout.items()}
+    for i in valid:
+        results[i] = dict(sr_u8=outs[i], segments=plans[i])
+    return results
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -1,0 +1,107 @@
+"""Text-line images of mixed widths end to end (host uint8 in, host uint8 out, every copy inside the timed region):
+pipeline.restore_images at max_lines 1, 4 and 8, against the loop a user writes today -- restore_image on each crop of the same
+plan, then a device->host copy of its bytes.
+
+    python tools/bench_images.py [--images 42] [--passes 3] [--warmup 1]
+
+The image set reuses the 17 (h, w) sizes of the reference's Testsets/LQs (resized LQ widths 92 to 464 pixels, all inside the
+512-pixel canvas) and adds lines 2 to 4 times wider than the canvas, which test_sr.py refuses (:107-110), with one character box
+per 28 LQ pixels.  Host clock around whole passes over the set (each ends synchronised).  Prints one JSON line with the card's
+name and power limit read in the same run.  Not part of the product path.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+TESTSET_SIZES = [(22, 181), (12, 108), (17, 49), (20, 112), (17, 86), (15, 61), (14, 47), (12, 52), (49, 304), (14, 45), (14, 44),
+                 (15, 55), (32, 388), (128, 1472), (128, 1268), (128, 1160), (128, 1856)]
+WIDE_LINES = [(32, 1100), (40, 1536), (24, 2040), (64, 1300)]        # (h, LQ width)
+
+
+def make_image_set(n, seed=0):
+    """n seeded uint8 line images cycling through TESTSET_SIZES and WIDE_LINES, one character box per 28 LQ pixels."""
+    rng = np.random.default_rng(seed)
+    sizes = TESTSET_SIZES + [(h, round(lq_w * h / 32)) for h, lq_w in WIDE_LINES]
+    images, labels, boxes = [], [], []
+    for i in range(n):
+        h, w = sizes[i % len(sizes)]
+        pitch = 28 * h / 32
+        k = max(1, int(w // pitch))
+        images.append(rng.integers(0, 256, (h, w, 3), dtype=np.uint8))
+        boxes.append([[int(j * pitch + 0.15 * pitch), 0, int(j * pitch + 0.85 * pitch), h] for j in range(k)])
+        labels.append(rng.integers(0, 6735, k).tolist())
+    return images, labels, boxes
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--images", type=int, default=42)
+    ap.add_argument("--passes", type=int, default=3, help="timed passes over the image set per arm")
+    ap.add_argument("--warmup", type=int, default=1, help="untimed passes per arm first")
+    args = ap.parse_args()
+    from marconet_b200 import pipeline
+    from marconet_b200.models import networks
+    from marconet_b200.testing import synth
+
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_images.py: no CUDA device (the product path has no CPU fallback)")
+    dev = torch.device("cuda:0")
+    sds = synth.make_checkpoints(0)
+    nets = {}
+    for key, cls in (("tspgan", networks.TSPGAN), ("encoder", networks.TextContextEncoderV2), ("sr", networks.TSPSRNet)):
+        m = cls()
+        m.load_state_dict(sds[key], strict=True)
+        nets[key] = m.eval().to(dev)
+    enc, gen, sr = nets["encoder"], nets["tspgan"], nets["sr"]
+
+    images, labels, boxes = make_image_set(args.images)
+    plans = [pipeline.plan_segments(im.shape[0], im.shape[1], b) for im, b in zip(images, boxes)]
+    crops = [(np.ascontiguousarray(im[:, s.crop[0]:s.crop[1]]), lab[s.chars[0]:s.chars[1]], s.boxes)
+             for im, lab, p in zip(images, labels, plans) for s in p if s.chars[1] > s.chars[0]]
+    n_chars = sum(len(l) for l in labels)
+
+    def loop():
+        for c, lab, bx in crops:
+            pipeline.restore_image(enc, gen, sr, c, lab, bx)["sr_u8"].cpu()
+
+    arms = {f"restore_images_max_lines_{m}": (lambda m=m: pipeline.restore_images(enc, gen, sr, images, labels, boxes, max_lines=m,
+                                                                                  to_host=True)) for m in (1, 4, 8)}
+    arms["restore_image_loop_over_crops"] = loop
+    out = {}
+    with torch.no_grad():
+        for fn in arms.values():
+            for _ in range(max(1, args.warmup)):
+                fn()
+        for name, fn in arms.items():
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            for _ in range(args.passes):
+                fn()
+            torch.cuda.synchronize()
+            s = (time.perf_counter() - t0) / args.passes
+            out[name] = {"s_per_pass": s, "images_per_sec": len(images) / s, "chars_per_sec": n_chars / s}
+    card = {"name": torch.cuda.get_device_name(dev)}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=10).stdout.strip()
+        card["power_limit"] = q or None
+    except Exception as exc:
+        card["power_limit"] = f"unavailable ({type(exc).__name__})"
+    print(json.dumps({"metric": "images_e2e", "images": len(images), "lines": sum(len(p) for p in plans), "crops_with_chars": len(crops),
+                      "chars": n_chars, "wide_images": sum(len(p) > 1 for p in plans), "passes": args.passes,
+                      "warmup_passes": max(1, args.warmup), "arms": out, "gpu": card,
+                      "workload": f"{len(images)} seeded uint8 line images cycling through the 17 sizes of the reference's Testsets/LQs "
+                                  f"and {len(WIDE_LINES)} lines 2-4x wider than the canvas, one character per 28 LQ pixels; "
+                                  f"host numpy in, host numpy out"}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
