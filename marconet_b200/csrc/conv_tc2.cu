@@ -1,11 +1,13 @@
 // conv_tc2.cu -- wgmma operand-split implicit-GEMM convolution for sm_90a, the tensor-core path of mn_conv2d_nhwc.
 // x*w ~= xh*wh + (xh*wl + xl*wh) with 16-bit halves (three MMAs, cross terms in their own fp32 accumulator: the tensor core
-// truncates when it adds into fp32, see the epilogue's dfix).  One work item = 128 pixels x 64 channels (x one k-slice).
+// truncates when it adds into fp32, see the epilogue's dfix).  One work item = 128 pixels x NT channels (x one k-slice), NT = 64
+// or 128 chosen per layer by the plan.
 // HALO: one TMA box per 64-channel block brings the zero-padded (TH+2) x (TW+2) halo; the taps are shifted reads of it (shapes
-// whose halo does not fit take one shifted 128-pixel box per tap: mn_conv_tc_*).  SPLIT: four warps turn it into hi / lo planes in
-// place (fused GroupNorm(+swish) here).  MMA: two consumer warpgroups ldmatrix the shifted rows into the register A fragments of
-// wgmma.m64n64k16, B = the 128B-swizzled weight tile, TMA-multicast to a 2-CTA cluster.  Persistent CTAs; epilogue staged
-// through shared memory.  Warps: 0..3 split, 4..7 / 8..11 consumers (rows 0-63 / 64-127), 12 weight producer, 13 A producer.
+// whose halo does not fit take one shifted 128-pixel box per tap: mn_conv_tc_*).  SPLIT: a warpgroup turns it into hi / lo planes
+// in place (fused GroupNorm(+swish) here).  MMA: two consumer warpgroups ldmatrix the shifted rows into the register A fragments
+// of wgmma.m64n{NT}k16, B = the 128B-swizzled weight tile, TMA-multicast to a 2-CTA cluster; a weight / A stage is released once
+// per warpgroup.  Persistent CTAs; epilogue staged through shared memory in 64-column halves.  Warpgroups (setmaxnreg moves registers to the consumers): 0 split, 1 producers (warp 4 weights,
+// warp 5 A tiles), 2 / 3 consumers (rows 0-63 / 64-127).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -18,13 +20,15 @@ namespace {
 using namespace tcptx;
 
 constexpr int KB = 64;                          // channels per k-block
-constexpr int NT = 64;                          // output channels per work item
-constexpr int NUM_THREADS2 = 448;               // 14 warps: see the role list in the header comment
+constexpr int NUM_THREADS2 = 512;               // 4 warpgroups: see the role list in the header comment
+// registers per thread of each role after setmaxnreg (4 x 128 threads x 128 at launch = 128 x (SPLIT + PROD + 2 CONS))
+constexpr int REG_SPLIT = 88, REG_PROD = 24, REG_CONS = 200;
+static_assert(REG_SPLIT + REG_PROD + 2 * REG_CONS <= 4 * 128, "register budget");
 constexpr int MAX_HS = 3;
 constexpr int MAX_BSTAGES = 4;
-constexpr int B_HALF = NT * 128;                // one (hi or lo) weight tile: 64 channels x 64 k x 2 B
-constexpr int B_STAGE = 2 * B_HALF;
-constexpr int STG_PITCH = 72;                   // floats per staged row: conflict-free float2 stores of the accumulator layout
+__host__ __device__ constexpr int b_half(int nt) { return nt * 128; }   // one (hi or lo) weight tile: nt channels x 64 k x 2 B
+__host__ __device__ constexpr int b_stage(int nt) { return 2 * b_half(nt); }
+constexpr int STG_PITCH = 72;                   // floats per staged row (64 columns): conflict-free float2 stores of the accumulators
 constexpr int STG_BYTES = 128 * STG_PITCH * 4;
 constexpr int SMEM_LIMIT = 232448;              // 227 KB
 
@@ -38,15 +42,17 @@ struct Tc2Geom {
     int bstages, cs;
     int hstages;        // depth of the A-tile ring
     int per_tap;        // 0: one halo per channel block; 1: one shifted 128-pixel box per (channel block, tap)
+    int nt;             // output channels per work item: 64 or 128 (the kernel's NT)
     const float* wscale;
     int prec;
 };
 
 // MODE: 0 = f16x3, 1 = bf16x3, 2 = f16x1 (a template parameter: the wgmma operand registers must not depend on a runtime branch)
-template <bool GN, int MODE>
+template <bool GN, int MODE, int NT>
 __global__ void __launch_bounds__(NUM_THREADS2, 1)
 conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
                 const __grid_constant__ CUtensorMap tmBlo, const ConvGeom g, const Tc2Geom t) {
+    constexpr int B_HALF = b_half(NT), B_STAGE = b_stage(NT);
     extern __shared__ uint8_t smem_raw[];
     // keep the pointer in the shared address space (offset arithmetic on the array) so loads compile to LDS, not generic LD
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -66,7 +72,10 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     const int cs = t.cs;
     const uint32_t crank = cs > 1 ? cluster_ctarank() : 0u;
     const uint16_t cmask = (uint16_t)((1u << cs) - 1u);
-    const int cluster_id = blockIdx.x / cs, num_clusters = gridDim.x / cs;
+    const int num_clusters = gridDim.x / cs;
+    // first work item of this CTA's cluster; read inside each role, after its setmaxnreg, so that no register value has to live
+    // across the register reallocation (ptxas spills such values)
+    auto first_work = [&]() { return (int)(blockIdx.x / cs); };
     const int total_work = t.m_groups * t.n_tiles * t.ksplit;
     const int BS = t.bstages;
     const int units = t.per_tap ? t.cbps * t.taps : t.cbps;      // A tiles per work item
@@ -80,9 +89,9 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBhi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBlo) : "memory");
-        for (int s = 0; s < MAX_HS; ++s) { mbar_init(bar(I_HF + s), 1); mbar_init(bar(I_HE + s), 8); mbar_init(bar(I_SD + s), 128); }
-        // B stage s of every CTA of the cluster is written by every CTA's multicast: one arrival per consumer warp of each CTA
-        for (int s = 0; s < MAX_BSTAGES; ++s) { mbar_init(bar(I_BF + s), 1); mbar_init(bar(I_BE + s), 8 * cs); }
+        for (int s = 0; s < MAX_HS; ++s) { mbar_init(bar(I_HF + s), 1); mbar_init(bar(I_HE + s), 2); mbar_init(bar(I_SD + s), 128); }
+        // B stage s of every CTA of the cluster is written by every CTA's multicast: one arrival per consumer warpgroup of each CTA
+        for (int s = 0; s < MAX_BSTAGES; ++s) { mbar_init(bar(I_BF + s), 1); mbar_init(bar(I_BE + s), 2 * cs); }
         fence_barrier_init();
     }
     __syncthreads();
@@ -100,57 +109,61 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         n0 = m_tile * t.TN; oy0 = th_i * t.TH; ox0 = tw_i * t.TW;
     };
 
-    if (warp == 12) {
-        // =========================== weight (B) producer ===========================
-        uint32_t s = 0, ph = 0;
-        const int rows = NT / cs;
-        const uint32_t dst0 = smem_base + off_b + crank * rows * 128;
-        for (int work = cluster_id; work < total_work; work += num_clusters) {
-            const int row0 = work_nt(work) * NT + (int)crank * rows;
-            const int cb0 = work_ks(work) * t.cbps;
-            for (int cb = cb0; cb < cb0 + t.cbps; ++cb) {
-                for (int tap = 0; tap < t.taps; ++tap) {
-                    mbar_wait(bar(I_BE + s), ph ^ 1);
-                    if (elect_one_sync()) {
-                        const uint32_t dst = dst0 + s * B_STAGE;
-                        mbar_expect_tx(bar(I_BF + s), B_STAGE);
-                        if (cs > 1) {
-                            tma_load_3d_mc(&tmBhi, bar(I_BF + s), dst, cb * KB, row0, tap, cmask);
-                            tma_load_3d_mc(&tmBlo, bar(I_BF + s), dst + B_HALF, cb * KB, row0, tap, cmask);
-                        } else {
-                            tma_load_3d(&tmBhi, bar(I_BF + s), dst, cb * KB, row0, tap);
-                            tma_load_3d(&tmBlo, bar(I_BF + s), dst + B_HALF, cb * KB, row0, tap);
+    if (warp >= 4 && warp < 8) {
+        setmaxnreg_dec<REG_PROD>();
+        if (warp == 4) {
+            // =========================== weight (B) producer ===========================
+            uint32_t s = 0, ph = 0;
+            const int rows = NT / cs;
+            const uint32_t dst0 = smem_base + off_b + crank * rows * 128;
+            for (int work = first_work(); work < total_work; work += num_clusters) {
+                const int row0 = work_nt(work) * NT + (int)crank * rows;
+                const int cb0 = work_ks(work) * t.cbps;
+                for (int cb = cb0; cb < cb0 + t.cbps; ++cb) {
+                    for (int tap = 0; tap < t.taps; ++tap) {
+                        mbar_wait(bar(I_BE + s), ph ^ 1);
+                        if (elect_one_sync()) {
+                            const uint32_t dst = dst0 + s * B_STAGE;
+                            mbar_expect_tx(bar(I_BF + s), B_STAGE);
+                            if (cs > 1) {
+                                tma_load_3d_mc(&tmBhi, bar(I_BF + s), dst, cb * KB, row0, tap, cmask);
+                                tma_load_3d_mc(&tmBlo, bar(I_BF + s), dst + B_HALF, cb * KB, row0, tap, cmask);
+                            } else {
+                                tma_load_3d(&tmBhi, bar(I_BF + s), dst, cb * KB, row0, tap);
+                                tma_load_3d(&tmBlo, bar(I_BF + s), dst + B_HALF, cb * KB, row0, tap);
+                            }
                         }
+                        __syncwarp();
+                        if (++s == (uint32_t)BS) { s = 0; ph ^= 1; }
                     }
-                    __syncwarp();
-                    if (++s == (uint32_t)BS) { s = 0; ph ^= 1; }
                 }
             }
-        }
-    } else if (warp == 13) {
-        // =========================== A (halo or per-tap box) producer ===========================
-        uint32_t hs = 0, ph = 0;
-        for (int work = cluster_id; work < total_work; work += num_clusters) {
-            int n0, oy0, ox0;
-            tile_origin(work, n0, oy0, ox0);
-            const int cb0 = work_ks(work) * t.cbps;
-            for (int u = 0; u < units; ++u) {
-                const int cb = cb0 + (t.per_tap ? u / t.taps : u);
-                const int tap = t.per_tap ? u % t.taps : 0;
-                const int ky = tap / t.KW, kx = tap - ky * t.KW;
-                mbar_wait(bar(I_HE + hs), ph ^ 1);
-                if (elect_one_sync()) {
-                    mbar_expect_tx(bar(I_HF + hs), 2u * t.halo_rows * 128u);
-                    const uint32_t dst = smem_base + hs * t.halo_stage_bytes;
-                    tma_load_4d(&tmA, bar(I_HF + hs), dst, cb * KB, ox0 + kx - t.pw, oy0 + ky - t.ph, n0);
-                    tma_load_4d(&tmA, bar(I_HF + hs), dst + t.box_bytes, cb * KB + 32, ox0 + kx - t.pw, oy0 + ky - t.ph, n0);
+        } else if (warp == 5) {
+            // =========================== A (halo or per-tap box) producer ===========================
+            uint32_t hs = 0, ph = 0;
+            for (int work = first_work(); work < total_work; work += num_clusters) {
+                int n0, oy0, ox0;
+                tile_origin(work, n0, oy0, ox0);
+                const int cb0 = work_ks(work) * t.cbps;
+                for (int u = 0; u < units; ++u) {
+                    const int cb = cb0 + (t.per_tap ? u / t.taps : u);
+                    const int tap = t.per_tap ? u % t.taps : 0;
+                    const int ky = tap / t.KW, kx = tap - ky * t.KW;
+                    mbar_wait(bar(I_HE + hs), ph ^ 1);
+                    if (elect_one_sync()) {
+                        mbar_expect_tx(bar(I_HF + hs), 2u * t.halo_rows * 128u);
+                        const uint32_t dst = smem_base + hs * t.halo_stage_bytes;
+                        tma_load_4d(&tmA, bar(I_HF + hs), dst, cb * KB, ox0 + kx - t.pw, oy0 + ky - t.ph, n0);
+                        tma_load_4d(&tmA, bar(I_HF + hs), dst + t.box_bytes, cb * KB + 32, ox0 + kx - t.pw, oy0 + ky - t.ph, n0);
+                    }
+                    __syncwarp();
+                    if (++hs == (uint32_t)HS) { hs = 0; ph ^= 1; }
                 }
-                __syncwarp();
-                if (++hs == (uint32_t)HS) { hs = 0; ph ^= 1; }
             }
         }
     } else if (warp < 4) {
         // =========================== split warps: fp32 A tile -> (hi, lo) 16-bit planes, in place ===========================
+        setmaxnreg_dec<REG_SPLIT>();
         const int sidx = threadIdx.x;
         const bool bf = t.prec == MN_PREC_BF16X3_TC;
         const uint32_t mask = bf ? 0xFFFF0000u : 0xFFFFE000u;
@@ -160,7 +173,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         const int G = g.Cin >> 5;
         const int qs = sidx & 3, rs0 = sidx >> 2;            // 16-channel slice of the block, first halo row of this lane
         const int rows_up = (t.halo_rows + 31) & ~31;        // whole warps run every trip (__syncwarp inside)
-        for (int work = cluster_id; work < total_work; work += num_clusters) {
+        for (int work = first_work(); work < total_work; work += num_clusters) {
             int hn0 = 0, hoy0 = 0, hox0 = 0, gvw = 0x7fffffff;
             if (GN) {
                 tile_origin(work, hn0, hoy0, hox0);
@@ -196,38 +209,49 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 mbar_wait(bar(I_HF + hs), hph);
                 uint8_t* halo = smem + hs * t.halo_stage_bytes;
                 if constexpr (!GN) {
-                    // Plain split: one lane per halo row.
+                    // Plain split: one lane per halo row, stored as it converts.  row0 (channels 0-31) becomes the hi plane and row1
+                    // (channels 32-63) the lo plane, chunks 0-3 of each holding channels 0-31: once row0 is in registers its hi words
+                    // can overwrite it, but its lo words have to wait until row1 has been read.
+                    auto load8 = [&](const uint8_t* src, int sw, float4 (&v)[8]) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) v[j] = *reinterpret_cast<const float4*>(src + ((j ^ sw) << 4));
+                    };
+                    auto split16 = [&](float4 (&vv)[8], uint32_t (&hi)[16], uint32_t (&lo)[16]) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            float4 v = vv[j];
+                            v.x *= xs; v.y *= xs; v.z *= xs; v.w *= xs;
+                            amax = fmaxf(fmaxf(amax, fabsf(v.x)), fmaxf(fabsf(v.y), fmaxf(fabsf(v.z), fabsf(v.w))));
+                            const float h0 = __uint_as_float(__float_as_uint(v.x) & mask), h1 = __uint_as_float(__float_as_uint(v.y) & mask);
+                            const float h2 = __uint_as_float(__float_as_uint(v.z) & mask), h3 = __uint_as_float(__float_as_uint(v.w) & mask);
+                            if (bf) {
+                                hi[2 * j] = pack_bf16(h0, h1); hi[2 * j + 1] = pack_bf16(h2, h3);
+                                lo[2 * j] = pack_bf16(v.x - h0, v.y - h1); lo[2 * j + 1] = pack_bf16(v.z - h2, v.w - h3);
+                            } else {
+                                hi[2 * j] = pack_f16(h0, h1); hi[2 * j + 1] = pack_f16(h2, h3);
+                                lo[2 * j] = pack_f16(v.x - h0, v.y - h1); lo[2 * j + 1] = pack_f16(v.z - h2, v.w - h3);
+                            }
+                        }
+                    };
+                    auto store4 = [&](uint8_t* dst, int sw, int jj0, const uint32_t (&w)[16]) {
+#pragma unroll
+                        for (int jj = 0; jj < 4; ++jj)
+                            *reinterpret_cast<uint4*>(dst + (((jj0 + jj) ^ sw) << 4)) = make_uint4(w[4 * jj], w[4 * jj + 1], w[4 * jj + 2], w[4 * jj + 3]);
+                    };
                     for (int rho = sidx; rho < t.halo_rows; rho += 128) {
                         uint8_t* row0 = halo + rho * 128;
                         uint8_t* row1 = row0 + t.box_bytes;
                         const int sw = rho & 7;
-                        uint32_t hi[32], lo[32];
-#pragma unroll
-                        for (int box = 0; box < 2; ++box) {
-                            const uint8_t* bsrc = box ? row1 : row0;
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                float4 v = *reinterpret_cast<const float4*>(bsrc + ((j ^ sw) << 4));
-                                v.x *= xs; v.y *= xs; v.z *= xs; v.w *= xs;
-                                amax = fmaxf(fmaxf(amax, fabsf(v.x)), fmaxf(fabsf(v.y), fmaxf(fabsf(v.z), fabsf(v.w))));
-                                const float h0 = __uint_as_float(__float_as_uint(v.x) & mask), h1 = __uint_as_float(__float_as_uint(v.y) & mask);
-                                const float h2 = __uint_as_float(__float_as_uint(v.z) & mask), h3 = __uint_as_float(__float_as_uint(v.w) & mask);
-                                const int c = box * 16 + j * 2;
-                                if (bf) {
-                                    hi[c] = pack_bf16(h0, h1); hi[c + 1] = pack_bf16(h2, h3);
-                                    lo[c] = pack_bf16(v.x - h0, v.y - h1); lo[c + 1] = pack_bf16(v.z - h2, v.w - h3);
-                                } else {
-                                    hi[c] = pack_f16(h0, h1); hi[c + 1] = pack_f16(h2, h3);
-                                    lo[c] = pack_f16(v.x - h0, v.y - h1); lo[c + 1] = pack_f16(v.z - h2, v.w - h3);
-                                }
-                            }
-                        }
-                        // all 256 B of this row are in registers now: overwrite it (row0 <- hi plane, row1 <- lo plane)
-#pragma unroll
-                        for (int jj = 0; jj < 8; ++jj) {
-                            *reinterpret_cast<uint4*>(row0 + ((jj ^ sw) << 4)) = make_uint4(hi[4 * jj], hi[4 * jj + 1], hi[4 * jj + 2], hi[4 * jj + 3]);
-                            *reinterpret_cast<uint4*>(row1 + ((jj ^ sw) << 4)) = make_uint4(lo[4 * jj], lo[4 * jj + 1], lo[4 * jj + 2], lo[4 * jj + 3]);
-                        }
+                        float4 v[8];
+                        uint32_t hi[16], lo[16];
+                        load8(row0, sw, v);
+                        split16(v, hi, lo);
+                        store4(row0, sw, 0, hi);
+                        load8(row1, sw, v);
+                        store4(row1, sw, 0, lo);
+                        split16(v, hi, lo);
+                        store4(row0, sw, 4, hi);
+                        store4(row1, sw, 4, lo);
                     }
                 } else
                 for (int rho = rs0; rho < rows_up; rho += 32) {
@@ -291,8 +315,9 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         conv_range_report(g, __float_as_uint(amax), t.prec == MN_PREC_F16X3_TC || t.prec == MN_PREC_F16X1_TC);
     } else {
         // =========================== consumer warpgroups: ldmatrix A fragments + wgmma + epilogue ===========================
-        const int wg = (warp - 4) >> 2, wq = warp & 3;       // warpgroup (pixel rows 64wg..), warp within it (16 rows each)
-        const int wtid = threadIdx.x - 128 - wg * 128;        // 0..127 inside the warpgroup
+        setmaxnreg_inc<REG_CONS>();
+        const int wg = (warp - 8) >> 2, wq = warp & 3;       // warpgroup (pixel rows 64wg..), warp within it (16 rows each)
+        const int wtid = threadIdx.x - 256 - wg * 128;        // 0..127 inside the warpgroup
         constexpr bool bf = MODE == 1, three = MODE != 2;
         // the tile row this lane addresses for ldmatrix (rows 0-15 of the warp's 16-row slice, k-chunk lane >> 4)
         const int r = wg * 64 + wq * 16 + (lane & 15);
@@ -308,11 +333,27 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         // expected shrink of D (K/16 steps); Dc is 2^-11 of the result and needs nothing.
         const float dfix = 1.f + 1.5e-8f * (float)(t.taps * t.cbps * (KB / 16));
         float* wstg = stg + wg * 64 * STG_PITCH;
+        // Stage releases, once per warpgroup, after the wgmma group that read the stage has retired (the group's completion covers
+        // every warp's ldmatrix and B reads).  A weight stage is filled by the multicast of every CTA of the cluster: warp c of the
+        // warpgroup arrives on CTA c's barrier.
+        auto release_b = [&](uint32_t s) {
+            if (cs > 1) { if (lane == 0 && wq < cs) mbar_arrive_cluster(mapa_u32(bar(I_BE + s), (uint32_t)wq)); }
+            else if (wtid == 0) mbar_arrive(bar(I_BE + s));
+        };
+        auto release_a = [&](uint32_t s) { if (wtid == 0) mbar_arrive(bar(I_HE + s)); };
+        constexpr int ND = NT / 2;                            // accumulator registers per thread (64 rows x NT columns / 128 threads)
         uint32_t hs = 0, hph = 0, bs = 0, bph = 0;
-        for (int work = cluster_id; work < total_work; work += num_clusters) {
-            float d[32], dc[32];
+        for (int work = first_work(); work < total_work; work += num_clusters) {
+            float d[ND], dc[ND];
 #pragma unroll
-            for (int i = 0; i < 32; ++i) { d[i] = 0.f; dc[i] = 0.f; }
+            for (int i = 0; i < ND; ++i) { d[i] = 0.f; dc[i] = 0.f; }
+            auto fence_acc = [&]() {
+#pragma unroll
+                for (int i = 0; i < ND; ++i) { wg_fence_operand(d[i]); if (three) wg_fence_operand(dc[i]); }
+            };
+            // One wgmma group per tap, drained with wait_group 0: ptxas serializes register-A wgmmas (C7513) when ldmatrix writes
+            // fragment registers while a group is still in flight, so within a warpgroup the taps stay sequential and the overlap
+            // comes from the other consumer warpgroup (128-wide items give it twice the MMA time per tap to cover).
             int kb = 0;
             for (int u = 0; u < units; ++u) {
                 mbar_wait(bar(I_SD + hs), hph);
@@ -333,146 +374,140 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                     mbar_wait(bar(I_BF + bs), bph);
                     const uint64_t dh0 = desc0 + (uint64_t)((bs * B_STAGE) >> 4);   // start-address field is in 16-byte units
                     const uint64_t dl0 = dh0 + (uint64_t)(B_HALF >> 4);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) { wg_fence_operand(d[i]); wg_fence_operand(dc[i]); }
+                    fence_acc();
                     wg_fence();
 #pragma unroll
                     for (int j = 0; j < 4; ++j) {
                         const uint32_t acc = (kb | j) != 0;
-                        wgmma_m64n64k16_rs<bf>(d, ah[j], dh0 + 2 * j, acc);
-                        if (three) { wgmma_m64n64k16_rs<bf>(dc, ah[j], dl0 + 2 * j, acc); wgmma_m64n64k16_rs<bf>(dc, al[j], dh0 + 2 * j, 1); }
+                        wgmma_k16_rs<NT, bf>(d, ah[j], dh0 + 2 * j, acc);
+                        if (three) { wgmma_k16_rs<NT, bf>(dc, ah[j], dl0 + 2 * j, acc); wgmma_k16_rs<NT, bf>(dc, al[j], dh0 + 2 * j, 1); }
                     }
                     wg_commit();
                     wg_wait<0>();
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) { wg_fence_operand(d[i]); wg_fence_operand(dc[i]); }
-                    // this warp's reads of B stage bs are complete: release it in every CTA that multicasts into it
-                    __syncwarp();
-                    if (lane == 0) {
-                        if (cs > 1) { for (int c = 0; c < cs; ++c) mbar_arrive_cluster(mapa_u32(bar(I_BE + bs), c)); }
-                        else mbar_arrive(bar(I_BE + bs));
-                    }
+                    fence_acc();
+                    release_b(bs);
                     if (++bs == (uint32_t)BS) { bs = 0; bph ^= 1; }
                 }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar(I_HE + hs));          // every tap of this A tile has been read
+                release_a(hs);                                        // every tap of this A tile has been read
                 if (++hs == (uint32_t)HS) { hs = 0; hph ^= 1; }
             }
 
-            // ---- epilogue: accumulators -> staging rows (this warpgroup's 64 rows) -> fused epilogue with float4 row stores ----
+            // ---- epilogue, per 64-column half: accumulators -> staging rows (this warpgroup's 64 rows) -> fused epilogue with
+            // float4 row stores ----
+#pragma unroll
+            for (int i = 0; i < ND; ++i) d[i] = three ? fmaf(d[i], dfix, dc[i]) * wscale : d[i] * wscale;
             const int nt_i = work_nt(work);
             const int ks = work_ks(work);
             int n0, oy0, ox0;
             tile_origin(work, n0, oy0, ox0);
-            named_bar_sync(1 + wg, 128);                              // the previous item's rows have been stored
-            if (wtid < 64) {
-                const int rr = wg * 64 + wtid;
-                const int tn2 = rr / (t.TH * t.TW), rem2 = rr - tn2 * (t.TH * t.TW);
-                const int th2 = rem2 / t.TW, tw2 = rem2 - th2 * t.TW;
-                const int n = n0 + tn2, oy = oy0 + th2, ox = ox0 + tw2;
-                const bool ok = tn2 < t.TN && n < g.N && oy < g.OH && ox < g.OW;
-                rowm[rr] = ok ? (n * g.OH + oy) * g.OW + ox : -1;
-                rowm[128 + rr] = ok ? (n | ((g.valid_w && ox >= g.valid_w[n]) ? (1 << 30) : 0)) : 0;
-            }
-            {
-                // accumulator layout of wgmma m64nN: d[4i + {0,1}] = row (lane >> 2), cols 8i + 2(lane & 3) + {0,1}; d[4i + {2,3}] = row + 8
-                const int row = wq * 16 + (lane >> 2), col = 2 * (lane & 3);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    float v0, v1, v2, v3;
-                    if (three) {
-                        v0 = fmaf(d[4 * i], dfix, dc[4 * i]) * wscale; v1 = fmaf(d[4 * i + 1], dfix, dc[4 * i + 1]) * wscale;
-                        v2 = fmaf(d[4 * i + 2], dfix, dc[4 * i + 2]) * wscale; v3 = fmaf(d[4 * i + 3], dfix, dc[4 * i + 3]) * wscale;
-                    } else {
-                        v0 = d[4 * i] * wscale; v1 = d[4 * i + 1] * wscale; v2 = d[4 * i + 2] * wscale; v3 = d[4 * i + 3] * wscale;
-                    }
-                    *reinterpret_cast<float2*>(wstg + row * STG_PITCH + 8 * i + col) = make_float2(v0, v1);
-                    *reinterpret_cast<float2*>(wstg + (row + 8) * STG_PITCH + 8 * i + col) = make_float2(v2, v3);
+#pragma unroll 1
+            for (int h = 0; h < NT / 64; ++h) {
+                named_bar_sync(1 + wg, 128);                              // the previous half's / item's rows have been stored
+                if (h == 0 && wtid < 64) {
+                    const int rr = wg * 64 + wtid;
+                    const int tn2 = rr / (t.TH * t.TW), rem2 = rr - tn2 * (t.TH * t.TW);
+                    const int th2 = rem2 / t.TW, tw2 = rem2 - th2 * t.TW;
+                    const int n = n0 + tn2, oy = oy0 + th2, ox = ox0 + tw2;
+                    const bool ok = tn2 < t.TN && n < g.N && oy < g.OH && ox < g.OW;
+                    rowm[rr] = ok ? (n * g.OH + oy) * g.OW + ox : -1;
+                    rowm[128 + rr] = ok ? (n | ((g.valid_w && ox >= g.valid_w[n]) ? (1 << 30) : 0)) : 0;
                 }
-            }
-            named_bar_sync(1 + wg, 128);
-            {
-                const int col = (lane & 15) * 4;
-                const int o = nt_i * NT + col;
-                const int rbase = wg * 64 + wq * 16 + (lane >> 4);   // tile rows rbase + 2i, i < 8
-                if (t.ksplit > 1) {
-                    // raw partial sum of this k-slice; conv_splitk_reduce_kernel adds the slices and runs the epilogue
-#pragma unroll 4
+                {
+                    // accumulator layout of wgmma m64nN: d[4i + {0,1}] = row (lane >> 2), cols 8i + 2(lane & 3) + {0,1}; d[4i + {2,3}] = row + 8
+                    const int row = wq * 16 + (lane >> 2), col = 2 * (lane & 3);
+#pragma unroll
                     for (int i = 0; i < 8; ++i) {
-                        const int row = rbase + 2 * i;
-                        const int m = rowm[row];
-                        if (m >= 0)
-                            *reinterpret_cast<float4*>(g.ws + ((size_t)ks * g.M + m) * g.Cout + o) =
-                                *reinterpret_cast<const float4*>(stg + row * STG_PITCH + col);
+                        const int i1 = ND - 32 + 4 * i;                   // columns 64 + 8i.. of the second half (== 4i when NT == 64)
+                        const float v0 = h ? d[i1] : d[4 * i], v1 = h ? d[i1 + 1] : d[4 * i + 1];
+                        const float v2 = h ? d[i1 + 2] : d[4 * i + 2], v3 = h ? d[i1 + 3] : d[4 * i + 3];
+                        *reinterpret_cast<float2*>(wstg + row * STG_PITCH + 8 * i + col) = make_float2(v0, v1);
+                        *reinterpret_cast<float2*>(wstg + (row + 8) * STG_PITCH + 8 * i + col) = make_float2(v2, v3);
                     }
-                } else {
-                    const float4 bias4 = g.bias ? ldg4(g.bias + o) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    // one sample per tile (every layer except the 4x4 .. 8x8 maps): its per-sample scale vectors are loaded once
-                    const bool one_n = t.TN == 1;
-                    float4 os4 = make_float4(1.f, 1.f, 1.f, 1.f), y2s4 = os4;
-                    float* y2base = g.y2;
-                    if (one_n && n0 < g.N) {
-                        if (g.out_scale) os4 = ldg4(g.out_scale + (size_t)n0 * g.os_stride + o);
-                        if (g.y2 && g.y2_scale) y2s4 = ldg4(g.y2_scale + (size_t)n0 * g.y2s_stride + o);
-                        // per-sample (possibly peer-GPU) destination of the second output, rebased so that row index m addresses it
-                        if (g.y2_ptrs) y2base = g.y2_ptrs[n0] - (size_t)n0 * g.OH * g.OW * g.y2_cs;
-                    }
-                    float gs = 0.f, gq = 0.f;       // GroupNorm statistics of this thread's 8 rows x 4 channels (one group)
-                    // One sample per tile and the tile inside the tensor (the plans guarantee H % TH == 0, W % TW == 0 and a power-of-two
-                    // TW): every row is valid and its pixel index is arithmetic -- no rowm look-ups, no per-row branch.
-                    const bool dense_tile = one_n && n0 < g.N;
-                    const int tws = __ffs(t.TW) - 1;
-                    const int m00 = (n0 * g.OH + oy0) * g.OW + ox0;
-                    const int vwn = (dense_tile && g.valid_w) ? g.valid_w[n0] : 0x7fffffff;
-                    auto rows_dense = [&](auto tag) {
-                        constexpr int ACT = decltype(tag)::value;
-#pragma unroll 8
-                        for (int i = 0; i < 8; ++i) {
-                            const int row = rbase + 2 * i;
-                            const int th3 = row >> tws, tw3 = row & (t.TW - 1);
-                            const int m = m00 + th3 * g.OW + tw3;
-                            const float4 uv = *reinterpret_cast<const float4*>(stg + row * STG_PITCH + col);
-                            const float4 w4 = conv_epilogue_row4<ACT>(g, m, n0, ox0 + tw3 >= vwn, o, uv, bias4, true, os4, true, y2s4, y2base);
-                            if (g.gn_stats_out) {
-                                gs += (w4.x + w4.y) + (w4.z + w4.w);
-                                gq = fmaf(w4.x, w4.x, fmaf(w4.y, w4.y, fmaf(w4.z, w4.z, fmaf(w4.w, w4.w, gq))));
-                            }
-                        }
-                    };
-                    auto rows = [&](auto tag) {
-                        constexpr int ACT = decltype(tag)::value;
-                        if (dense_tile) { rows_dense(tag); return; }
-                        if (one_n) return;                       // padding CTA of a cluster: nothing to store
+                }
+                named_bar_sync(1 + wg, 128);
+                {
+                    const int col = (lane & 15) * 4;
+                    const int o = nt_i * NT + h * 64 + col;
+                    const int rbase = wg * 64 + wq * 16 + (lane >> 4);   // tile rows rbase + 2i, i < 8
+                    if (t.ksplit > 1) {
+                        // raw partial sum of this k-slice; conv_splitk_reduce_kernel adds the slices and runs the epilogue
 #pragma unroll 4
                         for (int i = 0; i < 8; ++i) {
                             const int row = rbase + 2 * i;
                             const int m = rowm[row];
-                            if (m >= 0) {
-                                const int nn = rowm[128 + row];
+                            if (m >= 0)
+                                *reinterpret_cast<float4*>(g.ws + ((size_t)ks * g.M + m) * g.Cout + o) =
+                                    *reinterpret_cast<const float4*>(stg + row * STG_PITCH + col);
+                        }
+                    } else {
+                        const float4 bias4 = g.bias ? ldg4(g.bias + o) : make_float4(0.f, 0.f, 0.f, 0.f);
+                        // one sample per tile (every layer except the 4x4 .. 8x8 maps): its per-sample scale vectors are loaded once
+                        const bool one_n = t.TN == 1;
+                        float4 os4 = make_float4(1.f, 1.f, 1.f, 1.f), y2s4 = os4;
+                        float* y2base = g.y2;
+                        if (one_n && n0 < g.N) {
+                            if (g.out_scale) os4 = ldg4(g.out_scale + (size_t)n0 * g.os_stride + o);
+                            if (g.y2 && g.y2_scale) y2s4 = ldg4(g.y2_scale + (size_t)n0 * g.y2s_stride + o);
+                            // per-sample (possibly peer-GPU) destination of the second output, rebased so that row index m addresses it
+                            if (g.y2_ptrs) y2base = g.y2_ptrs[n0] - (size_t)n0 * g.OH * g.OW * g.y2_cs;
+                        }
+                        float gs = 0.f, gq = 0.f;       // GroupNorm statistics of this thread's 8 rows x 4 channels (one group)
+                        // One sample per tile and the tile inside the tensor (the plans guarantee H % TH == 0, W % TW == 0 and a power-of-two
+                        // TW): every row is valid and its pixel index is arithmetic -- no rowm look-ups, no per-row branch.
+                        const bool dense_tile = one_n && n0 < g.N;
+                        const int tws = __ffs(t.TW) - 1;
+                        const int m00 = (n0 * g.OH + oy0) * g.OW + ox0;
+                        const int vwn = (dense_tile && g.valid_w) ? g.valid_w[n0] : 0x7fffffff;
+                        auto rows_dense = [&](auto tag) {
+                            constexpr int ACT = decltype(tag)::value;
+#pragma unroll 8
+                            for (int i = 0; i < 8; ++i) {
+                                const int row = rbase + 2 * i;
+                                const int th3 = row >> tws, tw3 = row & (t.TW - 1);
+                                const int m = m00 + th3 * g.OW + tw3;
                                 const float4 uv = *reinterpret_cast<const float4*>(stg + row * STG_PITCH + col);
-                                const float4 w4 = conv_epilogue_row4<ACT>(g, m, nn & 0x3FFFFFFF, (nn >> 30) != 0, o, uv, bias4, one_n, os4, one_n, y2s4, y2base);
+                                const float4 w4 = conv_epilogue_row4<ACT>(g, m, n0, ox0 + tw3 >= vwn, o, uv, bias4, true, os4, true, y2s4, y2base);
                                 if (g.gn_stats_out) {
                                     gs += (w4.x + w4.y) + (w4.z + w4.w);
                                     gq = fmaf(w4.x, w4.x, fmaf(w4.y, w4.y, fmaf(w4.z, w4.z, fmaf(w4.w, w4.w, gq))));
                                 }
                             }
+                        };
+                        auto rows = [&](auto tag) {
+                            constexpr int ACT = decltype(tag)::value;
+                            if (dense_tile) { rows_dense(tag); return; }
+                            if (one_n) return;                       // padding CTA of a cluster: nothing to store
+#pragma unroll 4
+                            for (int i = 0; i < 8; ++i) {
+                                const int row = rbase + 2 * i;
+                                const int m = rowm[row];
+                                if (m >= 0) {
+                                    const int nn = rowm[128 + row];
+                                    const float4 uv = *reinterpret_cast<const float4*>(stg + row * STG_PITCH + col);
+                                    const float4 w4 = conv_epilogue_row4<ACT>(g, m, nn & 0x3FFFFFFF, (nn >> 30) != 0, o, uv, bias4, one_n, os4, one_n, y2s4, y2base);
+                                    if (g.gn_stats_out) {
+                                        gs += (w4.x + w4.y) + (w4.z + w4.w);
+                                        gq = fmaf(w4.x, w4.x, fmaf(w4.y, w4.y, fmaf(w4.z, w4.z, fmaf(w4.w, w4.w, gq))));
+                                    }
+                                }
+                            }
+                        };
+                        switch (g.act) {
+                            case MN_ACT_NONE: rows(ActTag<MN_ACT_NONE>{}); break;
+                            case MN_ACT_RELU: rows(ActTag<MN_ACT_RELU>{}); break;
+                            case MN_ACT_LRELU02: rows(ActTag<MN_ACT_LRELU02>{}); break;
+                            default: rows(ActTag<-1>{}); break;
                         }
-                    };
-                    switch (g.act) {
-                        case MN_ACT_NONE: rows(ActTag<MN_ACT_NONE>{}); break;
-                        case MN_ACT_RELU: rows(ActTag<MN_ACT_RELU>{}); break;
-                        case MN_ACT_LRELU02: rows(ActTag<MN_ACT_LRELU02>{}); break;
-                        default: rows(ActTag<-1>{}); break;
-                    }
-                    if (g.gn_stats_out) {
-                        // lanes 0-7 / 8-15 (and 16-23 / 24-31, the odd rows) hold the two 32-channel groups of this 64-column tile
+                        if (g.gn_stats_out) {
+                            // lanes 0-7 / 8-15 (and 16-23 / 24-31, the odd rows) hold the two 32-channel groups of this 64-column half
 #pragma unroll
-                        for (int sh = 1; sh <= 4; sh <<= 1) { gs += __shfl_xor_sync(0xffffffffu, gs, sh); gq += __shfl_xor_sync(0xffffffffu, gq, sh); }
-                        gs += __shfl_xor_sync(0xffffffffu, gs, 16); gq += __shfl_xor_sync(0xffffffffu, gq, 16);
-                        if ((lane & 23) == 0 && n0 < g.N) {        // lanes 0 and 8
-                            double* dst = g.gn_stats_out + ((size_t)n0 * (g.Cout >> 5) + (o >> 5)) * 2;
-                            atomicAdd(dst, (double)gs);
-                            atomicAdd(dst + 1, (double)gq);
+                            for (int sh = 1; sh <= 4; sh <<= 1) { gs += __shfl_xor_sync(0xffffffffu, gs, sh); gq += __shfl_xor_sync(0xffffffffu, gq, sh); }
+                            gs += __shfl_xor_sync(0xffffffffu, gs, 16); gq += __shfl_xor_sync(0xffffffffu, gq, 16);
+                            if ((lane & 23) == 0 && n0 < g.N) {        // lanes 0 and 8
+                                double* dst = g.gn_stats_out + ((size_t)n0 * (g.Cout >> 5) + (o >> 5)) * 2;
+                                atomicAdd(dst, (double)gs);
+                                atomicAdd(dst + 1, (double)gq);
+                            }
                         }
                     }
                 }
@@ -518,18 +553,14 @@ bool plan_common(const ConvGeom& g, Tc2Plan& p) {
         return fail("epilogue operands must be 16-byte aligned with channel strides that are multiples of 4");
     p.t.KW = g.KW;
     p.t.cblocks = g.Cin / KB; p.t.taps = g.KH * g.KW;
-    p.t.n_tiles = g.Cout / NT;
     return true;
 }
 
-// cluster pairing, split-K and the shared-memory rings, once the pixel tile is known
-bool plan_finish(const ConvGeom& g, Tc2Plan& p, bool allow_ksplit) {
+// split-K, the shared-memory rings and the plan's size for work items of nt output channels
+void plan_nt(const ConvGeom& g, Tc2Plan& p, bool allow_ksplit, int nt) {
     Tc2Geom& t = p.t;
-    t.box_bytes = (t.halo_rows * 128 + 1023) & ~1023;
-    t.halo_stage_bytes = 2 * t.box_bytes;
-    t.m_tiles = t.tiles_w * t.tiles_h * t.tiles_n;
-    t.cs = t.m_tiles >= 2 ? 2 : 1;
-    t.m_groups = (t.m_tiles + t.cs - 1) / t.cs;
+    t.nt = nt;
+    t.n_tiles = g.Cout / nt;
     // split-K: few tiles but a deep K loop (4x4 / 8x8 generator layers, ResNet stages at batch 1) -> spread the channel blocks of
     // a tile over several CTAs; partial sums go to the caller's workspace and conv_splitk_reduce_kernel finishes the job.
     t.ksplit = 1;
@@ -544,13 +575,41 @@ bool plan_finish(const ConvGeom& g, Tc2Plan& p, bool allow_ksplit) {
     const int other = STG_BYTES + 1024 + 256 + 1024;
     const int units = t.per_tap ? t.cbps * t.taps : t.cbps;
     t.hstages = 2;
-    if (3 * t.halo_stage_bytes + other + 3 * B_STAGE <= SMEM_LIMIT && (t.per_tap || (units <= 4 && units >= 2))) t.hstages = 3;
+    if (3 * t.halo_stage_bytes + other + 3 * b_stage(nt) <= SMEM_LIMIT && (t.per_tap || (units <= 4 && units >= 2))) t.hstages = 3;
     const int fixed = t.hstages * t.halo_stage_bytes + other;
-    int bs = (SMEM_LIMIT - fixed) / B_STAGE;
+    int bs = (SMEM_LIMIT - fixed) / b_stage(nt);
     if (bs > MAX_BSTAGES) bs = MAX_BSTAGES;
-    if (bs < 2) { p.ok = false; p.why = "not enough shared memory for 2 weight stages"; return false; }
     t.bstages = bs;
-    p.smem = fixed + bs * B_STAGE;
+    p.smem = fixed + bs * b_stage(nt);
+}
+
+// persistent-grid makespan of a plan in units of one 64-channel x 64-k x tap block per pixel tile
+int64_t plan_cost(const Tc2Geom& t) {
+    const int clusters = mn_num_sms() / t.cs;
+    const int64_t waves = (t.m_groups * t.n_tiles * t.ksplit + clusters - 1) / clusters;
+    return waves * (t.nt / 64) * t.cbps;
+}
+
+// cluster pairing, the work-item width, split-K and the shared-memory rings, once the pixel tile is known
+bool plan_finish(const ConvGeom& g, Tc2Plan& p, bool allow_ksplit) {
+    Tc2Geom& t = p.t;
+    t.box_bytes = (t.halo_rows * 128 + 1023) & ~1023;
+    t.halo_stage_bytes = 2 * t.box_bytes;
+    t.m_tiles = t.tiles_w * t.tiles_h * t.tiles_n;
+    t.cs = t.m_tiles >= 2 ? 2 : 1;
+    t.m_groups = (t.m_tiles + t.cs - 1) / t.cs;
+    // 128-channel work items read each A fragment and split each halo for twice the outputs.  Take them unless they leave
+    // fewer than 3 weight stages or halving the number of items lengthens the persistent grid's makespan (Cout = 64 layers,
+    // few-tile layers at batch 1).  Equal makespans go to the wider items only if they need no deeper split-K: on small layers
+    // the extra partial sums and reduce launch cost more than the wider tile saves.
+    plan_nt(g, p, allow_ksplit, 64);
+    if (g.Cout % 128 == 0) {
+        Tc2Plan wide = p;
+        plan_nt(g, wide, allow_ksplit, 128);
+        const int64_t cw = plan_cost(wide.t), cn = plan_cost(p.t);
+        if (wide.t.bstages >= 3 && (cw < cn || (cw == cn && wide.t.ksplit <= p.t.ksplit))) p = wide;
+    }
+    if (t.bstages < 2) { p.ok = false; p.why = "not enough shared memory for 2 weight stages"; return false; }
     p.ok = true;
     return true;
 }
@@ -608,10 +667,10 @@ Tc2Plan plan_tc1(const ConvGeom& g) {
     return p;
 }
 
-template <bool GN, int MODE>
+template <bool GN, int MODE, int NT>
 int launch_tc2(const CUtensorMap& ma, const CUtensorMap& mbh, const CUtensorMap& mbl, const ConvGeom& g, const Tc2Plan& p, cudaStream_t st) {
     static unsigned long long smem_done = 0;
-    MN_CUDA_CHECK(mn_ensure_dyn_smem(conv_tc2_kernel<GN, MODE>, SMEM_LIMIT, &smem_done));
+    MN_CUDA_CHECK(mn_ensure_dyn_smem(conv_tc2_kernel<GN, MODE, NT>, SMEM_LIMIT, &smem_done));
     const Tc2Geom& t = p.t;
     const int total_work = t.m_groups * t.n_tiles * t.ksplit;
     int sms = mn_num_sms();
@@ -630,8 +689,13 @@ int launch_tc2(const CUtensorMap& ma, const CUtensorMap& mbh, const CUtensorMap&
     attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = mn_pdl_enabled() ? 2 : 1;
-    MN_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_tc2_kernel<GN, MODE>, ma, mbh, mbl, g, t));
+    MN_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_tc2_kernel<GN, MODE, NT>, ma, mbh, mbl, g, t));
     return MN_OK;
+}
+
+template <bool GN, int MODE>
+int launch_tc2_nt(const CUtensorMap& ma, const CUtensorMap& mbh, const CUtensorMap& mbl, const ConvGeom& g, const Tc2Plan& p, cudaStream_t st) {
+    return p.t.nt == 128 ? launch_tc2<GN, MODE, 128>(ma, mbh, mbl, g, p, st) : launch_tc2<GN, MODE, 64>(ma, mbh, mbl, g, p, st);
 }
 
 int launch_plan(const ConvGeom& g, Tc2Plan& p, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st) {
@@ -654,7 +718,7 @@ int launch_plan(const ConvGeom& g, Tc2Plan& p, const void* w_hi, const void* w_l
     for (int which = 0; which < 2; ++which) {
         cuuint64_t dims[3] = {(cuuint64_t)g.Cin, (cuuint64_t)g.Cout, (cuuint64_t)(g.KH * g.KW)};
         cuuint64_t strides[2] = {(cuuint64_t)g.Cin * 2, (cuuint64_t)g.Cin * g.Cout * 2};
-        cuuint32_t box[3] = {64, (cuuint32_t)(NT / t.cs), 1};
+        cuuint32_t box[3] = {64, (cuuint32_t)(t.nt / t.cs), 1};
         cuuint32_t es[3] = {1, 1, 1};
         CUresult r = enc(which ? &mbl : &mbh, dt, 3, const_cast<void*>(which ? w_lo : w_hi), dims, strides, box, es,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -664,9 +728,9 @@ int launch_plan(const ConvGeom& g, Tc2Plan& p, const void* w_hi, const void* w_l
     t.wscale = w_scale + 1;
     t.prec = prec;
     int rc;
-    if (prec == MN_PREC_BF16X3_TC) rc = g.gn_mr ? launch_tc2<true, 1>(ma, mbh, mbl, g, p, st) : launch_tc2<false, 1>(ma, mbh, mbl, g, p, st);
-    else if (prec == MN_PREC_F16X1_TC) rc = g.gn_mr ? launch_tc2<true, 2>(ma, mbh, mbl, g, p, st) : launch_tc2<false, 2>(ma, mbh, mbl, g, p, st);
-    else rc = g.gn_mr ? launch_tc2<true, 0>(ma, mbh, mbl, g, p, st) : launch_tc2<false, 0>(ma, mbh, mbl, g, p, st);
+    if (prec == MN_PREC_BF16X3_TC) rc = g.gn_mr ? launch_tc2_nt<true, 1>(ma, mbh, mbl, g, p, st) : launch_tc2_nt<false, 1>(ma, mbh, mbl, g, p, st);
+    else if (prec == MN_PREC_F16X1_TC) rc = g.gn_mr ? launch_tc2_nt<true, 2>(ma, mbh, mbl, g, p, st) : launch_tc2_nt<false, 2>(ma, mbh, mbl, g, p, st);
+    else rc = g.gn_mr ? launch_tc2_nt<true, 0>(ma, mbh, mbl, g, p, st) : launch_tc2_nt<false, 0>(ma, mbh, mbl, g, p, st);
     if (rc != MN_OK || t.ksplit == 1) return rc;
     ConvGeom gr = g;
     gr.splits = t.ksplit;

@@ -84,11 +84,11 @@ __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.
 // keeps the compiler from moving accumulator accesses across the asynchronous MMA window
 __device__ __forceinline__ void wg_fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
-// D[64 x 64] (+)= A[64 x 16, registers] * B[16 x 64, shared-memory descriptor, K-major]; BF selects bf16 over fp16 operands.
-template <bool BF>
-__device__ __forceinline__ void wgmma_m64n64k16_rs(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 16, registers] * B[16 x N, shared-memory descriptor, K-major], N = 64 or 128; BF selects bf16 over fp16.
+template <int N, bool BF>
+__device__ __forceinline__ void wgmma_k16_rs(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
 #define MN_WG_D8(i) "+f"(d[i + 0]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
-#define MN_WG_ASM(TY)                                                                                                           \
+#define MN_WG_ASM64(TY)                                                                                                         \
     asm volatile(                                                                                                               \
         "{\n\t.reg .pred p;\n\t"                                                                                                \
         "setp.ne.b32 p, %38, 0;\n\t"                                                                                            \
@@ -99,11 +99,37 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs(float* d, const uint32_t* a, 
         : MN_WG_D8(0), MN_WG_D8(8), MN_WG_D8(16), MN_WG_D8(24)                                                                  \
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "n"(0), "r"(accumulate)                                      \
         : "memory")
-    if (BF) MN_WG_ASM("bf16");
-    else MN_WG_ASM("f16");
-#undef MN_WG_ASM
+#define MN_WG_ASM128(TY)                                                                                                        \
+    asm volatile(                                                                                                               \
+        "{\n\t.reg .pred p;\n\t"                                                                                                \
+        "setp.ne.b32 p, %70, 0;\n\t"                                                                                            \
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " "                                                            \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                               \
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                                      \
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                                      \
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "                                     \
+        "{%64, %65, %66, %67}, %68, p, 1, 1, %69;\n\t}"                                                                         \
+        : MN_WG_D8(0), MN_WG_D8(8), MN_WG_D8(16), MN_WG_D8(24), MN_WG_D8(32), MN_WG_D8(40), MN_WG_D8(48), MN_WG_D8(56)          \
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "n"(0), "r"(accumulate)                                      \
+        : "memory")
+    static_assert(N == 64 || N == 128, "wgmma_k16_rs: N must be 64 or 128");
+    if constexpr (N == 64) {
+        if (BF) MN_WG_ASM64("bf16");
+        else MN_WG_ASM64("f16");
+    } else {
+        if (BF) MN_WG_ASM128("bf16");
+        else MN_WG_ASM128("f16");
+    }
+#undef MN_WG_ASM128
+#undef MN_WG_ASM64
 #undef MN_WG_D8
 }
+
+// Hand registers between warpgroups (every warp of the warpgroup executes it): dec returns them to the CTA's pool, inc waits for them.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // One elected lane of a fully converged warp.  Code under `if (elect_one_sync())` inside warp-uniform control flow lets ptxas
 // feed TMA uniform-register operands with plain R2UR instead of the loop it emits under a divergent `lane == 0` branch.

@@ -1,6 +1,7 @@
 """Per-layer timing of every mn_conv2d_nhwc call of one 16-character line (developer tool): CUDA events around each eager call,
 warm caches, module graphs off.  Prints the layers sorted by time with their algorithmic TFLOP/s and, for the tensor-core layers, the
-fraction of the tensor pipe (3 fp16 MMA passes per fp32-grade product, against MEASURED_PEAKS.json's bf16 burst peak).
+fraction of the tensor pipe (3 fp16 MMA passes per fp32-grade product, against MEASURED_PEAKS.json's bf16 burst peak when present,
+else the H100 SXM data sheet's 989 TFLOP/s dense bf16, a 700 W figure).
 
     MN_MODULE_GRAPHS=0 python tools/profile_conv_layers.py [--chars 16] [--iters 10]
 """
@@ -71,7 +72,7 @@ def main():
     for _ in range(args.iters):
         one_pass()
     torch.cuda.synchronize()
-    peak = 1685.4
+    peak = 989.0      # NVIDIA H100 SXM data sheet, dense bf16 (700 W card), as bench.py uses
     try:
         peak = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["bf16_tflops"]
     except Exception:
