@@ -184,6 +184,14 @@ int mn_demod_batched(const float* s_all, int s_stride, const mn_demod_desc* desc
  * models/networks.py:268,293,318,360,370,415-416 (and the per-sample style multiply of :284). */
 int mn_resample_modulate(const float* x, int x_cs, float* y, int y_cs, const float* s, int s_stride,
                          int N, int H, int W, int C, int up, void* stream);
+/* Ragged-width bilinear x2 of the SR decoder (models/networks.py:360,370,415-416 -- the trunk's two up-samples, conv_up.0 and
+ * conv_final.2 -- for a batch whose lines have their own widths): sample n is the first valid_w[n] <= W columns of its W-wide
+ * rows.  The source column clamps at valid_w[n]-1 (the right edge of that line's own tensor in the reference) instead of W-1;
+ * output columns >= 2*valid_w[n] of the [N, 2H, 2W, C] output are written as 0.  s (may be NULL; 16B aligned, s_stride % 4 == 0)
+ * is the per-sample channel scale of mn_resample_modulate.  Each sample equals mn_resample_modulate(up=1) run on it alone at its
+ * exact width, bit for bit. */
+int mn_resample_modulate_ragged(const float* x, int x_cs, float* y, int y_cs, const float* s, int s_stride,
+                                const int32_t* valid_w, int N, int H, int W, int C, void* stream);
 
 /* ToRGB, models/networks.py:313-321: 1x1 modulated conv to 3 channels WITHOUT demodulation
  * + bias + bilinear-x2(skip) + tanh.
@@ -246,6 +254,12 @@ int mn_window_scatter(const float* feat, int feat_cs, const float* scale, const 
  *   becomes a zero-width window. */
 int mn_char_windows(const float* locs, int locs_stride, const int32_t* line_first, int B, int max_chars, int W, int half,
                     mn_window* win, int32_t* valid, int32_t* owner, int32_t* err, void* stream);
+/* mn_char_windows for lines of their own widths (device int32 line_w[B], each <= W), models/networks.py:426-441 / :460-474 run on
+ * each line's own tensor: center = (int)(locs[b*locs_stride + 2c] * line_w[b]), x2 = min(center+half, line_w[b]); owner[b*W+x]
+ * is filled for x < line_w[b] and -1 beyond.  Error bits as in mn_char_windows.  A width larger than W is not reported: it is
+ * clamped to W (the caller guarantees line_w[b] <= W). */
+int mn_char_windows_ragged(const float* locs, int locs_stride, const int32_t* line_first, const int32_t* line_w, int B, int max_chars,
+                           int W, int half, mn_window* win, int32_t* valid, int32_t* owner, int32_t* err, void* stream);
 
 /* The reference module's standalone helper functions on NCHW-contiguous tensors (rows = B*C, len = H*W); the hot path uses
  * the fused NHWC kernels above.

@@ -144,11 +144,16 @@ constexpr int UP_RX = 4;
 __device__ __forceinline__ float4 up_hblend(const float4& a, const float4& b, float hx, float lx) {
     return make_float4(hx * a.x + lx * b.x, hx * a.y + lx * b.y, hx * a.z + lx * b.z, hx * a.w + lx * b.w);
 }
+// RAGGED: sample n is the first valid_w[n] columns of its row (row pitch stays W): the source column clamps at valid_w[n]-1, the
+// edge of that line's own tensor in the reference, and output columns >= 2*valid_w[n] are written as 0.  Each sample is then
+// bit-identical to the non-ragged instantiation run on that sample alone at width valid_w[n].
+template <bool RAGGED>
 __global__ void __launch_bounds__(256) resample_up2_kernel(const float* __restrict__ x, int x_cs, float* __restrict__ y, int y_cs,
-                                                           const float* __restrict__ s, int s_stride, int N, int H, int W, int C) {
+                                                           const float* __restrict__ s, int s_stride, int N, int H, int W_pitch, int C,
+                                                           const int32_t* __restrict__ valid_w) {
     mn_pdl_prologue();
     const int c4 = C >> 2;
-    const int runs = (W + UP_RX - 1) / UP_RX;
+    const int runs = (W_pitch + UP_RX - 1) / UP_RX;
     const uint32_t total = (uint32_t)N * H * runs * c4;              // host guarantees the output (16x more) fits 31 bits
     const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= total) return;
@@ -158,9 +163,24 @@ __global__ void __launch_bounds__(256) resample_up2_kernel(const float* __restri
     t /= runs;
     const int iy = (int)(t % H);
     const int n = (int)(t / H);
-    const float* xn = x + (size_t)n * H * W * x_cs + c;
-    const float* row[3] = {xn + (size_t)(iy > 0 ? iy - 1 : 0) * W * x_cs, xn + (size_t)iy * W * x_cs,
-                           xn + (size_t)(iy < H - 1 ? iy + 1 : iy) * W * x_cs};
+    const int W = RAGGED ? min(valid_w[n], W_pitch) : W_pitch;       // clamp bound: the sample's own width
+    const int OH = 2 * H, OW = 2 * W_pitch;
+    float* y0p = y + ((size_t)n * OH + 2 * iy) * OW * y_cs + c;
+    float* y1p = y0p + (size_t)OW * y_cs;
+    if (RAGGED) {                                  // columns of this run beyond the sample's width: zeros
+        const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+        const int xe = min(xs + UP_RX, W_pitch);
+        for (int ix = max(xs, W); ix < xe; ++ix)
+#pragma unroll
+            for (int dx = 0; dx < 2; ++dx) {
+                *reinterpret_cast<float4*>(y0p + (size_t)(2 * ix + dx) * y_cs) = z;
+                *reinterpret_cast<float4*>(y1p + (size_t)(2 * ix + dx) * y_cs) = z;
+            }
+        if (xs >= W) return;
+    }
+    const float* xn = x + (size_t)n * H * W_pitch * x_cs + c;
+    const float* row[3] = {xn + (size_t)(iy > 0 ? iy - 1 : 0) * W_pitch * x_cs, xn + (size_t)iy * W_pitch * x_cs,
+                           xn + (size_t)(iy < H - 1 ? iy + 1 : iy) * W_pitch * x_cs};
     float4 sv = make_float4(1.f, 1.f, 1.f, 1.f);
     if (s) sv = *reinterpret_cast<const float4*>(s + (size_t)n * s_stride + c);
     // vertical taps of the two output rows (2iy, 2iy+1): which of {row above, this row, row below} and with what weight
@@ -169,9 +189,6 @@ __global__ void __launch_bounds__(256) resample_up2_kernel(const float* __restri
     bilin_coords(2 * iy + 1, H, yb0, yb1, lyb);
     const bool top = iy == 0;                      // even output row of the first input row: taps (row 0, row 1) with weight 0 on row 1
     const float hya = 1.f - lya, hyb = 1.f - lyb;
-    const int OH = 2 * H, OW = 2 * W;
-    float* y0p = y + ((size_t)n * OH + 2 * iy) * OW * y_cs + c;
-    float* y1p = y0p + (size_t)OW * y_cs;
 
     float4 L[3], M[3], R[3], Nx[3];
     const int xl = xs > 0 ? xs - 1 : 0, xr = xs + 1 < W ? xs + 1 : W - 1;
@@ -343,11 +360,26 @@ extern "C" int mn_resample_modulate(const float* x, int x_cs, float* y, int y_cs
     const int64_t total = (int64_t)N * OH * OW * (C >> 2);
     MN_REQUIRE(total < (1ll << 31), "tensor too large for 32-bit indexing");
     if (up && (!s || ((s_stride & 3) == 0 && ((uintptr_t)s & 15) == 0))) {
-        MN_CUDA_CHECK((mn_launch(resample_up2_kernel, dim3((unsigned)mn_cdiv64((int64_t)N * H * mn_cdiv(W, UP_RX) * (C >> 2), 256)), dim3(256), 0, (cudaStream_t)stream, x, x_cs, y, y_cs, s, s_stride, N, H, W, C)));
+        MN_CUDA_CHECK((mn_launch(resample_up2_kernel<false>, dim3((unsigned)mn_cdiv64((int64_t)N * H * mn_cdiv(W, UP_RX) * (C >> 2), 256)), dim3(256), 0, (cudaStream_t)stream, x, x_cs, y, y_cs, s, s_stride, N, H, W, C,
+                                 (const int32_t*)nullptr)));
         MN_LAUNCH_CHECK();
         return MN_OK;
     }
     MN_CUDA_CHECK((mn_launch(resample_modulate_kernel, dim3((unsigned)mn_cdiv64(total, 256)), dim3(256), 0, (cudaStream_t)stream, x, x_cs, y, y_cs, s, s_stride, N, H, W, C, up)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_resample_modulate_ragged(const float* x, int x_cs, float* y, int y_cs, const float* s, int s_stride,
+                                           const int32_t* valid_w, int N, int H, int W, int C, void* stream) {
+    MN_REQUIRE(x && y && valid_w && N > 0 && H > 0 && W > 0 && C > 0, "mn_resample_modulate_ragged: bad args");
+    MN_REQUIRE((C & 3) == 0 && (x_cs & 3) == 0 && (y_cs & 3) == 0, "mn_resample_modulate_ragged: channels must be multiples of 4");
+    MN_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)y & 15) == 0 && (!s || ((s_stride & 3) == 0 && ((uintptr_t)s & 15) == 0)),
+               "mn_resample_modulate_ragged: x, y and s must be 16B aligned (s_stride a multiple of 4)");
+    const int64_t total = (int64_t)N * 2 * H * 2 * W * (C >> 2);
+    MN_REQUIRE(total < (1ll << 31), "tensor too large for 32-bit indexing");
+    MN_CUDA_CHECK((mn_launch(resample_up2_kernel<true>, dim3((unsigned)mn_cdiv64((int64_t)N * H * mn_cdiv(W, UP_RX) * (C >> 2), 256)), dim3(256), 0,
+                             (cudaStream_t)stream, x, x_cs, y, y_cs, s, s_stride, N, H, W, C, valid_w)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

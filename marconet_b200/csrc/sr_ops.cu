@@ -292,19 +292,23 @@ __global__ void window_scatter_kernel(const float* __restrict__ feat, int feat_c
 // (fp32 multiply, truncation toward zero).  Phase 2: one thread per column finds its owner = the LAST character in
 // program order whose window covers it (networks.py:448,481).  An empty window (the reference dies on the empty slice
 // at networks.py:443) raises bit 1 of *err and is replaced by a zero-width window so that no consumer reads out of bounds.
+// line_w (mn_char_windows_ragged): line b is the first line_w[b] columns of the W-wide map; its centres and clipping use line_w[b]
+// and its owner row holds -1 from column line_w[b] on.
 __global__ void char_windows_kernel(const float* __restrict__ locs, int locs_stride, const int32_t* __restrict__ line_first,
                                     int W, int half, mn_window* __restrict__ win, int32_t* __restrict__ valid,
-                                    int32_t* __restrict__ owner, int32_t* __restrict__ err) {
+                                    int32_t* __restrict__ owner, int32_t* __restrict__ err, const int32_t* __restrict__ line_w) {
     mn_pdl_prologue();
     extern __shared__ int32_t sw[];            // [n][2] = x1, x2 of this line's characters
     const int b = blockIdx.x;
     const int first = line_first[b], n = line_first[b + 1] - first;
+    const int Wb = line_w ? min(line_w[b], W) : W;   // clamped to the map: the values live on the device, unchecked by the host wrapper
+                                                     // (TSPSRNet validates its widths on the host before they are uploaded)
     for (int c = threadIdx.x; c < n; c += blockDim.x) {
-        const int center = __float2int_rz(__fmul_rn(locs[(size_t)b * locs_stride + 2 * c], (float)W));
+        const int center = __float2int_rz(__fmul_rn(locs[(size_t)b * locs_stride + 2 * c], (float)Wb));
         int x1 = center < half ? 0 : center - half;
-        int x2 = center + half > W ? W : center + half;
+        int x2 = center + half > Wb ? Wb : center + half;
         int wv = x2 - x1;
-        if (wv <= 0 || x1 >= W) { atomicOr(err, 2); x1 = 0; x2 = 0; wv = 0; }
+        if (wv <= 0 || x1 >= Wb) { atomicOr(err, 2); x1 = 0; x2 = 0; wv = 0; }
         mn_window w;
         w.line = b; w.x1 = x1; w.x2 = x2; w.y1 = half - wv / 2;
         win[first + c] = w;
@@ -498,7 +502,18 @@ extern "C" int mn_char_windows(const float* locs, int locs_stride, const int32_t
     MN_REQUIRE(locs && line_first && win && valid && owner && err, "mn_char_windows: null pointer");
     MN_REQUIRE(B > 0 && W > 0 && half > 0 && max_chars >= 0 && max_chars <= 4096, "mn_char_windows: bad dims");
     MN_CUDA_CHECK((mn_launch(char_windows_kernel, dim3(B), dim3(256), (size_t)max_chars * 2 * sizeof(int32_t), (cudaStream_t)stream,
-                             locs, locs_stride, line_first, W, half, win, valid, owner, err)));
+                             locs, locs_stride, line_first, W, half, win, valid, owner, err, (const int32_t*)nullptr)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_char_windows_ragged(const float* locs, int locs_stride, const int32_t* line_first, const int32_t* line_w, int B,
+                                      int max_chars, int W, int half, mn_window* win, int32_t* valid, int32_t* owner, int32_t* err,
+                                      void* stream) {
+    MN_REQUIRE(locs && line_first && line_w && win && valid && owner && err, "mn_char_windows_ragged: null pointer");
+    MN_REQUIRE(B > 0 && W > 0 && half > 0 && max_chars >= 0 && max_chars <= 4096, "mn_char_windows_ragged: bad dims");
+    MN_CUDA_CHECK((mn_launch(char_windows_kernel, dim3(B), dim3(256), (size_t)max_chars * 2 * sizeof(int32_t), (cudaStream_t)stream,
+                             locs, locs_stride, line_first, W, half, win, valid, owner, err, line_w)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -34,7 +34,7 @@ SQRT2 = math.sqrt(2.0)
 
 class _CapturedCall:
     """One module forward for one input signature, recorded into a CUDA graph: static inputs, a device error flag, static outputs."""
-    __slots__ = ("graph", "inputs", "outputs", "flag", "pinned", "h2d_done")
+    __slots__ = ("graph", "inputs", "outputs", "flag", "pinned", "h2d_done", "keep")
 
 
 def _copy_sources(ent, sources):
@@ -88,11 +88,12 @@ class _PackedModule(nn.Module):
         self._mg = None
         self._mg_hits = {}
 
-    def _mg_run(self, key, sources, fn, fill=None):
+    def _mg_run(self, key, sources, fn, fill=None, keep=None):
         """Replay (or, on the second sighting of ``key``, record) ``fn(*static_inputs) -> tuple of tensors``.  ``sources`` are the
         caller's tensors (device or host) that are copied into the static inputs -- or, with ``fill``, (shape, dtype) specs of the
-        static inputs, which ``fill(static_inputs)`` then writes.  Returns the captured call (static outputs, flag) or None when
-        this call must run eagerly."""
+        static inputs, which ``fill(static_inputs)`` then writes.  ``keep``: device tensors that ``fn`` reads besides its inputs
+        (tables from a module cache): the recording holds them for as long as it lives, since its kernels hold their addresses.
+        Returns the captured call (static outputs, flag) or None when this call must run eagerly."""
         if not ops.graphs_allowed():
             return None
         import collections
@@ -108,6 +109,8 @@ class _PackedModule(nn.Module):
             if n < 2:
                 return None
             ent = self._mg_capture(sources, fn, fill)
+            if ent != "eager":
+                ent.keep = keep
             self._mg[key] = ent
             self._mg_hits.pop(key, None)
             while len(self._mg) > self._MG_LIMIT:
@@ -135,7 +138,7 @@ class _PackedModule(nn.Module):
         dev = next(self.parameters()).device
         try:
             ent = _CapturedCall()
-            ent.pinned = ent.h2d_done = None
+            ent.pinned = ent.h2d_done = ent.keep = None
             if fill is not None:
                 ent.inputs = [torch.empty(tuple(shape), dtype=dtype, device=dev) for shape, dtype in sources]
                 fill(ent.inputs)
@@ -600,25 +603,34 @@ def _two(pk, x, valid_w=None):
     return ops.conv2d(t, pk[1][0], 3, 3, pad=(1, 1), bias=pk[1][1], valid_w=valid_w)
 
 
-def _char_windows_np(arr, counts, width, half):
+def _up2(x, valid_w, out=None):
+    """Bilinear x2 of the SR decoder; ``valid_w`` (device int32 [N]) makes it ragged (mn_resample_modulate_ragged)."""
+    if valid_w is None:
+        return ops.resample_modulate(x, None, up=True, out=out)
+    return ops.resample_up2_ragged(x, valid_w, out=out)
+
+
+def _char_windows_np(arr, counts, width, half, line_w=None):
     """Vectorised core of char_windows.  ``arr``: fp32 numpy [B, >= 2*n].  The centre is the fp32 product truncated toward zero,
     exactly like ``(locs[b][2*c] * W).int()`` (numpy float32 array x np.float32 scalar is an fp32 multiply; astype(int32) truncates).
+    ``line_w``: per-line widths (each <= width) of a ragged batch -- line b's centres and clipping use line_w[b], as the reference
+    does on that line's own tensor, and its owner row stays -1 from column line_w[b] on.
     Returns (wins int32 [Nc,4] = (line, x1, x2, y1), valid int32 [Nc], owner int32 [B, W])."""
     import numpy as np
     nc = sum(counts)
     wins = np.empty((nc, 4), np.int32)
     valid = np.empty((nc,), np.int32)
     owner = np.full((len(counts), width), -1, np.int32)
-    w32 = np.float32(width)
     i = 0
     for b, n in enumerate(counts):
         if n == 0:
             continue
-        cen = (arr[b, 0:2 * n:2].astype(np.float32, copy=False) * w32).astype(np.int32)
+        wb = width if line_w is None else int(line_w[b])
+        cen = (arr[b, 0:2 * n:2].astype(np.float32, copy=False) * np.float32(wb)).astype(np.int32)
         x1 = np.where(cen < half, 0, cen - half)
-        x2 = np.where(cen + half > width, width, cen + half)
+        x2 = np.where(cen + half > wb, wb, cen + half)
         wv = x2 - x1
-        bad = np.nonzero((wv <= 0) | (x1 >= width))[0]
+        bad = np.nonzero((wv <= 0) | (x1 >= wb))[0]
         if bad.size:
             c = int(bad[0])
             raise RuntimeError(f"character {c} of line {b}: empty window (centre {int(cen[c])}); the reference "
@@ -634,14 +646,15 @@ def _char_windows_np(arr, counts, width, half):
     return wins, valid, owner
 
 
-def char_windows(locs_host, counts, width, half):
+def char_windows(locs_host, counts, width, half, line_w=None):
     """Bit-exact restatement of the window integers of reference networks.py:426-441 / :460-474.
 
     ``locs_host`` is a CPU fp32 tensor [B, 2*n]; the centre is ``(locs[b][2c] * W).int()`` (fp32
     multiply, truncation).  Returns (windows [(line,x1,x2,y1)], valid widths, owner[b][x]) with
-    "last character in program order wins" ownership (networks.py:448,481).
+    "last character in program order wins" ownership (networks.py:448,481).  ``line_w``: per-line
+    widths of a ragged batch (see _char_windows_np).
     """
-    wins, valid, owner = _char_windows_np(locs_host.detach().to(torch.float32).contiguous().numpy(), counts, width, half)
+    wins, valid, owner = _char_windows_np(locs_host.detach().to(torch.float32).contiguous().numpy(), counts, width, half, line_w)
     return [tuple(int(v) for v in r) for r in wins], [int(v) for v in valid], owner.tolist()
 
 
@@ -669,6 +682,7 @@ class TSPSRNet(_PackedModule):
         self.conv_64_fuse = nn.Sequential(ResTextBlockV2(2 * d, d))
         self.dim = d
         self._line_first_cache = {}
+        self._widths_cache = {}
 
     def _pack(self, device):
         pk = {}
@@ -701,9 +715,45 @@ class TSPSRNet(_PackedModule):
             self._line_first_cache[key] = t
         return t
 
-    def _fuse(self, pk, lvl, feat, prior, locs, counts, half):
+    def _valid_widths(self, widths, dev):
+        """Device int32 [5, B] valid widths of a ragged batch at each level: rows = widths, widths/2, widths/4 (32 rows),
+        2*widths (64 rows), 4*widths (128 rows).  Cached (bounded; a recorded graph that reads a table holds it itself, see
+        _forward_graphed)."""
+        key = (tuple(widths), dev)
+        t = self._widths_cache.get(key)
+        if t is None:
+            w = torch.tensor(widths, dtype=torch.int32)
+            t = torch.stack([w, w // 2, w // 4, 2 * w, 4 * w]).contiguous().to(dev)
+            if len(self._widths_cache) > 64:
+                self._widths_cache.clear()
+            self._widths_cache[key] = t
+        return t
+
+    @staticmethod
+    def _check_widths(widths, lq):
+        """None when the call is not ragged (no widths, or every width equals the canvas): today's code path, bit for bit."""
+        if widths is None:
+            return None
+        if lq.dim() != 4:
+            raise RuntimeError("TSPSRNet: widths needs a batched lq [B, 3, H, W]")
+        bsz, wc = lq.shape[0], lq.shape[-1]
+        widths = [int(v) for v in (widths.tolist() if isinstance(widths, torch.Tensor) else widths)]
+        if len(widths) != bsz:
+            raise ValueError(f"TSPSRNet: {len(widths)} widths for {bsz} lines")
+        for b, v in enumerate(widths):
+            if v < 4 or v % 4 or v > wc:
+                raise ValueError(f"TSPSRNet: widths[{b}] = {v} must be a positive multiple of 4 no larger than the canvas ({wc}): the "
+                                 f"stride-2 convs and the x2 up-samples of the reference need W % 4 == 0")
+        if all(v == wc for v in widths):
+            return None
+        if wc % 4:
+            raise ValueError(f"TSPSRNet: a ragged batch needs a canvas width that is a multiple of 4, got {wc}")
+        return tuple(widths)
+
+    def _fuse(self, pk, lvl, feat, prior, locs, counts, half, line_w=None):
         """Per-character prior fusion of one level as ONE ragged batch (reference loops :425-448/:459-481).
-        ``locs`` is a CPU tensor (eager checks) or, inside ops.deferred_checks, the device tensor itself."""
+        ``locs`` is a CPU tensor (eager checks) or, inside ops.deferred_checks, the device tensor itself.
+        ``line_w``: (host widths, device int32 [B]) of a ragged batch at this level."""
         dev = feat.device
         b, h, w, c = feat.shape
         nc = sum(counts)
@@ -712,10 +762,14 @@ class TSPSRNet(_PackedModule):
         wp = 2 * half
         flag = ops.deferred_flag()
         if flag is not None and locs.is_cuda:
-            win_dev, valid_dev, owner_dev = ops.char_windows(locs, self._line_first(counts, dev), counts, w, half, flag)
+            if line_w is None:
+                win_dev, valid_dev, owner_dev = ops.char_windows(locs, self._line_first(counts, dev), counts, w, half, flag)
+            else:
+                win_dev, valid_dev, owner_dev = ops.char_windows_ragged(locs, self._line_first(counts, dev), line_w[1], counts, w, half, flag)
             vw = valid_dev                                # widths are not known on the host: always mask
         else:
-            wins, valid, owner = _char_windows_np(locs.numpy() if isinstance(locs, torch.Tensor) else locs, counts, w, half)
+            wins, valid, owner = _char_windows_np(locs.numpy() if isinstance(locs, torch.Tensor) else locs, counts, w, half,
+                                                  None if line_w is None else line_w[0])
             win_dev = torch.from_numpy(wins).to(dev, non_blocking=True)
             valid_dev = torch.from_numpy(valid).to(dev, non_blocking=True)
             owner_dev = torch.from_numpy(owner).to(dev, non_blocking=True)
@@ -745,24 +799,32 @@ class TSPSRNet(_PackedModule):
             total += v.shape[0]
         return torch.as_strided(views[0], (total,) + tuple(views[0].shape[1:]), views[0].stride())
 
-    def _trunk(self, pk, lq):
-        """The LR trunk (reference networks.py:412-416): depends on the LR line only, not on the priors."""
+    def _trunk(self, pk, lq, widths=None):
+        """The LR trunk (reference networks.py:412-416): depends on the LR line only, not on the priors.
+        ``widths``: per-line widths of a ragged batch (see forward); every activation is zero beyond its line's valid width."""
         dev, d = lq.device, self.dim
         bsz = lq.shape[0]
         x = ops.nchw_to_nhwc(lq.float())
         h, w = x.shape[1], x.shape[2]
+        vw = [None] * 3
+        if widths is not None:
+            for b, wb in enumerate(widths):          # line b is lq[b, :, :, :wb]: what lies beyond is the zero padding of its convs
+                if wb < w:
+                    x[b, :, wb:].zero_()
+            vw = list(self._valid_widths(widths, dev)[:3])
         cat32 = torch.empty((bsz, h, w, d + d // 4), dtype=torch.float32, device=dev)        # [up(sq_f_16) | lq_f_32]
         cat16 = torch.empty((bsz, h // 2, w // 2, d + d // 2), dtype=torch.float32, device=dev)  # [up(lq_f_8) | lq_f_16]
         f32v, f16v = cat32[..., d:], cat16[..., d:]
-        ops.conv2d(x, pk["first_32"][0], 3, 3, pad=(1, 1), bias=pk["first_32"][1], act=ACT_LRELU02, out=f32v)
-        ops.conv2d(f32v, pk["first_16"][0], 3, 3, stride=(2, 2), pad=(1, 1), bias=pk["first_16"][1], act=ACT_LRELU02, out=f16v)
+        ops.conv2d(x, pk["first_32"][0], 3, 3, pad=(1, 1), bias=pk["first_32"][1], act=ACT_LRELU02, out=f32v, valid_w=vw[0])
+        ops.conv2d(f32v, pk["first_16"][0], 3, 3, stride=(2, 2), pad=(1, 1), bias=pk["first_16"][1], act=ACT_LRELU02, out=f16v,
+                   valid_w=vw[1])
         p8 = pk["conv_first_8"]
-        t = ops.conv2d(f16v, p8[0][0], 3, 3, stride=(2, 2), pad=(1, 1), bias=p8[0][1], act=ACT_LRELU02)
-        f8 = ops.conv2d(t, p8[1][0], 3, 3, pad=(1, 1), bias=p8[1][1])
-        ops.resample_modulate(f8, None, up=True, out=cat16[..., :d])
-        s16 = _two(pk["conv_body_16"], cat16)
-        ops.resample_modulate(s16, None, up=True, out=cat32[..., :d])
-        s32 = _two(pk["conv_body_32"], cat32)
+        t = ops.conv2d(f16v, p8[0][0], 3, 3, stride=(2, 2), pad=(1, 1), bias=p8[0][1], act=ACT_LRELU02, valid_w=vw[2])
+        f8 = ops.conv2d(t, p8[1][0], 3, 3, pad=(1, 1), bias=p8[1][1], valid_w=vw[2])
+        _up2(f8, vw[2], cat16[..., :d])
+        s16 = _two(pk["conv_body_16"], cat16, vw[1])
+        _up2(s16, vw[1], cat32[..., :d])
+        s32 = _two(pk["conv_body_32"], cat32, vw[0])
         return s32
 
     @torch.no_grad()
@@ -774,16 +836,24 @@ class TSPSRNet(_PackedModule):
             return self._trunk(self._get_packed(lq.device), lq)
 
     @torch.no_grad()
-    def forward(self, lq, priors64, priors32, locs, _trunk=None):
+    def forward(self, lq, priors64, priors32, locs, _trunk=None, *, widths=None):
+        """``widths`` (extension; the reference module has no such argument): per-line LQ widths of a ragged batch, each a multiple
+        of 4 no larger than ``lq.shape[-1]``.  Line b is then ``lq[b, :, :, :widths[b]]`` exactly as the reference would run it
+        alone -- its ``locs`` are normalised by widths[b] and every convolution sees the zero padding of that width -- and its
+        output occupies columns [0, 4 * widths[b]) of the returned canvas, zero beyond.  None (or all widths equal to the canvas):
+        the unchanged code path."""
         self._need_cuda(lq, "TSPSRNet")
+        widths = self._check_widths(widths, lq)
+        if widths is not None and _trunk is not None:
+            raise ValueError("TSPSRNet: widths and a precomputed _trunk cannot be combined")
         with ops.on_device(lq):
-            ent = self._forward_graphed(lq, priors64, priors32, locs) if _trunk is None else None
+            ent = self._forward_graphed(lq, priors64, priors32, locs, widths) if _trunk is None else None
             if ent is not None:
                 ops.raise_deferred(int(ent.flag.item()))      # the eager path raises on an empty window before launching; here after
                 return ent.outputs[0].clone()
-            return self._forward(lq, priors64, priors32, locs, _trunk)
+            return self._forward(lq, priors64, priors32, locs, _trunk, widths=widths)
 
-    def _forward_graphed(self, lq, priors64, priors32, locs):
+    def _forward_graphed(self, lq, priors64, priors32, locs, widths=None):
         """Module-level CUDA graph of the decoder for this (lines, characters-per-line) signature; None -> run eagerly."""
         if not ops.graphs_allowed() or lq.dim() != 4 or len(priors64) != len(priors32) or not isinstance(locs, torch.Tensor) or locs.dim() != 2:
             return None
@@ -816,12 +886,16 @@ class TSPSRNet(_PackedModule):
             l64, l32, o = [], [], 0
             for n in counts:
                 l64.append(p64_[o:o + n].permute(0, 3, 1, 2)); l32.append(p32_[o:o + n].permute(0, 3, 1, 2)); o += n
-            return (self._forward(lq_, l64[:len(priors64)], l32[:len(priors32)], locs_, None, _trunk_side=self._mg_side(lq_.device)),)
+            return (self._forward(lq_, l64[:len(priors64)], l32[:len(priors32)], locs_, None, _trunk_side=self._mg_side(lq_.device),
+                                  widths=widths),)
 
-        key = ("sr", tuple(lq.shape), tuple(counts), len(priors64), tuple(locs.shape), lq.device)
-        return self._mg_run(key, specs, run, fill)
+        # the widths are baked into the recording (cached device tensors): a recording for one widths tuple never replays for another,
+        # and the recording keeps its width table alive -- the cache may drop it while the graph still reads it
+        key = ("sr", tuple(lq.shape), tuple(counts), len(priors64), tuple(locs.shape), lq.device, widths)
+        keep = None if widths is None else (self._valid_widths(widths, lq.device),)
+        return self._mg_run(key, specs, run, fill, keep=keep)
 
-    def _forward(self, lq, priors64, priors32, locs, _trunk, _trunk_side=None):
+    def _forward(self, lq, priors64, priors32, locs, _trunk, _trunk_side=None, widths=None):
         """``_trunk_side`` = (stream, split-K scratch): compute the LR trunk on that stream while this one converts the 32-px priors
         (they are independent: networks.py:412-416 vs :424); joined before the first fuse stage.  Used inside recorded graphs."""
         dev = lq.device
@@ -838,6 +912,11 @@ class TSPSRNet(_PackedModule):
         else:
             locs_host = locs.detach().to("cpu", torch.float32).contiguous()      # the one device->host round trip (reference: ~6 per character)
 
+        vw = [None] * 5
+        lw32 = lw64 = None
+        if widths is not None:
+            vw = list(self._valid_widths(widths, dev))
+            lw32, lw64 = (widths, vw[0]), (tuple(2 * v for v in widths), vw[3])
         trunk_done = None
         if _trunk is not None:
             s32 = _trunk
@@ -846,32 +925,32 @@ class TSPSRNet(_PackedModule):
             main = torch.cuda.current_stream(dev)
             side.wait_stream(main)
             with torch.cuda.stream(side), ops.use_workspace(scratch):
-                s32 = self._trunk(pk, lq)
+                s32 = self._trunk(pk, lq, widths)
                 trunk_done = torch.cuda.Event()
                 trunk_done.record(side)
             s32.record_stream(main)
         else:
-            s32 = self._trunk(pk, lq)
+            s32 = self._trunk(pk, lq, widths)
 
         if sum(counts) > 0:
             p32 = _two(pk["conv_32_to256"], self._gather_priors(priors32, 512, 32))
             if trunk_done is not None:
                 torch.cuda.current_stream(dev).wait_event(trunk_done)
-            s32 = self._fuse(pk, 32, s32, p32, locs_host, counts, 16)
+            s32 = self._fuse(pk, 32, s32, p32, locs_host, counts, 16, lw32)
 
-        u = ops.resample_modulate(s32, None, up=True)
-        x, mr = ops.conv2d(u, pk["up_1"][0], 3, 3, pad=(1, 1), bias=pk["up_1"][1], act=ACT_LRELU02, gn_stats=True)
-        x = _res_block(pk["up_res"], x, mr1=mr)
-        s64 = ops.conv2d(x, pk["up_4"][0], 3, 3, pad=(1, 1), bias=pk["up_4"][1])
+        u = _up2(s32, vw[0])
+        x, mr = ops.conv2d(u, pk["up_1"][0], 3, 3, pad=(1, 1), bias=pk["up_1"][1], act=ACT_LRELU02, gn_stats=True, valid_w=vw[3])
+        x = _res_block(pk["up_res"], x, vw[3], mr1=mr)
+        s64 = ops.conv2d(x, pk["up_4"][0], 3, 3, pad=(1, 1), bias=pk["up_4"][1], valid_w=vw[3])
 
         if sum(counts) > 0:
-            s64 = self._fuse(pk, 64, s64, self._gather_priors(priors64, d, 64), locs_host, counts, 32)
+            s64 = self._fuse(pk, 64, s64, self._gather_priors(priors64, d, 64), locs_host, counts, 32, lw64)
 
-        x = ops.conv2d(s64, pk["fin_0"][0], 3, 3, pad=(1, 1), bias=pk["fin_0"][1], act=ACT_LRELU02)
-        u = ops.resample_modulate(x, None, up=True)
-        x, mr = ops.conv2d(u, pk["fin_3"][0], 3, 3, pad=(1, 1), bias=pk["fin_3"][1], act=ACT_LRELU02, gn_stats=True)
-        x = _res_block(pk["fin_res"], x, mr1=mr)
-        out = ops.conv2d(x, pk["fin_6"][0], 3, 3, pad=(1, 1), bias=pk["fin_6"][1], act=ACT_TANH)
+        x = ops.conv2d(s64, pk["fin_0"][0], 3, 3, pad=(1, 1), bias=pk["fin_0"][1], act=ACT_LRELU02, valid_w=vw[3])
+        u = _up2(x, vw[3])
+        x, mr = ops.conv2d(u, pk["fin_3"][0], 3, 3, pad=(1, 1), bias=pk["fin_3"][1], act=ACT_LRELU02, gn_stats=True, valid_w=vw[4])
+        x = _res_block(pk["fin_res"], x, vw[4], mr1=mr)
+        out = ops.conv2d(x, pk["fin_6"][0], 3, 3, pad=(1, 1), bias=pk["fin_6"][1], act=ACT_TANH, valid_w=vw[4])
         return ops.as_nchw_view(out)
 
 

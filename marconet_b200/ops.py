@@ -575,6 +575,29 @@ def char_windows(locs_dev, line_first_dev, counts, width, half, flag):
     return win, valid, owner
 
 
+def char_windows_ragged(locs_dev, line_first_dev, line_w_dev, counts, width, half, flag):
+    """mn_char_windows for lines of their own widths: line b's centres and clipping use ``line_w_dev[b]`` (device int32 [B], each
+    <= ``width``, the width of the owner map); owner is -1 from column line_w[b] on.  Returns (win, valid, owner) as char_windows."""
+    global LAUNCHES
+    _require_cuda(locs_dev, "locs")
+    if locs_dev.dtype != torch.float32 or locs_dev.dim() != 2 or locs_dev.stride(1) != 1:
+        raise RuntimeError("char_windows_ragged: locs must be fp32 [B, 2n] with unit inner stride")
+    b, nc = len(counts), sum(counts)
+    if locs_dev.shape[0] < b or (counts and locs_dev.shape[1] < 2 * max(counts)):
+        raise RuntimeError("char_windows_ragged: locs has fewer entries than characters")
+    if line_w_dev.dtype != torch.int32 or not line_w_dev.is_cuda or line_w_dev.numel() != b or not line_w_dev.is_contiguous():
+        raise RuntimeError("char_windows_ragged: line_w must be a contiguous int32 CUDA tensor with one width per line")
+    dev = locs_dev.device
+    win = torch.empty((nc, 4), dtype=torch.int32, device=dev)
+    valid = torch.empty((nc,), dtype=torch.int32, device=dev)
+    owner = torch.empty((b, width), dtype=torch.int32, device=dev)
+    _lib.check(_lib.load().mn_char_windows_ragged(_ptr(locs_dev), locs_dev.stride(0), _ptr(line_first_dev), _ptr(line_w_dev), b, max(counts),
+                                                  width, half, _ptr(win), _ptr(valid), _ptr(owner), _ptr(flag), _stream()),
+               "mn_char_windows_ragged")
+    LAUNCHES += 1
+    return win, valid, owner
+
+
 def select_text(emb, labels_dev, s, n, l):
     """emb: [classes, C]; labels_dev: int64 [n*l] on device; s: [n, C] view (row stride s.stride(0)) or None."""
     global LAUNCHES
@@ -629,6 +652,23 @@ def resample_modulate(x, s=None, up=False, out=None):
     _, _, _, _, y_cs = nhwc_info(y, "out")
     _lib.check(_lib.load().mn_resample_modulate(_ptr(x), x_cs, _ptr(y), y_cs, _ptr(s), 0 if s is None else s.stride(0),
                                                 n, h, w, c, 1 if up else 0, _stream()), "mn_resample_modulate")
+    LAUNCHES += 1
+    return y
+
+
+def resample_up2_ragged(x, valid_w, s=None, out=None):
+    """Bilinear x2 of a ragged batch (mn_resample_modulate_ragged): sample n is the first ``valid_w[n]`` columns of x (device int32
+    [N]); the output is zero from column 2*valid_w[n] on.  ``s``: optional per-sample channel scale [N, C] view."""
+    global LAUNCHES
+    n, h, w, c, x_cs = nhwc_info(x, "x")
+    if valid_w.dtype != torch.int32 or not valid_w.is_cuda or valid_w.numel() != n or not valid_w.is_contiguous():
+        raise RuntimeError("resample_up2_ragged: valid_w must be a contiguous int32 CUDA tensor with one width per sample")
+    y = out if out is not None else torch.empty((n, 2 * h, 2 * w, c), dtype=torch.float32, device=x.device)
+    yn, yh, yw, yc, y_cs = nhwc_info(y, "out")
+    if (yn, yh, yw, yc) != (n, 2 * h, 2 * w, c):
+        raise RuntimeError(f"resample_up2_ragged: out has shape {tuple(y.shape)}, expected {(n, 2 * h, 2 * w, c)}")
+    _lib.check(_lib.load().mn_resample_modulate_ragged(_ptr(x), x_cs, _ptr(y), y_cs, _ptr(s), 0 if s is None else s.stride(0), _ptr(valid_w),
+                                                       n, h, w, c, _stream()), "mn_resample_modulate_ragged")
     LAUNCHES += 1
     return y
 

@@ -272,8 +272,63 @@ def _as_image(img, i):
     return img
 
 
+def _device_images(ids, imgs, dev):
+    """The batch's images on the device: CUDA images as they are (dense pixels), host images through ONE pinned host->device
+    copy.  Returns {image index: uint8 CUDA view}."""
+    dimg, host = {}, []
+    for i in ids:
+        t = imgs[i]
+        if not t.is_cuda:
+            host.append(i)
+            continue
+        t = t.to(dev)
+        if t.stride(2) != 1 or t.stride(1) != 3:
+            t = t.contiguous()
+        dimg[i] = t
+    if host:
+        nbytes = sum(imgs[i].numel() for i in host)
+        stage, ev = _staging(nbytes, dev)
+        o = 0
+        for i in host:
+            stage[o:o + imgs[i].numel()].view(imgs[i].shape).copy_(imgs[i])
+            o += imgs[i].numel()
+        dbuf = stage[:nbytes].to(dev, non_blocking=True)
+        ev.record()
+        o = 0
+        for i in host:
+            dimg[i] = dbuf[o:o + imgs[i].numel()].view(imgs[i].shape)
+            o += imgs[i].numel()
+    return dimg
+
+
+def whole_line_width(h, w, canvas=512):
+    """(lq_w, Wc): the LQ width of an h x w image (cv2's dsize for fx = fy = 32/h) and the width of its decoder line.  A line that
+    fits the canvas keeps the 512 canvas; a wider one decodes in one piece at Wc = 4*ceil(lq_w/4) (the reference's stride-2 convs
+    and x2 up-samples need W % 4 == 0)."""
+    from .ops import round_half_even
+    lq_w = round_half_even(w * (32 / h))
+    return lq_w, (canvas if lq_w <= canvas else 4 * (-(-lq_w // 4)))
+
+
+def pack_by_columns(widths, max_lines, canvas=512):
+    """Decoder batches of lines with their own widths: lines sorted by width, a batch of k lines only while
+    k * (its widest line) <= max_lines * canvas (peak activation memory stays that of max_lines canvas-wide lines); a line wider
+    than that forms a batch of its own.  Returns lists of indices into ``widths``."""
+    order = sorted(range(len(widths)), key=lambda j: widths[j])
+    batches, cur = [], []
+    for j in order:
+        if cur and (len(cur) + 1) * widths[j] > max_lines * canvas:
+            batches.append(cur)
+            cur = []
+        cur.append(j)
+    if cur:
+        batches.append(cur)
+    return batches
+
+
 @torch.no_grad()
-def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, context=16, skip_invalid=False, to_host=False):
+def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, context=16, skip_invalid=False, to_host=False,
+                   whole_lines=False):
     """Text-line images of any sizes end to end, batched: the flow of restore_image for every image, each cut into crops that
     fit the 32x512 LQ canvas (plan_segments) and every crop of every image run as one line of a batch of at most ``max_lines``.
 
@@ -285,7 +340,17 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
     TSPSRNet, a synchronisation and ops.poll_range (the batch re-runs, at most 3 times, when a layer was re-routed for fp16
     range), then one stitch kernel (mn_postprocess_sr_u8_pieces) into the images' outputs.
     Returns one dict per image: sr_u8 (uint8 [128, W_i, 3], W_i = round_half_even(w_i*128/h_i), on the device, or numpy through
-    one pinned device->host copy with ``to_host``) and segments (the plan).  A single-segment image gives restore_image's bytes."""
+    one pinned device->host copy with ``to_host``) and segments (the plan).  A single-segment image gives restore_image's bytes.
+
+    ``whole_lines=True`` decodes every line wider than the canvas (lq_w = round_half_even(w*32/h) > 512) in ONE piece, so that no
+    column sees a crop edge: its decoder LQ is the cubic resize of the whole image to height 32, zero-filled to
+    Wc = 4*ceil(lq_w/4) columns, its locs are boxes_to_locs(boxes, h, Wc), and its output is columns
+    [0, min(round_half_even(w*128/h), 4*Wc)) of TSPSRNet(lq, [p64], [p32], locs) -- the reference module run on the whole line.
+    The encoder, whose patch and positional embeddings are sized for the 32x512 canvas, still runs on the plan's crops, and each
+    character's prior takes the style w of the crop that owns it.  Lines that fit the canvas are computed as without the flag.
+    Decoder lines of different widths share a batch (TSPSRNet's ``widths``); a batch holds k lines only while
+    k * (its widest Wc) <= max_lines * 512.  Per batch: one host->device copy, one crop kernel for the encoder crops, one for
+    the decoder lines, the encoder, one TSPGAN call, one ragged TSPSRNet call, the fp16-range re-run, one stitch kernel."""
     from . import ops
     n = len(images)
     if not (len(labels) == len(boxes) == n):
@@ -315,6 +380,8 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
     valid = [i for i in range(n) if plans[i] is not None]
     if not valid:
         return results
+    if whole_lines:
+        return _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, results, max_lines, to_host, dev)
     with torch.cuda.device(dev):
         layout, total = {}, 0
         for i in valid:
@@ -326,30 +393,7 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
         lines = [(i, k) for i in valid for k in range(len(plans[i]))]
         for b0 in range(0, len(lines), max_lines):
             batch = lines[b0:b0 + max_lines]
-            dimg = {}
-            host = []
-            for i in dict.fromkeys(i for i, _ in batch):
-                t = imgs[i]
-                if not t.is_cuda:
-                    host.append(i)
-                    continue
-                t = t.to(dev)
-                if t.stride(2) != 1 or t.stride(1) != 3:
-                    t = t.contiguous()
-                dimg[i] = t
-            if host:
-                nbytes = sum(imgs[i].numel() for i in host)
-                stage, ev = _staging(nbytes, dev)
-                o = 0
-                for i in host:
-                    stage[o:o + imgs[i].numel()].view(imgs[i].shape).copy_(imgs[i])
-                    o += imgs[i].numel()
-                dbuf = stage[:nbytes].to(dev, non_blocking=True)
-                ev.record()
-                o = 0
-                for i in host:
-                    dimg[i] = dbuf[o:o + imgs[i].numel()].view(imgs[i].shape)
-                    o += imgs[i].numel()
+            dimg = _device_images(dict.fromkeys(i for i, _ in batch), imgs, dev)
             segs = [plans[i][k] for i, k in batch]
             lq, _ = ops.preprocess_lq_crops([(dimg[i], s.crop[0], s.crop[1]) for (i, _), s in zip(batch, segs)])
             counts = [s.chars[1] - s.chars[0] for s in segs]
@@ -387,6 +431,64 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
             pinned.copy_(flat, non_blocking=True)
             torch.cuda.current_stream(dev).synchronize()
             outs = {i: pinned[o:o + 128 * wd * 3].view(128, wd, 3).numpy() for i, (o, wd, _) in layout.items()}
+    for i in valid:
+        results[i] = dict(sr_u8=outs[i], segments=plans[i])
+    return results
+
+
+def _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, results, max_lines, to_host, dev):
+    """restore_images(whole_lines=True) after validation: one decoder line per image (see restore_images)."""
+    from . import ops
+    with torch.cuda.device(dev):
+        geo = {i: whole_line_width(imgs[i].shape[0], imgs[i].shape[1]) for i in valid}
+        layout, total = {}, 0
+        for i in valid:
+            h, w = imgs[i].shape[:2]
+            wc = geo[i][1]
+            width = min(ops.round_half_even(w * (128 / h)), 4 * wc)
+            layout[i] = (total, width)
+            total += 128 * width * 3
+        flat = torch.empty(total, dtype=torch.uint8, device=dev)
+        outs = {i: flat[o:o + 128 * wd * 3].view(128, wd, 3) for i, (o, wd) in layout.items()}
+        for bidx in pack_by_columns([geo[i][1] for i in valid], max_lines):
+            batch = [valid[j] for j in bidx]
+            dimg = _device_images(batch, imgs, dev)
+            crops = [(i, s) for i in batch for s in plans[i]]              # encoder crops, 512 canvas
+            lq_enc, _ = ops.preprocess_lq_crops([(dimg[i], s.crop[0], s.crop[1]) for i, s in crops])
+            widths = [geo[i][1] for i in batch]
+            canvas = max(widths)
+            if canvas == 512:                 # only lines that fit: each is its single crop, exactly as without whole_lines
+                lq = lq_enc
+            else:
+                lq, _ = ops.preprocess_lq_crops([(dimg[i], 0, imgs[i].shape[1]) for i in batch], out_w=canvas)
+            counts = [len(labs[i]) for i in batch]
+            owner = []                                                   # encoder crop (row of lq_enc) of every character
+            c0 = 0
+            for i in batch:
+                for s in plans[i]:
+                    owner += [c0] * (s.chars[1] - s.chars[0])
+                    c0 += 1
+            owner_t = torch.tensor(owner, dtype=torch.long).to(dev, non_blocking=True)
+            lab_all = torch.tensor([v for i in batch for v in labs[i]], dtype=torch.long).reshape(-1, 1)
+            locs = torch.zeros(len(batch), 2 * max(counts), dtype=torch.float32)
+            for b, i in enumerate(batch):
+                locs[b, :2 * counts[b]] = boxes_to_locs(boxes[i], imgs[i].shape[0], widths[b])[0]
+            for attempt in range(4):
+                _, _, w = encoder(lq_enc)
+                _, f64, f32_ = tspgan(styles=w.index_select(0, owner_t), labels=lab_all, noise=None)
+                p64, p32, o = [], [], 0
+                for c in counts:
+                    p64.append(f64[o:o + c]); p32.append(f32_[o:o + c]); o += c
+                out = sr(lq, p64, p32, locs, widths=widths)
+                torch.cuda.synchronize(dev)
+                if not ops.poll_range(dev) or attempt == 3:
+                    break
+            ops.postprocess_sr_pieces(out, [(b, 0, outs[i]) for b, i in enumerate(batch)])
+        if to_host:
+            pinned = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+            pinned.copy_(flat, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+            outs = {i: pinned[o:o + 128 * wd * 3].view(128, wd, 3).numpy() for i, (o, wd) in layout.items()}
     for i in valid:
         results[i] = dict(sr_u8=outs[i], segments=plans[i])
     return results

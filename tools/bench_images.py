@@ -2,7 +2,11 @@
 pipeline.restore_images at max_lines 1, 4 and 8, against the loop a user writes today -- restore_image on each crop of the same
 plan, then a device->host copy of its bytes.
 
-    python tools/bench_images.py [--images 42] [--passes 3] [--warmup 1]
+    python tools/bench_images.py [--images 42] [--passes 3] [--warmup 1] [--whole-lines]
+
+--whole-lines compares the two ways restore_images decodes a line wider than the canvas, at max_lines 1 and 8: crop by crop
+(the default) and in one piece (whole_lines=True), with the arms' passes alternated, and reports each mode's decoder SR columns
+per pass (batch lines x SR canvas width, summed over the decoder calls).
 
 The image set reuses the 17 (h, w) sizes of the reference's Testsets/LQs (resized LQ widths 92 to 464 pixels, all inside the
 512-pixel canvas) and adds lines 2 to 4 times wider than the canvas, which test_sr.py refuses (:107-110), with one character box
@@ -41,11 +45,23 @@ def make_image_set(n, seed=0):
     return images, labels, boxes
 
 
+def sr_columns(arm, images, plans):
+    """SR columns the decoder computes in one pass of an arm: every crop line is a 2048-column canvas; in whole-line mode every
+    batch of pipeline.pack_by_columns is (lines) x 4 x (its widest Wc)."""
+    from marconet_b200 import pipeline
+    if "_whole_lines" not in arm:
+        return 4 * 512 * sum(len(p) for p in plans)
+    m = int(arm.rsplit("_", 1)[1])
+    wcs = [pipeline.whole_line_width(im.shape[0], im.shape[1])[1] for im in images]
+    return sum(4 * len(b) * max(wcs[j] for j in b) for b in pipeline.pack_by_columns(wcs, m))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--images", type=int, default=42)
     ap.add_argument("--passes", type=int, default=3, help="timed passes over the image set per arm")
     ap.add_argument("--warmup", type=int, default=1, help="untimed passes per arm first")
+    ap.add_argument("--whole-lines", action="store_true", help="crop-by-crop vs whole-line decoding of the wide lines")
     args = ap.parse_args()
     from marconet_b200 import pipeline
     from marconet_b200.models import networks
@@ -72,22 +88,32 @@ def main():
         for c, lab, bx in crops:
             pipeline.restore_image(enc, gen, sr, c, lab, bx)["sr_u8"].cpu()
 
-    arms = {f"restore_images_max_lines_{m}": (lambda m=m: pipeline.restore_images(enc, gen, sr, images, labels, boxes, max_lines=m,
-                                                                                  to_host=True)) for m in (1, 4, 8)}
-    arms["restore_image_loop_over_crops"] = loop
+    if args.whole_lines:
+        arms = {f"restore_images{'_whole_lines' if wl else ''}_max_lines_{m}":
+                (lambda m=m, wl=wl: pipeline.restore_images(enc, gen, sr, images, labels, boxes, max_lines=m, to_host=True, whole_lines=wl))
+                for m in (1, 8) for wl in (False, True)}
+    else:
+        arms = {f"restore_images_max_lines_{m}": (lambda m=m: pipeline.restore_images(enc, gen, sr, images, labels, boxes, max_lines=m,
+                                                                                      to_host=True)) for m in (1, 4, 8)}
+        arms["restore_image_loop_over_crops"] = loop
     out = {}
     with torch.no_grad():
         for fn in arms.values():
             for _ in range(max(1, args.warmup)):
                 fn()
-        for name, fn in arms.items():
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            for _ in range(args.passes):
+        secs = dict.fromkeys(arms, 0.0)
+        for _ in range(args.passes):              # arms alternated pass by pass: drift of a shared host hits all of them alike
+            for name, fn in arms.items():
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
                 fn()
-            torch.cuda.synchronize()
-            s = (time.perf_counter() - t0) / args.passes
+                torch.cuda.synchronize()
+                secs[name] += time.perf_counter() - t0
+        for name in arms:
+            s = secs[name] / args.passes
             out[name] = {"s_per_pass": s, "images_per_sec": len(images) / s, "chars_per_sec": n_chars / s}
+            if args.whole_lines:
+                out[name]["decoder_sr_columns_per_pass"] = sr_columns(name, images, plans)
     card = {"name": torch.cuda.get_device_name(dev)}
     try:
         q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
