@@ -365,6 +365,34 @@ typedef struct {
 int mn_postprocess_sr_u8_pieces(const float* sr, long long stride_n, long long stride_c, long long stride_h, long long stride_w,
                                 int C, int H, int W, const mn_sr_piece* pieces, int n_pieces, int max_width, void* stream);
 
+/* The figure test_sr.py writes per image (:206-231, cv2.imwrite of vstack(ShowLQ[:,:,::-1], ShowLocs[:,:,::-1], ShowSR, prior)),
+ * panels 1, 2 and 4 for a batch of images in one launch (DESIGN.md section 7b).  The figure is uint8 [512][W][3]; every panel is
+ * computed at the ShowLQ width S = round_half_even(w*128/h) and cropped to W <= S:
+ *   rows   0-127  ShowLQ[:, :, ::-1], ShowLQ = cv2.resize(img, (0,0), fx=128/h, fy=128/h, INTER_CUBIC) (:98; OpenCV's own cubic,
+ *                 the arithmetic of mn_preprocess_lq_u8);
+ *   rows 128-255  ShowLocs[:, :, ::-1] (:214-230): ShowLQ with (255, 0, 0) in rows 0-63 of the `n_top` marker column ranges and
+ *                 (0, 0, 255) in rows 64-127 of the `n_bot` ranges -- [start, stop) pairs, top ranges first, computed by the caller
+ *                 with the script's Python slice rules on a width-S row;
+ *   rows 256-383  not written (ShowSR: mn_postprocess_sr_u8_pieces with dst at row 256);
+ *   rows 384-511  prior (:206-211, not flipped): cv2.resize(hstack(prior_k*0.5+0.5 for k < n_chars), (S, 128), INTER_LINEAR)*255,
+ *                 OpenCV's float linear resize, then cvRound with saturation (cv2.imwrite).  Each character's [3][128][128] fp32
+ *                 prior is read in place through element strides (the channels_last generator output).
+ * images: DEVICE array of n_images records; marks and priors are DEVICE arrays (validated by the caller); max_width >= every W. */
+typedef struct {
+    const float* img;           /* [3][128][128] generator image in [-1, 1] */
+    int64_t stride_c, stride_h, stride_w;
+} mn_figure_prior;
+typedef struct {
+    const uint8_t* img;         /* row 0 of the h x w x 3 source image */
+    int64_t row_pitch;          /* bytes between rows of the source image */
+    uint8_t* fig;               /* row 0 of the [512][W][3] figure */
+    int64_t fig_pitch;          /* bytes between rows of the figure */
+    const int32_t* marks;       /* n_top + n_bot column ranges [start, stop), 0 <= start < stop <= S */
+    const mn_figure_prior* priors;
+    int32_t h, w, S, W, n_top, n_bot, n_chars;
+} mn_figure_image;
+int mn_figure_u8(const mn_figure_image* images, int n_images, int max_width, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -55,6 +55,15 @@ class SrPiece(Structure):
     _fields_ = [("line", c_int32), ("src_x0", c_int32), ("width", c_int32), ("dst", c_void_p), ("dst_pitch", c_int64)]
 
 
+class FigurePrior(Structure):
+    _fields_ = [("img", c_void_p), ("stride_c", c_int64), ("stride_h", c_int64), ("stride_w", c_int64)]
+
+
+class FigureImage(Structure):
+    _fields_ = [("img", c_void_p), ("row_pitch", c_int64), ("fig", c_void_p), ("fig_pitch", c_int64), ("marks", c_void_p), ("priors", c_void_p),
+                ("h", c_int32), ("w", c_int32), ("S", c_int32), ("W", c_int32), ("n_top", c_int32), ("n_bot", c_int32), ("n_chars", c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -101,6 +110,7 @@ SYMBOLS = {
     "mn_preprocess_lq_u8_batched": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
     "mn_postprocess_sr_u8_pieces": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_int, c_int, c_int, c_void_p, c_int, c_int,
                                             c_void_p]),
+    "mn_figure_u8": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

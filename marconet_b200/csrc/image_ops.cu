@@ -35,9 +35,10 @@ __device__ __forceinline__ CubicTaps cubic_taps(int d, double scale) {
 // One canvas element (idx over [out_h][out_w][cn]) of test_sr.py:98-111 for an 8-bit image whose rows start `row_pitch` bytes
 // apart.  The cubic taps replicate the border of [0, h) x [0, w): a crop passed as (pointer to its first column, the source
 // image's pitch, its own width) is resized as an isolated image, exactly what cv2.resize(img[:, a:b], ...) computes.
-__device__ __forceinline__ void preprocess_lq_element(const uint8_t* __restrict__ img, long long row_pitch, int h, int w, int cn,
-                                                      double scale_x, double scale_y, int dh, int dw, int idx,
-                                                      float* __restrict__ lq, uint8_t* __restrict__ lq_u8, int out_h, int out_w) {
+// Returns the resized byte (0 outside the dh x dw image); lq (fp32 canvas) and lq_u8 (resized bytes) are optional outputs.
+__device__ __forceinline__ int preprocess_lq_element(const uint8_t* __restrict__ img, long long row_pitch, int h, int w, int cn,
+                                                     double scale_x, double scale_y, int dh, int dw, int idx,
+                                                     float* __restrict__ lq, uint8_t* __restrict__ lq_u8, int out_h, int out_w) {
     const int c = idx % cn;
     const int dx = (idx / cn) % out_w;
     const int dy = idx / (cn * out_w);
@@ -70,9 +71,12 @@ __device__ __forceinline__ void preprocess_lq_element(const uint8_t* __restrict_
         v = min(max(v, 0), 255);
         if (lq_u8) lq_u8[((size_t)dy * dw + dx) * cn + c] = (uint8_t)v;
     }
-    // ToTensor: float(u8) / 255 ; Normalize: (x - 0.5) / 0.5
-    const float t = __fdiv_rn(__fsub_rn(__fdiv_rn((float)v, 255.f), 0.5f), 0.5f);
-    lq[((size_t)c * out_h + dy) * out_w + dx] = t;
+    if (lq) {
+        // ToTensor: float(u8) / 255 ; Normalize: (x - 0.5) / 0.5
+        const float t = __fdiv_rn(__fsub_rn(__fdiv_rn((float)v, 255.f), 0.5f), 0.5f);
+        lq[((size_t)c * out_h + dy) * out_w + dx] = t;
+    }
+    return v;
 }
 
 __global__ void preprocess_lq_kernel(const uint8_t* __restrict__ img, int h, int w, int cn, double scale_x, double scale_y,
@@ -126,6 +130,64 @@ __global__ void postprocess_sr_pieces_kernel(const float* __restrict__ sr, long 
     for (int c = 0; c < C; ++c) o[C - 1 - c] = sr_to_u8(p[c * sc]);
 }
 
+// test_sr.py:206-211 for one value of the prior strip hstack(prior*0.5+0.5): character k, channel c, row y, column x.
+__device__ __forceinline__ float prior_value(const mn_figure_prior* __restrict__ pr, int k, int c, int y, int x) {
+    const mn_figure_prior p = pr[k];
+    return __fadd_rn(__fmul_rn(p.img[c * p.stride_c + y * p.stride_h + x * p.stride_w], 0.5f), 0.5f);
+}
+
+// blockIdx.y = image; one thread per pixel (y, x) of the 128 x max_width panel rows, those at x >= the image's W exit.
+// Panels 1-2 (ShowLQ, ShowLocs; test_sr.py:98,214-231) share one cubic resize (preprocess_lq_element at fx = fy = 128/h, the
+// vector / tail split taken at width S); panel 4 is OpenCV's float INTER_LINEAR of the prior strip to width S (test_sr.py:210),
+// *255 and cvRound with saturation (cv2.imwrite).  Panel 3 (ShowSR) is written by postprocess_sr_pieces_kernel.
+__global__ void figure_kernel(const mn_figure_image* __restrict__ images, int max_width) {
+    mn_pdl_prologue();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= 128ll * max_width) return;
+    const mn_figure_image im = images[blockIdx.y];
+    const int x = (int)(idx % max_width), y = (int)(idx / max_width);
+    if (x >= im.W) return;
+    uint8_t* row = im.fig + (long long)y * im.fig_pitch + (long long)x * 3;
+
+    const double fx = __ddiv_rn(128.0, (double)im.h), scale = __ddiv_rn(1.0, fx);       // the script's fx=128/h
+    const int* marks = im.marks + (y < 64 ? 0 : 2 * im.n_top);
+    const int n_marks = y < 64 ? im.n_top : im.n_bot;
+    bool marked = false;
+    for (int m = 0; m < n_marks; ++m) marked |= (x >= marks[2 * m]) & (x < marks[2 * m + 1]);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const int v = preprocess_lq_element(im.img, im.row_pitch, im.h, im.w, 3, scale, scale, 128, im.S, (y * im.S + x) * 3 + c,
+                                            nullptr, nullptr, 128, im.S);
+        // ShowLocs: (255, 0, 0) at the x markers of rows 0-63, (0, 0, 255) at the y markers of rows 64-127; both panels flipped
+        const int mark = c == (y < 64 ? 0 : 2) ? 255 : 0;
+        row[2 - c] = (uint8_t)v;
+        row[128 * im.fig_pitch + 2 - c] = (uint8_t)(marked ? mark : v);
+    }
+
+    const int sw = 128 * im.n_chars;
+    float a1 = 0.f;
+    int sx = x;
+    if (im.S != sw) {                                    // cv2.resize copies when the size is unchanged
+        const double sc = __ddiv_rn(1.0, __ddiv_rn((double)im.S, (double)sw));
+        float f = __double2float_rn(__dsub_rn(__dmul_rn((double)x + 0.5, sc), 0.5));
+        sx = (int)floorf(f);
+        a1 = __fsub_rn(f, (float)sx);
+        if (sx < 0) sx = 0, a1 = 0.f;
+        if (sx >= sw - 1) sx = sw - 1, a1 = 0.f;
+    }
+    const float a0 = __fsub_rn(1.f, a1);
+    const int s1 = min(sx + 1, sw - 1);
+    uint8_t* prow = row + 384 * im.fig_pitch;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float v0 = prior_value(im.priors, sx >> 7, c, y, sx & 127);
+        float v = v0;
+        if (im.S != sw) v = __fadd_rn(__fmul_rn(v0, a0), __fmul_rn(prior_value(im.priors, s1 >> 7, c, y, s1 & 127), a1));
+        const int q = __float2int_rn(__fmul_rn(v, 255.f));
+        prow[c] = (uint8_t)min(max(q, 0), 255);          // not channel-flipped: the script writes the prior panel as RGB
+    }
+}
+
 }  // namespace
 
 extern "C" int mn_preprocess_lq_u8(const uint8_t* img, int h, int w, int cn, double fx, double fy, int dh, int dw,
@@ -168,6 +230,15 @@ extern "C" int mn_postprocess_sr_u8_pieces(const float* sr, long long stride_n, 
     const long long total = (long long)H * max_width;
     MN_CUDA_CHECK((mn_launch(postprocess_sr_pieces_kernel, dim3((unsigned)mn_cdiv64(total, 256), n_pieces), dim3(256), 0, (cudaStream_t)stream,
                              sr, stride_n, stride_c, stride_h, stride_w, C, H, pieces, max_width)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_figure_u8(const mn_figure_image* images, int n_images, int max_width, void* stream) {
+    MN_REQUIRE(images && n_images > 0 && n_images <= 65535 && max_width > 0, "mn_figure_u8: bad args");
+    const long long total = 128ll * max_width;
+    MN_CUDA_CHECK((mn_launch(figure_kernel, dim3((unsigned)mn_cdiv64(total, 256), n_images), dim3(256), 0, (cudaStream_t)stream,
+                             images, max_width)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

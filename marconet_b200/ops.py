@@ -972,3 +972,55 @@ def postprocess_sr_pieces(sr, pieces):
     _lib.check(_lib.load().mn_postprocess_sr_u8_pieces(_ptr(sr), sn, sc, sh, sw, c, h, w, _ptr(table), len(recs), mx, _stream()),
                "mn_postprocess_sr_u8_pieces")
     LAUNCHES += 1
+
+
+def figure_panels(items):
+    """Panels 1, 2 and 4 of test_sr.py's figure (:206-231) for many images in one launch (mn_figure_u8; DESIGN.md section 7b).
+    items: list of (img, fig, top, bottom, priors):
+      img     uint8 [h, w, 3] CUDA tensor with dense pixels (any row stride), read in place;
+      fig     uint8 [512, W, 3] CUDA view with dense pixels, W <= S = round_half_even(w*128/h); rows 0-255 and 384-511 are
+              written, rows 256-383 (the SR panel) are not;
+      top, bottom  the ShowLocs marker column ranges [start, stop) of rows 0-63 and 64-127 (pipeline.figure_markers);
+      priors  non-empty list of fp32 [3, 128, 128] CUDA views (any strides), the characters' generator images in label order."""
+    import numpy as np
+    global LAUNCHES
+    if not items:
+        raise ValueError("figure_panels: no images")
+    if len(items) > 65535:
+        raise ValueError("figure_panels: at most 65535 images per launch")
+    dev = items[0][1].device
+    n_prior = sum(len(it[4]) for it in items)
+    n_marks = sum(len(it[2]) + len(it[3]) for it in items)
+    isz, psz = ctypes.sizeof(_lib.FigureImage), ctypes.sizeof(_lib.FigurePrior)
+    buf = torch.empty(len(items) * isz + n_prior * psz + 8 * max(1, n_marks), dtype=torch.uint8, device=dev)
+    base = buf.data_ptr()
+    p_off, m_off = len(items) * isz, len(items) * isz + n_prior * psz
+    recs, prs, marks, mx = [], [], [], 0
+    for i, (img, fig, top, bot, priors) in enumerate(items):
+        for name, t in (("img", img), ("fig", fig)):
+            if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3 \
+                    or t.stride(2) != 1 or t.stride(1) != 3 or t.stride(0) < 3 * t.shape[1]:
+                raise RuntimeError(f"figure_panels: image {i}: {name} must be a uint8 [., ., 3] tensor with dense pixels on {dev}")
+        h, w = img.shape[:2]
+        S = round_half_even(w * (128 / h))
+        W = fig.shape[1]
+        if fig.shape[0] != 512 or not 1 <= W <= S or round_half_even(h * (128 / h)) != 128:
+            raise ValueError(f"figure_panels: image {i}: figure {tuple(fig.shape)} is not [512, W, 3] with 1 <= W <= S = {S}")
+        if not priors:
+            raise ValueError(f"figure_panels: image {i}: no prior images")
+        for a, b in list(top) + list(bot):
+            if not 0 <= int(a) < int(b) <= S:
+                raise ValueError(f"figure_panels: image {i}: marker columns [{a}, {b}) are not a non-empty range of [0, {S}]")
+        recs.append(_lib.FigureImage(img.data_ptr(), img.stride(0), fig.data_ptr(), fig.stride(0), base + m_off + 8 * len(marks),
+                                     base + p_off + psz * len(prs), h, w, S, W, len(top), len(bot), len(priors)))
+        marks += [(int(a), int(b)) for a, b in list(top) + list(bot)]
+        for k, p in enumerate(priors):
+            if not isinstance(p, torch.Tensor) or p.device != dev or p.dtype != torch.float32 or tuple(p.shape) != (3, 128, 128):
+                raise RuntimeError(f"figure_panels: image {i}, character {k}: prior must be an fp32 [3, 128, 128] tensor on {dev}")
+            prs.append(_lib.FigurePrior(p.data_ptr(), *p.stride()))
+        mx = max(mx, W)
+    host = bytes((_lib.FigureImage * len(recs))(*recs)) + bytes((_lib.FigurePrior * len(prs))(*prs)) + \
+        np.asarray(marks or [(0, 0)], dtype=np.int32).tobytes()
+    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    _lib.check(_lib.load().mn_figure_u8(_ptr(buf), len(recs), mx, _stream()), "mn_figure_u8")
+    LAUNCHES += 1

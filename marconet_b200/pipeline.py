@@ -100,19 +100,53 @@ def boxes_to_locs(boxes, h, lq_width=512):
     return locs
 
 
+def figure_markers(locs, S, M):
+    """The box markers of test_sr.py's ShowLocs panel (:214-230) on a width-S row, with img_max_width = M (2048 in the script):
+    locs = one line's fp32 (centre, half-width) pairs.  Returns (top, bottom): the [start, stop) column ranges painted in rows
+    0-63 (x = centre - width, pad 2) and rows 64-127 (y = centre + width, pad 1), by the script's own Python slice rules --
+    clipped to [0, S], a negative stop counting from the end; empty ranges are dropped."""
+    top, bot = [], []
+    for c in range(len(locs) // 2):
+        center, width = int(float(locs[2 * c]) * M), int(float(locs[2 * c + 1]) * M)
+        x, y = center - width, center + width
+        for out, a, b in ((top, max(0, x - 2), min(x + 2, M)), (bot, max(0, y - 1), min(y + 1, M))):
+            start, stop, _ = slice(a, b).indices(S)
+            if stop > start:
+                out.append((start, stop))
+    return top, bot
+
+
+def _figure_markers_for(h, w, boxes):
+    """figure_markers of an h x w image: locs = boxes_to_locs(boxes, h, Wc), M = 4*Wc, S = ShowLQ's width (DESIGN.md 7b)."""
+    from .ops import round_half_even
+    wc = whole_line_width(h, w)[1]
+    return figure_markers(boxes_to_locs(boxes, h, wc)[0].tolist(), round_half_even(w * (128 / h)), 4 * wc)
+
+
+def _to_host(flat):
+    """One pinned device->host copy of ``flat``; returns the pinned tensor once the copy has finished."""
+    pinned = torch.empty(flat.numel(), dtype=torch.uint8, pin_memory=True)
+    pinned.copy_(flat, non_blocking=True)
+    torch.cuda.current_stream(flat.device).synchronize()
+    return pinned
+
+
 @torch.no_grad()
-def restore_image(encoder, tspgan, sr, img_u8, labels, boxes):
+def restore_image(encoder, tspgan, sr, img_u8, labels, boxes, figure=False):
     """One text-line image end to end on the device (the body of test_sr.py's loop, :98-201, with the labels / boxes the
     detector and OCR produced): uint8 [h, w, 3] image (host numpy / tensor or CUDA tensor) -> dict(sr_u8 [128, W, 3] uint8 bytes
     as cv2.imwrite would store them, cropped to the line's width; sr fp32; lq; lq_width).
-    Pre- and post-processing run as CUDA kernels (mn_preprocess_lq_u8 / mn_postprocess_sr_u8)."""
+    Pre- and post-processing run as CUDA kernels (mn_preprocess_lq_u8 / mn_postprocess_sr_u8).
+    ``figure=True`` adds ``figure``: the uint8 [512, W, 3] image test_sr.py writes (:206-231; ShowLQ, ShowLocs, ShowSR, prior;
+    DESIGN.md section 7b), composed on the device (mn_figure_u8); ``sr_u8`` is then its view ``figure[256:384]``."""
     from . import ops
     dev = next(encoder.parameters()).device
     img = torch.as_tensor(img_u8)
     h = img.shape[0]
     img = img.to(dev, non_blocking=True).contiguous()
     lq, lq_w = ops.preprocess_lq(img)
-    locs = boxes_to_locs(boxes, h, lq.shape[-1]).to(dev)
+    locs_host = boxes_to_locs(boxes, h, lq.shape[-1])
+    locs = locs_host.to(dev)
     _, _, w = encoder(lq)
     lab = torch.as_tensor(labels, dtype=torch.long).reshape(-1, 1)
     if lab.shape[0] == 0:
@@ -120,8 +154,14 @@ def restore_image(encoder, tspgan, sr, img_u8, labels, boxes):
     img_prior, f64, f32_ = tspgan(styles=w[:1].repeat(lab.shape[0], 1), labels=lab, noise=None)
     out = sr(lq, [f64], [f32_], locs)
     show_w = ops.round_half_even(img.shape[1] * (128 / h))    # ShowLQ = cv2.resize(img, fx=128/h, ...) (test_sr.py:98)
-    sr_u8 = ops.postprocess_sr(out)[0, :, :show_w]            # ShowSR = sr[:, :ShowLQ.shape[1]] (test_sr.py:201)
-    return dict(sr_u8=sr_u8, sr=out, lq=lq, lq_width=lq_w, prior=img_prior, locs=locs)
+    if not figure:
+        sr_u8 = ops.postprocess_sr(out)[0, :, :show_w]        # ShowSR = sr[:, :ShowLQ.shape[1]] (test_sr.py:201)
+        return dict(sr_u8=sr_u8, sr=out, lq=lq, lq_width=lq_w, prior=img_prior, locs=locs)
+    fig = torch.empty((512, min(show_w, out.shape[-1]), 3), dtype=torch.uint8, device=dev)
+    ops.postprocess_sr_pieces(out, [(0, 0, fig[256:384])])
+    top, bot = figure_markers(locs_host[0].tolist(), show_w, 4 * lq.shape[-1])
+    ops.figure_panels([(img, fig, top, bot, list(img_prior))])
+    return dict(sr_u8=fig[256:384], figure=fig, sr=out, lq=lq, lq_width=lq_w, prior=img_prior, locs=locs)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -328,7 +368,7 @@ def pack_by_columns(widths, max_lines, canvas=512):
 
 @torch.no_grad()
 def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, context=16, skip_invalid=False, to_host=False,
-                   whole_lines=False):
+                   whole_lines=False, figure=False):
     """Text-line images of any sizes end to end, batched: the flow of restore_image for every image, each cut into crops that
     fit the 32x512 LQ canvas (plan_segments) and every crop of every image run as one line of a batch of at most ``max_lines``.
 
@@ -350,7 +390,14 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
     character's prior takes the style w of the crop that owns it.  Lines that fit the canvas are computed as without the flag.
     Decoder lines of different widths share a batch (TSPSRNet's ``widths``); a batch holds k lines only while
     k * (its widest Wc) <= max_lines * 512.  Per batch: one host->device copy, one crop kernel for the encoder crops, one for
-    the decoder lines, the encoder, one TSPGAN call, one ragged TSPSRNet call, the fp16-range re-run, one stitch kernel."""
+    the decoder lines, the encoder, one TSPGAN call, one ragged TSPSRNet call, the fp16-range re-run, one stitch kernel.
+
+    ``figure=True`` (either mode) adds ``figure`` to every result: the uint8 [512, W_i, 3] image test_sr.py writes (:206-231;
+    DESIGN.md section 7b) -- ShowLQ and ShowLocs (markers at locs = boxes_to_locs(boxes, h, Wc), img_max_width = 4*Wc), the
+    image's sr_u8, and the priors this call generated (each character's in the style of the crop that owns it), all cropped to
+    sr_u8's width.  ``sr_u8`` becomes the view ``figure[256:384]``, its bytes unchanged.  The batch that holds an image's last
+    crop composes its figure: one more launch (mn_figure_u8) per batch, and the prior images are kept until then.  With
+    ``to_host`` the figures come back through the same single pinned copy.  Error entries have no figure."""
     from . import ops
     n = len(images)
     if not (len(labels) == len(boxes) == n):
@@ -381,16 +428,20 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
     if not valid:
         return results
     if whole_lines:
-        return _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, results, max_lines, to_host, dev)
+        return _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, results, max_lines, to_host, dev, figure)
+    rows = 512 if figure else 128
     with torch.cuda.device(dev):
         layout, total = {}, 0
         for i in valid:
             width, pieces = stitch_pieces(imgs[i].shape[0], imgs[i].shape[1], plans[i])
             layout[i] = (total, width, pieces)
-            total += 128 * width * 3
+            total += rows * width * 3
         flat = torch.empty(total, dtype=torch.uint8, device=dev)
-        outs = {i: flat[o:o + 128 * wd * 3].view(128, wd, 3) for i, (o, wd, _) in layout.items()}
+        figs = {i: flat[o:o + rows * wd * 3].view(rows, wd, 3) for i, (o, wd, _) in layout.items()}
+        outs = {i: f[256:384] for i, f in figs.items()} if figure else figs
         lines = [(i, k) for i in valid for k in range(len(plans[i]))]
+        last_batch = {i: b0 for b0 in range(0, len(lines), max_lines) for i, _ in lines[b0:b0 + max_lines]}
+        priors = {i: [] for i in valid}
         for b0 in range(0, len(lines), max_lines):
             batch = lines[b0:b0 + max_lines]
             dimg = _device_images(dict.fromkeys(i for i, _ in batch), imgs, dev)
@@ -405,10 +456,10 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
                     locs[b, :2 * counts[b]] = boxes_to_locs(s.boxes, imgs[i].shape[0], lq.shape[-1])[0]
             for attempt in range(4):
                 _, _, w = encoder(lq)
-                p64, p32 = [], []
+                p64, p32, img_p = [], [], None
                 if lab_all.shape[0] > 0:
                     styles = torch.cat([w[b:b + 1].expand(c, -1) for b, c in enumerate(counts) if c > 0], dim=0)
-                    _, f64, f32_ = tspgan(styles=styles, labels=lab_all, noise=None)
+                    img_p, f64, f32_ = tspgan(styles=styles, labels=lab_all, noise=None)
                     o = 0
                     for c in counts:
                         p64.append(f64[o:o + c]); p32.append(f32_[o:o + c]); o += c
@@ -426,19 +477,30 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
                         pieces.append((b, src, outs[i][:, x0:x0 + wd]))
             if pieces:
                 ops.postprocess_sr_pieces(out, pieces)
+            if figure:
+                o = 0
+                for (i, _), c in zip(batch, counts):            # crops in label order: the characters' priors in label order
+                    priors[i] += list(img_p[o:o + c]) if c else []
+                    o += c
+                done = [i for i in dict.fromkeys(i for i, _ in batch) if last_batch[i] == b0]
+                if done:
+                    ops.figure_panels([(dimg[i], figs[i]) + _figure_markers_for(*imgs[i].shape[:2], boxes[i]) + (priors.pop(i),)
+                                       for i in done])
         if to_host:
-            pinned = torch.empty(total, dtype=torch.uint8, pin_memory=True)
-            pinned.copy_(flat, non_blocking=True)
-            torch.cuda.current_stream(dev).synchronize()
-            outs = {i: pinned[o:o + 128 * wd * 3].view(128, wd, 3).numpy() for i, (o, wd, _) in layout.items()}
+            pinned = _to_host(flat)
+            figs = {i: pinned[o:o + rows * wd * 3].view(rows, wd, 3).numpy() for i, (o, wd, _) in layout.items()}
+            outs = {i: f[256:384] for i, f in figs.items()} if figure else figs
     for i in valid:
         results[i] = dict(sr_u8=outs[i], segments=plans[i])
+        if figure:
+            results[i]["figure"] = figs[i]
     return results
 
 
-def _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, results, max_lines, to_host, dev):
+def _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, results, max_lines, to_host, dev, figure):
     """restore_images(whole_lines=True) after validation: one decoder line per image (see restore_images)."""
     from . import ops
+    rows = 512 if figure else 128
     with torch.cuda.device(dev):
         geo = {i: whole_line_width(imgs[i].shape[0], imgs[i].shape[1]) for i in valid}
         layout, total = {}, 0
@@ -447,9 +509,10 @@ def _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, r
             wc = geo[i][1]
             width = min(ops.round_half_even(w * (128 / h)), 4 * wc)
             layout[i] = (total, width)
-            total += 128 * width * 3
+            total += rows * width * 3
         flat = torch.empty(total, dtype=torch.uint8, device=dev)
-        outs = {i: flat[o:o + 128 * wd * 3].view(128, wd, 3) for i, (o, wd) in layout.items()}
+        figs = {i: flat[o:o + rows * wd * 3].view(rows, wd, 3) for i, (o, wd) in layout.items()}
+        outs = {i: f[256:384] for i, f in figs.items()} if figure else figs
         for bidx in pack_by_columns([geo[i][1] for i in valid], max_lines):
             batch = [valid[j] for j in bidx]
             dimg = _device_images(batch, imgs, dev)
@@ -475,7 +538,7 @@ def _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, r
                 locs[b, :2 * counts[b]] = boxes_to_locs(boxes[i], imgs[i].shape[0], widths[b])[0]
             for attempt in range(4):
                 _, _, w = encoder(lq_enc)
-                _, f64, f32_ = tspgan(styles=w.index_select(0, owner_t), labels=lab_all, noise=None)
+                img_p, f64, f32_ = tspgan(styles=w.index_select(0, owner_t), labels=lab_all, noise=None)
                 p64, p32, o = [], [], 0
                 for c in counts:
                     p64.append(f64[o:o + c]); p32.append(f32_[o:o + c]); o += c
@@ -484,13 +547,20 @@ def _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, r
                 if not ops.poll_range(dev) or attempt == 3:
                     break
             ops.postprocess_sr_pieces(out, [(b, 0, outs[i]) for b, i in enumerate(batch)])
+            if figure:                                          # every image of the batch is complete
+                offs = [0]
+                for c in counts:
+                    offs.append(offs[-1] + c)
+                ops.figure_panels([(dimg[i], figs[i]) + _figure_markers_for(*imgs[i].shape[:2], boxes[i]) +
+                                   (list(img_p[offs[b]:offs[b + 1]]),) for b, i in enumerate(batch)])
         if to_host:
-            pinned = torch.empty(total, dtype=torch.uint8, pin_memory=True)
-            pinned.copy_(flat, non_blocking=True)
-            torch.cuda.current_stream(dev).synchronize()
-            outs = {i: pinned[o:o + 128 * wd * 3].view(128, wd, 3).numpy() for i, (o, wd) in layout.items()}
+            pinned = _to_host(flat)
+            figs = {i: pinned[o:o + rows * wd * 3].view(rows, wd, 3).numpy() for i, (o, wd) in layout.items()}
+            outs = {i: f[256:384] for i, f in figs.items()} if figure else figs
     for i in valid:
         results[i] = dict(sr_u8=outs[i], segments=plans[i])
+        if figure:
+            results[i]["figure"] = figs[i]
     return results
 
 

@@ -2,11 +2,17 @@
 pipeline.restore_images at max_lines 1, 4 and 8, against the loop a user writes today -- restore_image on each crop of the same
 plan, then a device->host copy of its bytes.
 
-    python tools/bench_images.py [--images 42] [--passes 3] [--warmup 1] [--whole-lines]
+    python tools/bench_images.py [--images 42] [--passes 3] [--warmup 1] [--whole-lines | --figures]
 
 --whole-lines compares the two ways restore_images decodes a line wider than the canvas, at max_lines 1 and 8: crop by crop
 (the default) and in one piece (whole_lines=True), with the arms' passes alternated, and reports each mode's decoder SR columns
 per pass (batch lines x SR canvas width, summed over the decoder calls).
+
+--figures times test_sr.py's four-panel figure at max_lines 8: restore_images without figures, with figure=True (composed on the
+device, one pinned copy back), and the host path a user has without it -- restore_images' SR bytes, then every character's prior
+image copied back (fp32 [3, 128, 128]) and the figure composed with cv2 as test_sr.py:206-231 does (ShowLQ cubic resize, markers,
+INTER_LINEAR prior strip, vstack).  The host arm reads priors generated once before timing (the generator's work is already
+inside restore_images; only the copy back and the cv2 work are added).
 
 The image set reuses the 17 (h, w) sizes of the reference's Testsets/LQs (resized LQ widths 92 to 464 pixels, all inside the
 512-pixel canvas) and adds lines 2 to 4 times wider than the canvas, which test_sr.py refuses (:107-110), with one character box
@@ -56,12 +62,55 @@ def sr_columns(arm, images, plans):
     return sum(4 * len(b) * max(wcs[j] for j in b) for b in pipeline.pack_by_columns(wcs, m))
 
 
+def host_figure(img, boxes, priors_host, sr_u8):
+    """test_sr.py:98,206-231 on the host with cv2: the figure of one image from its SR bytes and its priors (fp32 numpy)."""
+    import cv2
+    from marconet_b200 import pipeline
+    h, w = img.shape[:2]
+    show_lq = cv2.resize(img, (0, 0), fx=128 / h, fy=128 / h, interpolation=cv2.INTER_CUBIC)
+    wc = pipeline.whole_line_width(h, w)[1]
+    top, bot = pipeline.figure_markers(pipeline.boxes_to_locs(boxes, h, wc)[0].tolist(), show_lq.shape[1], 4 * wc)
+    show_locs = show_lq.copy()
+    for a, b in top:
+        show_locs[:64, a:b] = (255, 0, 0)
+    for a, b in bot:
+        show_locs[64:, a:b] = (0, 0, 255)
+    strip = np.hstack(list((priors_host * 0.5 + 0.5).transpose(0, 2, 3, 1)))
+    prior = cv2.resize(strip, (show_lq.shape[1], 128)) * 255
+    W = sr_u8.shape[1]
+    return np.vstack((show_lq[:, :W, ::-1], show_locs[:, :W, ::-1], sr_u8, np.clip(np.rint(prior[:, :W]), 0, 255).astype(np.uint8)))
+
+
+def figure_arms(enc, gen, sr, images, labels, boxes, dev, max_lines=8):
+    from marconet_b200 import pipeline
+    n_chars = sum(len(l) for l in labels)
+    with torch.no_grad():                                   # stand-in device priors, as many as the set has characters
+        lab = torch.tensor([v for l in labels for v in l], dtype=torch.long).reshape(-1, 1)
+        priors_dev = torch.cat([gen(styles=torch.zeros(min(256, n_chars - o), 512, device=dev), labels=lab[o:o + 256], noise=None)[0]
+                                for o in range(0, n_chars, 256)])
+
+    def host():
+        res = pipeline.restore_images(enc, gen, sr, images, labels, boxes, max_lines=max_lines, to_host=True)
+        pri = priors_dev.cpu().numpy()
+        o = 0
+        for im, l, bx, r in zip(images, labels, boxes, res):
+            host_figure(im, bx, pri[o:o + len(l)], r["sr_u8"])
+            o += len(l)
+
+    return {f"restore_images_max_lines_{max_lines}": lambda: pipeline.restore_images(enc, gen, sr, images, labels, boxes,
+                                                                                     max_lines=max_lines, to_host=True),
+            f"restore_images_max_lines_{max_lines}_figure": lambda: pipeline.restore_images(enc, gen, sr, images, labels, boxes,
+                                                                                            max_lines=max_lines, to_host=True, figure=True),
+            f"restore_images_max_lines_{max_lines}_host_cv2_figure": host}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--images", type=int, default=42)
     ap.add_argument("--passes", type=int, default=3, help="timed passes over the image set per arm")
     ap.add_argument("--warmup", type=int, default=1, help="untimed passes per arm first")
     ap.add_argument("--whole-lines", action="store_true", help="crop-by-crop vs whole-line decoding of the wide lines")
+    ap.add_argument("--figures", action="store_true", help="test_sr.py's figure on the device vs on the host with cv2")
     args = ap.parse_args()
     from marconet_b200 import pipeline
     from marconet_b200.models import networks
@@ -88,7 +137,9 @@ def main():
         for c, lab, bx in crops:
             pipeline.restore_image(enc, gen, sr, c, lab, bx)["sr_u8"].cpu()
 
-    if args.whole_lines:
+    if args.figures:
+        arms = figure_arms(enc, gen, sr, images, labels, boxes, dev)
+    elif args.whole_lines:
         arms = {f"restore_images{'_whole_lines' if wl else ''}_max_lines_{m}":
                 (lambda m=m, wl=wl: pipeline.restore_images(enc, gen, sr, images, labels, boxes, max_lines=m, to_host=True, whole_lines=wl))
                 for m in (1, 8) for wl in (False, True)}
