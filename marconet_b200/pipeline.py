@@ -54,38 +54,48 @@ def restore_lines(encoder, tspgan, sr, lq, labels=None, locs=None, max_chars=16,
     check_range: synchronise at the end and look at the fp16-range flags (ops.poll_range); when a tensor-core conv overflowed the
     fp16 hi/lo split its layer is re-routed to the bf16 split and the step is re-run (at most 3 times) -- the caller never sees
     the Inf/NaN result."""
-    if check_range:
-        from . import ops
-        for attempt in range(4):
-            out = restore_lines(encoder, tspgan, sr, lq, labels, locs, max_chars, check_range=False)
-            torch.cuda.synchronize(lq.device)
-            if not ops.poll_range(lq.device) or attempt == 3:
-                return out
+    def step():
+        return _step(encoder, tspgan, sr, lq, labels, locs, max_chars=max_chars)
+    return _rerun(step, lq.device) if check_range else step()
+
+
+def _step(encoder, tspgan, sr, lq, labels, locs, max_chars=16, owner=None, lq_sr=None, widths=None):
+    """One pass of the three modules over a batch -> restore_lines' dict.  The encoder reads ``lq`` (32x512 crops), TSPSRNet
+    reads ``lq_sr`` (default: lq, one decoder line per crop) with ``widths``.  labels: one int64 [n_b, 1] tensor per decoder line
+    (None: the encoder's decoded labels, at most ``max_chars``); locs None: the encoder's boxes.  One TSPGAN call generates every
+    character; character j takes the style w[owner[j]] (default: the crop of its own line)."""
     logits, locs_lr, w = encoder(lq)
     if labels is None:
-        labels = []
-        for b in range(lq.shape[0]):
-            lab = decode_labels(logits[b])[:max_chars]
-            labels.append(torch.tensor(lab, dtype=torch.long).reshape(-1, 1))
+        labels = [torch.tensor(decode_labels(logits[b])[:max_chars], dtype=torch.long).reshape(-1, 1) for b in range(lq.shape[0])]
     if locs is None:
         locs = lr_to_center_halfwidth(locs_lr)
     counts = [int(l.shape[0]) for l in labels]
-    total = sum(counts)
-    p64, p32, priors = [], [], []
-    if total > 0:
-        styles = torch.cat([w[b:b + 1].expand(counts[b], -1) for b in range(lq.shape[0]) if counts[b] > 0], dim=0)
-        lab_all = torch.cat([l for l in labels if l.shape[0] > 0], dim=0)
-        img, f64, f32_ = tspgan(styles=styles, labels=lab_all, noise=None)       # one generator call for every character
-        o = 0
-        for n in counts:
-            p64.append(f64[o:o + n]); p32.append(f32_[o:o + n]); priors.append(img[o:o + n]); o += n
+    dev = lq.device
+    if sum(counts) > 0:
+        if owner is None:
+            owner = [b for b, c in enumerate(counts) for _ in range(c)]
+        # through pinned memory, which the caching host allocator keeps until the copy has read it: a non_blocking copy straight
+        # from this temporary gave styles that differed from run to run once the modules replay CUDA graphs
+        styles = w.index_select(0, torch.tensor(owner, dtype=torch.long).pin_memory().to(dev, non_blocking=True))
+        img, f64, f32_ = tspgan(styles=styles, labels=torch.cat([l for l in labels if l.shape[0] > 0]), noise=None)
+        priors, p64, p32 = list(img.split(counts)), list(f64.split(counts)), list(f32_.split(counts))
     else:
-        dev = lq.device
-        for _ in counts:
-            p64.append(torch.zeros(0, 256, 64, 64, device=dev)); p32.append(torch.zeros(0, 512, 32, 32, device=dev))
-            priors.append(torch.zeros(0, 3, 128, 128, device=dev))
-    out = sr(lq, p64, p32, locs)
+        priors = [torch.zeros(0, 3, 128, 128, device=dev) for _ in counts]
+        p64 = [torch.zeros(0, 256, 64, 64, device=dev) for _ in counts]
+        p32 = [torch.zeros(0, 512, 32, 32, device=dev) for _ in counts]
+    out = sr(lq if lq_sr is None else lq_sr, p64, p32, locs, widths=widths)
     return dict(sr=out, prior=priors, labels=labels, locs=locs, w=w, logits=logits)
+
+
+def _rerun(step, device):
+    """``step()``, then a synchronisation and a look at the fp16-range flags (ops.poll_range): a tensor-core conv that overflowed
+    the fp16 hi/lo split has been re-routed to the bf16 split, and the step runs again (at most 3 times)."""
+    from . import ops
+    for attempt in range(4):
+        out = step()
+        torch.cuda.synchronize(device)
+        if not ops.poll_range(device) or attempt == 3:
+            return out
 
 
 def boxes_to_locs(boxes, h, lq_width=512):
@@ -366,6 +376,67 @@ def pack_by_columns(widths, max_lines, canvas=512):
     return batches
 
 
+class LineBatch(NamedTuple):
+    """One batch of restore_images, planned on the host (plan_batches).  Images are indices into the call's lists."""
+    crops: list         # encoder rows: (image, a, b), source columns resized onto the 32x512 canvas
+    lines: list         # decoder lines: (image, x0, x1), source columns
+    widths: list        # each decoder line's LQ width: Wc for a whole line wider than the canvas, else 512
+    counts: list        # characters per decoder line
+    labels: list        # the batch's labels, line by line, each line's in label order
+    owner: list         # the encoder row (index into crops) whose style each character takes: the crop that owns it
+    locs: torch.Tensor  # fp32 [lines, 2*max(1, max(counts))]: boxes_to_locs of each line's boxes at its width, zero-padded
+    pieces: list        # stitch: (line, src_x0, image, out_x0, width)
+    done: list          # images whose last line is in this batch: their figures are composed after it
+    reuse: bool         # every decoder line is its own encoder crop at 512: the decoder reads the encoder's LQ
+
+
+def plan_batches(shapes, labels, boxes, plans, max_lines, whole_lines=False):
+    """restore_images' batches, on the host.  shapes / labels / boxes / plans: per image, its (h, w), label list, detector boxes
+    and plan_segments' Segments; an image whose plan is None is left out.  A decoder line is one crop at 512 or, with
+    ``whole_lines``, a whole image wider than the canvas at Wc (whole_line_width).  Lines keep image and segment order;
+    pack_by_columns forms the batches (with every width 512: consecutive chunks of max_lines lines).
+    Returns ({image: output width}, [LineBatch])."""
+    from .ops import round_half_even
+    out_w, lines = {}, []       # (image, x0, x1, width, segment indices, boxes, [(src_x0, out_x0, width)])
+    for i, segs in enumerate(plans):
+        if segs is None:
+            continue
+        h, w = shapes[i]
+        wc = whole_line_width(h, w)[1] if whole_lines else 512
+        if wc > 512:
+            out_w[i] = min(round_half_even(w * (128 / h)), 4 * wc)
+            lines.append((i, 0, w, wc, range(len(segs)), boxes[i], [(0, 0, out_w[i])]))
+            continue
+        out_w[i], pieces = stitch_pieces(h, w, segs)
+        for k, s in enumerate(segs):
+            lines.append((i, *s.crop, 512, [k], s.boxes, [(src, x0, wd) for kk, x0, src, wd in pieces if kk == k]))
+    groups = pack_by_columns([line[3] for line in lines], max_lines)
+    last = {lines[j][0]: g for g, idx in enumerate(groups) for j in idx}
+    batches = []
+    for g, idx in enumerate(groups):
+        crops, dec, widths, counts, labs, owner, pieces = [], [], [], [], [], [], []
+        for b, j in enumerate(idx):
+            i, x0, x1, wd, ks, _, pcs = lines[j]
+            n0 = len(labs)
+            for k in ks:
+                s = plans[i][k]
+                owner += [len(crops)] * (s.chars[1] - s.chars[0])
+                labs += labels[i][s.chars[0]:s.chars[1]]
+                crops.append((i, *s.crop))
+            dec.append((i, x0, x1))
+            widths.append(wd)
+            counts.append(len(labs) - n0)
+            pieces += [(b, src, i, o0, pw) for src, o0, pw in pcs]
+        locs = torch.zeros(len(idx), 2 * max(1, max(counts)), dtype=torch.float32)
+        for b, j in enumerate(idx):
+            if counts[b]:
+                locs[b, :2 * counts[b]] = boxes_to_locs(lines[j][5], shapes[lines[j][0]][0], widths[b])[0]
+        done = [i for i in dict.fromkeys(i for i, _, _ in dec) if last[i] == g]
+        batches.append(LineBatch(crops, dec, widths, counts, labs, owner, locs, pieces, done,
+                                 crops == dec and max(widths) == 512))
+    return out_w, batches
+
+
 @torch.no_grad()
 def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, context=16, skip_invalid=False, to_host=False,
                    whole_lines=False, figure=False):
@@ -390,7 +461,8 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
     character's prior takes the style w of the crop that owns it.  Lines that fit the canvas are computed as without the flag.
     Decoder lines of different widths share a batch (TSPSRNet's ``widths``); a batch holds k lines only while
     k * (its widest Wc) <= max_lines * 512.  Per batch: one host->device copy, one crop kernel for the encoder crops, one for
-    the decoder lines, the encoder, one TSPGAN call, one ragged TSPSRNet call, the fp16-range re-run, one stitch kernel.
+    the decoder lines when the batch holds a line wider than the canvas, the encoder, one TSPGAN call, one ragged TSPSRNet call,
+    the fp16-range re-run, one stitch kernel.  Both modes run the batches of plan_batches through the same loop.
 
     ``figure=True`` (either mode) adds ``figure`` to every result: the uint8 [512, W_i, 3] image test_sr.py writes (:206-231;
     DESIGN.md section 7b) -- ShowLQ and ShowLocs (markers at locs = boxes_to_locs(boxes, h, Wc), img_max_width = 4*Wc), the
@@ -424,140 +496,39 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
             results[i] = dict(error=f"{type(e).__name__}: {e}")
             continue
         imgs[i], labs[i], plans[i] = img, lab, segs
-    valid = [i for i in range(n) if plans[i] is not None]
-    if not valid:
+    if all(p is None for p in plans):
         return results
-    if whole_lines:
-        return _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, results, max_lines, to_host, dev, figure)
+    out_w, batches = plan_batches([None if im is None else im.shape[:2] for im in imgs], labs, boxes, plans, max_lines,
+                                  whole_lines)
     rows = 512 if figure else 128
     with torch.cuda.device(dev):
-        layout, total = {}, 0
-        for i in valid:
-            width, pieces = stitch_pieces(imgs[i].shape[0], imgs[i].shape[1], plans[i])
-            layout[i] = (total, width, pieces)
-            total += rows * width * 3
+        offs, total = {}, 0
+        for i, wd in out_w.items():
+            offs[i] = total
+            total += rows * wd * 3
         flat = torch.empty(total, dtype=torch.uint8, device=dev)
-        figs = {i: flat[o:o + rows * wd * 3].view(rows, wd, 3) for i, (o, wd, _) in layout.items()}
+        figs = {i: flat[o:o + rows * out_w[i] * 3].view(rows, out_w[i], 3) for i, o in offs.items()}
         outs = {i: f[256:384] for i, f in figs.items()} if figure else figs
-        lines = [(i, k) for i in valid for k in range(len(plans[i]))]
-        last_batch = {i: b0 for b0 in range(0, len(lines), max_lines) for i, _ in lines[b0:b0 + max_lines]}
-        priors = {i: [] for i in valid}
-        for b0 in range(0, len(lines), max_lines):
-            batch = lines[b0:b0 + max_lines]
-            dimg = _device_images(dict.fromkeys(i for i, _ in batch), imgs, dev)
-            segs = [plans[i][k] for i, k in batch]
-            lq, _ = ops.preprocess_lq_crops([(dimg[i], s.crop[0], s.crop[1]) for (i, _), s in zip(batch, segs)])
-            counts = [s.chars[1] - s.chars[0] for s in segs]
-            lab_all = torch.tensor([v for (i, _), s in zip(batch, segs) for v in labs[i][s.chars[0]:s.chars[1]]],
-                                   dtype=torch.long).reshape(-1, 1)
-            locs = torch.zeros(len(batch), 2 * max(1, max(counts)), dtype=torch.float32)
-            for b, ((i, _), s) in enumerate(zip(batch, segs)):
-                if counts[b]:
-                    locs[b, :2 * counts[b]] = boxes_to_locs(s.boxes, imgs[i].shape[0], lq.shape[-1])[0]
-            for attempt in range(4):
-                _, _, w = encoder(lq)
-                p64, p32, img_p = [], [], None
-                if lab_all.shape[0] > 0:
-                    styles = torch.cat([w[b:b + 1].expand(c, -1) for b, c in enumerate(counts) if c > 0], dim=0)
-                    img_p, f64, f32_ = tspgan(styles=styles, labels=lab_all, noise=None)
-                    o = 0
-                    for c in counts:
-                        p64.append(f64[o:o + c]); p32.append(f32_[o:o + c]); o += c
-                else:
-                    p64 = [torch.zeros(0, 256, 64, 64, device=dev) for _ in counts]
-                    p32 = [torch.zeros(0, 512, 32, 32, device=dev) for _ in counts]
-                out = sr(lq, p64, p32, locs)
-                torch.cuda.synchronize(dev)
-                if not ops.poll_range(dev) or attempt == 3:
-                    break
-            pieces = []
-            for b, (i, k) in enumerate(batch):
-                for kk, x0, src, wd in layout[i][2]:
-                    if kk == k:
-                        pieces.append((b, src, outs[i][:, x0:x0 + wd]))
-            if pieces:
-                ops.postprocess_sr_pieces(out, pieces)
+        priors = {i: [] for i in out_w}
+        for bt in batches:
+            dimg = _device_images(dict.fromkeys(i for i, _, _ in bt.lines), imgs, dev)
+            lq, _ = ops.preprocess_lq_crops([(dimg[i], a, b) for i, a, b in bt.crops])
+            lq_sr = lq if bt.reuse else ops.preprocess_lq_crops([(dimg[i], a, b) for i, a, b in bt.lines], out_w=max(bt.widths))[0]
+            lab = list(torch.tensor(bt.labels, dtype=torch.long).reshape(-1, 1).split(bt.counts))
+            res = _rerun(lambda: _step(encoder, tspgan, sr, lq, lab, bt.locs, owner=bt.owner, lq_sr=lq_sr, widths=bt.widths), dev)
+            if bt.pieces:
+                ops.postprocess_sr_pieces(res["sr"], [(b, src, outs[i][:, x0:x0 + wd]) for b, src, i, x0, wd in bt.pieces])
             if figure:
-                o = 0
-                for (i, _), c in zip(batch, counts):            # crops in label order: the characters' priors in label order
-                    priors[i] += list(img_p[o:o + c]) if c else []
-                    o += c
-                done = [i for i in dict.fromkeys(i for i, _ in batch) if last_batch[i] == b0]
-                if done:
+                for (i, _, _), p in zip(bt.lines, res["prior"]):      # lines in label order: the priors in label order
+                    priors[i] += list(p)
+                if bt.done:
                     ops.figure_panels([(dimg[i], figs[i]) + _figure_markers_for(*imgs[i].shape[:2], boxes[i]) + (priors.pop(i),)
-                                       for i in done])
+                                       for i in bt.done])
         if to_host:
             pinned = _to_host(flat)
-            figs = {i: pinned[o:o + rows * wd * 3].view(rows, wd, 3).numpy() for i, (o, wd, _) in layout.items()}
+            figs = {i: pinned[o:o + rows * out_w[i] * 3].view(rows, out_w[i], 3).numpy() for i, o in offs.items()}
             outs = {i: f[256:384] for i, f in figs.items()} if figure else figs
-    for i in valid:
-        results[i] = dict(sr_u8=outs[i], segments=plans[i])
-        if figure:
-            results[i]["figure"] = figs[i]
-    return results
-
-
-def _restore_whole_lines(encoder, tspgan, sr, imgs, labs, boxes, plans, valid, results, max_lines, to_host, dev, figure):
-    """restore_images(whole_lines=True) after validation: one decoder line per image (see restore_images)."""
-    from . import ops
-    rows = 512 if figure else 128
-    with torch.cuda.device(dev):
-        geo = {i: whole_line_width(imgs[i].shape[0], imgs[i].shape[1]) for i in valid}
-        layout, total = {}, 0
-        for i in valid:
-            h, w = imgs[i].shape[:2]
-            wc = geo[i][1]
-            width = min(ops.round_half_even(w * (128 / h)), 4 * wc)
-            layout[i] = (total, width)
-            total += rows * width * 3
-        flat = torch.empty(total, dtype=torch.uint8, device=dev)
-        figs = {i: flat[o:o + rows * wd * 3].view(rows, wd, 3) for i, (o, wd) in layout.items()}
-        outs = {i: f[256:384] for i, f in figs.items()} if figure else figs
-        for bidx in pack_by_columns([geo[i][1] for i in valid], max_lines):
-            batch = [valid[j] for j in bidx]
-            dimg = _device_images(batch, imgs, dev)
-            crops = [(i, s) for i in batch for s in plans[i]]              # encoder crops, 512 canvas
-            lq_enc, _ = ops.preprocess_lq_crops([(dimg[i], s.crop[0], s.crop[1]) for i, s in crops])
-            widths = [geo[i][1] for i in batch]
-            canvas = max(widths)
-            if canvas == 512:                 # only lines that fit: each is its single crop, exactly as without whole_lines
-                lq = lq_enc
-            else:
-                lq, _ = ops.preprocess_lq_crops([(dimg[i], 0, imgs[i].shape[1]) for i in batch], out_w=canvas)
-            counts = [len(labs[i]) for i in batch]
-            owner = []                                                   # encoder crop (row of lq_enc) of every character
-            c0 = 0
-            for i in batch:
-                for s in plans[i]:
-                    owner += [c0] * (s.chars[1] - s.chars[0])
-                    c0 += 1
-            owner_t = torch.tensor(owner, dtype=torch.long).to(dev, non_blocking=True)
-            lab_all = torch.tensor([v for i in batch for v in labs[i]], dtype=torch.long).reshape(-1, 1)
-            locs = torch.zeros(len(batch), 2 * max(counts), dtype=torch.float32)
-            for b, i in enumerate(batch):
-                locs[b, :2 * counts[b]] = boxes_to_locs(boxes[i], imgs[i].shape[0], widths[b])[0]
-            for attempt in range(4):
-                _, _, w = encoder(lq_enc)
-                img_p, f64, f32_ = tspgan(styles=w.index_select(0, owner_t), labels=lab_all, noise=None)
-                p64, p32, o = [], [], 0
-                for c in counts:
-                    p64.append(f64[o:o + c]); p32.append(f32_[o:o + c]); o += c
-                out = sr(lq, p64, p32, locs, widths=widths)
-                torch.cuda.synchronize(dev)
-                if not ops.poll_range(dev) or attempt == 3:
-                    break
-            ops.postprocess_sr_pieces(out, [(b, 0, outs[i]) for b, i in enumerate(batch)])
-            if figure:                                          # every image of the batch is complete
-                offs = [0]
-                for c in counts:
-                    offs.append(offs[-1] + c)
-                ops.figure_panels([(dimg[i], figs[i]) + _figure_markers_for(*imgs[i].shape[:2], boxes[i]) +
-                                   (list(img_p[offs[b]:offs[b + 1]]),) for b, i in enumerate(batch)])
-        if to_host:
-            pinned = _to_host(flat)
-            figs = {i: pinned[o:o + rows * wd * 3].view(rows, wd, 3).numpy() for i, (o, wd) in layout.items()}
-            outs = {i: f[256:384] for i, f in figs.items()} if figure else figs
-    for i in valid:
+    for i in out_w:
         results[i] = dict(sr_u8=outs[i], segments=plans[i])
         if figure:
             results[i]["figure"] = figs[i]
