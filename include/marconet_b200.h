@@ -393,6 +393,35 @@ typedef struct {
 } mn_figure_image;
 int mn_figure_u8(const mn_figure_image* images, int n_images, int max_width, void* stream);
 
+/* Characters predicted by TextContextEncoderV2 on detection windows (DESIGN.md section 7b, "Predicted characters"), one CTA per
+ * encoder row b < n_rows, the record rows[b] telling where the window lies and where its result goes:
+ *   1. idx[t] = argmax over the C classes of logits[b][t] (t < T <= 64), torch.max(dim) semantics: the first maximal index wins,
+ *      a NaN is larger than any number (the first NaN wins);
+ *   2. CTC collapse (test_w.py:34-40): keep t iff (t == 0 || idx[t] != idx[t-1]) && idx[t] < n_alphabet; the first
+ *      MN_PRED_SLOTS kept indices are the decoded characters, character j taking box slot j;
+ *   3. box: l = locs_lr[b][2j], r = locs_lr[b][2j+1]; c = (r+l)/2, hw = (r-l)/2 in fp32 (tspgan_model.py:331-337); in fp64
+ *      x1 = a + (c - hw)*scale, x2 = a + (c + hw)*scale, each operation rounded on its own (no contraction);
+ *   4. core: the character is kept iff lo <= (x1+x2)/2 < hi (a NaN centre is never kept).
+ * out receives the kept characters compacted in decode order (label, x1, x2; unused slots label -1, x1 = x2 = 0), n_kept and
+ * n_decoded (the decoded count before the core test).  logits: fp32 rows `logits_row_stride` elements apart, each [T][C] dense,
+ * C % 4 == 0 and 16-byte aligned; locs_lr: fp32 rows `locs_row_stride` apart, 2*MN_PRED_SLOTS values each.  rows: DEVICE
+ * array (validated by the caller). */
+#define MN_PRED_SLOTS 16
+typedef struct {
+    double x1[MN_PRED_SLOTS];
+    double x2[MN_PRED_SLOTS];
+    int32_t label[MN_PRED_SLOTS];
+    int32_t n_kept, n_decoded;
+} mn_char_pred;
+typedef struct {
+    double a;                   /* source column of the window's first column */
+    double scale;               /* source columns per unit of canvas width: 16*h for a 32x512 canvas */
+    double lo, hi;              /* the window's core [lo, hi) in source columns (+-inf at the line's ends) */
+    mn_char_pred* out;
+} mn_pred_row;
+int mn_decode_predictions(const float* logits, long long logits_row_stride, int T, int C, const float* locs_lr, long long locs_row_stride,
+                          const mn_pred_row* rows, int n_rows, int n_alphabet, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -64,6 +64,18 @@ class FigureImage(Structure):
                 ("h", c_int32), ("w", c_int32), ("S", c_int32), ("W", c_int32), ("n_top", c_int32), ("n_bot", c_int32), ("n_chars", c_int32)]
 
 
+PRED_SLOTS = 16     # MN_PRED_SLOTS
+
+
+class CharPred(Structure):
+    _fields_ = [("x1", c_double * PRED_SLOTS), ("x2", c_double * PRED_SLOTS), ("label", c_int32 * PRED_SLOTS), ("n_kept", c_int32),
+                ("n_decoded", c_int32)]
+
+
+class PredRow(Structure):
+    _fields_ = [("a", c_double), ("scale", c_double), ("lo", c_double), ("hi", c_double), ("out", c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -111,6 +123,7 @@ SYMBOLS = {
     "mn_postprocess_sr_u8_pieces": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_int, c_int, c_int, c_void_p, c_int, c_int,
                                             c_void_p]),
     "mn_figure_u8": (c_int, [c_void_p, c_int, c_int, c_void_p]),
+    "mn_decode_predictions": (c_int, [c_void_p, c_longlong, c_int, c_int, c_void_p, c_longlong, c_void_p, c_int, c_int, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -1024,3 +1024,48 @@ def figure_panels(items):
     buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
     _lib.check(_lib.load().mn_figure_u8(_ptr(buf), len(recs), mx, _stream()), "mn_figure_u8")
     LAUNCHES += 1
+
+
+# ---- characters predicted by the encoder on detection windows (DESIGN.md 7b, "Predicted characters") -----------------
+PRED_SLOTS = _lib.PRED_SLOTS
+
+
+def pred_dtype():
+    """numpy view of an mn_char_pred record (the output of mn_decode_predictions)."""
+    import numpy as np
+    return np.dtype([("x1", "<f8", PRED_SLOTS), ("x2", "<f8", PRED_SLOTS), ("label", "<i4", PRED_SLOTS), ("n_kept", "<i4"),
+                     ("n_decoded", "<i4")])
+
+
+def prediction_table(windows, device):
+    """windows: one (a, scale, lo, hi) per encoder row -- the window's first source column, source columns per unit of canvas
+    width (16*h), its core [lo, hi) -> (rows, out): the device table of mn_pred_row records and the device buffer of
+    mn_char_pred records they point to (row r writes record r; read it back as ``pred_dtype()``)."""
+    if not windows:
+        raise ValueError("prediction_table: no rows")
+    isz = ctypes.sizeof(_lib.CharPred)
+    out = torch.empty(len(windows) * isz, dtype=torch.uint8, device=device)
+    recs = [_lib.PredRow(float(a), float(s), float(lo), float(hi), out.data_ptr() + r * isz) for r, (a, s, lo, hi) in enumerate(windows)]
+    return _table(_lib.PredRow, recs, device), out
+
+
+def decode_predictions(logits, locs_lr, rows, first=0, n_alphabet=6735):
+    """mn_decode_predictions, one launch: encoder row b of logits (fp32 [B, T, 6736], T <= 64) and locs_lr (fp32 [B, 32], the
+    (left, right) pairs) -> argmax, CTC collapse, the first 16 characters' boxes in source columns and the core test, into the
+    record that entry first + b of ``rows`` (prediction_table) points to.  Both tensors are read in place."""
+    global LAUNCHES
+    _require_cuda(logits, "logits")
+    _require_cuda(locs_lr, "locs_lr")
+    if logits.dtype != torch.float32 or logits.dim() != 3 or logits.stride(2) != 1 or logits.stride(1) != logits.shape[2]:
+        raise RuntimeError("decode_predictions: logits must be fp32 [B, T, C] with dense rows")
+    b, t, c = logits.shape
+    if locs_lr.dtype != torch.float32 or locs_lr.dim() != 2 or locs_lr.shape[0] != b or locs_lr.shape[1] < 2 * PRED_SLOTS \
+            or locs_lr.stride(1) != 1:
+        raise RuntimeError(f"decode_predictions: locs_lr must be fp32 [{b}, >= {2 * PRED_SLOTS}] with dense rows")
+    if not isinstance(rows, torch.Tensor) or rows.device != logits.device or rows.dtype != torch.uint8 \
+            or not 0 <= first or (first + b) * ctypes.sizeof(_lib.PredRow) > rows.numel():
+        raise ValueError(f"decode_predictions: rows [{first}, {first + b}) are not in the table")
+    _lib.check(_lib.load().mn_decode_predictions(_ptr(logits), logits.stride(0), t, c, _ptr(locs_lr), locs_lr.stride(0),
+                                                 rows.data_ptr() + first * ctypes.sizeof(_lib.PredRow), b, n_alphabet, _stream()),
+               "mn_decode_predictions")
+    LAUNCHES += 1

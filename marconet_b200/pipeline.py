@@ -3,8 +3,9 @@
 The reference's ``test_sr.py`` takes character labels and boxes from a third-party YOLO + OCR front-end; the original
 single-model flow uses the encoder's own predictions instead: CTC-style de-duplicated argmax labels (test_w.py:34-40) and
 boxes converted from the encoder's (left, right) pairs to (centre, half-width) exactly as the training model does
-(Train/tspgan/models/tspgan_model.py:331-337).  Integer outputs (labels) are computed on the host, bit-exactly like the
-reference; everything numeric runs through the module API (and therefore through the CUDA kernels).
+(Train/tspgan/models/tspgan_model.py:331-337).  restore_lines decodes labels on the host, bit-exactly like the reference;
+predict_characters decodes them, and the boxes, on the device (mn_decode_predictions) for images of any width.  Everything
+numeric runs through the module API (and therefore through the CUDA kernels).
 """
 import threading
 from typing import NamedTuple
@@ -142,16 +143,38 @@ def _to_host(flat):
 
 
 @torch.no_grad()
-def restore_image(encoder, tspgan, sr, img_u8, labels, boxes, figure=False):
+def restore_image(encoder, tspgan, sr, img_u8, labels=None, boxes=None, figure=False):
     """One text-line image end to end on the device (the body of test_sr.py's loop, :98-201, with the labels / boxes the
     detector and OCR produced): uint8 [h, w, 3] image (host numpy / tensor or CUDA tensor) -> dict(sr_u8 [128, W, 3] uint8 bytes
     as cv2.imwrite would store them, cropped to the line's width; sr fp32; lq; lq_width).
     Pre- and post-processing run as CUDA kernels (mn_preprocess_lq_u8 / mn_postprocess_sr_u8).
     ``figure=True`` adds ``figure``: the uint8 [512, W, 3] image test_sr.py writes (:206-231; ShowLQ, ShowLocs, ShowSR, prior;
-    DESIGN.md section 7b), composed on the device (mn_figure_u8); ``sr_u8`` is then its view ``figure[256:384]``."""
+    DESIGN.md section 7b), composed on the device (mn_figure_u8); ``sr_u8`` is then its view ``figure[256:384]``.
+    ``boxes=None``: the encoder predicts them (predict_characters), and the labels too when ``labels`` is None (given labels are
+    paired in order with the predicted boxes); the result then gains ``labels`` and ``boxes``.  Only for a line that fits the
+    canvas: restore_images predicts on lines of any width."""
+    img = torch.as_tensor(img_u8)
+    h = img.shape[0]
+    predicted = None
+    if boxes is None:
+        img = _as_image(img, 0)
+        lq_w = whole_line_width(h, img.shape[1])[0]
+        if lq_w > 512:
+            raise ValueError(f"LQ width {lq_w} exceeds 512: restore_image predicts characters only on a line that fits the "
+                             f"canvas; restore_images(..., labels=None, boxes=None) reads lines of any width")
+        labels, boxes = predicted = _use_prediction(0, labels, _predict(encoder, [img], 1, 64)[0])
+    elif labels is None:
+        raise ValueError("boxes without labels (predicted labels pair only with predicted boxes)")
+    res = _restore_one(encoder, tspgan, sr, img, labels, boxes, figure)
+    if predicted is not None:
+        res["labels"], res["boxes"] = predicted
+    return res
+
+
+def _restore_one(encoder, tspgan, sr, img, labels, boxes, figure):
+    """restore_image with labels and boxes."""
     from . import ops
     dev = next(encoder.parameters()).device
-    img = torch.as_tensor(img_u8)
     h = img.shape[0]
     img = img.to(dev, non_blocking=True).contiguous()
     lq, lq_w = ops.preprocess_lq(img)
@@ -437,9 +460,117 @@ def plan_batches(shapes, labels, boxes, plans, max_lines, whole_lines=False):
     return out_w, batches
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# Predicted characters (DESIGN.md section 7b).  Without a detector, the encoder's own CTC labels and (left, right) boxes stand in
+# for test_sr.py's YOLO + OCR front-end: the line is read through detection windows that fit the canvas, each window's characters
+# are decoded on the device (mn_decode_predictions), and a character belongs to the window whose core holds its box centre.
+# ---------------------------------------------------------------------------------------------------------------------
+class Window(NamedTuple):
+    """One detection window of a text-line image: ``crop`` [a, b) the source columns the encoder reads (resized onto the 32x512
+    canvas as test_sr.py resizes a hand-cut crop), ``core`` [lo, hi) the source columns whose predicted characters it owns."""
+    crop: tuple
+    core: tuple
+
+
+def plan_windows(h, w, canvas=512, overlap=64):
+    """Where the encoder looks on an h x w image.  A line that fits (round_half_even(w*32/h) <= canvas) is one window (0, w) whose
+    core is the whole real line.  A wider one: windows of W* = (2*canvas-1)*h // 64 source columns (the widest crop that fits the
+    canvas, as in plan_segments) at stride s = W* - v, v = ceil(overlap*h/32) (``overlap`` LQ pixels), K = 1 + ceil((w-W*)/s)
+    windows, the last one [w - W*, w).  The core boundary between windows k and k+1 is floor((a_k+1 + b_k)/2); the first core
+    starts at -inf and the last ends at +inf, so the cores partition the real line."""
+    from .ops import round_half_even
+    h, w = int(h), int(w)
+    if h < 1 or w < 1:
+        raise ValueError(f"empty image ({h}x{w})")
+    if not 0 <= overlap <= 256:
+        raise ValueError(f"overlap must lie in [0, 256] LQ pixels, got {overlap}")
+    inf = float("inf")
+    if round_half_even(w * (32 / h)) <= canvas:
+        return [Window((0, w), (-inf, inf))]
+    wmax = (2 * canvas - 1) * h // 64
+    s = wmax - (-(-int(overlap) * h // 32))
+    k = 1 + -(-(w - wmax) // s)
+    crops = [(j * s, j * s + wmax) for j in range(k - 1)] + [(w - wmax, w)]
+    cuts = [-inf] + [(crops[j + 1][0] + crops[j][1]) // 2 for j in range(k - 1)] + [inf]
+    return [Window(crops[j], (cuts[j], cuts[j + 1])) for j in range(k)]
+
+
+def merge_predictions(h, w, windows, rows):
+    """One image's characters from its windows' decoded rows: rows[k] = (labels, x1s, x2s), the characters window k kept in
+    decode order with their boxes in source columns.  Concatenated in window order, each box clamped to the image
+    ([clamp(min(x1, x2), 0, w), 0, clamp(max(x1, x2), 0, w), h]), then stable-sorted by box centre (pairs stay together).
+    Returns (labels, boxes)."""
+    pairs = []
+    for (labs, x1s, x2s), _ in zip(rows, windows):
+        for lab, x1, x2 in zip(labs, x1s, x2s):
+            lo, hi = min(max(min(x1, x2), 0.0), float(w)), min(max(max(x1, x2), 0.0), float(w))
+            pairs.append((int(lab), [lo, 0, hi, h]))
+    pairs.sort(key=lambda p: (p[1][0] + p[1][2]) / 2.0)
+    return [p[0] for p in pairs], [p[1] for p in pairs]
+
+
+def _predict(encoder, imgs, max_lines, overlap):
+    """predict_characters on validated uint8 [h, w, 3] tensors."""
+    from . import ops
+    dev = next(encoder.parameters()).device
+    plans = [plan_windows(im.shape[0], im.shape[1], overlap=overlap) for im in imgs]
+    rows = [(i, k) for i, p in enumerate(plans) for k in range(len(p))]
+    if not rows:
+        return []
+    with torch.cuda.device(dev):
+        table, out = ops.prediction_table([(plans[i][k].crop[0], 16.0 * imgs[i].shape[0], *plans[i][k].core) for i, k in rows], dev)
+        dimg = _device_images(range(len(imgs)), imgs, dev)
+        for r0 in range(0, len(rows), max_lines):
+            batch = rows[r0:r0 + max_lines]
+            lq, _ = ops.preprocess_lq_crops([(dimg[i], *plans[i][k].crop) for i, k in batch])
+            logits, locs_lr, _ = encoder(lq)
+            ops.decode_predictions(logits, locs_lr, table, r0)
+        rec = _to_host(out).numpy().view(ops.pred_dtype())
+    res, r = [], 0
+    for i, p in enumerate(plans):
+        dec = []
+        for k in range(len(p)):
+            n = int(rec[r]["n_kept"])
+            dec.append((rec[r]["label"][:n].tolist(), rec[r]["x1"][:n].tolist(), rec[r]["x2"][:n].tolist()))
+            r += 1
+        labels, boxes = merge_predictions(imgs[i].shape[0], imgs[i].shape[1], p, dec)
+        res.append(dict(labels=labels, boxes=boxes, windows=p))
+    return res
+
+
 @torch.no_grad()
-def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, context=16, skip_invalid=False, to_host=False,
-                   whole_lines=False, figure=False):
+def predict_characters(encoder, images, max_lines=8, overlap=64):
+    """The characters TextContextEncoderV2 predicts on text-line images of any width, in place of a detector + OCR front-end
+    (the reference's single-model flow, SURVEY.md section 8f row n3; DESIGN.md section 7b, "Predicted characters").
+
+    images: uint8 [h, w, 3] numpy arrays or CPU / CUDA tensors.  Each image is read through plan_windows' detection windows, each
+    window resized onto the 32x512 canvas exactly as preprocess_lq_crops resizes a crop.  Per batch of at most ``max_lines``
+    windows (image, then window order): one crop launch, the encoder, one mn_decode_predictions launch (argmax, CTC collapse,
+    first 16 characters, boxes in source columns, core test) into one device table for the call; then one pinned device->host
+    copy and one synchronisation.  Host images go to the device once, in one pinned copy.
+    Returns one dict per image: labels (ints), boxes ([x1, 0, x2, h] floats, clamped to the image, sorted by centre; what
+    restore_images takes) and windows (the plan)."""
+    if max_lines < 1:
+        raise ValueError("max_lines must be >= 1")
+    return _predict(encoder, [_as_image(im, i) for i, im in enumerate(images)], max_lines, overlap)
+
+
+def _use_prediction(i, lab, pred):
+    """The labels and boxes image i restores with, given its prediction: the predicted ones, or the given labels paired in
+    order with the predicted boxes (the reference README's manual-label mode)."""
+    if lab is None:
+        if not pred["labels"]:
+            raise ValueError(f"image {i}: the encoder predicted no character")
+        return list(pred["labels"]), pred["boxes"]
+    lab = [int(v) for v in torch.as_tensor(lab, dtype=torch.long).reshape(-1).tolist()]
+    if len(lab) != len(pred["labels"]):
+        raise ValueError(f"image {i}: {len(lab)} labels given, the encoder predicted {len(pred['labels'])} characters")
+    return lab, pred["boxes"]
+
+
+@torch.no_grad()
+def restore_images(encoder, tspgan, sr, images, labels=None, boxes=None, max_lines=8, context=16, skip_invalid=False,
+                   to_host=False, whole_lines=False, figure=False, overlap=64):
     """Text-line images of any sizes end to end, batched: the flow of restore_image for every image, each cut into crops that
     fit the 32x512 LQ canvas (plan_segments) and every crop of every image run as one line of a batch of at most ``max_lines``.
 
@@ -469,9 +600,19 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
     image's sr_u8, and the priors this call generated (each character's in the style of the crop that owns it), all cropped to
     sr_u8's width.  ``sr_u8`` becomes the view ``figure[256:384]``, its bytes unchanged.  The batch that holds an image's last
     crop composes its figure: one more launch (mn_figure_u8) per batch, and the prior images are kept until then.  With
-    ``to_host`` the figures come back through the same single pinned copy.  Error entries have no figure."""
+    ``to_host`` the figures come back through the same single pinned copy.  Error entries have no figure.
+
+    Without a detector: ``labels`` / ``boxes`` may be None, or lists with None entries.  An image whose boxes are None is first
+    read by the encoder (predict_characters, with ``max_lines`` and ``overlap``): labels None takes the predicted labels and
+    boxes; given labels are paired in order with the predicted boxes (their counts must match).  Labels None with given boxes
+    is a ValueError.  The call then is restore_images(images, labels, boxes) with the predicted values, every option applying on
+    top, and those results gain ``labels`` and ``boxes`` (what the restoration used).  No character predicted, a count mismatch
+    or a predicted box plan_segments rejects are ValueErrors naming the image (error entries with ``skip_invalid``).  Images
+    with both labels and boxes given do not enter the prediction stage."""
     from . import ops
     n = len(images)
+    labels = [None] * n if labels is None else labels
+    boxes = [None] * n if boxes is None else boxes
     if not (len(labels) == len(boxes) == n):
         raise ValueError(f"{n} images, {len(labels)} label lists, {len(boxes)} box lists")
     if max_lines < 1:
@@ -479,10 +620,32 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
     dev = next(encoder.parameters()).device
     n_cls = tspgan.TextGenerator.input_text.TextEmbeddings.shape[0]
     results, imgs, labs, plans = [None] * n, [None] * n, [None] * n, [None] * n
+    boxes, predicted, ask = list(boxes), {}, {}
+    for i in range(n):                                   # the prediction stage: images without boxes
+        try:
+            if boxes[i] is None:
+                ask[i] = _as_image(images[i], i)
+            elif labels[i] is None:
+                raise ValueError(f"image {i}: boxes without labels (predicted labels pair only with predicted boxes)")
+        except ValueError as e:
+            if not skip_invalid:
+                raise
+            results[i] = dict(error=f"{type(e).__name__}: {e}")
+    for i, pred in zip(ask, _predict(encoder, list(ask.values()), max_lines, overlap) if ask else []):
+        try:
+            predicted[i] = _use_prediction(i, labels[i], pred)
+            boxes[i] = predicted[i][1]
+        except ValueError as e:
+            if not skip_invalid:
+                raise
+            results[i] = dict(error=f"{type(e).__name__}: {e}")
     for i in range(n):
+        if results[i] is not None:
+            continue
         try:
             img = _as_image(images[i], i)
-            lab = [int(v) for v in torch.as_tensor(labels[i], dtype=torch.long).reshape(-1).tolist()]
+            lab = predicted[i][0] if i in predicted else \
+                [int(v) for v in torch.as_tensor(labels[i], dtype=torch.long).reshape(-1).tolist()]
             if not lab:
                 raise ValueError(f"image {i}: no character labels (test_sr.py:168-170 skips such images)")
             segs = plan_segments(img.shape[0], img.shape[1], boxes[i], labels=lab, context=context, name=f"image {i}")
@@ -532,6 +695,8 @@ def restore_images(encoder, tspgan, sr, images, labels, boxes, max_lines=8, cont
         results[i] = dict(sr_u8=outs[i], segments=plans[i])
         if figure:
             results[i]["figure"] = figs[i]
+        if i in predicted:
+            results[i]["labels"], results[i]["boxes"] = predicted[i]
     return results
 
 

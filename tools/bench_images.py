@@ -2,7 +2,7 @@
 pipeline.restore_images at max_lines 1, 4 and 8, against the loop a user writes today -- restore_image on each crop of the same
 plan, then a device->host copy of its bytes.
 
-    python tools/bench_images.py [--images 42] [--passes 3] [--warmup 1] [--whole-lines | --figures]
+    python tools/bench_images.py [--images 42] [--passes 3] [--warmup 1] [--whole-lines | --figures | --predicted]
 
 --whole-lines compares the two ways restore_images decodes a line wider than the canvas, at max_lines 1 and 8: crop by crop
 (the default) and in one piece (whole_lines=True), with the arms' passes alternated, and reports each mode's decoder SR columns
@@ -13,6 +13,12 @@ device, one pinned copy back), and the host path a user has without it -- restor
 image copied back (fp32 [3, 128, 128]) and the figure composed with cv2 as test_sr.py:206-231 does (ShowLQ cubic resize, markers,
 INTER_LINEAR prior strip, vstack).  The host arm reads priors generated once before timing (the generator's work is already
 inside restore_images; only the copy back and the cv2 work are added).
+
+--predicted times restore_images at max_lines 8 with the set's labels and boxes given against labels=None, boxes=None (the
+encoder predicts both on its detection windows first, pipeline.predict_characters; skip_invalid, since the synthetic weights'
+boxes need not fit a plan), and predict_characters alone, whose time over the predicted arm's is the share spent in detection.
+Run it with MN_MODULE_GRAPHS=0: the synthetic weights predict 16 characters on every crop, and six recorded TSPSRNet signatures
+of such batches outgrow an 80 GB card.
 
 The image set reuses the 17 (h, w) sizes of the reference's Testsets/LQs (resized LQ widths 92 to 464 pixels, all inside the
 512-pixel canvas) and adds lines 2 to 4 times wider than the canvas, which test_sr.py refuses (:107-110), with one character box
@@ -111,6 +117,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=1, help="untimed passes per arm first")
     ap.add_argument("--whole-lines", action="store_true", help="crop-by-crop vs whole-line decoding of the wide lines")
     ap.add_argument("--figures", action="store_true", help="test_sr.py's figure on the device vs on the host with cv2")
+    ap.add_argument("--predicted", action="store_true", help="given labels and boxes vs encoder-predicted ones")
     args = ap.parse_args()
     from marconet_b200 import pipeline
     from marconet_b200.models import networks
@@ -139,6 +146,11 @@ def main():
 
     if args.figures:
         arms = figure_arms(enc, gen, sr, images, labels, boxes, dev)
+    elif args.predicted:
+        arms = {"restore_images_max_lines_8": lambda: pipeline.restore_images(enc, gen, sr, images, labels, boxes, max_lines=8, to_host=True),
+                "restore_images_max_lines_8_predicted": lambda: pipeline.restore_images(enc, gen, sr, images, None, None, max_lines=8,
+                                                                                         to_host=True, skip_invalid=True),
+                "predict_characters_max_lines_8": lambda: pipeline.predict_characters(enc, images, max_lines=8)}
     elif args.whole_lines:
         arms = {f"restore_images{'_whole_lines' if wl else ''}_max_lines_{m}":
                 (lambda m=m, wl=wl: pipeline.restore_images(enc, gen, sr, images, labels, boxes, max_lines=m, to_host=True, whole_lines=wl))
@@ -165,6 +177,13 @@ def main():
             out[name] = {"s_per_pass": s, "images_per_sec": len(images) / s, "chars_per_sec": n_chars / s}
             if args.whole_lines:
                 out[name]["decoder_sr_columns_per_pass"] = sr_columns(name, images, plans)
+        if args.predicted:
+            res = pipeline.restore_images(enc, gen, sr, images, None, None, max_lines=8, to_host=True, skip_invalid=True)
+            out["restore_images_max_lines_8_predicted"].update(
+                restored=sum("error" not in r for r in res), predicted_chars=sum(len(r.get("labels", [])) for r in res),
+                windows=sum(len(pipeline.plan_windows(*im.shape[:2])) for im in images))
+            out["detection_share"] = out["predict_characters_max_lines_8"]["s_per_pass"] / \
+                out["restore_images_max_lines_8_predicted"]["s_per_pass"]
     card = {"name": torch.cuda.get_device_name(dev)}
     try:
         q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
