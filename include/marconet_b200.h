@@ -421,6 +421,40 @@ typedef struct {
 } mn_pred_row;
 int mn_decode_predictions(const float* logits, long long logits_row_stride, int T, int C, const float* locs_lr, long long locs_row_stride,
                           const mn_pred_row* rows, int n_rows, int n_alphabet, void* stream);
+/* Every character the encoder reads on a line that fits the canvas (test_w.py:34-40, 99: all of clear_labels(logits[0]), no cap):
+ * steps 1-2 of mn_decode_predictions (the same argmax and CTC collapse) over all T <= 64 timesteps of row b < n_rows of logits,
+ * one CTA per row.  out[b] receives the count n and the labels in timestep order (unused slots -1); the first
+ * min(n, MN_PRED_SLOTS) labels are the characters mn_decode_predictions decodes on the same row. */
+#define MN_LABEL_SLOTS 64
+typedef struct {
+    int32_t n;
+    int32_t label[MN_LABEL_SLOTS];
+} mn_label_row;
+int mn_decode_labels(const float* logits, long long logits_row_stride, int T, int C, mn_label_row* out, int n_rows, int n_alphabet,
+                     void* stream);
+
+/* Font-style interpolation (test_w.py:107, new_w = w1*scale + w2*(1-scale)) for every style row of a sweep in one launch:
+ *   out[r*out_stride + d] = fl(fl(w[w1*w_stride + d] * s) + fl(w[w2*w_stride + d] * t)),   d < dim,
+ * each multiply and the add rounded on its own (no FMA): the bits of torch's fp32 ``w1 * s + w2 * (1 - s)`` for s = float32(scale)
+ * and t = float32(1 - scale), 1 - scale computed in double.  rows: DEVICE array of n_rows records (indices validated by the
+ * caller); w: the encoder style rows. */
+typedef struct {
+    int32_t w1, w2;             /* rows of w: the content character's style and the donor's */
+    float s, t;
+} mn_lerp_row;
+int mn_style_lerp(const float* w, int w_stride, const mn_lerp_row* rows, int n_rows, int dim, float* out, int out_stride, void* stream);
+
+/* The 8-bit strip test_w.py writes per style (:109-114, cv2.imwrite(hstack(prior*0.5+0.5)*255.0)), tile by tile: generator image
+ * n < n_rows (fp32 [3][128][128] in [-1, 1], addressed through element strides: the channels_last output is read in place) goes
+ * to the 128 x 128 x 3 tile at tiles[n].dst, rows tiles[n].dst_pitch bytes apart:
+ *   dst[y*pitch + x*3 + c] = saturate_u8(cvRound(fl(fl(fl(p*0.5) + 0.5) * 255))),   not channel-flipped,
+ * the arithmetic of panel 4 of mn_figure_u8 at its identity width.  tiles: DEVICE array (validated by the caller). */
+typedef struct {
+    uint8_t* dst;               /* row 0, first column of the tile */
+    int64_t dst_pitch;          /* bytes between rows of the strip */
+} mn_prior_tile;
+int mn_prior_tiles_u8(const float* priors, long long stride_n, long long stride_c, long long stride_h, long long stride_w,
+                      const mn_prior_tile* tiles, int n_rows, void* stream);
 
 #ifdef __cplusplus
 }

@@ -76,6 +76,21 @@ class PredRow(Structure):
     _fields_ = [("a", c_double), ("scale", c_double), ("lo", c_double), ("hi", c_double), ("out", c_void_p)]
 
 
+LABEL_SLOTS = 64    # MN_LABEL_SLOTS
+
+
+class LabelRow(Structure):
+    _fields_ = [("n", c_int32), ("label", c_int32 * LABEL_SLOTS)]
+
+
+class LerpRow(Structure):
+    _fields_ = [("w1", c_int32), ("w2", c_int32), ("s", c_float), ("t", c_float)]
+
+
+class PriorTile(Structure):
+    _fields_ = [("dst", c_void_p), ("dst_pitch", c_int64)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -124,6 +139,9 @@ SYMBOLS = {
                                             c_void_p]),
     "mn_figure_u8": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "mn_decode_predictions": (c_int, [c_void_p, c_longlong, c_int, c_int, c_void_p, c_longlong, c_void_p, c_int, c_int, c_void_p]),
+    "mn_decode_labels": (c_int, [c_void_p, c_longlong, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "mn_style_lerp": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "mn_prior_tiles_u8": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_void_p, c_int, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

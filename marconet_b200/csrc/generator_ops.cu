@@ -324,6 +324,20 @@ __global__ void check_labels_kernel(const int64_t* __restrict__ labels, int64_t*
     clamped[i] = l;
 }
 
+// ---------------------------------------------------------------- font-style interpolation (test_w.py:107)
+// One thread per (style row, 4 dims): new_w = w1*s + w2*t with each multiply and the add rounded on its own, as torch computes
+// ``w1 * scale + w2 * (1 - scale)`` on fp32 tensors (explicit-rounding intrinsics: nvcc must not contract into an FMA).
+__global__ void style_lerp_kernel(const float* __restrict__ w, int w_stride, const mn_lerp_row* __restrict__ rows, int n_rows,
+                                  int dim, float* __restrict__ out, int out_stride) {
+    mn_pdl_prologue();
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int r = (int)(i / dim), d = (int)(i % dim);
+    if (r >= n_rows) return;
+    const mn_lerp_row row = rows[r];
+    out[(long long)r * out_stride + d] = __fadd_rn(__fmul_rn(w[(long long)row.w1 * w_stride + d], row.s),
+                                                   __fmul_rn(w[(long long)row.w2 * w_stride + d], row.t));
+}
+
 }  // namespace
 
 extern "C" int mn_pixelnorm(const float* x, float* y, int N, int C, void* stream) {
@@ -418,6 +432,16 @@ extern "C" int mn_demod_batched(const float* s_all, int s_stride, const mn_demod
 extern "C" int mn_check_labels(const int64_t* labels, int64_t* clamped, int n, int classes, int32_t* err, void* stream) {
     MN_REQUIRE(labels && clamped && err && n > 0 && classes > 0, "mn_check_labels: bad args");
     MN_CUDA_CHECK((mn_launch(check_labels_kernel, dim3(mn_cdiv(n, 128)), dim3(128), 0, (cudaStream_t)stream, labels, clamped, n, classes, err)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_style_lerp(const float* w, int w_stride, const mn_lerp_row* rows, int n_rows, int dim, float* out, int out_stride,
+                             void* stream) {
+    MN_REQUIRE(w && rows && out && n_rows > 0 && dim > 0 && w_stride >= dim && out_stride >= dim, "mn_style_lerp: bad args");
+    const long long total = (long long)n_rows * dim;
+    MN_CUDA_CHECK((mn_launch(style_lerp_kernel, dim3((unsigned)mn_cdiv64(total, 256)), dim3(256), 0, (cudaStream_t)stream, w, w_stride,
+                             rows, n_rows, dim, out, out_stride)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

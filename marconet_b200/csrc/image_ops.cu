@@ -136,6 +136,12 @@ __device__ __forceinline__ float prior_value(const mn_figure_prior* __restrict__
     return __fadd_rn(__fmul_rn(p.img[c * p.stride_c + y * p.stride_h + x * p.stride_w], 0.5f), 0.5f);
 }
 
+// *255, cvRound and saturation: how cv2.imwrite stores a float prior value (test_sr.py:210-231, test_w.py:114).
+__device__ __forceinline__ uint8_t prior_u8(float v) {
+    const int q = __float2int_rn(__fmul_rn(v, 255.f));
+    return (uint8_t)min(max(q, 0), 255);
+}
+
 // blockIdx.y = image; one thread per pixel (y, x) of the 128 x max_width panel rows, those at x >= the image's W exit.
 // Panels 1-2 (ShowLQ, ShowLocs; test_sr.py:98,214-231) share one cubic resize (preprocess_lq_element at fx = fy = 128/h, the
 // vector / tail split taken at width S); panel 4 is OpenCV's float INTER_LINEAR of the prior strip to width S (test_sr.py:210),
@@ -183,9 +189,22 @@ __global__ void figure_kernel(const mn_figure_image* __restrict__ images, int ma
         const float v0 = prior_value(im.priors, sx >> 7, c, y, sx & 127);
         float v = v0;
         if (im.S != sw) v = __fadd_rn(__fmul_rn(v0, a0), __fmul_rn(prior_value(im.priors, s1 >> 7, c, y, s1 & 127), a1));
-        const int q = __float2int_rn(__fmul_rn(v, 255.f));
-        prow[c] = (uint8_t)min(max(q, 0), 255);          // not channel-flipped: the script writes the prior panel as RGB
+        prow[c] = prior_u8(v);                           // not channel-flipped: the script writes the prior panel as RGB
     }
+}
+
+// blockIdx.y = generator image n; one thread per pixel of its 128 x 128 tile: the figure's prior panel at its identity width.
+__global__ void prior_tiles_kernel(const float* __restrict__ priors, long long sn, long long sc, long long sh, long long sw,
+                                   const mn_prior_tile* __restrict__ tiles) {
+    mn_pdl_prologue();
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= 128 * 128) return;
+    const int x = idx & 127, y = idx >> 7;
+    const mn_figure_prior p{priors + blockIdx.y * sn, sc, sh, sw};
+    const mn_prior_tile t = tiles[blockIdx.y];
+    uint8_t* o = t.dst + (long long)y * t.dst_pitch + (long long)x * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = prior_u8(prior_value(&p, 0, c, y, x));
 }
 
 }  // namespace
@@ -239,6 +258,15 @@ extern "C" int mn_figure_u8(const mn_figure_image* images, int n_images, int max
     const long long total = 128ll * max_width;
     MN_CUDA_CHECK((mn_launch(figure_kernel, dim3((unsigned)mn_cdiv64(total, 256), n_images), dim3(256), 0, (cudaStream_t)stream,
                              images, max_width)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_prior_tiles_u8(const float* priors, long long stride_n, long long stride_c, long long stride_h, long long stride_w,
+                                 const mn_prior_tile* tiles, int n_rows, void* stream) {
+    MN_REQUIRE(priors && tiles && n_rows > 0 && n_rows <= 65535, "mn_prior_tiles_u8: bad args");
+    MN_CUDA_CHECK((mn_launch(prior_tiles_kernel, dim3(128 * 128 / 256, n_rows), dim3(256), 0, (cudaStream_t)stream, priors, stride_n,
+                             stride_c, stride_h, stride_w, tiles)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -1,6 +1,7 @@
 // Characters predicted by the encoder on detection windows (DESIGN.md 7b, "Predicted characters"): argmax over the classes of
 // every timestep, the CTC collapse of test_w.py:34-40, the (left, right) -> source-column box conversion and the window's core
-// test, for every window row of an encoder batch in one launch.  Each row reads its 64 x 6736 logits (1.7 MB) once: HBM and
+// test, for every window row of an encoder batch in one launch; mn_decode_labels shares the argmax and the collapse and keeps every
+// character of a row (test_w.py:99).  Each row reads its 64 x 6736 logits (1.7 MB) once: HBM and
 // launch-latency bound.  The fp64 box arithmetic uses explicit-rounding intrinsics so that nvcc cannot contract it into an FMA
 // the host twin (oracle/predict.py, Python floats) does not have.
 #include "mn_common.cuh"
@@ -18,13 +19,12 @@ __device__ __forceinline__ bool pred_better(float a, int ia, float b, int ib) {
     return a > b || (a == b && ia < ib);
 }
 
-__global__ void __launch_bounds__(kPredThreads) decode_predictions_kernel(
-        const float* __restrict__ logits, long long logits_row_stride, int T, int C, const float* __restrict__ locs_lr,
-        long long locs_row_stride, const mn_pred_row* __restrict__ rows, int n_alphabet) {
-    mn_pdl_prologue();
-    __shared__ int s_idx[kMaxT];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = kPredThreads / 32;
-    const float* row = logits + (long long)blockIdx.x * logits_row_stride;
+// Steps 1-2 of both decode kernels for the row at `row` (T x C fp32, dense): every warp of the CTA takes timesteps and writes
+// their torch.max(dim) argmax into s_idx; then warp 0 (the only warp that returns true) computes the CTC keep masks of timesteps
+// lane (m0) and lane + 32 (m1) of test_w.py:34-40.
+__device__ __forceinline__ bool decode_ctc(const float* __restrict__ row, int T, int C, int n_alphabet, int* s_idx, unsigned& m0,
+                                           unsigned& m1) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
 
     // 1. one warp per timestep: each lane scans its float4 chunks in index order, then the warp combines
     const int c4 = C >> 2;
@@ -49,13 +49,26 @@ __global__ void __launch_bounds__(kPredThreads) decode_predictions_kernel(
         if (lane == 0) s_idx[t] = bi;
     }
     __syncthreads();
-    if (warp != 0) return;
+    if (warp != 0) return false;
 
     // 2. CTC collapse: timesteps lane and lane + 32, ranks from ballots
     const bool k0 = lane < T && (lane == 0 || s_idx[lane] != s_idx[lane - 1]) && s_idx[lane] < n_alphabet;
     const int t1 = lane + 32;
     const bool k1 = t1 < T && s_idx[t1] != s_idx[t1 - 1] && s_idx[t1] < n_alphabet;
-    const unsigned m0 = __ballot_sync(0xffffffffu, k0), m1 = __ballot_sync(0xffffffffu, k1);
+    m0 = __ballot_sync(0xffffffffu, k0);
+    m1 = __ballot_sync(0xffffffffu, k1);
+    return true;
+}
+
+__global__ void __launch_bounds__(kPredThreads) decode_predictions_kernel(
+        const float* __restrict__ logits, long long logits_row_stride, int T, int C, const float* __restrict__ locs_lr,
+        long long locs_row_stride, const mn_pred_row* __restrict__ rows, int n_alphabet) {
+    mn_pdl_prologue();
+    __shared__ int s_idx[kMaxT];
+    unsigned m0, m1;
+    if (!decode_ctc(logits + (long long)blockIdx.x * logits_row_stride, T, C, n_alphabet, s_idx, m0, m1)) return;
+    const int lane = threadIdx.x & 31, t1 = lane + 32;
+    const bool k0 = (m0 >> lane) & 1u, k1 = (m1 >> lane) & 1u;
     const unsigned lt = (1u << lane) - 1u;
     __shared__ int s_lab[MN_PRED_SLOTS];
     const int r0 = __popc(m0 & lt), r1 = __popc(m0) + __popc(m1 & lt);
@@ -97,6 +110,24 @@ __global__ void __launch_bounds__(kPredThreads) decode_predictions_kernel(
     }
 }
 
+// Every character of the row: the whole CTC collapse (up to T <= 64 labels), compacted in timestep order.
+__global__ void __launch_bounds__(kPredThreads) decode_labels_kernel(const float* __restrict__ logits, long long logits_row_stride,
+                                                                     int T, int C, mn_label_row* __restrict__ out, int n_alphabet) {
+    mn_pdl_prologue();
+    __shared__ int s_idx[kMaxT];
+    unsigned m0, m1;
+    if (!decode_ctc(logits + (long long)blockIdx.x * logits_row_stride, T, C, n_alphabet, s_idx, m0, m1)) return;
+    const int lane = threadIdx.x & 31, t1 = lane + 32;
+    const unsigned lt = (1u << lane) - 1u;
+    const int n = __popc(m0) + __popc(m1);
+    mn_label_row* o = out + blockIdx.x;
+    if ((m0 >> lane) & 1u) o->label[__popc(m0 & lt)] = s_idx[lane];
+    if ((m1 >> lane) & 1u) o->label[__popc(m0) + __popc(m1 & lt)] = s_idx[t1];
+    if (lane >= n) o->label[lane] = -1;
+    if (t1 >= n) o->label[t1] = -1;
+    if (lane == 0) o->n = n;
+}
+
 }  // namespace
 
 extern "C" int mn_decode_predictions(const float* logits, long long logits_row_stride, int T, int C, const float* locs_lr,
@@ -108,6 +139,18 @@ extern "C" int mn_decode_predictions(const float* logits, long long logits_row_s
     MN_REQUIRE(locs_row_stride >= 2 * MN_PRED_SLOTS, "mn_decode_predictions: locs rows hold fewer than %d values", 2 * MN_PRED_SLOTS);
     MN_CUDA_CHECK((mn_launch(decode_predictions_kernel, dim3(n_rows), dim3(kPredThreads), 0, (cudaStream_t)stream, logits,
                              logits_row_stride, T, C, locs_lr, locs_row_stride, rows, n_alphabet)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_decode_labels(const float* logits, long long logits_row_stride, int T, int C, mn_label_row* out, int n_rows,
+                                int n_alphabet, void* stream) {
+    MN_REQUIRE(logits && out && n_rows > 0 && n_rows <= 65535 && T > 0 && T <= kMaxT && C > 0 && n_alphabet >= 0,
+               "mn_decode_labels: bad args");
+    MN_REQUIRE(C % 4 == 0 && logits_row_stride % 4 == 0 && ((uintptr_t)logits & 15) == 0 && logits_row_stride >= (long long)T * C,
+               "mn_decode_labels: logits rows must be dense [T][C] fp32 with C %% 4 == 0, 16-byte aligned (C = %d)", C);
+    MN_CUDA_CHECK((mn_launch(decode_labels_kernel, dim3(n_rows), dim3(kPredThreads), 0, (cudaStream_t)stream, logits,
+                             logits_row_stride, T, C, out, n_alphabet)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -1037,14 +1037,18 @@ def pred_dtype():
                      ("n_decoded", "<i4")])
 
 
-def prediction_table(windows, device):
+def prediction_table(windows, device, out=None):
     """windows: one (a, scale, lo, hi) per encoder row -- the window's first source column, source columns per unit of canvas
     width (16*h), its core [lo, hi) -> (rows, out): the device table of mn_pred_row records and the device buffer of
-    mn_char_pred records they point to (row r writes record r; read it back as ``pred_dtype()``)."""
+    mn_char_pred records they point to (row r writes record r; read it back as ``pred_dtype()``).  ``out``: a uint8 CUDA buffer
+    (8-byte aligned) to hold the records instead of a new one."""
     if not windows:
         raise ValueError("prediction_table: no rows")
     isz = ctypes.sizeof(_lib.CharPred)
-    out = torch.empty(len(windows) * isz, dtype=torch.uint8, device=device)
+    if out is None:
+        out = torch.empty(len(windows) * isz, dtype=torch.uint8, device=device)
+    elif out.dtype != torch.uint8 or out.device != torch.device(device) or out.numel() < len(windows) * isz or out.data_ptr() % 8:
+        raise ValueError(f"prediction_table: out must be an 8-byte aligned uint8 buffer of >= {len(windows) * isz} bytes on {device}")
     recs = [_lib.PredRow(float(a), float(s), float(lo), float(hi), out.data_ptr() + r * isz) for r, (a, s, lo, hi) in enumerate(windows)]
     return _table(_lib.PredRow, recs, device), out
 
@@ -1068,4 +1072,96 @@ def decode_predictions(logits, locs_lr, rows, first=0, n_alphabet=6735):
     _lib.check(_lib.load().mn_decode_predictions(_ptr(logits), logits.stride(0), t, c, _ptr(locs_lr), locs_lr.stride(0),
                                                  rows.data_ptr() + first * ctypes.sizeof(_lib.PredRow), b, n_alphabet, _stream()),
                "mn_decode_predictions")
+    LAUNCHES += 1
+
+
+# ---- font-style interpolation (test_w.py:95-114; DESIGN.md 7b, "Font-style interpolation") ------------------------------
+LABEL_SLOTS = _lib.LABEL_SLOTS
+
+
+def label_dtype():
+    """numpy view of an mn_label_row record (the output of mn_decode_labels)."""
+    import numpy as np
+    return np.dtype([("n", "<i4"), ("label", "<i4", LABEL_SLOTS)])
+
+
+def decode_labels(logits, out, first=0, n_alphabet=6735):
+    """mn_decode_labels, one launch: every character of encoder row b of logits (fp32 [B, T, 6736], T <= 64, read in place) --
+    the argmax and CTC collapse of decode_predictions over all T timesteps (test_w.py:34-40) -- into record first + b of ``out``
+    (a uint8 CUDA buffer of mn_label_row records; read it back as ``label_dtype()``)."""
+    global LAUNCHES
+    _require_cuda(logits, "logits")
+    if logits.dim() != 3 or logits.stride(2) != 1 or logits.stride(1) != logits.shape[2]:
+        raise RuntimeError("decode_labels: logits must be fp32 [B, T, C] with dense rows")
+    b, t, c = logits.shape
+    isz = ctypes.sizeof(_lib.LabelRow)
+    if not isinstance(out, torch.Tensor) or out.device != logits.device or out.dtype != torch.uint8 or out.data_ptr() % 4 \
+            or not 0 <= first or (first + b) * isz > out.numel():
+        raise ValueError(f"decode_labels: records [{first}, {first + b}) are not in the output buffer")
+    _lib.check(_lib.load().mn_decode_labels(_ptr(logits), logits.stride(0), t, c, out.data_ptr() + first * isz, b, n_alphabet,
+                                            _stream()), "mn_decode_labels")
+    LAUNCHES += 1
+
+
+def lerp_rows(rows, n_w):
+    """rows: (w1, w2, scale) per style row, w1 / w2 row indices of a style table with n_w rows and scale a finite Python number ->
+    bytes of mn_lerp_row records with s = float32(scale), t = float32(1 - scale) (1 - scale computed in double, as test_w.py's
+    ``1 - scale``)."""
+    import math
+    recs = []
+    for r, (w1, w2, scale) in enumerate(rows):
+        w1, w2, scale = int(w1), int(w2), float(scale)
+        if not (0 <= w1 < n_w and 0 <= w2 < n_w) or not math.isfinite(scale):
+            raise ValueError(f"lerp_rows: row {r}: styles ({w1}, {w2}) of {n_w}, scale {scale}")
+        recs.append(_lib.LerpRow(w1, w2, scale, 1.0 - scale))
+    return bytes((_lib.LerpRow * len(recs))(*recs))
+
+
+def style_lerp(w, rows, n_rows):
+    """mn_style_lerp, one launch: w fp32 [n_w, dim] (unit inner stride), rows a uint8 CUDA tensor holding n_rows mn_lerp_row
+    records (lerp_rows) -> fp32 [n_rows, dim], row r = w[w1]*s + w[w2]*t with every operation rounded on its own."""
+    global LAUNCHES
+    _require_cuda(w, "w")
+    if w.dim() != 2 or w.stride(1) != 1:
+        raise RuntimeError("style_lerp: w must be fp32 [n, dim] with unit inner stride")
+    if not isinstance(rows, torch.Tensor) or rows.device != w.device or rows.dtype != torch.uint8 or rows.data_ptr() % 4 \
+            or n_rows < 1 or n_rows * ctypes.sizeof(_lib.LerpRow) > rows.numel():
+        raise ValueError(f"style_lerp: the table does not hold {n_rows} rows")
+    out = torch.empty((n_rows, w.shape[1]), dtype=torch.float32, device=w.device)
+    _lib.check(_lib.load().mn_style_lerp(_ptr(w), w.stride(0), _ptr(rows), n_rows, w.shape[1], _ptr(out), out.stride(0), _stream()),
+               "mn_style_lerp")
+    LAUNCHES += 1
+    return out
+
+
+def prior_tile_rows(tiles):
+    """tiles: (strip, c) per generator image, strip a contiguous uint8 CUDA [128, 128 n, 3] view (one style's strip) and c < n
+    the character's column -> bytes of mn_prior_tile records pointing at strip[:, 128 c:128 c + 128]."""
+    recs = []
+    for r, (strip, c) in enumerate(tiles):
+        c = int(c)
+        if not isinstance(strip, torch.Tensor) or not strip.is_cuda or strip.dtype != torch.uint8 or strip.dim() != 3 \
+                or strip.shape[0] != 128 or strip.shape[2] != 3 or strip.shape[1] % 128 or not strip.is_contiguous():
+            raise RuntimeError(f"prior_tile_rows: row {r}: the strip must be a contiguous uint8 [128, 128 n, 3] CUDA tensor")
+        if not 0 <= c < strip.shape[1] // 128:
+            raise ValueError(f"prior_tile_rows: row {r}: character {c} outside the {strip.shape[1] // 128}-character strip")
+        recs.append(_lib.PriorTile(strip.data_ptr() + 384 * c, strip.stride(0)))
+    return bytes((_lib.PriorTile * len(recs))(*recs))
+
+
+def prior_tiles(priors, tiles, first=0):
+    """mn_prior_tiles_u8, one launch: generator image n of priors (fp32 [N, 3, 128, 128], any strides: the channels_last
+    output is read in place) -> 8-bit tile at record first + n of ``tiles`` (a uint8 CUDA tensor of prior_tile_rows records),
+    the bytes cv2.imwrite stores for prior*0.5 + 0.5 times 255 (test_w.py:109-114)."""
+    global LAUNCHES
+    _require_cuda(priors, "priors")
+    if priors.dim() != 4 or tuple(priors.shape[1:]) != (3, 128, 128):
+        raise RuntimeError("prior_tiles: priors must be fp32 [N, 3, 128, 128]")
+    n = priors.shape[0]
+    isz = ctypes.sizeof(_lib.PriorTile)
+    if not isinstance(tiles, torch.Tensor) or tiles.device != priors.device or tiles.dtype != torch.uint8 or tiles.data_ptr() % 8 \
+            or not 0 <= first or (first + n) * isz > tiles.numel() or not 1 <= n <= 65535:
+        raise ValueError(f"prior_tiles: records [{first}, {first + n}) are not in the table (at most 65535 per launch)")
+    _lib.check(_lib.load().mn_prior_tiles_u8(_ptr(priors), *priors.stride(), tiles.data_ptr() + first * isz, n, _stream()),
+               "mn_prior_tiles_u8")
     LAUNCHES += 1

@@ -500,13 +500,19 @@ def merge_predictions(h, w, windows, rows):
     decode order with their boxes in source columns.  Concatenated in window order, each box clamped to the image
     ([clamp(min(x1, x2), 0, w), 0, clamp(max(x1, x2), 0, w), h]), then stable-sorted by box centre (pairs stay together).
     Returns (labels, boxes)."""
+    merged = _merge_windows(h, w, windows, rows)
+    return [m[0] for m in merged], [m[1] for m in merged]
+
+
+def _merge_windows(h, w, windows, rows):
+    """merge_predictions' characters as (label, box, index of the window that kept it), in merged order."""
     pairs = []
-    for (labs, x1s, x2s), _ in zip(rows, windows):
+    for k, ((labs, x1s, x2s), _) in enumerate(zip(rows, windows)):
         for lab, x1, x2 in zip(labs, x1s, x2s):
             lo, hi = min(max(min(x1, x2), 0.0), float(w)), min(max(max(x1, x2), 0.0), float(w))
-            pairs.append((int(lab), [lo, 0, hi, h]))
+            pairs.append((int(lab), [lo, 0, hi, h], k))
     pairs.sort(key=lambda p: (p[1][0] + p[1][2]) / 2.0)
-    return [p[0] for p in pairs], [p[1] for p in pairs]
+    return pairs
 
 
 def _predict(encoder, imgs, max_lines, overlap):
@@ -697,6 +703,189 @@ def restore_images(encoder, tspgan, sr, images, labels=None, boxes=None, max_lin
             results[i]["figure"] = figs[i]
         if i in predicted:
             results[i]["labels"], results[i]["boxes"] = predicted[i]
+    return results
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Font-style interpolation (DESIGN.md section 7b, "Font-style interpolation"): test_w.py's mode, batched.  The script encodes two
+# images, decodes image 1's characters, and generates them in the style w1*s + w2*(1-s) for 11 scales, one generator call per
+# scale.  Here every (pair, scale, character) style row of a call is built by one mn_style_lerp launch, the generator runs over
+# chunks of those rows and mn_prior_tiles_u8 writes each image into its strip as the 8-bit PNG bytes the script stores.
+# ---------------------------------------------------------------------------------------------------------------------
+class SweepRow(NamedTuple):
+    """One generator image of interpolate_styles: character ``char`` of pair ``pair``'s strip ``scale``, in the style
+    w[w1]*s + w[w2]*(1-s) (rows of the call's encoder style table)."""
+    pair: int
+    scale: int
+    char: int
+    w1: int
+    w2: int
+    label: int
+
+
+def plan_sweep(chars, donors, n_scales, max_chars):
+    """interpolate_styles' generator rows, on the host.  chars[p]: pair p's characters in strip order as (style row, label), or
+    None for a pair left out; donors[p]: its donor's style row.  Returns (rows in (pair, scale, character) order, chunks [r0, r1)
+    of at most ``max_chars`` consecutive rows: one generator call each)."""
+    rows = [SweepRow(p, k, c, w1, donors[p], lab) for p, cs in enumerate(chars) if cs
+            for k in range(n_scales) for c, (w1, lab) in enumerate(cs)]
+    return rows, [(r0, min(r0 + max_chars, len(rows))) for r0 in range(0, len(rows), max_chars)]
+
+
+def _pair_image(img, p, which):
+    try:
+        return _as_image(img, p)
+    except (ValueError, TypeError) as e:
+        raise ValueError(f"pair {p}: the {which} is not a uint8 [h, w, 3] image ({e})") from None
+
+
+@torch.no_grad()
+def interpolate_styles(encoder, tspgan, pairs, scales=tuple(i / 10 for i in range(11)), max_lines=8, max_chars=128, overlap=64,
+                       to_host=False, skip_invalid=False):
+    """test_w.py's font-style interpolation (:95-114) for many (content, donor) pairs of text-line images, on the device.
+
+    pairs: (content, donor) uint8 [h, w, 3] images (numpy arrays or CPU / CUDA tensors, as restore_images takes them; the arrays
+    test_w.py holds after cv2.cvtColor).  scales: non-empty sequence of finite numbers; the style at scale s is w1*s + w2*(1-s)
+    (test_w.py:107), w1 the content's and w2 the donor's, so s = 1 is the content's own style.
+    Returns one dict per pair: strips (uint8 [len(scales), 128, 128 n, 3]: strip k holds the n characters' generator images at
+    scales[k], the bytes cv2.imwrite stores for w_{s:.2f}.png; on the device, or numpy through ONE pinned copy with ``to_host``),
+    labels (the n characters, in strip order) and windows (the content's plan_windows plan).
+
+    A content line that fits the canvas (round_half_even(w*32/h) <= 512) gives test_w.py's bytes: its characters are all of
+    clear_labels(logits[0]) (up to 64), its style the encoder w of the whole image.  A wider one is read through plan_windows(h, w,
+    overlap): its characters are predict_characters' labels in the same order, each in the style of the detection window that
+    kept it.  Donors must fit the canvas.  A donor wider than the canvas, a content line without a decoded character or a
+    malformed image make the pair invalid: ValueError naming the pair, or dict(error=...) with ``skip_invalid``.
+
+    Read stage: one pinned host->device copy of the host images; per batch of at most ``max_lines`` encoder rows (fitting
+    content, then wide-content windows, then donors): one crop launch, the encoder, one mn_decode_labels launch for the fitting
+    content rows and one mn_decode_predictions launch for the windows; one pinned device->host copy and one synchronisation.
+    Sweep stage: one pinned copy of the style rows, labels and tile table; one mn_style_lerp launch; per chunk of at most
+    ``max_chars`` rows the generator (run eagerly: no module graph is recorded, since the chunk shapes vary from call to call) and
+    one mn_prior_tiles_u8 launch; one synchronisation, and a re-run when the fp16-range guard re-routed a layer (ops.poll_range)."""
+    import ctypes
+    import math
+    import numpy as np
+    from . import _lib, ops
+    if max_lines < 1:
+        raise ValueError("max_lines must be >= 1")
+    if max_chars < 1:
+        raise ValueError("max_chars must be >= 1")
+    if not 0 <= overlap <= 256:
+        raise ValueError(f"overlap must lie in [0, 256] LQ pixels, got {overlap}")
+    scales = list(scales)
+    if not scales or any(isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) for v in scales):
+        raise ValueError(f"scales must be a non-empty sequence of finite numbers, got {scales}")
+    scales = [float(v) for v in scales]
+    dev = next(encoder.parameters()).device
+    n = len(pairs)
+    results, imgs, plans = [None] * n, [], {}
+
+    def failed(p, e):
+        if not skip_invalid:
+            raise e
+        results[p] = dict(error=f"{type(e).__name__}: {e}")
+
+    for p, pair in enumerate(pairs):
+        try:
+            if not isinstance(pair, (tuple, list)) or len(pair) != 2:
+                raise ValueError(f"pair {p}: expected a (content, donor) pair of images")
+            content, donor = _pair_image(pair[0], p, "content"), _pair_image(pair[1], p, "donor")
+            lq_w = whole_line_width(*donor.shape[:2])[0]
+            if lq_w > 512:
+                raise ValueError(f"pair {p}: the donor's LQ width {lq_w} exceeds the 512-pixel canvas (a line wider than the canvas "
+                                 f"has no single style w; test_w.py:88 exits on it)")
+        except ValueError as e:
+            failed(p, e)
+            continue
+        plans[p] = (plan_windows(*content.shape[:2], overlap=overlap), len(imgs), len(imgs) + 1)
+        imgs += [content, donor]
+    # encoder rows (image, a, b, pair, window), kind by kind: fitting content, wide-content windows, donors
+    fit = [(ci, 0, imgs[ci].shape[1], p, 0) for p, (win, ci, _) in plans.items() if len(win) == 1]
+    wide = [(ci, *wn.crop, p, k) for p, (win, ci, _) in plans.items() if len(win) > 1 for k, wn in enumerate(win)]
+    donors = [(di, 0, imgs[di].shape[1], p, -1) for p, (_, _, di) in plans.items()]
+    rows = fit + wide + donors
+    if not rows:
+        return results
+    isz_p, isz_l = ctypes.sizeof(_lib.CharPred), ctypes.sizeof(_lib.LabelRow)
+    with torch.cuda.device(dev):
+        rec = torch.empty(len(wide) * isz_p + len(fit) * isz_l, dtype=torch.uint8, device=dev)
+        ptable = ops.prediction_table([(a, 16.0 * imgs[i].shape[0], *plans[p][0][k].core) for i, a, _, p, k in wide], dev,
+                                      out=rec)[0] if wide else None
+        labs_d = rec[len(wide) * isz_p:]
+        wtab = torch.empty((len(rows), 512), dtype=torch.float32, device=dev)
+        dimg = _device_images(range(len(imgs)), imgs, dev)
+        nf, nw = len(fit), len(fit) + len(wide)
+        for r0 in range(0, len(rows), max_lines):
+            r1 = min(r0 + max_lines, len(rows))
+            lq, _ = ops.preprocess_lq_crops([(dimg[i], a, b) for i, a, b, _, _ in rows[r0:r1]])
+            logits, locs_lr, w = encoder(lq)
+            wtab[r0:r1].copy_(w)
+            if r0 < nf:
+                ops.decode_labels(logits[:min(r1, nf) - r0], labs_d, r0)
+            if max(r0, nf) < min(r1, nw):
+                a0, a1 = max(r0, nf) - r0, min(r1, nw) - r0
+                ops.decode_predictions(logits[a0:a1], locs_lr[a0:a1], ptable, r0 + a0 - nf)
+        host = _to_host(rec).numpy()
+    pred = host[:len(wide) * isz_p].view(ops.pred_dtype())
+    labs = host[len(wide) * isz_p:].view(ops.label_dtype())
+    chars, donor_row = [None] * n, [None] * n
+    for r, (_, _, _, p, _) in enumerate(donors):
+        donor_row[p] = nw + r
+    for r, (_, _, _, p, _) in enumerate(fit):
+        chars[p] = [(r, int(v)) for v in labs[r]["label"][:int(labs[r]["n"])]]
+    first = {}
+    for r, (ci, _, _, p, k) in enumerate(wide):
+        first.setdefault(p, nf + r)
+    for p, r0 in first.items():
+        win, ci, _ = plans[p]
+        dec = []
+        for k in range(len(win)):
+            m = int(pred[r0 - nf + k]["n_kept"])
+            rr = pred[r0 - nf + k]
+            dec.append((rr["label"][:m].tolist(), rr["x1"][:m].tolist(), rr["x2"][:m].tolist()))
+        chars[p] = [(r0 + k, lab) for lab, _, k in _merge_windows(*imgs[ci].shape[:2], win, dec)]
+    for p in plans:
+        if not chars[p]:
+            chars[p] = None
+            failed(p, ValueError(f"pair {p}: no character decoded from the content"))
+    srows, chunks = plan_sweep(chars, donor_row, len(scales), max_chars)
+    if not srows:
+        return results
+    with torch.cuda.device(dev):
+        offs, total = {}, 0
+        for p, cs in enumerate(chars):
+            if cs:
+                offs[p] = total
+                total += len(scales) * 128 * 128 * len(cs) * 3
+        flat = torch.empty(total, dtype=torch.uint8, device=dev)
+
+        def strips_of(buf):
+            return {p: buf[o:o + len(scales) * 128 * 128 * len(chars[p]) * 3].view(len(scales), 128, 128 * len(chars[p]), 3)
+                    for p, o in offs.items()}
+        strips = strips_of(flat)
+        tiles = ops.prior_tile_rows([(strips[r.pair][r.scale], r.char) for r in srows])
+        lerp = ops.lerp_rows([(r.w1, r.w2, scales[r.scale]) for r in srows], len(rows))
+        host_tab = tiles + lerp + np.asarray([r.label for r in srows], np.int64).tobytes()
+        pinned = torch.empty(len(host_tab), dtype=torch.uint8, pin_memory=True)
+        pinned.numpy()[:] = np.frombuffer(host_tab, np.uint8)
+        tab = pinned.to(dev, non_blocking=True)
+        lerp_d = tab[len(tiles):len(tiles) + len(lerp)]
+        lab_d = tab[len(tiles) + len(lerp):].view(torch.int64)
+        flag = torch.zeros(1, dtype=torch.int32, device=dev)
+
+        def sweep():
+            styles = ops.style_lerp(wtab, lerp_d, len(srows))
+            with ops.deferred_checks(flag):          # device-side label check; also keeps the generator off its module graphs
+                for r0, r1 in chunks:
+                    img, _, _ = tspgan(styles=styles[r0:r1], labels=lab_d[r0:r1].view(-1, 1), noise=None)
+                    ops.prior_tiles(img, tab, r0)
+        _rerun(sweep, dev)
+        ops.raise_deferred(int(flag.item()))
+        if to_host:
+            strips = {p: s.numpy() for p, s in strips_of(_to_host(flat)).items()}
+    for p in offs:
+        results[p] = dict(strips=strips[p], labels=[lab for _, lab in chars[p]], windows=plans[p][0])
     return results
 
 
