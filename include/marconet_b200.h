@@ -139,6 +139,24 @@ int64_t mn_conv2d_workspace_bytes(const mn_conv_params* p);
 int mn_conv2d_tc_supported(const mn_conv_params* p);
 /* 2: the halo-tiled tensor-core kernel (fused input transforms) runs this problem; 1: only the per-tap tiling; 0: neither. */
 int mn_conv2d_tc_version(const mn_conv_params* p);
+
+typedef enum {
+    MN_CONV_KERNEL_SMALL = 0,   /* direct 3x3 kernel for Cout <= 4 (fp32)                       */
+    MN_CONV_KERNEL_SIMT = 1,    /* fp32 CUDA-core implicit GEMM (+ split-K reduce)              */
+    MN_CONV_KERNEL_TC1 = 2,     /* tensor-core per-tap tiling                                   */
+    MN_CONV_KERNEL_TC2 = 3      /* tensor-core halo tiling (+ split-K reduce)                   */
+} mn_conv_kernel;
+
+/* What mn_conv2d_nhwc would launch for *p, filled in without launching anything. */
+typedef struct {
+    int kernel;                 /* mn_conv_kernel                                               */
+    int precision;              /* the precision that runs (MN_PREC_FP32_SIMT for small / simt) */
+    int nt;                     /* tensor-core kernels: output channels per work item (64/128)  */
+    int TN, TH, TW;             /* tensor-core kernels: samples x rows x columns of a pixel tile */
+    int splits;                 /* split-K factor of the simt or halo-tiled kernel (1: none)    */
+} mn_conv_plan;
+/* MN_OK and *out filled in, or the status and message mn_conv2d_nhwc would return for *p. */
+int mn_conv2d_plan(const mn_conv_params* p, mn_conv_plan* out);
 /* Split fp32 weights w:[taps*Cin][Cout] (the layout mn_conv2d_nhwc takes) into hi/lo 16-bit planes
  * [taps][Cout][Cin], pre-scaled by a power of two so the lo plane stays in the fp16 normal range.
  * hi, lo: taps*Cin*Cout 16-bit elements each; scale2: 2 floats {abs-max, 2^-S}. */

@@ -38,6 +38,13 @@ class ConvParams(Structure):
     ]
 
 
+CONV_KERNELS = ("small", "simt", "tc1", "tc2")     # mn_conv_kernel
+
+
+class ConvPlan(Structure):
+    _fields_ = [("kernel", c_int), ("precision", c_int), ("nt", c_int), ("TN", c_int), ("TH", c_int), ("TW", c_int), ("splits", c_int)]
+
+
 class DemodDesc(Structure):
     _fields_ = [("wsq", c_void_p), ("s_off", c_int32), ("cin", c_int32), ("cout", c_int32), ("out_off", c_int32)]
 
@@ -101,6 +108,7 @@ SYMBOLS = {
     "mn_conv2d_workspace_bytes": (c_int64, [POINTER(ConvParams)]),
     "mn_conv2d_tc_supported": (c_int, [POINTER(ConvParams)]),
     "mn_conv2d_tc_version": (c_int, [POINTER(ConvParams)]),
+    "mn_conv2d_plan": (c_int, [POINTER(ConvParams), POINTER(ConvPlan)]),
     "mn_groupnorm_stats": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "mn_groupnorm_finalize": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
     "mn_groupnorm_apply": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,

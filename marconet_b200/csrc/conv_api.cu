@@ -51,34 +51,66 @@ extern "C" int64_t mn_conv2d_workspace_bytes(const mn_conv_params* p) {
     return splits > 1 ? (int64_t)splits * g.M * g.Cout * 4 : 0;
 }
 
-extern "C" int mn_conv2d_nhwc(const mn_conv_params* p, void* stream) {
-    ConvGeom g;
-    int rc = make_geom(p, g);
-    if (rc != MN_OK) return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool v2 = p->precision != MN_PREC_FP32_SIMT && !tc_force_v1() && mn_conv_tc2_supported(g, nullptr);
-    if ((g.y2_ptrs || g.gn_stats_out) && !v2) {
+// Features only the halo-tiled kernel has: refuse them elsewhere.  Sets *v2 to whether that kernel runs the problem.
+static int check_v2_features(const mn_conv_params* p, const ConvGeom& g, bool* v2) {
+    *v2 = p->precision != MN_PREC_FP32_SIMT && !tc_force_v1() && mn_conv_tc2_supported(g, nullptr);
+    if ((g.y2_ptrs || g.gn_stats_out) && !*v2) {
         mn_set_error("mn_conv2d_nhwc: per-sample output pointers (y2_ptrs) / epilogue GroupNorm statistics (gn_stats_out) exist only in the halo-tiled tensor-core kernel");
         return MN_ERR_UNSUPPORTED;
     }
-    if (g.gn_mr && !v2) {
+    if (g.gn_mr && !*v2) {
         mn_set_error("mn_conv2d_nhwc: the fused GroupNorm input transform exists only in the halo-tiled tensor-core kernel (check mn_conv2d_tc_version)");
         return MN_ERR_UNSUPPORTED;
     }
+    return MN_OK;
+}
+
+// The one dispatch decision: which kernel runs *p, with which tile and split count.  mn_conv2d_nhwc launches what it returns and
+// mn_conv2d_plan reports it, so the two cannot disagree.
+static int plan_conv(const mn_conv_params* p, ConvGeom& g, mn_conv_plan* r) {
+    int rc = make_geom(p, g);
+    if (rc != MN_OK) return rc;
+    bool v2;
+    if ((rc = check_v2_features(p, g, &v2)) != MN_OK) return rc;
+    *r = mn_conv_plan{};
+    r->precision = p->precision;
+    r->splits = 1;
     switch (p->precision) {
         case MN_PREC_FP32_SIMT:
-            if (mn_conv_small_supported(g)) return mn_conv_small_launch(g, st);
-            g.splits = mn_conv_simt_plan_splits(g, p->workspace ? p->workspace_bytes : 0, p->split_k);
-            return mn_conv_simt_launch(g, nullptr, st);
+            if (mn_conv_small_supported(g)) { r->kernel = MN_CONV_KERNEL_SMALL; return MN_OK; }
+            r->kernel = MN_CONV_KERNEL_SIMT;
+            r->splits = mn_conv_simt_plan_splits(g, p->workspace ? p->workspace_bytes : 0, p->split_k);
+            return MN_OK;
         case MN_PREC_F16X3_TC:
         case MN_PREC_BF16X3_TC:
         case MN_PREC_F16X1_TC:
-            if (!tc_force_v1() && mn_conv_tc2_supported(g, nullptr))
-                return mn_conv_tc2_launch(g, p->w_tc_hi, p->w_tc_lo, p->w_tc_scale, p->precision, st);
-            return mn_conv_tc_launch(g, p->w_tc_hi, p->w_tc_lo, p->w_tc_scale, p->precision, st);
+            return mn_conv_tc_plan_info(g, v2, r) ? MN_OK : MN_ERR_UNSUPPORTED;
         default:
             mn_set_error("mn_conv2d_nhwc: unknown precision mode %d", p->precision);
             return MN_ERR_UNSUPPORTED;
+    }
+}
+
+extern "C" int mn_conv2d_plan(const mn_conv_params* p, mn_conv_plan* out) {
+    MN_REQUIRE(out != nullptr, "mn_conv2d_plan: null output");
+    ConvGeom g;
+    mn_conv_plan r;
+    const int rc = plan_conv(p, g, &r);
+    if (rc == MN_OK) *out = r;
+    return rc;
+}
+
+extern "C" int mn_conv2d_nhwc(const mn_conv_params* p, void* stream) {
+    ConvGeom g;
+    mn_conv_plan r;
+    const int rc = plan_conv(p, g, &r);
+    if (rc != MN_OK) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    switch (r.kernel) {
+        case MN_CONV_KERNEL_SMALL: return mn_conv_small_launch(g, st);
+        case MN_CONV_KERNEL_SIMT: g.splits = r.splits; return mn_conv_simt_launch(g, nullptr, st);
+        case MN_CONV_KERNEL_TC2: return mn_conv_tc2_launch(g, p->w_tc_hi, p->w_tc_lo, p->w_tc_scale, p->precision, st);
+        default: return mn_conv_tc_launch(g, p->w_tc_hi, p->w_tc_lo, p->w_tc_scale, p->precision, st);
     }
 }
 

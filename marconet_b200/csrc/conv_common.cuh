@@ -151,6 +151,8 @@ int mn_conv_tc_launch(const ConvGeom& g, const void* w_hi, const void* w_lo, con
 // tensor-core path, halo tiling: halo tiles + weight multicast + persistent CTAs (conv_tc2.cu)
 int mn_conv_tc2_supported(const ConvGeom& g, const char** why);
 int mn_conv_tc2_launch(const ConvGeom& g, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st);
+// the plan either tensor-core tiling would launch (halo: plan_tc2, else plan_tc1) into *out; 0 when it cannot run the problem
+int mn_conv_tc_plan_info(const ConvGeom& g, bool halo, mn_conv_plan* out);
 // direct 3x3 conv for Cout <= 4 (conv_small.cu)
 bool mn_conv_small_supported(const ConvGeom& g);
 int mn_conv_small_launch(const ConvGeom& g, cudaStream_t st);

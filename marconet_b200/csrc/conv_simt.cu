@@ -254,7 +254,9 @@ int mn_conv_simt_plan_splits(const ConvGeom& g0, int64_t ws_bytes, int requested
         if (ws_bytes < per * 2) return 1;
         if (per * splits > ws_bytes) splits = (int)(ws_bytes / per);
     }
-    return splits < 1 ? 1 : splits;
+    if (splits < 1) splits = 1;
+    // the count mn_conv_simt_launch runs: whole k-tiles per split, no empty split at the end
+    return mn_cdiv(ktiles, mn_cdiv(ktiles, splits));
 }
 
 int mn_conv_simt_launch(ConvGeom g, const float* x_ptr_for_align, cudaStream_t st) {

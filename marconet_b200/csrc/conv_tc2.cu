@@ -47,6 +47,28 @@ struct Tc2Geom {
     int prec;
 };
 
+// One thread's share of the epilogue GroupNorm statistics (sum and sum of squares of y per sample and group).  Summing y and y*y
+// directly in fp32 loses the variance to cancellation when |mean| >> std (E[y^2] - mean^2: ~1e-3 relative at mean/std = 300):
+// the values are summed about a pivot (the thread's first value) in fp32 and turned into sum / sum of squares in fp64, where
+// the finaliser's E[y^2] - mean^2 has 29 more bits to cancel.
+struct GnAcc {
+    float p = 0.f, s = 0.f, q = 0.f;
+    int c = 0;
+    __device__ __forceinline__ void add(const float4 w) {
+        if (c == 0) p = w.x;
+        const float d0 = w.x - p, d1 = w.y - p, d2 = w.z - p, d3 = w.w - p;
+        s += (d0 + d1) + (d2 + d3);
+        q = fmaf(d0, d0, fmaf(d1, d1, fmaf(d2, d2, fmaf(d3, d3, q))));
+        c += 4;
+    }
+    // sum y = c p + s ;  sum y^2 = q + 2 p s + c p^2
+    __device__ __forceinline__ void sums(double& sum, double& sq) const {
+        const double pd = p, cd = c;
+        sum = cd * pd + s;
+        sq = (double)q + 2.0 * pd * s + cd * pd * pd;
+    }
+};
+
 // MODE: 0 = f16x3, 1 = bf16x3, 2 = f16x1 (a template parameter: the wgmma operand registers must not depend on a runtime branch)
 template <bool GN, int MODE, int NT>
 __global__ void __launch_bounds__(NUM_THREADS2, 1)
@@ -451,32 +473,32 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                             // per-sample (possibly peer-GPU) destination of the second output, rebased so that row index m addresses it
                             if (g.y2_ptrs) y2base = g.y2_ptrs[n0] - (size_t)n0 * g.OH * g.OW * g.y2_cs;
                         }
-                        float gs = 0.f, gq = 0.f;       // GroupNorm statistics of this thread's 8 rows x 4 channels (one group)
-                        // One sample per tile and the tile inside the tensor (the plans guarantee H % TH == 0, W % TW == 0 and a power-of-two
-                        // TW): every row is valid and its pixel index is arithmetic -- no rowm look-ups, no per-row branch.
-                        const bool dense_tile = one_n && n0 < g.N;
+                        GnAcc ga;                       // GroupNorm statistics of this thread's 8 rows x 4 channels (one group)
+                        // One sample per tile, the tile inside the tensor (the plans guarantee H % TH == 0, W % TW == 0 and a power-of-two
+                        // TW) and 128 pixels in it: every row is valid and its pixel index is arithmetic -- no rowm look-ups, no per-row
+                        // branch.  Tiles of one sample with fewer pixels (4x16, 2x32, 1x64 maps: the halo cap of plan_tc2 leaves TN = 1
+                        // with TH * TW = 64) take the rowm path, which drops the MMA rows past the tile.
+                        const bool dense_tile = one_n && n0 < g.N && t.TH * t.TW == 128;
                         const int tws = __ffs(t.TW) - 1;
                         const int m00 = (n0 * g.OH + oy0) * g.OW + ox0;
                         const int vwn = (dense_tile && g.valid_w) ? g.valid_w[n0] : 0x7fffffff;
                         auto rows_dense = [&](auto tag) {
                             constexpr int ACT = decltype(tag)::value;
-#pragma unroll 8
+#pragma unroll 4     // 8 spills once the per-row path also serves one-sample tiles (ptxas -v)
                             for (int i = 0; i < 8; ++i) {
                                 const int row = rbase + 2 * i;
                                 const int th3 = row >> tws, tw3 = row & (t.TW - 1);
                                 const int m = m00 + th3 * g.OW + tw3;
                                 const float4 uv = *reinterpret_cast<const float4*>(stg + row * STG_PITCH + col);
-                                const float4 w4 = conv_epilogue_row4<ACT>(g, m, n0, ox0 + tw3 >= vwn, o, uv, bias4, true, os4, true, y2s4, y2base);
-                                if (g.gn_stats_out) {
-                                    gs += (w4.x + w4.y) + (w4.z + w4.w);
-                                    gq = fmaf(w4.x, w4.x, fmaf(w4.y, w4.y, fmaf(w4.z, w4.z, fmaf(w4.w, w4.w, gq))));
-                                }
+                                const bool masked = ox0 + tw3 >= vwn;
+                                const float4 w4 = conv_epilogue_row4<ACT>(g, m, n0, masked, o, uv, bias4, true, os4, true, y2s4, y2base);
+                                if (g.gn_stats_out && !masked) ga.add(w4);
                             }
                         };
                         auto rows = [&](auto tag) {
                             constexpr int ACT = decltype(tag)::value;
                             if (dense_tile) { rows_dense(tag); return; }
-                            if (one_n) return;                       // padding CTA of a cluster: nothing to store
+                            if (one_n && n0 >= g.N) return;          // padding CTA of a cluster: nothing to store
 #pragma unroll 4
                             for (int i = 0; i < 8; ++i) {
                                 const int row = rbase + 2 * i;
@@ -484,11 +506,9 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                                 if (m >= 0) {
                                     const int nn = rowm[128 + row];
                                     const float4 uv = *reinterpret_cast<const float4*>(stg + row * STG_PITCH + col);
-                                    const float4 w4 = conv_epilogue_row4<ACT>(g, m, nn & 0x3FFFFFFF, (nn >> 30) != 0, o, uv, bias4, one_n, os4, one_n, y2s4, y2base);
-                                    if (g.gn_stats_out) {
-                                        gs += (w4.x + w4.y) + (w4.z + w4.w);
-                                        gq = fmaf(w4.x, w4.x, fmaf(w4.y, w4.y, fmaf(w4.z, w4.z, fmaf(w4.w, w4.w, gq))));
-                                    }
+                                    const bool masked = (nn >> 30) != 0;
+                                    const float4 w4 = conv_epilogue_row4<ACT>(g, m, nn & 0x3FFFFFFF, masked, o, uv, bias4, one_n, os4, one_n, y2s4, y2base);
+                                    if (g.gn_stats_out && !masked) ga.add(w4);
                                 }
                             }
                         };
@@ -499,14 +519,16 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                             default: rows(ActTag<-1>{}); break;
                         }
                         if (g.gn_stats_out) {
+                            double gs, gq;
+                            ga.sums(gs, gq);
                             // lanes 0-7 / 8-15 (and 16-23 / 24-31, the odd rows) hold the two 32-channel groups of this 64-column half
 #pragma unroll
                             for (int sh = 1; sh <= 4; sh <<= 1) { gs += __shfl_xor_sync(0xffffffffu, gs, sh); gq += __shfl_xor_sync(0xffffffffu, gq, sh); }
                             gs += __shfl_xor_sync(0xffffffffu, gs, 16); gq += __shfl_xor_sync(0xffffffffu, gq, 16);
                             if ((lane & 23) == 0 && n0 < g.N) {        // lanes 0 and 8
                                 double* dst = g.gn_stats_out + ((size_t)n0 * (g.Cout >> 5) + (o >> 5)) * 2;
-                                atomicAdd(dst, (double)gs);
-                                atomicAdd(dst + 1, (double)gq);
+                                atomicAdd(dst, gs);
+                                atomicAdd(dst + 1, gq);
                             }
                         }
                     }
@@ -749,6 +771,14 @@ int mn_conv_tc2_launch(const ConvGeom& g, const void* w_hi, const void* w_lo, co
     Tc2Plan p = plan_tc2(g);
     if (!p.ok) { mn_set_error("mn_conv2d_nhwc: tensor-core halo tiling does not support this shape (%s)", p.why); return MN_ERR_UNSUPPORTED; }
     return launch_plan(g, p, w_hi, w_lo, w_scale, prec, st);
+}
+
+int mn_conv_tc_plan_info(const ConvGeom& g, bool halo, mn_conv_plan* out) {
+    const Tc2Plan p = halo ? plan_tc2(g) : plan_tc1(g);
+    if (!p.ok) { mn_set_error("tensor-core %s tiling does not support this shape (%s)", halo ? "halo" : "per-tap", p.why); return 0; }
+    out->kernel = halo ? MN_CONV_KERNEL_TC2 : MN_CONV_KERNEL_TC1;
+    out->nt = p.t.nt; out->TN = p.t.TN; out->TH = p.t.TH; out->TW = p.t.TW; out->splits = p.t.ksplit;
+    return 1;
 }
 
 int mn_conv_tc_supported(const ConvGeom& g, const char** why) {

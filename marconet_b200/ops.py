@@ -340,8 +340,10 @@ TC_MIN_FLOP = 3.0e7    # tiny launches are latency-bound either way and stay on 
 
 def conv2d(x, w, kh, kw, stride=(1, 1), pad=(0, 0), bias=None, out_scale=None, residual=None,
            res_broadcast=False, act=ACT_NONE, gain=1.0, out=None, out2=None, y2_scale=None,
-           valid_w=None, precision=None, want_y=True, split_k=0, gn=None, gn_fuse=None, out2_ptrs=None, gn_stats=False):
+           valid_w=None, precision=None, want_y=True, split_k=0, gn=None, gn_fuse=None, out2_ptrs=None, gn_stats=False, plan=None):
     """mn_conv2d_nhwc.  ``w`` is the packed [KH*KW*Cin, Cout] matrix.  Returns y (or (y, y2)).
+    ``plan``: a dict that receives what was launched (mn_conv2d_plan): ``kernel`` ("small" / "simt" / "tc1" / "tc2"), ``precision``,
+    ``nt``, ``TN``, ``TH``, ``TW``, ``splits`` (split-K), ``gn_fused``, ``gn_stats_out`` (statistics from the epilogue) and ``x_scale``.
     ``gn=(mean_rstd, gamma, beta)``: the conv input is swish(GroupNorm(x)); fused into the halo-tiled tensor-core kernel's operand-split
     stage when ``gn_fuse`` is true and that kernel runs the layer, otherwise applied by mn_groupnorm_apply first.
     (Default on since the fused instantiation runs four lanes per halo row with the GroupNorm constants in registers: all eight
@@ -415,9 +417,11 @@ def conv2d(x, w, kh, kw, stride=(1, 1), pad=(0, 0), bias=None, out_scale=None, r
             calib = getattr(_TLS, "calib", None)
             if calib is not None:
                 p.x_absmax = calib.slot(cw).data_ptr()
-            if gn is not None and ver == 2 and h * wd >= 128 and (_fuse_gn(cout) if gn_fuse is None else gn_fuse):   # one sample per 128-pixel tile
+            if gn is not None and ver == 2 and (_fuse_gn(cout) if gn_fuse is None else gn_fuse):
                 p.gn_mean_rstd = gn[0].data_ptr(); p.gn_gamma = gn[1].data_ptr(); p.gn_beta = gn[2].data_ptr(); p.gn_swish = 1
-                gn_fused = True
+                gn_fused = lib.mn_conv2d_tc_version(ctypes.byref(p)) == 2    # the plan needs one sample per 128-pixel tile (TN == 1)
+                if not gn_fused:
+                    p.gn_mean_rstd = p.gn_gamma = p.gn_beta = None; p.gn_swish = 0
         elif precision is not None:
             raise RuntimeError("conv2d: tensor-core precision requested explicitly but this layer/shape is not supported: "
                                + lib.mn_last_error().decode(errors="replace"))
@@ -426,14 +430,22 @@ def conv2d(x, w, kh, kw, stride=(1, 1), pad=(0, 0), bias=None, out_scale=None, r
             _note_fallback(cw, (n, h, wd, cin, cout, kh, kw, stride), 2.0 * n * oh * ow * cout * kh * kw * cin, p)
     p.precision = prec
     stats_ws = None
-    if gn_stats and prec != PREC_FP32_SIMT and ver == 2 and oh * ow >= 128 and cout % 32 == 0 and y is not None and out2_ptrs is None:
+    if gn_stats and prec != PREC_FP32_SIMT and ver == 2 and cout % 32 == 0 and y is not None and out2_ptrs is None:
         stats_ws = torch.zeros((n * (cout // 32) * 2,), dtype=torch.float64, device=x.device)
         p.gn_stats_out = stats_ws.data_ptr()
+        if lib.mn_conv2d_tc_version(ctypes.byref(p)) != 2:     # epilogue statistics need one sample per 128-pixel tile (TN == 1)
+            p.gn_stats_out = None
+            stats_ws = None
     if gn is not None and not gn_fused:      # no fused kernel for this layer: normalise into a temporary first
         xg = groupnorm_apply(x, gn[0], gn[1], gn[2], valid_w=valid_w)
         p.x = xg.data_ptr(); p.x_cs = xg.shape[3]
     _lib.check(lib.mn_conv2d_nhwc(ctypes.byref(p), _stream()), "mn_conv2d_nhwc")
     LAUNCHES += 1
+    if plan is not None:
+        cp = _lib.ConvPlan()
+        _lib.check(lib.mn_conv2d_plan(ctypes.byref(p), ctypes.byref(cp)), "mn_conv2d_plan")
+        plan.update(kernel=_lib.CONV_KERNELS[cp.kernel], precision=cp.precision, nt=cp.nt, TN=cp.TN, TH=cp.TH, TW=cp.TW,
+                    splits=cp.splits, gn_fused=gn_fused, gn_stats_out=stats_ws is not None, x_scale=p.x_scale if p.x_scale > 0 else 1.0)
     calib = getattr(_TLS, "calib", None)
     if calib is not None and calib.compare and cw is not None and prec != PREC_FP32_SIMT and precision is None:
         # tuning tool only (pipeline.tune_precision): the same layer through the exact fp32 kernel and both split formats

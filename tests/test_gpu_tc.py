@@ -52,6 +52,9 @@ TC_CASES = [
     (1, 8, 512, 256, 256, 3),     # ResNet stage at batch 1 (split-K 2)
     (2, 6, 128, 64, 64, 3),       # H = 6: no halo tiling, per-tap tiling (one shifted box per tap)
     (1, 12, 256, 128, 64, 3),     # H % 8 != 0: per-tap tiling, two pixel tiles per row (2-CTA cluster)
+    (3, 4, 16, 64, 64, 3),        # one sample per tile of 64 pixels (two samples' halos exceed the buffer): MMA rows 64-127 unused
+    (3, 2, 32, 64, 64, 3),        # the same at 2 rows x 32
+    (3, 1, 64, 64, 64, 3),        # the same at 1 row x 64
 ]
 # tensor-core fp32 accumulation truncates (round-toward-zero): the error grows ~linearly with K/16 accumulation steps
 TOL = {"f16x3": 4e-5, "bf16x3": 2e-4, "f16x1": 4e-3}
@@ -101,13 +104,16 @@ def test_conv_tc_epilogue_and_slices():
             assert y[i, :, :, v:].abs().max().item() == 0
 
 
-@pytest.mark.parametrize("shape", [(3, 32, 32, 128, 128), (1, 16, 256, 64, 64), (5, 16, 16, 256, 128), (2, 8, 8, 64, 64)],
-                         ids=["n3_32x32_128to128", "n1_16x256_64to64", "n5_16x16_256to128", "n2_8x8_two_pass_fallback"])
+@pytest.mark.parametrize("shape", [(3, 32, 32, 128, 128), (1, 16, 256, 64, 64), (5, 16, 16, 256, 128), (2, 8, 8, 64, 64),
+                                   (2, 16, 8, 64, 64), (2, 32, 4, 64, 64)],
+                         ids=["n3_32x32_128to128", "n1_16x256_64to64", "n5_16x16_256to128", "n2_8x8_two_pass_fallback",
+                              "n2_16x8_two_samples_per_tile", "n2_32x4_two_samples_per_tile"])
 @pytest.mark.parametrize("ragged", [False, True])
 def test_conv_tc_fused_groupnorm_swish(ragged, shape):
     """swish(GroupNorm(x)) built inside the conv's operand-split stage == GroupNorm + swish + conv in fp64: 128- and 64-wide tiles,
-    several channel blocks, an odd number of samples (padding CTA of the last pair), ragged windows; maps smaller than one 128-pixel
-    tile (8x8) take the two-pass form transparently."""
+    several channel blocks, an odd number of samples (padding CTA of the last pair), ragged windows; maps whose 128-pixel tiles hold
+    more than one sample (8x8, and 16x8 / 32x4, whose samples are 128 pixels but whose tiles are 8 rows deep) take the two-pass form
+    transparently."""
     from marconet_b200 import ops
     d = _dev()
     n, h, w, cin, cout = shape
