@@ -99,7 +99,8 @@ typedef struct {
     /* tensor-core precisions only: weights pre-split by mn_conv_pack_weights_tc()                */
     const void* w_tc_hi; const void* w_tc_lo;  /* 16-bit [KH*KW][Cout][Cin] (K-major)            */
     const float* w_tc_scale;                   /* the 2-float scale record written by the packer */
-    /* optional input transform fused into the halo-tiled tensor-core kernel's operand-split stage (mn_conv2d_tc_version() == 2 only):
+    /* optional input transform fused into the halo-tiled tensor-core kernel's operand-split stage: a request, which
+     * mn_conv2d_plan reports as gn_fused (dropped by every other kernel and by tiles of several samples):
      *   x' = swish( (x - mean[n,g]) * rstd[n,g] * gamma[c] + beta[c] ),  zero outside the image / beyond valid_w[n]
      * i.e. GroupNorm(32 channels per group) + swish of models/networks.py:508-512 applied while the A operand is built (its own
      * kernel instantiation: four lanes per halo row, constants in registers).  Needs OH*OW >= 128 (one sample per 128-pixel tile);
@@ -127,18 +128,12 @@ typedef struct {
     /* GroupNorm statistics of the OUTPUT accumulated by the epilogue (models/networks.py:508-512: the tensor this convolution writes
      * is normalised next): per (sample, group of 32 output channels) sum and sum of squares of y, fp32 partials per warp and tile
      * added into [N][Cout/32][2] doubles with atomics (the caller zeroes the buffer; columns beyond valid_w contribute 0).
-     * halo-tiled tensor-core kernel, whole-tile samples (OH*OW >= 128), no split-K; finish with mn_groupnorm_finalize. */
+     * halo-tiled tensor-core kernel, whole-tile samples (OH*OW >= 128), no split-K: a request, like gn_mean_rstd, which
+     * mn_conv2d_plan reports as gn_stats_out; finish with mn_groupnorm_finalize. */
     double* gn_stats_out;
 } mn_conv_params;
 
 int mn_conv2d_nhwc(const mn_conv_params* p, void* stream);
-/* Bytes of workspace mn_conv2d_nhwc wants for this problem (0 if it will not split). */
-int64_t mn_conv2d_workspace_bytes(const mn_conv_params* p);
-/* 1 if the tensor-core path can run this geometry (stride 1, 3x3/pad1 or 1x1, Cin%64==0, Cout%64==0,
- * pixel tiles of 128 that tile [N,H,W] exactly); 0 otherwise (mn_last_error() says why). */
-int mn_conv2d_tc_supported(const mn_conv_params* p);
-/* 2: the halo-tiled tensor-core kernel (fused input transforms) runs this problem; 1: only the per-tap tiling; 0: neither. */
-int mn_conv2d_tc_version(const mn_conv_params* p);
 
 typedef enum {
     MN_CONV_KERNEL_SMALL = 0,   /* direct 3x3 kernel for Cout <= 4 (fp32)                       */
@@ -147,15 +142,23 @@ typedef enum {
     MN_CONV_KERNEL_TC2 = 3      /* tensor-core halo tiling (+ split-K reduce)                   */
 } mn_conv_kernel;
 
-/* What mn_conv2d_nhwc would launch for *p, filled in without launching anything. */
+/* What mn_conv2d_nhwc would launch for *p, filled in without launching anything or reading memory. */
 typedef struct {
     int kernel;                 /* mn_conv_kernel                                               */
     int precision;              /* the precision that runs (MN_PREC_FP32_SIMT for small / simt) */
     int nt;                     /* tensor-core kernels: output channels per work item (64/128)  */
     int TN, TH, TW;             /* tensor-core kernels: samples x rows x columns of a pixel tile */
     int splits;                 /* split-K factor of the simt or halo-tiled kernel (1: none)    */
+    int gn_fused;               /* 1: the kernel applies the gn_mean_rstd input transform       */
+    int gn_stats_out;           /* 1: the kernel accumulates the gn_stats_out statistics        */
 } mn_conv_plan;
-/* MN_OK and *out filled in, or the status and message mn_conv2d_nhwc would return for *p. */
+/* The one dispatch decision: MN_OK and *out filled in, or the status and message mn_conv2d_nhwc would return for *p.
+ * A tensor-core precision picks the halo tiling when it runs the geometry, else the per-tap tiling; it fails
+ * (MN_ERR_UNSUPPORTED, mn_last_error() says why) when neither does.  The optional requests gn_mean_rstd and gn_stats_out
+ * never make it fail: where they cannot be honoured (fp32 kernels, per-tap tiling, tiles of several samples; the halo
+ * tiling's Cin / Cout % 64 covers the groups of 32 channels) they are dropped -- gn_fused / gn_stats_out = 0 -- and the
+ * problem is planned as if they had never been made (split-K allowed again).  Only their NULL-ness is read.
+ * mn_conv2d_nhwc refuses a request its plan drops.  y2_ptrs is no request: without the halo tiling the plan fails. */
 int mn_conv2d_plan(const mn_conv_params* p, mn_conv_plan* out);
 /* Split fp32 weights w:[taps*Cin][Cout] (the layout mn_conv2d_nhwc takes) into hi/lo 16-bit planes
  * [taps][Cout][Cin], pre-scaled by a power of two so the lo plane stays in the fp16 normal range.

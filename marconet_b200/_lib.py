@@ -42,7 +42,8 @@ CONV_KERNELS = ("small", "simt", "tc1", "tc2")     # mn_conv_kernel
 
 
 class ConvPlan(Structure):
-    _fields_ = [("kernel", c_int), ("precision", c_int), ("nt", c_int), ("TN", c_int), ("TH", c_int), ("TW", c_int), ("splits", c_int)]
+    _fields_ = [("kernel", c_int), ("precision", c_int), ("nt", c_int), ("TN", c_int), ("TH", c_int), ("TW", c_int), ("splits", c_int),
+                ("gn_fused", c_int), ("gn_stats_out", c_int)]
 
 
 class DemodDesc(Structure):
@@ -105,9 +106,6 @@ SYMBOLS = {
     "mn_device_is_sm90": (c_int, []),
     "mn_set_max_ctas": (c_int, [c_int]),
     "mn_conv2d_nhwc": (c_int, [POINTER(ConvParams), c_void_p]),
-    "mn_conv2d_workspace_bytes": (c_int64, [POINTER(ConvParams)]),
-    "mn_conv2d_tc_supported": (c_int, [POINTER(ConvParams)]),
-    "mn_conv2d_tc_version": (c_int, [POINTER(ConvParams)]),
     "mn_conv2d_plan": (c_int, [POINTER(ConvParams), POINTER(ConvPlan)]),
     "mn_groupnorm_stats": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "mn_groupnorm_finalize": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),

@@ -1,13 +1,6 @@
-// mn_conv2d_nhwc: argument validation and dispatch between the convolution kernels.
+// mn_conv2d_nhwc / mn_conv2d_plan: argument validation and the one dispatch decision between the convolution kernels.
 #include "mn_common.cuh"
 #include "conv_common.cuh"
-
-#include <stdlib.h>
-static bool tc_force_v1() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("MN_TC_V1"); v = (e && e[0] == '1') ? 1 : 0; }
-    return v == 1;
-}
 
 static int make_geom(const mn_conv_params* p, ConvGeom& g) {
     MN_REQUIRE(p != nullptr, "mn_conv2d_nhwc: null params");
@@ -20,7 +13,7 @@ static int make_geom(const mn_conv_params* p, ConvGeom& g) {
     g.bias = p->bias; g.out_scale = p->out_scale; g.residual = p->residual; g.y2_scale = p->y2_scale;
     g.valid_w = p->valid_w; g.ws = p->workspace; g.ws_bytes = p->workspace ? p->workspace_bytes : 0;
     g.gn_mr = reinterpret_cast<const float2*>(p->gn_mean_rstd); g.gn_gamma = p->gn_gamma; g.gn_beta = p->gn_beta; g.gn_swish = p->gn_swish;
-    MN_REQUIRE(!p->gn_mean_rstd || (p->gn_gamma && p->gn_beta && p->Cin % 32 == 0), "mn_conv2d_nhwc: fused GroupNorm needs gamma, beta and Cin % 32 == 0");
+    MN_REQUIRE(!p->gn_mean_rstd || (p->gn_gamma && p->gn_beta), "mn_conv2d_nhwc: fused GroupNorm needs gamma and beta");
     g.N = p->N; g.H = p->H; g.W = p->W; g.Cin = p->Cin; g.x_cs = p->x_cs;
     g.KH = p->KH; g.KW = p->KW; g.sh = p->stride_h; g.sw = p->stride_w; g.ph = p->pad_h; g.pw = p->pad_w; g.Cout = p->Cout;
     g.OH = (p->H + 2 * p->pad_h - p->KH) / p->stride_h + 1;
@@ -39,63 +32,57 @@ static int make_geom(const mn_conv_params* p, ConvGeom& g) {
     g.ktiles = g.ktiles_per_split = 0; g.splits = 1;
     g.x_scale = p->x_scale > 0.f ? p->x_scale : 1.f; g.x_absmax = p->x_absmax; g.range_flag = p->range_flag; g.range_tag = p->range_tag;
     g.y2_ptrs = p->y2_ptrs; g.gn_stats_out = p->gn_stats_out;
-    MN_REQUIRE(!p->gn_stats_out || (p->Cout % 32 == 0 && p->y), "mn_conv2d_nhwc: gn_stats_out needs Cout % 32 == 0 and the y output");
+    MN_REQUIRE(!p->gn_stats_out || p->y, "mn_conv2d_nhwc: gn_stats_out needs the y output");
     MN_REQUIRE(!p->y2_ptrs || p->y2, "mn_conv2d_nhwc: y2_ptrs needs the second output enabled (y2 != NULL)");
     return MN_OK;
 }
 
-extern "C" int64_t mn_conv2d_workspace_bytes(const mn_conv_params* p) {
-    ConvGeom g;
-    if (make_geom(p, g) != MN_OK) return -1;
-    const int splits = mn_conv_simt_plan_splits(g, (int64_t)1 << 60, p->split_k);
-    return splits > 1 ? (int64_t)splits * g.M * g.Cout * 4 : 0;
-}
-
-// Features only the halo-tiled kernel has: refuse them elsewhere.  Sets *v2 to whether that kernel runs the problem.
-static int check_v2_features(const mn_conv_params* p, const ConvGeom& g, bool* v2) {
-    *v2 = p->precision != MN_PREC_FP32_SIMT && !tc_force_v1() && mn_conv_tc2_supported(g, nullptr);
-    if ((g.y2_ptrs || g.gn_stats_out) && !*v2) {
-        mn_set_error("mn_conv2d_nhwc: per-sample output pointers (y2_ptrs) / epilogue GroupNorm statistics (gn_stats_out) exist only in the halo-tiled tensor-core kernel");
-        return MN_ERR_UNSUPPORTED;
-    }
-    if (g.gn_mr && !*v2) {
-        mn_set_error("mn_conv2d_nhwc: the fused GroupNorm input transform exists only in the halo-tiled tensor-core kernel (check mn_conv2d_tc_version)");
-        return MN_ERR_UNSUPPORTED;
-    }
-    return MN_OK;
-}
-
-// The one dispatch decision: which kernel runs *p, with which tile and split count.  mn_conv2d_nhwc launches what it returns and
-// mn_conv2d_plan reports it, so the two cannot disagree.
-static int plan_conv(const mn_conv_params* p, ConvGeom& g, mn_conv_plan* r) {
-    int rc = make_geom(p, g);
+// The one dispatch decision: which kernel runs *p, with which tile and split count, and which of the optional requests of the
+// halo tiling (fused GroupNorm input, epilogue statistics) it honours; the ones it drops are cleared in g.  mn_conv2d_nhwc launches
+// what it returns and mn_conv2d_plan reports it, so the two cannot disagree.
+static int plan_conv(const mn_conv_params* p, ConvGeom& g, mn_conv_plan* r, Tc2Plan* tc) {
+    const int rc = make_geom(p, g);
     if (rc != MN_OK) return rc;
-    bool v2;
-    if ((rc = check_v2_features(p, g, &v2)) != MN_OK) return rc;
     *r = mn_conv_plan{};
     r->precision = p->precision;
     r->splits = 1;
     switch (p->precision) {
         case MN_PREC_FP32_SIMT:
-            if (mn_conv_small_supported(g)) { r->kernel = MN_CONV_KERNEL_SMALL; return MN_OK; }
-            r->kernel = MN_CONV_KERNEL_SIMT;
-            r->splits = mn_conv_simt_plan_splits(g, p->workspace ? p->workspace_bytes : 0, p->split_k);
-            return MN_OK;
+            if (g.y2_ptrs) {
+                mn_set_error("mn_conv2d_nhwc: per-sample output pointers (y2_ptrs) exist only in the tensor-core halo tiling");
+                return MN_ERR_UNSUPPORTED;
+            }
+            g.gn_mr = nullptr; g.gn_stats_out = nullptr;
+            if (mn_conv_small_supported(g)) {
+                r->kernel = MN_CONV_KERNEL_SMALL;
+            } else {
+                r->kernel = MN_CONV_KERNEL_SIMT;
+                r->splits = mn_conv_simt_plan_splits(g, g.ws_bytes, p->split_k);
+            }
+            break;
         case MN_PREC_F16X3_TC:
         case MN_PREC_BF16X3_TC:
         case MN_PREC_F16X1_TC:
-            return mn_conv_tc_plan_info(g, v2, r) ? MN_OK : MN_ERR_UNSUPPORTED;
+            *tc = mn_conv_tc_plan(g);
+            if (!tc->ok) return MN_ERR_UNSUPPORTED;
+            r->kernel = tc->t.per_tap ? MN_CONV_KERNEL_TC1 : MN_CONV_KERNEL_TC2;
+            r->nt = tc->t.nt; r->TN = tc->t.TN; r->TH = tc->t.TH; r->TW = tc->t.TW; r->splits = tc->t.ksplit;
+            break;
         default:
             mn_set_error("mn_conv2d_nhwc: unknown precision mode %d", p->precision);
             return MN_ERR_UNSUPPORTED;
     }
+    r->gn_fused = g.gn_mr != nullptr;
+    r->gn_stats_out = g.gn_stats_out != nullptr;
+    return MN_OK;
 }
 
 extern "C" int mn_conv2d_plan(const mn_conv_params* p, mn_conv_plan* out) {
     MN_REQUIRE(out != nullptr, "mn_conv2d_plan: null output");
     ConvGeom g;
     mn_conv_plan r;
-    const int rc = plan_conv(p, g, &r);
+    Tc2Plan tc;
+    const int rc = plan_conv(p, g, &r, &tc);
     if (rc == MN_OK) *out = r;
     return rc;
 }
@@ -103,29 +90,19 @@ extern "C" int mn_conv2d_plan(const mn_conv_params* p, mn_conv_plan* out) {
 extern "C" int mn_conv2d_nhwc(const mn_conv_params* p, void* stream) {
     ConvGeom g;
     mn_conv_plan r;
-    const int rc = plan_conv(p, g, &r);
+    Tc2Plan tc;
+    const int rc = plan_conv(p, g, &r, &tc);
     if (rc != MN_OK) return rc;
+    // a request the plan drops is refused, not ignored: the caller would get an input never normalised or statistics never written
+    if ((p->gn_mean_rstd && !r.gn_fused) || (p->gn_stats_out && !r.gn_stats_out)) {
+        mn_set_error("mn_conv2d_nhwc: the fused GroupNorm input (gn_mean_rstd) and the epilogue statistics (gn_stats_out) need the "
+                     "tensor-core halo tiling with one sample per pixel tile; mn_conv2d_plan drops them for this problem");
+        return MN_ERR_UNSUPPORTED;
+    }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     switch (r.kernel) {
         case MN_CONV_KERNEL_SMALL: return mn_conv_small_launch(g, st);
-        case MN_CONV_KERNEL_SIMT: g.splits = r.splits; return mn_conv_simt_launch(g, nullptr, st);
-        case MN_CONV_KERNEL_TC2: return mn_conv_tc2_launch(g, p->w_tc_hi, p->w_tc_lo, p->w_tc_scale, p->precision, st);
-        default: return mn_conv_tc_launch(g, p->w_tc_hi, p->w_tc_lo, p->w_tc_scale, p->precision, st);
+        case MN_CONV_KERNEL_SIMT: g.splits = r.splits; return mn_conv_simt_launch(g, st);
+        default: return mn_conv_tc_launch(g, tc, p->w_tc_hi, p->w_tc_lo, p->w_tc_scale, p->precision, st);
     }
-}
-
-extern "C" int mn_conv2d_tc_supported(const mn_conv_params* p) {
-    ConvGeom g;
-    if (make_geom(p, g) != MN_OK) return 0;
-    const char* why = "";
-    const int ok = (!tc_force_v1() && mn_conv_tc2_supported(g, nullptr)) || mn_conv_tc_supported(g, &why);
-    if (!ok) mn_set_error("tensor-core path unsupported: %s", why);
-    return ok;
-}
-
-extern "C" int mn_conv2d_tc_version(const mn_conv_params* p) {
-    ConvGeom g;
-    if (make_geom(p, g) != MN_OK) return 0;
-    if (!tc_force_v1() && mn_conv_tc2_supported(g, nullptr)) return 2;
-    return mn_conv_tc_supported(g, nullptr) ? 1 : 0;
 }

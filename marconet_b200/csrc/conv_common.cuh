@@ -142,17 +142,30 @@ __device__ __forceinline__ float4 conv_epilogue_row4(const ConvGeom& g, int m, i
 }
 
 int mn_conv_simt_plan_splits(const ConvGeom& g, int64_t ws_bytes, int requested);
-int mn_conv_simt_launch(ConvGeom g, const float* unused, cudaStream_t st);
+int mn_conv_simt_launch(ConvGeom g, cudaStream_t st);
 int mn_conv_splitk_reduce_launch(const ConvGeom& g, cudaStream_t st);   // sums g.splits partial tiles in g.ws and runs the fused epilogue
 
-// tensor-core path, per-tap tiling (conv_tc2.cu; weight packing in conv_tc.cu)
-int mn_conv_tc_supported(const ConvGeom& g, const char** why);
-int mn_conv_tc_launch(const ConvGeom& g, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st);
-// tensor-core path, halo tiling: halo tiles + weight multicast + persistent CTAs (conv_tc2.cu)
-int mn_conv_tc2_supported(const ConvGeom& g, const char** why);
-int mn_conv_tc2_launch(const ConvGeom& g, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st);
-// the plan either tensor-core tiling would launch (halo: plan_tc2, else plan_tc1) into *out; 0 when it cannot run the problem
-int mn_conv_tc_plan_info(const ConvGeom& g, bool halo, mn_conv_plan* out);
+// tensor-core path (conv_tc2.cu; weight packing in conv_tc.cu): the tiling of one problem, as the kernel receives it
+struct Tc2Geom {
+    int TW, TH, TN, HWd, HHt, halo_rows, box_bytes, halo_stage_bytes;
+    int tiles_w, tiles_h, tiles_n, m_tiles, m_groups, n_tiles;
+    int cblocks, taps, KW, ph, pw;
+    int ksplit, cbps;   // split-K over channel blocks for layers with too few tiles: work = (tile, k-slice), cbps channel blocks each
+    int bstages, cs;
+    int hstages;        // depth of the A-tile ring
+    int per_tap;        // 0: one halo per channel block; 1: one shifted 128-pixel box per (channel block, tap)
+    int nt;             // output channels per work item: 64 or 128 (the kernel's NT)
+    const float* wscale;
+    int prec;
+};
+struct Tc2Plan { bool ok; const char* why; int smem; Tc2Geom t; };
+// The tensor-core plan of g: the halo tiling (halo tiles + weight multicast + persistent CTAs) when it runs g, else the per-tap
+// tiling.  The requests only the halo tiling with one sample per pixel tile honours -- the fused GroupNorm input (g.gn_mr) and the
+// epilogue statistics (g.gn_stats_out) -- are dropped (cleared in g) when the plan cannot honour them, and g is planned as if they
+// had never been made.  Per-sample output pointers (g.y2_ptrs) are not optional: without the halo tiling the plan fails.
+// !ok: no tiling runs g (mn_last_error says why).
+Tc2Plan mn_conv_tc_plan(ConvGeom& g);
+int mn_conv_tc_launch(const ConvGeom& g, Tc2Plan& p, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st);
 // direct 3x3 conv for Cout <= 4 (conv_small.cu)
 bool mn_conv_small_supported(const ConvGeom& g);
 int mn_conv_small_launch(const ConvGeom& g, cudaStream_t st);

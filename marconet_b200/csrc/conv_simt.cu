@@ -259,13 +259,12 @@ int mn_conv_simt_plan_splits(const ConvGeom& g0, int64_t ws_bytes, int requested
     return mn_cdiv(ktiles, mn_cdiv(ktiles, splits));
 }
 
-int mn_conv_simt_launch(ConvGeom g, const float* x_ptr_for_align, cudaStream_t st) {
+int mn_conv_simt_launch(ConvGeom g, cudaStream_t st) {
     g.ktiles = mn_cdiv(g.K, BK);
     g.ktiles_per_split = mn_cdiv(g.ktiles, g.splits);
     g.splits = mn_cdiv(g.ktiles, g.ktiles_per_split);
     const bool vec_a = (g.Cin % BK == 0) && (g.x_cs % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.x) & 15) == 0);
     const bool vec_b = (g.Cout % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.w) & 15) == 0);
-    (void)x_ptr_for_align;
     int rc = (g.Cout > 64) ? launch_simt<128>(g, vec_a, vec_b, st) : launch_simt<64>(g, vec_a, vec_b, st);
     if (rc != MN_OK) return rc;
     if (g.splits > 1) {

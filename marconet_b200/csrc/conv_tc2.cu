@@ -34,19 +34,6 @@ constexpr int SMEM_LIMIT = 232448;              // 227 KB
 
 template <int A> struct ActTag { static constexpr int value = A; };
 
-struct Tc2Geom {
-    int TW, TH, TN, HWd, HHt, halo_rows, box_bytes, halo_stage_bytes;
-    int tiles_w, tiles_h, tiles_n, m_tiles, m_groups, n_tiles;
-    int cblocks, taps, KW, ph, pw;
-    int ksplit, cbps;   // split-K over channel blocks for layers with too few tiles: work = (tile, k-slice), cbps channel blocks each
-    int bstages, cs;
-    int hstages;        // depth of the A-tile ring
-    int per_tap;        // 0: one halo per channel block; 1: one shifted 128-pixel box per (channel block, tap)
-    int nt;             // output channels per work item: 64 or 128 (the kernel's NT)
-    const float* wscale;
-    int prec;
-};
-
 // One thread's share of the epilogue GroupNorm statistics (sum and sum of squares of y per sample and group).  Summing y and y*y
 // directly in fp32 loses the variance to cancellation when |mean| >> std (E[y^2] - mean^2: ~1e-3 relative at mean/std = 300):
 // the values are summed about a pivot (the thread's first value) in fp32 and turned into sum / sum of squares in fp64, where
@@ -555,8 +542,6 @@ PFN_encodeTiled get_encode2() {
     return fn;
 }
 
-struct Tc2Plan { bool ok; const char* why; int smem; Tc2Geom t; };
-
 bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
 // checks shared by both tilings; fills the fields that do not depend on the pixel tile
@@ -636,8 +621,8 @@ bool plan_finish(const ConvGeom& g, Tc2Plan& p, bool allow_ksplit) {
     return true;
 }
 
-// halo tiling ("version 2"): one (TH+2) x (TW+2) halo per channel block
-Tc2Plan plan_tc2(const ConvGeom& g) {
+// halo tiling ("version 2"): one (TH+2) x (TW+2) halo per channel block; drops the optional requests of tiles of several samples
+Tc2Plan plan_tc2(ConvGeom& g) {
     Tc2Plan p{};
     auto fail = [&](const char* w) { p.ok = false; p.why = w; return p; };
     if (!plan_common(g, p)) return p;
@@ -656,9 +641,8 @@ Tc2Plan plan_tc2(const ConvGeom& g) {
     while (t.TN > 1 && t.TN * t.HHt * t.HWd > 208) t.TN >>= 1;
     t.halo_rows = t.TN * t.HHt * t.HWd;
     if (t.halo_rows > 208) return fail("halo tile too large for shared memory");
-    if ((g.y2_ptrs || g.gn_stats_out) && t.TN != 1)
-        return fail("per-sample output pointers / epilogue GroupNorm statistics need samples of at least one whole pixel tile (OH*OW >= 128)");
-    if (g.gn_mr && t.TN != 1) return fail("fused GroupNorm input transform needs samples of at least one whole pixel tile (H*W >= 128)");
+    if (g.y2_ptrs && t.TN != 1) return fail("per-sample output pointers need samples of at least one whole pixel tile (OH*OW >= 128)");
+    if (t.TN != 1) { g.gn_mr = nullptr; g.gn_stats_out = nullptr; }    // both work per sample: one sample per tile or not at all
     if (t.HWd > 256 || t.HHt > 256 || t.TN > 256) return fail("TMA box dim");
     t.tiles_w = g.W / t.TW; t.tiles_h = g.H / t.TH; t.tiles_n = (g.N + t.TN - 1) / t.TN;
     plan_finish(g, p, true);
@@ -720,7 +704,23 @@ int launch_tc2_nt(const CUtensorMap& ma, const CUtensorMap& mbh, const CUtensorM
     return p.t.nt == 128 ? launch_tc2<GN, MODE, 128>(ma, mbh, mbl, g, p, st) : launch_tc2<GN, MODE, 64>(ma, mbh, mbl, g, p, st);
 }
 
-int launch_plan(const ConvGeom& g, Tc2Plan& p, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st) {
+}  // namespace
+
+Tc2Plan mn_conv_tc_plan(ConvGeom& g) {
+    const Tc2Plan halo = plan_tc2(g);
+    if (halo.ok) return halo;
+    if (g.y2_ptrs) {
+        mn_set_error("mn_conv2d_nhwc: per-sample output pointers (y2_ptrs) exist only in the tensor-core halo tiling, which does not run this shape (%s)", halo.why);
+        return halo;
+    }
+    g.gn_mr = nullptr; g.gn_stats_out = nullptr;      // requests of the halo tiling only
+    const Tc2Plan per_tap = plan_tc1(g);
+    if (!per_tap.ok)
+        mn_set_error("tensor-core path unsupported: halo tiling: %s; per-tap tiling: %s", halo.why, per_tap.why);
+    return per_tap;
+}
+
+int mn_conv_tc_launch(const ConvGeom& g, Tc2Plan& p, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st) {
     if (!w_hi || !w_lo || !w_scale) { mn_set_error("mn_conv2d_nhwc: tensor-core precision needs packed w_tc_hi/w_tc_lo/w_tc_scale"); return MN_ERR_INVALID; }
     PFN_encodeTiled enc = get_encode2();
     if (!enc) { mn_set_error("cuTensorMapEncodeTiled not available from the driver"); return MN_ERR_CUDA; }
@@ -757,38 +757,4 @@ int launch_plan(const ConvGeom& g, Tc2Plan& p, const void* w_hi, const void* w_l
     ConvGeom gr = g;
     gr.splits = t.ksplit;
     return mn_conv_splitk_reduce_launch(gr, st);
-}
-
-}  // namespace
-
-int mn_conv_tc2_supported(const ConvGeom& g, const char** why) {
-    Tc2Plan p = plan_tc2(g);
-    if (why) *why = p.ok ? "" : p.why;
-    return p.ok ? 1 : 0;
-}
-
-int mn_conv_tc2_launch(const ConvGeom& g, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st) {
-    Tc2Plan p = plan_tc2(g);
-    if (!p.ok) { mn_set_error("mn_conv2d_nhwc: tensor-core halo tiling does not support this shape (%s)", p.why); return MN_ERR_UNSUPPORTED; }
-    return launch_plan(g, p, w_hi, w_lo, w_scale, prec, st);
-}
-
-int mn_conv_tc_plan_info(const ConvGeom& g, bool halo, mn_conv_plan* out) {
-    const Tc2Plan p = halo ? plan_tc2(g) : plan_tc1(g);
-    if (!p.ok) { mn_set_error("tensor-core %s tiling does not support this shape (%s)", halo ? "halo" : "per-tap", p.why); return 0; }
-    out->kernel = halo ? MN_CONV_KERNEL_TC2 : MN_CONV_KERNEL_TC1;
-    out->nt = p.t.nt; out->TN = p.t.TN; out->TH = p.t.TH; out->TW = p.t.TW; out->splits = p.t.ksplit;
-    return 1;
-}
-
-int mn_conv_tc_supported(const ConvGeom& g, const char** why) {
-    Tc2Plan p = plan_tc1(g);
-    if (why) *why = p.ok ? "" : p.why;
-    return p.ok ? 1 : 0;
-}
-
-int mn_conv_tc_launch(const ConvGeom& g, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st) {
-    Tc2Plan p = plan_tc1(g);
-    if (!p.ok) { mn_set_error("mn_conv2d_nhwc: tensor-core path does not support this shape (%s)", p.why); return MN_ERR_UNSUPPORTED; }
-    return launch_plan(g, p, w_hi, w_lo, w_scale, prec, st);
 }

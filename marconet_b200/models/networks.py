@@ -587,8 +587,8 @@ class ResTextBlockV2(nn.Module):
 def _res_block(pk, x, valid_w=None, mr1=None):
     """GN -> swish -> conv -> GN -> swish -> conv (+ 1x1 skip), reference networks.py:506-516.
     ``mr1``: statistics of x when the convolution that produced x already accumulated them in its epilogue."""
-    # normalise + swish is the tensor-core kernel's operand transform (ops.FUSE_GN, default on: no separate pass over x); layers the
-    # fp32 kernel runs, or MN_FUSE_GN=0, take mn_groupnorm_apply first
+    # normalise + swish is the tensor-core kernel's operand transform (no separate pass over x); layers whose plan drops it (fp32
+    # kernel, per-tap tiling, tiles of several samples) take mn_groupnorm_apply first
     if mr1 is None:
         mr1 = ops.groupnorm_stats(x, valid_w=valid_w)
     # the statistics of h (input of norm2) are accumulated by the epilogue of the conv that writes h: no separate read pass

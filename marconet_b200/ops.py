@@ -32,7 +32,7 @@ def set_default_precision(p):
 
 def graph_key():
     """Everything process-global that a captured CUDA graph of this library bakes in."""
-    return (_DEFAULT_PRECISION, PLAN_VERSION, MAX_CTAS, FUSE_GN)
+    return (_DEFAULT_PRECISION, PLAN_VERSION, MAX_CTAS)
 
 
 def graphs_allowed():
@@ -306,52 +306,39 @@ class calibration:
 TC_FALLBACKS = {}      # shape key -> (layer name, GFLOP, reason): convs that a tensor-core default ran on the fp32 CUDA-core kernel
 
 
-def _note_fallback(cw, key, flop, p):
+def _note_fallback(cw, key, flop, reason):
     """A tensor-core precision was the default but this conv runs on the exact fp32 kernel (unsupported geometry: Cin/Cout not
     multiples of 64, stride != 1, tiny launch ...).  Logged ONCE per shape so that a checkpoint with different channel counts does
     not quietly run 6x slower (VERDICT r1); ``ops.TC_FALLBACKS`` keeps the list, bench.py reports it."""
     if key in TC_FALLBACKS:
         return
-    if flop < TC_MIN_FLOP:
-        reason = f"below TC_MIN_FLOP ({flop / 1e6:.1f} MFLOP)"
-    elif cw is None or not cw.tc_capable():
-        reason = "Cin or Cout is not a multiple of 64"
-    elif key[7] != (1, 1):
-        reason = "stride != 1"
-    else:
-        lib = _lib.load()
-        lib.mn_conv2d_tc_supported(ctypes.byref(p))           # fills mn_last_error() with the kernel's own reason
-        reason = lib.mn_last_error().decode(errors="replace") or "unsupported geometry"
     name = cw.name if cw is not None else "unnamed"
     TC_FALLBACKS[key] = (name, flop / 1e9, reason)
     import logging
     logging.getLogger("marconet_b200").info("conv %s %s runs on the fp32 CUDA-core kernel: %s", name, key, reason)
 
 
-# fused GroupNorm(+swish) input transform of the tensor-core conv (MN_FUSE_GN): "1" (default) every layer that kernel runs, "0" never
-# (mn_groupnorm_apply writes a normalised copy first), "auto" only the layers with 128-wide tiles (Cout % 128 == 0)
-FUSE_GN = {"0": 0, "1": 1, "auto": 2, "2": 2}.get(_os.environ.get("MN_FUSE_GN", "1"), 1)
-
-
-def _fuse_gn(cout):
-    return FUSE_GN == 1 or (FUSE_GN == 2 and cout % 128 == 0)
 TC_MIN_FLOP = 3.0e7    # tiny launches are latency-bound either way and stay on the exact fp32 path
 
 
 def conv2d(x, w, kh, kw, stride=(1, 1), pad=(0, 0), bias=None, out_scale=None, residual=None,
            res_broadcast=False, act=ACT_NONE, gain=1.0, out=None, out2=None, y2_scale=None,
-           valid_w=None, precision=None, want_y=True, split_k=0, gn=None, gn_fuse=None, out2_ptrs=None, gn_stats=False, plan=None):
+           valid_w=None, precision=None, want_y=True, split_k=0, gn=None, gn_fuse=True, out2_ptrs=None, gn_stats=False, plan=None):
     """mn_conv2d_nhwc.  ``w`` is the packed [KH*KW*Cin, Cout] matrix.  Returns y (or (y, y2)).
     ``plan``: a dict that receives what was launched (mn_conv2d_plan): ``kernel`` ("small" / "simt" / "tc1" / "tc2"), ``precision``,
     ``nt``, ``TN``, ``TH``, ``TW``, ``splits`` (split-K), ``gn_fused``, ``gn_stats_out`` (statistics from the epilogue) and ``x_scale``.
     ``gn=(mean_rstd, gamma, beta)``: the conv input is swish(GroupNorm(x)); fused into the halo-tiled tensor-core kernel's operand-split
-    stage when ``gn_fuse`` is true and that kernel runs the layer, otherwise applied by mn_groupnorm_apply first.
+    stage when ``gn_fuse`` is true and the plan honours it (that kernel, one sample per pixel tile), otherwise applied by
+    mn_groupnorm_apply first; ``gn_fuse=False`` forces the two passes.
     (Default on since the fused instantiation runs four lanes per halo row with the GroupNorm constants in registers: all eight
     normalise passes gone, 1.3 % per line on the same box; its first form -- one lane per row, per-row
     global loads of mean / rstd -- measured 8.7 vs 7.1 ms.)
     ``gn_stats=True``: also return the GroupNorm statistics (mean / rstd [N, Cout/32, 2]) of the OUTPUT, for the GroupNorm that
     follows this conv (networks.py:508-512): accumulated by the tensor-core kernel's epilogue (mn_conv_params.gn_stats_out, no read
-    pass over y) when that kernel runs the layer, by mn_groupnorm_stats otherwise.  Returns (y, mean_rstd)."""
+    pass over y) when the plan honours it, by mn_groupnorm_stats otherwise.  Returns (y, mean_rstd).
+    The library decides what runs (mn_conv2d_plan: asked once, and again only after a fall-back to fp32); this wrapper only picks the precision requested -- explicit, then
+    the layer's plan, then the process default -- and keeps a default tensor-core request away from tiny launches (TC_MIN_FLOP) and
+    from raw weights, which have no tensor-core planes."""
     global LAUNCHES
     lib = _lib.load()
     n, h, wd, cin, x_cs = nhwc_info(x, "x")
@@ -402,50 +389,50 @@ def conv2d(x, w, kh, kw, stride=(1, 1), pad=(0, 0), bias=None, out_scale=None, r
     p.workspace = ws.data_ptr(); p.workspace_bytes = ws.numel() * 4
     p.split_k = split_k
     prec = precision if precision is not None else (cw.precision if (cw is not None and cw.precision is not None) else _DEFAULT_PRECISION)
-    gn_fused = False
-    if prec != PREC_FP32_SIMT:
-        ver = 0
-        if (cw is not None and cw.tc_capable() and stride == (1, 1)
-                and (precision is not None or 2.0 * n * oh * ow * cout * kh * kw * cin >= TC_MIN_FLOP)):
-            ver = lib.mn_conv2d_tc_version(ctypes.byref(p))
-        use_tc = ver > 0
-        if use_tc:
-            hi, lo, sc = cw.tc(prec)
-            p.w_tc_hi = hi.data_ptr(); p.w_tc_lo = lo.data_ptr(); p.w_tc_scale = sc.data_ptr()
-            p.x_scale = cw.x_scale
-            p.range_flag = range_flags(x.device).data_ptr() + 4 * (cw.tag % _RANGE_SLOTS); p.range_tag = cw.tag
-            calib = getattr(_TLS, "calib", None)
-            if calib is not None:
-                p.x_absmax = calib.slot(cw).data_ptr()
-            if gn is not None and ver == 2 and (_fuse_gn(cout) if gn_fuse is None else gn_fuse):
-                p.gn_mean_rstd = gn[0].data_ptr(); p.gn_gamma = gn[1].data_ptr(); p.gn_beta = gn[2].data_ptr(); p.gn_swish = 1
-                gn_fused = lib.mn_conv2d_tc_version(ctypes.byref(p)) == 2    # the plan needs one sample per 128-pixel tile (TN == 1)
-                if not gn_fused:
-                    p.gn_mean_rstd = p.gn_gamma = p.gn_beta = None; p.gn_swish = 0
-        elif precision is not None:
-            raise RuntimeError("conv2d: tensor-core precision requested explicitly but this layer/shape is not supported: "
-                               + lib.mn_last_error().decode(errors="replace"))
-        else:
-            prec = PREC_FP32_SIMT
-            _note_fallback(cw, (n, h, wd, cin, cout, kh, kw, stride), 2.0 * n * oh * ow * cout * kh * kw * cin, p)
+    # the optional requests of the halo-tiled tensor-core kernel: the plan says which of them it honours
+    if gn is not None and gn_fuse:
+        p.gn_mean_rstd = gn[0].data_ptr(); p.gn_gamma = gn[1].data_ptr(); p.gn_beta = gn[2].data_ptr(); p.gn_swish = 1
+    if gn_stats and y is not None and out2_ptrs is None:
+        p.gn_stats_out = 1          # the plan reads the pointer as NULL / non-NULL only: the buffer follows once the plan accepts
     p.precision = prec
+    cp = _lib.ConvPlan()
+    if prec != PREC_FP32_SIMT:
+        flop = 2.0 * n * oh * ow * cout * kh * kw * cin
+        if cw is None:
+            why = "a raw weight has no tensor-core planes (pass a ConvWeight)"
+        elif precision is None and flop < TC_MIN_FLOP:
+            why = f"below TC_MIN_FLOP ({flop / 1e6:.1f} MFLOP)"
+        else:
+            why = lib.mn_last_error().decode(errors="replace") if lib.mn_conv2d_plan(ctypes.byref(p), ctypes.byref(cp)) else None
+        if why is not None:
+            if precision is not None:
+                raise RuntimeError("conv2d: tensor-core precision requested explicitly but this layer/shape is not supported: " + why)
+            _note_fallback(cw, (n, h, wd, cin, cout, kh, kw, stride), flop, why)
+            prec = p.precision = PREC_FP32_SIMT
+    if prec == PREC_FP32_SIMT:
+        _lib.check(lib.mn_conv2d_plan(ctypes.byref(p), ctypes.byref(cp)), "mn_conv2d_plan")
+    else:
+        hi, lo, sc = cw.tc(prec)
+        p.w_tc_hi = hi.data_ptr(); p.w_tc_lo = lo.data_ptr(); p.w_tc_scale = sc.data_ptr()
+        p.x_scale = cw.x_scale
+        p.range_flag = range_flags(x.device).data_ptr() + 4 * (cw.tag % _RANGE_SLOTS); p.range_tag = cw.tag
+        calib = getattr(_TLS, "calib", None)
+        if calib is not None:
+            p.x_absmax = calib.slot(cw).data_ptr()
     stats_ws = None
-    if gn_stats and prec != PREC_FP32_SIMT and ver == 2 and cout % 32 == 0 and y is not None and out2_ptrs is None:
+    if cp.gn_stats_out:
         stats_ws = torch.zeros((n * (cout // 32) * 2,), dtype=torch.float64, device=x.device)
-        p.gn_stats_out = stats_ws.data_ptr()
-        if lib.mn_conv2d_tc_version(ctypes.byref(p)) != 2:     # epilogue statistics need one sample per 128-pixel tile (TN == 1)
-            p.gn_stats_out = None
-            stats_ws = None
-    if gn is not None and not gn_fused:      # no fused kernel for this layer: normalise into a temporary first
-        xg = groupnorm_apply(x, gn[0], gn[1], gn[2], valid_w=valid_w)
-        p.x = xg.data_ptr(); p.x_cs = xg.shape[3]
+    p.gn_stats_out = _ptr(stats_ws)
+    if not cp.gn_fused:
+        p.gn_mean_rstd = p.gn_gamma = p.gn_beta = None; p.gn_swish = 0
+        if gn is not None:          # normalise into a temporary first
+            xg = groupnorm_apply(x, gn[0], gn[1], gn[2], valid_w=valid_w)
+            p.x = xg.data_ptr(); p.x_cs = xg.shape[3]
     _lib.check(lib.mn_conv2d_nhwc(ctypes.byref(p), _stream()), "mn_conv2d_nhwc")
     LAUNCHES += 1
     if plan is not None:
-        cp = _lib.ConvPlan()
-        _lib.check(lib.mn_conv2d_plan(ctypes.byref(p), ctypes.byref(cp)), "mn_conv2d_plan")
-        plan.update(kernel=_lib.CONV_KERNELS[cp.kernel], precision=cp.precision, nt=cp.nt, TN=cp.TN, TH=cp.TH, TW=cp.TW,
-                    splits=cp.splits, gn_fused=gn_fused, gn_stats_out=stats_ws is not None, x_scale=p.x_scale if p.x_scale > 0 else 1.0)
+        plan.update(kernel=_lib.CONV_KERNELS[cp.kernel], precision=cp.precision, nt=cp.nt, TN=cp.TN, TH=cp.TH, TW=cp.TW, splits=cp.splits,
+                    gn_fused=bool(cp.gn_fused), gn_stats_out=bool(cp.gn_stats_out), x_scale=p.x_scale if p.x_scale > 0 else 1.0)
     calib = getattr(_TLS, "calib", None)
     if calib is not None and calib.compare and cw is not None and prec != PREC_FP32_SIMT and precision is None:
         # tuning tool only (pipeline.tune_precision): the same layer through the exact fp32 kernel and both split formats

@@ -224,17 +224,3 @@ def test_precision_plan_survives_repack_by_name():
         ops.PLAN.clear()
         ops.PLAN.update(saved)
 
-
-def test_groupnorm_fusion_policy_and_graph_key(monkeypatch):
-    """MN_FUSE_GN policy (ops.FUSE_GN): 1 = every tensor-core layer (default), 0 = never, 2 ("auto") = 128-wide-tile layers only;
-    the policy is part of the module-graph key, so a recorded forward is never replayed under another policy."""
-    from marconet_b200 import ops
-    assert ops.FUSE_GN in (0, 1, 2)
-    monkeypatch.setattr(ops, "FUSE_GN", 1)
-    assert ops._fuse_gn(64) and ops._fuse_gn(256)
-    k1 = ops.graph_key()
-    monkeypatch.setattr(ops, "FUSE_GN", 2)
-    assert not ops._fuse_gn(64) and ops._fuse_gn(128) and ops._fuse_gn(256)
-    assert ops.graph_key() != k1
-    monkeypatch.setattr(ops, "FUSE_GN", 0)
-    assert not ops._fuse_gn(256)
