@@ -6,8 +6,11 @@ namespace {
 
 // ---------------------------------------------------------------- GroupNorm statistics
 // Each thread owns 4 consecutive channels (float4 loads, fully coalesced rows); a block walks a pixel chunk with
-// blockDim/(C/4) pixels per iteration.  fp32 partials are flushed to fp64 every 32 pixels, reduced over the 8 lanes of a
-// 32-channel group by shuffles, over the block in shared memory, then one fp64 atomicAdd per (block, group, moment).
+// blockDim/(C/4) pixels per iteration.  Each thread sums its values about a pivot (its first value) in fp32, flushed to fp64
+// every 32 pixels, and turns the deviations into sum / sum of squares in fp64 (as conv_tc2.cu's GnAcc): summing x and x*x
+// directly in fp32 lost the variance to cancellation in E[x^2] - mean^2 when |mean| >> std (rstd 4.9e-4 off at mean/std
+// = 300, 3.8e-2 at 3000 on an H100; profiles/r12_offset_stats.txt).  The sums are reduced over the 8 lanes of a 32-channel
+// group by shuffles, over the block in shared memory, then one fp64 atomicAdd per (block, group, moment).
 __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__ x, int x_cs, int H, int W, int C, int cpg,
                                                        const int32_t* __restrict__ valid_w, double* __restrict__ stats, int pix_per_block) {
     mn_pdl_prologue();
@@ -21,9 +24,9 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
     const int p_begin = blockIdx.x * pix_per_block;
     const int p_end = min(HW, p_begin + pix_per_block);
     const float* xn = x + (size_t)n * HW * x_cs + my_c;
-    float s = 0.f, ss = 0.f;
+    float piv = 0.f, s = 0.f, ss = 0.f;            // fp32 run of deviations from piv
     double ds = 0.0, dss = 0.0;
-    int cnt = 0;
+    int cnt = 0, npix = 0;
     if (my_p < ppi) {
         // 4 pixels per trip: the four 128-bit loads are issued before any of them is consumed
         for (int p = p_begin + my_p; p < p_end; p += 4 * ppi) {
@@ -38,13 +41,20 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 if (!on[k]) continue;
-                s += (v[k].x + v[k].y) + (v[k].z + v[k].w);
-                ss = fmaf(v[k].x, v[k].x, ss); ss = fmaf(v[k].y, v[k].y, ss); ss = fmaf(v[k].z, v[k].z, ss); ss = fmaf(v[k].w, v[k].w, ss);
+                if (npix++ == 0) piv = v[k].x;
+                const float d0 = v[k].x - piv, d1 = v[k].y - piv, d2 = v[k].z - piv, d3 = v[k].w - piv;
+                s += (d0 + d1) + (d2 + d3);
+                ss = fmaf(d0, d0, ss); ss = fmaf(d1, d1, ss); ss = fmaf(d2, d2, ss); ss = fmaf(d3, d3, ss);
                 if (++cnt == 32) { ds += (double)s; dss += (double)ss; s = 0.f; ss = 0.f; cnt = 0; }
             }
         }
     }
     ds += (double)s; dss += (double)ss;
+    {   // deviations -> sum x = m p + ds ;  sum x^2 = dss + 2 p ds + m p^2   (m = 4 * npix values)
+        const double pd = piv, md = 4.0 * npix;
+        dss += pd * (2.0 * ds + md * pd);
+        ds += md * pd;
+    }
     const int lpg = cpg >> 2;                      // lanes per group (8 for 32-channel groups)
     for (int o = lpg >> 1; o > 0; o >>= 1) {
         ds += __shfl_xor_sync(0xffffffffu, ds, o);
@@ -153,11 +163,13 @@ __global__ void __launch_bounds__(256) adain_stats_kernel(const float* __restric
     const int p_begin = blockIdx.x * pix_per_block, p_end = min(npix, p_begin + pix_per_block);
     const float* pr = prior + (size_t)i * H * Wp * prior_cs + my_c;
     const float* ft = feat + (size_t)wn.line * H * W * feat_cs + my_c;
-    float4 sp = make_float4(0.f, 0.f, 0.f, 0.f), qp = sp, sl = sp, ql = sp;
+    // fp32 runs of deviations from per-channel pivots (the thread's first pixel), turned into sums about zero in fp64 below: see
+    // gn_stats_kernel (plain fp32 sums of x and x*x lose the variance to cancellation when |mean| >> std)
+    float4 sp = make_float4(0.f, 0.f, 0.f, 0.f), qp = sp, sl = sp, ql = sp, pp = sp, pl = sp;
     double acc[16];
 #pragma unroll
     for (int k = 0; k < 16; ++k) acc[k] = 0.0;
-    int cnt = 0;
+    int cnt = 0, nval = 0;
     auto flush = [&]() {
         acc[0] += sp.x; acc[1] += sp.y; acc[2] += sp.z; acc[3] += sp.w; acc[4] += qp.x; acc[5] += qp.y; acc[6] += qp.z; acc[7] += qp.w;
         acc[8] += sl.x; acc[9] += sl.y; acc[10] += sl.z; acc[11] += sl.w; acc[12] += ql.x; acc[13] += ql.y; acc[14] += ql.z; acc[15] += ql.w;
@@ -166,21 +178,30 @@ __global__ void __launch_bounds__(256) adain_stats_kernel(const float* __restric
     };
     if (my_p < ppi && wv > 0) {
         // four pixels per trip, all eight loads issued before the first add (two loads in flight per thread left the kernel at
-        // ~2.7 TB/s); same pixel order and flush cadence per thread, the zero-filled tail adds nothing: bit-identical sums
+        // ~2.7 TB/s); same pixel order and flush cadence per thread.  The tail past p_end is filled with the pivots: it adds nothing
         for (int p = p_begin + my_p; p < p_end; p += 4 * ppi) {
             float4 a[4], b[4];
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
                 const int pu = p + u * ppi;
-                a[u] = b[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+                a[u] = pp; b[u] = pl;
                 if (pu < p_end) {
                     const int yy = pu / wv, xx = pu - yy * wv;
                     a[u] = *reinterpret_cast<const float4*>(pr + ((size_t)yy * Wp + wn.y1 + xx) * prior_cs);
                     b[u] = *reinterpret_cast<const float4*>(ft + ((size_t)yy * W + wn.x1 + xx) * feat_cs);
+                    ++nval;
                 }
+            }
+            if (p == p_begin + my_p) {              // first trip: pixel p is in range, its values are the pivots
+                pp = a[0]; pl = b[0];
+#pragma unroll
+                for (int u = 1; u < 4; ++u)
+                    if (p + u * ppi >= p_end) { a[u] = pp; b[u] = pl; }
             }
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
+                a[u].x -= pp.x; a[u].y -= pp.y; a[u].z -= pp.z; a[u].w -= pp.w;
+                b[u].x -= pl.x; b[u].y -= pl.y; b[u].z -= pl.z; b[u].w -= pl.w;
                 sp.x += a[u].x; sp.y += a[u].y; sp.z += a[u].z; sp.w += a[u].w;
                 qp.x = fmaf(a[u].x, a[u].x, qp.x); qp.y = fmaf(a[u].y, a[u].y, qp.y); qp.z = fmaf(a[u].z, a[u].z, qp.z); qp.w = fmaf(a[u].w, a[u].w, qp.w);
                 sl.x += b[u].x; sl.y += b[u].y; sl.z += b[u].z; sl.w += b[u].w;
@@ -191,6 +212,17 @@ __global__ void __launch_bounds__(256) adain_stats_kernel(const float* __restric
         }
     }
     flush();
+    {   // deviations -> sum x = m p + s ;  sum x^2 = q + 2 p s + m p^2   (m = nval pixels)
+        const float pv[8] = {pp.x, pp.y, pp.z, pp.w, pl.x, pl.y, pl.z, pl.w};
+        const double md = nval;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int si = (j < 4 ? 0 : 8) + (j & 3), qi = si + 4;
+            const double pd = pv[j];
+            acc[qi] += pd * (2.0 * acc[si] + md * pd);
+            acc[si] += md * pd;
+        }
+    }
     // reduce the ppi pixel slots of the block in shared memory, then one atomic per (block, channel, moment)
     __shared__ double red[256][17];
 #pragma unroll

@@ -1,6 +1,6 @@
 """Times the HBM-bound operators at the shapes of the bench step (1 line x 16 chars) with CUDA events, L2 flushed
 between launches, and prints achieved GB/s against the algorithmic bytes (minimal fp32 read + write of the operands,
-SURVEY 8d).  Usage (on the GPU box):  python tools/bench_hbm_ops.py [--iters 20]
+SURVEY 8d).  Usage (on the GPU box):  python tools/bench_hbm_ops.py [--iters 20] [--only NAME]
 """
 import argparse
 import json
@@ -31,12 +31,15 @@ def timeit(fn, iters, flush):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--only", default="", help="time only the operators whose name contains this string (e.g. 'groupnorm_stats')")
     args = ap.parse_args()
     dev = torch.device("cuda:0")
     flush = torch.empty(64 << 20, dtype=torch.float32, device=dev)
     rows = []
 
     def add(name, fn, nbytes):
+        if args.only not in name:
+            return
         us = timeit(fn, args.iters, flush)
         rows.append({"op": name, "us": round(us, 1), "MB": round(nbytes / 1e6, 1), "GB/s": round(nbytes / us / 1e3, 0)})
 
@@ -57,6 +60,14 @@ def main():
         add(f"groupnorm_stats [{n},{h},{w},{c}]", lambda: ops.groupnorm_stats(x), x.numel() * 4)
         add(f"groupnorm_apply+swish [{n},{h},{w},{c}]", lambda: ops.groupnorm_apply(x, mr, ga, be, out=y), 2 * x.numel() * 4)
         del x, y
+    # AdaIN + concat (statistics pass, then apply): 16 characters on a 512-wide line, windows 32 columns wide; bytes = prior crops and
+    # feature windows read once, the [Nc, H, wp, 2C] output written once
+    for nc, h, wp, c in ((16, 32, 32, 256), (16, 64, 64, 256)):
+        prior = torch.randn(nc, h, wp, c, device=dev)
+        feat = torch.randn(1, h, nc * wp, c, device=dev)
+        win = torch.tensor([[0, i * wp, (i + 1) * wp, 0] for i in range(nc)], dtype=torch.int32, device=dev)
+        add(f"adain_concat [{nc},{h},{wp},{c}]", lambda: ops.adain_concat(prior, feat, win, nc, wp), 4 * nc * h * wp * c * 4)
+        del prior, feat
     # ToRGB
     for n, h, c in ((16, 128, 128), (16, 64, 256), (16, 32, 512)):
         x = torch.randn(n, h, h, c, device=dev)
