@@ -477,6 +477,45 @@ typedef struct {
 int mn_prior_tiles_u8(const float* priors, long long stride_n, long long stride_c, long long stride_h, long long stride_w,
                       const mn_prior_tile* tiles, int n_rows, void* stream);
 
+/* Text regions in whole images (DESIGN.md section 7b, "Text regions in whole images").
+ * OpenCV's own 8-bit INTER_CUBIC resize (the arithmetic of mn_preprocess_lq_u8) of n images in one launch, blockIdx.y = image:
+ * images[i].dst [dh][dw][cn] = cv2.resize(src [h][w][cn], (dw, dh), INTER_CUBIC) computed at scale_x / scale_y (cv::resize's
+ * 1/fx, 1/fy: 1/s for the fx = fy = s background, 1/((double)dw/w) for the dsize form).  Pixels are addressed by row and column
+ * with 64-bit byte offsets, so a destination may exceed 2^31 bytes.  max_pixels >= every dh*dw.  images: DEVICE array of
+ * records (validated by the caller). */
+typedef struct {
+    const uint8_t* src;         /* row 0 of the source image */
+    int64_t src_pitch;          /* bytes between rows of the source image */
+    int32_t h, w;
+    uint8_t* dst;               /* row 0 of the destination image */
+    int64_t dst_pitch;          /* bytes between rows of the destination */
+    int32_t dh, dw;
+    double scale_x, scale_y;
+} mn_resize_image;
+int mn_resize_cubic_u8_batched(const mn_resize_image* images, int n, int cn, long long max_pixels, void* stream);
+
+/* The restored regions of whole images composed over their cubic backgrounds, every region of every page in one launch,
+ * blockIdx.y = region, one thread per output pixel (X, Y) of its rectangle [x0, x1) x [y0, y1) (output pixels).  P = the cubic
+ * resize (mn_resize_cubic_u8_batched's arithmetic, dsize form, split at the rectangle's width) of the region's restored bytes
+ * sr [sr_h][sr_w][3] (cv2.imwrite order; channel c of P reads channel 2 - c) onto the rectangle; a = min(1, fl((float)d + 0.5)/F),
+ * d the distance to the nearest side not on the page border (a = 1 when F = 0 or every side lies on it); then
+ *   page = sat_u8(rint_half_even(fl(fl(a*P) + fl(fl(1 - a)*page)))),   every operation rounded on its own.
+ * A pixel is written by exactly one thread: the one of the last region of its chain that contains it, which composes the
+ * background through every containing region of the chain in order.  chain: the indices (into `regions`) of every region of the
+ * same page whose rectangle meets this one, itself included, increasing.  regions: DEVICE array of records whose chains point
+ * into device memory (validated by the caller); max_pixels >= every rectangle's pixel count. */
+typedef struct {
+    uint8_t* page;              /* row 0 of the page [page_h][page_w][3], holding its background */
+    int64_t page_pitch;
+    const uint8_t* sr;          /* row 0 of the region's restored bytes */
+    int64_t sr_pitch;
+    const int32_t* chain;
+    int32_t page_h, page_w, sr_h, sr_w;
+    int32_t x0, y0, x1, y1;
+    int32_t feather, n_chain;
+} mn_region;
+int mn_composite_regions_u8(const mn_region* regions, int n, long long max_pixels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -99,6 +99,17 @@ class PriorTile(Structure):
     _fields_ = [("dst", c_void_p), ("dst_pitch", c_int64)]
 
 
+class ResizeImage(Structure):
+    _fields_ = [("src", c_void_p), ("src_pitch", c_int64), ("h", c_int32), ("w", c_int32), ("dst", c_void_p), ("dst_pitch", c_int64),
+                ("dh", c_int32), ("dw", c_int32), ("scale_x", c_double), ("scale_y", c_double)]
+
+
+class Region(Structure):
+    _fields_ = [("page", c_void_p), ("page_pitch", c_int64), ("sr", c_void_p), ("sr_pitch", c_int64), ("chain", c_void_p),
+                ("page_h", c_int32), ("page_w", c_int32), ("sr_h", c_int32), ("sr_w", c_int32),
+                ("x0", c_int32), ("y0", c_int32), ("x1", c_int32), ("y1", c_int32), ("feather", c_int32), ("n_chain", c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -148,6 +159,8 @@ SYMBOLS = {
     "mn_decode_labels": (c_int, [c_void_p, c_longlong, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
     "mn_style_lerp": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]),
     "mn_prior_tiles_u8": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_void_p, c_int, c_void_p]),
+    "mn_resize_cubic_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
+    "mn_composite_regions_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -32,9 +32,41 @@ __device__ __forceinline__ CubicTaps cubic_taps(int d, double scale) {
     return r;
 }
 
+// OpenCV's 8-bit INTER_CUBIC value of one destination element: source channel sc at the destination pixel whose taps are
+// (tx, ty), for an h x w image whose rows start `row_pitch` bytes apart.  The taps replicate the border of [0, h) x [0, w): a crop
+// passed as (pointer to its first pixel, the source image's pitch, its own size) is resized as an isolated image.  `vec`: the
+// element lies in the vector body of VResizeCubicVec_32s8u (the first floor(dw*cn/8)*8 elements of a destination row, dw*cn
+// counted in the destination's channel order), else in the fixed-point tail.  Byte offsets are 64-bit.
+__device__ __forceinline__ int cubic_u8(const uint8_t* __restrict__ img, long long row_pitch, int h, int w, int cn, int sc,
+                                        const CubicTaps& tx, const CubicTaps& ty, bool vec) {
+    int S[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int yy = min(max(ty.ofs - 1 + r, 0), h - 1);
+        int acc = 0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int xx = min(max(tx.ofs - 1 + j, 0), w - 1);
+            acc += (int)img[(long long)yy * row_pitch + (long long)xx * cn + sc] * tx.t[j];
+        }
+        S[r] = acc;
+    }
+    int v;
+    if (vec) {                                            // vector body of VResizeCubicVec_32s8u: fp32, mul then add, rows 3..0
+        const float f = 1.f / (2048.f * 2048.f);
+        float acc = __fmul_rn((float)S[3], __fmul_rn((float)ty.t[3], f));
+        acc = __fadd_rn(__fmul_rn((float)S[2], __fmul_rn((float)ty.t[2], f)), acc);
+        acc = __fadd_rn(__fmul_rn((float)S[1], __fmul_rn((float)ty.t[1], f)), acc);
+        acc = __fadd_rn(__fmul_rn((float)S[0], __fmul_rn((float)ty.t[0], f)), acc);
+        v = __float2int_rn(acc);
+    } else {                                              // scalar tail: FixedPtCast<int, uchar, 22>
+        v = (S[0] * ty.t[0] + S[1] * ty.t[1] + S[2] * ty.t[2] + S[3] * ty.t[3] + (1 << 21)) >> 22;
+    }
+    return min(max(v, 0), 255);
+}
+
 // One canvas element (idx over [out_h][out_w][cn]) of test_sr.py:98-111 for an 8-bit image whose rows start `row_pitch` bytes
-// apart.  The cubic taps replicate the border of [0, h) x [0, w): a crop passed as (pointer to its first column, the source
-// image's pitch, its own width) is resized as an isolated image, exactly what cv2.resize(img[:, a:b], ...) computes.
+// apart (cubic_u8: a crop is resized as an isolated image, exactly what cv2.resize(img[:, a:b], ...) computes).
 // Returns the resized byte (0 outside the dh x dw image); lq (fp32 canvas) and lq_u8 (resized bytes) are optional outputs.
 __device__ __forceinline__ int preprocess_lq_element(const uint8_t* __restrict__ img, long long row_pitch, int h, int w, int cn,
                                                      double scale_x, double scale_y, int dh, int dw, int idx,
@@ -44,31 +76,7 @@ __device__ __forceinline__ int preprocess_lq_element(const uint8_t* __restrict__
     const int dy = idx / (cn * out_w);
     int v = 0;                                            // the canvas is zero outside the resized image (test_sr.py:104-106)
     if (dx < dw && dy < dh) {
-        const CubicTaps tx = cubic_taps(dx, scale_x), ty = cubic_taps(dy, scale_y);
-        int S[4];
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int yy = min(max(ty.ofs - 1 + r, 0), h - 1);
-            int acc = 0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int xx = min(max(tx.ofs - 1 + j, 0), w - 1);
-                acc += (int)img[(size_t)yy * row_pitch + (size_t)xx * cn + c] * tx.t[j];
-            }
-            S[r] = acc;
-        }
-        const int e = dx * cn + c, nvec = (dw * cn / 8) * 8;
-        if (e < nvec) {                                   // vector body of VResizeCubicVec_32s8u: fp32, mul then add, rows 3..0
-            const float sc = 1.f / (2048.f * 2048.f);
-            float acc = __fmul_rn((float)S[3], __fmul_rn((float)ty.t[3], sc));
-            acc = __fadd_rn(__fmul_rn((float)S[2], __fmul_rn((float)ty.t[2], sc)), acc);
-            acc = __fadd_rn(__fmul_rn((float)S[1], __fmul_rn((float)ty.t[1], sc)), acc);
-            acc = __fadd_rn(__fmul_rn((float)S[0], __fmul_rn((float)ty.t[0], sc)), acc);
-            v = __float2int_rn(acc);
-        } else {                                          // scalar tail: FixedPtCast<int, uchar, 22>
-            v = (S[0] * ty.t[0] + S[1] * ty.t[1] + S[2] * ty.t[2] + S[3] * ty.t[3] + (1 << 21)) >> 22;
-        }
-        v = min(max(v, 0), 255);
+        v = cubic_u8(img, row_pitch, h, w, cn, c, cubic_taps(dx, scale_x), cubic_taps(dy, scale_y), dx * cn + c < (dw * cn / 8) * 8);
         if (lq_u8) lq_u8[((size_t)dy * dw + dx) * cn + c] = (uint8_t)v;
     }
     if (lq) {
@@ -207,7 +215,98 @@ __global__ void prior_tiles_kernel(const float* __restrict__ priors, long long s
     for (int c = 0; c < 3; ++c) o[c] = prior_u8(prior_value(&p, 0, c, y, x));
 }
 
+// blockIdx.y = image; one thread per destination pixel (row y, column x) of the [dh][dw][cn] resized image, those past its
+// dh*dw pixels exit.  cv2.resize(src, (dw, dh), interpolation=INTER_CUBIC), the split at the destination's width.
+__global__ void resize_cubic_batched_kernel(const mn_resize_image* __restrict__ images, int cn) {
+    mn_pdl_prologue();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const mn_resize_image im = images[blockIdx.y];
+    if (idx >= (long long)im.dh * im.dw) return;
+    const int x = (int)(idx % im.dw), y = (int)(idx / im.dw);
+    const CubicTaps tx = cubic_taps(x, im.scale_x), ty = cubic_taps(y, im.scale_y);
+    const long long nvec = ((long long)im.dw * cn / 8) * 8;
+    uint8_t* o = im.dst + (long long)y * im.dst_pitch + (long long)x * cn;
+    for (int c = 0; c < cn; ++c) o[c] = (uint8_t)cubic_u8(im.src, im.src_pitch, im.h, im.w, cn, c, tx, ty, (long long)x * cn + c < nvec);
+}
+
+__device__ __forceinline__ bool region_holds(const mn_region& r, int X, int Y) {
+    return X >= r.x0 && X < r.x1 && Y >= r.y0 && Y < r.y1;
+}
+
+// alpha of output pixel (X, Y) inside region r: the distance d to the nearest side not on the page border,
+// min(1, fl((float)d + 0.5) / F); 1 when F = 0 or every side lies on the border.
+__device__ __forceinline__ float region_alpha(const mn_region& r, int X, int Y) {
+    int d = INT_MAX;
+    if (r.x0 > 0) d = min(d, X - r.x0);
+    if (r.x1 < r.page_w) d = min(d, r.x1 - 1 - X);
+    if (r.y0 > 0) d = min(d, Y - r.y0);
+    if (r.y1 < r.page_h) d = min(d, r.y1 - 1 - Y);
+    if (r.feather == 0 || d == INT_MAX) return 1.f;
+    return fminf(1.f, __fdiv_rn(__fadd_rn((float)d, 0.5f), (float)r.feather));
+}
+
+// blockIdx.y = region; one thread per output pixel of its rectangle, those past its pixels exit.  The pixel belongs to the last
+// region of its chain (every region of the page whose rectangle meets this one, in page order) that contains it; only that
+// region's thread writes it, composing the page's background through every containing region in order:
+//   out = sat_u8(rint(fl(fl(a*P) + fl(fl(1 - a)*out)))),
+// P the cubic resize of the region's restored bytes (read through their pitch, channels flipped back) onto its rectangle, at
+// OpenCV's dsize scale 1/((double)dw/sw) per axis, the vector / tail split taken at the rectangle's width.
+__global__ void composite_regions_kernel(const mn_region* __restrict__ regions) {
+    mn_pdl_prologue();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int me = blockIdx.y;
+    const mn_region r = regions[me];
+    const int rw = r.x1 - r.x0;
+    if (idx >= (long long)rw * (r.y1 - r.y0)) return;
+    const int X = r.x0 + (int)(idx % rw), Y = r.y0 + (int)(idx / rw);
+    for (int k = r.n_chain - 1; k >= 0; --k) {
+        const int j = r.chain[k];
+        if (j == me) break;
+        if (region_holds(regions[j], X, Y)) return;                     // a later region owns the pixel
+    }
+    uint8_t* o = r.page + (long long)Y * r.page_pitch + (long long)X * 3;
+    int v[3] = {o[0], o[1], o[2]};
+    for (int k = 0; k < r.n_chain; ++k) {
+        const int j = r.chain[k];
+        const mn_region q = regions[j];
+        if (region_holds(q, X, Y)) {
+            const int dw = q.x1 - q.x0, dh = q.y1 - q.y0, dx = X - q.x0, dy = Y - q.y0;
+            const CubicTaps tx = cubic_taps(dx, __ddiv_rn(1.0, __ddiv_rn((double)dw, (double)q.sr_w)));
+            const CubicTaps ty = cubic_taps(dy, __ddiv_rn(1.0, __ddiv_rn((double)dh, (double)q.sr_h)));
+            const float a = region_alpha(q, X, Y), b = __fsub_rn(1.f, a);
+            const int nvec = (dw * 3 / 8) * 8;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const int p = cubic_u8(q.sr, q.sr_pitch, q.sr_h, q.sr_w, 3, 2 - c, tx, ty, dx * 3 + c < nvec);
+                const int t = __float2int_rn(__fadd_rn(__fmul_rn(a, (float)p), __fmul_rn(b, (float)v[c])));
+                v[c] = min(max(t, 0), 255);
+            }
+        }
+        if (j == me) break;
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = (uint8_t)v[c];
+}
+
 }  // namespace
+
+extern "C" int mn_resize_cubic_u8_batched(const mn_resize_image* images, int n, int cn, long long max_pixels, void* stream) {
+    MN_REQUIRE(images && n > 0 && n <= 65535 && cn > 0 && cn <= 4 && max_pixels > 0, "mn_resize_cubic_u8_batched: bad args");
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_resize_cubic_u8_batched: %lld pixels exceed the grid", max_pixels);
+    MN_CUDA_CHECK((mn_launch(resize_cubic_batched_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
+                             (cudaStream_t)stream, images, cn)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_composite_regions_u8(const mn_region* regions, int n, long long max_pixels, void* stream) {
+    MN_REQUIRE(regions && n > 0 && n <= 65535 && max_pixels > 0, "mn_composite_regions_u8: bad args");
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_composite_regions_u8: %lld pixels exceed the grid", max_pixels);
+    MN_CUDA_CHECK((mn_launch(composite_regions_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
+                             (cudaStream_t)stream, regions)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
 
 extern "C" int mn_preprocess_lq_u8(const uint8_t* img, int h, int w, int cn, double fx, double fy, int dh, int dw,
                                    float* lq, uint8_t* lq_u8, int out_h, int out_w, void* stream) {

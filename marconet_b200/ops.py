@@ -1164,3 +1164,85 @@ def prior_tiles(priors, tiles, first=0):
     _lib.check(_lib.load().mn_prior_tiles_u8(_ptr(priors), *priors.stride(), tiles.data_ptr() + first * isz, n, _stream()),
                "mn_prior_tiles_u8")
     LAUNCHES += 1
+
+
+# ---- text regions in whole images (DESIGN.md 7b, "Text regions in whole images") -----------------------------------------
+def _dense_u8(t, dev, cn, what):
+    """Checks a uint8 [h, w, cn] CUDA view with dense pixels (any row stride) on ``dev``."""
+    if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != cn \
+            or t.shape[0] < 1 or t.shape[1] < 1 or t.stride(2) != 1 or t.stride(1) != cn or t.stride(0) < cn * t.shape[1]:
+        raise RuntimeError(f"{what} must be a non-empty uint8 [h, w, {cn}] tensor with dense pixels on {dev}")
+
+
+def resize_cubic(items):
+    """cv2.resize(src, (dw, dh), interpolation=INTER_CUBIC) -- OpenCV's own 8-bit path, as preprocess_lq -- for many images in one
+    launch (mn_resize_cubic_u8_batched).  items: list of (src, dst), uint8 [h, w, cn] and [dh, dw, cn] CUDA views with dense
+    pixels (any row stride; dst may exceed 2^31 bytes).  The scales are the dsize form's 1/((double)dw/w) and 1/((double)dh/h);
+    for dw = s*w, dh = s*h they equal 1/s, so dst is also cv2.resize(src, (0, 0), fx=s, fy=s, interpolation=INTER_CUBIC)."""
+    global LAUNCHES
+    if not items:
+        raise ValueError("resize_cubic: no images")
+    if len(items) > 65535:
+        raise ValueError("resize_cubic: at most 65535 images per launch")
+    dev = items[0][0].device
+    cn = items[0][0].shape[2] if isinstance(items[0][0], torch.Tensor) and items[0][0].dim() == 3 else 3
+    if not 1 <= cn <= 4:
+        raise RuntimeError(f"resize_cubic: {cn} channels (1 to 4)")
+    recs, mx = [], 0
+    for i, (src, dst) in enumerate(items):
+        _dense_u8(src, dev, cn, f"resize_cubic: image {i}: src")
+        _dense_u8(dst, dev, cn, f"resize_cubic: image {i}: dst")
+        (h, w), (dh, dw) = src.shape[:2], dst.shape[:2]
+        recs.append(_lib.ResizeImage(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw,
+                                     1.0 / (dw / w), 1.0 / (dh / h)))
+        mx = max(mx, dh * dw)
+    table = _table(_lib.ResizeImage, recs, dev)
+    _lib.check(_lib.load().mn_resize_cubic_u8_batched(_ptr(table), len(recs), cn, mx, _stream()), "mn_resize_cubic_u8_batched")
+    LAUNCHES += 1
+
+
+def composite_regions(regions, feather):
+    """Restored regions composed over their pages in one launch (mn_composite_regions_u8; DESIGN.md 7b).  regions: list of
+    (page, sr, rect, chain):
+      page   uint8 [H, W, 3] CUDA view with dense pixels holding the background (written in place);
+      sr     uint8 [h, w, 3] CUDA view with dense pixels: the region's restored bytes in cv2.imwrite order, read in place;
+      rect   (x0, y0, x1, y1), the region's rectangle in page pixels, non-empty and inside the page;
+      chain  indices into ``regions`` of every region of the same page whose rectangle meets this one, itself included, increasing.
+    ``feather`` >= 0: the ramp width F in page pixels.  Inside its rectangle each region's cubic resize P of sr (channels flipped
+    back) is blended over the page with weight a = min(1, fl((float)d + 0.5)/F), d the distance to the nearest side not on the
+    page border; regions later in the list compose over earlier ones, and each pixel is written once."""
+    import numpy as np
+    global LAUNCHES
+    if not regions:
+        raise ValueError("composite_regions: no regions")
+    if len(regions) > 65535:
+        raise ValueError("composite_regions: at most 65535 regions per launch")
+    feather = int(feather)
+    if feather < 0:
+        raise ValueError(f"composite_regions: feather {feather} < 0")
+    dev = regions[0][0].device
+    n_chain = sum(len(r[3]) for r in regions)
+    isz = ctypes.sizeof(_lib.Region)
+    buf = torch.empty(len(regions) * isz + 4 * max(1, n_chain), dtype=torch.uint8, device=dev)
+    c_base = buf.data_ptr() + len(regions) * isz
+    recs, chains, mx = [], [], 0
+    for i, (page, sr, rect, chain) in enumerate(regions):
+        _dense_u8(page, dev, 3, f"composite_regions: region {i}: page")
+        _dense_u8(sr, dev, 3, f"composite_regions: region {i}: sr")
+        x0, y0, x1, y1 = (int(v) for v in rect)
+        ph, pw = page.shape[:2]
+        if not (0 <= x0 < x1 <= pw and 0 <= y0 < y1 <= ph):
+            raise ValueError(f"composite_regions: region {i}: rectangle {(x0, y0, x1, y1)} is not a non-empty part of the {ph}x{pw} page")
+        chain = [int(j) for j in chain]
+        if i not in chain or any(b <= a for a, b in zip(chain, chain[1:])) or not 0 <= chain[0] or chain[-1] >= len(regions) \
+                or any(regions[j][0].data_ptr() != page.data_ptr() for j in chain):
+            raise ValueError(f"composite_regions: region {i}: chain {chain} is not an increasing list of regions of its page "
+                             f"that holds the region itself")
+        recs.append(_lib.Region(page.data_ptr(), page.stride(0), sr.data_ptr(), sr.stride(0), c_base + 4 * len(chains), ph, pw,
+                                sr.shape[0], sr.shape[1], x0, y0, x1, y1, feather, len(chain)))
+        chains += chain
+        mx = max(mx, (x1 - x0) * (y1 - y0))
+    host = bytes((_lib.Region * len(recs))(*recs)) + np.asarray(chains or [0], dtype=np.int32).tobytes()
+    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    _lib.check(_lib.load().mn_composite_regions_u8(_ptr(buf), len(recs), mx, _stream()), "mn_composite_regions_u8")
+    LAUNCHES += 1

@@ -890,6 +890,172 @@ def interpolate_styles(encoder, tspgan, pairs, scales=tuple(i / 10 for i in rang
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# Text regions in whole images (DESIGN.md section 7b, "Text regions in whole images").  A photo, scan or screenshot with a few
+# rectangles of small text: the page is upscaled by s with OpenCV's cubic resize, each rectangle is restored as a text-line image
+# of its own (restore_images on a view of the uploaded page), its 128-row result is resized onto the rectangle's s-times output
+# and blended in with a linear ramp of F output pixels along every side that is not on the page border.
+# ---------------------------------------------------------------------------------------------------------------------
+class RegionPlan(NamedTuple):
+    """One region of restore_regions, planned on the host: region ``region`` of image ``image``, ``rect`` (x0, y0, x1, y1) in
+    source pixels, ``out`` the same rectangle in output pixels, ``overlaps`` the indices (into the plan) of the earlier regions
+    of the same image whose rectangles meet this one, and the labels and boxes restore_images gets for the crop (boxes shifted
+    by (-x0, -y0); None: predicted)."""
+    image: int
+    region: int
+    rect: tuple
+    out: tuple
+    overlaps: list
+    labels: list
+    boxes: list
+
+
+def _per_image(v, n, what):
+    v = [None] * n if v is None else list(v)
+    if len(v) != n:
+        raise ValueError(f"{what}: {len(v)} entries for {n}")
+    return v
+
+
+def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None):
+    """restore_regions' host plan, validated before any launch.  shapes: (H, W) per image; regions: per image, a list of integer
+    half-open rectangles (x0, y0, x1, y1); labels / boxes: None, or per image None or a list with one entry per region (None:
+    predicted, else the region's labels / its detector boxes [x1, y1, x2, y2] in IMAGE coordinates).  Returns the RegionPlans of
+    every region, image by image in region order.
+    Raises ValueError: scale not an integer in [1, 8], feather < 0, and, naming the image and the region, a rectangle that is
+    empty or leaves the image, a label / box count mismatch, boxes without labels, a box outside the region's columns."""
+    if isinstance(scale, bool) or not isinstance(scale, int) or not 1 <= scale <= 8:
+        raise ValueError(f"scale must be an integer in [1, 8], got {scale!r}")
+    if feather is not None and (isinstance(feather, bool) or not isinstance(feather, int) or feather < 0):
+        raise ValueError(f"feather must be an integer >= 0 output pixels, got {feather!r}")
+    n = len(shapes)
+    regions, labels, boxes = (_per_image(v, n, f"{what} (one list per image)") for v, what in
+                              ((regions, "regions"), (labels, "labels"), (boxes, "boxes")))
+    plan = []
+    for i, (H, W) in enumerate(shapes):
+        rects = list(regions[i] or [])
+        labs = _per_image(labels[i], len(rects), f"image {i}: labels (one entry per region)")
+        bxs = _per_image(boxes[i], len(rects), f"image {i}: boxes (one entry per region)")
+        first = len(plan)
+        for r, rect in enumerate(rects):
+            name = f"image {i}, region {r}"
+            try:
+                x0, y0, x1, y1 = (int(v) for v in rect)
+                if (x0, y0, x1, y1) != tuple(rect):
+                    raise ValueError
+            except (TypeError, ValueError):
+                raise ValueError(f"{name}: expected an integer rectangle (x0, y0, x1, y1), got {rect!r}") from None
+            if not (0 <= x0 < x1 <= W and 0 <= y0 < y1 <= H):
+                raise ValueError(f"{name}: rectangle {(x0, y0, x1, y1)} is empty or outside the {W}x{H} image")
+            lab, bx = labs[r], bxs[r]
+            if lab is not None:
+                lab = [int(v) for v in torch.as_tensor(lab, dtype=torch.long).reshape(-1).tolist()]
+            if bx is not None:
+                if lab is None:
+                    raise ValueError(f"{name}: boxes without labels (predicted labels pair only with predicted boxes)")
+                if len(lab) != len(bx):
+                    raise ValueError(f"{name}: {len(lab)} labels for {len(bx)} boxes")
+                for k, b in enumerate(bx):
+                    b = [float(v) for v in b]
+                    if len(b) != 4 or not x0 <= b[0] <= b[2] <= x1:
+                        raise ValueError(f"{name}, character {k}: box {b} is outside the region's columns [{x0}, {x1}]")
+                bx = [[float(b[0]) - x0, float(b[1]) - y0, float(b[2]) - x0, float(b[3]) - y0] for b in bx]
+            overlaps = [first + j for j, q in enumerate(plan[first:]) if max(x0, q.rect[0]) < min(x1, q.rect[2])
+                        and max(y0, q.rect[1]) < min(y1, q.rect[3])]
+            s = scale
+            plan.append(RegionPlan(i, r, (x0, y0, x1, y1), (s * x0, s * y0, s * x1, s * y1), overlaps, lab, bx))
+    return plan
+
+
+def region_chains(plan, ok):
+    """The chains mn_composite_regions_u8 reads: for each region k of ``ok`` (increasing indices into the plan: the regions that
+    are composed), the positions in ``ok`` of every region of ok whose rectangle meets k's, k included, in order."""
+    later = {k: [] for k in range(len(plan))}
+    for k, p in enumerate(plan):
+        for j in p.overlaps:
+            later[j].append(k)
+    index = {k: j for j, k in enumerate(ok)}
+    return [[index[j] for j in plan[k].overlaps + [k] + later[k] if j in index] for k in ok]
+
+
+def _to_host_all(tensors):
+    """Device tensors -> numpy arrays of the same shapes, through ONE pinned buffer and one synchronisation."""
+    total = sum(t.numel() for t in tensors)
+    pinned = torch.empty(max(total, 1), dtype=torch.uint8, pin_memory=True)
+    out, o = [], 0
+    for t in tensors:
+        v = pinned[o:o + t.numel()].view(t.shape)
+        v.copy_(t, non_blocking=True)
+        out.append(v)
+        o += t.numel()
+    if tensors:
+        torch.cuda.current_stream(tensors[0].device).synchronize()
+    return [v.numpy() for v in out]
+
+
+@torch.no_grad()
+def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=None, scale=4, feather=None, max_lines=8, context=16,
+                    overlap=64, whole_lines=False, skip_invalid=False, to_host=False):
+    """Restore rectangles of small text inside whole images and compose them into the images upscaled ``scale`` times
+    (DESIGN.md section 7b, "Text regions in whole images").
+
+    images: uint8 [H, W, 3] numpy arrays or CPU / CUDA tensors, in any channel order; regions: per image, a list of integer
+    rectangles (x0, y0, x1, y1), 0 <= x0 < x1 <= W, 0 <= y0 < y1 <= H, in the order they compose; labels / boxes: as
+    plan_regions takes them (boxes in image coordinates; None entries are predicted, exactly as restore_images predicts).
+    scale s: an integer in [1, 8]; feather F >= 0 output pixels (default 2 s).
+    The result of an image is out = B = cv2.resize(img, (0, 0), fx=s, fy=s, INTER_CUBIC) (OpenCV's own path), then for each region
+    that did not fail, in order, over its rectangle R = [s x0, s x1) x [s y0, s y1):
+      P = cv2.resize(T[..., ::-1], (s (x1 - x0), s (y1 - y0)), INTER_CUBIC), T = restore_images' sr_u8 of img[y0:y1, x0:x1];
+      out = sat_u8(rint(fl(fl(a P) + fl(fl(1 - a) out)))), a = min(1, fl((float)d + 0.5) / F), d the distance to the nearest
+      side of R that is not on the image border (a = 1 when F = 0 or no side counts).
+    One call: the host images go to the device in one pinned copy; restore_images runs on views of the uploaded images (every
+    region of every image shares its batches; max_lines, context, overlap, whole_lines and skip_invalid are passed on); one
+    launch computes every background (mn_resize_cubic_u8_batched) and one composes every region (mn_composite_regions_u8).
+    Returns one dict per image: image (uint8 [s H, s W, 3]) and regions, one entry per region: dict(sr_u8, segments, labels,
+    boxes) -- boxes in image coordinates, predicted ones shifted back -- or, with ``skip_invalid``, dict(error=...) for a region
+    restore_images rejected, whose rectangle keeps the background.  Results stay on the device, or come back as numpy arrays
+    through one pinned buffer and one synchronisation with ``to_host``.  plan_regions' errors are raised whatever skip_invalid."""
+    from . import ops
+    imgs = [_as_image(im, i) for i, im in enumerate(images)]
+    plan = plan_regions([im.shape[:2] for im in imgs], regions, labels, boxes, scale, feather)
+    feather = 2 * scale if feather is None else feather
+    if not imgs:
+        return []
+    dev = next(encoder.parameters()).device
+    with torch.cuda.device(dev):
+        dimg = _device_images(range(len(imgs)), imgs, dev)
+        res = restore_images(encoder, tspgan, sr, [dimg[p.image][p.rect[1]:p.rect[3], p.rect[0]:p.rect[2]] for p in plan],
+                             [p.labels for p in plan], [p.boxes for p in plan], max_lines=max_lines, context=context,
+                             skip_invalid=skip_invalid, whole_lines=whole_lines, overlap=overlap) if plan else []
+        sizes = [scale * scale * im.shape[0] * im.shape[1] * 3 for im in imgs]
+        flat = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
+        offs = [sum(sizes[:i]) for i in range(len(imgs))]
+        pages = [flat[o:o + n].view(scale * im.shape[0], scale * im.shape[1], 3) for o, n, im in zip(offs, sizes, imgs)]
+        ops.resize_cubic([(dimg[i], pages[i]) for i in range(len(imgs))])
+        ok = [k for k, r in enumerate(res) if "error" not in r]
+        if ok:
+            ops.composite_regions([(pages[plan[k].image], res[k]["sr_u8"], plan[k].out, chain)
+                                   for k, chain in zip(ok, region_chains(plan, ok))], feather)
+        srs = {k: res[k]["sr_u8"] for k in ok}
+        if to_host:
+            host = _to_host_all([flat] + list(srs.values()))
+            pages = [host[0][o:o + n].reshape(pg.shape) for o, n, pg in zip(offs, sizes, pages)]
+            srs = dict(zip(srs, host[1:]))
+    out = [dict(image=pages[i], regions=[]) for i in range(len(imgs))]
+    for k, p in enumerate(plan):
+        r = res[k]
+        if "error" in r:
+            entry = dict(error=r["error"])
+        elif "boxes" in r:
+            x0, y0 = p.rect[:2]
+            entry = dict(sr_u8=srs[k], segments=r["segments"], labels=r["labels"],
+                         boxes=[[b[0] + x0, b[1] + y0, b[2] + x0, b[3] + y0] for b in r["boxes"]])
+        else:
+            entry = dict(sr_u8=srs[k], segments=r["segments"], labels=p.labels, boxes=boxes[p.image][p.region])
+        out[p.image]["regions"].append(entry)
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # Per-layer precision plan (SURVEY.md section 8f row n4): fp16x3 / bf16x3 / fp32 and a power-of-two input scale per conv layer,
 # chosen on calibration inputs against the exact fp32 kernels.  Needed the day real checkpoints replace the synthetic ones: the
 # default fp16 hi/lo split (conv_tc2.cu) has fp32-grade mantissa but fp16's exponent range.

@@ -1,0 +1,173 @@
+"""Text regions in whole pages end to end (host uint8 in, host uint8 out, every copy inside the timed region):
+pipeline.restore_regions against the host path a user writes without it -- restore_images(to_host=True) on the regions cut out of
+the pages, then cv2's cubic resize of every page and of every restored region (IPP off) and the numpy feather blend
+(oracle/regions.py).
+
+    MN_MODULE_GRAPHS=0 python tools/bench_regions.py [--pages 8] [--lines 12] [--passes 3] [--scale 4]
+
+The pages are seeded: tools/bench_images.make_image_set lines (the reference test set's sizes and lines 2 to 4 times wider than the
+LQ canvas) pasted one under another onto a noise background, each line a region with its character boxes.  The arms alternate pass
+by pass; both must give the same bytes.  The two new kernels (mn_resize_cubic_u8_batched, mn_composite_regions_u8) are timed with
+CUDA events around their launches inside the restore_regions passes.  MN_MODULE_GRAPHS defaults to 0 here: recorded module graphs
+of 16-character crop batches outgrow an 80 GB card (DESIGN.md section 7b).  Prints one JSON line per arm and one for the kernels,
+with the card's name and power limit read in the same run.  Not part of the product path.
+"""
+import argparse
+import json
+import os
+import sys
+import time
+
+os.environ.setdefault("MN_MODULE_GRAPHS", "0")
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+
+def make_pages(n_pages, n_lines, seed=0):
+    """n_pages noise pages, each holding n_lines make_image_set lines one under another (8-pixel gaps, left margin 8 + 4k):
+    (pages, regions, labels, boxes), boxes in page coordinates."""
+    from bench_images import make_image_set
+    images, labels, boxes = make_image_set(n_pages * n_lines, seed)
+    rng = np.random.default_rng(seed + 1)
+    pages, rects, labs, bxs = [], [], [], []
+    for p in range(n_pages):
+        idx = range(p * n_lines, (p + 1) * n_lines)
+        W = max(images[i].shape[1] + 8 + 4 * (k % 8) for k, i in enumerate(idx)) + 8
+        H = sum(images[i].shape[0] + 8 for i in idx) + 8
+        page = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
+        rr, ll, bb, y = [], [], [], 8
+        for k, i in enumerate(idx):
+            h, w = images[i].shape[:2]
+            x = 8 + 4 * (k % 8)
+            page[y:y + h, x:x + w] = images[i]
+            rr.append((x, y, x + w, y + h))
+            ll.append(labels[i])
+            bb.append([[b[0] + x, b[1] + y, b[2] + x, b[3] + y] for b in boxes[i]])
+            y += h + 8
+        pages.append(page)
+        rects.append(rr)
+        labs.append(ll)
+        bxs.append(bb)
+    return pages, rects, labs, bxs
+
+
+def host_path(m, pages, rects, labels, boxes, s, feather, max_lines):
+    """restore_images on the cut-out regions, then cv2 resizes and the numpy blend on the host."""
+    import cv2
+    from marconet_b200 import pipeline
+    from oracle import regions
+    crops, labs, rel = [], [], []
+    for pg, rr, ll, bb in zip(pages, rects, labels, boxes):
+        for (x0, y0, x1, y1), lab, bx in zip(rr, ll, bb):
+            crops.append(pg[y0:y1, x0:x1])
+            labs.append(lab)
+            rel.append([[b[0] - x0, b[1] - y0, b[2] - x0, b[3] - y0] for b in bx])
+    res = pipeline.restore_images(*m, crops, labs, rel, max_lines=max_lines, to_host=True)
+    out, k = [], 0
+    for pg, rr in zip(pages, rects):
+        o = cv2.resize(pg, (0, 0), fx=s, fy=s, interpolation=cv2.INTER_CUBIC)
+        for x0, y0, x1, y1 in rr:
+            r = (s * x0, s * y0, s * x1, s * y1)
+            p = cv2.resize(np.ascontiguousarray(res[k]["sr_u8"][..., ::-1]), (r[2] - r[0], r[3] - r[1]), interpolation=cv2.INTER_CUBIC)
+            o[r[1]:r[3], r[0]:r[2]] = regions.blend(o[r[1]:r[3], r[0]:r[2]], p, regions.alpha(r, o.shape[:2], feather))
+            k += 1
+        out.append(o)
+    return out
+
+
+def _card():
+    import subprocess
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                       text=True)
+    name, _, power = q.stdout.strip().partition(", ")
+    return {"gpu": name or torch.cuda.get_device_name(0), "power_limit": power or None}
+
+
+def main():
+    import cv2
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--pages", type=int, default=8)
+    ap.add_argument("--lines", type=int, default=12)
+    ap.add_argument("--passes", type=int, default=3)
+    ap.add_argument("--scale", type=int, default=4)
+    ap.add_argument("--max-lines", type=int, default=8)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit("bench_regions.py needs a CUDA device")
+    cv2.ipp.setUseIPP(False)
+    from marconet_b200 import _lib, pipeline
+    from marconet_b200.models import networks
+    from marconet_b200.testing import synth
+    dev = torch.device("cuda:0")
+    sds = synth.make_checkpoints(0)
+    m = []
+    for key, cls in (("encoder", networks.TextContextEncoderV2), ("tspgan", networks.TSPGAN), ("sr", networks.TSPSRNet)):
+        net = cls()
+        net.load_state_dict(sds[key], strict=True)
+        m.append(net.eval().to(dev))
+    pages, rects, labels, boxes = make_pages(args.pages, args.lines)
+    s, feather = args.scale, 2 * args.scale
+
+    lib = _lib.load()
+    events = {"mn_resize_cubic_u8_batched": [], "mn_composite_regions_u8": []}
+    timing = [False]
+    for name in events:
+        fn = getattr(lib, name)
+
+        def timed(*a, _fn=fn, _name=name):
+            if not timing[0]:
+                return _fn(*a)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            rc = _fn(*a)
+            e1.record()
+            events[_name].append((e0, e1))
+            return rc
+        setattr(lib, name, timed)
+
+    def api():
+        out = pipeline.restore_regions(*m, pages, rects, labels, boxes, scale=s, feather=feather, max_lines=args.max_lines,
+                                       to_host=True)
+        return [o["image"] for o in out]
+
+    def host():
+        return host_path(m, pages, rects, labels, boxes, s, feather, args.max_lines)
+
+    arms = {"restore_regions": api, "host_path": host}
+    outs = {name: fn() for name, fn in arms.items()}                 # warm-up pass of each arm
+    same = all(np.array_equal(a, b) for a, b in zip(outs["restore_regions"], outs["host_path"]))
+    diff = max(int(np.abs(a.astype(np.int16) - b.astype(np.int16)).max()) for a, b in zip(outs["restore_regions"], outs["host_path"]))
+    times = {name: [] for name in arms}
+    for _ in range(args.passes):
+        for name, fn in arms.items():
+            timing[0] = name == "restore_regions"
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            times[name].append(time.perf_counter() - t0)
+            timing[0] = False
+    torch.cuda.synchronize()
+    card = _card()
+    out_px = sum(s * s * p.shape[0] * p.shape[1] for p in pages)
+    common = dict(pages=args.pages, lines_per_page=args.lines, scale=s, feather=feather, max_lines=args.max_lines,
+                  page_sizes=[list(p.shape[:2]) for p in pages], output_megapixels=round(out_px / 1e6, 2),
+                  module_graphs=os.environ.get("MN_MODULE_GRAPHS"), same_bytes=same, max_abs_diff=diff, **card)
+    for name, ts in times.items():
+        print(json.dumps(dict(metric="regions_e2e", arm=name, pass_s=[round(t, 4) for t in ts],
+                              pages_per_s=round(args.pages / min(ts), 3), **common)), flush=True)
+    kern = {name: [e0.elapsed_time(e1) for e0, e1 in ev] for name, ev in events.items()}
+    print(json.dumps(dict(metric="regions_kernels", **{f"{k}_ms": [round(v, 4) for v in vs] for k, vs in kern.items()},
+                          background_gbytes_per_s=round(3 * out_px / (min(kern["mn_resize_cubic_u8_batched"]) * 1e-3) / 1e9, 1),
+                          **common)), flush=True)
+    if not same:
+        sys.exit("the arms' bytes differ")
+
+
+if __name__ == "__main__":
+    main()
