@@ -516,6 +516,47 @@ typedef struct {
 } mn_region;
 int mn_composite_regions_u8(const mn_region* regions, int n, long long max_pixels, void* stream);
 
+/* Oriented text regions (DESIGN.md section 7b, "Oriented text regions").
+ * cv2.warpAffine(src, M, (dw, dh), INTER_CUBIC | WARP_INVERSE_MAP, BORDER_REPLICATE), OpenCV's own 8-bit path (IPP off), of n
+ * images in one launch, blockIdx.y = image, one thread per destination pixel.  m = M row by row: destination pixel (x, y) ->
+ * source pixel (m[0] x + m[1] y + m[2], m[3] x + m[4] y + m[5]).  OpenCV's fixed-point coordinates in 1/32 pixel,
+ * Xq = (cvRound(fl(fl(m[1] y) + m[2]) * 1024) + 16 + cvRound(fl(m[0] x) * 1024)) >> 5 (fp64, no contraction), then remap's
+ * 2-D cubic table (fp32 interpolateCubic at i/32, rint(fl(vy vx) 32768) saturated to int16, the sum's excess moved onto the
+ * taps at rows and columns 2..3), the 16 taps with replicated borders and (sum + 2^14) >> 15 saturated.  cv2 keeps the integer
+ * source coordinates as int16; with h, w <= 32767 that saturation changes no value, and callers keep every
+ * |fixed-point coordinate| below 2^30.  Byte offsets are 64-bit.  max_pixels >= every dh*dw.  images: DEVICE array of records
+ * (validated by the caller). */
+typedef struct {
+    const uint8_t* src;         /* row 0 of the source image */
+    int64_t src_pitch;
+    int32_t h, w;
+    uint8_t* dst;               /* row 0 of the destination image */
+    int64_t dst_pitch;
+    int32_t dh, dw;
+    double m[6];
+} mn_warp_image;
+int mn_warp_affine_u8_batched(const mn_warp_image* images, int n, int cn, long long max_pixels, void* stream);
+
+/* mn_composite_regions_u8 for pages that hold oriented regions: every region of every page in one launch, blockIdx.y = region,
+ * one thread per output pixel of r's rectangle [x0, x1) x [y0, y1).  kind MN_REGION_RECT: r is an mn_region record, composed
+ * exactly as mn_composite_regions_u8 composes it (the same device functions).  kind MN_REGION_AFFINE: r's rectangle is the
+ * bounding box of the region's footprint; n maps page pixel (X, Y) to pixel indices of the restored bytes T = sr [sr_h][sr_w][3]
+ * (cv2.imwrite order), (Xq, Yq) are mn_warp_affine_u8_batched's fixed-point coordinates of (X, Y) under n, and the pixel
+ * belongs to the region iff -16 <= Xq < 32 sr_w - 16 and -16 <= Yq < 32 sr_h - 16.  There
+ *   P = mn_warp_affine_u8_batched's value of T[..., ::-1] at (Xq, Yq),
+ *   u = (Xq + 16)/32, v = (Yq + 16)/32,  a = min(1, fl(min(fl(kx min(u, sr_w - u)), fl(ky min(v, sr_h - v))) / F)), 1 when F = 0,
+ * and the blend and the owner rule are mn_composite_regions_u8's; chains index this array. */
+#define MN_REGION_RECT 0
+#define MN_REGION_AFFINE 1
+typedef struct {
+    mn_region r;
+    int32_t kind;
+    float kx, ky;               /* feather slopes of an affine region, output pixels per T pixel across its sides */
+    int32_t pad;
+    double n[6];                /* affine region: page pixel -> T pixel, row by row */
+} mn_region_affine;
+int mn_composite_regions_affine_u8(const mn_region_affine* regions, int n, long long max_pixels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -110,6 +110,18 @@ class Region(Structure):
                 ("x0", c_int32), ("y0", c_int32), ("x1", c_int32), ("y1", c_int32), ("feather", c_int32), ("n_chain", c_int32)]
 
 
+class WarpImage(Structure):
+    _fields_ = [("src", c_void_p), ("src_pitch", c_int64), ("h", c_int32), ("w", c_int32), ("dst", c_void_p), ("dst_pitch", c_int64),
+                ("dh", c_int32), ("dw", c_int32), ("m", c_double * 6)]
+
+
+REGION_RECT, REGION_AFFINE = 0, 1
+
+
+class RegionAffine(Structure):
+    _fields_ = [("r", Region), ("kind", c_int32), ("kx", c_float), ("ky", c_float), ("pad", c_int32), ("n", c_double * 6)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -161,6 +173,8 @@ SYMBOLS = {
     "mn_prior_tiles_u8": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_void_p, c_int, c_void_p]),
     "mn_resize_cubic_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
     "mn_composite_regions_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
+    "mn_warp_affine_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
+    "mn_composite_regions_affine_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

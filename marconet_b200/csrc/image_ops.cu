@@ -13,18 +13,23 @@ namespace {
 
 struct CubicTaps { int ofs; int t[4]; };
 
+// OpenCV's interpolateCubic (A = -0.75) at fraction f, every fp32 operation rounded on its own.
+__device__ __forceinline__ void cubic_coeffs(float f, float c[4]) {
+    const float A = -0.75f;
+    const float xp1 = __fadd_rn(f, 1.f), omx = __fsub_rn(1.f, f);
+    c[0] = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(A, xp1), 5.f * A), xp1), 8.f * A), xp1), 4.f * A);
+    c[1] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A + 2.f, f), A + 3.f), f), f), 1.f);
+    c[2] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A + 2.f, omx), A + 3.f), omx), omx), 1.f);
+    c[3] = __fsub_rn(__fsub_rn(__fsub_rn(1.f, c[0]), c[1]), c[2]);
+}
+
 __device__ __forceinline__ CubicTaps cubic_taps(int d, double scale) {
     // fx = (float)((dx+0.5)*scale_x - 0.5); sx = cvFloor(fx); fx -= sx;  ialpha = saturate_cast<short>(coeff * 2048)
     float f = __double2float_rn(__dsub_rn(__dmul_rn((double)d + 0.5, scale), 0.5));
     const int s = (int)floorf(f);
     f = __fsub_rn(f, (float)s);
-    const float A = -0.75f;
-    const float xp1 = __fadd_rn(f, 1.f), omx = __fsub_rn(1.f, f);
     float c[4];
-    c[0] = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(A, xp1), 5.f * A), xp1), 8.f * A), xp1), 4.f * A);
-    c[1] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A + 2.f, f), A + 3.f), f), f), 1.f);
-    c[2] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A + 2.f, omx), A + 3.f), omx), omx), 1.f);
-    c[3] = __fsub_rn(__fsub_rn(__fsub_rn(1.f, c[0]), c[1]), c[2]);
+    cubic_coeffs(f, c);
     CubicTaps r;
     r.ofs = s;
 #pragma unroll
@@ -245,47 +250,165 @@ __device__ __forceinline__ float region_alpha(const mn_region& r, int X, int Y) 
     return fminf(1.f, __fdiv_rn(__fadd_rn((float)d, 0.5f), (float)r.feather));
 }
 
-// blockIdx.y = region; one thread per output pixel of its rectangle, those past its pixels exit.  The pixel belongs to the last
-// region of its chain (every region of the page whose rectangle meets this one, in page order) that contains it; only that
-// region's thread writes it, composing the page's background through every containing region in order:
-//   out = sat_u8(rint(fl(fl(a*P) + fl(fl(1 - a)*out)))),
-// P the cubic resize of the region's restored bytes (read through their pitch, channels flipped back) onto its rectangle, at
-// OpenCV's dsize scale 1/((double)dw/sw) per axis, the vector / tail split taken at the rectangle's width.
-__global__ void composite_regions_kernel(const mn_region* __restrict__ regions) {
-    mn_pdl_prologue();
+// P of rectangle q at output pixel (X, Y) blended over v: the cubic resize of the region's restored bytes (read through their
+// pitch, channels flipped back) onto its rectangle, at OpenCV's dsize scale 1/((double)dw/sw) per axis, the vector / tail split
+// taken at the rectangle's width;  v = sat_u8(rint(fl(fl(a*P) + fl(fl(1 - a)*v)))).
+__device__ __forceinline__ void region_blend(const mn_region& q, int X, int Y, int v[3]) {
+    const int dw = q.x1 - q.x0, dh = q.y1 - q.y0, dx = X - q.x0, dy = Y - q.y0;
+    const CubicTaps tx = cubic_taps(dx, __ddiv_rn(1.0, __ddiv_rn((double)dw, (double)q.sr_w)));
+    const CubicTaps ty = cubic_taps(dy, __ddiv_rn(1.0, __ddiv_rn((double)dh, (double)q.sr_h)));
+    const float a = region_alpha(q, X, Y), b = __fsub_rn(1.f, a);
+    const int nvec = (dw * 3 / 8) * 8;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const int p = cubic_u8(q.sr, q.sr_pitch, q.sr_h, q.sr_w, 3, 2 - c, tx, ty, dx * 3 + c < nvec);
+        const int t = __float2int_rn(__fadd_rn(__fmul_rn(a, (float)p), __fmul_rn(b, (float)v[c])));
+        v[c] = min(max(t, 0), 255);
+    }
+}
+
+// cv2.warpAffine's fixed-point source coordinates of destination pixel (x, y) under m (WARP_INVERSE_MAP), in 1/32 pixel:
+// X0 = cvRound(fl(fl(m1 y) + m2) * 1024) + 16 (the row's start, round_delta = 1024/32/2), adelta = cvRound(fl(m0 x) * 1024),
+// Xq = (X0 + adelta) >> 5; the source pixel is Xq >> 5 and the fraction Xq & 31.  Callers keep |fixed-point values| < 2^30.
+struct WarpCoord { int xq, yq; };
+__device__ __forceinline__ WarpCoord warp_coord(const double* m, int x, int y) {
+    const double xd = (double)x, yd = (double)y;
+    const int x0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[1], yd), m[2]), 1024.0)) + 16;
+    const int y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[4], yd), m[5]), 1024.0)) + 16;
+    const int ad = __double2int_rn(__dmul_rn(__dmul_rn(m[0], xd), 1024.0));
+    const int bd = __double2int_rn(__dmul_rn(__dmul_rn(m[3], xd), 1024.0));
+    return {(x0 + ad) >> 5, (y0 + bd) >> 5};
+}
+
+// remap's 8-bit INTER_CUBIC value at fixed-point source coordinates c with BORDER_REPLICATE: source channel sc of the h x w
+// image whose rows start row_pitch bytes apart.  The 2-D taps are initInterTab2D's: w = saturate_cast<short>(fl(vy vx) * 32768)
+// of the fp32 interpolateCubic weights at (Yq & 31)/32 and (Xq & 31)/32; a sum other than 32768 is corrected on the smallest
+// (too large) or largest (too small) tap among rows and columns 2..3, the first found in row-major order (OpenCV searches from
+// ksize/2).  Then (sum + 2^14) >> 15 saturated.  Integer sums, so the tap order is free.
+__device__ __forceinline__ void warp_taps(const WarpCoord& c, int w[16]) {
+    float cy[4], cx[4];
+    cubic_coeffs(__fmul_rn((float)(c.yq & 31), 1.f / 32.f), cy);
+    cubic_coeffs(__fmul_rn((float)(c.xq & 31), 1.f / 32.f), cx);
+    int isum = 0;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+        w[k] = min(max(__float2int_rn(__fmul_rn(__fmul_rn(cy[k >> 2], cx[k & 3]), 32768.f)), -32768), 32767);
+        isum += w[k];
+    }
+    const int diff = isum - 32768;
+    int mk = 10, Mk = 10, mv = w[10], Mv = w[10];         // from tap (2, 2) over (2, 3), (3, 2), (3, 3)
+#pragma unroll
+    for (int k = 11; k < 16; k += (k == 11) ? 3 : 1) {
+        if (w[k] < mv) mv = w[k], mk = k;
+        else if (w[k] > Mv) Mv = w[k], Mk = k;
+    }
+    const int fix = diff < 0 ? Mk : mk;
+#pragma unroll
+    for (int k = 10; k < 16; ++k) w[k] -= (diff != 0 && k == fix) ? diff : 0;
+}
+
+__device__ __forceinline__ int warp_cubic_u8(const uint8_t* __restrict__ img, long long row_pitch, int h, int w, int cn, int sc,
+                                             const WarpCoord& c, const int wt[16]) {
+    const int ix = c.xq >> 5, iy = c.yq >> 5;
+    int acc = 0;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const uint8_t* row = img + (long long)min(max(iy - 1 + r, 0), h - 1) * row_pitch + sc;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc += (int)row[(long long)min(max(ix - 1 + j, 0), w - 1) * cn] * wt[4 * r + j];
+    }
+    return min(max((acc + (1 << 14)) >> 15, 0), 255);
+}
+
+__device__ __forceinline__ bool footprint_holds(const mn_region_affine& q, const WarpCoord& c) {
+    return c.xq >= -16 && c.xq < 32 * q.r.sr_w - 16 && c.yq >= -16 && c.yq < 32 * q.r.sr_h - 16;
+}
+
+__device__ __forceinline__ bool region_holds(const mn_region_affine& q, int X, int Y) {
+    if (!region_holds(q.r, X, Y)) return false;
+    return q.kind == MN_REGION_RECT || footprint_holds(q, warp_coord(q.n, X, Y));
+}
+
+__device__ __forceinline__ void region_blend(const mn_region_affine& q, int X, int Y, int v[3]) {
+    if (q.kind == MN_REGION_RECT) {
+        region_blend(q.r, X, Y, v);
+        return;
+    }
+    const WarpCoord wc = warp_coord(q.n, X, Y);
+    float a = 1.f;
+    if (q.r.feather != 0) {
+        const float u = __fmul_rn((float)(wc.xq + 16), 1.f / 32.f), t = __fmul_rn((float)(wc.yq + 16), 1.f / 32.f);
+        const float du = __fmul_rn(q.kx, fminf(u, __fsub_rn((float)q.r.sr_w, u)));
+        const float dv = __fmul_rn(q.ky, fminf(t, __fsub_rn((float)q.r.sr_h, t)));
+        a = fminf(1.f, __fdiv_rn(fminf(du, dv), (float)q.r.feather));
+    }
+    const float b = __fsub_rn(1.f, a);
+    int wt[16];
+    warp_taps(wc, wt);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const int p = warp_cubic_u8(q.r.sr, q.r.sr_pitch, q.r.sr_h, q.r.sr_w, 3, 2 - c, wc, wt);
+        const int t = __float2int_rn(__fadd_rn(__fmul_rn(a, (float)p), __fmul_rn(b, (float)v[c])));
+        v[c] = min(max(t, 0), 255);
+    }
+}
+
+__device__ __forceinline__ const mn_region& rect_of(const mn_region& r) { return r; }
+__device__ __forceinline__ const mn_region& rect_of(const mn_region_affine& r) { return r.r; }
+
+// blockIdx.y = region; one thread per output pixel of its rectangle, those past its pixels (or outside its footprint) exit.  The
+// pixel belongs to the last region of its chain (every region of the page whose rectangle meets this one, in page order) that
+// holds it; only that region's thread writes it, composing the page's background through every region of the chain that holds
+// it, in order (region_blend).
+template <class Region>
+__device__ __forceinline__ void composite_pixel(const Region* __restrict__ regions) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const int me = blockIdx.y;
-    const mn_region r = regions[me];
-    const int rw = r.x1 - r.x0;
-    if (idx >= (long long)rw * (r.y1 - r.y0)) return;
-    const int X = r.x0 + (int)(idx % rw), Y = r.y0 + (int)(idx / rw);
-    for (int k = r.n_chain - 1; k >= 0; --k) {
-        const int j = r.chain[k];
+    const Region r = regions[me];
+    const mn_region& rr = rect_of(r);
+    const int rw = rr.x1 - rr.x0;
+    if (idx >= (long long)rw * (rr.y1 - rr.y0)) return;
+    const int X = rr.x0 + (int)(idx % rw), Y = rr.y0 + (int)(idx / rw);
+    if (!region_holds(r, X, Y)) return;
+    for (int k = rr.n_chain - 1; k >= 0; --k) {
+        const int j = rr.chain[k];
         if (j == me) break;
         if (region_holds(regions[j], X, Y)) return;                     // a later region owns the pixel
     }
-    uint8_t* o = r.page + (long long)Y * r.page_pitch + (long long)X * 3;
+    uint8_t* o = rr.page + (long long)Y * rr.page_pitch + (long long)X * 3;
     int v[3] = {o[0], o[1], o[2]};
-    for (int k = 0; k < r.n_chain; ++k) {
-        const int j = r.chain[k];
-        const mn_region q = regions[j];
-        if (region_holds(q, X, Y)) {
-            const int dw = q.x1 - q.x0, dh = q.y1 - q.y0, dx = X - q.x0, dy = Y - q.y0;
-            const CubicTaps tx = cubic_taps(dx, __ddiv_rn(1.0, __ddiv_rn((double)dw, (double)q.sr_w)));
-            const CubicTaps ty = cubic_taps(dy, __ddiv_rn(1.0, __ddiv_rn((double)dh, (double)q.sr_h)));
-            const float a = region_alpha(q, X, Y), b = __fsub_rn(1.f, a);
-            const int nvec = (dw * 3 / 8) * 8;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const int p = cubic_u8(q.sr, q.sr_pitch, q.sr_h, q.sr_w, 3, 2 - c, tx, ty, dx * 3 + c < nvec);
-                const int t = __float2int_rn(__fadd_rn(__fmul_rn(a, (float)p), __fmul_rn(b, (float)v[c])));
-                v[c] = min(max(t, 0), 255);
-            }
-        }
+    for (int k = 0; k < rr.n_chain; ++k) {
+        const int j = rr.chain[k];
+        const Region q = regions[j];
+        if (region_holds(q, X, Y)) region_blend(q, X, Y, v);
         if (j == me) break;
     }
 #pragma unroll
     for (int c = 0; c < 3; ++c) o[c] = (uint8_t)v[c];
+}
+
+__global__ void composite_regions_kernel(const mn_region* __restrict__ regions) {
+    mn_pdl_prologue();
+    composite_pixel(regions);
+}
+
+__global__ void composite_regions_affine_kernel(const mn_region_affine* __restrict__ regions) {
+    mn_pdl_prologue();
+    composite_pixel(regions);
+}
+
+// blockIdx.y = image; one thread per destination pixel of its [dh][dw][cn] image, those past its dh*dw pixels exit.
+__global__ void warp_affine_batched_kernel(const mn_warp_image* __restrict__ images, int cn) {
+    mn_pdl_prologue();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const mn_warp_image im = images[blockIdx.y];
+    if (idx >= (long long)im.dh * im.dw) return;
+    const int x = (int)(idx % im.dw), y = (int)(idx / im.dw);
+    const WarpCoord wc = warp_coord(im.m, x, y);
+    int wt[16];
+    warp_taps(wc, wt);
+    uint8_t* o = im.dst + (long long)y * im.dst_pitch + (long long)x * cn;
+    for (int c = 0; c < cn; ++c) o[c] = (uint8_t)warp_cubic_u8(im.src, im.src_pitch, im.h, im.w, cn, c, wc, wt);
 }
 
 }  // namespace
@@ -303,6 +426,24 @@ extern "C" int mn_composite_regions_u8(const mn_region* regions, int n, long lon
     MN_REQUIRE(regions && n > 0 && n <= 65535 && max_pixels > 0, "mn_composite_regions_u8: bad args");
     MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_composite_regions_u8: %lld pixels exceed the grid", max_pixels);
     MN_CUDA_CHECK((mn_launch(composite_regions_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
+                             (cudaStream_t)stream, regions)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_warp_affine_u8_batched(const mn_warp_image* images, int n, int cn, long long max_pixels, void* stream) {
+    MN_REQUIRE(images && n > 0 && n <= 65535 && cn > 0 && cn <= 4 && max_pixels > 0, "mn_warp_affine_u8_batched: bad args");
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_warp_affine_u8_batched: %lld pixels exceed the grid", max_pixels);
+    MN_CUDA_CHECK((mn_launch(warp_affine_batched_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
+                             (cudaStream_t)stream, images, cn)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_composite_regions_affine_u8(const mn_region_affine* regions, int n, long long max_pixels, void* stream) {
+    MN_REQUIRE(regions && n > 0 && n <= 65535 && max_pixels > 0, "mn_composite_regions_affine_u8: bad args");
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_composite_regions_affine_u8: %lld pixels exceed the grid", max_pixels);
+    MN_CUDA_CHECK((mn_launch(composite_regions_affine_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
                              (cudaStream_t)stream, regions)));
     MN_LAUNCH_CHECK();
     return MN_OK;

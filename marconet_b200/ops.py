@@ -1201,6 +1201,46 @@ def resize_cubic(items):
     LAUNCHES += 1
 
 
+def _region_records(regions, feather, what, record):
+    """Validated mn_region records of composite_regions' (page, sr, rect, chain, ...) tuples, their chains, the largest rectangle's
+    pixel count and a device buffer for the ``record``-type table followed by the chains."""
+    if not regions:
+        raise ValueError(f"{what}: no regions")
+    if len(regions) > 65535:
+        raise ValueError(f"{what}: at most 65535 regions per launch")
+    if feather < 0:
+        raise ValueError(f"{what}: feather {feather} < 0")
+    dev = regions[0][0].device
+    n_chain = sum(len(r[3]) for r in regions)
+    isz = ctypes.sizeof(record)
+    buf = torch.empty(len(regions) * isz + 4 * max(1, n_chain), dtype=torch.uint8, device=dev)
+    c_base = buf.data_ptr() + len(regions) * isz
+    recs, chains, mx = [], [], 0
+    for i, (page, sr, rect, chain) in enumerate(r[:4] for r in regions):
+        _dense_u8(page, dev, 3, f"{what}: region {i}: page")
+        _dense_u8(sr, dev, 3, f"{what}: region {i}: sr")
+        x0, y0, x1, y1 = (int(v) for v in rect)
+        ph, pw = page.shape[:2]
+        if not (0 <= x0 < x1 <= pw and 0 <= y0 < y1 <= ph):
+            raise ValueError(f"{what}: region {i}: rectangle {(x0, y0, x1, y1)} is not a non-empty part of the {ph}x{pw} page")
+        chain = [int(j) for j in chain]
+        if i not in chain or any(b <= a for a, b in zip(chain, chain[1:])) or not 0 <= chain[0] or chain[-1] >= len(regions) \
+                or any(regions[j][0].data_ptr() != page.data_ptr() for j in chain):
+            raise ValueError(f"{what}: region {i}: chain {chain} is not an increasing list of regions of its page "
+                             f"that holds the region itself")
+        recs.append(_lib.Region(page.data_ptr(), page.stride(0), sr.data_ptr(), sr.stride(0), c_base + 4 * len(chains), ph, pw,
+                                sr.shape[0], sr.shape[1], x0, y0, x1, y1, feather, len(chain)))
+        chains += chain
+        mx = max(mx, (x1 - x0) * (y1 - y0))
+    return recs, chains, mx, buf
+
+
+def _upload_records(buf, recs, chains):
+    import numpy as np
+    host = bytes((type(recs[0]) * len(recs))(*recs)) + np.asarray(chains or [0], dtype=np.int32).tobytes()
+    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+
+
 def composite_regions(regions, feather):
     """Restored regions composed over their pages in one launch (mn_composite_regions_u8; DESIGN.md 7b).  regions: list of
     (page, sr, rect, chain):
@@ -1211,38 +1251,65 @@ def composite_regions(regions, feather):
     ``feather`` >= 0: the ramp width F in page pixels.  Inside its rectangle each region's cubic resize P of sr (channels flipped
     back) is blended over the page with weight a = min(1, fl((float)d + 0.5)/F), d the distance to the nearest side not on the
     page border; regions later in the list compose over earlier ones, and each pixel is written once."""
-    import numpy as np
     global LAUNCHES
-    if not regions:
-        raise ValueError("composite_regions: no regions")
-    if len(regions) > 65535:
-        raise ValueError("composite_regions: at most 65535 regions per launch")
-    feather = int(feather)
-    if feather < 0:
-        raise ValueError(f"composite_regions: feather {feather} < 0")
-    dev = regions[0][0].device
-    n_chain = sum(len(r[3]) for r in regions)
-    isz = ctypes.sizeof(_lib.Region)
-    buf = torch.empty(len(regions) * isz + 4 * max(1, n_chain), dtype=torch.uint8, device=dev)
-    c_base = buf.data_ptr() + len(regions) * isz
-    recs, chains, mx = [], [], 0
-    for i, (page, sr, rect, chain) in enumerate(regions):
-        _dense_u8(page, dev, 3, f"composite_regions: region {i}: page")
-        _dense_u8(sr, dev, 3, f"composite_regions: region {i}: sr")
-        x0, y0, x1, y1 = (int(v) for v in rect)
-        ph, pw = page.shape[:2]
-        if not (0 <= x0 < x1 <= pw and 0 <= y0 < y1 <= ph):
-            raise ValueError(f"composite_regions: region {i}: rectangle {(x0, y0, x1, y1)} is not a non-empty part of the {ph}x{pw} page")
-        chain = [int(j) for j in chain]
-        if i not in chain or any(b <= a for a, b in zip(chain, chain[1:])) or not 0 <= chain[0] or chain[-1] >= len(regions) \
-                or any(regions[j][0].data_ptr() != page.data_ptr() for j in chain):
-            raise ValueError(f"composite_regions: region {i}: chain {chain} is not an increasing list of regions of its page "
-                             f"that holds the region itself")
-        recs.append(_lib.Region(page.data_ptr(), page.stride(0), sr.data_ptr(), sr.stride(0), c_base + 4 * len(chains), ph, pw,
-                                sr.shape[0], sr.shape[1], x0, y0, x1, y1, feather, len(chain)))
-        chains += chain
-        mx = max(mx, (x1 - x0) * (y1 - y0))
-    host = bytes((_lib.Region * len(recs))(*recs)) + np.asarray(chains or [0], dtype=np.int32).tobytes()
-    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    recs, chains, mx, buf = _region_records(regions, int(feather), "composite_regions", _lib.Region)
+    _upload_records(buf, recs, chains)
     _lib.check(_lib.load().mn_composite_regions_u8(_ptr(buf), len(recs), mx, _stream()), "mn_composite_regions_u8")
+    LAUNCHES += 1
+
+
+def warp_affine(items):
+    """cv2.warpAffine(src, M, (dw, dh), flags=INTER_CUBIC | WARP_INVERSE_MAP, borderMode=BORDER_REPLICATE) -- OpenCV's own 8-bit
+    path (IPP off) -- for many images in one launch (mn_warp_affine_u8_batched; DESIGN.md 7b, "Oriented text regions").  items:
+    list of (src, dst, M): uint8 [h, w, cn] and [dh, dw, cn] CUDA views with dense pixels (any row stride), h, w <= 32767, and M
+    a 2 x 3 map from dst pixel indices to src pixel indices whose fixed-point coordinates over dst stay below 2^30 / 1024 pixels
+    in magnitude (pipeline.oriented_maps keeps them so)."""
+    global LAUNCHES
+    if not items:
+        raise ValueError("warp_affine: no images")
+    if len(items) > 65535:
+        raise ValueError("warp_affine: at most 65535 images per launch")
+    dev = items[0][0].device
+    cn = items[0][0].shape[2] if isinstance(items[0][0], torch.Tensor) and items[0][0].dim() == 3 else 3
+    if not 1 <= cn <= 4:
+        raise RuntimeError(f"warp_affine: {cn} channels (1 to 4)")
+    recs, mx = [], 0
+    for i, (src, dst, m) in enumerate(items):
+        _dense_u8(src, dev, cn, f"warp_affine: image {i}: src")
+        _dense_u8(dst, dev, cn, f"warp_affine: image {i}: dst")
+        (h, w), (dh, dw) = src.shape[:2], dst.shape[:2]
+        if max(h, w) > 32767:
+            raise ValueError(f"warp_affine: image {i}: a {h}x{w} source exceeds OpenCV's int16 source coordinates")
+        m = [float(v) for row in m for v in row]
+        if len(m) != 6:
+            raise ValueError(f"warp_affine: image {i}: M must be 2 x 3")
+        recs.append(_lib.WarpImage(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw, (ctypes.c_double * 6)(*m)))
+        mx = max(mx, dh * dw)
+    table = _table(_lib.WarpImage, recs, dev)
+    _lib.check(_lib.load().mn_warp_affine_u8_batched(_ptr(table), len(recs), cn, mx, _stream()), "mn_warp_affine_u8_batched")
+    LAUNCHES += 1
+
+
+def composite_regions_affine(regions, feather):
+    """composite_regions for pages that hold oriented regions (mn_composite_regions_affine_u8; DESIGN.md 7b, "Oriented text
+    regions"), one launch.  regions: list of (page, sr, rect, chain, maps) as composite_regions takes them, maps None for a
+    rectangle (composed exactly as composite_regions composes it) or (N, kx, ky) for an oriented region: N (2 x 3, fp64) maps page
+    pixels to sr's pixel indices, kx, ky its fp32 feather slopes, and rect is the bounding box of its footprint in page pixels
+    (pipeline.oriented_maps).  A page pixel belongs to an oriented region where its fixed-point sr coordinates fall in
+    [-1/2, w - 1/2) x [-1/2, h - 1/2)."""
+    global LAUNCHES
+    recs, chains, mx, buf = _region_records(regions, int(feather), "composite_regions_affine", _lib.RegionAffine)
+    out = []
+    for i, (r, rec) in enumerate(zip(regions, recs)):
+        maps = r[4]
+        if maps is None:
+            out.append(_lib.RegionAffine(rec, _lib.REGION_RECT, 0.0, 0.0, 0, (ctypes.c_double * 6)()))
+            continue
+        n, kx, ky = maps
+        n = [float(v) for row in n for v in row]
+        if len(n) != 6 or not (kx > 0 and ky > 0):
+            raise ValueError(f"composite_regions_affine: region {i}: expected (N 2 x 3, kx > 0, ky > 0)")
+        out.append(_lib.RegionAffine(rec, _lib.REGION_AFFINE, kx, ky, 0, (ctypes.c_double * 6)(*n)))
+    _upload_records(buf, out, chains)
+    _lib.check(_lib.load().mn_composite_regions_affine_u8(_ptr(buf), len(out), mx, _stream()), "mn_composite_regions_affine_u8")
     LAUNCHES += 1

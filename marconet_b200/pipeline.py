@@ -7,6 +7,7 @@ boxes converted from the encoder's (left, right) pairs to (centre, half-width) e
 predict_characters decodes them, and the boxes, on the device (mn_decode_predictions) for images of any width.  Everything
 numeric runs through the module API (and therefore through the CUDA kernels).
 """
+import math
 import threading
 from typing import NamedTuple
 
@@ -899,7 +900,10 @@ class RegionPlan(NamedTuple):
     """One region of restore_regions, planned on the host: region ``region`` of image ``image``, ``rect`` (x0, y0, x1, y1) in
     source pixels, ``out`` the same rectangle in output pixels, ``overlaps`` the indices (into the plan) of the earlier regions
     of the same image whose rectangles meet this one, and the labels and boxes restore_images gets for the crop (boxes shifted
-    by (-x0, -y0); None: predicted)."""
+    by (-x0, -y0); None: predicted).  An oriented region (DESIGN.md 7b, "Oriented text regions") also has ``oriented`` (the
+    OrientedRegion), ``matrix`` (M, its rectified crop's map) and ``size`` ((w_r, h_r), the crop's size); its ``rect`` is the
+    bounding box of its corners in source pixels clipped to the image, ``out`` the bounding box of its footprint in output pixels,
+    ``overlaps`` compares the ``out`` boxes, and its boxes are in the crop's frame, unshifted."""
     image: int
     region: int
     rect: tuple
@@ -907,6 +911,121 @@ class RegionPlan(NamedTuple):
     overlaps: list
     labels: list
     boxes: list
+    oriented: tuple = None
+    matrix: object = None
+    size: tuple = None
+
+
+class OrientedRegion(NamedTuple):
+    """A text line as a parallelogram (DESIGN.md 7b, "Oriented text regions"): its top-left, top-right and bottom-left corners as
+    it is read, (x, y) points in continuous image coordinates (pixel (i, j) covers [j, j+1) x [i, i+1)).  e = tr - tl runs along
+    the line and f = bl - tl down it.  The rectangle (x0, y0, x1, y1) is OrientedRegion((x0, y0), (x1, y0), (x0, y1))."""
+    tl: tuple
+    tr: tuple
+    bl: tuple
+
+    @classmethod
+    def from_rotated(cls, cx, cy, w, h, angle):
+        """The w x h line centred at (cx, cy), turned ``angle`` degrees counter-clockwise as seen on screen (y points down):
+        e = w (cos a, -sin a), f = h (sin a, cos a), tl = c - e/2 - f/2."""
+        a = math.radians(angle)
+        ex, ey, fx, fy = w * math.cos(a), -w * math.sin(a), h * math.sin(a), h * math.cos(a)
+        tlx, tly = cx - ex / 2 - fx / 2, cy - ey / 2 - fy / 2
+        return cls((tlx, tly), (tlx + ex, tly + ey), (tlx + fx, tly + fy))
+
+
+class OrientedMaps(NamedTuple):
+    """oriented_maps' result: ``matrix`` M (fp64 [2, 3]: rectified crop pixel indices -> image pixel indices), ``size``
+    (w_r, h_r), ``page_map`` N (fp64 [2, 3]: output page pixel indices -> pixel indices of the restored line T), ``kx`` and
+    ``ky`` (the feather slopes, fp32 values) and ``t_width`` (W_T)."""
+    matrix: object
+    size: tuple
+    page_map: object
+    kx: float
+    ky: float
+    t_width: int
+
+
+def oriented_maps(region, scale, t_width=None):
+    """The fp64 maps of an OrientedRegion (DESIGN.md 7b, "Oriented text regions"), computed here once for the kernels and the
+    numpy twin alike.  w_r = round_half_even(|e|), h_r = round_half_even(|f|);
+      M = [[ex/w_r, fx/h_r, tlx + 0.5 ex/w_r + 0.5 fx/h_r - 0.5], [ey/w_r, fy/h_r, tly + 0.5 ey/w_r + 0.5 fy/h_r - 0.5]];
+    N takes output pixel (X, Y) at scale s to T's pixel indices (a W_T - 0.5, 128 b - 0.5), where ((X + 0.5)/s, (Y + 0.5)/s) - tl
+    = a e + b f; kx = fl32(s |e x f| / (|f| W_T)), ky = fl32(s |e x f| / (128 |e|)).  W_T (``t_width``) defaults to
+    round_half_even(w_r 128 / h_r), the width restore_images gives a line that fits its canvas; pass T's own width otherwise.
+    For integer axis-aligned corners M = [[1, 0, x0], [0, 1, y0]] exactly."""
+    import numpy as np
+    from .ops import round_half_even
+    (tlx, tly), (trx, try_), (blx, bly) = ((float(p[0]), float(p[1])) for p in region)
+    ex, ey, fx, fy = trx - tlx, try_ - tly, blx - tlx, bly - tly
+    le, lf = math.hypot(ex, ey), math.hypot(fx, fy)
+    w_r, h_r = round_half_even(le), round_half_even(lf)
+    a, b, c, d = ex / w_r, fx / h_r, ey / w_r, fy / h_r
+    m = np.array([[a, b, tlx + 0.5 * a + 0.5 * b - 0.5], [c, d, tly + 0.5 * c + 0.5 * d - 0.5]], np.float64)
+    wt = round_half_even(w_r * (128 / h_r)) if t_width is None else int(t_width)
+    s, cross, h = scale, ex * fy - ey * fx, 0.5 / scale
+    n = np.array([[wt * fy / (s * cross), -wt * fx / (s * cross), wt * (fy * (h - tlx) - fx * (h - tly)) / cross - 0.5],
+                  [-128 * ey / (s * cross), 128 * ex / (s * cross), 128 * (ex * (h - tly) - ey * (h - tlx)) / cross - 0.5]],
+                 np.float64)
+    kx = float(np.float32(s * abs(cross) / (lf * wt)))
+    ky = float(np.float32(s * abs(cross) / (le * 128)))
+    return OrientedMaps(m, (w_r, h_r), n, kx, ky, wt)
+
+
+def footprint_box(region, maps, scale, page_hw):
+    """(X0, Y0, X1, Y1): output pixels that hold every pixel of the region's footprint, on a page of page_hw = (H, W) output
+    pixels.  The parallelogram is widened by one T pixel on every side (far more than the 1/32-pixel rounding of the fixed-point
+    coordinates) and each pixel whose centre it may cover is taken."""
+    (tlx, tly), (trx, try_), (blx, bly) = ((float(p[0]), float(p[1])) for p in region)
+    ex, ey, fx, fy = trx - tlx, try_ - tly, blx - tlx, bly - tly
+    da, db = 1 / maps.t_width, 1 / 128
+    xs = [tlx + a * ex + b * fx for a in (-da, 1 + da) for b in (-db, 1 + db)]
+    ys = [tly + a * ey + b * fy for a in (-da, 1 + da) for b in (-db, 1 + db)]
+    s, (ph, pw) = scale, page_hw
+    return (max(0, math.floor(s * min(xs) - 0.5)), max(0, math.floor(s * min(ys) - 0.5)),
+            min(pw, math.ceil(s * max(xs) - 0.5) + 1), min(ph, math.ceil(s * max(ys) - 0.5) + 1))
+
+
+def _fixed_point_fits(m, box):
+    """cv2.warpAffine's int32 fixed-point coordinates (1/1024 pixel) of every destination pixel of box = (x0, y0, x1, y1) under
+    m stay below 2^30: both the row start (m1 y + m2) * 1024 and the column step m0 x * 1024."""
+    x0, y0, x1, y1 = box
+    return all(abs(r[0]) * x1 + max(abs(r[1] * y0 + r[2]), abs(r[1] * y1 + r[2])) < 2.0 ** 20 for r in m)
+
+
+def _plan_oriented(reg, H, W, scale, name):
+    """Validates an OrientedRegion of an H x W image: (maps, rect, out)."""
+    try:
+        pts = [(float(p[0]), float(p[1])) for p in reg]
+        if len(pts) != 3 or any(len(p) != 2 for p in reg):
+            raise ValueError
+    except (TypeError, ValueError):
+        raise ValueError(f"{name}: expected three (x, y) corners, got {reg!r}") from None
+    if not all(math.isfinite(v) for p in pts for v in p):
+        raise ValueError(f"{name}: corners {pts} are not finite")
+    (tlx, tly), (trx, try_), (blx, bly) = pts
+    ex, ey, fx, fy = trx - tlx, try_ - tly, blx - tlx, bly - tly
+    le, lf, cross = math.hypot(ex, ey), math.hypot(fx, fy), ex * fy - ey * fx
+    if le < 1 or lf < 1:
+        raise ValueError(f"{name}: sides |e| = {le:.4g} and |f| = {lf:.4g} must both be at least 1 pixel")
+    if cross <= 0:
+        raise ValueError(f"{name}: the region is mirrored (e x f = {cross:.4g} <= 0; give tl, tr, bl as the line is read)")
+    if cross < 0.5 * le * lf:
+        raise ValueError(f"{name}: the region is sheared past |e x f| >= |e| |f| / 2")
+    cx, cy = tlx + ex / 2 + fx / 2, tly + ey / 2 + fy / 2
+    if not (0 <= cx < W and 0 <= cy < H):
+        raise ValueError(f"{name}: the centre ({cx:.6g}, {cy:.6g}) is outside the {W}x{H} image")
+    maps = oriented_maps(pts, scale)
+    (w_r, h_r), wt = maps.size, maps.t_width
+    if max(w_r, h_r, wt, H, W) > 32767:
+        raise ValueError(f"{name}: crop {w_r}x{h_r}, restored width {wt} or image {W}x{H} exceeds 32767 pixels "
+                         f"(OpenCV's warp holds source coordinates as int16)")
+    out = footprint_box(pts, maps, scale, (scale * H, scale * W))
+    if not _fixed_point_fits(maps.page_map, out):
+        raise ValueError(f"{name}: the map onto its {out} output box exceeds OpenCV's 32-bit fixed-point coordinates")
+    xs, ys = (tlx, trx, blx, trx + fx), (tly, try_, bly, try_ + fy)
+    rect = (max(0, math.floor(min(xs))), max(0, math.floor(min(ys))), min(W, math.ceil(max(xs))), min(H, math.ceil(max(ys))))
+    return maps, rect, out
 
 
 def _per_image(v, n, what):
@@ -918,11 +1037,15 @@ def _per_image(v, n, what):
 
 def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None):
     """restore_regions' host plan, validated before any launch.  shapes: (H, W) per image; regions: per image, a list of integer
-    half-open rectangles (x0, y0, x1, y1); labels / boxes: None, or per image None or a list with one entry per region (None:
-    predicted, else the region's labels / its detector boxes [x1, y1, x2, y2] in IMAGE coordinates).  Returns the RegionPlans of
-    every region, image by image in region order.
+    half-open rectangles (x0, y0, x1, y1) and OrientedRegions; labels / boxes: None, or per image None or a list with one entry
+    per region (None: predicted, else the region's labels / its detector boxes [x1, y1, x2, y2], in IMAGE coordinates for a
+    rectangle and in the rectified crop's frame for an oriented region).  Returns the RegionPlans of every region, image by
+    image in region order.
     Raises ValueError: scale not an integer in [1, 8], feather < 0, and, naming the image and the region, a rectangle that is
-    empty or leaves the image, a label / box count mismatch, boxes without labels, a box outside the region's columns."""
+    empty or leaves the image, an oriented region with corners that are not finite, a side shorter than 1 pixel, mirrored or
+    sheared past |e x f| < |e| |f| / 2, its centre outside the image, a crop, restored width or image side over 32767 pixels or
+    a page map beyond OpenCV's fixed-point range, a label / box count mismatch, boxes without labels, a box outside the region's
+    columns ([x0, x1] for a rectangle, [0, w_r] for an oriented region)."""
     if isinstance(scale, bool) or not isinstance(scale, int) or not 1 <= scale <= 8:
         raise ValueError(f"scale must be an integer in [1, 8], got {scale!r}")
     if feather is not None and (isinstance(feather, bool) or not isinstance(feather, int) or feather < 0):
@@ -936,16 +1059,24 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
         labs = _per_image(labels[i], len(rects), f"image {i}: labels (one entry per region)")
         bxs = _per_image(boxes[i], len(rects), f"image {i}: boxes (one entry per region)")
         first = len(plan)
+        s = scale
         for r, rect in enumerate(rects):
             name = f"image {i}, region {r}"
-            try:
-                x0, y0, x1, y1 = (int(v) for v in rect)
-                if (x0, y0, x1, y1) != tuple(rect):
-                    raise ValueError
-            except (TypeError, ValueError):
-                raise ValueError(f"{name}: expected an integer rectangle (x0, y0, x1, y1), got {rect!r}") from None
-            if not (0 <= x0 < x1 <= W and 0 <= y0 < y1 <= H):
-                raise ValueError(f"{name}: rectangle {(x0, y0, x1, y1)} is empty or outside the {W}x{H} image")
+            maps = None
+            if isinstance(rect, OrientedRegion):
+                maps, (x0, y0, x1, y1), out = _plan_oriented(rect, H, W, s, name)
+                cols = (0, maps.size[0])
+            else:
+                try:
+                    x0, y0, x1, y1 = (int(v) for v in rect)
+                    if (x0, y0, x1, y1) != tuple(rect):
+                        raise ValueError
+                except (TypeError, ValueError):
+                    raise ValueError(f"{name}: expected an integer rectangle (x0, y0, x1, y1) or an OrientedRegion, "
+                                     f"got {rect!r}") from None
+                if not (0 <= x0 < x1 <= W and 0 <= y0 < y1 <= H):
+                    raise ValueError(f"{name}: rectangle {(x0, y0, x1, y1)} is empty or outside the {W}x{H} image")
+                out, cols = (s * x0, s * y0, s * x1, s * y1), (x0, x1)
             lab, bx = labs[r], bxs[r]
             if lab is not None:
                 lab = [int(v) for v in torch.as_tensor(lab, dtype=torch.long).reshape(-1).tolist()]
@@ -956,13 +1087,14 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
                     raise ValueError(f"{name}: {len(lab)} labels for {len(bx)} boxes")
                 for k, b in enumerate(bx):
                     b = [float(v) for v in b]
-                    if len(b) != 4 or not x0 <= b[0] <= b[2] <= x1:
-                        raise ValueError(f"{name}, character {k}: box {b} is outside the region's columns [{x0}, {x1}]")
-                bx = [[float(b[0]) - x0, float(b[1]) - y0, float(b[2]) - x0, float(b[3]) - y0] for b in bx]
-            overlaps = [first + j for j, q in enumerate(plan[first:]) if max(x0, q.rect[0]) < min(x1, q.rect[2])
-                        and max(y0, q.rect[1]) < min(y1, q.rect[3])]
-            s = scale
-            plan.append(RegionPlan(i, r, (x0, y0, x1, y1), (s * x0, s * y0, s * x1, s * y1), overlaps, lab, bx))
+                    if len(b) != 4 or not cols[0] <= b[0] <= b[2] <= cols[1]:
+                        raise ValueError(f"{name}, character {k}: box {b} is outside the region's columns [{cols[0]}, {cols[1]}]")
+                dx, dy = (0, 0) if maps else (x0, y0)
+                bx = [[float(b[0]) - dx, float(b[1]) - dy, float(b[2]) - dx, float(b[3]) - dy] for b in bx]
+            overlaps = [first + j for j, q in enumerate(plan[first:]) if max(out[0], q.out[0]) < min(out[2], q.out[2])
+                        and max(out[1], q.out[1]) < min(out[3], q.out[3])]
+            extra = (OrientedRegion(*((float(p[0]), float(p[1])) for p in rect)), maps.matrix, maps.size) if maps else ()
+            plan.append(RegionPlan(i, r, (x0, y0, x1, y1), out, overlaps, lab, bx, *extra))
     return plan
 
 
@@ -999,8 +1131,9 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     (DESIGN.md section 7b, "Text regions in whole images").
 
     images: uint8 [H, W, 3] numpy arrays or CPU / CUDA tensors, in any channel order; regions: per image, a list of integer
-    rectangles (x0, y0, x1, y1), 0 <= x0 < x1 <= W, 0 <= y0 < y1 <= H, in the order they compose; labels / boxes: as
-    plan_regions takes them (boxes in image coordinates; None entries are predicted, exactly as restore_images predicts).
+    rectangles (x0, y0, x1, y1), 0 <= x0 < x1 <= W, 0 <= y0 < y1 <= H, and OrientedRegions, in the order they compose; labels /
+    boxes: as plan_regions takes them (boxes in image coordinates; None entries are predicted, exactly as restore_images
+    predicts).
     scale s: an integer in [1, 8]; feather F >= 0 output pixels (default 2 s).
     The result of an image is out = B = cv2.resize(img, (0, 0), fx=s, fy=s, INTER_CUBIC) (OpenCV's own path), then for each region
     that did not fail, in order, over its rectangle R = [s x0, s x1) x [s y0, s y1):
@@ -1013,7 +1146,12 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     Returns one dict per image: image (uint8 [s H, s W, 3]) and regions, one entry per region: dict(sr_u8, segments, labels,
     boxes) -- boxes in image coordinates, predicted ones shifted back -- or, with ``skip_invalid``, dict(error=...) for a region
     restore_images rejected, whose rectangle keeps the background.  Results stay on the device, or come back as numpy arrays
-    through one pinned buffer and one synchronisation with ``to_host``.  plan_regions' errors are raised whatever skip_invalid."""
+    through one pinned buffer and one synchronisation with ``to_host``.  plan_regions' errors are raised whatever skip_invalid.
+    An OrientedRegion (DESIGN.md 7b, "Oriented text regions") is restored from its rectified crop
+    C = cv2.warpAffine(img, M, (w_r, h_r), INTER_CUBIC | WARP_INVERSE_MAP, BORDER_REPLICATE) (oriented_maps; every crop of the
+    call in one mn_warp_affine_u8_batched launch), its labels and boxes given and returned in C's frame, and its entry gains
+    ``matrix`` (M) and ``size`` ((w_r, h_r)).  Its T is warped back by N onto its footprint with a feather on all four sides, and
+    a call that holds one composes every region with mn_composite_regions_affine_u8 instead of mn_composite_regions_u8."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     plan = plan_regions([im.shape[:2] for im in imgs], regions, labels, boxes, scale, feather)
@@ -1023,9 +1161,18 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     dev = next(encoder.parameters()).device
     with torch.cuda.device(dev):
         dimg = _device_images(range(len(imgs)), imgs, dev)
-        res = restore_images(encoder, tspgan, sr, [dimg[p.image][p.rect[1]:p.rect[3], p.rect[0]:p.rect[2]] for p in plan],
-                             [p.labels for p in plan], [p.boxes for p in plan], max_lines=max_lines, context=context,
-                             skip_invalid=skip_invalid, whole_lines=whole_lines, overlap=overlap) if plan else []
+        crops = [dimg[p.image][p.rect[1]:p.rect[3], p.rect[0]:p.rect[2]] for p in plan]
+        oriented = [k for k, p in enumerate(plan) if p.oriented is not None]
+        if oriented:                                     # every oriented region rectified in one launch
+            n_crop = [3 * plan[k].size[0] * plan[k].size[1] for k in oriented]
+            cbuf = torch.empty(sum(n_crop), dtype=torch.uint8, device=dev)
+            o = 0
+            for k, nb in zip(oriented, n_crop):
+                crops[k] = cbuf[o:o + nb].view(plan[k].size[1], plan[k].size[0], 3)
+                o += nb
+            ops.warp_affine([(dimg[plan[k].image], crops[k], plan[k].matrix) for k in oriented])
+        res = restore_images(encoder, tspgan, sr, crops, [p.labels for p in plan], [p.boxes for p in plan], max_lines=max_lines,
+                             context=context, skip_invalid=skip_invalid, whole_lines=whole_lines, overlap=overlap) if plan else []
         sizes = [scale * scale * im.shape[0] * im.shape[1] * 3 for im in imgs]
         flat = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
         offs = [sum(sizes[:i]) for i in range(len(imgs))]
@@ -1033,8 +1180,13 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         ops.resize_cubic([(dimg[i], pages[i]) for i in range(len(imgs))])
         ok = [k for k, r in enumerate(res) if "error" not in r]
         if ok:
-            ops.composite_regions([(pages[plan[k].image], res[k]["sr_u8"], plan[k].out, chain)
-                                   for k, chain in zip(ok, region_chains(plan, ok))], feather)
+            items = [(pages[plan[k].image], res[k]["sr_u8"], plan[k].out, chain) for k, chain in zip(ok, region_chains(plan, ok))]
+            if oriented:
+                maps = [None if plan[k].oriented is None else oriented_maps(plan[k].oriented, scale, res[k]["sr_u8"].shape[1])
+                        for k in ok]
+                ops.composite_regions_affine([it + (m and (m.page_map, m.kx, m.ky),) for it, m in zip(items, maps)], feather)
+            else:
+                ops.composite_regions(items, feather)
         srs = {k: res[k]["sr_u8"] for k in ok}
         if to_host:
             host = _to_host_all([flat] + list(srs.values()))
@@ -1046,11 +1198,13 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         if "error" in r:
             entry = dict(error=r["error"])
         elif "boxes" in r:
-            x0, y0 = p.rect[:2]
+            x0, y0 = (0, 0) if p.oriented else p.rect[:2]
             entry = dict(sr_u8=srs[k], segments=r["segments"], labels=r["labels"],
                          boxes=[[b[0] + x0, b[1] + y0, b[2] + x0, b[3] + y0] for b in r["boxes"]])
         else:
             entry = dict(sr_u8=srs[k], segments=r["segments"], labels=p.labels, boxes=boxes[p.image][p.region])
+        if p.oriented and "error" not in r:
+            entry.update(matrix=p.matrix.copy(), size=p.size)
         out[p.image]["regions"].append(entry)
     return out
 

@@ -3,7 +3,7 @@ pipeline.restore_regions against the host path a user writes without it -- resto
 the pages, then cv2's cubic resize of every page and of every restored region (IPP off) and the numpy feather blend
 (oracle/regions.py).
 
-    MN_MODULE_GRAPHS=0 python tools/bench_regions.py [--pages 8] [--lines 12] [--passes 3] [--scale 4]
+    MN_MODULE_GRAPHS=0 python tools/bench_regions.py [--pages 8] [--lines 12] [--passes 3] [--scale 4] [--max-angle 0]
 
 The pages are seeded: tools/bench_images.make_image_set lines (the reference test set's sizes and lines 2 to 4 times wider than the
 LQ canvas) pasted one under another onto a noise background, each line a region with its character boxes.  The arms alternate pass
@@ -11,6 +11,12 @@ by pass; both must give the same bytes.  The two new kernels (mn_resize_cubic_u8
 CUDA events around their launches inside the restore_regions passes.  MN_MODULE_GRAPHS defaults to 0 here: recorded module graphs
 of 16-character crop batches outgrow an 80 GB card (DESIGN.md section 7b).  Prints one JSON line per arm and one for the kernels,
 with the card's name and power limit read in the same run.  Not part of the product path.
+
+With --max-angle DEG > 0 every line is pasted turned by a seeded angle in [-DEG, DEG] and given as a pipeline.OrientedRegion
+(DESIGN.md section 7b, "Oriented text regions").  The host arm then rectifies each line with cv2.warpAffine, runs
+restore_images(to_host=True) on the crops, resizes the pages with cv2, warps each restored line back with cv2.warpAffine and
+blends it over its footprint with the numpy feather (oracle/oriented_regions.py); the timed kernels are mn_warp_affine_u8_batched,
+mn_resize_cubic_u8_batched and mn_composite_regions_affine_u8.
 """
 import argparse
 import json
@@ -56,6 +62,75 @@ def make_pages(n_pages, n_lines, seed=0):
     return pages, rects, labs, bxs
 
 
+def make_rotated_pages(n_pages, n_lines, max_angle, seed=0):
+    """make_pages' lines, each turned by a seeded angle in [-max_angle, max_angle] and pasted (nearest pixel) one under another
+    by their bounding boxes onto a noise page: (pages, regions, labels, boxes), regions OrientedRegions and boxes in each line's
+    own frame."""
+    import cv2
+    from bench_images import make_image_set
+    from marconet_b200.pipeline import OrientedRegion, oriented_maps
+    images, labels, boxes = make_image_set(n_pages * n_lines, seed)
+    rng = np.random.default_rng(seed + 1)
+    pages, regs, labs, bxs = [], [], [], []
+    for p in range(n_pages):
+        idx = range(p * n_lines, (p + 1) * n_lines)
+        angles = rng.uniform(-max_angle, max_angle, n_lines)
+        ext = []
+        for i, a in zip(idx, angles):
+            h, w = images[i].shape[:2]
+            c, sn = abs(np.cos(np.radians(a))), abs(np.sin(np.radians(a)))
+            ext.append((w * c + h * sn, w * sn + h * c))
+        W = int(max(e[0] for e in ext)) + 24
+        H = int(sum(e[1] + 8 for e in ext)) + 16
+        page = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
+        rr, y = [], 8.0
+        for i, a, (bw, bh) in zip(idx, angles, ext):
+            h, w = images[i].shape[:2]
+            reg = OrientedRegion.from_rotated(8 + bw / 2, y + bh / 2, w, h, a)
+            m = oriented_maps(reg, 1)
+            assert m.size == (w, h)
+            warped = cv2.warpAffine(images[i], m.matrix, (W, H), flags=cv2.INTER_NEAREST)
+            inside = cv2.warpAffine(np.ones((h, w), np.uint8), m.matrix, (W, H), flags=cv2.INTER_NEAREST).astype(bool)
+            page[inside] = warped[inside]
+            rr.append(reg)
+            y += bh + 8
+        pages.append(page)
+        regs.append(rr)
+        labs.append([labels[i] for i in idx])
+        bxs.append([boxes[i] for i in idx])
+    return pages, regs, labs, bxs
+
+
+def host_path_oriented(m, pages, regs, labels, boxes, s, feather, max_lines):
+    """cv2 rectify, restore_images on the crops, cv2 background and cv2 warp of each restored line back (onto the rows and
+    columns up to its footprint's far corner, so that its fixed-point coordinates are the whole page's), the numpy blend."""
+    import cv2
+    from marconet_b200 import pipeline
+    from oracle import oriented_regions as regions
+    flags = cv2.INTER_CUBIC | cv2.WARP_INVERSE_MAP
+    crops, labs, bxs = [], [], []
+    for pg, rr, ll, bb in zip(pages, regs, labels, boxes):
+        for reg, lab, bx in zip(rr, ll, bb):
+            mp = pipeline.oriented_maps(reg, 1)
+            crops.append(cv2.warpAffine(pg, mp.matrix, mp.size, flags=flags, borderMode=cv2.BORDER_REPLICATE))
+            labs.append(lab)
+            bxs.append(bx)
+    res = pipeline.restore_images(*m, crops, labs, bxs, max_lines=max_lines, to_host=True)
+    out, k = [], 0
+    for pg, rr in zip(pages, regs):
+        o = cv2.resize(pg, (0, 0), fx=s, fy=s, interpolation=cv2.INTER_CUBIC)
+        for reg in rr:
+            t = res[k]["sr_u8"]
+            (x0, y0, x1, y1), _, _, mask, a = regions.oriented_footprint(t.shape, reg, s, o.shape[:2], feather)
+            n = pipeline.oriented_maps(reg, s, t.shape[1]).page_map
+            p = cv2.warpAffine(np.ascontiguousarray(t[..., ::-1]), n, (x1, y1), flags=flags, borderMode=cv2.BORDER_REPLICATE)
+            sl = o[y0:y1, x0:x1]
+            sl[mask] = regions.blend(sl, p[y0:y1, x0:x1], a)[mask]
+            k += 1
+        out.append(o)
+    return out
+
+
 def host_path(m, pages, rects, labels, boxes, s, feather, max_lines):
     """restore_images on the cut-out regions, then cv2 resizes and the numpy blend on the host."""
     import cv2
@@ -96,6 +171,7 @@ def main():
     ap.add_argument("--passes", type=int, default=3)
     ap.add_argument("--scale", type=int, default=4)
     ap.add_argument("--max-lines", type=int, default=8)
+    ap.add_argument("--max-angle", type=float, default=0.0, help="turn every line by up to this many degrees (oriented regions)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_regions.py needs a CUDA device")
@@ -110,11 +186,16 @@ def main():
         net = cls()
         net.load_state_dict(sds[key], strict=True)
         m.append(net.eval().to(dev))
-    pages, rects, labels, boxes = make_pages(args.pages, args.lines)
+    oriented = args.max_angle > 0
+    if oriented:
+        pages, rects, labels, boxes = make_rotated_pages(args.pages, args.lines, args.max_angle)
+    else:
+        pages, rects, labels, boxes = make_pages(args.pages, args.lines)
     s, feather = args.scale, 2 * args.scale
 
     lib = _lib.load()
-    events = {"mn_resize_cubic_u8_batched": [], "mn_composite_regions_u8": []}
+    events = {"mn_warp_affine_u8_batched": [], "mn_resize_cubic_u8_batched": [], "mn_composite_regions_affine_u8": []} \
+        if oriented else {"mn_resize_cubic_u8_batched": [], "mn_composite_regions_u8": []}
     timing = [False]
     for name in events:
         fn = getattr(lib, name)
@@ -136,7 +217,7 @@ def main():
         return [o["image"] for o in out]
 
     def host():
-        return host_path(m, pages, rects, labels, boxes, s, feather, args.max_lines)
+        return (host_path_oriented if oriented else host_path)(m, pages, rects, labels, boxes, s, feather, args.max_lines)
 
     arms = {"restore_regions": api, "host_path": host}
     outs = {name: fn() for name, fn in arms.items()}                 # warm-up pass of each arm
@@ -156,6 +237,7 @@ def main():
     card = _card()
     out_px = sum(s * s * p.shape[0] * p.shape[1] for p in pages)
     common = dict(pages=args.pages, lines_per_page=args.lines, scale=s, feather=feather, max_lines=args.max_lines,
+                  max_angle=args.max_angle,
                   page_sizes=[list(p.shape[:2]) for p in pages], output_megapixels=round(out_px / 1e6, 2),
                   module_graphs=os.environ.get("MN_MODULE_GRAPHS"), same_bytes=same, max_abs_diff=diff, **card)
     for name, ts in times.items():
