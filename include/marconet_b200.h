@@ -557,6 +557,43 @@ typedef struct {
 } mn_region_affine;
 int mn_composite_regions_affine_u8(const mn_region_affine* regions, int n, long long max_pixels, void* stream);
 
+/* Perspective text regions (DESIGN.md section 7b, "Perspective text regions").
+ * cv2.warpPerspective(src, M, (dw, dh), INTER_CUBIC | WARP_INVERSE_MAP, BORDER_REPLICATE), OpenCV's own 8-bit path (IPP off), of
+ * n images in one launch, blockIdx.y = image, one thread per destination pixel.  m = M row by row: destination pixel (x, y) ->
+ * source pixel ((m[0] x + m[1] y + m[2]) / w, (m[3] x + m[4] y + m[5]) / w), w = m[6] x + m[7] y + m[8].  OpenCV's fixed-point
+ * coordinates in 1/32 pixel (fp64, no contraction), formed in column blocks of bw = min(1024 / min(16, dh), dw): at the block's
+ * first column xb, X0 = fl(fl(fl(m[0] xb) + fl(m[1] y)) + m[2]), Y0 and W0 likewise; with x1 = x - xb, W = fl(W0 + fl(m[6] x1)),
+ * W = W ? fl(32 / W) : 0, Xq = cvRound(clamp(fl(fl(X0 + fl(m[0] x1)) W), INT_MIN, INT_MAX)) and likewise Yq; then remap's cubic
+ * sampler exactly as mn_warp_affine_u8_batched uses it.  Byte offsets are 64-bit.  max_pixels >= every dh*dw.  images: DEVICE
+ * array of records (validated by the caller). */
+typedef struct {
+    const uint8_t* src;         /* row 0 of the source image */
+    int64_t src_pitch;
+    int32_t h, w;
+    uint8_t* dst;               /* row 0 of the destination image */
+    int64_t dst_pitch;
+    int32_t dh, dw;
+    double m[9];
+} mn_warp_perspective_image;
+int mn_warp_perspective_u8_batched(const mn_warp_perspective_image* images, int n, int cn, long long max_pixels, void* stream);
+
+/* mn_composite_regions_affine_u8 for pages that also hold perspective regions: every region of every page in one launch,
+ * blockIdx.y = region.  Kinds MN_REGION_RECT and MN_REGION_AFFINE (n[0..5] = the affine N) are composed exactly as
+ * mn_composite_regions_affine_u8 composes them (the same device functions).  Kind MN_REGION_PERSPECTIVE: r's rectangle is the
+ * bounding box of the region's footprint; n (3 x 3) maps page pixel (X, Y) to pixel indices of the restored bytes T, (Xq, Yq) are
+ * mn_warp_perspective_u8_batched's fixed-point coordinates of (X, Y) under n with the whole page [page_h][page_w] as the
+ * destination (its column blocks start at page column 0), and the footprint test, the feather, P, the blend
+ * and the owner rule are the affine kind's; chains index this array. */
+#define MN_REGION_PERSPECTIVE 2
+typedef struct {
+    mn_region r;
+    int32_t kind;
+    float kx, ky;               /* feather slopes of an affine or perspective region */
+    int32_t pad;
+    double n[9];                /* affine region: n[0..5], page pixel -> T pixel, row by row; perspective region: all nine */
+} mn_region_quad;
+int mn_composite_regions_quad_u8(const mn_region_quad* regions, int n, long long max_pixels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

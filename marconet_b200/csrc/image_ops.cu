@@ -320,13 +320,51 @@ __device__ __forceinline__ int warp_cubic_u8(const uint8_t* __restrict__ img, lo
     return min(max((acc + (1 << 14)) >> 15, 0), 255);
 }
 
-__device__ __forceinline__ bool footprint_holds(const mn_region_affine& q, const WarpCoord& c) {
-    return c.xq >= -16 && c.xq < 32 * q.r.sr_w - 16 && c.yq >= -16 && c.yq < 32 * q.r.sr_h - 16;
+// cv2.warpPerspective's fixed-point source coordinates of pixel (x, y) of a dw x dh destination under the 3 x 3 m
+// (WARP_INVERSE_MAP), in 1/32 pixel.  OpenCV walks the destination in column blocks of bw = min(1024 / min(16, dh), dw) and at
+// each block's first column xb forms X0 = fl(fl(fl(m0 xb) + fl(m1 y)) + m2) (Y0, W0 likewise); then with x1 = x - xb,
+// W = fl(W0 + fl(m6 x1)), W = W ? fl(32 / W) : 0, Xq = cvRound(clamp(fl(fl(X0 + fl(m0 x1)) W), INT_MIN, INT_MAX)).  The block
+// origin changes the rounding, so it is part of the result.
+__device__ __forceinline__ WarpCoord warp_coord_perspective(const double* m, int x, int y, int dw, int dh) {
+    const int bw = min(1024 / min(16, dh), dw);
+    const double xb = (double)(x - x % bw), x1 = (double)(x % bw), yd = (double)y;
+    const double x0 = __dadd_rn(__dadd_rn(__dmul_rn(m[0], xb), __dmul_rn(m[1], yd)), m[2]);
+    const double y0 = __dadd_rn(__dadd_rn(__dmul_rn(m[3], xb), __dmul_rn(m[4], yd)), m[5]);
+    const double w0 = __dadd_rn(__dadd_rn(__dmul_rn(m[6], xb), __dmul_rn(m[7], yd)), m[8]);
+    double w = __dadd_rn(w0, __dmul_rn(m[6], x1));
+    w = w != 0.0 ? __ddiv_rn(32.0, w) : 0.0;
+    const double fx = fmin(fmax(__dmul_rn(__dadd_rn(x0, __dmul_rn(m[0], x1)), w), (double)INT_MIN), (double)INT_MAX);
+    const double fy = fmin(fmax(__dmul_rn(__dadd_rn(y0, __dmul_rn(m[3], x1)), w), (double)INT_MIN), (double)INT_MAX);
+    return {__double2int_rn(fx), __double2int_rn(fy)};
+}
+
+__device__ __forceinline__ bool footprint_holds(const mn_region& r, const WarpCoord& c) {
+    return c.xq >= -16 && c.xq < 32 * r.sr_w - 16 && c.yq >= -16 && c.yq < 32 * r.sr_h - 16;
 }
 
 __device__ __forceinline__ bool region_holds(const mn_region_affine& q, int X, int Y) {
     if (!region_holds(q.r, X, Y)) return false;
-    return q.kind == MN_REGION_RECT || footprint_holds(q, warp_coord(q.n, X, Y));
+    return q.kind == MN_REGION_RECT || footprint_holds(q.r, warp_coord(q.n, X, Y));
+}
+
+// P of a warped region r (T = r.sr) at fixed-point T coordinates wc, feathered with slopes kx, ky on all four sides, blended over v.
+__device__ __forceinline__ void footprint_blend(const mn_region& r, float kx, float ky, const WarpCoord& wc, int v[3]) {
+    float a = 1.f;
+    if (r.feather != 0) {
+        const float u = __fmul_rn((float)(wc.xq + 16), 1.f / 32.f), t = __fmul_rn((float)(wc.yq + 16), 1.f / 32.f);
+        const float du = __fmul_rn(kx, fminf(u, __fsub_rn((float)r.sr_w, u)));
+        const float dv = __fmul_rn(ky, fminf(t, __fsub_rn((float)r.sr_h, t)));
+        a = fminf(1.f, __fdiv_rn(fminf(du, dv), (float)r.feather));
+    }
+    const float b = __fsub_rn(1.f, a);
+    int wt[16];
+    warp_taps(wc, wt);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const int p = warp_cubic_u8(r.sr, r.sr_pitch, r.sr_h, r.sr_w, 3, 2 - c, wc, wt);
+        const int t = __float2int_rn(__fadd_rn(__fmul_rn(a, (float)p), __fmul_rn(b, (float)v[c])));
+        v[c] = min(max(t, 0), 255);
+    }
 }
 
 __device__ __forceinline__ void region_blend(const mn_region_affine& q, int X, int Y, int v[3]) {
@@ -334,27 +372,30 @@ __device__ __forceinline__ void region_blend(const mn_region_affine& q, int X, i
         region_blend(q.r, X, Y, v);
         return;
     }
-    const WarpCoord wc = warp_coord(q.n, X, Y);
-    float a = 1.f;
-    if (q.r.feather != 0) {
-        const float u = __fmul_rn((float)(wc.xq + 16), 1.f / 32.f), t = __fmul_rn((float)(wc.yq + 16), 1.f / 32.f);
-        const float du = __fmul_rn(q.kx, fminf(u, __fsub_rn((float)q.r.sr_w, u)));
-        const float dv = __fmul_rn(q.ky, fminf(t, __fsub_rn((float)q.r.sr_h, t)));
-        a = fminf(1.f, __fdiv_rn(fminf(du, dv), (float)q.r.feather));
+    footprint_blend(q.r, q.kx, q.ky, warp_coord(q.n, X, Y), v);
+}
+
+// The T coordinates of page pixel (X, Y) under an affine or perspective region's n (the whole page is the destination).
+__device__ __forceinline__ WarpCoord quad_coord(const mn_region_quad& q, int X, int Y) {
+    return q.kind == MN_REGION_PERSPECTIVE ? warp_coord_perspective(q.n, X, Y, q.r.page_w, q.r.page_h) : warp_coord(q.n, X, Y);
+}
+
+__device__ __forceinline__ bool region_holds(const mn_region_quad& q, int X, int Y) {
+    if (!region_holds(q.r, X, Y)) return false;
+    return q.kind == MN_REGION_RECT || footprint_holds(q.r, quad_coord(q, X, Y));
+}
+
+__device__ __forceinline__ void region_blend(const mn_region_quad& q, int X, int Y, int v[3]) {
+    if (q.kind == MN_REGION_RECT) {
+        region_blend(q.r, X, Y, v);
+        return;
     }
-    const float b = __fsub_rn(1.f, a);
-    int wt[16];
-    warp_taps(wc, wt);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        const int p = warp_cubic_u8(q.r.sr, q.r.sr_pitch, q.r.sr_h, q.r.sr_w, 3, 2 - c, wc, wt);
-        const int t = __float2int_rn(__fadd_rn(__fmul_rn(a, (float)p), __fmul_rn(b, (float)v[c])));
-        v[c] = min(max(t, 0), 255);
-    }
+    footprint_blend(q.r, q.kx, q.ky, quad_coord(q, X, Y), v);
 }
 
 __device__ __forceinline__ const mn_region& rect_of(const mn_region& r) { return r; }
 __device__ __forceinline__ const mn_region& rect_of(const mn_region_affine& r) { return r.r; }
+__device__ __forceinline__ const mn_region& rect_of(const mn_region_quad& r) { return r.r; }
 
 // blockIdx.y = region; one thread per output pixel of its rectangle, those past its pixels (or outside its footprint) exit.  The
 // pixel belongs to the last region of its chain (every region of the page whose rectangle meets this one, in page order) that
@@ -411,6 +452,25 @@ __global__ void warp_affine_batched_kernel(const mn_warp_image* __restrict__ ima
     for (int c = 0; c < cn; ++c) o[c] = (uint8_t)warp_cubic_u8(im.src, im.src_pitch, im.h, im.w, cn, c, wc, wt);
 }
 
+__global__ void composite_regions_quad_kernel(const mn_region_quad* __restrict__ regions) {
+    mn_pdl_prologue();
+    composite_pixel(regions);
+}
+
+// blockIdx.y = image; one thread per destination pixel of its [dh][dw][cn] image, those past its dh*dw pixels exit.
+__global__ void warp_perspective_batched_kernel(const mn_warp_perspective_image* __restrict__ images, int cn) {
+    mn_pdl_prologue();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const mn_warp_perspective_image im = images[blockIdx.y];
+    if (idx >= (long long)im.dh * im.dw) return;
+    const int x = (int)(idx % im.dw), y = (int)(idx / im.dw);
+    const WarpCoord wc = warp_coord_perspective(im.m, x, y, im.dw, im.dh);
+    int wt[16];
+    warp_taps(wc, wt);
+    uint8_t* o = im.dst + (long long)y * im.dst_pitch + (long long)x * cn;
+    for (int c = 0; c < cn; ++c) o[c] = (uint8_t)warp_cubic_u8(im.src, im.src_pitch, im.h, im.w, cn, c, wc, wt);
+}
+
 }  // namespace
 
 extern "C" int mn_resize_cubic_u8_batched(const mn_resize_image* images, int n, int cn, long long max_pixels, void* stream) {
@@ -444,6 +504,25 @@ extern "C" int mn_composite_regions_affine_u8(const mn_region_affine* regions, i
     MN_REQUIRE(regions && n > 0 && n <= 65535 && max_pixels > 0, "mn_composite_regions_affine_u8: bad args");
     MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_composite_regions_affine_u8: %lld pixels exceed the grid", max_pixels);
     MN_CUDA_CHECK((mn_launch(composite_regions_affine_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
+                             (cudaStream_t)stream, regions)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_warp_perspective_u8_batched(const mn_warp_perspective_image* images, int n, int cn, long long max_pixels,
+                                              void* stream) {
+    MN_REQUIRE(images && n > 0 && n <= 65535 && cn > 0 && cn <= 4 && max_pixels > 0, "mn_warp_perspective_u8_batched: bad args");
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_warp_perspective_u8_batched: %lld pixels exceed the grid", max_pixels);
+    MN_CUDA_CHECK((mn_launch(warp_perspective_batched_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
+                             (cudaStream_t)stream, images, cn)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_composite_regions_quad_u8(const mn_region_quad* regions, int n, long long max_pixels, void* stream) {
+    MN_REQUIRE(regions && n > 0 && n <= 65535 && max_pixels > 0, "mn_composite_regions_quad_u8: bad args");
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_composite_regions_quad_u8: %lld pixels exceed the grid", max_pixels);
+    MN_CUDA_CHECK((mn_launch(composite_regions_quad_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
                              (cudaStream_t)stream, regions)));
     MN_LAUNCH_CHECK();
     return MN_OK;

@@ -1264,29 +1264,43 @@ def warp_affine(items):
     list of (src, dst, M): uint8 [h, w, cn] and [dh, dw, cn] CUDA views with dense pixels (any row stride), h, w <= 32767, and M
     a 2 x 3 map from dst pixel indices to src pixel indices whose fixed-point coordinates over dst stay below 2^30 / 1024 pixels
     in magnitude (pipeline.oriented_maps keeps them so)."""
+    _warp(items, "warp_affine", 2, _lib.WarpImage, "mn_warp_affine_u8_batched")
+
+
+def warp_perspective(items):
+    """cv2.warpPerspective(src, M, (dw, dh), flags=INTER_CUBIC | WARP_INVERSE_MAP, borderMode=BORDER_REPLICATE) -- OpenCV's own
+    8-bit path (IPP off) -- for many images in one launch (mn_warp_perspective_u8_batched; DESIGN.md 7b, "Perspective text
+    regions").  items: list of (src, dst, M) as warp_affine takes them, M a 3 x 3 homogeneous map from dst pixel indices to src
+    pixel indices whose denominator is positive over dst and whose fixed-point coordinates stay below 2^30 / 32 pixels in
+    magnitude (pipeline.quad_maps keeps them so)."""
+    _warp(items, "warp_perspective", 3, _lib.WarpPerspectiveImage, "mn_warp_perspective_u8_batched")
+
+
+def _warp(items, what, rows, record, symbol):
+    """One launch of ``symbol`` over warp_affine's / warp_perspective's items, M ``rows`` x 3."""
     global LAUNCHES
     if not items:
-        raise ValueError("warp_affine: no images")
+        raise ValueError(f"{what}: no images")
     if len(items) > 65535:
-        raise ValueError("warp_affine: at most 65535 images per launch")
+        raise ValueError(f"{what}: at most 65535 images per launch")
     dev = items[0][0].device
     cn = items[0][0].shape[2] if isinstance(items[0][0], torch.Tensor) and items[0][0].dim() == 3 else 3
     if not 1 <= cn <= 4:
-        raise RuntimeError(f"warp_affine: {cn} channels (1 to 4)")
+        raise RuntimeError(f"{what}: {cn} channels (1 to 4)")
     recs, mx = [], 0
     for i, (src, dst, m) in enumerate(items):
-        _dense_u8(src, dev, cn, f"warp_affine: image {i}: src")
-        _dense_u8(dst, dev, cn, f"warp_affine: image {i}: dst")
+        _dense_u8(src, dev, cn, f"{what}: image {i}: src")
+        _dense_u8(dst, dev, cn, f"{what}: image {i}: dst")
         (h, w), (dh, dw) = src.shape[:2], dst.shape[:2]
         if max(h, w) > 32767:
-            raise ValueError(f"warp_affine: image {i}: a {h}x{w} source exceeds OpenCV's int16 source coordinates")
+            raise ValueError(f"{what}: image {i}: a {h}x{w} source exceeds OpenCV's int16 source coordinates")
         m = [float(v) for row in m for v in row]
-        if len(m) != 6:
-            raise ValueError(f"warp_affine: image {i}: M must be 2 x 3")
-        recs.append(_lib.WarpImage(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw, (ctypes.c_double * 6)(*m)))
+        if len(m) != 3 * rows:
+            raise ValueError(f"{what}: image {i}: M must be {rows} x 3")
+        recs.append(record(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw, (ctypes.c_double * (3 * rows))(*m)))
         mx = max(mx, dh * dw)
-    table = _table(_lib.WarpImage, recs, dev)
-    _lib.check(_lib.load().mn_warp_affine_u8_batched(_ptr(table), len(recs), cn, mx, _stream()), "mn_warp_affine_u8_batched")
+    table = _table(record, recs, dev)
+    _lib.check(getattr(_lib.load(), symbol)(_ptr(table), len(recs), cn, mx, _stream()), symbol)
     LAUNCHES += 1
 
 
@@ -1312,4 +1326,29 @@ def composite_regions_affine(regions, feather):
         out.append(_lib.RegionAffine(rec, _lib.REGION_AFFINE, kx, ky, 0, (ctypes.c_double * 6)(*n)))
     _upload_records(buf, out, chains)
     _lib.check(_lib.load().mn_composite_regions_affine_u8(_ptr(buf), len(out), mx, _stream()), "mn_composite_regions_affine_u8")
+    LAUNCHES += 1
+
+
+def composite_regions_quad(regions, feather):
+    """composite_regions_affine for pages that also hold perspective regions (mn_composite_regions_quad_u8; DESIGN.md 7b,
+    "Perspective text regions"), one launch.  regions: list of (page, sr, rect, chain, maps) as composite_regions_affine takes
+    them; maps may also be (N, kx, ky) with N 3 x 3 (fp64): a perspective region whose page map is homogeneous, with a positive
+    denominator over rect, the bounding box of its footprint in page pixels (pipeline.quad_maps).  The footprint test is the
+    affine one on its fixed-point sr coordinates."""
+    global LAUNCHES
+    recs, chains, mx, buf = _region_records(regions, int(feather), "composite_regions_quad", _lib.RegionQuad)
+    out = []
+    for i, (r, rec) in enumerate(zip(regions, recs)):
+        maps = r[4]
+        if maps is None:
+            out.append(_lib.RegionQuad(rec, _lib.REGION_RECT, 0.0, 0.0, 0, (ctypes.c_double * 9)()))
+            continue
+        n, kx, ky = maps
+        n = [float(v) for row in n for v in row]
+        if len(n) not in (6, 9) or not (kx > 0 and ky > 0):
+            raise ValueError(f"composite_regions_quad: region {i}: expected (N 2 x 3 or 3 x 3, kx > 0, ky > 0)")
+        kind = _lib.REGION_AFFINE if len(n) == 6 else _lib.REGION_PERSPECTIVE
+        out.append(_lib.RegionQuad(rec, kind, kx, ky, 0, (ctypes.c_double * 9)(*n)))
+    _upload_records(buf, out, chains)
+    _lib.check(_lib.load().mn_composite_regions_quad_u8(_ptr(buf), len(out), mx, _stream()), "mn_composite_regions_quad_u8")
     LAUNCHES += 1

@@ -903,7 +903,8 @@ class RegionPlan(NamedTuple):
     by (-x0, -y0); None: predicted).  An oriented region (DESIGN.md 7b, "Oriented text regions") also has ``oriented`` (the
     OrientedRegion), ``matrix`` (M, its rectified crop's map) and ``size`` ((w_r, h_r), the crop's size); its ``rect`` is the
     bounding box of its corners in source pixels clipped to the image, ``out`` the bounding box of its footprint in output pixels,
-    ``overlaps`` compares the ``out`` boxes, and its boxes are in the crop's frame, unshifted."""
+    ``overlaps`` compares the ``out`` boxes, and its boxes are in the crop's frame, unshifted.  A perspective region (DESIGN.md
+    7b, "Perspective text regions") has ``quad`` (the QuadRegion) instead of ``oriented``, and ``matrix`` is its 3 x 3 M."""
     image: int
     region: int
     rect: tuple
@@ -914,6 +915,7 @@ class RegionPlan(NamedTuple):
     oriented: tuple = None
     matrix: object = None
     size: tuple = None
+    quad: tuple = None
 
 
 class OrientedRegion(NamedTuple):
@@ -1028,6 +1030,147 @@ def _plan_oriented(reg, H, W, scale, name):
     return maps, rect, out
 
 
+class QuadRegion(NamedTuple):
+    """A text line seen in perspective (DESIGN.md 7b, "Perspective text regions"): its top-left, top-right, bottom-right and
+    bottom-left corners as it is read, (x, y) points in continuous image coordinates (pixel (i, j) covers [j, j+1) x [i, i+1)).
+    The rectangle (x0, y0, x1, y1) is QuadRegion((x0, y0), (x1, y0), (x1, y1), (x0, y1))."""
+    tl: tuple
+    tr: tuple
+    br: tuple
+    bl: tuple
+
+
+class QuadMaps(NamedTuple):
+    """quad_maps' result: ``matrix`` M (fp64 [3, 3]: rectified crop pixel indices -> image pixel indices, homogeneous), ``size``
+    (w_r, h_r), ``page_map`` N (fp64 [3, 3]: output page pixel indices -> pixel indices of the restored line T), ``kx`` and ``ky``
+    (the feather slopes, fp32 values), ``t_width`` (W_T) and ``homography`` H (the unit square -> the quad, rows of floats)."""
+    matrix: object
+    size: tuple
+    page_map: object
+    kx: float
+    ky: float
+    t_width: int
+    homography: tuple
+
+
+def _quad_homography(pts):
+    """Heckbert's closed-form H taking the unit square's (0, 0), (1, 0), (1, 1), (0, 1) to p0..p3, as rows (a, b, c), (d, e, f),
+    (g, h, 1)."""
+    (x0, y0), (x1, y1), (x2, y2), (x3, y3) = pts
+    sx, sy = x0 - x1 + x2 - x3, y0 - y1 + y2 - y3
+    dx1, dx2, dy1, dy2 = x1 - x2, x3 - x2, y1 - y2, y3 - y2
+    den = dx1 * dy2 - dx2 * dy1
+    g = (sx * dy2 - sy * dx2) / den
+    h = (dx1 * sy - dy1 * sx) / den
+    return (x1 - x0 + g * x1, x3 - x0 + h * x3, x0), (y1 - y0 + g * y1, y3 - y0 + h * y3, y0), (g, h, 1.0)
+
+
+def quad_maps(region, scale, t_width=None):
+    """The fp64 maps of a QuadRegion (DESIGN.md 7b, "Perspective text regions"), computed here once in plain Python floats with a
+    fixed operation order for the kernels and the numpy twin alike.  w_r = round_half_even(max(|tr - tl|, |br - bl|)),
+    h_r = round_half_even(max(|bl - tl|, |br - tr|)); with H = [[a, b, c], [d, e, f], [g, h, 1]] the unit square -> quad
+    homography, M's rows are [(a - 0.5 g)/w_r, (b - 0.5 h)/h_r, c - 0.5 + 0.5 (a - 0.5 g)/w_r + 0.5 (b - 0.5 h)/h_r], the same with
+    d, e, f, and [g/w_r, h/h_r, 1 + 0.5 g/w_r + 0.5 h/h_r].  N = A_T adj(H) A_page, A_page = [[1/s, 0, 0.5/s], [0, 1/s, 0.5/s],
+    [0, 0, 1]], A_T = [[W_T, 0, -0.5], [0, 128, -0.5], [0, 0, 1]], all nine entries divided by its third row's value at the
+    footprint's centre (the page pixel of H(0.5, 0.5)).  kx = fl32(s A / (L_f W_T)), ky = fl32(s A / (L_e 128)): A the shoelace
+    area, L_e the mean of the top and bottom side lengths, L_f of the left and right ones.  W_T (``t_width``) defaults to
+    round_half_even(w_r 128 / h_r); pass T's own width otherwise.  For integer axis-aligned corners M = [[1, 0, x0], [0, 1, y0],
+    [0, 0, 1]] exactly, and at h = 32, s = 4, N = [[1, 0, -4 x0], [0, 1, -4 y0], [0, 0, 1]]."""
+    import numpy as np
+    from .ops import round_half_even
+    pts = [(float(p[0]), float(p[1])) for p in region]
+    (x0, y0), (x1, y1), (x2, y2), (x3, y3) = pts
+    top, bottom = math.hypot(x1 - x0, y1 - y0), math.hypot(x2 - x3, y2 - y3)
+    left, right = math.hypot(x3 - x0, y3 - y0), math.hypot(x2 - x1, y2 - y1)
+    w_r, h_r = round_half_even(max(top, bottom)), round_half_even(max(left, right))
+    hom = _quad_homography(pts)
+    (a, b, c), (d, e, f), (g, h, _) = hom
+    ra, rb, rd, re, rg, rh = (a - 0.5 * g) / w_r, (b - 0.5 * h) / h_r, (d - 0.5 * g) / w_r, (e - 0.5 * h) / h_r, g / w_r, h / h_r
+    m = np.array([[ra, rb, c - 0.5 + 0.5 * ra + 0.5 * rb], [rd, re, f - 0.5 + 0.5 * rd + 0.5 * re],
+                  [rg, rh, 1.0 + 0.5 * rg + 0.5 * rh]], np.float64)
+    wt = round_half_even(w_r * (128 / h_r)) if t_width is None else int(t_width)
+    s = scale
+    adj = ((e - f * h, c * h - b, b * f - c * e), (f * g - d, a - c * g, c * d - a * f), (d * h - e * g, b * g - a * h, a * e - b * d))
+    hs = 0.5 / s
+    k = [(r[0] / s, r[1] / s, r[0] * hs + r[1] * hs + r[2]) for r in adj]
+    n = [[wt * k[0][j] - 0.5 * k[2][j] for j in range(3)], [128 * k[1][j] - 0.5 * k[2][j] for j in range(3)], list(k[2])]
+    cw = 0.5 * g + 0.5 * h + 1.0
+    xc, yc = s * ((0.5 * a + 0.5 * b + c) / cw) - 0.5, s * ((0.5 * d + 0.5 * e + f) / cw) - 0.5
+    den = n[2][0] * xc + n[2][1] * yc + n[2][2]
+    n = np.array([[v / den for v in row] for row in n], np.float64)
+    area = 0.5 * abs((x0 * y1 - x1 * y0) + (x1 * y2 - x2 * y1) + (x2 * y3 - x3 * y2) + (x3 * y0 - x0 * y3))
+    l_e, l_f = 0.5 * (top + bottom), 0.5 * (left + right)
+    kx = float(np.float32(s * area / (l_f * wt)))
+    ky = float(np.float32(s * area / (l_e * 128)))
+    return QuadMaps(m, (w_r, h_r), n, kx, ky, wt, hom)
+
+
+def quad_footprint_box(maps, scale, page_hw):
+    """(X0, Y0, X1, Y1): output pixels that hold every pixel of a quad's footprint, on a page of page_hw = (H, W) output pixels:
+    the images under H of the corners of [-1/W_T, 1 + 1/W_T] x [-1/128, 1 + 1/128] (the quad widened by one T pixel on every
+    side), each pixel whose centre their hull may cover.  None when H's denominator is not positive at one of those corners."""
+    (a, b, c), (d, e, f), (g, h, _) = maps.homography
+    da, db = 1 / maps.t_width, 1 / 128
+    xs, ys = [], []
+    for u in (-da, 1 + da):
+        for v in (-db, 1 + db):
+            w = g * u + h * v + 1.0
+            if not w > 0:
+                return None
+            xs.append((a * u + b * v + c) / w)
+            ys.append((d * u + e * v + f) / w)
+    s, (ph, pw) = scale, page_hw
+    return (max(0, math.floor(s * min(xs) - 0.5)), max(0, math.floor(s * min(ys) - 0.5)),
+            min(pw, math.ceil(s * max(xs) - 0.5) + 1), min(ph, math.ceil(s * max(ys) - 0.5) + 1))
+
+
+def _plan_quad(reg, H, W, scale, name):
+    """Validates a QuadRegion of an H x W image: (maps, rect, out)."""
+    try:
+        pts = [(float(p[0]), float(p[1])) for p in reg]
+        if len(pts) != 4 or any(len(p) != 2 for p in reg):
+            raise ValueError
+    except (TypeError, ValueError):
+        raise ValueError(f"{name}: expected four (x, y) corners, got {reg!r}") from None
+    if not all(math.isfinite(v) for p in pts for v in p):
+        raise ValueError(f"{name}: corners {pts} are not finite")
+    sides = [math.hypot(pts[(k + 1) % 4][0] - pts[k][0], pts[(k + 1) % 4][1] - pts[k][1]) for k in range(4)]
+    if min(sides) < 1:
+        raise ValueError(f"{name}: sides {[round(v, 4) for v in sides]} must all be at least 1 pixel")
+    for k, corner in enumerate(("tl", "tr", "br", "bl")):
+        (px, py), (nx, ny), (qx, qy) = pts[k], pts[(k + 1) % 4], pts[k - 1]
+        turn = (nx - px) * (qy - py) - (ny - py) * (qx - px)
+        if turn <= 0:
+            raise ValueError(f"{name}: the quad is not strictly convex in reading order (turn {turn:.4g} <= 0 at {corner}; "
+                             f"give tl, tr, br, bl as the line is read)")
+        if turn < 0.5 * sides[k] * sides[k - 1]:
+            raise ValueError(f"{name}: the interior angle at {corner} is outside [30, 150] degrees")
+    cx, cy = sum(p[0] for p in pts) / 4, sum(p[1] for p in pts) / 4
+    if not (0 <= cx < W and 0 <= cy < H):
+        raise ValueError(f"{name}: the centre ({cx:.6g}, {cy:.6g}) is outside the {W}x{H} image")
+    g, h, _ = _quad_homography(pts)[2]
+    ws = (1.0, 1.0 + g, 1.0 + h, 1.0 + g + h)
+    if not min(ws) > 0 or max(ws) > 4 * min(ws):
+        raise ValueError(f"{name}: the foreshortening {max(ws) / min(ws) if min(ws) > 0 else math.inf:.4g} exceeds 4")
+    maps = quad_maps(pts, scale)
+    (w_r, h_r), wt = maps.size, maps.t_width
+    if max(w_r, h_r, wt, H, W) > 32767:
+        raise ValueError(f"{name}: crop {w_r}x{h_r}, restored width {wt} or image {W}x{H} exceeds 32767 pixels "
+                         f"(OpenCV's warp holds source coordinates as int16)")
+    out = quad_footprint_box(maps, scale, (scale * H, scale * W))
+    n = maps.page_map
+    corners = [] if out is None else [(x, y) for x in (out[0], out[2] - 1) for y in (out[1], out[3] - 1)]
+    dens = [n[2][0] * x + n[2][1] * y + n[2][2] for x, y in corners]
+    if out is None or not min(dens) > 0:
+        raise ValueError(f"{name}: the page map's denominator is not positive over the footprint box {out}")
+    reach = max(abs(n[r][0] * x + n[r][1] * y + n[r][2]) for r in range(2) for x, y in corners)
+    if 32 * reach / min(dens) >= 2.0 ** 30:
+        raise ValueError(f"{name}: the map onto its {out} output box exceeds OpenCV's 32-bit fixed-point coordinates")
+    xs, ys = [p[0] for p in pts], [p[1] for p in pts]
+    rect = (max(0, math.floor(min(xs))), max(0, math.floor(min(ys))), min(W, math.ceil(max(xs))), min(H, math.ceil(max(ys))))
+    return maps, rect, out
+
+
 def _per_image(v, n, what):
     v = [None] * n if v is None else list(v)
     if len(v) != n:
@@ -1045,7 +1188,10 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
     empty or leaves the image, an oriented region with corners that are not finite, a side shorter than 1 pixel, mirrored or
     sheared past |e x f| < |e| |f| / 2, its centre outside the image, a crop, restored width or image side over 32767 pixels or
     a page map beyond OpenCV's fixed-point range, a label / box count mismatch, boxes without labels, a box outside the region's
-    columns ([x0, x1] for a rectangle, [0, w_r] for an oriented region)."""
+    columns ([x0, x1] for a rectangle, [0, w_r] for an oriented region).  QuadRegions are validated likewise (DESIGN.md 7b,
+    "Perspective text regions"): corners not finite, a side shorter than 1 pixel, not strictly convex in reading order, an
+    interior angle outside [30, 150] degrees, foreshortening beyond 4, the centre outside the image, a side over 32767 pixels,
+    a page map whose denominator is not positive over the footprint box or whose fixed-point coordinates leave +-2^30."""
     if isinstance(scale, bool) or not isinstance(scale, int) or not 1 <= scale <= 8:
         raise ValueError(f"scale must be an integer in [1, 8], got {scale!r}")
     if feather is not None and (isinstance(feather, bool) or not isinstance(feather, int) or feather < 0):
@@ -1065,6 +1211,9 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
             maps = None
             if isinstance(rect, OrientedRegion):
                 maps, (x0, y0, x1, y1), out = _plan_oriented(rect, H, W, s, name)
+                cols = (0, maps.size[0])
+            elif isinstance(rect, QuadRegion):
+                maps, (x0, y0, x1, y1), out = _plan_quad(rect, H, W, s, name)
                 cols = (0, maps.size[0])
             else:
                 try:
@@ -1093,7 +1242,11 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
                 bx = [[float(b[0]) - dx, float(b[1]) - dy, float(b[2]) - dx, float(b[3]) - dy] for b in bx]
             overlaps = [first + j for j, q in enumerate(plan[first:]) if max(out[0], q.out[0]) < min(out[2], q.out[2])
                         and max(out[1], q.out[1]) < min(out[3], q.out[3])]
-            extra = (OrientedRegion(*((float(p[0]), float(p[1])) for p in rect)), maps.matrix, maps.size) if maps else ()
+            corners = tuple((float(p[0]), float(p[1])) for p in rect) if maps else ()
+            if isinstance(rect, QuadRegion):
+                extra = (None, maps.matrix, maps.size, QuadRegion(*corners))
+            else:
+                extra = (OrientedRegion(*corners), maps.matrix, maps.size) if maps else ()
             plan.append(RegionPlan(i, r, (x0, y0, x1, y1), out, overlaps, lab, bx, *extra))
     return plan
 
@@ -1151,7 +1304,10 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     C = cv2.warpAffine(img, M, (w_r, h_r), INTER_CUBIC | WARP_INVERSE_MAP, BORDER_REPLICATE) (oriented_maps; every crop of the
     call in one mn_warp_affine_u8_batched launch), its labels and boxes given and returned in C's frame, and its entry gains
     ``matrix`` (M) and ``size`` ((w_r, h_r)).  Its T is warped back by N onto its footprint with a feather on all four sides, and
-    a call that holds one composes every region with mn_composite_regions_affine_u8 instead of mn_composite_regions_u8."""
+    a call that holds one composes every region with mn_composite_regions_affine_u8 instead of mn_composite_regions_u8.
+    A QuadRegion (DESIGN.md 7b, "Perspective text regions") is handled alike through quad_maps: C = cv2.warpPerspective(img, M,
+    (w_r, h_r), INTER_CUBIC | WARP_INVERSE_MAP, BORDER_REPLICATE) (every quad of the call in one mn_warp_perspective_u8_batched
+    launch), T warped back by the 3 x 3 N, and a call that holds one composes every region with mn_composite_regions_quad_u8."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     plan = plan_regions([im.shape[:2] for im in imgs], regions, labels, boxes, scale, feather)
@@ -1163,14 +1319,18 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         dimg = _device_images(range(len(imgs)), imgs, dev)
         crops = [dimg[p.image][p.rect[1]:p.rect[3], p.rect[0]:p.rect[2]] for p in plan]
         oriented = [k for k, p in enumerate(plan) if p.oriented is not None]
-        if oriented:                                     # every oriented region rectified in one launch
-            n_crop = [3 * plan[k].size[0] * plan[k].size[1] for k in oriented]
+        quads = [k for k, p in enumerate(plan) if p.quad is not None]
+        if oriented or quads:                            # every region of a kind rectified in one launch
+            n_crop = [3 * plan[k].size[0] * plan[k].size[1] for k in oriented + quads]
             cbuf = torch.empty(sum(n_crop), dtype=torch.uint8, device=dev)
             o = 0
-            for k, nb in zip(oriented, n_crop):
+            for k, nb in zip(oriented + quads, n_crop):
                 crops[k] = cbuf[o:o + nb].view(plan[k].size[1], plan[k].size[0], 3)
                 o += nb
-            ops.warp_affine([(dimg[plan[k].image], crops[k], plan[k].matrix) for k in oriented])
+            if oriented:
+                ops.warp_affine([(dimg[plan[k].image], crops[k], plan[k].matrix) for k in oriented])
+            if quads:
+                ops.warp_perspective([(dimg[plan[k].image], crops[k], plan[k].matrix) for k in quads])
         res = restore_images(encoder, tspgan, sr, crops, [p.labels for p in plan], [p.boxes for p in plan], max_lines=max_lines,
                              context=context, skip_invalid=skip_invalid, whole_lines=whole_lines, overlap=overlap) if plan else []
         sizes = [scale * scale * im.shape[0] * im.shape[1] * 3 for im in imgs]
@@ -1181,7 +1341,12 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         ok = [k for k, r in enumerate(res) if "error" not in r]
         if ok:
             items = [(pages[plan[k].image], res[k]["sr_u8"], plan[k].out, chain) for k, chain in zip(ok, region_chains(plan, ok))]
-            if oriented:
+            if quads:
+                maps = [quad_maps(plan[k].quad, scale, res[k]["sr_u8"].shape[1]) if plan[k].quad is not None else
+                        oriented_maps(plan[k].oriented, scale, res[k]["sr_u8"].shape[1]) if plan[k].oriented is not None else None
+                        for k in ok]
+                ops.composite_regions_quad([it + (m and (m.page_map, m.kx, m.ky),) for it, m in zip(items, maps)], feather)
+            elif oriented:
                 maps = [None if plan[k].oriented is None else oriented_maps(plan[k].oriented, scale, res[k]["sr_u8"].shape[1])
                         for k in ok]
                 ops.composite_regions_affine([it + (m and (m.page_map, m.kx, m.ky),) for it, m in zip(items, maps)], feather)
@@ -1198,12 +1363,12 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         if "error" in r:
             entry = dict(error=r["error"])
         elif "boxes" in r:
-            x0, y0 = (0, 0) if p.oriented else p.rect[:2]
+            x0, y0 = (0, 0) if p.oriented or p.quad else p.rect[:2]
             entry = dict(sr_u8=srs[k], segments=r["segments"], labels=r["labels"],
                          boxes=[[b[0] + x0, b[1] + y0, b[2] + x0, b[3] + y0] for b in r["boxes"]])
         else:
             entry = dict(sr_u8=srs[k], segments=r["segments"], labels=p.labels, boxes=boxes[p.image][p.region])
-        if p.oriented and "error" not in r:
+        if (p.oriented or p.quad) and "error" not in r:
             entry.update(matrix=p.matrix.copy(), size=p.size)
         out[p.image]["regions"].append(entry)
     return out

@@ -4,6 +4,7 @@ the pages, then cv2's cubic resize of every page and of every restored region (I
 (oracle/regions.py).
 
     MN_MODULE_GRAPHS=0 python tools/bench_regions.py [--pages 8] [--lines 12] [--passes 3] [--scale 4] [--max-angle 0]
+                                                     [--perspective 0]
 
 The pages are seeded: tools/bench_images.make_image_set lines (the reference test set's sizes and lines 2 to 4 times wider than the
 LQ canvas) pasted one under another onto a noise background, each line a region with its character boxes.  The arms alternate pass
@@ -17,6 +18,12 @@ With --max-angle DEG > 0 every line is pasted turned by a seeded angle in [-DEG,
 restore_images(to_host=True) on the crops, resizes the pages with cv2, warps each restored line back with cv2.warpAffine and
 blends it over its footprint with the numpy feather (oracle/oriented_regions.py); the timed kernels are mn_warp_affine_u8_batched,
 mn_resize_cubic_u8_batched and mn_composite_regions_affine_u8.
+
+With --perspective K > 1 every line is pasted seen in perspective: its far (right) end shrunk by a seeded foreshortening ratio in
+[1, K] and given as a pipeline.QuadRegion (DESIGN.md section 7b, "Perspective text regions").  The host arm then rectifies each
+line with cv2.warpPerspective, runs restore_images(to_host=True) on the crops, resizes the pages with cv2, warps each restored line
+back with cv2.warpPerspective and blends it over its footprint with the numpy feather (oracle/quad_regions.py); the timed kernels
+are mn_warp_perspective_u8_batched, mn_resize_cubic_u8_batched and mn_composite_regions_quad_u8.
 """
 import argparse
 import json
@@ -101,6 +108,76 @@ def make_rotated_pages(n_pages, n_lines, max_angle, seed=0):
     return pages, regs, labs, bxs
 
 
+def make_perspective_pages(n_pages, n_lines, max_ratio, seed=0):
+    """make_pages' lines, each seen in perspective -- its right side shrunk about its middle by a seeded ratio in [1, max_ratio] --
+    and pasted (nearest pixel, resized to its rectified crop's size) one under another onto a noise page: (pages, regions,
+    labels, boxes), regions QuadRegions and boxes in each line's rectified frame."""
+    import cv2
+    from bench_images import make_image_set
+    from marconet_b200.pipeline import QuadRegion, quad_maps
+    images, labels, boxes = make_image_set(n_pages * n_lines, seed)
+    rng = np.random.default_rng(seed + 1)
+    pages, regs, labs, bxs = [], [], [], []
+    for p in range(n_pages):
+        idx = range(p * n_lines, (p + 1) * n_lines)
+        ratios = rng.uniform(1, max_ratio, n_lines)
+        W = max(images[i].shape[1] for i in idx) + 24
+        H = sum(images[i].shape[0] + 8 for i in idx) + 8
+        page = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
+        rr, bb, y = [], [], 8
+        for i, k in zip(idx, ratios):
+            h, w = images[i].shape[:2]
+            d = (h - h / k) / 2
+            reg = QuadRegion((8, y), (8 + w, y + d), (8 + w, y + h - d), (8, y + h))
+            qm = quad_maps(reg, 1)
+            (w_r, h_r), m = qm.size, qm.matrix
+            line = cv2.resize(images[i], qm.size, interpolation=cv2.INTER_NEAREST)
+            warped = cv2.warpPerspective(line, m, (W, H), flags=cv2.INTER_NEAREST)
+            inside = cv2.warpPerspective(np.ones((h_r, w_r), np.uint8), m, (W, H), flags=cv2.INTER_NEAREST).astype(bool)
+            page[inside] = warped[inside]
+            fx, fy = w_r / w, h_r / h
+            bb.append([[min(b[0] * fx, w_r), b[1] * fy, min(b[2] * fx, w_r), b[3] * fy] for b in boxes[i]])
+            rr.append(reg)
+            y += h + 8
+        pages.append(page)
+        regs.append(rr)
+        labs.append([labels[i] for i in idx])
+        bxs.append(bb)
+    return pages, regs, labs, bxs
+
+
+def host_path_perspective(m, pages, regs, labels, boxes, s, feather, max_lines):
+    """cv2 rectify, restore_images on the crops, cv2 background and cv2 warp of each restored line back (onto the rows and
+    columns up to its footprint's far corner: at least 64 columns and 16 rows, so that cv2's 64-column blocks start where the
+    whole page's do), the numpy blend."""
+    import cv2
+    from marconet_b200 import pipeline
+    from oracle import quad_regions as regions
+    flags = cv2.INTER_CUBIC | cv2.WARP_INVERSE_MAP
+    crops, labs, bxs = [], [], []
+    for pg, rr, ll, bb in zip(pages, regs, labels, boxes):
+        for reg, lab, bx in zip(rr, ll, bb):
+            mp = pipeline.quad_maps(reg, 1)
+            crops.append(cv2.warpPerspective(pg, mp.matrix, mp.size, flags=flags, borderMode=cv2.BORDER_REPLICATE))
+            labs.append(lab)
+            bxs.append(bx)
+    res = pipeline.restore_images(*m, crops, labs, bxs, max_lines=max_lines, to_host=True)
+    out, k = [], 0
+    for pg, rr in zip(pages, regs):
+        o = cv2.resize(pg, (0, 0), fx=s, fy=s, interpolation=cv2.INTER_CUBIC)
+        for reg in rr:
+            t = res[k]["sr_u8"]
+            (x0, y0, x1, y1), _, _, mask, a = regions.quad_footprint(t.shape, reg, s, o.shape[:2], feather)
+            n = pipeline.quad_maps(reg, s, t.shape[1]).page_map
+            dw, dh = max(x1, 64), max(y1, 16)
+            p = cv2.warpPerspective(np.ascontiguousarray(t[..., ::-1]), n, (dw, dh), flags=flags, borderMode=cv2.BORDER_REPLICATE)
+            sl = o[y0:y1, x0:x1]
+            sl[mask] = regions.blend(sl, p[y0:y1, x0:x1], a)[mask]
+            k += 1
+        out.append(o)
+    return out
+
+
 def host_path_oriented(m, pages, regs, labels, boxes, s, feather, max_lines):
     """cv2 rectify, restore_images on the crops, cv2 background and cv2 warp of each restored line back (onto the rows and
     columns up to its footprint's far corner, so that its fixed-point coordinates are the whole page's), the numpy blend."""
@@ -172,7 +249,11 @@ def main():
     ap.add_argument("--scale", type=int, default=4)
     ap.add_argument("--max-lines", type=int, default=8)
     ap.add_argument("--max-angle", type=float, default=0.0, help="turn every line by up to this many degrees (oriented regions)")
+    ap.add_argument("--perspective", type=float, default=0.0,
+                    help="shrink every line's far end by a foreshortening ratio up to this (> 1; perspective regions)")
     args = ap.parse_args()
+    if args.perspective and (args.max_angle > 0 or not 1 < args.perspective <= 4):
+        sys.exit("--perspective takes a ratio in (1, 4] and does not combine with --max-angle")
     if not torch.cuda.is_available():
         sys.exit("bench_regions.py needs a CUDA device")
     cv2.ipp.setUseIPP(False)
@@ -186,16 +267,22 @@ def main():
         net = cls()
         net.load_state_dict(sds[key], strict=True)
         m.append(net.eval().to(dev))
-    oriented = args.max_angle > 0
-    if oriented:
+    oriented, perspective = args.max_angle > 0, args.perspective > 1
+    if perspective:
+        pages, rects, labels, boxes = make_perspective_pages(args.pages, args.lines, args.perspective)
+    elif oriented:
         pages, rects, labels, boxes = make_rotated_pages(args.pages, args.lines, args.max_angle)
     else:
         pages, rects, labels, boxes = make_pages(args.pages, args.lines)
     s, feather = args.scale, 2 * args.scale
 
     lib = _lib.load()
-    events = {"mn_warp_affine_u8_batched": [], "mn_resize_cubic_u8_batched": [], "mn_composite_regions_affine_u8": []} \
-        if oriented else {"mn_resize_cubic_u8_batched": [], "mn_composite_regions_u8": []}
+    if perspective:
+        events = {"mn_warp_perspective_u8_batched": [], "mn_resize_cubic_u8_batched": [], "mn_composite_regions_quad_u8": []}
+    elif oriented:
+        events = {"mn_warp_affine_u8_batched": [], "mn_resize_cubic_u8_batched": [], "mn_composite_regions_affine_u8": []}
+    else:
+        events = {"mn_resize_cubic_u8_batched": [], "mn_composite_regions_u8": []}
     timing = [False]
     for name in events:
         fn = getattr(lib, name)
@@ -217,7 +304,8 @@ def main():
         return [o["image"] for o in out]
 
     def host():
-        return (host_path_oriented if oriented else host_path)(m, pages, rects, labels, boxes, s, feather, args.max_lines)
+        path = host_path_perspective if perspective else host_path_oriented if oriented else host_path
+        return path(m, pages, rects, labels, boxes, s, feather, args.max_lines)
 
     arms = {"restore_regions": api, "host_path": host}
     outs = {name: fn() for name, fn in arms.items()}                 # warm-up pass of each arm
@@ -237,7 +325,7 @@ def main():
     card = _card()
     out_px = sum(s * s * p.shape[0] * p.shape[1] for p in pages)
     common = dict(pages=args.pages, lines_per_page=args.lines, scale=s, feather=feather, max_lines=args.max_lines,
-                  max_angle=args.max_angle,
+                  max_angle=args.max_angle, **({"perspective": args.perspective} if perspective else {}),
                   page_sizes=[list(p.shape[:2]) for p in pages], output_megapixels=round(out_px / 1e6, 2),
                   module_graphs=os.environ.get("MN_MODULE_GRAPHS"), same_bytes=same, max_abs_diff=diff, **card)
     for name, ts in times.items():
