@@ -594,6 +594,29 @@ typedef struct {
 } mn_region_quad;
 int mn_composite_regions_quad_u8(const mn_region_quad* regions, int n, long long max_pixels, void* stream);
 
+/* Vertical text columns (DESIGN.md section 7b, "Vertical text columns").  Two integer gathers of 3-byte pixels, each over every
+ * column of a call in one launch, blockIdx.y = column, one thread per destination pixel of its [dh][dw][3] destination, those
+ * past its dh*dw pixels exit.  Byte offsets are 64-bit; max_pixels >= every dh*dw.  cells points at n_cells records of
+ * int32 values built on the host; clamp(v, lo, hi) = min(max(v, lo), hi).  columns: DEVICE array of records whose cell tables
+ * point into device memory (validated by the caller: every pixel read lies inside src).
+ * mn_vertical_layout_u8_batched: src = the column crop C [h_r][w][3], dst = its line L [H_L][n_cells w][3], cells 3 per cell
+ * (c_k, p_k, t_k): L[i][k w + j] = C[c_k + clamp(i - p_k, 0, t_k - 1)][j].
+ * mn_vertical_unlayout_u8_batched: src = the restored line T [128][W_T][3], dst = the restored column T_col [H_c][W_c][3],
+ * cells 5 per cell (R(c_k), R(p_k), R(p_k + t_k), R(k w_r), min(R((k+1) w_r), W_T)), R(0) = 0: row i belongs to the last cell k
+ * with R(c_k) <= i, and T_col[i][j] = T[clamp(R(p_k) + i - R(c_k), R(p_k), R(p_k + t_k) - 1)]
+ * [clamp(R(k w_r) + j, R(k w_r), min(R((k+1) w_r), W_T) - 1)]; w is unused. */
+typedef struct {
+    const uint8_t* src;         /* row 0 of the source: C (layout) or T (unlayout) */
+    int64_t src_pitch;
+    uint8_t* dst;               /* row 0 of the destination: L (layout) or T_col (unlayout) */
+    int64_t dst_pitch;
+    const int32_t* cells;       /* the column's cell table */
+    int32_t dh, dw;
+    int32_t n_cells, w;         /* w: the column's width w_r (layout) */
+} mn_vertical_column;
+int mn_vertical_layout_u8_batched(const mn_vertical_column* columns, int n, long long max_pixels, void* stream);
+int mn_vertical_unlayout_u8_batched(const mn_vertical_column* columns, int n, long long max_pixels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

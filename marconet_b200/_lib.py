@@ -134,6 +134,11 @@ class RegionQuad(Structure):
     _fields_ = [("r", Region), ("kind", c_int32), ("kx", c_float), ("ky", c_float), ("pad", c_int32), ("n", c_double * 9)]
 
 
+class VerticalColumn(Structure):
+    _fields_ = [("src", c_void_p), ("src_pitch", c_int64), ("dst", c_void_p), ("dst_pitch", c_int64), ("cells", c_void_p),
+                ("dh", c_int32), ("dw", c_int32), ("n_cells", c_int32), ("w", c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -189,6 +194,8 @@ SYMBOLS = {
     "mn_composite_regions_affine_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_warp_perspective_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
     "mn_composite_regions_quad_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
+    "mn_vertical_layout_u8_batched": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
+    "mn_vertical_unlayout_u8_batched": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -471,7 +471,58 @@ __global__ void warp_perspective_batched_kernel(const mn_warp_perspective_image*
     for (int c = 0; c < cn; ++c) o[c] = (uint8_t)warp_cubic_u8(im.src, im.src_pitch, im.h, im.w, cn, c, wc, wt);
 }
 
+// blockIdx.y = column; one thread per destination pixel of its [dh][dw][3] destination, those past its dh*dw pixels exit.
+// kUnlayout false: the layout of C into the line L, the cell picked by the destination column; true: the inverse layout of T
+// into T_col, the cell picked by the destination row (the last k with R(c_k) <= y, a binary search over the table).
+template <bool kUnlayout>
+__global__ void vertical_gather_kernel(const mn_vertical_column* __restrict__ columns) {
+    mn_pdl_prologue();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const mn_vertical_column col = columns[blockIdx.y];
+    if (idx >= (long long)col.dh * col.dw) return;
+    const int x = (int)(idx % col.dw), y = (int)(idx / col.dw);
+    int sy, sx;
+    if (!kUnlayout) {
+        const int k = x / col.w;
+        const int* t = col.cells + 3 * k;
+        sy = t[0] + min(max(y - t[1], 0), t[2] - 1);
+        sx = x - k * col.w;
+    } else {
+        int lo = 0, hi = col.n_cells - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (col.cells[5 * mid] <= y) lo = mid; else hi = mid - 1;
+        }
+        const int* t = col.cells + 5 * lo;
+        sy = min(max(t[1] + y - t[0], t[1]), t[2] - 1);
+        sx = min(max(t[3] + x, t[3]), t[4] - 1);
+    }
+    const uint8_t* s = col.src + (long long)sy * col.src_pitch + (long long)sx * 3;
+    uint8_t* o = col.dst + (long long)y * col.dst_pitch + (long long)x * 3;
+    o[0] = s[0];
+    o[1] = s[1];
+    o[2] = s[2];
+}
+
 }  // namespace
+
+template <bool kUnlayout>
+static int vertical_gather(const mn_vertical_column* columns, int n, long long max_pixels, void* stream, const char* what) {
+    MN_REQUIRE(columns && n > 0 && n <= 65535 && max_pixels > 0, "%s: bad args", what);
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "%s: %lld pixels exceed the grid", what, max_pixels);
+    MN_CUDA_CHECK((mn_launch(vertical_gather_kernel<kUnlayout>, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
+                             (cudaStream_t)stream, columns)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_vertical_layout_u8_batched(const mn_vertical_column* columns, int n, long long max_pixels, void* stream) {
+    return vertical_gather<false>(columns, n, max_pixels, stream, "mn_vertical_layout_u8_batched");
+}
+
+extern "C" int mn_vertical_unlayout_u8_batched(const mn_vertical_column* columns, int n, long long max_pixels, void* stream) {
+    return vertical_gather<true>(columns, n, max_pixels, stream, "mn_vertical_unlayout_u8_batched");
+}
 
 extern "C" int mn_resize_cubic_u8_batched(const mn_resize_image* images, int n, int cn, long long max_pixels, void* stream) {
     MN_REQUIRE(images && n > 0 && n <= 65535 && cn > 0 && cn <= 4 && max_pixels > 0, "mn_resize_cubic_u8_batched: bad args");

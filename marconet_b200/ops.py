@@ -1352,3 +1352,61 @@ def composite_regions_quad(regions, feather):
     _upload_records(buf, out, chains)
     _lib.check(_lib.load().mn_composite_regions_quad_u8(_ptr(buf), len(out), mx, _stream()), "mn_composite_regions_quad_u8")
     LAUNCHES += 1
+
+
+def _vertical_gather(items, what, width, symbol):
+    """One launch of ``symbol`` over vertical_layout's / vertical_unlayout's items, ``width`` int32 values per cell."""
+    import numpy as np
+    global LAUNCHES
+    if not items:
+        raise ValueError(f"{what}: no columns")
+    if len(items) > 65535:
+        raise ValueError(f"{what}: at most 65535 columns per launch")
+    dev = items[0][0].device
+    tables = []
+    for i, (src, dst, cells) in enumerate(items):
+        _dense_u8(src, dev, 3, f"{what}: column {i}: src")
+        _dense_u8(dst, dev, 3, f"{what}: column {i}: dst")
+        t = np.asarray(cells, dtype=np.int64).reshape(-1, width)
+        (sh, sw), (dh, dw) = src.shape[:2], dst.shape[:2]
+        if width == 3:                                   # (c_k, p_k, t_k): rows [c_k, c_k + t_k) of C, columns [0, w)
+            ok = len(t) >= 1 and dw % len(t) == 0 and dw // len(t) <= sw and (t[:, 2] >= 1).all() and (t[:, 0] >= 0).all() \
+                and (t[:, 0] + t[:, 2] <= sh).all()
+        else:                                            # rows [min(R(p), R(p+t) - 1), R(p+t)), columns [min(lo, hi - 1), hi)
+            ok = len(t) >= 1 and t[0, 0] == 0 and (np.diff(t[:, 0]) >= 0).all() and (t[:, 2] <= sh).all() \
+                and (np.minimum(t[:, 1], t[:, 2] - 1) >= 0).all() and (t[:, 4] <= sw).all() \
+                and (np.minimum(t[:, 3], t[:, 4] - 1) >= 0).all()
+        if not ok or t.max() >= 2 ** 31:
+            raise ValueError(f"{what}: column {i}: its cell table reads outside the {sh}x{sw} source")
+        tables.append(t.astype(np.int32))
+    isz = ctypes.sizeof(_lib.VerticalColumn)
+    n_int = sum(t.size for t in tables)
+    buf = torch.empty(len(items) * isz + 4 * n_int, dtype=torch.uint8, device=dev)
+    base, o, recs, mx = buf.data_ptr() + len(items) * isz, 0, [], 0
+    for (src, dst, _), t in zip(items, tables):
+        dh, dw = dst.shape[:2]
+        recs.append(_lib.VerticalColumn(src.data_ptr(), src.stride(0), dst.data_ptr(), dst.stride(0), base + 4 * o, dh, dw, len(t),
+                                        dw // len(t) if width == 3 else 0))
+        o += t.size
+        mx = max(mx, dh * dw)
+    host = bytes((_lib.VerticalColumn * len(recs))(*recs)) + b"".join(t.tobytes() for t in tables)
+    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    _lib.check(getattr(_lib.load(), symbol)(_ptr(buf), len(recs), mx, _stream()), symbol)
+    LAUNCHES += 1
+
+
+def vertical_layout(items):
+    """Vertical text columns laid out as horizontal lines, every column in one launch (mn_vertical_layout_u8_batched; DESIGN.md
+    7b, "Vertical text columns").  items: list of (C, L, cells): uint8 [h_r, w_r, 3] and [H_L, n w_r, 3] CUDA views with dense
+    pixels (any row stride; C may be read in place through a page's pitch), cells the n (c_k, p_k, t_k) of
+    pipeline.vertical_plan: L[i, k w_r + j] = C[c_k + clamp(i - p_k, 0, t_k - 1), j]."""
+    _vertical_gather(items, "vertical_layout", 3, "mn_vertical_layout_u8_batched")
+
+
+def vertical_unlayout(items):
+    """Restored lines put back into columns, every column in one launch (mn_vertical_unlayout_u8_batched; DESIGN.md 7b,
+    "Vertical text columns").  items: list of (T, T_col, cells): uint8 [128, W_T, 3] and [H_c, W_c, 3] CUDA views with dense
+    pixels (T read in place through its pitch), cells the n (R(c_k), R(p_k), R(p_k + t_k), R(k w_r), min(R((k+1) w_r), W_T)) of
+    pipeline.unlayout_cells.  Row i of T_col belongs to the last cell k with R(c_k) <= i and reads T at row
+    clamp(R(p_k) + i - R(c_k), R(p_k), R(p_k + t_k) - 1), column clamp(R(k w_r) + j, R(k w_r), min(R((k+1) w_r), W_T) - 1)."""
+    _vertical_gather(items, "vertical_unlayout", 5, "mn_vertical_unlayout_u8_batched")

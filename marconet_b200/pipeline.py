@@ -7,6 +7,7 @@ boxes converted from the encoder's (left, right) pairs to (centre, half-width) e
 predict_characters decodes them, and the boxes, on the device (mn_decode_predictions) for images of any width.  Everything
 numeric runs through the module API (and therefore through the CUDA kernels).
 """
+import itertools
 import math
 import threading
 from typing import NamedTuple
@@ -904,7 +905,9 @@ class RegionPlan(NamedTuple):
     OrientedRegion), ``matrix`` (M, its rectified crop's map) and ``size`` ((w_r, h_r), the crop's size); its ``rect`` is the
     bounding box of its corners in source pixels clipped to the image, ``out`` the bounding box of its footprint in output pixels,
     ``overlaps`` compares the ``out`` boxes, and its boxes are in the crop's frame, unshifted.  A perspective region (DESIGN.md
-    7b, "Perspective text regions") has ``quad`` (the QuadRegion) instead of ``oriented``, and ``matrix`` is its 3 x 3 M."""
+    7b, "Perspective text regions") has ``quad`` (the QuadRegion) instead of ``oriented``, and ``matrix`` is its 3 x 3 M.  A
+    vertical column (DESIGN.md 7b, "Vertical text columns") is planned as its shape, with ``out`` sized for its restored column,
+    and has ``vertical`` (its VerticalPlan); its ``boxes`` are the given boxes moved onto the line L."""
     image: int
     region: int
     rect: tuple
@@ -916,6 +919,7 @@ class RegionPlan(NamedTuple):
     matrix: object = None
     size: tuple = None
     quad: tuple = None
+    vertical: tuple = None
 
 
 class OrientedRegion(NamedTuple):
@@ -948,14 +952,15 @@ class OrientedMaps(NamedTuple):
     t_width: int
 
 
-def oriented_maps(region, scale, t_width=None):
+def oriented_maps(region, scale, t_width=None, t_height=128):
     """The fp64 maps of an OrientedRegion (DESIGN.md 7b, "Oriented text regions"), computed here once for the kernels and the
     numpy twin alike.  w_r = round_half_even(|e|), h_r = round_half_even(|f|);
       M = [[ex/w_r, fx/h_r, tlx + 0.5 ex/w_r + 0.5 fx/h_r - 0.5], [ey/w_r, fy/h_r, tly + 0.5 ey/w_r + 0.5 fy/h_r - 0.5]];
-    N takes output pixel (X, Y) at scale s to T's pixel indices (a W_T - 0.5, 128 b - 0.5), where ((X + 0.5)/s, (Y + 0.5)/s) - tl
-    = a e + b f; kx = fl32(s |e x f| / (|f| W_T)), ky = fl32(s |e x f| / (128 |e|)).  W_T (``t_width``) defaults to
+    N takes output pixel (X, Y) at scale s to T's pixel indices (a W_T - 0.5, H_T b - 0.5), where ((X + 0.5)/s, (Y + 0.5)/s) - tl
+    = a e + b f; kx = fl32(s |e x f| / (|f| W_T)), ky = fl32(s |e x f| / (H_T |e|)).  W_T (``t_width``) defaults to
     round_half_even(w_r 128 / h_r), the width restore_images gives a line that fits its canvas; pass T's own width otherwise.
-    For integer axis-aligned corners M = [[1, 0, x0], [0, 1, y0]] exactly."""
+    H_T (``t_height``) is 128, restore_images' height, except for a vertical column's restored T_col (DESIGN.md 7b, "Vertical
+    text columns").  For integer axis-aligned corners M = [[1, 0, x0], [0, 1, y0]] exactly."""
     import numpy as np
     from .ops import round_half_even
     (tlx, tly), (trx, try_), (blx, bly) = ((float(p[0]), float(p[1])) for p in region)
@@ -965,22 +970,22 @@ def oriented_maps(region, scale, t_width=None):
     a, b, c, d = ex / w_r, fx / h_r, ey / w_r, fy / h_r
     m = np.array([[a, b, tlx + 0.5 * a + 0.5 * b - 0.5], [c, d, tly + 0.5 * c + 0.5 * d - 0.5]], np.float64)
     wt = round_half_even(w_r * (128 / h_r)) if t_width is None else int(t_width)
-    s, cross, h = scale, ex * fy - ey * fx, 0.5 / scale
+    s, cross, h, ht = scale, ex * fy - ey * fx, 0.5 / scale, t_height
     n = np.array([[wt * fy / (s * cross), -wt * fx / (s * cross), wt * (fy * (h - tlx) - fx * (h - tly)) / cross - 0.5],
-                  [-128 * ey / (s * cross), 128 * ex / (s * cross), 128 * (ex * (h - tly) - ey * (h - tlx)) / cross - 0.5]],
+                  [-ht * ey / (s * cross), ht * ex / (s * cross), ht * (ex * (h - tly) - ey * (h - tlx)) / cross - 0.5]],
                  np.float64)
     kx = float(np.float32(s * abs(cross) / (lf * wt)))
-    ky = float(np.float32(s * abs(cross) / (le * 128)))
+    ky = float(np.float32(s * abs(cross) / (le * ht)))
     return OrientedMaps(m, (w_r, h_r), n, kx, ky, wt)
 
 
-def footprint_box(region, maps, scale, page_hw):
+def footprint_box(region, maps, scale, page_hw, t_height=128):
     """(X0, Y0, X1, Y1): output pixels that hold every pixel of the region's footprint, on a page of page_hw = (H, W) output
     pixels.  The parallelogram is widened by one T pixel on every side (far more than the 1/32-pixel rounding of the fixed-point
-    coordinates) and each pixel whose centre it may cover is taken."""
+    coordinates) and each pixel whose centre it may cover is taken.  t_height: T's height, as oriented_maps took it."""
     (tlx, tly), (trx, try_), (blx, bly) = ((float(p[0]), float(p[1])) for p in region)
     ex, ey, fx, fy = trx - tlx, try_ - tly, blx - tlx, bly - tly
-    da, db = 1 / maps.t_width, 1 / 128
+    da, db = 1 / maps.t_width, 1 / t_height
     xs = [tlx + a * ex + b * fx for a in (-da, 1 + da) for b in (-db, 1 + db)]
     ys = [tly + a * ey + b * fy for a in (-da, 1 + da) for b in (-db, 1 + db)]
     s, (ph, pw) = scale, page_hw
@@ -995,8 +1000,9 @@ def _fixed_point_fits(m, box):
     return all(abs(r[0]) * x1 + max(abs(r[1] * y0 + r[2]), abs(r[1] * y1 + r[2])) < 2.0 ** 20 for r in m)
 
 
-def _plan_oriented(reg, H, W, scale, name):
-    """Validates an OrientedRegion of an H x W image: (maps, rect, out)."""
+def _plan_oriented(reg, H, W, scale, name, column=None):
+    """Validates an OrientedRegion of an H x W image: (maps, rect, out).  column: None, or for the shape of a VerticalRegion a
+    function of the crop's (w_r, h_r) that returns the column's restored size (W_c, H_c), which then sizes N and ``out``."""
     try:
         pts = [(float(p[0]), float(p[1])) for p in reg]
         if len(pts) != 3 or any(len(p) != 2 for p in reg):
@@ -1022,7 +1028,11 @@ def _plan_oriented(reg, H, W, scale, name):
     if max(w_r, h_r, wt, H, W) > 32767:
         raise ValueError(f"{name}: crop {w_r}x{h_r}, restored width {wt} or image {W}x{H} exceeds 32767 pixels "
                          f"(OpenCV's warp holds source coordinates as int16)")
-    out = footprint_box(pts, maps, scale, (scale * H, scale * W))
+    ht = 128
+    if column is not None:
+        wt, ht = column(w_r, h_r)
+        maps = oriented_maps(pts, scale, wt, ht)
+    out = footprint_box(pts, maps, scale, (scale * H, scale * W), ht)
     if not _fixed_point_fits(maps.page_map, out):
         raise ValueError(f"{name}: the map onto its {out} output box exceeds OpenCV's 32-bit fixed-point coordinates")
     xs, ys = (tlx, trx, blx, trx + fx), (tly, try_, bly, try_ + fy)
@@ -1065,16 +1075,16 @@ def _quad_homography(pts):
     return (x1 - x0 + g * x1, x3 - x0 + h * x3, x0), (y1 - y0 + g * y1, y3 - y0 + h * y3, y0), (g, h, 1.0)
 
 
-def quad_maps(region, scale, t_width=None):
+def quad_maps(region, scale, t_width=None, t_height=128):
     """The fp64 maps of a QuadRegion (DESIGN.md 7b, "Perspective text regions"), computed here once in plain Python floats with a
     fixed operation order for the kernels and the numpy twin alike.  w_r = round_half_even(max(|tr - tl|, |br - bl|)),
     h_r = round_half_even(max(|bl - tl|, |br - tr|)); with H = [[a, b, c], [d, e, f], [g, h, 1]] the unit square -> quad
     homography, M's rows are [(a - 0.5 g)/w_r, (b - 0.5 h)/h_r, c - 0.5 + 0.5 (a - 0.5 g)/w_r + 0.5 (b - 0.5 h)/h_r], the same with
     d, e, f, and [g/w_r, h/h_r, 1 + 0.5 g/w_r + 0.5 h/h_r].  N = A_T adj(H) A_page, A_page = [[1/s, 0, 0.5/s], [0, 1/s, 0.5/s],
-    [0, 0, 1]], A_T = [[W_T, 0, -0.5], [0, 128, -0.5], [0, 0, 1]], all nine entries divided by its third row's value at the
-    footprint's centre (the page pixel of H(0.5, 0.5)).  kx = fl32(s A / (L_f W_T)), ky = fl32(s A / (L_e 128)): A the shoelace
+    [0, 0, 1]], A_T = [[W_T, 0, -0.5], [0, H_T, -0.5], [0, 0, 1]], all nine entries divided by its third row's value at the
+    footprint's centre (the page pixel of H(0.5, 0.5)).  kx = fl32(s A / (L_f W_T)), ky = fl32(s A / (L_e H_T)): A the shoelace
     area, L_e the mean of the top and bottom side lengths, L_f of the left and right ones.  W_T (``t_width``) defaults to
-    round_half_even(w_r 128 / h_r); pass T's own width otherwise.  For integer axis-aligned corners M = [[1, 0, x0], [0, 1, y0],
+    round_half_even(w_r 128 / h_r); pass T's own width otherwise.  H_T (``t_height``) is 128 except for a vertical column's T_col.  For integer axis-aligned corners M = [[1, 0, x0], [0, 1, y0],
     [0, 0, 1]] exactly, and at h = 32, s = 4, N = [[1, 0, -4 x0], [0, 1, -4 y0], [0, 0, 1]]."""
     import numpy as np
     from .ops import round_half_even
@@ -1093,7 +1103,7 @@ def quad_maps(region, scale, t_width=None):
     adj = ((e - f * h, c * h - b, b * f - c * e), (f * g - d, a - c * g, c * d - a * f), (d * h - e * g, b * g - a * h, a * e - b * d))
     hs = 0.5 / s
     k = [(r[0] / s, r[1] / s, r[0] * hs + r[1] * hs + r[2]) for r in adj]
-    n = [[wt * k[0][j] - 0.5 * k[2][j] for j in range(3)], [128 * k[1][j] - 0.5 * k[2][j] for j in range(3)], list(k[2])]
+    n = [[wt * k[0][j] - 0.5 * k[2][j] for j in range(3)], [t_height * k[1][j] - 0.5 * k[2][j] for j in range(3)], list(k[2])]
     cw = 0.5 * g + 0.5 * h + 1.0
     xc, yc = s * ((0.5 * a + 0.5 * b + c) / cw) - 0.5, s * ((0.5 * d + 0.5 * e + f) / cw) - 0.5
     den = n[2][0] * xc + n[2][1] * yc + n[2][2]
@@ -1101,16 +1111,17 @@ def quad_maps(region, scale, t_width=None):
     area = 0.5 * abs((x0 * y1 - x1 * y0) + (x1 * y2 - x2 * y1) + (x2 * y3 - x3 * y2) + (x3 * y0 - x0 * y3))
     l_e, l_f = 0.5 * (top + bottom), 0.5 * (left + right)
     kx = float(np.float32(s * area / (l_f * wt)))
-    ky = float(np.float32(s * area / (l_e * 128)))
+    ky = float(np.float32(s * area / (l_e * t_height)))
     return QuadMaps(m, (w_r, h_r), n, kx, ky, wt, hom)
 
 
-def quad_footprint_box(maps, scale, page_hw):
+def quad_footprint_box(maps, scale, page_hw, t_height=128):
     """(X0, Y0, X1, Y1): output pixels that hold every pixel of a quad's footprint, on a page of page_hw = (H, W) output pixels:
-    the images under H of the corners of [-1/W_T, 1 + 1/W_T] x [-1/128, 1 + 1/128] (the quad widened by one T pixel on every
-    side), each pixel whose centre their hull may cover.  None when H's denominator is not positive at one of those corners."""
+    the images under H of the corners of [-1/W_T, 1 + 1/W_T] x [-1/H_T, 1 + 1/H_T] (the quad widened by one T pixel on every
+    side; H_T = t_height, as quad_maps took it), each pixel whose centre their hull may cover.  None when H's denominator is not
+    positive at one of those corners."""
     (a, b, c), (d, e, f), (g, h, _) = maps.homography
-    da, db = 1 / maps.t_width, 1 / 128
+    da, db = 1 / maps.t_width, 1 / t_height
     xs, ys = [], []
     for u in (-da, 1 + da):
         for v in (-db, 1 + db):
@@ -1124,8 +1135,8 @@ def quad_footprint_box(maps, scale, page_hw):
             min(pw, math.ceil(s * max(xs) - 0.5) + 1), min(ph, math.ceil(s * max(ys) - 0.5) + 1))
 
 
-def _plan_quad(reg, H, W, scale, name):
-    """Validates a QuadRegion of an H x W image: (maps, rect, out)."""
+def _plan_quad(reg, H, W, scale, name, column=None):
+    """Validates a QuadRegion of an H x W image: (maps, rect, out); column as _plan_oriented takes it."""
     try:
         pts = [(float(p[0]), float(p[1])) for p in reg]
         if len(pts) != 4 or any(len(p) != 2 for p in reg):
@@ -1157,7 +1168,11 @@ def _plan_quad(reg, H, W, scale, name):
     if max(w_r, h_r, wt, H, W) > 32767:
         raise ValueError(f"{name}: crop {w_r}x{h_r}, restored width {wt} or image {W}x{H} exceeds 32767 pixels "
                          f"(OpenCV's warp holds source coordinates as int16)")
-    out = quad_footprint_box(maps, scale, (scale * H, scale * W))
+    ht = 128
+    if column is not None:
+        wt, ht = column(w_r, h_r)
+        maps = quad_maps(pts, scale, wt, ht)
+    out = quad_footprint_box(maps, scale, (scale * H, scale * W), ht)
     n = maps.page_map
     corners = [] if out is None else [(x, y) for x in (out[0], out[2] - 1) for y in (out[1], out[3] - 1)]
     dens = [n[2][0] * x + n[2][1] * y + n[2][2] for x, y in corners]
@@ -1169,6 +1184,110 @@ def _plan_quad(reg, H, W, scale, name):
     xs, ys = [p[0] for p in pts], [p[1] for p in pts]
     rect = (max(0, math.floor(min(xs))), max(0, math.floor(min(ys))), min(W, math.ceil(max(xs))), min(H, math.ceil(max(ys))))
     return maps, rect, out
+
+
+class VerticalRegion(NamedTuple):
+    """A column of upright characters read top to bottom (DESIGN.md 7b, "Vertical text columns").  ``shape`` is its footprint: an
+    integer rectangle (x0, y0, x1, y1), an OrientedRegion or a QuadRegion, with tl -> tr across the column and tl -> bl down it.
+    Its crop C (img[y0:y1, x0:x1], or the shape's rectified crop) is cut into character cells laid side by side as a horizontal
+    line, which is restored and put back into a column.  ``cells``: the number of equal cells when no boxes are given (default:
+    round_half_even(h_r / w_r), glyphs being about square)."""
+    shape: object
+    cells: object = None
+
+
+class VerticalPlan(NamedTuple):
+    """vertical_plan's result for a column crop C of ``size`` (w_r, h_r): ``cells`` the boundaries [c_0 = 0, ..., c_n = h_r],
+    ``heights`` t_k = c_{k+1} - c_k, ``line_height`` H_L = max t_k, ``pads`` p_k = (H_L - t_k) // 2, ``t_size`` (W_c, H_c) =
+    (R(w_r), R(h_r)), the restored column's size, and ``boxes`` the given boxes moved onto the line L [H_L, n w_r] (None when
+    they are predicted)."""
+    cells: list
+    size: tuple
+    heights: list
+    line_height: int
+    pads: list
+    t_size: tuple
+    boxes: list
+
+
+def vertical_r(y, line_height):
+    """R(y) = round_half_even(y (128 / H_L)): where row or column y of the line L lands in its restored line T (stitch_pieces'
+    r(x), so that R(n w_r) is T's width)."""
+    from .ops import round_half_even
+    return round_half_even(y * (128 / line_height))
+
+
+def vertical_plan(w_r, h_r, cells=None, boxes=None, name="column"):
+    """The cell plan of a w_r x h_r column crop (DESIGN.md 7b, "Vertical text columns"), in integers and fp64.  With boxes
+    [x1, y1, x2, y2] (C's frame, reading order), c_k = floor((y2_{k-1} + y1_k) / 2) for k = 1 .. n-1; else c_k = (k h_r) // n with
+    n = ``cells`` or clamp(round_half_even(h_r / w_r), 1, h_r).  Raises ValueError, naming ``name``: cells not an integer in
+    [1, h_r] or given with boxes, a box outside C, box centres that go up, boundaries not strictly increasing inside (0, h_r)
+    (these name the character), a
+    line n w_r or a restored size W_c, H_c or W_T = R(n w_r) over 32767 pixels."""
+    from .ops import round_half_even
+    if cells is not None and boxes is not None:
+        raise ValueError(f"{name}: cells and boxes are both given (boxes fix the cells)")
+    if boxes is not None:
+        bx = []
+        for k, b in enumerate(boxes):
+            b = [float(v) for v in b]
+            if len(b) != 4 or not (0 <= b[0] <= b[2] <= w_r and 0 <= b[1] <= b[3] <= h_r):
+                raise ValueError(f"{name}, character {k}: box {b} is outside the column crop [0, {w_r}] x [0, {h_r}]")
+            bx.append(b)
+        c = [0]
+        for k in range(1, len(bx)):
+            y, y0 = (bx[k][1] + bx[k][3]) / 2, (bx[k - 1][1] + bx[k - 1][3]) / 2
+            if y < y0:
+                raise ValueError(f"{name}, character {k}: the box's centre {y:g} lies above the previous character's {y0:g} "
+                                 f"(boxes are listed in reading order, down the column)")
+            c.append(math.floor((bx[k - 1][3] + bx[k][1]) / 2))
+            if not c[-2] < c[-1] < h_r:
+                raise ValueError(f"{name}, character {k}: the cell boundary {c[-1]} between it and the previous character is "
+                                 f"not strictly inside ({c[-2]}, {h_r})")
+        c.append(h_r)
+    else:
+        if cells is None:
+            n = min(max(round_half_even(h_r / w_r), 1), h_r)
+        elif isinstance(cells, bool) or not isinstance(cells, int) or not 1 <= cells <= h_r:
+            raise ValueError(f"{name}: cells must be an integer in [1, {h_r}] (the crop's rows), got {cells!r}")
+        else:
+            n = cells
+        c = [(k * h_r) // n for k in range(n + 1)]
+    n = len(c) - 1
+    t = [c[k + 1] - c[k] for k in range(n)]
+    hl = max(t)
+    p = [(hl - v) // 2 for v in t]
+    wc, hc, wt = vertical_r(w_r, hl), vertical_r(h_r, hl), vertical_r(n * w_r, hl)
+    if max(n * w_r, wc, hc, wt) > 32767:
+        raise ValueError(f"{name}: line width {n * w_r}, restored column {wc}x{hc} or restored line width {wt} exceeds 32767 pixels")
+    lb = None if boxes is None else [[k * w_r + b[0], p[k] + b[1] - c[k], k * w_r + b[2], p[k] + b[3] - c[k]]
+                                     for k, b in enumerate(bx)]
+    return VerticalPlan(c, (w_r, h_r), t, hl, p, (wc, hc), lb)
+
+
+def layout_cells(vp):
+    """ops.vertical_layout's table: (c_k, p_k, t_k) per cell."""
+    return [(vp.cells[k], vp.pads[k], vp.heights[k]) for k in range(len(vp.heights))]
+
+
+def unlayout_cells(vp, t_width):
+    """ops.vertical_unlayout's table for a restored line T of width W_T = t_width: (R(c_k), R(p_k), R(p_k + t_k), R(k w_r),
+    min(R((k+1) w_r), W_T)) per cell."""
+    hl, w = vp.line_height, vp.size[0]
+    return [(vertical_r(vp.cells[k], hl), vertical_r(vp.pads[k], hl), vertical_r(vp.pads[k] + vp.heights[k], hl),
+             vertical_r(k * w, hl), min(vertical_r((k + 1) * w, hl), t_width)) for k in range(len(vp.heights))]
+
+
+def column_boxes(vp, boxes):
+    """Boxes predicted on the line L -> the column crop C's frame, each through the cell that holds its centre: x - k w_r clipped
+    to [0, w_r], y - p_k + c_k clipped to [c_k, c_{k+1}]."""
+    w, n, out = vp.size[0], len(vp.heights), []
+    for b in boxes:
+        k = min(max(math.floor((b[0] + b[2]) / 2 / w), 0), n - 1)
+        lo, hi, dy = vp.cells[k], vp.cells[k + 1], vp.cells[k] - vp.pads[k]
+        out.append([min(max(b[0] - k * w, 0), w), min(max(b[1] + dy, lo), hi), min(max(b[2] - k * w, 0), w),
+                    min(max(b[3] + dy, lo), hi)])
+    return out
 
 
 def _per_image(v, n, what):
@@ -1191,7 +1310,9 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
     columns ([x0, x1] for a rectangle, [0, w_r] for an oriented region).  QuadRegions are validated likewise (DESIGN.md 7b,
     "Perspective text regions"): corners not finite, a side shorter than 1 pixel, not strictly convex in reading order, an
     interior angle outside [30, 150] degrees, foreshortening beyond 4, the centre outside the image, a side over 32767 pixels,
-    a page map whose denominator is not positive over the footprint box or whose fixed-point coordinates leave +-2^30."""
+    a page map whose denominator is not positive over the footprint box or whose fixed-point coordinates leave +-2^30.
+    A VerticalRegion (DESIGN.md 7b, "Vertical text columns") is validated as its shape, its labels and boxes in its crop C's frame,
+    and further rejected for a shape that is itself a VerticalRegion and for vertical_plan's errors."""
     if isinstance(scale, bool) or not isinstance(scale, int) or not 1 <= scale <= 8:
         raise ValueError(f"scale must be an integer in [1, 8], got {scale!r}")
     if feather is not None and (isinstance(feather, bool) or not isinstance(feather, int) or feather < 0):
@@ -1208,12 +1329,27 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
         s = scale
         for r, rect in enumerate(rects):
             name = f"image {i}, region {r}"
-            maps = None
+            maps, column, vplan = None, None, []
+            lab, bx = labs[r], bxs[r]
+            if isinstance(rect, VerticalRegion):
+                vreg, rect = rect, rect.shape
+                if isinstance(rect, VerticalRegion):
+                    raise ValueError(f"{name}: the shape of a VerticalRegion is itself a VerticalRegion")
+                if lab is not None:
+                    lab = [int(v) for v in torch.as_tensor(lab, dtype=torch.long).reshape(-1).tolist()]
+                if bx is not None and lab is None:
+                    raise ValueError(f"{name}: boxes without labels (predicted labels pair only with predicted boxes)")
+                if bx is not None and len(lab) != len(bx):
+                    raise ValueError(f"{name}: {len(lab)} labels for {len(bx)} boxes")
+
+                def column(w_r, h_r, _v=vreg, _bx=bx, _name=name, _out=vplan):
+                    _out.append(vertical_plan(w_r, h_r, _v.cells, _bx, _name))
+                    return _out[0].t_size
             if isinstance(rect, OrientedRegion):
-                maps, (x0, y0, x1, y1), out = _plan_oriented(rect, H, W, s, name)
+                maps, (x0, y0, x1, y1), out = _plan_oriented(rect, H, W, s, name, column)
                 cols = (0, maps.size[0])
             elif isinstance(rect, QuadRegion):
-                maps, (x0, y0, x1, y1), out = _plan_quad(rect, H, W, s, name)
+                maps, (x0, y0, x1, y1), out = _plan_quad(rect, H, W, s, name, column)
                 cols = (0, maps.size[0])
             else:
                 try:
@@ -1226,10 +1362,13 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
                 if not (0 <= x0 < x1 <= W and 0 <= y0 < y1 <= H):
                     raise ValueError(f"{name}: rectangle {(x0, y0, x1, y1)} is empty or outside the {W}x{H} image")
                 out, cols = (s * x0, s * y0, s * x1, s * y1), (x0, x1)
-            lab, bx = labs[r], bxs[r]
-            if lab is not None:
+                if column is not None:
+                    column(x1 - x0, y1 - y0)
+            if column is not None:
+                bx = vplan[0].boxes
+            elif lab is not None:
                 lab = [int(v) for v in torch.as_tensor(lab, dtype=torch.long).reshape(-1).tolist()]
-            if bx is not None:
+            if bx is not None and column is None:
                 if lab is None:
                     raise ValueError(f"{name}: boxes without labels (predicted labels pair only with predicted boxes)")
                 if len(lab) != len(bx):
@@ -1247,7 +1386,7 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
                 extra = (None, maps.matrix, maps.size, QuadRegion(*corners))
             else:
                 extra = (OrientedRegion(*corners), maps.matrix, maps.size) if maps else ()
-            plan.append(RegionPlan(i, r, (x0, y0, x1, y1), out, overlaps, lab, bx, *extra))
+            plan.append(RegionPlan(i, r, (x0, y0, x1, y1), out, overlaps, lab, bx, *extra, vertical=vplan[0] if vplan else None))
     return plan
 
 
@@ -1260,6 +1399,13 @@ def region_chains(plan, ok):
             later[j].append(k)
     index = {k: j for j, k in enumerate(ok)}
     return [[index[j] for j in plan[k].overlaps + [k] + later[k] if j in index] for k in ok]
+
+
+def _flat_views(shapes, dev):
+    """uint8 [h, w, 3] views, one per (h, w) of ``shapes``, packed in one device buffer."""
+    n = [3 * h * w for h, w in shapes]
+    buf = torch.empty(sum(n), dtype=torch.uint8, device=dev)
+    return [buf[o - k:o].view(h, w, 3) for k, o, (h, w) in zip(n, itertools.accumulate(n), shapes)]
 
 
 def _to_host_all(tensors):
@@ -1307,7 +1453,12 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     a call that holds one composes every region with mn_composite_regions_affine_u8 instead of mn_composite_regions_u8.
     A QuadRegion (DESIGN.md 7b, "Perspective text regions") is handled alike through quad_maps: C = cv2.warpPerspective(img, M,
     (w_r, h_r), INTER_CUBIC | WARP_INVERSE_MAP, BORDER_REPLICATE) (every quad of the call in one mn_warp_perspective_u8_batched
-    launch), T warped back by the 3 x 3 N, and a call that holds one composes every region with mn_composite_regions_quad_u8."""
+    launch), T warped back by the 3 x 3 N, and a call that holds one composes every region with mn_composite_regions_quad_u8.
+    A VerticalRegion (DESIGN.md 7b, "Vertical text columns") takes its shape's crop C (rectified in its kind's launch), lays its
+    cells side by side as the line L (vertical_plan; every column of the call in one mn_vertical_layout_u8_batched launch before
+    restore_images), restores L to T and puts T back into the column T_col [H_c, W_c] (one mn_vertical_unlayout_u8_batched launch
+    after it), which is composed as its shape composes T.  Its labels and boxes are given and returned in C's frame; its entry's
+    sr_u8 is T_col, and it gains line_u8 (T) and cells ([c_0, ..., c_n])."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     plan = plan_regions([im.shape[:2] for im in imgs], regions, labels, boxes, scale, feather)
@@ -1331,43 +1482,61 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
                 ops.warp_affine([(dimg[plan[k].image], crops[k], plan[k].matrix) for k in oriented])
             if quads:
                 ops.warp_perspective([(dimg[plan[k].image], crops[k], plan[k].matrix) for k in quads])
+        verts = [k for k, p in enumerate(plan) if p.vertical is not None]
+        if verts:                                        # every column laid out as a line in one launch
+            lines = _flat_views([(plan[k].vertical.line_height, len(plan[k].vertical.heights) * plan[k].vertical.size[0])
+                                 for k in verts], dev)
+            ops.vertical_layout([(crops[k], line, layout_cells(plan[k].vertical)) for k, line in zip(verts, lines)])
+            for k, line in zip(verts, lines):
+                crops[k] = line
         res = restore_images(encoder, tspgan, sr, crops, [p.labels for p in plan], [p.boxes for p in plan], max_lines=max_lines,
                              context=context, skip_invalid=skip_invalid, whole_lines=whole_lines, overlap=overlap) if plan else []
+        ts = {k: r["sr_u8"] for k, r in enumerate(res) if "error" not in r}
+        vok = [k for k in verts if k in ts]
+        if vok:                                          # every restored line put back into its column in one launch
+            cols = _flat_views([plan[k].vertical.t_size[::-1] for k in vok], dev)
+            ops.vertical_unlayout([(ts[k], col, unlayout_cells(plan[k].vertical, ts[k].shape[1])) for k, col in zip(vok, cols)])
+            ts.update(zip(vok, cols))
         sizes = [scale * scale * im.shape[0] * im.shape[1] * 3 for im in imgs]
         flat = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
         offs = [sum(sizes[:i]) for i in range(len(imgs))]
         pages = [flat[o:o + n].view(scale * im.shape[0], scale * im.shape[1], 3) for o, n, im in zip(offs, sizes, imgs)]
         ops.resize_cubic([(dimg[i], pages[i]) for i in range(len(imgs))])
         ok = [k for k, r in enumerate(res) if "error" not in r]
-        if ok:
-            items = [(pages[plan[k].image], res[k]["sr_u8"], plan[k].out, chain) for k, chain in zip(ok, region_chains(plan, ok))]
+        if ok:                                           # a column composes its T_col where any other region composes its T
+            items = [(pages[plan[k].image], ts[k], plan[k].out, chain) for k, chain in zip(ok, region_chains(plan, ok))]
             if quads:
-                maps = [quad_maps(plan[k].quad, scale, res[k]["sr_u8"].shape[1]) if plan[k].quad is not None else
-                        oriented_maps(plan[k].oriented, scale, res[k]["sr_u8"].shape[1]) if plan[k].oriented is not None else None
+                maps = [quad_maps(plan[k].quad, scale, *ts[k].shape[1::-1]) if plan[k].quad is not None else
+                        oriented_maps(plan[k].oriented, scale, *ts[k].shape[1::-1]) if plan[k].oriented is not None else None
                         for k in ok]
                 ops.composite_regions_quad([it + (m and (m.page_map, m.kx, m.ky),) for it, m in zip(items, maps)], feather)
             elif oriented:
-                maps = [None if plan[k].oriented is None else oriented_maps(plan[k].oriented, scale, res[k]["sr_u8"].shape[1])
+                maps = [None if plan[k].oriented is None else oriented_maps(plan[k].oriented, scale, *ts[k].shape[1::-1])
                         for k in ok]
                 ops.composite_regions_affine([it + (m and (m.page_map, m.kx, m.ky),) for it, m in zip(items, maps)], feather)
             else:
                 ops.composite_regions(items, feather)
-        srs = {k: res[k]["sr_u8"] for k in ok}
+        srs, lines = ts, {k: res[k]["sr_u8"] for k in vok}
         if to_host:
-            host = _to_host_all([flat] + list(srs.values()))
+            host = _to_host_all([flat] + list(srs.values()) + list(lines.values()))
             pages = [host[0][o:o + n].reshape(pg.shape) for o, n, pg in zip(offs, sizes, pages)]
-            srs = dict(zip(srs, host[1:]))
+            srs = dict(zip(srs, host[1:1 + len(srs)]))
+            lines = dict(zip(lines, host[1 + len(srs):]))
     out = [dict(image=pages[i], regions=[]) for i in range(len(imgs))]
     for k, p in enumerate(plan):
         r = res[k]
         if "error" in r:
             entry = dict(error=r["error"])
+        elif "boxes" in r and p.vertical is not None:
+            entry = dict(sr_u8=srs[k], segments=r["segments"], labels=r["labels"], boxes=column_boxes(p.vertical, r["boxes"]))
         elif "boxes" in r:
             x0, y0 = (0, 0) if p.oriented or p.quad else p.rect[:2]
             entry = dict(sr_u8=srs[k], segments=r["segments"], labels=r["labels"],
                          boxes=[[b[0] + x0, b[1] + y0, b[2] + x0, b[3] + y0] for b in r["boxes"]])
         else:
             entry = dict(sr_u8=srs[k], segments=r["segments"], labels=p.labels, boxes=boxes[p.image][p.region])
+        if p.vertical is not None and "error" not in r:
+            entry.update(line_u8=lines[k], cells=list(p.vertical.cells))
         if (p.oriented or p.quad) and "error" not in r:
             entry.update(matrix=p.matrix.copy(), size=p.size)
         out[p.image]["regions"].append(entry)

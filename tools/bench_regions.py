@@ -24,6 +24,15 @@ With --perspective K > 1 every line is pasted seen in perspective: its far (righ
 line with cv2.warpPerspective, runs restore_images(to_host=True) on the crops, resizes the pages with cv2, warps each restored line
 back with cv2.warpPerspective and blends it over its footprint with the numpy feather (oracle/quad_regions.py); the timed kernels
 are mn_warp_perspective_u8_batched, mn_resize_cubic_u8_batched and mn_composite_regions_quad_u8.
+
+With --vertical every line becomes a column of upright characters: its first --cells character cells (each cut at its box and
+resized, nearest pixel, to a square of the line's height) stacked down the page, the columns side by side, each given as a
+pipeline.VerticalRegion of its rectangle with boxes in the column's frame (DESIGN.md section 7b, "Vertical text columns").  The
+host arm then lays every column out as a line with numpy (oracle/vertical_regions.py), runs restore_images(to_host=True) on the
+lines, puts each restored line back into a column with numpy, resizes the pages and each column with cv2 and blends with the
+numpy feather; the timed kernels are mn_vertical_layout_u8_batched, mn_vertical_unlayout_u8_batched, mn_resize_cubic_u8_batched
+and mn_composite_regions_u8.  --profile adds one restore_regions pass under torch.profiler (after the timed passes, in the same
+run) and prints the device time of every kernel of that pass by name.
 """
 import argparse
 import json
@@ -146,6 +155,72 @@ def make_perspective_pages(n_pages, n_lines, max_ratio, seed=0):
     return pages, regs, labs, bxs
 
 
+def make_vertical_pages(n_pages, n_cols, max_cells, seed=0):
+    """make_image_set lines turned into columns: each line's first max_cells characters, cut at their boxes and resized (nearest
+    pixel) to h x h squares, stacked one under another and the columns pasted side by side (8-pixel gaps) onto a noise page:
+    (pages, regions, labels, boxes), regions VerticalRegions of rectangles and boxes in each column's frame."""
+    import cv2
+    from bench_images import make_image_set
+    from marconet_b200.pipeline import VerticalRegion
+    images, labels, boxes = make_image_set(n_pages * n_cols, seed)
+    rng = np.random.default_rng(seed + 1)
+    pages, regs, labs, bxs = [], [], [], []
+    for p in range(n_pages):
+        idx = range(p * n_cols, (p + 1) * n_cols)
+        cols, ll, bb = [], [], []
+        for i in idx:
+            h = images[i].shape[0]
+            chars = boxes[i][:max_cells]
+            cols.append(np.concatenate([cv2.resize(images[i][:, b[0]:b[2]], (h, h), interpolation=cv2.INTER_NEAREST)
+                                        for b in chars], 0))
+            ll.append(labels[i][:len(chars)])
+            bb.append([[1, k * h + 1, h - 1, (k + 1) * h - 1] for k in range(len(chars))])
+        W = sum(c.shape[1] + 8 for c in cols) + 8
+        H = max(c.shape[0] for c in cols) + 16
+        page = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
+        rr, x = [], 8
+        for c in cols:
+            page[8:8 + c.shape[0], x:x + c.shape[1]] = c
+            rr.append(VerticalRegion((x, 8, x + c.shape[1], 8 + c.shape[0])))
+            x += c.shape[1] + 8
+        pages.append(page)
+        regs.append(rr)
+        labs.append(ll)
+        bxs.append(bb)
+    return pages, regs, labs, bxs
+
+
+def host_path_vertical(m, pages, regs, labels, boxes, s, feather, max_lines):
+    """numpy layout of every column, restore_images on the lines, numpy inverse layout, cv2 background and cv2 resize of each
+    restored column onto its rectangle, the numpy blend."""
+    import cv2
+    from marconet_b200 import pipeline
+    from oracle import regions
+    from oracle import vertical_regions as V
+    lines, labs, lbx, cells = [], [], [], []
+    for pg, rr, ll, bb in zip(pages, regs, labels, boxes):
+        for reg, lab, bx in zip(rr, ll, bb):
+            x0, y0, x1, y1 = reg.shape
+            c = V.cells(y1 - y0, x1 - x0, boxes=bx)
+            lines.append(V.layout(pg[y0:y1, x0:x1], c))
+            labs.append(lab)
+            lbx.append(V.line_boxes(c, x1 - x0, bx))
+            cells.append(c)
+    res = pipeline.restore_images(*m, lines, labs, lbx, max_lines=max_lines, to_host=True)
+    out, k = [], 0
+    for pg, rr in zip(pages, regs):
+        o = cv2.resize(pg, (0, 0), fx=s, fy=s, interpolation=cv2.INTER_CUBIC)
+        for reg in rr:
+            x0, y0, x1, y1 = reg.shape
+            tc = V.unlayout(res[k]["sr_u8"], cells[k], x1 - x0)
+            r = (s * x0, s * y0, s * x1, s * y1)
+            p = cv2.resize(np.ascontiguousarray(tc[..., ::-1]), (r[2] - r[0], r[3] - r[1]), interpolation=cv2.INTER_CUBIC)
+            o[r[1]:r[3], r[0]:r[2]] = regions.blend(o[r[1]:r[3], r[0]:r[2]], p, regions.alpha(r, o.shape[:2], feather))
+            k += 1
+        out.append(o)
+    return out
+
+
 def host_path_perspective(m, pages, regs, labels, boxes, s, feather, max_lines):
     """cv2 rectify, restore_images on the crops, cv2 background and cv2 warp of each restored line back (onto the rows and
     columns up to its footprint's far corner: at least 64 columns and 16 rows, so that cv2's 64-column blocks start where the
@@ -251,7 +326,12 @@ def main():
     ap.add_argument("--max-angle", type=float, default=0.0, help="turn every line by up to this many degrees (oriented regions)")
     ap.add_argument("--perspective", type=float, default=0.0,
                     help="shrink every line's far end by a foreshortening ratio up to this (> 1; perspective regions)")
+    ap.add_argument("--vertical", action="store_true", help="vertical text columns (--lines columns per page)")
+    ap.add_argument("--cells", type=int, default=16, help="characters per column with --vertical")
+    ap.add_argument("--profile", action="store_true", help="one more restore_regions pass under torch.profiler")
     args = ap.parse_args()
+    if args.vertical and (args.max_angle > 0 or args.perspective):
+        sys.exit("--vertical does not combine with --max-angle or --perspective")
     if args.perspective and (args.max_angle > 0 or not 1 < args.perspective <= 4):
         sys.exit("--perspective takes a ratio in (1, 4] and does not combine with --max-angle")
     if not torch.cuda.is_available():
@@ -268,7 +348,9 @@ def main():
         net.load_state_dict(sds[key], strict=True)
         m.append(net.eval().to(dev))
     oriented, perspective = args.max_angle > 0, args.perspective > 1
-    if perspective:
+    if args.vertical:
+        pages, rects, labels, boxes = make_vertical_pages(args.pages, args.lines, args.cells)
+    elif perspective:
         pages, rects, labels, boxes = make_perspective_pages(args.pages, args.lines, args.perspective)
     elif oriented:
         pages, rects, labels, boxes = make_rotated_pages(args.pages, args.lines, args.max_angle)
@@ -277,7 +359,10 @@ def main():
     s, feather = args.scale, 2 * args.scale
 
     lib = _lib.load()
-    if perspective:
+    if args.vertical:
+        events = {"mn_vertical_layout_u8_batched": [], "mn_vertical_unlayout_u8_batched": [], "mn_resize_cubic_u8_batched": [],
+                  "mn_composite_regions_u8": []}
+    elif perspective:
         events = {"mn_warp_perspective_u8_batched": [], "mn_resize_cubic_u8_batched": [], "mn_composite_regions_quad_u8": []}
     elif oriented:
         events = {"mn_warp_affine_u8_batched": [], "mn_resize_cubic_u8_batched": [], "mn_composite_regions_affine_u8": []}
@@ -304,7 +389,8 @@ def main():
         return [o["image"] for o in out]
 
     def host():
-        path = host_path_perspective if perspective else host_path_oriented if oriented else host_path
+        path = host_path_vertical if args.vertical else host_path_perspective if perspective else \
+            host_path_oriented if oriented else host_path
         return path(m, pages, rects, labels, boxes, s, feather, args.max_lines)
 
     arms = {"restore_regions": api, "host_path": host}
@@ -326,6 +412,7 @@ def main():
     out_px = sum(s * s * p.shape[0] * p.shape[1] for p in pages)
     common = dict(pages=args.pages, lines_per_page=args.lines, scale=s, feather=feather, max_lines=args.max_lines,
                   max_angle=args.max_angle, **({"perspective": args.perspective} if perspective else {}),
+                  **({"vertical": True, "cells_per_column": args.cells} if args.vertical else {}),
                   page_sizes=[list(p.shape[:2]) for p in pages], output_megapixels=round(out_px / 1e6, 2),
                   module_graphs=os.environ.get("MN_MODULE_GRAPHS"), same_bytes=same, max_abs_diff=diff, **card)
     for name, ts in times.items():
@@ -335,6 +422,21 @@ def main():
     print(json.dumps(dict(metric="regions_kernels", **{f"{k}_ms": [round(v, 4) for v in vs] for k, vs in kern.items()},
                           background_gbytes_per_s=round(3 * out_px / (min(kern["mn_resize_cubic_u8_batched"]) * 1e-3) / 1e9, 1),
                           **common)), flush=True)
+    if args.profile:
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            api()
+            torch.cuda.synchronize()
+        dev_ms = {}
+        for ev in prof.events():
+            if ev.device_type == torch.autograd.DeviceType.CUDA:
+                dev_ms.setdefault(ev.name, []).append(ev.device_time_total / 1e3)
+        total = sum(sum(v) for v in dev_ms.values())
+        top = sorted(dev_ms.items(), key=lambda kv: -sum(kv[1]))
+        print(json.dumps(dict(metric="regions_profile", device_ms_total=round(total, 3),
+                              kernels={k: dict(calls=len(v), ms=round(sum(v), 4)) for k, v in top
+                                       if "vertical" in k or "composite" in k or "resize_cubic" in k or k in dict(top[:8])},
+                              **common)), flush=True)
     if not same:
         sys.exit("the arms' bytes differ")
 
