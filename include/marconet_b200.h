@@ -151,6 +151,12 @@ typedef struct {
     int splits;                 /* split-K factor of the simt or halo-tiled kernel (1: none)    */
     int gn_fused;               /* 1: the kernel applies the gn_mean_rstd input transform       */
     int gn_stats_out;           /* 1: the kernel accumulates the gn_stats_out statistics        */
+    /* tensor-core kernels only (0 for the fp32 kernels): */
+    int cs;                     /* CTAs per cluster (2: the weight tile is multicast to a pair)  */
+    int m_tiles;                /* pixel tiles                                                  */
+    int work_items;             /* (pixel tiles / cs, rounded up) x (Cout / nt) x splits         */
+    int hstages, bstages;       /* depths of the A-tile and weight-tile rings                   */
+    int ctas;                   /* grid of the launch under the current mn_set_max_ctas cap      */
 } mn_conv_plan;
 /* The one dispatch decision: MN_OK and *out filled in, or the status and message mn_conv2d_nhwc would return for *p.
  * A tensor-core precision picks the halo tiling when it runs the geometry, else the per-tap tiling; it fails

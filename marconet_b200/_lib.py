@@ -43,7 +43,8 @@ CONV_KERNELS = ("small", "simt", "tc1", "tc2")     # mn_conv_kernel
 
 class ConvPlan(Structure):
     _fields_ = [("kernel", c_int), ("precision", c_int), ("nt", c_int), ("TN", c_int), ("TH", c_int), ("TW", c_int), ("splits", c_int),
-                ("gn_fused", c_int), ("gn_stats_out", c_int)]
+                ("gn_fused", c_int), ("gn_stats_out", c_int), ("cs", c_int), ("m_tiles", c_int), ("work_items", c_int),
+                ("hstages", c_int), ("bstages", c_int), ("ctas", c_int)]
 
 
 class DemodDesc(Structure):

@@ -67,6 +67,8 @@ static int plan_conv(const mn_conv_params* p, ConvGeom& g, mn_conv_plan* r, Tc2P
             if (!tc->ok) return MN_ERR_UNSUPPORTED;
             r->kernel = tc->t.per_tap ? MN_CONV_KERNEL_TC1 : MN_CONV_KERNEL_TC2;
             r->nt = tc->t.nt; r->TN = tc->t.TN; r->TH = tc->t.TH; r->TW = tc->t.TW; r->splits = tc->t.ksplit;
+            r->cs = tc->t.cs; r->m_tiles = tc->t.m_tiles; r->work_items = tc->t.m_groups * tc->t.n_tiles * tc->t.ksplit;
+            r->hstages = tc->t.hstages; r->bstages = tc->t.bstages; r->ctas = mn_conv_tc_ctas(tc->t);
             break;
         default:
             mn_set_error("mn_conv2d_nhwc: unknown precision mode %d", p->precision);

@@ -165,6 +165,8 @@ struct Tc2Plan { bool ok; const char* why; int smem; Tc2Geom t; };
 // had never been made.  Per-sample output pointers (g.y2_ptrs) are not optional: without the halo tiling the plan fails.
 // !ok: no tiling runs g (mn_last_error says why).
 Tc2Plan mn_conv_tc_plan(ConvGeom& g);
+// CTAs of the persistent grid mn_conv_tc_launch uses for plan t under the current mn_max_ctas() cap (a multiple of t.cs)
+int mn_conv_tc_ctas(const Tc2Geom& t);
 int mn_conv_tc_launch(const ConvGeom& g, Tc2Plan& p, const void* w_hi, const void* w_lo, const float* w_scale, int prec, cudaStream_t st);
 // direct 3x3 conv for Cout <= 4 (conv_small.cu)
 bool mn_conv_small_supported(const ConvGeom& g);

@@ -678,14 +678,8 @@ int launch_tc2(const CUtensorMap& ma, const CUtensorMap& mbh, const CUtensorMap&
     static unsigned long long smem_done = 0;
     MN_CUDA_CHECK(mn_ensure_dyn_smem(conv_tc2_kernel<GN, MODE, NT>, SMEM_LIMIT, &smem_done));
     const Tc2Geom& t = p.t;
-    const int total_work = t.m_groups * t.n_tiles * t.ksplit;
-    int sms = mn_num_sms();
-    if (mn_max_ctas() > 0 && mn_max_ctas() < sms) sms = mn_max_ctas();
-    int clusters = sms / t.cs;
-    if (clusters < 1) clusters = 1;
-    if (clusters > total_work) clusters = total_work;
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(clusters * t.cs, 1, 1);
+    cfg.gridDim = dim3(mn_conv_tc_ctas(t), 1, 1);
     cfg.blockDim = dim3(NUM_THREADS2, 1, 1);
     cfg.dynamicSmemBytes = p.smem;
     cfg.stream = st;
@@ -705,6 +699,16 @@ int launch_tc2_nt(const CUtensorMap& ma, const CUtensorMap& mbh, const CUtensorM
 }
 
 }  // namespace
+
+int mn_conv_tc_ctas(const Tc2Geom& t) {
+    const int total_work = t.m_groups * t.n_tiles * t.ksplit;
+    int sms = mn_num_sms();
+    if (mn_max_ctas() > 0 && mn_max_ctas() < sms) sms = mn_max_ctas();
+    int clusters = sms / t.cs;
+    if (clusters < 1) clusters = 1;
+    if (clusters > total_work) clusters = total_work;
+    return clusters * t.cs;
+}
 
 Tc2Plan mn_conv_tc_plan(ConvGeom& g) {
     const Tc2Plan halo = plan_tc2(g);

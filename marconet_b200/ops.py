@@ -326,7 +326,9 @@ def conv2d(x, w, kh, kw, stride=(1, 1), pad=(0, 0), bias=None, out_scale=None, r
            valid_w=None, precision=None, want_y=True, split_k=0, gn=None, gn_fuse=True, out2_ptrs=None, gn_stats=False, plan=None):
     """mn_conv2d_nhwc.  ``w`` is the packed [KH*KW*Cin, Cout] matrix.  Returns y (or (y, y2)).
     ``plan``: a dict that receives what was launched (mn_conv2d_plan): ``kernel`` ("small" / "simt" / "tc1" / "tc2"), ``precision``,
-    ``nt``, ``TN``, ``TH``, ``TW``, ``splits`` (split-K), ``gn_fused``, ``gn_stats_out`` (statistics from the epilogue) and ``x_scale``.
+    ``nt``, ``TN``, ``TH``, ``TW``, ``splits`` (split-K), ``gn_fused``, ``gn_stats_out`` (statistics from the epilogue), ``x_scale`` and,
+    for the tensor-core kernels (0 otherwise), ``cs`` (cluster size), ``m_tiles``, ``work_items``, ``hstages`` / ``bstages`` (ring
+    depths) and ``ctas`` (the grid under the current ``set_max_ctas`` cap).
     ``gn=(mean_rstd, gamma, beta)``: the conv input is swish(GroupNorm(x)); fused into the halo-tiled tensor-core kernel's operand-split
     stage when ``gn_fuse`` is true and the plan honours it (that kernel, one sample per pixel tile), otherwise applied by
     mn_groupnorm_apply first; ``gn_fuse=False`` forces the two passes.
@@ -432,7 +434,8 @@ def conv2d(x, w, kh, kw, stride=(1, 1), pad=(0, 0), bias=None, out_scale=None, r
     LAUNCHES += 1
     if plan is not None:
         plan.update(kernel=_lib.CONV_KERNELS[cp.kernel], precision=cp.precision, nt=cp.nt, TN=cp.TN, TH=cp.TH, TW=cp.TW, splits=cp.splits,
-                    gn_fused=bool(cp.gn_fused), gn_stats_out=bool(cp.gn_stats_out), x_scale=p.x_scale if p.x_scale > 0 else 1.0)
+                    gn_fused=bool(cp.gn_fused), gn_stats_out=bool(cp.gn_stats_out), x_scale=p.x_scale if p.x_scale > 0 else 1.0,
+                    cs=cp.cs, m_tiles=cp.m_tiles, work_items=cp.work_items, hstages=cp.hstages, bstages=cp.bstages, ctas=cp.ctas)
     calib = getattr(_TLS, "calib", None)
     if calib is not None and calib.compare and cw is not None and prec != PREC_FP32_SIMT and precision is None:
         # tuning tool only (pipeline.tune_precision): the same layer through the exact fp32 kernel and both split formats

@@ -16,6 +16,8 @@ It also returns the magnitude A = sum_k |x'_k w[k,o]| of each dot product.  The 
 where L_act is the activation's Lipschitz constant and the last term is the rounding of the stored value itself.  A bound per
 element (rather than one scaled by the tensor's max) sees an error in a small output -- a row of the wrong sample's scale, a dropped
 bias -- that a max-norm bound hides.
+
+``conv_ref_full`` evaluates the same reference and bound for every output element (an fp64 ``F.conv2d`` on the input's device).
 """
 import math
 
@@ -161,6 +163,57 @@ def conv_ref(d, w, act=0, gain=1.0, drop=(), shift=0):
     out = dict(y=v, bound=torch.where(masked[:, None], torch.zeros_like(bound), bound), masked=masked)
     y2s = _row_vec(d.get("y2_scale"), pn, cout, shift)
     if y2s is not None:
+        out["y2"] = v * y2s
+        out["bound2"] = out["bound"] * y2s.abs()
+    return out
+
+
+def conv_ref_full(x, w, kh, kw, stride, pad, gn=None, valid_w=None, residual=None, res_broadcast=False, out_scale=None, y2_scale=None,
+                  bias=None, act=0, gain=1.0):
+    """``conv_ref`` over every output element at once: an fp64 ``F.conv2d`` on x's device (on the GPU when x is there).  Arguments as
+    ``gather`` and ``conv_ref`` take them (call it on copies made before the op runs); ``w`` [KH*KW*Cin, Cout].  Returns NHWC
+    dict(y=[N,OH,OW,Cout], bound (the bracket of the tolerance, as ``conv_ref``), masked=[N,OH,OW] bool, and y2 / bound2 when
+    ``y2_scale`` is given)."""
+    import torch.nn.functional as F
+    dev = x.device
+    n, h, wd, cin = x.shape
+    xs = x.permute(0, 3, 1, 2).double()
+    w4 = w.double().to(dev).reshape(kh, kw, cin, -1).permute(3, 2, 0, 1)
+    cout = w4.shape[0]
+    vw = None if valid_w is None else valid_w.long().to(dev)
+    if gn is not None:
+        mr, gamma, beta = (t.double().to(dev) for t in gn)
+        grp = torch.arange(cin, device=dev) // 32
+        t = (xs - mr[:, grp, 0, None, None]) * mr[:, grp, 1, None, None] * gamma[None, :cin, None, None] + beta[None, :cin, None, None]
+        xs = t * torch.sigmoid(t)
+        if vw is not None:
+            xs = xs * (torch.arange(wd, device=dev)[None, :] < vw[:, None])[:, None, None, :]
+    acc = F.conv2d(xs, w4, stride=stride, padding=pad).permute(0, 2, 3, 1)
+    mag = F.conv2d(xs.abs(), w4.abs(), stride=stride, padding=pad).permute(0, 2, 3, 1)
+    if out_scale is not None:
+        os_ = out_scale.double().to(dev)[:, None, None, :cout]
+        acc = acc * os_
+        mag = mag * os_.abs()
+    if bias is not None:
+        b = bias.double().to(dev)[:cout]
+        acc = acc + b
+        mag = mag + b.abs()
+    if residual is not None:
+        r = residual.double().to(dev)[..., :cout]
+        if res_broadcast:
+            r = r[:1]
+        acc = acc + r
+        mag = mag + r.abs()
+    v = act64(acc, act) * gain
+    oh, ow = v.shape[1], v.shape[2]
+    masked = torch.zeros(n, oh, ow, dtype=torch.bool, device=dev)
+    if vw is not None:
+        masked = (torch.arange(ow, device=dev)[None, :] >= vw[:, None])[:, None, :].expand(n, oh, ow)
+    v = torch.where(masked[..., None], torch.zeros_like(v), v)
+    bound = abs(gain) * LIPSCHITZ[act] * mag
+    out = dict(y=v, bound=torch.where(masked[..., None], torch.zeros_like(bound), bound), masked=masked)
+    if y2_scale is not None:
+        y2s = y2_scale.double().to(dev)[:, None, None, :cout]
         out["y2"] = v * y2s
         out["bound2"] = out["bound"] * y2s.abs()
     return out

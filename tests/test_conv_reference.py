@@ -14,9 +14,9 @@ def _rand(*shape, seed):
     return torch.randn(*shape, generator=torch.Generator().manual_seed(seed))
 
 
-def _full_ref(x, w4, stride, pad, gn=None, valid_w=None, out_scale=None, bias=None, residual=None, res_broadcast=False, act=0,
+def _hand_ref(x, w4, stride, pad, gn=None, valid_w=None, out_scale=None, bias=None, residual=None, res_broadcast=False, act=0,
               gain=1.0, y2_scale=None):
-    """The whole op over every pixel, NCHW fp64, the straightforward way."""
+    """The whole op over every pixel, NCHW fp64, the straightforward way (no shared code with oracle/conv_ref.py)."""
     x = x.permute(0, 3, 1, 2).double()
     n, c, h, wd = x.shape
     if gn is not None:
@@ -42,6 +42,12 @@ def _full_ref(x, w4, stride, pad, gn=None, valid_w=None, out_scale=None, bias=No
             v[i, :, :, int(valid_w[i]):] = 0
     v = v.permute(0, 2, 3, 1)
     return v, (None if y2_scale is None else v * y2_scale.double()[:, None, None, :])
+
+
+def _close(a, b, scale):
+    """|a - b| <= 1e-12 * scale everywhere (scale: the bound of a value, which two summation orders may differ by a multiple of
+    2^-52 of; the value itself for the bound, a sum of magnitudes).  Zero scale demands equality."""
+    return bool(((a - b).abs() <= 1e-12 * scale).all())
 
 
 FEATURES = ["plain", "demod_bias_lrelu_y2", "residual_relu", "res_broadcast_tanh", "gelu", "sigmoid", "valid_w", "gn_swish_valid_w"]
@@ -75,7 +81,7 @@ def test_sampled_reference_equals_fp64_conv(feature, stride, k, pad):
         kw = dict(gn=(mr, _rand(cin, seed=11) * 0.3 + 1, _rand(cin, seed=12) * 0.2), valid_w=torch.tensor([w, 7, 13]))
         if stride != (1, 1):
             kw["valid_w"] = None
-    full, full2 = _full_ref(x, w4, stride, pad, **kw)
+    full, full2 = _hand_ref(x, w4, stride, pad, **kw)
     w2d = w4.permute(2, 3, 1, 0).reshape(k * k * cin, cout)
     pix = R.sample_pixels(n, oh, ow, th=4, tw=8, tn=2, m_tile=128, valid_w=kw.get("valid_w"), count=60, seed=3)
     g = {key: kw[key] for key in ("gn", "valid_w", "residual", "res_broadcast", "out_scale", "y2_scale", "bias") if kw.get(key) is not None}
@@ -85,6 +91,17 @@ def test_sampled_reference_equals_fp64_conv(feature, stride, k, pad):
     assert torch.allclose(ref["y"], want, rtol=1e-12, atol=1e-12)
     if full2 is not None:
         assert torch.allclose(ref["y2"], full2[pix[:, 0], pix[:, 1], pix[:, 2]], rtol=1e-12, atol=1e-12)
+    # the whole-tensor reference at the sampled pixels: the same values, bounds and masks as the sampled one
+    whole = R.conv_ref_full(x, w2d, k, k, stride, (pad, pad), act=kw.get("act", 0), gain=kw.get("gain", 1.0), **g)
+    assert whole["y"].shape == (n, oh, ow, cout) and _close(whole["y"], full, whole["bound"] + full.abs())
+    at = lambda t: t[pix[:, 0], pix[:, 1], pix[:, 2]]          # noqa: E731
+    assert torch.equal(at(whole["masked"]), ref["masked"])
+    assert _close(at(whole["bound"]), ref["bound"], ref["bound"])
+    assert _close(at(whole["y"]), ref["y"], ref["bound"] + ref["y"].abs())
+    assert ("y2" in whole) == ("y2" in ref)
+    if "y2" in ref:
+        assert _close(at(whole["bound2"]), ref["bound2"], ref["bound2"])
+        assert _close(at(whole["y2"]), ref["y2"], ref["bound2"] + ref["y2"].abs())
     # the bound dominates the exact error of an fp32 evaluation of the same numbers
     got = want.float()
     assert R.ratio(got, ref["y"], ref["bound"], 1e-6) <= 1.0

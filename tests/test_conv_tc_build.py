@@ -1,10 +1,32 @@
 """ptxas -v for sm_90a: every instantiation of the wgmma convolution keeps its roles in registers (setmaxnreg budgets) and keeps
-its wgmma groups asynchronous."""
+its wgmma groups asynchronous.  The ctypes layouts of the convolution's C ABI records follow the header."""
+import ctypes
 import os
 import re
 import subprocess
 
+import pytest
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def _fields(header, name):
+    body = re.search(r"typedef struct \{([^{}]*)\}\s*" + name + ";", header).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    names = []
+    for decl in body.split(";"):
+        parts = [p.strip() for p in decl.strip().split(",") if p.strip()]
+        names += [re.findall(r"[A-Za-z_0-9]+$", p)[0] for p in parts]
+    return names
+
+
+@pytest.mark.parametrize("c_name,py_name,size", [("mn_conv_params", "ConvParams", 296), ("mn_conv_plan", "ConvPlan", 60)])
+def test_conv_structs_match_header(c_name, py_name, size):
+    from marconet_b200 import _lib
+    header = open(os.path.join(ROOT, "include", "marconet_b200.h")).read()
+    cls = getattr(_lib, py_name)
+    assert _fields(header, c_name) == [f[0] for f in cls._fields_]
+    assert ctypes.sizeof(cls) == size        # x86-64 / aarch64 natural alignment, as the library is compiled
 
 
 def test_conv_tc2_kernels_build_without_spills(tmp_path):
