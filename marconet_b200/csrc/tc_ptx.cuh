@@ -167,10 +167,12 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
     return r;
 }
-// Arrive on an mbarrier of a CTA of the cluster (release at cluster scope: the arriving warp's shared-memory reads of the stage
-// are ordered before the peer's TMA refill of it).
+// Arrive on an mbarrier of a CTA of the cluster, with the default semantics (release at CTA scope).  For a stage read only by
+// wgmma that is enough: wgmma.wait_group has completed the reads before the arrive, so the peer's TMA refill cannot overtake
+// them.  (.release.cluster compiles to MEMBAR.ALL.GPU before the arrive: a GPU-scope fence per tap in the releasing warps that also
+// waits for their outstanding epilogue stores.)
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 

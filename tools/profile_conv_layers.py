@@ -1,7 +1,8 @@
 """Per-layer timing of every mn_conv2d_nhwc call of one 16-character line (developer tool): CUDA events around each eager call,
 warm caches, module graphs off.  Prints the layers sorted by time with their algorithmic TFLOP/s and, for the tensor-core layers, the
 fraction of the tensor pipe (3 fp16 MMA passes per fp32-grade product, against MEASURED_PEAKS.json's bf16 burst peak when present,
-else the H100 SXM data sheet's 989 TFLOP/s dense bf16, a 700 W figure).
+else the H100 SXM data sheet's 989 TFLOP/s dense bf16, a 700 W figure).  The last column is the plan that ran: kernel / NT (the
+tensor-core work-item width, 0 for the fp32 kernels) and, when split, ksS.
 
     MN_MODULE_GRAPHS=0 python tools/profile_conv_layers.py [--chars 16] [--iters 10]
 """
@@ -38,11 +39,15 @@ def main():
     locs = synth.make_locs(1, C).to(dev)
     enc, gen, sr = nets["encoder"], nets["tspgan"], nets["sr"]
     recs = defaultdict(list)
+    plans = {}      # call index -> "kernel/NT [ksS]" of the plan that ran
     real = ops.conv2d
     seq = [0]
 
     def timed(x, w, kh, kw, *a, **k):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        if k.get("plan") is None:
+            k["plan"] = {}
+        plan = k["plan"]
         e0.record()
         out = real(x, w, kh, kw, *a, **k)
         e1.record()
@@ -52,6 +57,7 @@ def main():
         oh, ow = (y.shape[1], y.shape[2]) if y is not None else (h, wd)
         name = getattr(w, "name", None) or "?"
         recs[(seq[0], name, n, h, wd, cin, cout, kh, oh, ow)].append((e0, e1))
+        plans[seq[0]] = f"{plan['kernel']}/{plan['nt']}" + (f" ks{plan['splits']}" if plan["splits"] > 1 else "")
         seq[0] += 1
         return out
 
@@ -82,11 +88,11 @@ def main():
         ts = sorted(a.elapsed_time(b) * 1e3 for a, b in evs)
         us = ts[len(ts) // 2]
         flop = 2.0 * n * oh * ow * cout * cin * kh * kh
-        rows.append((us, s, name, f"N{n} {h}x{wd} {cin}->{cout} k{kh}", flop / us * 1e-6))
+        rows.append((us, s, name, f"N{n} {h}x{wd} {cin}->{cout} k{kh}", flop / us * 1e-6, plans[s]))
     total = sum(r[0] for r in rows)
     print(f"{len(rows)} conv calls, {total:.0f} us per line in convs (eager, event-timed incl. launch gaps); tensor-pipe column assumes 3 MMA passes")
-    for us, s, name, shape, tf in sorted(rows, reverse=True):
-        print(f"{us:8.1f} us {100 * us / total:5.1f}%  #{s:<3d} {name:<44s} {shape:<28s} {tf:7.1f} TF  pipe {3 * tf / peak:5.2f}")
+    for us, s, name, shape, tf, pl in sorted(rows, reverse=True):
+        print(f"{us:8.1f} us {100 * us / total:5.1f}%  #{s:<3d} {name:<44s} {shape:<28s} {tf:7.1f} TF  pipe {3 * tf / peak:5.2f}  {pl}")
 
 
 if __name__ == "__main__":
