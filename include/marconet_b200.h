@@ -623,6 +623,49 @@ typedef struct {
 int mn_vertical_layout_u8_batched(const mn_vertical_column* columns, int n, long long max_pixels, void* stream);
 int mn_vertical_unlayout_u8_batched(const mn_vertical_column* columns, int n, long long max_pixels, void* stream);
 
+/* Curved text regions (DESIGN.md section 7b, "Curved text regions").  A curve table is an fp64 array built on the host
+ * (pipeline.curved_maps): curve[0] = s, the page's scale (unused by the rectify kernel); curve[1 .. k+1] = the column fractions
+ * c_0 = 0, ..., c_k = 1; then the top curve's 3k+1 (x, y) points and the bottom curve's 3k+1 points, x and y interleaved.
+ * Segment m of a curve is the cubic Bezier of its points 3m .. 3m+3, evaluated by de Casteljau per coordinate with s = 1 - t and
+ * three levels of lerps fl(fl(s A) + fl(t B)), every fp64 operation rounded on its own.
+ * mn_remap_curved_u8_batched: cv2.remap(src, mapx, mapy, INTER_CUBIC, BORDER_REPLICATE) with fp32 maps, OpenCV's own 8-bit path
+ * (IPP off), of n images in one launch, blockIdx.y = image, one thread per destination pixel (x, y) of the [dh][dw][cn] crop
+ * (w_r = dw, h_r = dh): a = (x + 0.5)/w_r, b = (y + 0.5)/h_r, m the last segment with c_m <= a (at most k - 1),
+ * t = (a - c_m)/(c_{m+1} - c_m), mapx = fl(fl(fl(1 - b) T_m(t).x) + fl(b B_m(t).x)) - 0.5 and mapy likewise (fp64), then
+ * Xq = rint(fl32(mapx) 32), Yq = rint(fl32(mapy) 32) and remap's cubic sampler exactly as mn_warp_affine_u8_batched uses it.
+ * Callers keep every |map value| below 2^14.  Byte offsets are 64-bit.  max_pixels >= every dh*dw.  images: DEVICE array of
+ * records whose curve tables point into device memory (validated by the caller). */
+typedef struct {
+    const uint8_t* src;         /* row 0 of the source image */
+    int64_t src_pitch;
+    int32_t h, w;
+    uint8_t* dst;               /* row 0 of the destination crop */
+    int64_t dst_pitch;
+    int32_t dh, dw;
+    const double* curve;        /* the region's curve table */
+    int32_t n_seg, pad;         /* k */
+} mn_remap_curved_image;
+int mn_remap_curved_u8_batched(const mn_remap_curved_image* images, int n, int cn, long long max_pixels, void* stream);
+
+/* mn_composite_regions_quad_u8 for pages that also hold curved regions: every region of every page in one launch, blockIdx.y =
+ * region.  Kinds MN_REGION_RECT, MN_REGION_AFFINE and MN_REGION_PERSPECTIVE (q as mn_region_quad) are composed exactly as
+ * mn_composite_regions_quad_u8 composes them (the same device functions).  Kind MN_REGION_CURVED: q.r's rectangle is the
+ * bounding box of the region's control points in page pixels, widened by one pixel; page pixel (X, Y) is the point
+ * p = ((X + 0.5)/s, (Y + 0.5)/s).  The segments m = 0 .. k-1 are tried in order, skipping one whose 8 control points' bounding box
+ * does not hold p; with d = B_m(t) - T_m(t), r = p - T_m(t) and g(t) = fl(fl(d.x r.y) - fl(d.y r.x)), a segment whose g(0) < 0
+ * and g(1) < 0 agree has no root; otherwise 48 bisection steps (mid = fl(0.5 fl(lo + hi)), lo keeps g(0)'s sign), then
+ * t* = fl(0.5 fl(lo + hi)) and b = fl(dot(r, d) / dot(d, d)) at t*.  The first segment with 0 <= b <= 1 gives
+ * a = c_m + t* (c_{m+1} - c_m), u = fl(a sr_w) - 0.5, v = fl(b sr_h) - 0.5, Xq = rint(fl32(u) 32), Yq = rint(fl32(v) 32); the
+ * pixel belongs to the region iff a segment was accepted and -16 <= Xq < 32 sr_w - 16, -16 <= Yq < 32 sr_h - 16.  The feather
+ * (q.kx, q.ky), P, the blend and the owner rule are the affine kind's; chains index this array. */
+#define MN_REGION_CURVED 3
+typedef struct {
+    mn_region_quad q;           /* q.kind MN_REGION_CURVED: q.kx, q.ky are its feather slopes and q.n is unused */
+    const double* curve;        /* curved region: its curve table */
+    int32_t n_seg, pad;         /* curved region: k */
+} mn_region_curved;
+int mn_composite_regions_curved_u8(const mn_region_curved* regions, int n, long long max_pixels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -140,6 +140,18 @@ class VerticalColumn(Structure):
                 ("dh", c_int32), ("dw", c_int32), ("n_cells", c_int32), ("w", c_int32)]
 
 
+class RemapCurvedImage(Structure):
+    _fields_ = [("src", c_void_p), ("src_pitch", c_int64), ("h", c_int32), ("w", c_int32), ("dst", c_void_p), ("dst_pitch", c_int64),
+                ("dh", c_int32), ("dw", c_int32), ("curve", c_void_p), ("n_seg", c_int32), ("pad", c_int32)]
+
+
+REGION_CURVED = 3
+
+
+class RegionCurved(Structure):
+    _fields_ = [("q", RegionQuad), ("curve", c_void_p), ("n_seg", c_int32), ("pad", c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -197,6 +209,8 @@ SYMBOLS = {
     "mn_composite_regions_quad_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_vertical_layout_u8_batched": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_vertical_unlayout_u8_batched": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
+    "mn_remap_curved_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
+    "mn_composite_regions_curved_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -397,6 +397,107 @@ __device__ __forceinline__ const mn_region& rect_of(const mn_region& r) { return
 __device__ __forceinline__ const mn_region& rect_of(const mn_region_affine& r) { return r.r; }
 __device__ __forceinline__ const mn_region& rect_of(const mn_region_quad& r) { return r.r; }
 
+// Curved text regions (DESIGN.md 7b, "Curved text regions").  One lerp of de Casteljau's: fl(fl(s a) + fl(t b)), s = 1 - t.
+__device__ __forceinline__ double bez_lerp(double a, double b, double s, double t) {
+    return __dadd_rn(__dmul_rn(s, a), __dmul_rn(t, b));
+}
+
+// The cubic Bezier of the 4 (x, y) points at p (x, y interleaved) at t, three levels of lerps per coordinate.
+struct Pt { double x, y; };
+__device__ __forceinline__ Pt bezier(const double* __restrict__ p, double t) {
+    const double s = __dsub_rn(1.0, t);
+    double c[2];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        const double a0 = bez_lerp(p[k], p[2 + k], s, t), a1 = bez_lerp(p[2 + k], p[4 + k], s, t);
+        const double a2 = bez_lerp(p[4 + k], p[6 + k], s, t);
+        c[k] = bez_lerp(bez_lerp(a0, a1, s, t), bez_lerp(a1, a2, s, t), s, t);
+    }
+    return {c[0], c[1]};
+}
+
+// The top and bottom control points of segment m of a curve table with k segments (layout: mn_remap_curved_image).
+__device__ __forceinline__ const double* curve_top(const double* curve, int k, int m) { return curve + k + 2 + 6 * m; }
+__device__ __forceinline__ const double* curve_bottom(const double* curve, int k, int m) { return curve + 7 * k + 4 + 6 * m; }
+
+// The crop map of crop pixel (x, y) of a dw x dh rectified crop, as fixed-point remap coordinates rint(fl32(map) 32).
+__device__ __forceinline__ WarpCoord curved_crop_coord(const double* __restrict__ curve, int k, int x, int y, int dw, int dh) {
+    const double a = __ddiv_rn(__dadd_rn((double)x, 0.5), (double)dw), b = __ddiv_rn(__dadd_rn((double)y, 0.5), (double)dh);
+    const double* c = curve + 1;
+    int m = 0;
+    for (int j = 1; j < k; ++j) m = c[j] <= a ? j : m;
+    const double t = __ddiv_rn(__dsub_rn(a, c[m]), __dsub_rn(c[m + 1], c[m]));
+    const Pt T = bezier(curve_top(curve, k, m), t), B = bezier(curve_bottom(curve, k, m), t);
+    const double omb = __dsub_rn(1.0, b);
+    const double mx = __dsub_rn(__dadd_rn(__dmul_rn(omb, T.x), __dmul_rn(b, B.x)), 0.5);
+    const double my = __dsub_rn(__dadd_rn(__dmul_rn(omb, T.y), __dmul_rn(b, B.y)), 0.5);
+    return {__float2int_rn(__fmul_rn(__double2float_rn(mx), 32.f)), __float2int_rn(__fmul_rn(__double2float_rn(my), 32.f))};
+}
+
+// g(t) = cross(d, p - T) of segment (top, bot) at t, d = B - T: the side of the ruling at t on which p lies.
+__device__ __forceinline__ double ruling_side(const double* __restrict__ top, const double* __restrict__ bot, double px, double py,
+                                              double t) {
+    const Pt T = bezier(top, t), B = bezier(bot, t);
+    const double dx = __dsub_rn(B.x, T.x), dy = __dsub_rn(B.y, T.y);
+    return __dsub_rn(__dmul_rn(dx, __dsub_rn(py, T.y)), __dmul_rn(dy, __dsub_rn(px, T.x)));
+}
+
+// The T coordinates of page pixel (X, Y) under a curved region: false where no segment accepts the pixel.
+__device__ __forceinline__ bool curved_coord(const mn_region_curved& q, int X, int Y, WarpCoord& wc) {
+    const double* curve = q.curve;
+    const int k = q.n_seg;
+    const double s = curve[0];
+    const double px = __ddiv_rn(__dadd_rn((double)X, 0.5), s), py = __ddiv_rn(__dadd_rn((double)Y, 0.5), s);
+    for (int m = 0; m < k; ++m) {
+        const double* top = curve_top(curve, k, m);
+        const double* bot = curve_bottom(curve, k, m);
+        double x0 = top[0], x1 = top[0], y0 = top[1], y1 = top[1];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            x0 = fmin(x0, fmin(top[2 * j], bot[2 * j])), x1 = fmax(x1, fmax(top[2 * j], bot[2 * j]));
+            y0 = fmin(y0, fmin(top[2 * j + 1], bot[2 * j + 1])), y1 = fmax(y1, fmax(top[2 * j + 1], bot[2 * j + 1]));
+        }
+        if (!(px >= x0 && px <= x1 && py >= y0 && py <= y1)) continue;
+        const bool neg = ruling_side(top, bot, px, py, 0.0) < 0.0;
+        if (neg == (ruling_side(top, bot, px, py, 1.0) < 0.0)) continue;
+        double lo = 0.0, hi = 1.0;
+        for (int it = 0; it < 48; ++it) {
+            const double mid = __dmul_rn(0.5, __dadd_rn(lo, hi));
+            if ((ruling_side(top, bot, px, py, mid) < 0.0) == neg) lo = mid; else hi = mid;
+        }
+        const double t = __dmul_rn(0.5, __dadd_rn(lo, hi));
+        const Pt T = bezier(top, t), B = bezier(bot, t);
+        const double dx = __dsub_rn(B.x, T.x), dy = __dsub_rn(B.y, T.y), rx = __dsub_rn(px, T.x), ry = __dsub_rn(py, T.y);
+        const double b = __ddiv_rn(__dadd_rn(__dmul_rn(rx, dx), __dmul_rn(ry, dy)), __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
+        if (!(b >= 0.0 && b <= 1.0)) continue;
+        const double* c = curve + 1;
+        const double a = __dadd_rn(c[m], __dmul_rn(t, __dsub_rn(c[m + 1], c[m])));
+        const double u = __dsub_rn(__dmul_rn(a, (double)q.q.r.sr_w), 0.5), v = __dsub_rn(__dmul_rn(b, (double)q.q.r.sr_h), 0.5);
+        wc = {__float2int_rn(__fmul_rn(__double2float_rn(u), 32.f)), __float2int_rn(__fmul_rn(__double2float_rn(v), 32.f))};
+        return true;
+    }
+    return false;
+}
+
+__device__ __forceinline__ bool region_holds(const mn_region_curved& q, int X, int Y) {
+    if (q.q.kind != MN_REGION_CURVED) return region_holds(q.q, X, Y);
+    if (!region_holds(q.q.r, X, Y)) return false;
+    WarpCoord wc;
+    return curved_coord(q, X, Y, wc) && footprint_holds(q.q.r, wc);
+}
+
+__device__ __forceinline__ void region_blend(const mn_region_curved& q, int X, int Y, int v[3]) {
+    if (q.q.kind != MN_REGION_CURVED) {
+        region_blend(q.q, X, Y, v);
+        return;
+    }
+    WarpCoord wc;
+    curved_coord(q, X, Y, wc);                             // region_holds accepted the pixel
+    footprint_blend(q.q.r, q.q.kx, q.q.ky, wc, v);
+}
+
+__device__ __forceinline__ const mn_region& rect_of(const mn_region_curved& r) { return r.q.r; }
+
 // blockIdx.y = region; one thread per output pixel of its rectangle, those past its pixels (or outside its footprint) exit.  The
 // pixel belongs to the last region of its chain (every region of the page whose rectangle meets this one, in page order) that
 // holds it; only that region's thread writes it, composing the page's background through every region of the chain that holds
@@ -465,6 +566,25 @@ __global__ void warp_perspective_batched_kernel(const mn_warp_perspective_image*
     if (idx >= (long long)im.dh * im.dw) return;
     const int x = (int)(idx % im.dw), y = (int)(idx / im.dw);
     const WarpCoord wc = warp_coord_perspective(im.m, x, y, im.dw, im.dh);
+    int wt[16];
+    warp_taps(wc, wt);
+    uint8_t* o = im.dst + (long long)y * im.dst_pitch + (long long)x * cn;
+    for (int c = 0; c < cn; ++c) o[c] = (uint8_t)warp_cubic_u8(im.src, im.src_pitch, im.h, im.w, cn, c, wc, wt);
+}
+
+__global__ void composite_regions_curved_kernel(const mn_region_curved* __restrict__ regions) {
+    mn_pdl_prologue();
+    composite_pixel(regions);
+}
+
+// blockIdx.y = image; one thread per destination pixel of its [dh][dw][cn] crop, those past its dh*dw pixels exit.
+__global__ void remap_curved_batched_kernel(const mn_remap_curved_image* __restrict__ images, int cn) {
+    mn_pdl_prologue();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const mn_remap_curved_image im = images[blockIdx.y];
+    if (idx >= (long long)im.dh * im.dw) return;
+    const int x = (int)(idx % im.dw), y = (int)(idx / im.dw);
+    const WarpCoord wc = curved_crop_coord(im.curve, im.n_seg, x, y, im.dw, im.dh);
     int wt[16];
     warp_taps(wc, wt);
     uint8_t* o = im.dst + (long long)y * im.dst_pitch + (long long)x * cn;
@@ -574,6 +694,24 @@ extern "C" int mn_composite_regions_quad_u8(const mn_region_quad* regions, int n
     MN_REQUIRE(regions && n > 0 && n <= 65535 && max_pixels > 0, "mn_composite_regions_quad_u8: bad args");
     MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_composite_regions_quad_u8: %lld pixels exceed the grid", max_pixels);
     MN_CUDA_CHECK((mn_launch(composite_regions_quad_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
+                             (cudaStream_t)stream, regions)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_remap_curved_u8_batched(const mn_remap_curved_image* images, int n, int cn, long long max_pixels, void* stream) {
+    MN_REQUIRE(images && n > 0 && n <= 65535 && cn > 0 && cn <= 4 && max_pixels > 0, "mn_remap_curved_u8_batched: bad args");
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_remap_curved_u8_batched: %lld pixels exceed the grid", max_pixels);
+    MN_CUDA_CHECK((mn_launch(remap_curved_batched_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
+                             (cudaStream_t)stream, images, cn)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_composite_regions_curved_u8(const mn_region_curved* regions, int n, long long max_pixels, void* stream) {
+    MN_REQUIRE(regions && n > 0 && n <= 65535 && max_pixels > 0, "mn_composite_regions_curved_u8: bad args");
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_composite_regions_curved_u8: %lld pixels exceed the grid", max_pixels);
+    MN_CUDA_CHECK((mn_launch(composite_regions_curved_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0,
                              (cudaStream_t)stream, regions)));
     MN_LAUNCH_CHECK();
     return MN_OK;

@@ -6,6 +6,7 @@ computation below is a kernel from libmarconet_b200.so.  Activations are NHWC fp
 slices of a concatenation buffer).
 """
 import ctypes
+from typing import NamedTuple
 
 import torch
 
@@ -1204,9 +1205,9 @@ def resize_cubic(items):
     LAUNCHES += 1
 
 
-def _region_records(regions, feather, what, record):
+def _region_records(regions, feather, what, record, extra=0):
     """Validated mn_region records of composite_regions' (page, sr, rect, chain, ...) tuples, their chains, the largest rectangle's
-    pixel count and a device buffer for the ``record``-type table followed by the chains."""
+    pixel count and a device buffer for the ``record``-type table followed by the chains (and ``extra`` bytes after them)."""
     if not regions:
         raise ValueError(f"{what}: no regions")
     if len(regions) > 65535:
@@ -1216,7 +1217,7 @@ def _region_records(regions, feather, what, record):
     dev = regions[0][0].device
     n_chain = sum(len(r[3]) for r in regions)
     isz = ctypes.sizeof(record)
-    buf = torch.empty(len(regions) * isz + 4 * max(1, n_chain), dtype=torch.uint8, device=dev)
+    buf = torch.empty(len(regions) * isz + 4 * max(1, n_chain) + extra, dtype=torch.uint8, device=dev)
     c_base = buf.data_ptr() + len(regions) * isz
     recs, chains, mx = [], [], 0
     for i, (page, sr, rect, chain) in enumerate(r[:4] for r in regions):
@@ -1354,6 +1355,121 @@ def composite_regions_quad(regions, feather):
         out.append(_lib.RegionQuad(rec, kind, kx, ky, 0, (ctypes.c_double * 9)(*n)))
     _upload_records(buf, out, chains)
     _lib.check(_lib.load().mn_composite_regions_quad_u8(_ptr(buf), len(out), mx, _stream()), "mn_composite_regions_quad_u8")
+    LAUNCHES += 1
+
+
+class CurveTable(NamedTuple):
+    """A curved region's curve table (DESIGN.md 7b, "Curved text regions"; layout in include/marconet_b200.h): ``scale`` s (the
+    page's; unused when rectifying), the column fractions ``c`` [c_0 = 0, ..., c_k = 1] and the ``top`` and ``bottom`` curves,
+    3k+1 (x, y) points each (segment m: points 3m .. 3m+3)."""
+    scale: float
+    c: tuple
+    top: tuple
+    bottom: tuple
+
+    def values(self, what):
+        """The fp64 table: s, c_0 .. c_k, the top points, the bottom points (x, y interleaved).  Raises ValueError naming ``what``."""
+        import numpy as np
+        k = len(self.c) - 1
+        top = np.asarray(self.top, np.float64).reshape(-1)
+        bottom = np.asarray(self.bottom, np.float64).reshape(-1)
+        if not 1 <= k <= 8 or top.size != 6 * k + 2 or bottom.size != 6 * k + 2 or float(self.c[0]) != 0.0 \
+                or float(self.c[-1]) != 1.0:
+            raise ValueError(f"{what}: expected 1 <= k <= 8 segments, c_0 = 0, c_k = 1 and 3k+1 (x, y) points per curve")
+        return np.concatenate([[float(self.scale)], np.asarray(self.c, np.float64), top, bottom]), k
+
+
+def _align8(n):
+    return (n + 7) & ~7
+
+
+def remap_curved(items):
+    """Curved text regions rectified, every crop in one launch (mn_remap_curved_u8_batched; DESIGN.md 7b, "Curved text regions"):
+    cv2.remap(src, mapx, mapy, INTER_CUBIC, borderMode=BORDER_REPLICATE) with the fp32 crop maps of each region's curves, OpenCV's
+    own 8-bit path (IPP off).  items: list of (src, dst, curve): uint8 [h, w, cn] and [h_r, w_r, cn] CUDA views with dense pixels
+    (any row stride), h, w <= 32767, and curve a CurveTable whose crop map stays below 2^14 pixels in magnitude
+    (pipeline.plan_regions keeps it so).  The curve tables go up with the records in one copy."""
+    import numpy as np
+    global LAUNCHES
+    if not items:
+        raise ValueError("remap_curved: no images")
+    if len(items) > 65535:
+        raise ValueError("remap_curved: at most 65535 images per launch")
+    dev = items[0][0].device
+    cn = items[0][0].shape[2] if isinstance(items[0][0], torch.Tensor) and items[0][0].dim() == 3 else 3
+    if not 1 <= cn <= 4:
+        raise RuntimeError(f"remap_curved: {cn} channels (1 to 4)")
+    tables = []
+    for i, (src, dst, curve) in enumerate(items):
+        _dense_u8(src, dev, cn, f"remap_curved: image {i}: src")
+        _dense_u8(dst, dev, cn, f"remap_curved: image {i}: dst")
+        if max(src.shape[:2]) > 32767:
+            raise ValueError(f"remap_curved: image {i}: a {src.shape[0]}x{src.shape[1]} source exceeds OpenCV's int16 source "
+                             f"coordinates")
+        tables.append(curve.values(f"remap_curved: image {i}"))
+    isz = ctypes.sizeof(_lib.RemapCurvedImage)
+    n_tab = sum(t.size for t, _ in tables)
+    buf = torch.empty(len(items) * isz + 8 * n_tab, dtype=torch.uint8, device=dev)
+    base, o, recs, mx = buf.data_ptr() + len(items) * isz, 0, [], 0
+    for (src, dst, _), (t, k) in zip(items, tables):
+        (h, w), (dh, dw) = src.shape[:2], dst.shape[:2]
+        recs.append(_lib.RemapCurvedImage(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw, base + 8 * o,
+                                          k, 0))
+        o += t.size
+        mx = max(mx, dh * dw)
+    host = bytes((_lib.RemapCurvedImage * len(recs))(*recs)) + np.concatenate([t for t, _ in tables]).tobytes()
+    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    _lib.check(_lib.load().mn_remap_curved_u8_batched(_ptr(buf), len(recs), cn, mx, _stream()), "mn_remap_curved_u8_batched")
+    LAUNCHES += 1
+
+
+def composite_regions_curved(regions, feather):
+    """composite_regions_quad for pages that also hold curved regions (mn_composite_regions_curved_u8; DESIGN.md 7b, "Curved text
+    regions"), one launch.  regions: list of (page, sr, rect, chain, maps) as composite_regions_quad takes them; maps may also be
+    (curve, kx, ky) with curve a CurveTable whose scale is the page's: a curved region, rect the bounding box of its control points
+    in page pixels widened by one pixel (pipeline.curved_footprint_box).  Rectangles, oriented and perspective regions are
+    composed exactly as composite_regions_quad composes them.  The records, chains and curve tables go up in one copy."""
+    import numpy as np
+    global LAUNCHES
+    tables = {}
+    for i, r in enumerate(regions):
+        if r[4] is not None and isinstance(r[4][0], CurveTable):
+            t, k = r[4][0].values(f"composite_regions_curved: region {i}")
+            if not t[0] >= 1:
+                raise ValueError(f"composite_regions_curved: region {i}: scale {t[0]} < 1")
+            tables[i] = (t, k)
+    n_tab = sum(t.size for t, _ in tables.values())
+    recs, chains, mx, buf = _region_records(regions, int(feather), "composite_regions_curved", _lib.RegionCurved,
+                                            extra=8 + 8 * n_tab)
+    isz = ctypes.sizeof(_lib.RegionCurved)
+    head = len(regions) * isz + 4 * max(1, len(chains))
+    t_off = _align8(buf.data_ptr() + head) - buf.data_ptr()
+    out, o = [], 0
+    for i, (r, rec) in enumerate(zip(regions, recs)):
+        maps = r[4]
+        if maps is None:
+            out.append(_lib.RegionCurved(_lib.RegionQuad(rec, _lib.REGION_RECT, 0.0, 0.0, 0, (ctypes.c_double * 9)()), None, 0, 0))
+            continue
+        n, kx, ky = maps
+        if not (kx > 0 and ky > 0):
+            raise ValueError(f"composite_regions_curved: region {i}: feather slopes kx = {kx}, ky = {ky} must be > 0")
+        if i in tables:
+            t, k = tables[i]
+            out.append(_lib.RegionCurved(_lib.RegionQuad(rec, _lib.REGION_CURVED, kx, ky, 0, (ctypes.c_double * 9)()),
+                                         buf.data_ptr() + t_off + 8 * o, k, 0))
+            o += t.size
+            continue
+        n = [float(v) for row in n for v in row]
+        if len(n) not in (6, 9):
+            raise ValueError(f"composite_regions_curved: region {i}: expected (N 2 x 3 or 3 x 3, kx, ky) or (CurveTable, kx, ky)")
+        kind = _lib.REGION_AFFINE if len(n) == 6 else _lib.REGION_PERSPECTIVE
+        out.append(_lib.RegionCurved(_lib.RegionQuad(rec, kind, kx, ky, 0, (ctypes.c_double * 9)(*n)), None, 0, 0))
+    host = bytes((_lib.RegionCurved * len(out))(*out)) + np.asarray(chains or [0], dtype=np.int32).tobytes()
+    host += bytes(t_off - head)
+    if tables:
+        host += np.concatenate([tables[i][0] for i in sorted(tables)]).tobytes()
+    buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    _lib.check(_lib.load().mn_composite_regions_curved_u8(_ptr(buf), len(out), mx, _stream()), "mn_composite_regions_curved_u8")
     LAUNCHES += 1
 
 

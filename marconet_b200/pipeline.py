@@ -907,7 +907,9 @@ class RegionPlan(NamedTuple):
     ``overlaps`` compares the ``out`` boxes, and its boxes are in the crop's frame, unshifted.  A perspective region (DESIGN.md
     7b, "Perspective text regions") has ``quad`` (the QuadRegion) instead of ``oriented``, and ``matrix`` is its 3 x 3 M.  A
     vertical column (DESIGN.md 7b, "Vertical text columns") is planned as its shape, with ``out`` sized for its restored column,
-    and has ``vertical`` (its VerticalPlan); its ``boxes`` are the given boxes moved onto the line L."""
+    and has ``vertical`` (its VerticalPlan); its ``boxes`` are the given boxes moved onto the line L.  A curved region (DESIGN.md
+    7b, "Curved text regions") has ``curved`` (the CurvedRegion, its points as float pairs) and ``size``, no ``matrix``; its
+    ``rect`` is the bounding box of its control points clipped to the image and ``out`` curved_footprint_box's."""
     image: int
     region: int
     rect: tuple
@@ -920,6 +922,7 @@ class RegionPlan(NamedTuple):
     size: tuple = None
     quad: tuple = None
     vertical: tuple = None
+    curved: tuple = None
 
 
 class OrientedRegion(NamedTuple):
@@ -1186,6 +1189,231 @@ def _plan_quad(reg, H, W, scale, name, column=None):
     return maps, rect, out
 
 
+class CurvedRegion(NamedTuple):
+    """A text line on a curve (DESIGN.md 7b, "Curved text regions"): ``top`` and ``bottom`` are chains of k cubic Beziers
+    (1 <= k <= 8), 3k+1 (x, y) points each in continuous image coordinates (pixel (i, j) covers [j, j+1) x [i, i+1)); segment m of
+    a curve is its points 3m .. 3m+3.  Both run in reading order, ``top`` along the characters' heads.  The line is rectified
+    into a straight crop whose column a runs along the mid curve by arc length between segments and uniformly in t within one
+    (ABCNet's BezierAlign), and whose row b runs from top to bottom along the straight ruling between T(t) and B(t)."""
+    top: tuple
+    bottom: tuple
+
+    @classmethod
+    def from_arc(cls, cx, cy, r_top, r_bottom, start, end):
+        """Text on a circle centred at (cx, cy): the top edge at radius r_top, the bottom edge at r_bottom, read from angle
+        ``start`` to ``end`` (degrees, counter-clockwise on screen: a point is (cx + r cos a, cy - r sin a)), 0 < |end - start| <
+        360.  The top of a seal read left to right is start 150, end 30, r_top > r_bottom.  The arc is split into
+        k = ceil(|end - start| / 90) equal segments whose handles lie along the tangents at r (4/3) tan(phi/4), phi the segment's
+        signed span."""
+        span = float(end) - float(start)
+        if not 0 < abs(span) < 360:
+            raise ValueError(f"from_arc: the span end - start = {span:g} degrees must satisfy 0 < |span| < 360")
+        k = math.ceil(abs(span) / 90)
+        h = 4 / 3 * math.tan(math.radians(span / k) / 4)
+
+        def curve(r):
+            pts = []
+            for m in range(k):
+                a0, a1 = math.radians(start + span * m / k), math.radians(start + span * (m + 1) / k)
+                p0 = (cx + r * math.cos(a0), cy - r * math.sin(a0))
+                p3 = (cx + r * math.cos(a1), cy - r * math.sin(a1))
+                if m == 0:
+                    pts.append(p0)
+                pts += [(p0[0] - h * r * math.sin(a0), p0[1] - h * r * math.cos(a0)),       # p0 + h dP/da(a0)
+                        (p3[0] + h * r * math.sin(a1), p3[1] + h * r * math.cos(a1)), p3]    # p3 - h dP/da(a1)
+            return tuple(pts)
+        return cls(curve(float(r_top)), curve(float(r_bottom)))
+
+
+class CurvedMaps(NamedTuple):
+    """curved_maps' result: ``size`` (w_r, h_r), ``c`` the column fractions [c_0 = 0, ..., c_k = 1], ``kx`` and ``ky`` (the
+    feather slopes, fp32 values), ``t_width`` (W_T), ``top`` and ``bottom`` (the curves' points as float pairs), ``lengths``
+    (the mid curve's sampled length L_m per segment) and ``rulings`` (every sampled ruling length |B(t_i) - T(t_i)|, segment by
+    segment)."""
+    size: tuple
+    c: tuple
+    kx: float
+    ky: float
+    t_width: int
+    top: tuple
+    bottom: tuple
+    lengths: tuple
+    rulings: tuple
+
+    def curve(self, scale):
+        """The kernels' curve table (ops.CurveTable) at page scale ``scale``."""
+        from .ops import CurveTable
+        return CurveTable(float(scale), self.c, self.top, self.bottom)
+
+
+def bezier_point(p, t):
+    """De Casteljau's point of the cubic Bezier p (4 (x, y) points) at t: s = 1 - t and three levels of lerps
+    fl(fl(s A) + fl(t B)) per coordinate, in plain Python floats (every operation rounded on its own)."""
+    s = 1.0 - t
+    out = []
+    for k in (0, 1):
+        a0, a1, a2 = s * p[0][k] + t * p[1][k], s * p[1][k] + t * p[2][k], s * p[2][k] + t * p[3][k]
+        b0, b1 = s * a0 + t * a1, s * a1 + t * a2
+        out.append(s * b0 + t * b1)
+    return out[0], out[1]
+
+
+def _curve_points(region):
+    """(top, bottom, k): the region's points as float pairs.  Raises TypeError / ValueError for anything else."""
+    top, bottom = ([(float(p[0]), float(p[1])) for p in c] for c in region)
+    if any(len(p) != 2 for c in region for p in c):
+        raise ValueError
+    return tuple(top), tuple(bottom), (len(top) - 1) // 3
+
+
+def _curve_samples(top, bottom, k):
+    """Per segment, the 33 samples t_i = i/32 of (T, B): the mid curve's lengths L_m (sqrt of fl(fl(dx dx) + fl(dy dy)) between
+    consecutive Mid = fl(0.5 fl(T + B)), summed in order) and every ruling length, in order."""
+    lengths, rulings = [], []
+    for m in range(k):
+        tp, bp = top[3 * m:3 * m + 4], bottom[3 * m:3 * m + 4]
+        L, prev = 0.0, None
+        for i in range(33):
+            (tx, ty), (bx, by) = bezier_point(tp, i / 32), bezier_point(bp, i / 32)
+            rx, ry = bx - tx, by - ty
+            rulings.append(math.sqrt(rx * rx + ry * ry))
+            mid = (0.5 * (tx + bx), 0.5 * (ty + by))
+            if prev is not None:
+                dx, dy = mid[0] - prev[0], mid[1] - prev[1]
+                L += math.sqrt(dx * dx + dy * dy)
+            prev = mid
+        lengths.append(L)
+    return lengths, rulings
+
+
+def curved_maps(region, scale, t_width=None, t_height=128):
+    """The maps of a CurvedRegion (DESIGN.md 7b, "Curved text regions"), computed here once in plain Python floats with a fixed
+    operation order for the kernels and the numpy twin alike.  Per segment m, 33 samples at t_i = i/32 give the mid curve's
+    length L_m (_curve_samples) and the ruling lengths; L = L_0 + ... + L_{k-1} in order, c_m = (L_0 + ... + L_{m-1}) / L
+    (c_0 = 0, c_k = 1), w_r = round_half_even(L), h_r = round_half_even(the longest sampled ruling), W_T (``t_width``) defaults to
+    round_half_even(w_r 128 / h_r); kx = fl32(s L / W_T), ky = fl32(s h / H_T), h the mean sampled ruling length (summed in
+    order) and H_T = ``t_height``."""
+    import numpy as np
+    from .ops import round_half_even
+    top, bottom, k = _curve_points(region)
+    lengths, rulings = _curve_samples(top, bottom, k)
+    L = 0.0
+    c = [0.0]
+    for v in lengths:
+        L += v
+    acc = 0.0
+    for m in range(1, k):
+        acc += lengths[m - 1]
+        c.append(acc / L)
+    c.append(1.0)
+    w_r, h_r = round_half_even(L), round_half_even(max(rulings))
+    wt = round_half_even(w_r * (128 / h_r)) if t_width is None else int(t_width)
+    hsum = 0.0
+    for v in rulings:
+        hsum += v
+    kx = float(np.float32(scale * L / wt))
+    ky = float(np.float32(scale * (hsum / len(rulings)) / t_height))
+    return CurvedMaps((w_r, h_r), tuple(c), kx, ky, wt, top, bottom, tuple(lengths), tuple(rulings))
+
+
+def curved_footprint_box(region, scale, page_hw):
+    """(X0, Y0, X1, Y1): the output pixels that hold every pixel of a curved region's footprint on a page of page_hw = (H, W)
+    output pixels: the bounding box of all its control points (which holds both curves and every ruling between them) at scale s,
+    widened by one pixel and clipped to the page."""
+    top, bottom, _ = _curve_points(region)
+    xs, ys = [p[0] for p in top + bottom], [p[1] for p in top + bottom]
+    s, (ph, pw) = scale, page_hw
+    return (max(0, math.floor(s * min(xs)) - 1), max(0, math.floor(s * min(ys)) - 1),
+            min(pw, math.ceil(s * max(xs)) + 1), min(ph, math.ceil(s * max(ys)) + 1))
+
+
+def _bezier_rows(maps, b):
+    """numpy fp64 [2, w_r]: the crop map (x, y) of row b (a float) at every column, as mn_remap_curved_u8_batched computes it."""
+    import numpy as np
+    w_r, k = maps.size[0], len(maps.c) - 1
+    a = (np.arange(w_r, dtype=np.float64) + 0.5) / w_r
+    c = np.asarray(maps.c, np.float64)
+    m = np.searchsorted(c[1:k], a, side="right")
+    t = (a - c[m]) / (c[m + 1] - c[m])
+    s = 1.0 - t
+    out = []
+    for k_ in (0, 1):
+        pts = []
+        for curve in (maps.top, maps.bottom):
+            p = np.asarray(curve, np.float64)[:, k_]
+            v = [p[3 * m + j] for j in range(4)]
+            a0, a1, a2 = s * v[0] + t * v[1], s * v[1] + t * v[2], s * v[2] + t * v[3]
+            b0, b1 = s * a0 + t * a1, s * a1 + t * a2
+            pts.append(s * b0 + t * b1)
+        out.append((1.0 - b) * pts[0] + b * pts[1] - 0.5)
+    return np.stack(out)
+
+
+def _plan_curved(reg, H, W, scale, name):
+    """Validates a CurvedRegion of an H x W image: (maps, rect, out)."""
+    try:
+        top, bottom, k = _curve_points(reg)
+        if len(reg) != 2:
+            raise ValueError
+    except (TypeError, ValueError):
+        raise ValueError(f"{name}: expected two curves of (x, y) points, got {reg!r}") from None
+    if not all(math.isfinite(v) for p in top + bottom for v in p):
+        raise ValueError(f"{name}: the control points are not all finite")
+    if len(top) != len(bottom) or len(top) % 3 != 1 or not 1 <= k <= 8:
+        raise ValueError(f"{name}: the curves have {len(top)} and {len(bottom)} points; both need 3k+1 points, 1 <= k <= 8")
+    import numpy as np
+    from .ops import round_half_even
+    lengths, rulings = _curve_samples(top, bottom, k)
+    h_r = round_half_even(max(rulings))
+    if h_r < 1 or round_half_even(sum(lengths)) < 1:
+        raise ValueError(f"{name}: the band is {max(rulings):.4g} pixels high and {sum(lengths):.4g} long (at least 1 each)")
+    for m, v in enumerate(lengths):
+        if v < h_r / 8:
+            raise ValueError(f"{name}: segment {m}'s mid curve is {v:.4g} pixels long, below h_r / 8 = {h_r / 8:g}")
+    for m in range(k):
+        tp, bp = top[3 * m:3 * m + 4], bottom[3 * m:3 * m + 4]
+        turn, lo, hi, prev = 0.0, 0.0, 0.0, None
+        for i in range(33):
+            t = i / 32
+            (tx, ty), (bx, by) = bezier_point(tp, t), bezier_point(bp, t)
+            dt = [3 * ((1 - t) ** 2 * (p[1][j] - p[0][j]) + 2 * (1 - t) * t * (p[2][j] - p[1][j]) + t * t * (p[3][j] - p[2][j]))
+                  for p in (tp, bp) for j in (0, 1)]
+            rx, ry = bx - tx, by - ty
+            for b in (0.0, 0.25, 0.5, 0.75, 1.0):
+                jac = ((1 - b) * dt[0] + b * dt[2]) * ry - ((1 - b) * dt[1] + b * dt[3]) * rx
+                if not jac > 0:
+                    raise ValueError(f"{name}: the band folds or runs against its reading order (Jacobian {jac:.4g} <= 0 at "
+                                     f"segment {m}, t = {t:g}, b = {b:g}; give top and bottom as the line is read)")
+            if prev is not None:
+                turn += math.atan2(prev[0] * ry - prev[1] * rx, prev[0] * rx + prev[1] * ry)
+                lo, hi = min(lo, turn), max(hi, turn)
+            prev = (rx, ry)
+        if hi - lo > math.pi / 2:
+            raise ValueError(f"{name}: the ruling B - T turns by {math.degrees(hi - lo):.4g} degrees within segment {m} "
+                             f"(at most 90)")
+    if max(rulings) > 4 * min(rulings):
+        raise ValueError(f"{name}: the longest ruling {max(rulings):.4g} is more than 4 times the shortest {min(rulings):.4g}")
+    maps = curved_maps((top, bottom), scale)
+    c = maps.c
+    m = max(j for j in range(k) if c[j] <= 0.5)
+    t = (0.5 - c[m]) / (c[m + 1] - c[m])
+    (tx, ty), (bx, by) = bezier_point(top[3 * m:3 * m + 4], t), bezier_point(bottom[3 * m:3 * m + 4], t)
+    cx, cy = 0.5 * tx + 0.5 * bx, 0.5 * ty + 0.5 * by
+    if not (0 <= cx < W and 0 <= cy < H):
+        raise ValueError(f"{name}: the mid point ({cx:.6g}, {cy:.6g}) is outside the {W}x{H} image")
+    (w_r, h_r), wt = maps.size, maps.t_width
+    if max(w_r, h_r, wt, H, W) > 32767:
+        raise ValueError(f"{name}: crop {w_r}x{h_r}, restored width {wt} or image {W}x{H} exceeds 32767 pixels "
+                         f"(OpenCV's remap holds source coordinates as int16)")
+    reach = max(np.abs(_bezier_rows(maps, b)).max() for b in (0.5 / h_r, (h_r - 0.5) / h_r))
+    if not reach < 2.0 ** 14:
+        raise ValueError(f"{name}: the crop map reaches {reach:.6g} pixels, beyond OpenCV's int16 remap coordinates (2^14)")
+    out = curved_footprint_box((top, bottom), scale, (scale * H, scale * W))
+    xs, ys = [p[0] for p in top + bottom], [p[1] for p in top + bottom]
+    rect = (max(0, math.floor(min(xs))), max(0, math.floor(min(ys))), min(W, math.ceil(max(xs))), min(H, math.ceil(max(ys))))
+    return maps, rect, out
+
+
 class VerticalRegion(NamedTuple):
     """A column of upright characters read top to bottom (DESIGN.md 7b, "Vertical text columns").  ``shape`` is its footprint: an
     integer rectangle (x0, y0, x1, y1), an OrientedRegion or a QuadRegion, with tl -> tr across the column and tl -> bl down it.
@@ -1312,7 +1540,13 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
     interior angle outside [30, 150] degrees, foreshortening beyond 4, the centre outside the image, a side over 32767 pixels,
     a page map whose denominator is not positive over the footprint box or whose fixed-point coordinates leave +-2^30.
     A VerticalRegion (DESIGN.md 7b, "Vertical text columns") is validated as its shape, its labels and boxes in its crop C's frame,
-    and further rejected for a shape that is itself a VerticalRegion and for vertical_plan's errors."""
+    and further rejected for a shape that is itself a VerticalRegion or a CurvedRegion and for vertical_plan's errors.
+    A CurvedRegion (DESIGN.md 7b, "Curved text regions") is rejected for points that are not finite, curves without 3k+1 points,
+    with different k or k outside [1, 8], a band under one pixel, a segment whose mid curve is shorter than h_r / 8, a Jacobian of
+    P(t, b) = (1 - b) T + b B that is not positive on the 33 x 5 grid of a segment (folds, mirrored or reversed reading order), a
+    ruling B - T that turns by more than 90 degrees within a segment, a longest ruling over 4 times the shortest, the mid point
+    at a = 0.5 outside the image, a side over 32767 pixels and a crop map beyond +-2^14; its labels and boxes are in its crop's
+    frame."""
     if isinstance(scale, bool) or not isinstance(scale, int) or not 1 <= scale <= 8:
         raise ValueError(f"scale must be an integer in [1, 8], got {scale!r}")
     if feather is not None and (isinstance(feather, bool) or not isinstance(feather, int) or feather < 0):
@@ -1335,6 +1569,8 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
                 vreg, rect = rect, rect.shape
                 if isinstance(rect, VerticalRegion):
                     raise ValueError(f"{name}: the shape of a VerticalRegion is itself a VerticalRegion")
+                if isinstance(rect, CurvedRegion):
+                    raise ValueError(f"{name}: the shape of a VerticalRegion is a CurvedRegion (curved columns are not supported)")
                 if lab is not None:
                     lab = [int(v) for v in torch.as_tensor(lab, dtype=torch.long).reshape(-1).tolist()]
                 if bx is not None and lab is None:
@@ -1350,6 +1586,9 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
                 cols = (0, maps.size[0])
             elif isinstance(rect, QuadRegion):
                 maps, (x0, y0, x1, y1), out = _plan_quad(rect, H, W, s, name, column)
+                cols = (0, maps.size[0])
+            elif isinstance(rect, CurvedRegion):
+                maps, (x0, y0, x1, y1), out = _plan_curved(rect, H, W, s, name)
                 cols = (0, maps.size[0])
             else:
                 try:
@@ -1381,7 +1620,11 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
                 bx = [[float(b[0]) - dx, float(b[1]) - dy, float(b[2]) - dx, float(b[3]) - dy] for b in bx]
             overlaps = [first + j for j, q in enumerate(plan[first:]) if max(out[0], q.out[0]) < min(out[2], q.out[2])
                         and max(out[1], q.out[1]) < min(out[3], q.out[3])]
-            corners = tuple((float(p[0]), float(p[1])) for p in rect) if maps else ()
+            corners = tuple((float(p[0]), float(p[1])) for p in rect) if maps and not isinstance(rect, CurvedRegion) else ()
+            if isinstance(rect, CurvedRegion):
+                plan.append(RegionPlan(i, r, (x0, y0, x1, y1), out, overlaps, lab, bx, size=maps.size,
+                                       curved=CurvedRegion(maps.top, maps.bottom)))
+                continue
             if isinstance(rect, QuadRegion):
                 extra = (None, maps.matrix, maps.size, QuadRegion(*corners))
             else:
@@ -1458,7 +1701,12 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     cells side by side as the line L (vertical_plan; every column of the call in one mn_vertical_layout_u8_batched launch before
     restore_images), restores L to T and puts T back into the column T_col [H_c, W_c] (one mn_vertical_unlayout_u8_batched launch
     after it), which is composed as its shape composes T.  Its labels and boxes are given and returned in C's frame; its entry's
-    sr_u8 is T_col, and it gains line_u8 (T) and cells ([c_0, ..., c_n])."""
+    sr_u8 is T_col, and it gains line_u8 (T) and cells ([c_0, ..., c_n]).
+    A CurvedRegion (DESIGN.md 7b, "Curved text regions") is restored from its rectified crop C = cv2.remap(img, fl32(mapx),
+    fl32(mapy), INTER_CUBIC, BORDER_REPLICATE) with curved_maps' crop map (every curved crop of the call in one
+    mn_remap_curved_u8_batched launch), its labels and boxes given and returned in C's frame, and its entry gains ``size``
+    ((w_r, h_r)).  Each page pixel of its footprint is inverted onto T by bisection along the curves, feathered on all four
+    sides, and a call that holds one composes every region with mn_composite_regions_curved_u8."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     plan = plan_regions([im.shape[:2] for im in imgs], regions, labels, boxes, scale, feather)
@@ -1471,17 +1719,21 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         crops = [dimg[p.image][p.rect[1]:p.rect[3], p.rect[0]:p.rect[2]] for p in plan]
         oriented = [k for k, p in enumerate(plan) if p.oriented is not None]
         quads = [k for k, p in enumerate(plan) if p.quad is not None]
-        if oriented or quads:                            # every region of a kind rectified in one launch
-            n_crop = [3 * plan[k].size[0] * plan[k].size[1] for k in oriented + quads]
+        curved = [k for k, p in enumerate(plan) if p.curved is not None]
+        if oriented or quads or curved:                  # every region of a kind rectified in one launch
+            n_crop = [3 * plan[k].size[0] * plan[k].size[1] for k in oriented + quads + curved]
             cbuf = torch.empty(sum(n_crop), dtype=torch.uint8, device=dev)
             o = 0
-            for k, nb in zip(oriented + quads, n_crop):
+            for k, nb in zip(oriented + quads + curved, n_crop):
                 crops[k] = cbuf[o:o + nb].view(plan[k].size[1], plan[k].size[0], 3)
                 o += nb
             if oriented:
                 ops.warp_affine([(dimg[plan[k].image], crops[k], plan[k].matrix) for k in oriented])
             if quads:
                 ops.warp_perspective([(dimg[plan[k].image], crops[k], plan[k].matrix) for k in quads])
+            if curved:
+                ops.remap_curved([(dimg[plan[k].image], crops[k], curved_maps(plan[k].curved, scale).curve(scale))
+                                  for k in curved])
         verts = [k for k, p in enumerate(plan) if p.vertical is not None]
         if verts:                                        # every column laid out as a line in one launch
             lines = _flat_views([(plan[k].vertical.line_height, len(plan[k].vertical.heights) * plan[k].vertical.size[0])
@@ -1505,7 +1757,14 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         ok = [k for k, r in enumerate(res) if "error" not in r]
         if ok:                                           # a column composes its T_col where any other region composes its T
             items = [(pages[plan[k].image], ts[k], plan[k].out, chain) for k, chain in zip(ok, region_chains(plan, ok))]
-            if quads:
+            if curved:
+                maps = [curved_maps(plan[k].curved, scale, *ts[k].shape[1::-1]) if plan[k].curved is not None else
+                        quad_maps(plan[k].quad, scale, *ts[k].shape[1::-1]) if plan[k].quad is not None else
+                        oriented_maps(plan[k].oriented, scale, *ts[k].shape[1::-1]) if plan[k].oriented is not None else None
+                        for k in ok]
+                ops.composite_regions_curved([it + (m and ((m.curve(scale) if isinstance(m, CurvedMaps) else m.page_map),
+                                                           m.kx, m.ky),) for it, m in zip(items, maps)], feather)
+            elif quads:
                 maps = [quad_maps(plan[k].quad, scale, *ts[k].shape[1::-1]) if plan[k].quad is not None else
                         oriented_maps(plan[k].oriented, scale, *ts[k].shape[1::-1]) if plan[k].oriented is not None else None
                         for k in ok]
@@ -1530,7 +1789,7 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         elif "boxes" in r and p.vertical is not None:
             entry = dict(sr_u8=srs[k], segments=r["segments"], labels=r["labels"], boxes=column_boxes(p.vertical, r["boxes"]))
         elif "boxes" in r:
-            x0, y0 = (0, 0) if p.oriented or p.quad else p.rect[:2]
+            x0, y0 = (0, 0) if p.oriented or p.quad or p.curved else p.rect[:2]
             entry = dict(sr_u8=srs[k], segments=r["segments"], labels=r["labels"],
                          boxes=[[b[0] + x0, b[1] + y0, b[2] + x0, b[3] + y0] for b in r["boxes"]])
         else:
@@ -1539,6 +1798,8 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
             entry.update(line_u8=lines[k], cells=list(p.vertical.cells))
         if (p.oriented or p.quad) and "error" not in r:
             entry.update(matrix=p.matrix.copy(), size=p.size)
+        if p.curved and "error" not in r:
+            entry.update(size=p.size)
         out[p.image]["regions"].append(entry)
     return out
 

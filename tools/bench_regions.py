@@ -4,7 +4,7 @@ the pages, then cv2's cubic resize of every page and of every restored region (I
 (oracle/regions.py).
 
     MN_MODULE_GRAPHS=0 python tools/bench_regions.py [--pages 8] [--lines 12] [--passes 3] [--scale 4] [--max-angle 0]
-                                                     [--perspective 0]
+                                                     [--perspective 0] [--curved]
 
 The pages are seeded: tools/bench_images.make_image_set lines (the reference test set's sizes and lines 2 to 4 times wider than the
 LQ canvas) pasted one under another onto a noise background, each line a region with its character boxes.  The arms alternate pass
@@ -31,8 +31,18 @@ pipeline.VerticalRegion of its rectangle with boxes in the column's frame (DESIG
 host arm then lays every column out as a line with numpy (oracle/vertical_regions.py), runs restore_images(to_host=True) on the
 lines, puts each restored line back into a column with numpy, resizes the pages and each column with cv2 and blends with the
 numpy feather; the timed kernels are mn_vertical_layout_u8_batched, mn_vertical_unlayout_u8_batched, mn_resize_cubic_u8_batched
-and mn_composite_regions_u8.  --profile adds one restore_regions pass under torch.profiler (after the timed passes, in the same
-run) and prints the device time of every kernel of that pass by name.
+and mn_composite_regions_u8.
+
+With --curved every line is pasted on a curve, alternately a seal-like arc of 40 to 120 degrees (pipeline.CurvedRegion.from_arc)
+and a two-segment S-curve, and given as a pipeline.CurvedRegion (DESIGN.md section 7b, "Curved text regions").  The lines are the
+reference test set's sizes up to 49 rows, so that the host arm's numpy inversion stays within minutes.  The host arm then
+rectifies each line with cv2.remap through the numpy twin's crop maps (oracle/curved_regions.py), runs
+restore_images(to_host=True) on the crops, resizes the pages with cv2, inverts every pixel of each footprint box with the twin,
+remaps each restored line back with cv2.remap and blends it with the numpy feather; the timed kernels are
+mn_remap_curved_u8_batched, mn_resize_cubic_u8_batched and mn_composite_regions_curved_u8.
+
+--profile adds one restore_regions pass under torch.profiler (after the timed passes, in the same run) and prints the device time
+of every kernel of that pass by name.
 """
 import argparse
 import json
@@ -155,6 +165,59 @@ def make_perspective_pages(n_pages, n_lines, max_ratio, seed=0):
     return pages, regs, labs, bxs
 
 
+def make_curved_pages(n_pages, n_lines, seed=0):
+    """Lines of the reference test set's sizes up to 49 rows, each bent into an arc (even lines: 40 to 120 degrees, read left to
+    right over its top) or a two-segment S-curve (odd lines) and pasted (nearest pixel, each crop pixel to its rounded crop-map
+    position) one under another onto a noise page: (pages, regions, labels, boxes), regions CurvedRegions and boxes in each line's
+    rectified frame."""
+    from bench_images import TESTSET_SIZES
+    from marconet_b200.pipeline import CurvedRegion, curved_maps
+    from oracle import curved_regions as R
+    rng = np.random.default_rng(seed + 1)
+    sizes = [hw for hw in TESTSET_SIZES if hw[0] <= 49]
+    pages, regs, labs, bxs = [], [], [], []
+    for p in range(n_pages):
+        lines, W, H = [], 0, 8.0
+        for j in range(n_lines):
+            h, w = sizes[(p * n_lines + j) % len(sizes)]
+            if j % 2 == 0:
+                phi = np.radians(rng.uniform(40, 120))
+                r = w / phi
+                half = np.degrees(phi) / 2
+                ro = r + h / 2
+                bw, bh = 2 * ro * np.sin(phi / 2), ro - (r - h / 2) * np.cos(phi / 2)
+                reg = CurvedRegion.from_arc(8 + bw / 2, H + ro, ro, r - h / 2, 90 + half, 90 - half)
+            else:
+                amp = rng.uniform(0.02, 0.06) * w
+                xs = np.linspace(0, w, 7)
+                ys = H + amp + amp * np.array([0, -1, 1, 0, -1, 1, 0])
+                bw, bh = w, h + 2 * amp
+                reg = CurvedRegion(tuple((8 + x, y) for x, y in zip(xs, ys)), tuple((8 + x, y + h) for x, y in zip(xs, ys)))
+            lines.append((reg, h, w))
+            W, H = max(W, int(bw) + 24), H + bh + 8
+        H = int(H) + 8
+        page = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
+        rr, ll, bb = [], [], []
+        for reg, h, w in lines:
+            m = curved_maps(reg, 1)
+            (w_r, h_r) = m.size
+            pitch = 28 * h_r / 32
+            k = max(1, int(w_r // pitch))
+            line = rng.integers(0, 256, (h_r, w_r, 3), dtype=np.uint8)
+            mx, my = R.crop_map(m)
+            xi, yi = np.rint(mx).astype(np.int64), np.rint(my).astype(np.int64)
+            inside = (xi >= 0) & (xi < W) & (yi >= 0) & (yi < H)
+            page[yi[inside], xi[inside]] = line[inside]
+            rr.append(reg)
+            bb.append([[int(j * pitch + 0.15 * pitch), 0, int(j * pitch + 0.85 * pitch), h_r] for j in range(k)])
+            ll.append(rng.integers(0, 6735, k).tolist())
+        pages.append(page)
+        regs.append(rr)
+        labs.append(ll)
+        bxs.append(bb)
+    return pages, regs, labs, bxs
+
+
 def make_vertical_pages(n_pages, n_cols, max_cells, seed=0):
     """make_image_set lines turned into columns: each line's first max_cells characters, cut at their boxes and resized (nearest
     pixel) to h x h squares, stacked one under another and the columns pasted side by side (8-pixel gaps) onto a noise page:
@@ -216,6 +279,44 @@ def host_path_vertical(m, pages, regs, labels, boxes, s, feather, max_lines):
             r = (s * x0, s * y0, s * x1, s * y1)
             p = cv2.resize(np.ascontiguousarray(tc[..., ::-1]), (r[2] - r[0], r[3] - r[1]), interpolation=cv2.INTER_CUBIC)
             o[r[1]:r[3], r[0]:r[2]] = regions.blend(o[r[1]:r[3], r[0]:r[2]], p, regions.alpha(r, o.shape[:2], feather))
+            k += 1
+        out.append(o)
+    return out
+
+
+def host_path_curved(m, pages, regs, labels, boxes, s, feather, max_lines):
+    """cv2.remap rectify through the twin's crop maps, restore_images on the crops, cv2 background, the twin's inversion of every
+    pixel of each footprint box, cv2.remap of each restored line back at those T coordinates and the numpy blend."""
+    import cv2
+    from marconet_b200 import pipeline
+    from oracle import curved_regions as R
+    crops, labs, bxs = [], [], []
+    for pg, rr, ll, bb in zip(pages, regs, labels, boxes):
+        for reg, lab, bx in zip(rr, ll, bb):
+            mx, my = R.crop_map(pipeline.curved_maps(reg, 1))
+            crops.append(cv2.remap(pg, mx.astype(np.float32), my.astype(np.float32), cv2.INTER_CUBIC,
+                                   borderMode=cv2.BORDER_REPLICATE))
+            labs.append(lab)
+            bxs.append(bx)
+    res = pipeline.restore_images(*m, crops, labs, bxs, max_lines=max_lines, to_host=True)
+    out, k = [], 0
+    for pg, rr in zip(pages, regs):
+        o = cv2.resize(pg, (0, 0), fx=s, fy=s, interpolation=cv2.INTER_CUBIC)
+        for reg in rr:
+            t = res[k]["sr_u8"]
+            th, tw = t.shape[:2]
+            n = pipeline.curved_maps(reg, s, tw)
+            x0, y0, x1, y1 = pipeline.curved_footprint_box(reg, s, o.shape[:2])
+            qx, qy = np.meshgrid((np.arange(x0, x1) + 0.5) / s, (np.arange(y0, y1) + 0.5) / s)
+            ok, mm, tt, bb = R.invert(n, qx, qy)
+            u, v = R.t_maps(n, mm, tt, bb, (th, tw))
+            u, v = np.where(ok, u, 0).reshape(qx.shape).astype(np.float32), np.where(ok, v, 0).reshape(qx.shape).astype(np.float32)
+            xq, yq = np.rint(u * np.float32(32)).astype(np.int64), np.rint(v * np.float32(32)).astype(np.int64)
+            mask = ok.reshape(qx.shape) & (xq >= -16) & (xq < 32 * tw - 16) & (yq >= -16) & (yq < 32 * th - 16)
+            a = R.feather_alpha(xq, yq, (th, tw), n.kx, n.ky, feather)
+            p = cv2.remap(np.ascontiguousarray(t[..., ::-1]), u, v, cv2.INTER_CUBIC, borderMode=cv2.BORDER_REPLICATE)
+            sl = o[y0:y1, x0:x1]
+            sl[mask] = R.blend(sl, p, a)[mask]
             k += 1
         out.append(o)
     return out
@@ -328,12 +429,15 @@ def main():
                     help="shrink every line's far end by a foreshortening ratio up to this (> 1; perspective regions)")
     ap.add_argument("--vertical", action="store_true", help="vertical text columns (--lines columns per page)")
     ap.add_argument("--cells", type=int, default=16, help="characters per column with --vertical")
+    ap.add_argument("--curved", action="store_true", help="arcs and S-curves (curved regions)")
     ap.add_argument("--profile", action="store_true", help="one more restore_regions pass under torch.profiler")
     args = ap.parse_args()
     if args.vertical and (args.max_angle > 0 or args.perspective):
         sys.exit("--vertical does not combine with --max-angle or --perspective")
     if args.perspective and (args.max_angle > 0 or not 1 < args.perspective <= 4):
         sys.exit("--perspective takes a ratio in (1, 4] and does not combine with --max-angle")
+    if args.curved and (args.vertical or args.max_angle > 0 or args.perspective):
+        sys.exit("--curved does not combine with --vertical, --max-angle or --perspective")
     if not torch.cuda.is_available():
         sys.exit("bench_regions.py needs a CUDA device")
     cv2.ipp.setUseIPP(False)
@@ -350,6 +454,8 @@ def main():
     oriented, perspective = args.max_angle > 0, args.perspective > 1
     if args.vertical:
         pages, rects, labels, boxes = make_vertical_pages(args.pages, args.lines, args.cells)
+    elif args.curved:
+        pages, rects, labels, boxes = make_curved_pages(args.pages, args.lines)
     elif perspective:
         pages, rects, labels, boxes = make_perspective_pages(args.pages, args.lines, args.perspective)
     elif oriented:
@@ -362,6 +468,8 @@ def main():
     if args.vertical:
         events = {"mn_vertical_layout_u8_batched": [], "mn_vertical_unlayout_u8_batched": [], "mn_resize_cubic_u8_batched": [],
                   "mn_composite_regions_u8": []}
+    elif args.curved:
+        events = {"mn_remap_curved_u8_batched": [], "mn_resize_cubic_u8_batched": [], "mn_composite_regions_curved_u8": []}
     elif perspective:
         events = {"mn_warp_perspective_u8_batched": [], "mn_resize_cubic_u8_batched": [], "mn_composite_regions_quad_u8": []}
     elif oriented:
@@ -389,7 +497,8 @@ def main():
         return [o["image"] for o in out]
 
     def host():
-        path = host_path_vertical if args.vertical else host_path_perspective if perspective else \
+        path = host_path_vertical if args.vertical else host_path_curved if args.curved else \
+            host_path_perspective if perspective else \
             host_path_oriented if oriented else host_path
         return path(m, pages, rects, labels, boxes, s, feather, args.max_lines)
 
@@ -413,6 +522,7 @@ def main():
     common = dict(pages=args.pages, lines_per_page=args.lines, scale=s, feather=feather, max_lines=args.max_lines,
                   max_angle=args.max_angle, **({"perspective": args.perspective} if perspective else {}),
                   **({"vertical": True, "cells_per_column": args.cells} if args.vertical else {}),
+                  **({"curved": True} if args.curved else {}),
                   page_sizes=[list(p.shape[:2]) for p in pages], output_megapixels=round(out_px / 1e6, 2),
                   module_graphs=os.environ.get("MN_MODULE_GRAPHS"), same_bytes=same, max_abs_diff=diff, **card)
     for name, ts in times.items():
@@ -435,7 +545,7 @@ def main():
         top = sorted(dev_ms.items(), key=lambda kv: -sum(kv[1]))
         print(json.dumps(dict(metric="regions_profile", device_ms_total=round(total, 3),
                               kernels={k: dict(calls=len(v), ms=round(sum(v), 4)) for k, v in top
-                                       if "vertical" in k or "composite" in k or "resize_cubic" in k or k in dict(top[:8])},
+                                       if "vertical" in k or "curved" in k or "composite" in k or "resize_cubic" in k or k in dict(top[:8])},
                               **common)), flush=True)
     if not same:
         sys.exit("the arms' bytes differ")
