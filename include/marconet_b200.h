@@ -666,6 +666,48 @@ typedef struct {
 } mn_region_curved;
 int mn_composite_regions_curved_u8(const mn_region_curved* regions, int n, long long max_pixels, void* stream);
 
+/* Text blocks split into lines (DESIGN.md section 7b, "Text blocks").  Block i reads the crop C = img[y0:y1][x0:x1] (h x w,
+ * three channels, in place through the image's pitch) and runs on the transposed crop when `vertical` is set: L = h, M = w
+ * (horizontal) or L = w, M = h (vertical) are the lengths across and along its lines.  mn_find_lines_u8 issues four launches for
+ * every block of a call, whatever their number:
+ *   1. histogram: hist[g] = #{g(x, y) = g}, g = (c0 + c1 + c2 + 1) / 3, tiles of 32 x 32 pixels, blockIdx.y = block;
+ *   2. threshold, one thread per block: t = OpenCV's Otsu threshold of hist (getThreshVal_Otsu_8u's fp64 loop, every operation
+ *      rounded on its own), D = #{g <= t}; ink = polarity, or for MN_INK_AUTO dark (g <= t) iff 2 D <= h w, else light (g > t);
+ *   3. profile over the tiles: for every index l < L, prof[l] = the ink count, prof[L + l] = M - (the least ink index along the
+ *      line), prof[2 L + l] = the largest ink index along the line + 1 (0 where there is no ink);
+ *   4. segmentation, one CTA per block: the runs of indices with prof[l] >= m (m = min_ink, default max(1, M / 128)), merged
+ *      across gaps <= G (gap, default max(1, Hm / 4), Hm the lower median of the run lengths), those shorter than min_height
+ *      dropped (default max(2, Hm' / 3), Hm' the lower median of the merged lengths), each kept line padded by
+ *      p = (b - a + 3) / 4 and bounded by its neighbours' midpoints, its extent along the line the ink's over [a, b) padded by p.
+ * out->rect[k] is line k in image pixels (x0, y0, x1, y1) in reading order: top to bottom, right to left for a vertical block.
+ * out->n_lines is the number of lines, or minus it when it exceeds MN_BLOCK_MAX_LINES (then no rectangle is written).
+ * hist, prof and scratch are device memory of 256, 3 L and 2 L + 4 int32 values; work (work_bytes) covers every hist and prof
+ * of the call and is zeroed by the call.  max_tiles >= every block's ceil(w / 32) ceil(h / 32).  blocks: DEVICE array
+ * (validated by the caller: 1 <= w, h <= 32767, the crop inside its image). */
+#define MN_BLOCK_MAX_LINES 256
+#define MN_INK_AUTO 0
+#define MN_INK_DARK 1
+#define MN_INK_LIGHT 2
+typedef struct {
+    int32_t n_lines;
+    int32_t threshold;
+    int32_t ink;                /* MN_INK_DARK or MN_INK_LIGHT */
+    int32_t pad;
+    int32_t rect[MN_BLOCK_MAX_LINES][4];
+} mn_block_lines;
+typedef struct {
+    const uint8_t* img;         /* row 0 of the image */
+    int64_t pitch;
+    int32_t x0, y0, w, h;       /* the crop */
+    int32_t vertical, polarity; /* polarity: MN_INK_AUTO, MN_INK_DARK or MN_INK_LIGHT */
+    int32_t min_ink, gap, min_height, pad;   /* 0: the default */
+    int32_t* hist;
+    int32_t* prof;
+    int32_t* scratch;
+    mn_block_lines* out;
+} mn_text_block;
+int mn_find_lines_u8(const mn_text_block* blocks, int n, long long max_tiles, void* work, long long work_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -152,6 +152,21 @@ class RegionCurved(Structure):
     _fields_ = [("q", RegionQuad), ("curve", c_void_p), ("n_seg", c_int32), ("pad", c_int32)]
 
 
+BLOCK_MAX_LINES = 256   # MN_BLOCK_MAX_LINES
+INK_AUTO, INK_DARK, INK_LIGHT = 0, 1, 2
+
+
+class BlockLines(Structure):
+    _fields_ = [("n_lines", c_int32), ("threshold", c_int32), ("ink", c_int32), ("pad", c_int32),
+                ("rect", c_int32 * (4 * BLOCK_MAX_LINES))]
+
+
+class TextBlock(Structure):
+    _fields_ = [("img", c_void_p), ("pitch", c_int64), ("x0", c_int32), ("y0", c_int32), ("w", c_int32), ("h", c_int32),
+                ("vertical", c_int32), ("polarity", c_int32), ("min_ink", c_int32), ("gap", c_int32), ("min_height", c_int32),
+                ("pad", c_int32), ("hist", c_void_p), ("prof", c_void_p), ("scratch", c_void_p), ("out", c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -211,6 +226,7 @@ SYMBOLS = {
     "mn_vertical_unlayout_u8_batched": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_remap_curved_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
     "mn_composite_regions_curved_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
+    "mn_find_lines_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

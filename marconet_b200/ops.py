@@ -1522,6 +1522,58 @@ def vertical_layout(items):
     _vertical_gather(items, "vertical_layout", 3, "mn_vertical_layout_u8_batched")
 
 
+def block_lines_dtype():
+    """numpy view of an mn_block_lines record (the output of mn_find_lines_u8)."""
+    import numpy as np
+    return np.dtype([("n_lines", "<i4"), ("threshold", "<i4"), ("ink", "<i4"), ("pad", "<i4"),
+                     ("rect", "<i4", (_lib.BLOCK_MAX_LINES, 4))])
+
+
+def find_lines(blocks):
+    """Text blocks split into lines, every block in four launches whatever their number (mn_find_lines_u8; DESIGN.md 7b, "Text
+    blocks").  blocks: list of (img, rect, vertical, polarity, min_ink, gap, min_height): img a uint8 [H, W, 3] CUDA view with
+    dense pixels (any row stride) read in place, rect (x0, y0, x1, y1) a non-empty crop inside it with sides <= 32767, vertical a
+    bool, polarity _lib.INK_AUTO / INK_DARK / INK_LIGHT, and min_ink, gap, min_height positive integers or None for the
+    default.  Returns the uint8 CUDA tensor of the blocks' mn_block_lines records, in order (read it back as
+    ``block_lines_dtype()``)."""
+    import numpy as np
+    global LAUNCHES
+    if not blocks:
+        raise ValueError("find_lines: no blocks")
+    if len(blocks) > 65535:
+        raise ValueError("find_lines: at most 65535 blocks per launch")
+    dev = blocks[0][0].device
+    osz, rsz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.TextBlock)
+    dims = []
+    for i, (img, rect, vertical, polarity, *knobs) in enumerate(blocks):
+        _dense_u8(img, dev, 3, f"find_lines: block {i}: img")
+        x0, y0, x1, y1 = (int(v) for v in rect)
+        if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
+            raise ValueError(f"find_lines: block {i}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
+                             f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
+        if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or \
+                any(v is not None and not 1 <= v < 2 ** 31 for v in knobs):
+            raise ValueError(f"find_lines: block {i}: bad polarity {polarity!r} or min_ink / gap / min_height {knobs!r}")
+        dims.append((x0, y0, x1 - x0, y1 - y0, y1 - y0 if not vertical else x1 - x0))
+    n_work = sum(256 + 3 * d[4] for d in dims)
+    n_scratch = sum(2 * d[4] + 4 for d in dims)
+    head = len(blocks) * (osz + rsz)
+    buf = torch.empty(head + 4 * (n_work + n_scratch), dtype=torch.uint8, device=dev)
+    out, work = buf.data_ptr(), buf.data_ptr() + head
+    scratch, w, s, recs, tiles = work + 4 * n_work, 0, 0, [], 0
+    for i, ((img, _, vertical, polarity, min_ink, gap, min_height), (x0, y0, bw, bh, L)) in enumerate(zip(blocks, dims)):
+        recs.append(_lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, min_ink or 0,
+                                   gap or 0, min_height or 0, 0, work + 4 * w, work + 4 * (w + 256), scratch + 4 * s, out + i * osz))
+        w += 256 + 3 * L
+        s += 2 * L + 4
+        tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
+    rec = buf[len(blocks) * osz:head]
+    rec.copy_(torch.from_numpy(np.frombuffer(bytes((_lib.TextBlock * len(recs))(*recs)), dtype=np.uint8).copy()))
+    _lib.check(_lib.load().mn_find_lines_u8(_ptr(rec), len(recs), tiles, work, 4 * n_work, _stream()), "mn_find_lines_u8")
+    LAUNCHES += 4
+    return buf[:len(blocks) * osz]
+
+
 def vertical_unlayout(items):
     """Restored lines put back into columns, every column in one launch (mn_vertical_unlayout_u8_batched; DESIGN.md 7b,
     "Vertical text columns").  items: list of (T, T_col, cells): uint8 [128, W_T, 3] and [H_c, W_c, 3] CUDA views with dense

@@ -1525,6 +1525,183 @@ def _per_image(v, n, what):
     return v
 
 
+class TextBlock(NamedTuple):
+    """A block of text lines inside an image (DESIGN.md 7b, "Text blocks").  ``rect``: an integer rectangle (x0, y0, x1, y1)
+    around the lines.  ``direction``: "horizontal" (lines read top to bottom) or "vertical" (columns read right to left).
+    ``min_ink``, ``gap``, ``min_height``: positive integers in place of the segmentation's defaults.  ``polarity``: "auto" (the
+    minority side of the Otsu threshold is ink), "dark" or "light".  find_lines splits it into lines; restore_regions restores
+    each line in its place."""
+    rect: object
+    direction: str = "horizontal"
+    min_ink: object = None
+    gap: object = None
+    min_height: object = None
+    polarity: str = "auto"
+
+
+_INK = {"auto": 0, "dark": 1, "light": 2}
+
+
+def _check_block(blk, H, W, name):
+    """The rectangle (x0, y0, x1, y1) of the TextBlock ``blk`` of an H x W image, validated.  Raises ValueError naming ``name``."""
+    try:
+        if isinstance(blk.rect, (OrientedRegion, QuadRegion, CurvedRegion, VerticalRegion)):
+            raise ValueError
+        x0, y0, x1, y1 = (int(v) for v in blk.rect)
+        if (x0, y0, x1, y1) != tuple(blk.rect):
+            raise ValueError
+    except (TypeError, ValueError):
+        raise ValueError(f"{name}: a text block is an integer rectangle (x0, y0, x1, y1), got {blk.rect!r} (oriented, "
+                         f"perspective and curved blocks are not supported)") from None
+    if not (0 <= x0 < x1 <= W and 0 <= y0 < y1 <= H):
+        raise ValueError(f"{name}: rectangle {(x0, y0, x1, y1)} is empty or outside the {W}x{H} image")
+    if max(x1 - x0, y1 - y0) > 32767:
+        raise ValueError(f"{name}: a side of rectangle {(x0, y0, x1, y1)} exceeds 32767 pixels")
+    if blk.direction not in ("horizontal", "vertical"):
+        raise ValueError(f"{name}: direction must be 'horizontal' or 'vertical', got {blk.direction!r}")
+    if blk.polarity not in _INK:
+        raise ValueError(f"{name}: polarity must be 'auto', 'dark' or 'light', got {blk.polarity!r}")
+    for what in ("min_ink", "gap", "min_height"):
+        v = getattr(blk, what)
+        if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 1 <= v < 2 ** 31):
+            raise ValueError(f"{name}: {what} must be a positive integer, got {v!r}")
+    return x0, y0, x1, y1
+
+
+def _find_lines(dimg, items):
+    """ops.find_lines over items (image index, TextBlock, rect) of the uploaded images ``dimg``, its table back through one pinned
+    copy and one synchronisation.  Returns per item dict(lines, threshold, ink), or the error message of a block with too many
+    lines."""
+    from . import ops
+    recs = ops.find_lines([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap, blk.min_height)
+                           for i, blk, rect in items])
+    table = _to_host(recs).numpy().view(ops.block_lines_dtype())
+    out = []
+    for (i, blk, rect), t in zip(items, table):
+        n = int(t["n_lines"])
+        if n < 0:
+            out.append(f"{-n} lines exceed the {ops._lib.BLOCK_MAX_LINES} a text block may hold")
+            continue
+        lines = [tuple(int(v) for v in q) for q in t["rect"][:n]]
+        if blk.direction == "vertical":
+            lines = [VerticalRegion(q) for q in lines]
+        out.append(dict(lines=lines, threshold=int(t["threshold"]), ink="dark" if t["ink"] == ops._lib.INK_DARK else "light"))
+    return out
+
+
+@torch.no_grad()
+def find_lines(images, blocks):
+    """The lines of text blocks (DESIGN.md 7b, "Text blocks"): Otsu's threshold of each block's grey crop, the ink's row profile
+    (column profile for a vertical block) and its runs, merged across small gaps, short ones dropped, padded.
+
+    images: uint8 [H, W, 3] numpy arrays or CPU / CUDA tensors, in any channel order; blocks: per image, a list of TextBlocks.
+    Every block of the call goes through the same four launches (ops.find_lines), and its line table comes back in one pinned
+    copy and one synchronisation; host images go to the device in one pinned copy.
+    Returns per image a list with one dict per block: lines, integer rectangles (x0, y0, x1, y1) in image pixels top to bottom
+    (VerticalRegions of such rectangles, right to left, for a vertical block), each one a region restore_regions takes;
+    threshold, Otsu's t; ink, "dark" or "light".  Raises ValueError naming the image and the block, before any launch, for a
+    block restore_regions would reject, and after the segmentation for a block of more than 256 lines."""
+    imgs = [_as_image(im, i) for i, im in enumerate(images)]
+    blocks = _per_image(blocks, len(imgs), "blocks (one list per image)")
+    items, names = [], []
+    for i, im in enumerate(imgs):
+        for r, blk in enumerate(blocks[i] or []):
+            names.append(f"image {i}, block {r}")
+            if not isinstance(blk, TextBlock):
+                raise ValueError(f"{names[-1]}: expected a TextBlock, got {blk!r}")
+            items.append((i, blk, _check_block(blk, im.shape[0], im.shape[1], names[-1])))
+    out = [[] for _ in imgs]
+    if not items:
+        return out
+    dev = next((im.device for im in imgs if im.is_cuda), torch.device("cuda", torch.cuda.current_device()))
+    with torch.cuda.device(dev):
+        res = _find_lines(_device_images(sorted({i for i, _, _ in items}), imgs, dev), items)
+    for (i, _, _), name, r in zip(items, names, res):
+        if isinstance(r, str):
+            raise ValueError(f"{name}: {r}")
+        out[i].append(r)
+    return out
+
+
+def _plan_blocks(shapes, regions, labels, boxes):
+    """restore_regions' text blocks, validated before any launch: [(image, region index, TextBlock, rect)], and the region lists
+    with each block in place of its rectangle (plan_regions validates the other regions on them)."""
+    n = len(shapes)
+    regions, labels, boxes = (_per_image(v, n, f"{what} (one list per image)") for v, what in
+                              ((regions, "regions"), (labels, "labels"), (boxes, "boxes")))
+    blocks, stand_in = [], []
+    for i, (H, W) in enumerate(shapes):
+        rects = list(regions[i] or [])
+        labs = _per_image(labels[i], len(rects), f"image {i}: labels (one entry per region)")
+        bxs = _per_image(boxes[i], len(rects), f"image {i}: boxes (one entry per region)")
+        for r, reg in enumerate(rects):
+            if isinstance(reg, TextBlock):
+                name = f"image {i}, region {r} (a text block)"
+                if labs[r] is not None or bxs[r] is not None:
+                    raise ValueError(f"{name}: labels or boxes are given, but its lines are only found on the device (call "
+                                     f"find_lines and give the lines with their labels)")
+                rects[r] = _check_block(reg, H, W, name)
+                blocks.append((i, r, reg, rects[r]))
+        stand_in.append(rects)
+    return blocks, stand_in
+
+
+def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid):
+    """The region, label and box lists with each text block replaced in place by its lines, and per image the layout of its given
+    regions: None for a region, the block's find_lines result (or dict(error=...) under ``skip_invalid``) for a block.  A block
+    with too many lines, or a vertical line that vertical_plan rejects, raises ValueError without ``skip_invalid``."""
+    found = {(i, r): res for (i, r, _, _), res in zip(blocks, found)}
+    n = len(regions)
+    labels, boxes = _per_image(labels, n, "labels"), _per_image(boxes, n, "boxes")
+    out_r, out_l, out_b, layout = [], [], [], []
+    for i in range(n):
+        rects = list(regions[i] or [])
+        labs, bxs = _per_image(labels[i], len(rects), "labels"), _per_image(boxes[i], len(rects), "boxes")
+        rs, ls, bs, lay = [], [], [], []
+        for r, reg in enumerate(rects):
+            res = found.get((i, r))
+            if res is None:
+                rs.append(reg), ls.append(labs[r]), bs.append(bxs[r]), lay.append(None)
+                continue
+            name = f"image {i}, region {r} (a text block)"
+            err = f"{name}: {res}" if isinstance(res, str) else None
+            try:
+                for k, q in enumerate(res["lines"] if err is None else []):
+                    if isinstance(q, VerticalRegion):
+                        vertical_plan(q.shape[2] - q.shape[0], q.shape[3] - q.shape[1], name=f"{name}, line {k}")
+            except ValueError as e:
+                err = str(e)
+            if err is not None:
+                if not skip_invalid:
+                    raise ValueError(err)
+                lay.append(dict(error=err))
+                continue
+            rs += res["lines"]
+            ls += [None] * len(res["lines"])
+            bs += [None] * len(res["lines"])
+            lay.append(res)
+        out_r.append(rs)
+        out_l.append(None if labels[i] is None else ls)
+        out_b.append(None if boxes[i] is None else bs)
+        layout.append(lay)
+    return out_r, out_l, out_b, layout
+
+
+def _regroup_blocks(out, layout):
+    """restore_regions' result with each block's line entries gathered into the block's own entry, in place."""
+    for img, lay in zip(out, layout):
+        flat, o, img["regions"] = img["regions"], 0, []
+        for res in lay:
+            if res is None:
+                img["regions"].append(flat[o])
+                o += 1
+            elif "error" in res:
+                img["regions"].append(res)
+            else:
+                img["regions"].append(dict(res, regions=flat[o:o + len(res["lines"])]))
+                o += len(res["lines"])
+
+
 def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None):
     """restore_regions' host plan, validated before any launch.  shapes: (H, W) per image; regions: per image, a list of integer
     half-open rectangles (x0, y0, x1, y1) and OrientedRegions; labels / boxes: None, or per image None or a list with one entry
@@ -1706,16 +1883,27 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     fl32(mapy), INTER_CUBIC, BORDER_REPLICATE) with curved_maps' crop map (every curved crop of the call in one
     mn_remap_curved_u8_batched launch), its labels and boxes given and returned in C's frame, and its entry gains ``size``
     ((w_r, h_r)).  Each page pixel of its footprint is inverted onto T by bisection along the curves, feathered on all four
-    sides, and a call that holds one composes every region with mn_composite_regions_curved_u8."""
+    sides, and a call that holds one composes every region with mn_composite_regions_curved_u8.
+    A TextBlock (DESIGN.md 7b, "Text blocks") is split into lines on the uploaded images first (find_lines: every block of the
+    call in the same four launches, one pinned copy of the line table and one synchronisation), and its lines, rectangles or
+    VerticalRegions, take its place in the region list; the call then goes on as if they had been given.  No labels or boxes
+    may be given for a block.  Its entry is dict(lines, threshold, ink, regions), regions one entry per line as above; a block
+    of more than 256 lines, or with a vertical line vertical_plan rejects, raises, or is dict(error=...) with ``skip_invalid``."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
-    plan = plan_regions([im.shape[:2] for im in imgs], regions, labels, boxes, scale, feather)
+    shapes = [im.shape[:2] for im in imgs]
+    blocks, stand_in = _plan_blocks(shapes, regions, labels, boxes)
+    plan = plan_regions(shapes, stand_in if blocks else regions, labels, boxes, scale, feather)
     feather = 2 * scale if feather is None else feather
     if not imgs:
         return []
     dev = next(encoder.parameters()).device
     with torch.cuda.device(dev):
         dimg = _device_images(range(len(imgs)), imgs, dev)
+        if blocks:                                       # every block's lines take its place in the region list
+            found = _find_lines(dimg, [(i, blk, rect) for i, _, blk, rect in blocks])
+            regions, labels, boxes, layout = _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid)
+            plan = plan_regions(shapes, regions, labels, boxes, scale, feather)
         crops = [dimg[p.image][p.rect[1]:p.rect[3], p.rect[0]:p.rect[2]] for p in plan]
         oriented = [k for k, p in enumerate(plan) if p.oriented is not None]
         quads = [k for k, p in enumerate(plan) if p.quad is not None]
@@ -1801,6 +1989,8 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         if p.curved and "error" not in r:
             entry.update(size=p.size)
         out[p.image]["regions"].append(entry)
+    if blocks:
+        _regroup_blocks(out, layout)
     return out
 
 
