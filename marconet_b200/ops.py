@@ -6,6 +6,7 @@ computation below is a kernel from libmarconet_b200.so.  Activations are NHWC fp
 slices of a concatenation buffer).
 """
 import ctypes
+import functools
 from typing import NamedTuple
 
 import torch
@@ -145,6 +146,7 @@ class ConvWeight:
     __slots__ = ("w", "taps", "cin", "cout", "_tc", "name", "precision", "x_scale", "tag", "__weakref__")
     _next_tag = 1
     _by_tag = {}
+    _slots = {}        # tag -> range-flag slot of the live layers that have launched on the tensor cores
 
     def __init__(self, w, taps, name=None):
         import weakref
@@ -157,7 +159,22 @@ class ConvWeight:
         ConvWeight._next_tag += 1
         self.name = name or f"conv#{self.tag}[{taps}x{self.cin}->{self.cout}]"
         self.precision, self.x_scale = PLAN.get(self.name, (None, 1.0))      # plans survive re-packing (keyed by layer name)
-        ConvWeight._by_tag[self.tag] = weakref.ref(self)
+        ConvWeight._by_tag[self.tag] = weakref.ref(self, functools.partial(ConvWeight._release, self.tag))
+
+    @classmethod
+    def _release(cls, tag, _ref=None):
+        """The layer with this tag died: forget it and give its range-flag slot back."""
+        cls._by_tag.pop(tag, None)
+        slot = cls._slots.pop(tag, None)
+        if slot is not None:
+            _RANGE_POOL.give(slot)
+
+    def range_slot(self):
+        """This layer's own element of the range-flag arrays: taken at its first tensor-core launch, released when it dies."""
+        slot = ConvWeight._slots.get(self.tag)
+        if slot is None:
+            slot = ConvWeight._slots[self.tag] = _RANGE_POOL.take()
+        return slot
 
     def set_plan(self, precision=None, x_scale=None):
         """Set this layer's precision / input scale and remember it under the layer's name (ops.PLAN)."""
@@ -199,19 +216,45 @@ class ConvWeight:
 
 # ---- fp16-range guard (ADVICE r1 / VERDICT r1 2.iii) ------------------------------------------------------------------
 # The default tensor-core precision splits fp32 operands into fp16 hi/lo pairs: an activation with |x * x_scale| >= 65504 would
-# become Inf.  Every tensor-core conv is launched with a pointer to a per-device flag in PINNED HOST memory; the operand-split
-# stage stores the layer's tag into it when an element leaves the range (or is Inf/NaN).  The host reads the flag without any
-# CUDA call: at the start of every module forward (``poll_range``: the offending layer is re-routed to the bf16 split, which has
-# fp32's exponent range, and a warning names it -- the overflowed call's own output contains Inf/NaN, never a silently wrong
-# number) and in ``check_range`` (raises FloatingPointError; GraphedLines.check and pipeline.restore_lines call it after their
-# synchronisation, the latter re-runs the step once with the new plan).
+# become Inf.  Every tensor-core conv is launched with a pointer to its layer's own element of a per-device flag array in PINNED
+# HOST memory; the operand-split stage stores the layer's tag into it when |x * x_scale| reaches 65504 (or Inf; NaN is not seen).
+# The host reads the flags without any CUDA call: at the start of every module forward (``poll_range``: the offending layer is
+# re-routed to the bf16 split, which has fp32's exponent range, and a warning names it) and in ``check_range`` (raises
+# FloatingPointError; GraphedLines.check and pipeline.restore_lines call it after their synchronisation, the latter re-runs the
+# step with the new plan).  The flag is the guarantee, not the overflowed call's own output: its dot products hold Inf/NaN, but a
+# ReLU epilogue (fmaxf) turns NaN and -Inf into 0, so that output may be finite and plausible.
 _RANGE_FLAGS = {}
 _RANGE_SLOTS = 2048
 RANGE_EVENTS = []        # (layer name, action) log of re-routes, newest last
 
 
+class _SlotPool:
+    """Indices [0, size) handed out one per live layer; released ones are reused first."""
+
+    def __init__(self, size):
+        self.size, self.next, self.free = size, 0, []
+
+    def take(self):
+        if not self.free and self.next == self.size:
+            import gc
+            gc.collect()                # dead layers still held by reference cycles give their slots back
+        if self.free:
+            return self.free.pop()
+        if self.next == self.size:
+            raise RuntimeError(f"marconet_b200: more than {self.size} live tensor-core conv layers; the fp16-range guard has one "
+                               f"flag slot per layer (ops._RANGE_SLOTS)")
+        self.next += 1
+        return self.next - 1
+
+    def give(self, slot):
+        self.free.append(slot)
+
+
+_RANGE_POOL = _SlotPool(_RANGE_SLOTS)
+
+
 def range_flags(device):
-    """Per-device int32[_RANGE_SLOTS] in pinned host memory; slot tag % _RANGE_SLOTS belongs to the layer with that tag."""
+    """Per-device int32[_RANGE_SLOTS] in pinned host memory; element ``cw.range_slot()`` belongs to layer ``cw`` while it lives."""
     key = device.index if device.index is not None else torch.cuda.current_device()
     f = _RANGE_FLAGS.get(key)
     if f is None:
@@ -247,7 +290,7 @@ def poll_range(device, reroute=True):
             cw.set_plan(precision=PREC_BF16X3_TC)
             RANGE_EVENTS.append((cw.name, "rerouted to bf16x3"))
             warnings.warn(f"marconet_b200: |activation * {cw.x_scale:g}| >= 65504 at conv layer {cw.name}: the fp16 hi/lo split "
-                          f"overflowed (that call's output holds Inf/NaN); the layer now uses the bf16 split (MN_PREC_BF16X3_TC). "
+                          f"overflowed (that call's output is wrong: Inf/NaN, or 0 after a ReLU); the layer now uses the bf16 split (MN_PREC_BF16X3_TC). "
                           f"Run pipeline.tune_precision() for a calibrated per-layer plan.")
     return hits
 
@@ -418,7 +461,7 @@ def conv2d(x, w, kh, kw, stride=(1, 1), pad=(0, 0), bias=None, out_scale=None, r
         hi, lo, sc = cw.tc(prec)
         p.w_tc_hi = hi.data_ptr(); p.w_tc_lo = lo.data_ptr(); p.w_tc_scale = sc.data_ptr()
         p.x_scale = cw.x_scale
-        p.range_flag = range_flags(x.device).data_ptr() + 4 * (cw.tag % _RANGE_SLOTS); p.range_tag = cw.tag
+        p.range_flag = range_flags(x.device).data_ptr() + 4 * cw.range_slot(); p.range_tag = cw.tag
         calib = getattr(_TLS, "calib", None)
         if calib is not None:
             p.x_absmax = calib.slot(cw).data_ptr()

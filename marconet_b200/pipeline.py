@@ -55,8 +55,8 @@ def restore_lines(encoder, tspgan, sr, lq, labels=None, locs=None, max_chars=16,
     labels: optional list (per line) of int64 [n_b, 1] tensors; default = the encoder's decoded labels (at most ``max_chars``).
     locs:   optional [B, 2*n] (centre, half-width) in units of the line width; default = converted encoder boxes.
     check_range: synchronise at the end and look at the fp16-range flags (ops.poll_range); when a tensor-core conv overflowed the
-    fp16 hi/lo split its layer is re-routed to the bf16 split and the step is re-run (at most 3 times) -- the caller never sees
-    the Inf/NaN result."""
+    fp16 hi/lo split its layer is re-routed to the bf16 split and the step is re-run until no run re-routes a layer (``_rerun``)
+    -- the caller never sees the overflowed result."""
     def step():
         return _step(encoder, tspgan, sr, lq, labels, locs, max_chars=max_chars)
     return _rerun(step, lq.device) if check_range else step()
@@ -92,12 +92,19 @@ def _step(encoder, tspgan, sr, lq, labels, locs, max_chars=16, owner=None, lq_sr
 
 def _rerun(step, device):
     """``step()``, then a synchronisation and a look at the fp16-range flags (ops.poll_range): a tensor-core conv that overflowed
-    the fp16 hi/lo split has been re-routed to the bf16 split, and the step runs again (at most 3 times)."""
+    the fp16 hi/lo split has been re-routed to the bf16 split, and the step runs again.  One overflow can hide the next: its NaN
+    becomes 0 after a ReLU, so a layer further on overflows only once the earlier one is re-routed (the encoder on a line
+    x1000 takes five runs).  So the step re-runs for as long as a run re-routes a layer -- each layer at most once, hence a bounded loop -- and
+    stops when a run raises no flag or flags only layers already on the bf16 split (their input itself held Inf / NaN).
+    A re-route made inside the step counts too: every module forward polls the flags at its start without synchronising, so a
+    later module of the same step (or a later chunk of a sweep) can already re-route a layer that overflowed earlier in it."""
     from . import ops
-    for attempt in range(4):
+    while True:
+        before = len(ops.RANGE_EVENTS)
         out = step()
         torch.cuda.synchronize(device)
-        if not ops.poll_range(device) or attempt == 3:
+        ops.poll_range(device)
+        if not any(what == "rerouted to bf16x3" for _, what in ops.RANGE_EVENTS[before:]):
             return out
 
 
@@ -587,8 +594,8 @@ def restore_images(encoder, tspgan, sr, images, labels=None, boxes=None, max_lin
     module would); with ``skip_invalid`` a bad image's entry becomes dict(error=...) and the others still run.  Per batch: one
     host->device copy of the batch's host images through pinned memory, one crop kernel (mn_preprocess_lq_u8_batched), the
     encoder, one TSPGAN call for all characters (each crop's characters take that crop's style w, as on a hand-made crop),
-    TSPSRNet, a synchronisation and ops.poll_range (the batch re-runs, at most 3 times, when a layer was re-routed for fp16
-    range), then one stitch kernel (mn_postprocess_sr_u8_pieces) into the images' outputs.
+    TSPSRNet, a synchronisation and ops.poll_range (the batch re-runs while a run re-routes a layer for fp16 range, see
+    ``_rerun``), then one stitch kernel (mn_postprocess_sr_u8_pieces) into the images' outputs.
     Returns one dict per image: sr_u8 (uint8 [128, W_i, 3], W_i = round_half_even(w_i*128/h_i), on the device, or numpy through
     one pinned device->host copy with ``to_host``) and segments (the plan).  A single-segment image gives restore_image's bytes.
 

@@ -224,3 +224,40 @@ def test_precision_plan_survives_repack_by_name():
         ops.PLAN.clear()
         ops.PLAN.update(saved)
 
+
+def test_range_slots_belong_to_live_layers_and_are_reused():
+    """Each live tensor-core layer has its own range-flag slot, whatever its tag: two layers whose tags are congruent modulo the
+    slot count (tags only grow, every re-pack makes new layers) must not share one.  A dead layer's slot goes back to the pool."""
+    import gc
+    import torch
+    from marconet_b200 import ops
+    gc.collect()                                     # dead layers of earlier tests give their slots back now, not below
+    a = ops.ConvWeight(torch.zeros(64, 64), 1, name="test.slot_a")
+    ops.ConvWeight._next_tag = a.tag + ops._RANGE_SLOTS
+    b = ops.ConvWeight(torch.zeros(64, 64), 1, name="test.slot_b")
+    assert b.tag % ops._RANGE_SLOTS == a.tag % ops._RANGE_SLOTS
+    sa, sb = a.range_slot(), b.range_slot()
+    assert sa != sb and a.range_slot() == sa and 0 <= min(sa, sb) and max(sa, sb) < ops._RANGE_SLOTS
+    tag_b = b.tag
+    del b
+    gc.collect()
+    assert ops.ConvWeight.from_tag(tag_b) is None and tag_b not in ops.ConvWeight._by_tag
+    free = list(ops._RANGE_POOL.free)
+    assert sb in free                                # b's slot went back to the pool
+    c = ops.ConvWeight(torch.zeros(64, 64), 1, name="test.slot_c")
+    assert c.range_slot() == free[-1] and c.range_slot() != sa     # a released slot is reused before a new one is taken
+    assert ops.ConvWeight.from_tag(a.tag) is a and a.range_slot() == sa
+
+
+def test_range_slot_pool_raises_beyond_its_size():
+    """More live layers than slots is an error naming the limit, not a silently shared flag; a released slot makes room again."""
+    import pytest
+    from marconet_b200 import ops
+    pool = ops._SlotPool(3)
+    got = [pool.take() for _ in range(3)]
+    assert sorted(got) == [0, 1, 2]
+    with pytest.raises(RuntimeError, match="more than 3 live tensor-core conv layers"):
+        pool.take()
+    pool.give(got[1])
+    assert pool.take() == got[1]
+
