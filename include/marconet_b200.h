@@ -708,6 +708,35 @@ typedef struct {
 } mn_text_block;
 int mn_find_lines_u8(const mn_text_block* blocks, int n, long long max_tiles, void* work, long long work_bytes, void* stream);
 
+/* Skewed text blocks (DESIGN.md section 7b, "Skewed blocks").  Block i is searched over the angle table table[0 .. n_ang) of
+ * fp64 (c, s) pairs uploaded by the host (a given angle is a one-entry table; no device trigonometry).  The frame is the
+ * crop's, transposed for a vertical block (wt x ht): X = x + 0.5 - wt / 2, Y = y + 0.5 - ht / 2, u = fl(fl(X c) - fl(Y s)),
+ * v = fl(fl(X s) + fl(Y c)), v_min / v_max and u_min / u_max over the four corner pixel centres, L = floor(v_max - v_min) + 1,
+ * M = floor(u_max - u_min) + 1, bin k = clamp(floor(v - v_min), 0, L - 1), index j = clamp(floor(u - u_min), 0, M - 1).
+ * mn_find_lines_skewed_u8 issues six launches for every block of a call, whatever their number:
+ *   1, 2. mn_find_lines_u8's histogram and threshold over blocks[];
+ *   3. angle profiles over 32 x 32 tiles (n_ang > 1 only): profiles[a stride + k] = #{ink pixels in bin k at angle a};
+ *   4. scores, one CTA per block: scores[a] = sum_k (r_a[k + 1] - r_a[k])^2 (int64), the chosen index the largest score,
+ *      ties to the least |a - (n_ang - 1) / 2|, then the least a; the chosen frame goes into chosen, L, M, u_min, v_min, c, s.
+ *      When s != 0 it also rewrites blocks[i] as the frame's record (x0 = y0 = 0, w = M, h = L, vertical = 0);
+ *   5. the chosen frame's profile into b.prof (3 L values laid out as mn_find_lines_u8's);
+ *   6. mn_find_lines_u8's segmentation over blocks[].
+ * out->rect[k] is therefore (c0, l0, c1, l1) in frame indices top to bottom when s != 0, and mn_find_lines_u8's rectangle
+ * otherwise.  blocks[i] and skew[i].b are the same crop record on entry.  work (work_bytes) covers every hist, prof, profiles
+ * and scores of the call and is zeroed by the call; prof and profiles hold 3 stride and n_ang stride int32, stride >= every
+ * L of the table; b.scratch 2 stride + 4 int32.  skew, blocks: DEVICE arrays (validated by the caller, |angle| < 45 degrees). */
+typedef struct {
+    mn_text_block b;            /* the crop record; b.prof receives the chosen frame's profile */
+    const double* table;        /* n_ang (c, s) pairs */
+    int64_t* scores;            /* n_ang values (written when n_ang > 1) */
+    int32_t* profiles;          /* n_ang x stride values (n_ang > 1) */
+    int32_t n_ang, stride;
+    int32_t chosen, L, M, pad;  /* written by the call */
+    double u_min, v_min, c, s;  /* written by the call: the chosen frame */
+} mn_skew_block;
+int mn_find_lines_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, int n, long long max_tiles, void* work, long long work_bytes,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -167,6 +167,12 @@ class TextBlock(Structure):
                 ("pad", c_int32), ("hist", c_void_p), ("prof", c_void_p), ("scratch", c_void_p), ("out", c_void_p)]
 
 
+class SkewBlock(Structure):
+    _fields_ = [("b", TextBlock), ("table", c_void_p), ("scores", c_void_p), ("profiles", c_void_p), ("n_ang", c_int32),
+                ("stride", c_int32), ("chosen", c_int32), ("L", c_int32), ("M", c_int32), ("pad", c_int32), ("u_min", c_double),
+                ("v_min", c_double), ("c", c_double), ("s", c_double)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -227,6 +233,7 @@ SYMBOLS = {
     "mn_remap_curved_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
     "mn_composite_regions_curved_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_find_lines_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
+    "mn_find_lines_skewed_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

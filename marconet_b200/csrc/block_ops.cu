@@ -1,7 +1,8 @@
 // Text blocks split into lines (DESIGN.md 7b, "Text blocks"): Otsu binarisation, a projection profile and line runs for every
 // block of a call in four launches (histogram, threshold, profile, segmentation).  The threshold is OpenCV's fp64 loop with
 // explicit-rounding intrinsics, so that nvcc cannot contract it into an FMA the host twin (oracle/blocks.py) does not have; the
-// rest is integer arithmetic.
+// rest is integer arithmetic.  Skewed blocks (DESIGN.md 7b, "Skewed blocks") add an angle search and a rotated profile around
+// the same kernels, in six launches.
 #include "mn_common.cuh"
 
 namespace {
@@ -272,6 +273,266 @@ __global__ void __launch_bounds__(kSegThreads) block_lines_kernel(const mn_text_
     if (threadIdx.x == 0) b.out->n_lines = nk;
 }
 
+// ---- Skewed blocks (DESIGN.md 7b, "Skewed blocks") ----
+// Every frame quantity is fp64 with each operation rounded on its own, as in the twin (oracle/skewed_blocks.py).  A tile of
+// 32 x 32 pixels spans at most floor(31 (|c| + |s|)) + 2 <= 45 bins at |angle| < 45 degrees; kBins leaves room, and a bin outside
+// it (which the bound rules out) would go straight to the global profile.
+constexpr int kBins = 64;
+constexpr int kScoreThreads = 1024;
+
+struct frame_t {
+    double u_min, v_min;
+    int L, M;
+};
+
+// Pixel centre x + 0.5 - n / 2 of index x on an axis of n pixels: exact in fp64.
+__device__ __forceinline__ double centre(int x, int n) { return (double)(2 * x + 1 - n) * 0.5; }
+__device__ __forceinline__ double frame_u(double X, double Y, double c, double s) {
+    return __dsub_rn(__dmul_rn(X, c), __dmul_rn(Y, s));
+}
+__device__ __forceinline__ double frame_v(double X, double Y, double c, double s) {
+    return __dadd_rn(__dmul_rn(X, s), __dmul_rn(Y, c));
+}
+__device__ __forceinline__ int frame_bin(double v, double v_min, int L) {
+    return min(max((int)floor(__dsub_rn(v, v_min)), 0), L - 1);
+}
+
+// The crop's frame dimensions: wt x ht, transposed for a vertical block.
+__device__ __forceinline__ void frame_dims(const mn_text_block& b, int& wt, int& ht) {
+    wt = b.vertical ? b.h : b.w;
+    ht = b.vertical ? b.w : b.h;
+}
+
+__device__ frame_t frame_of(int wt, int ht, double c, double s) {
+    const double xs[2] = {centre(0, wt), centre(wt - 1, wt)}, ys[2] = {centre(0, ht), centre(ht - 1, ht)};
+    double u_lo = 0, u_hi = 0, v_lo = 0, v_hi = 0;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const double u = frame_u(xs[q & 1], ys[q >> 1], c, s), v = frame_v(xs[q & 1], ys[q >> 1], c, s);
+        u_lo = q ? fmin(u_lo, u) : u;
+        u_hi = q ? fmax(u_hi, u) : u;
+        v_lo = q ? fmin(v_lo, v) : v;
+        v_hi = q ? fmax(v_hi, v) : v;
+    }
+    frame_t f;
+    f.u_min = u_lo;
+    f.v_min = v_lo;
+    f.L = (int)floor(__dsub_rn(v_hi, v_lo)) + 1;
+    f.M = (int)floor(__dsub_rn(u_hi, u_lo)) + 1;
+    return f;
+}
+
+// The tile's ink as 32 frame rows of bits: s_row[r] bit j = ink at frame pixel (fx0 + j, fy0 + r), where (fx0, fy0) is the
+// tile's origin in the frame ((tx, ty), or (ty, tx) for a vertical block).  s_m: 32 words of scratch.  Ends with a barrier.
+__device__ void tile_ink_rows(const mn_text_block& b, int tx, int ty, unsigned* s_m, unsigned* s_row) {
+    const int t = b.out->threshold;
+    const bool dark = b.out->ink == MN_INK_DARK;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, x = tx + lane;
+    for (int j = 0; j < kTile / 8; ++j) {
+        const int y = ty + warp + 8 * j;
+        bool ink = false;
+        if (x < b.w && y < b.h) {
+            const int g = block_grey(b, x, y);
+            ink = dark ? g <= t : g > t;
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, ink);
+        if (lane == 0) (b.vertical ? s_m : s_row)[warp + 8 * j] = m;
+    }
+    if (b.vertical) {
+        __syncthreads();
+        if (warp == 0) {                                // transpose: frame row r is the tile's column r
+            unsigned r = 0;
+            for (int y = 0; y < kTile; ++y) r |= ((s_m[y] >> lane) & 1u) << y;
+            s_row[lane] = r;
+        }
+    }
+    __syncthreads();
+}
+
+// The least bin of a tile of frame pixels [fx0, fx0 + nx) x [fy0, fy0 + ny): v is monotone in X and in Y (each rounded operation
+// is), so it is the least of the four corners' bins.
+__device__ __forceinline__ int tile_bin0(int fx0, int fy0, int nx, int ny, int wt, int ht, double c, double s, double v_min, int L) {
+    int k = L;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const double X = centre(fx0 + (q & 1) * (nx - 1), wt), Y = centre(fy0 + (q >> 1) * (ny - 1), ht);
+        k = min(k, frame_bin(frame_v(X, Y, c, s), v_min, L));
+    }
+    return k;
+}
+
+// 3. Angle profiles: each warp takes angles warp, warp + 8, ...; lane r walks frame row r of the tile, counting runs of equal
+// bins before adding them into the warp's shared bins, which then go to the angle's profile with one atomic per non-zero bin.
+__global__ void __launch_bounds__(kTileThreads) skew_angle_profile_kernel(const mn_skew_block* __restrict__ blocks) {
+    mn_pdl_prologue();
+    __shared__ unsigned s_m[kTile], s_row[kTile];
+    __shared__ int s_bins[kTileThreads / 32][kBins];
+    const mn_skew_block& sb = blocks[blockIdx.y];
+    const mn_text_block b = sb.b;
+    const int n_ang = sb.n_ang, stride = sb.stride;
+    if (n_ang < 2) return;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    tile_ink_rows(b, tx, ty, s_m, s_row);
+    int wt, ht;
+    frame_dims(b, wt, ht);
+    const int fx0 = b.vertical ? ty : tx, fy0 = b.vertical ? tx : ty;
+    const int nx = min(kTile, wt - fx0), ny = min(kTile, ht - fy0);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned row = lane < ny ? s_row[lane] : 0u;
+    const double Y = centre(fy0 + lane, ht);
+    int* bins = s_bins[warp];
+    for (int a = warp; a < n_ang; a += kTileThreads / 32) {
+        const double c = sb.table[2 * a], s = sb.table[2 * a + 1];
+        const frame_t f = frame_of(wt, ht, c, s);
+        const int k0 = tile_bin0(fx0, fy0, nx, ny, wt, ht, c, s, f.v_min, f.L);
+        int* prof = sb.profiles + (long long)a * stride;
+        bins[lane] = bins[lane + 32] = 0;
+        __syncwarp();
+        const double yc = __dmul_rn(Y, c);
+        int cur = -1, cnt = 0;
+        for (unsigned m = row; m; m &= m - 1) {
+            const int j = __ffs(m) - 1;
+            const int k = frame_bin(__dadd_rn(__dmul_rn(centre(fx0 + j, wt), s), yc), f.v_min, f.L);
+            if (k != cur) {
+                if (cnt) {
+                    if (cur - k0 >= 0 && cur - k0 < kBins) atomicAdd(&bins[cur - k0], cnt); else atomicAdd(&prof[cur], cnt);
+                }
+                cur = k;
+                cnt = 0;
+            }
+            ++cnt;
+        }
+        if (cnt) {
+            if (cur - k0 >= 0 && cur - k0 < kBins) atomicAdd(&bins[cur - k0], cnt); else atomicAdd(&prof[cur], cnt);
+        }
+        __syncwarp();
+        for (int d = lane; d < kBins; d += 32) {
+            if (bins[d]) atomicAdd(&prof[k0 + d], bins[d]);
+        }
+        __syncwarp();
+    }
+}
+
+// Is (score sa, index a) ahead of (sb, b)?  The larger score; ties to the least |index - mid|, then the least index.
+__device__ __forceinline__ bool ahead(long long sa, int a, long long sb, int b, int mid) {
+    if (sa != sb) return sa > sb;
+    const int da = abs(a - mid), db = abs(b - mid);
+    return da != db ? da < db : a < b;
+}
+
+// 4. Scores and the chosen angle, one CTA per block: one warp per angle, then a CTA-wide argmax.  Writes the chosen frame into
+// the skew record, and, for a frame that is not the crop's own (s != 0), the frame's record into blocks[] for the segmentation.
+__global__ void __launch_bounds__(kScoreThreads) skew_score_kernel(mn_text_block* blocks, mn_skew_block* skew) {
+    mn_pdl_prologue();
+    __shared__ long long s_best[kScoreThreads / 32];
+    __shared__ int s_arg[kScoreThreads / 32];
+    mn_skew_block& sb = skew[blockIdx.x];
+    const mn_text_block b = sb.b;
+    const int n_ang = sb.n_ang, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, mid = (n_ang - 1) / 2;
+    int wt, ht;
+    frame_dims(b, wt, ht);
+    int best = 0;
+    if (n_ang > 1) {
+        for (int a = warp; a < n_ang; a += kScoreThreads / 32) {
+            const int L = frame_of(wt, ht, sb.table[2 * a], sb.table[2 * a + 1]).L;
+            const int* r = sb.profiles + (long long)a * sb.stride;
+            long long acc = 0;
+            for (int k = lane; k + 1 < L; k += 32) {
+                const long long d = (long long)r[k + 1] - r[k];
+                acc += d * d;
+            }
+#pragma unroll
+            for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+            if (lane == 0) sb.scores[a] = acc;
+        }
+        __syncthreads();
+        long long bs = -1;
+        int ba = 0;
+        for (int a = threadIdx.x; a < n_ang; a += kScoreThreads) {
+            const long long v = sb.scores[a];
+            if (bs < 0 || ahead(v, a, bs, ba, mid)) bs = v, ba = a;
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            const long long os = __shfl_xor_sync(0xffffffffu, bs, o);
+            const int oa = __shfl_xor_sync(0xffffffffu, ba, o);
+            if (os >= 0 && (bs < 0 || ahead(os, oa, bs, ba, mid))) bs = os, ba = oa;
+        }
+        if (lane == 0) s_best[warp] = bs, s_arg[warp] = ba;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            for (int w = 1; w < kScoreThreads / 32; ++w) {
+                if (s_best[w] >= 0 && (bs < 0 || ahead(s_best[w], s_arg[w], bs, ba, mid))) bs = s_best[w], ba = s_arg[w];
+            }
+        }
+        best = ba;
+    }
+    if (threadIdx.x != 0) return;
+    const double c = sb.table[2 * best], s = sb.table[2 * best + 1];
+    const frame_t f = frame_of(wt, ht, c, s);
+    sb.chosen = best;
+    sb.L = f.L;
+    sb.M = f.M;
+    sb.u_min = f.u_min;
+    sb.v_min = f.v_min;
+    sb.c = c;
+    sb.s = s;
+    if (s != 0.0) {                                     // the segmentation runs in the frame: its table holds frame indices
+        mn_text_block g = b;
+        g.x0 = g.y0 = 0;
+        g.w = f.M;
+        g.h = f.L;
+        g.vertical = 0;
+        blocks[blockIdx.x] = g;
+    }
+}
+
+// 5. The chosen frame's profile over the tiles: per bin the ink count, M - the least j and the largest j + 1, gathered in
+// shared memory and added into b.prof with one atomic per bin and quantity (mn_find_lines_u8's layout, L = the frame's).
+__global__ void __launch_bounds__(kTileThreads) skew_profile_kernel(const mn_skew_block* __restrict__ blocks) {
+    mn_pdl_prologue();
+    __shared__ unsigned s_m[kTile], s_row[kTile];
+    __shared__ int s_cnt[kBins], s_lo[kBins], s_hi[kBins];
+    const mn_skew_block& sb = blocks[blockIdx.y];
+    const mn_text_block b = sb.b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    if (threadIdx.x < kBins) s_cnt[threadIdx.x] = s_lo[threadIdx.x] = s_hi[threadIdx.x] = 0;
+    tile_ink_rows(b, tx, ty, s_m, s_row);
+    int wt, ht;
+    frame_dims(b, wt, ht);
+    const int fx0 = b.vertical ? ty : tx, fy0 = b.vertical ? tx : ty;
+    const int nx = min(kTile, wt - fx0), ny = min(kTile, ht - fy0);
+    const double c = sb.c, s = sb.s, u_min = sb.u_min, v_min = sb.v_min;
+    const int L = sb.L, M = sb.M;
+    const int k0 = tile_bin0(fx0, fy0, nx, ny, wt, ht, c, s, v_min, L);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const double X = centre(fx0 + lane, wt);
+    for (int r = warp; r < ny; r += kTileThreads / 32) {
+        if (!((s_row[r] >> lane) & 1u)) continue;
+        const double Y = centre(fy0 + r, ht);
+        const int k = frame_bin(frame_v(X, Y, c, s), v_min, L);
+        const int j = min(max((int)floor(__dsub_rn(frame_u(X, Y, c, s), u_min)), 0), M - 1);
+        if (k - k0 >= 0 && k - k0 < kBins) {
+            atomicAdd(&s_cnt[k - k0], 1);
+            atomicMax(&s_lo[k - k0], M - j);
+            atomicMax(&s_hi[k - k0], j + 1);
+        } else {
+            atomicAdd(&b.prof[k], 1);
+            atomicMax(&b.prof[L + k], M - j);
+            atomicMax(&b.prof[2 * L + k], j + 1);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < kBins && s_cnt[threadIdx.x]) {
+        const int k = k0 + threadIdx.x;
+        atomicAdd(&b.prof[k], s_cnt[threadIdx.x]);
+        atomicMax(&b.prof[L + k], s_lo[threadIdx.x]);
+        atomicMax(&b.prof[2 * L + k], s_hi[threadIdx.x]);
+    }
+}
+
 }  // namespace
 
 extern "C" int mn_find_lines_u8(const mn_text_block* blocks, int n, long long max_tiles, void* work, long long work_bytes,
@@ -287,6 +548,29 @@ extern "C" int mn_find_lines_u8(const mn_text_block* blocks, int n, long long ma
     MN_CUDA_CHECK((mn_launch(block_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, blocks)));
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(block_lines_kernel, dim3(n), dim3(kSegThreads), 0, st, blocks)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_find_lines_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, int n, long long max_tiles, void* work,
+                                       long long work_bytes, void* stream) {
+    MN_REQUIRE(blocks && skew && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
+               "mn_find_lines_skewed_u8: bad args");
+    cudaStream_t st = (cudaStream_t)stream;
+    const mn_text_block* cblocks = blocks;
+    const mn_skew_block* cskew = skew;
+    MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
+    MN_CUDA_CHECK((mn_launch(block_hist_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cblocks)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(block_threshold_kernel, dim3(mn_cdiv(n, 128)), dim3(128), 0, st, cblocks, n)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(skew_angle_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cskew)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(skew_score_kernel, dim3(n), dim3(kScoreThreads), 0, st, blocks, skew)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(skew_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cskew)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(block_lines_kernel, dim3(n), dim3(kSegThreads), 0, st, cblocks)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -7,6 +7,7 @@ slices of a concatenation buffer).
 """
 import ctypes
 import functools
+import math
 from typing import NamedTuple
 
 import torch
@@ -1572,19 +1573,62 @@ def block_lines_dtype():
                      ("rect", "<i4", (_lib.BLOCK_MAX_LINES, 4))])
 
 
-def find_lines(blocks):
+SKEW_MAX_PROFILE = 1 << 24     # int32 values of one skewed block's angle profiles (64 MB)
+
+
+def skew_table(skew, max_skew, vertical):
+    """The frame angles of a skewed block's search (DESIGN.md 7b, "Skewed blocks"), in degrees: i / 20 for |i| <= round(20
+    max_skew) with skew "auto", else the given angle, negated for a vertical block (whose frame is the transposed crop)."""
+    if isinstance(skew, str):
+        n = round(20 * max_skew)
+        return [i / 20 for i in range(-n, n + 1)]
+    return [-float(skew) if vertical else float(skew)]
+
+
+def skew_cos_sin(angles):
+    """fp64 (c, s) of frame angles in degrees, computed on the host: the device has no trigonometry."""
+    return [(math.cos(math.radians(t)), math.sin(math.radians(t))) for t in angles]
+
+
+def skew_stride(w, h, vertical, cs):
+    """The largest number of bins L of a w x h crop's frames over the (c, s) of ``cs``, as the device computes it."""
+    import numpy as np
+    wt, ht = (h, w) if vertical else (w, h)
+    c, s = (np.array([p[k] for p in cs], np.float64) for k in (0, 1))
+    xs, ys = (0.5 - wt / 2, wt - 0.5 - wt / 2), (0.5 - ht / 2, ht - 0.5 - ht / 2)
+    v = np.stack([x * s + y * c for x in xs for y in ys])
+    return int((np.floor(v.max(axis=0) - v.min(axis=0)) + 1).max())
+
+
+def skew_block_dtype():
+    """numpy view of an mn_skew_block record after mn_find_lines_skewed_u8: the chosen index and frame."""
+    import numpy as np
+    return np.dtype([("b", np.uint8, ctypes.sizeof(_lib.TextBlock)), ("table", "<u8"), ("scores", "<u8"), ("profiles", "<u8"),
+                     ("n_ang", "<i4"), ("stride", "<i4"), ("chosen", "<i4"), ("L", "<i4"), ("M", "<i4"), ("pad", "<i4"),
+                     ("u_min", "<f8"), ("v_min", "<f8"), ("c", "<f8"), ("s", "<f8")])
+
+
+def find_lines(blocks, scores=False):
     """Text blocks split into lines, every block in four launches whatever their number (mn_find_lines_u8; DESIGN.md 7b, "Text
-    blocks").  blocks: list of (img, rect, vertical, polarity, min_ink, gap, min_height): img a uint8 [H, W, 3] CUDA view with
-    dense pixels (any row stride) read in place, rect (x0, y0, x1, y1) a non-empty crop inside it with sides <= 32767, vertical a
-    bool, polarity _lib.INK_AUTO / INK_DARK / INK_LIGHT, and min_ink, gap, min_height positive integers or None for the
-    default.  Returns the uint8 CUDA tensor of the blocks' mn_block_lines records, in order (read it back as
-    ``block_lines_dtype()``)."""
+    blocks").  blocks: list of (img, rect, vertical, polarity, min_ink, gap, min_height[, skew, max_skew]): img a uint8 [H, W, 3]
+    CUDA view with dense pixels (any row stride) read in place, rect (x0, y0, x1, y1) a non-empty crop inside it with sides
+    <= 32767, vertical a bool, polarity _lib.INK_AUTO / INK_DARK / INK_LIGHT, and min_ink, gap, min_height positive integers or
+    None for the default.  Returns the uint8 CUDA tensor of the blocks' mn_block_lines records, in order (read it back as
+    ``block_lines_dtype()``).
+    skew (DESIGN.md 7b, "Skewed blocks"): None, "auto" (search +-max_skew degrees) or a given angle in degrees, |skew| < 45.  A
+    call with any skewed block goes through mn_find_lines_skewed_u8's six launches instead, every block of it, whatever their
+    number; blocks with skew None keep their mn_block_lines records exactly.  The tensor then holds the n mn_block_lines records
+    followed by the n mn_skew_block records (``skew_block_dtype()``: the chosen index and frame).  ``scores`` (tests): also
+    return, per block, the int64 CUDA view of its per-angle scores (None unless it searched)."""
     import numpy as np
     global LAUNCHES
     if not blocks:
         raise ValueError("find_lines: no blocks")
     if len(blocks) > 65535:
         raise ValueError("find_lines: at most 65535 blocks per launch")
+    if any(len(b) > 7 and b[7] is not None for b in blocks):
+        return _find_lines_skewed(blocks, scores)
+    blocks = [b[:7] for b in blocks]
     dev = blocks[0][0].device
     osz, rsz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.TextBlock)
     dims = []
@@ -1614,7 +1658,78 @@ def find_lines(blocks):
     rec.copy_(torch.from_numpy(np.frombuffer(bytes((_lib.TextBlock * len(recs))(*recs)), dtype=np.uint8).copy()))
     _lib.check(_lib.load().mn_find_lines_u8(_ptr(rec), len(recs), tiles, work, 4 * n_work, _stream()), "mn_find_lines_u8")
     LAUNCHES += 4
-    return buf[:len(blocks) * osz]
+    out = buf[:len(blocks) * osz]
+    return (out, [None] * len(blocks)) if scores else out
+
+
+def _find_lines_skewed(blocks, want_scores):
+    """find_lines for a call that holds a skewed block: mn_find_lines_skewed_u8 over every block.  A block without skew searches
+    the one-entry table (1, 0), which leaves its crop record and so its mn_block_lines record as mn_find_lines_u8 writes it."""
+    import numpy as np
+    global LAUNCHES
+    dev = blocks[0][0].device
+    n = len(blocks)
+    osz, ssz, rsz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.SkewBlock), ctypes.sizeof(_lib.TextBlock)
+    dims, tables, keys = [], [], {}
+    for i, blk in enumerate(blocks):
+        img, rect, vertical, polarity, *knobs = blk[:7]
+        skew, max_skew = blk[7] if len(blk) > 7 else None, blk[8] if len(blk) > 8 else 10.0
+        _dense_u8(img, dev, 3, f"find_lines: block {i}: img")
+        x0, y0, x1, y1 = (int(v) for v in rect)
+        if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
+            raise ValueError(f"find_lines: block {i}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
+                             f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
+        if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or \
+                any(v is not None and not 1 <= v < 2 ** 31 for v in knobs):
+            raise ValueError(f"find_lines: block {i}: bad polarity {polarity!r} or min_ink / gap / min_height {knobs!r}")
+        if skew is None:
+            cs = [(1.0, 0.0)]
+        elif skew == "auto" if isinstance(skew, str) else math.isfinite(skew) and abs(skew) < 45:
+            if not (isinstance(skew, str) or max_skew == 10.0) or not 0 < max_skew <= 20:
+                raise ValueError(f"find_lines: block {i}: max_skew {max_skew!r} is outside (0, 20] or given without 'auto'")
+            cs = skew_cos_sin(skew_table(skew, max_skew, vertical))
+        else:
+            raise ValueError(f"find_lines: block {i}: bad skew {skew!r}")
+        stride = skew_stride(x1 - x0, y1 - y0, vertical, cs)
+        if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
+            raise ValueError(f"find_lines: block {i}: {len(cs)} angles x {stride} bins exceed the {SKEW_MAX_PROFILE} profile "
+                             f"values a skewed block may use")
+        key = tuple(cs)
+        if key not in keys:
+            keys[key] = sum(len(t) for t in tables)
+            tables.append(cs)
+        dims.append((x0, y0, x1 - x0, y1 - y0, len(cs), stride, keys[key]))
+    n_tab = sum(len(t) for t in tables)
+    n_scores = sum(d[4] for d in dims if d[4] > 1)
+    n_work = sum(256 + 3 * d[5] + (d[4] * d[5] if d[4] > 1 else 0) for d in dims)
+    n_scratch = sum(2 * d[5] + 4 for d in dims)
+    head = n * (osz + ssz + rsz) + 16 * n_tab
+    buf = torch.empty(head + 8 * n_scores + 4 * (n_work + n_scratch), dtype=torch.uint8, device=dev)
+    out, sk, seg = buf.data_ptr(), buf.data_ptr() + n * osz, buf.data_ptr() + n * (osz + ssz)
+    tab, work = seg + n * rsz, buf.data_ptr() + head
+    w32, scratch = work + 8 * n_scores, work + 8 * n_scores + 4 * n_work
+    recs, srecs, views, w, s, o, tiles = [], [], [], 0, 0, 0, 0
+    for i, (blk, (x0, y0, bw, bh, n_ang, stride, t)) in enumerate(zip(blocks, dims)):
+        img, _, vertical, polarity, min_ink, gap, min_height = blk[:7]
+        prof = w32 + 4 * (w + 256)
+        tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, min_ink or 0, gap or 0,
+                            min_height or 0, 0, w32 + 4 * w, prof, scratch + 4 * s, out + i * osz)
+        recs.append(tb)
+        srecs.append(_lib.SkewBlock(tb, tab + 16 * t, work + 8 * o if n_ang > 1 else 0, prof + 4 * 3 * stride if n_ang > 1 else 0,
+                                    n_ang, stride, 0, 0, 0, 0, 0.0, 0.0, 0.0, 0.0))
+        views.append(buf[head + 8 * o:head + 8 * (o + n_ang)].view(torch.int64) if n_ang > 1 else None)
+        o += n_ang if n_ang > 1 else 0
+        w += 256 + 3 * stride + (n_ang * stride if n_ang > 1 else 0)
+        s += 2 * stride + 4
+        tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
+    host = bytes((_lib.SkewBlock * n)(*srecs)) + bytes((_lib.TextBlock * n)(*recs)) + \
+        np.array([v for t in tables for p in t for v in p], np.float64).tobytes()
+    buf[n * osz:head].copy_(torch.from_numpy(np.frombuffer(host, dtype=np.uint8).copy()))
+    _lib.check(_lib.load().mn_find_lines_skewed_u8(ctypes.c_void_p(seg), ctypes.c_void_p(sk), n, tiles, work,
+                                                   8 * n_scores + 4 * n_work, _stream()), "mn_find_lines_skewed_u8")
+    LAUNCHES += 6
+    res = buf[:n * (osz + ssz)]
+    return (res, views) if want_scores else res
 
 
 def vertical_unlayout(items):

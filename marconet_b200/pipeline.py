@@ -9,6 +9,7 @@ numeric runs through the module API (and therefore through the CUDA kernels).
 """
 import itertools
 import math
+import numbers
 import threading
 from typing import NamedTuple
 
@@ -1537,13 +1538,17 @@ class TextBlock(NamedTuple):
     around the lines.  ``direction``: "horizontal" (lines read top to bottom) or "vertical" (columns read right to left).
     ``min_ink``, ``gap``, ``min_height``: positive integers in place of the segmentation's defaults.  ``polarity``: "auto" (the
     minority side of the Otsu threshold is ink), "dark" or "light".  find_lines splits it into lines; restore_regions restores
-    each line in its place."""
+    each line in its place.  ``skew`` (DESIGN.md 7b, "Skewed blocks"): None (level lines), a given angle in degrees with
+    |skew| < 45, counter-clockwise on screen as OrientedRegion.from_rotated's, or "auto": the angle is searched on the device
+    within +-``max_skew`` degrees (in (0, 20], only with "auto") and the lines are OrientedRegions of that angle."""
     rect: object
     direction: str = "horizontal"
     min_ink: object = None
     gap: object = None
     min_height: object = None
     polarity: str = "auto"
+    skew: object = None
+    max_skew: float = 10.0
 
 
 _INK = {"auto": 0, "dark": 1, "light": 2}
@@ -1572,6 +1577,23 @@ def _check_block(blk, H, W, name):
         v = getattr(blk, what)
         if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 1 <= v < 2 ** 31):
             raise ValueError(f"{name}: {what} must be a positive integer, got {v!r}")
+    sk, ms = blk.skew, blk.max_skew
+    auto = isinstance(sk, str) and sk == "auto"
+    if not (sk is None or auto or (isinstance(sk, numbers.Real) and not isinstance(sk, bool) and math.isfinite(sk)
+                                   and abs(sk) < 45)):
+        raise ValueError(f"{name}: skew must be None, 'auto' or a finite angle in degrees with |skew| < 45, got {sk!r}")
+    if isinstance(ms, bool) or not isinstance(ms, numbers.Real) or not 0 < ms <= 20:
+        raise ValueError(f"{name}: max_skew must be a number of degrees in (0, 20], got {ms!r}")
+    if ms != 10.0 and not auto:
+        raise ValueError(f"{name}: max_skew is given, but skew is {sk!r}, not 'auto'")
+    if sk is not None:
+        from . import ops
+        vertical = blk.direction == "vertical"
+        table = ops.skew_table(sk, ms, vertical)
+        stride = ops.skew_stride(x1 - x0, y1 - y0, vertical, ops.skew_cos_sin(table))
+        if len(table) > 1 and len(table) * stride > ops.SKEW_MAX_PROFILE:
+            raise ValueError(f"{name}: the angle search needs {len(table)} angles x {stride} bins, over the "
+                             f"{ops.SKEW_MAX_PROFILE} profile values a block may use (narrow max_skew or split the block)")
     return x0, y0, x1, y1
 
 
@@ -1580,20 +1602,50 @@ def _find_lines(dimg, items):
     copy and one synchronisation.  Returns per item dict(lines, threshold, ink), or the error message of a block with too many
     lines."""
     from . import ops
-    recs = ops.find_lines([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap, blk.min_height)
-                           for i, blk, rect in items])
-    table = _to_host(recs).numpy().view(ops.block_lines_dtype())
+    recs = ops.find_lines([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap, blk.min_height,
+                            blk.skew, blk.max_skew) for i, blk, rect in items])
+    host = _to_host(recs).numpy()
+    n_osz = len(items) * ops.block_lines_dtype().itemsize
+    table = host[:n_osz].view(ops.block_lines_dtype())
+    skew = host[n_osz:].view(ops.skew_block_dtype()) if len(host) > n_osz else [None] * len(items)
     out = []
-    for (i, blk, rect), t in zip(items, table):
+    for (i, blk, rect), t, sk in zip(items, table, skew):
         n = int(t["n_lines"])
         if n < 0:
             out.append(f"{-n} lines exceed the {ops._lib.BLOCK_MAX_LINES} a text block may hold")
             continue
         lines = [tuple(int(v) for v in q) for q in t["rect"][:n]]
-        if blk.direction == "vertical":
+        vertical = blk.direction == "vertical"
+        if blk.skew is not None and sk["s"] != 0:
+            lines = skew_lines(rect, vertical, float(sk["c"]), float(sk["s"]), float(sk["u_min"]), float(sk["v_min"]), lines)
+        elif vertical:
             lines = [VerticalRegion(q) for q in lines]
-        out.append(dict(lines=lines, threshold=int(t["threshold"]), ink="dark" if t["ink"] == ops._lib.INK_DARK else "light"))
+        res = dict(lines=lines, threshold=int(t["threshold"]), ink="dark" if t["ink"] == ops._lib.INK_DARK else "light")
+        if blk.skew is not None:
+            table_angles = ops.skew_table(blk.skew, blk.max_skew, vertical)
+            angle = table_angles[int(sk["chosen"])]
+            res["skew"] = float(blk.skew) if not isinstance(blk.skew, str) else 0.0 - angle if vertical else angle
+        out.append(res)
     return out
+
+
+def skew_lines(rect, vertical, c, s, u_min, v_min, frame_lines):
+    """The lines of a skewed block (DESIGN.md 7b, "Skewed blocks") from its frame lines (c0, l0, c1, l1): edges a = u_min - 0.5
+    + c and b = v_min - 0.5 + l along e = (c, -s) and f = (s, c) from the crop's centre O, each corner O + a e + b f in fp64.
+    OrientedRegions top to bottom, or for a vertical block (whose frame is the transposed crop) VerticalRegions of
+    OrientedRegions, tl -> tr across the column, right to left."""
+    x0, y0, x1, y1 = rect
+    ox, oy = (y0 + (y1 - y0) / 2, x0 + (x1 - x0) / 2) if vertical else (x0 + (x1 - x0) / 2, y0 + (y1 - y0) / 2)
+    ex, ey, fx, fy = c, -s, s, c
+    out = []
+    for c0, l0, c1, l1 in frame_lines:
+        a0, a1 = u_min - 0.5 + c0, u_min - 0.5 + c1
+        b0, b1 = v_min - 0.5 + l0, v_min - 0.5 + l1
+        tl = (ox + a0 * ex + b0 * fx, oy + a0 * ey + b0 * fy)
+        tr = (ox + a1 * ex + b0 * fx, oy + a1 * ey + b0 * fy)
+        bl = (ox + a0 * ex + b1 * fx, oy + a0 * ey + b1 * fy)
+        out.append(VerticalRegion(OrientedRegion(tl[::-1], bl[::-1], tr[::-1])) if vertical else OrientedRegion(tl, tr, bl))
+    return out[::-1] if vertical else out
 
 
 @torch.no_grad()
@@ -1607,7 +1659,11 @@ def find_lines(images, blocks):
     Returns per image a list with one dict per block: lines, integer rectangles (x0, y0, x1, y1) in image pixels top to bottom
     (VerticalRegions of such rectangles, right to left, for a vertical block), each one a region restore_regions takes;
     threshold, Otsu's t; ink, "dark" or "light".  Raises ValueError naming the image and the block, before any launch, for a
-    block restore_regions would reject, and after the segmentation for a block of more than 256 lines."""
+    block restore_regions would reject, and after the segmentation for a block of more than 256 lines.
+    A block with ``skew`` (DESIGN.md 7b, "Skewed blocks") has its angle searched (or given) on the device and is split in the
+    rotated frame; a call that holds one runs every block through ops.find_lines' six launches.  Its dict gains ``skew``, the
+    angle used in degrees, and its lines are OrientedRegions (VerticalRegions of OrientedRegions for a vertical block), or the
+    rectangles of skew=None when the angle is exactly 0."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     blocks = _per_image(blocks, len(imgs), "blocks (one list per image)")
     items, names = [], []
@@ -1653,10 +1709,11 @@ def _plan_blocks(shapes, regions, labels, boxes):
     return blocks, stand_in
 
 
-def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid):
+def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid, shapes=None, scale=4, feather=None):
     """The region, label and box lists with each text block replaced in place by its lines, and per image the layout of its given
     regions: None for a region, the block's find_lines result (or dict(error=...) under ``skip_invalid``) for a block.  A block
-    with too many lines, or a vertical line that vertical_plan rejects, raises ValueError without ``skip_invalid``."""
+    with too many lines, a vertical line that vertical_plan rejects, or an oriented line of a skewed block that plan_regions
+    rejects (on the image of ``shapes`` at ``scale`` and ``feather``) raises ValueError without ``skip_invalid``."""
     found = {(i, r): res for (i, r, _, _), res in zip(blocks, found)}
     n = len(regions)
     labels, boxes = _per_image(labels, n, "labels"), _per_image(boxes, n, "boxes")
@@ -1674,7 +1731,12 @@ def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid):
             err = f"{name}: {res}" if isinstance(res, str) else None
             try:
                 for k, q in enumerate(res["lines"] if err is None else []):
-                    if isinstance(q, VerticalRegion):
+                    if isinstance(q, OrientedRegion) or isinstance(q, VerticalRegion) and isinstance(q.shape, OrientedRegion):
+                        try:
+                            plan_regions([shapes[i]], [[q]], None, None, scale, feather)
+                        except ValueError as e:
+                            raise ValueError(f"{name}, line {k}: {str(e).split(': ', 1)[-1]}") from None
+                    elif isinstance(q, VerticalRegion):
                         vertical_plan(q.shape[2] - q.shape[0], q.shape[3] - q.shape[1], name=f"{name}, line {k}")
             except ValueError as e:
                 err = str(e)
@@ -1895,7 +1957,9 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     call in the same four launches, one pinned copy of the line table and one synchronisation), and its lines, rectangles or
     VerticalRegions, take its place in the region list; the call then goes on as if they had been given.  No labels or boxes
     may be given for a block.  Its entry is dict(lines, threshold, ink, regions), regions one entry per line as above; a block
-    of more than 256 lines, or with a vertical line vertical_plan rejects, raises, or is dict(error=...) with ``skip_invalid``."""
+    of more than 256 lines, or with a vertical line vertical_plan rejects, raises, or is dict(error=...) with ``skip_invalid``.
+    A skewed block (DESIGN.md 7b, "Skewed blocks") takes the place of its OrientedRegion lines alike, and its entry gains
+    ``skew``; a line plan_regions rejects makes the block's error."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     shapes = [im.shape[:2] for im in imgs]
@@ -1909,7 +1973,8 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         dimg = _device_images(range(len(imgs)), imgs, dev)
         if blocks:                                       # every block's lines take its place in the region list
             found = _find_lines(dimg, [(i, blk, rect) for i, _, blk, rect in blocks])
-            regions, labels, boxes, layout = _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid)
+            regions, labels, boxes, layout = _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid, shapes, scale,
+                                                            feather)
             plan = plan_regions(shapes, regions, labels, boxes, scale, feather)
         crops = [dimg[p.image][p.rect[1]:p.rect[3], p.rect[0]:p.rect[2]] for p in plan]
         oriented = [k for k, p in enumerate(plan) if p.oriented is not None]
