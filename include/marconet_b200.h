@@ -672,7 +672,8 @@ int mn_composite_regions_curved_u8(const mn_region_curved* regions, int n, long 
  * every block of a call, whatever their number:
  *   1. histogram: hist[g] = #{g(x, y) = g}, g = (c0 + c1 + c2 + 1) / 3, tiles of 32 x 32 pixels, blockIdx.y = block;
  *   2. threshold, one thread per block: t = OpenCV's Otsu threshold of hist (getThreshVal_Otsu_8u's fp64 loop, every operation
- *      rounded on its own), D = #{g <= t}; ink = polarity, or for MN_INK_AUTO dark (g <= t) iff 2 D <= h w, else light (g > t);
+ *      rounded on its own, over the n = h w pixels the histogram counts), D = #{g <= t}; ink = polarity, or for MN_INK_AUTO
+ *      dark (g <= t) iff 2 D <= n, else light (g > t); t = 0 when n = 0;
  *   3. profile over the tiles: for every index l < L, prof[l] = the ink count, prof[L + l] = M - (the least ink index along the
  *      line), prof[2 L + l] = the largest ink index along the line + 1 (0 where there is no ink);
  *   4. segmentation, one CTA per block: the runs of indices with prof[l] >= m (m = min_ink, default max(1, M / 128)), merged
@@ -785,6 +786,37 @@ typedef struct {
 } mn_text_page;
 int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, void* work, long long work_bytes,
                       void* stream);
+
+/* Skewed pages (DESIGN.md section 7b, "Skewed pages").  Page i is searched as a skewed block on skew[i] (skew[i].b, blocks[i] and
+ * pages[i].b the same crop record on entry; a page without skew the one-entry table (1, 0)), and the XY-cut of
+ * mn_find_blocks_u8 runs on a bitmap of frame cells.  mn_find_blocks_skewed_u8 issues 7 + 6 MN_PAGE_LEVELS launches for every
+ * page of a call, whatever the number of pages and nodes:
+ *   1-4. mn_find_lines_skewed_u8's histogram, threshold, angle profiles and scores (the chosen frame into skew[i]);
+ *   5. the frame bitmap: bit j & 31 of bits[k wpitch + j / 32] is set iff an ink pixel has cell (k, j) in the frame at (c, s),
+ *      or for a vertical page at (c, -s) on the untransposed crop (the transposed search frame with its axes swapped); the root
+ *      node, and pages[i].b.w = M, pages[i].b.h = L;
+ *   6-13. mn_find_blocks_u8's levels, text size and leaves, in frame cells.
+ * bits holds max L x wpitch words, wpitch >= max M / 32, and cap entries per list, max over the page's table; the angle
+ * profiles and scores are as mn_find_lines_skewed_u8's (b.prof unused).  work (work_bytes) is zeroed by the call. */
+int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles, void* work,
+                             long long work_bytes, void* stream);
+
+/* Windowed blocks (DESIGN.md section 7b, "Skewed pages").  Block i is the set of pixels of the crop wins[i].b whose frame cell
+ * (k, j) at (c, s) (the frame of "Skewed blocks", transposed crop for a vertical block) lies in [c0, c1) x [l0, l1).
+ * blocks[i] is its frame record: x0 = y0 = 0, w = c1 - c0, h = l1 - l0, vertical = 0, with hist, prof, scratch, out and the
+ * knobs shared with wins[i].b.  mn_find_lines_window_u8 issues four launches for every block of a call: the histogram of the
+ * set and the profile in bins k - l0 and indices j - c0, both over the tiles of the footprint [px0, px0 + pw) x
+ * [py0, py0 + ph) of crop pixels (which holds the set), and mn_find_lines_u8's threshold and segmentation over blocks[].
+ * out->rect[k] is therefore (c0', l0', c1', l1') in window cells, top to bottom.  max_tiles >= every footprint's tile count;
+ * work (work_bytes) covers every hist and prof of the call and is zeroed by the call. */
+typedef struct {
+    mn_text_block b;            /* the crop record */
+    double c, s;                /* the frame's angle */
+    int32_t c0, l0, c1, l1;     /* the window, in frame cells */
+    int32_t px0, py0, pw, ph;   /* its footprint, in crop pixels */
+} mn_window_block;
+int mn_find_lines_window_u8(const mn_text_block* blocks, const mn_window_block* wins, int n, long long max_tiles, void* work,
+                            long long work_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -173,6 +173,11 @@ class SkewBlock(Structure):
                 ("v_min", c_double), ("c", c_double), ("s", c_double)]
 
 
+class WindowBlock(Structure):
+    _fields_ = [("b", TextBlock), ("c", c_double), ("s", c_double), ("c0", c_int32), ("l0", c_int32), ("c1", c_int32),
+                ("l1", c_int32), ("px0", c_int32), ("py0", c_int32), ("pw", c_int32), ("ph", c_int32)]
+
+
 PAGE_LEVELS, PAGE_MAX_BLOCKS, PAGE_MAX_NODES = 24, 1024, 65536    # MN_PAGE_LEVELS, MN_PAGE_MAX_BLOCKS, MN_PAGE_MAX_NODES
 PAGE_REJECTED = 8                                                  # MN_PAGE_REJECTED
 PAGE_ERR_NODES, PAGE_ERR_BLOCKS = 1, 2
@@ -256,6 +261,8 @@ SYMBOLS = {
     "mn_find_lines_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_skewed_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_blocks_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
+    "mn_find_blocks_skewed_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
+    "mn_find_lines_window_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -3,7 +3,8 @@
 // explicit-rounding intrinsics, so that nvcc cannot contract it into an FMA the host twin (oracle/blocks.py) does not have; the
 // rest is integer arithmetic.  Skewed blocks (DESIGN.md 7b, "Skewed blocks") add an angle search and a rotated profile around
 // the same kernels, in six launches.  Text pages (DESIGN.md 7b, "Text pages") reuse the histogram and threshold kernels and find
-// blocks by a level-synchronous XY-cut over an ink bitmap.
+// blocks by a level-synchronous XY-cut over an ink bitmap.  Skewed pages (DESIGN.md 7b, "Skewed pages") run the same XY-cut on a
+// bitmap of rotated-frame cells, and their blocks are windows of that frame.
 #include "mn_common.cuh"
 
 namespace {
@@ -49,14 +50,16 @@ __global__ void block_threshold_kernel(const mn_text_block* __restrict__ blocks,
     if (i >= n) return;
     const mn_text_block b = blocks[i];
     const int* h = b.hist;
-    const double scale = __ddiv_rn(1.0, (double)(b.w * b.h));
+    long long count = 0;                                // the pixels counted: w h, or a window's pixel set
+    for (int k = 0; k < 256; ++k) count += h[k];
+    const double scale = __ddiv_rn(1.0, (double)count);
     double mu = 0.0;
     for (int k = 0; k < 256; ++k) mu = __dadd_rn(mu, __dmul_rn((double)k, (double)h[k]));
     mu = __dmul_rn(mu, scale);
     const double eps = 1.1920928955078125e-07;    // FLT_EPSILON
     double mu1 = 0.0, q1 = 0.0, max_sigma = 0.0;
     int t = 0;
-    for (int k = 0; k < 256; ++k) {
+    for (int k = 0; k < (count ? 256 : 0); ++k) {
         const double p = __dmul_rn((double)h[k], scale);
         mu1 = __dmul_rn(mu1, q1);
         q1 = __dadd_rn(q1, p);
@@ -74,7 +77,7 @@ __global__ void block_threshold_kernel(const mn_text_block* __restrict__ blocks,
     long long dark = 0;
     for (int k = 0; k <= t; ++k) dark += h[k];
     int ink = b.polarity;
-    if (ink == MN_INK_AUTO) ink = 2 * dark <= (long long)b.w * b.h ? MN_INK_DARK : MN_INK_LIGHT;
+    if (ink == MN_INK_AUTO) ink = 2 * dark <= count ? MN_INK_DARK : MN_INK_LIGHT;
     b.out->threshold = t;
     b.out->ink = ink;
 }
@@ -906,6 +909,164 @@ __global__ void __launch_bounds__(kScanThreads) page_blocks_kernel(mn_text_page*
     }
 }
 
+
+// ---- Skewed pages (DESIGN.md 7b, "Skewed pages") ----
+// The page's angle is searched by the skewed-block kernels on its mn_skew_block record; the XY-cut then runs unchanged on a
+// bitmap of frame cells, whose sides the page record takes.  A vertical page's bitmap is of the untransposed frame at the
+// reported angle: with the rounded operations u(X, Y, c, -s) = v(Y, X, c, s) and v(X, Y, c, -s) = u(Y, X, c, s), so negating s
+// on the untransposed crop swaps the axes of the transposed search frame exactly.
+
+// 3'. The frame bitmap: every ink pixel sets its cell's bit (bit j & 31 of bits[k wpitch + j / 32]); tile 0 writes the root
+// node and the frame's sides (M x L) into the page record.  At s = 0 the cell of (x, y) is (x, y): page_bits_kernel's words.
+__global__ void __launch_bounds__(kTileThreads) page_frame_bits_kernel(mn_text_page* pages, const mn_skew_block* __restrict__ skew) {
+    mn_pdl_prologue();
+    mn_text_page& p = pages[blockIdx.y];
+    const mn_skew_block& sb = skew[blockIdx.y];
+    const mn_text_block b = sb.b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    const double c = sb.c, s = b.vertical ? -sb.s : sb.s;
+    const frame_t f = frame_of(b.w, b.h, c, s);
+    const int t = b.out->threshold;
+    const bool dark = b.out->ink == MN_INK_DARK;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, x = tx + lane;
+    const double X = centre(x, b.w);
+    for (int j = 0; j < kTile / 8; ++j) {
+        const int y = ty + warp + 8 * j;
+        if (x >= b.w || y >= b.h) continue;
+        const int g = block_grey(b, x, y);
+        if (!(dark ? g <= t : g > t)) continue;
+        const double Y = centre(y, b.h);
+        const int k = frame_bin(frame_v(X, Y, c, s), f.v_min, f.L);
+        const int i = min(max((int)floor(__dsub_rn(frame_u(X, Y, c, s), f.u_min)), 0), f.M - 1);
+        atomicOr(&p.bits[(long long)k * p.wpitch + (i >> 5)], 1u << (i & 31));
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        mn_page_node r;
+        r.x0 = 0; r.y0 = 0; r.x1 = (int16_t)f.M; r.y1 = (int16_t)f.L;
+        r.st = b.vertical ? 0 : MN_PAGE_ROWS;
+        p.b.w = f.M;
+        p.b.h = f.L;
+        p.list[0][0] = r;
+        p.n[0] = 1;
+        p.src = 0;
+        p.open = 1;
+        p.gx = p.gy = 1;
+    }
+}
+
+// ---- Windowed blocks (DESIGN.md 7b, "Skewed pages") ----
+// A block that is the pixels of its crop whose frame cell at a given angle lies in a window.  Its histogram and profile cover
+// the tiles of the window's footprint and test every pixel's cell; the threshold and segmentation kernels run on the window's
+// own frame record.
+
+__device__ __forceinline__ bool window_tile(const mn_window_block& wb, int& tx, int& ty) {
+    const int tiles_x = (wb.pw + kTile - 1) / kTile, tiles_y = (wb.ph + kTile - 1) / kTile;
+    if ((long long)blockIdx.x >= (long long)tiles_x * tiles_y) return false;
+    tx = wb.px0 + (int)(blockIdx.x % tiles_x) * kTile;
+    ty = wb.py0 + (int)(blockIdx.x / tiles_x) * kTile;
+    return true;
+}
+
+// The cell (k, j) of frame pixel (fx, fy); true when it lies in the window.
+__device__ __forceinline__ bool window_cell(const mn_window_block& wb, const frame_t& f, int wt, int ht, int fx, int fy, int& k,
+                                            int& j) {
+    const double X = centre(fx, wt), Y = centre(fy, ht);
+    k = frame_bin(frame_v(X, Y, wb.c, wb.s), f.v_min, f.L);
+    j = min(max((int)floor(__dsub_rn(frame_u(X, Y, wb.c, wb.s), f.u_min)), 0), f.M - 1);
+    return k >= wb.l0 && k < wb.l1 && j >= wb.c0 && j < wb.c1;
+}
+
+__global__ void __launch_bounds__(kTileThreads) window_hist_kernel(const mn_window_block* __restrict__ wins) {
+    mn_pdl_prologue();
+    __shared__ int s_hist[256];
+    const mn_window_block& wb = wins[blockIdx.y];
+    const mn_text_block b = wb.b;
+    int tx, ty;
+    if (!window_tile(wb, tx, ty)) return;
+    s_hist[threadIdx.x] = 0;
+    __syncthreads();
+    int wt, ht;
+    frame_dims(b, wt, ht);
+    const frame_t f = frame_of(wt, ht, wb.c, wb.s);
+    const int x = tx + (threadIdx.x & 31);
+    if (x < b.w) {
+        for (int y = ty + (threadIdx.x >> 5); y < min(ty + kTile, b.h); y += 8) {
+            int k, j;
+            if (window_cell(wb, f, wt, ht, b.vertical ? y : x, b.vertical ? x : y, k, j)) atomicAdd(&s_hist[block_grey(b, x, y)], 1);
+        }
+    }
+    __syncthreads();
+    const int v = s_hist[threadIdx.x];
+    if (v) atomicAdd(&b.hist[threadIdx.x], v);
+}
+
+// The window's profile in its own frame: bin k - l0, index j - c0, laid out as mn_find_lines_u8's (L = l1 - l0, M = c1 - c0).
+__global__ void __launch_bounds__(kTileThreads) window_profile_kernel(const mn_window_block* __restrict__ wins) {
+    mn_pdl_prologue();
+    __shared__ unsigned s_m[kTile], s_row[kTile];
+    __shared__ int s_cnt[kBins], s_lo[kBins], s_hi[kBins];
+    const mn_window_block& wb = wins[blockIdx.y];
+    const mn_text_block b = wb.b;
+    int tx, ty;
+    if (!window_tile(wb, tx, ty)) return;
+    if (threadIdx.x < kBins) s_cnt[threadIdx.x] = s_lo[threadIdx.x] = s_hi[threadIdx.x] = 0;
+    tile_ink_rows(b, tx, ty, s_m, s_row);
+    int wt, ht;
+    frame_dims(b, wt, ht);
+    const int fx0 = b.vertical ? ty : tx, fy0 = b.vertical ? tx : ty;
+    const int nx = min(kTile, wt - fx0), ny = min(kTile, ht - fy0);
+    const frame_t f = frame_of(wt, ht, wb.c, wb.s);
+    const int L = wb.l1 - wb.l0, M = wb.c1 - wb.c0;
+    const int k0 = tile_bin0(fx0, fy0, nx, ny, wt, ht, wb.c, wb.s, f.v_min, f.L) - wb.l0;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int r = warp; r < ny; r += kTileThreads / 32) {
+        int k, j;
+        if (!((s_row[r] >> lane) & 1u) || !window_cell(wb, f, wt, ht, fx0 + lane, fy0 + r, k, j)) continue;
+        k -= wb.l0;
+        j -= wb.c0;
+        if (k - k0 >= 0 && k - k0 < kBins) {
+            atomicAdd(&s_cnt[k - k0], 1);
+            atomicMax(&s_lo[k - k0], M - j);
+            atomicMax(&s_hi[k - k0], j + 1);
+        } else {
+            atomicAdd(&b.prof[k], 1);
+            atomicMax(&b.prof[L + k], M - j);
+            atomicMax(&b.prof[2 * L + k], j + 1);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < kBins && s_cnt[threadIdx.x]) {
+        const int k = k0 + threadIdx.x;
+        atomicAdd(&b.prof[k], s_cnt[threadIdx.x]);
+        atomicMax(&b.prof[L + k], s_lo[threadIdx.x]);
+        atomicMax(&b.prof[2 * L + k], s_hi[threadIdx.x]);
+    }
+}
+
+// 4-11 of the XY-cut: both passes of levels, the text size between them and the leaves, on pages whose bitmap and root are
+// written.
+int page_levels(mn_text_page* pages, int n, cudaStream_t st) {
+    const dim3 grid((unsigned)max(1, 4 * mn_num_sms() / n), (unsigned)n);   // about four CTAs per SM over all pages
+    for (int pass = 0; pass < 2; ++pass) {
+        for (int level = 0; level < MN_PAGE_LEVELS; ++level) {
+            MN_CUDA_CHECK((mn_launch(page_count_kernel, grid, dim3(kPageThreads), 0, st, pages, level)));
+            MN_LAUNCH_CHECK();
+            MN_CUDA_CHECK((mn_launch(page_scan_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
+            MN_LAUNCH_CHECK();
+            MN_CUDA_CHECK((mn_launch(page_emit_kernel, grid, dim3(kPageThreads), 0, st, pages, level)));
+            MN_LAUNCH_CHECK();
+        }
+        if (pass == 0) {
+            MN_CUDA_CHECK((mn_launch(page_size_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
+            MN_LAUNCH_CHECK();
+        }
+    }
+    MN_CUDA_CHECK((mn_launch(page_blocks_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
 }  // namespace
 
 extern "C" int mn_find_lines_u8(const mn_text_block* blocks, int n, long long max_tiles, void* work, long long work_bytes,
@@ -953,7 +1114,6 @@ extern "C" int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* page
     MN_REQUIRE(blocks && pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
                "mn_find_blocks_u8: bad args");
     cudaStream_t st = (cudaStream_t)stream;
-    const dim3 grid((unsigned)max(1, 4 * mn_num_sms() / n), (unsigned)n);   // about four CTAs per SM over all pages
     MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
     MN_CUDA_CHECK((mn_launch(block_hist_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, blocks)));
     MN_LAUNCH_CHECK();
@@ -961,21 +1121,43 @@ extern "C" int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* page
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(page_bits_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, pages)));
     MN_LAUNCH_CHECK();
-    for (int pass = 0; pass < 2; ++pass) {
-        for (int level = 0; level < MN_PAGE_LEVELS; ++level) {
-            MN_CUDA_CHECK((mn_launch(page_count_kernel, grid, dim3(kPageThreads), 0, st, pages, level)));
-            MN_LAUNCH_CHECK();
-            MN_CUDA_CHECK((mn_launch(page_scan_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
-            MN_LAUNCH_CHECK();
-            MN_CUDA_CHECK((mn_launch(page_emit_kernel, grid, dim3(kPageThreads), 0, st, pages, level)));
-            MN_LAUNCH_CHECK();
-        }
-        if (pass == 0) {
-            MN_CUDA_CHECK((mn_launch(page_size_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
-            MN_LAUNCH_CHECK();
-        }
-    }
-    MN_CUDA_CHECK((mn_launch(page_blocks_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
+    return page_levels(pages, n, st);
+}
+
+extern "C" int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles,
+                                        void* work, long long work_bytes, void* stream) {
+    MN_REQUIRE(blocks && skew && pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
+               "mn_find_blocks_skewed_u8: bad args");
+    cudaStream_t st = (cudaStream_t)stream;
+    const mn_text_block* cblocks = blocks;
+    const mn_skew_block* cskew = skew;
+    MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
+    MN_CUDA_CHECK((mn_launch(block_hist_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cblocks)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(block_threshold_kernel, dim3(mn_cdiv(n, 128)), dim3(128), 0, st, cblocks, n)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(skew_angle_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cskew)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(skew_score_kernel, dim3(n), dim3(kScoreThreads), 0, st, blocks, skew)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(page_frame_bits_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, pages, cskew)));
+    MN_LAUNCH_CHECK();
+    return page_levels(pages, n, st);
+}
+
+extern "C" int mn_find_lines_window_u8(const mn_text_block* blocks, const mn_window_block* wins, int n, long long max_tiles,
+                                       void* work, long long work_bytes, void* stream) {
+    MN_REQUIRE(blocks && wins && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
+               "mn_find_lines_window_u8: bad args");
+    cudaStream_t st = (cudaStream_t)stream;
+    MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
+    MN_CUDA_CHECK((mn_launch(window_hist_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, wins)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(block_threshold_kernel, dim3(mn_cdiv(n, 128)), dim3(128), 0, st, blocks, n)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(window_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, wins)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(block_lines_kernel, dim3(n), dim3(kSegThreads), 0, st, blocks)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -1600,6 +1600,19 @@ def skew_stride(w, h, vertical, cs):
     return int((np.floor(v.max(axis=0) - v.min(axis=0)) + 1).max())
 
 
+def skew_frames(w, h, vertical, cs):
+    """(u_min, v_min, L, M) of a w x h crop's frames (transposed for a vertical crop) at each (c, s) of ``cs``, as the device's
+    frame_of computes them: fp64 arrays, every operation rounded on its own."""
+    import numpy as np
+    wt, ht = (h, w) if vertical else (w, h)
+    c, s = (np.array([p[k] for p in cs], np.float64) for k in (0, 1))
+    xs, ys = (0.5 - wt / 2, wt - 0.5 - wt / 2), (0.5 - ht / 2, ht - 0.5 - ht / 2)
+    u = np.stack([x * c - y * s for x in xs for y in ys])
+    v = np.stack([x * s + y * c for x in xs for y in ys])
+    return (u.min(axis=0), v.min(axis=0), (np.floor(v.max(axis=0) - v.min(axis=0)) + 1).astype(np.int64),
+            (np.floor(u.max(axis=0) - u.min(axis=0)) + 1).astype(np.int64))
+
+
 def skew_block_dtype():
     """numpy view of an mn_skew_block record after mn_find_lines_skewed_u8: the chosen index and frame."""
     import numpy as np
@@ -1732,6 +1745,80 @@ def _find_lines_skewed(blocks, want_scores):
     return (res, views) if want_scores else res
 
 
+def window_footprint(w, h, vertical, c, s, u_min, v_min, window):
+    """(px0, py0, px1, py1): the crop pixels that hold a window's pixel set, the fp64 bounding box of the window's corner pixel
+    centres (X = u c + v s, Y = v c - u s), padded by one pixel and clipped.  The padding covers the rounding of the frame."""
+    wt, ht = (h, w) if vertical else (w, h)
+    c0, l0, c1, l1 = window
+    xs, ys = [], []
+    for u in (u_min + c0, u_min + c1):
+        for v in (v_min + l0, v_min + l1):
+            xs.append(u * c + v * s + wt / 2 - 0.5)
+            ys.append(v * c - u * s + ht / 2 - 0.5)
+    fx0, fx1 = max(0, math.floor(min(xs)) - 1), min(wt, math.floor(max(xs)) + 2)
+    fy0, fy1 = max(0, math.floor(min(ys)) - 1), min(ht, math.floor(max(ys)) + 2)
+    return (fy0, fx0, fy1, fx1) if vertical else (fx0, fy0, fx1, fy1)
+
+
+def find_lines_window(blocks):
+    """Windowed text blocks split into lines, every block in four launches whatever their number (mn_find_lines_window_u8;
+    DESIGN.md 7b, "Skewed pages").  blocks: list of (img, rect, vertical, polarity, min_ink, gap, min_height, skew, window): as
+    find_lines', skew a given finite angle and window (c0, l0, c1, l1) a non-empty integer rectangle inside the crop's frame at
+    that angle (the transposed crop at the negated angle for a vertical block).  Returns the uint8 CUDA tensor of the blocks'
+    mn_block_lines records, in order, whose rectangles are (c0', l0', c1', l1') in cells of the window."""
+    import numpy as np
+    global LAUNCHES
+    if not blocks:
+        raise ValueError("find_lines_window: no blocks")
+    if len(blocks) > 65535:
+        raise ValueError("find_lines_window: at most 65535 blocks per launch")
+    dev = blocks[0][0].device
+    n = len(blocks)
+    osz, rsz, wsz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.TextBlock), ctypes.sizeof(_lib.WindowBlock)
+    dims = []
+    for i, (img, rect, vertical, polarity, min_ink, gap, min_height, skew, window) in enumerate(blocks):
+        _dense_u8(img, dev, 3, f"find_lines: block {i}: img")
+        x0, y0, x1, y1 = (int(v) for v in rect)
+        if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
+            raise ValueError(f"find_lines: block {i}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
+                             f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
+        if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or \
+                any(v is not None and not 1 <= v < 2 ** 31 for v in (min_ink, gap, min_height)):
+            raise ValueError(f"find_lines: block {i}: bad polarity {polarity!r} or min_ink / gap / min_height")
+        if isinstance(skew, str) or skew is None or not math.isfinite(skew) or abs(skew) >= 45:
+            raise ValueError(f"find_lines: block {i}: a window needs a given finite angle, got skew {skew!r}")
+        (c, s), = skew_cos_sin(skew_table(skew, 10.0, vertical))
+        u_min, v_min, L, M = (float(a[0]) for a in skew_frames(x1 - x0, y1 - y0, vertical, [(c, s)]))
+        c0, l0, c1, l1 = (int(v) for v in window)
+        if not (0 <= c0 < c1 <= M and 0 <= l0 < l1 <= L):
+            raise ValueError(f"find_lines: block {i}: window {(c0, l0, c1, l1)} is empty or outside the {int(M)}x{int(L)} frame")
+        fp = window_footprint(x1 - x0, y1 - y0, vertical, c, s, u_min, v_min, (c0, l0, c1, l1))
+        dims.append((x0, y0, x1 - x0, y1 - y0, c, s, (c0, l0, c1, l1), fp))
+    n_work = sum(256 + 3 * (d[6][3] - d[6][1]) for d in dims)
+    n_scratch = sum(2 * (d[6][3] - d[6][1]) + 4 for d in dims)
+    head = n * (osz + rsz + wsz)
+    buf = torch.empty(head + 4 * (n_work + n_scratch), dtype=torch.uint8, device=dev)
+    out, seg, wrec = buf.data_ptr(), buf.data_ptr() + n * osz, buf.data_ptr() + n * (osz + rsz)
+    work = buf.data_ptr() + head
+    scratch, w, sc, recs, wrecs, tiles = work + 4 * n_work, 0, 0, [], [], 0
+    for i, (blk, (x0, y0, bw, bh, c, s, (c0, l0, c1, l1), (px0, py0, px1, py1))) in enumerate(zip(blocks, dims)):
+        img, _, vertical, polarity, min_ink, gap, min_height = blk[:7]
+        hist, prof, scr = work + 4 * w, work + 4 * (w + 256), scratch + 4 * sc
+        knobs = (polarity, min_ink or 0, gap or 0, min_height or 0, 0, hist, prof, scr, out + i * osz)
+        recs.append(_lib.TextBlock(img.data_ptr(), img.stride(0), 0, 0, c1 - c0, l1 - l0, 0, *knobs))
+        crop = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), *knobs)
+        wrecs.append(_lib.WindowBlock(crop, c, s, c0, l0, c1, l1, px0, py0, px1 - px0, py1 - py0))
+        w += 256 + 3 * (l1 - l0)
+        sc += 2 * (l1 - l0) + 4
+        tiles = max(tiles, 1, -(-(px1 - px0) // 32) * -(-(py1 - py0) // 32))
+    host = bytes((_lib.TextBlock * n)(*recs)) + bytes((_lib.WindowBlock * n)(*wrecs))
+    buf[n * osz:head].copy_(torch.from_numpy(np.frombuffer(host, dtype=np.uint8).copy()))
+    _lib.check(_lib.load().mn_find_lines_window_u8(ctypes.c_void_p(seg), ctypes.c_void_p(wrec), n, tiles, work, 4 * n_work,
+                                                   _stream()), "mn_find_lines_window_u8")
+    LAUNCHES += 4
+    return buf[:n * osz]
+
+
 PAGE_MAX_WORK = 1 << 30        # bytes of device memory one find_blocks call may use
 
 
@@ -1749,20 +1836,43 @@ def page_bytes(w, h):
             + ctypes.sizeof(_lib.BlockLines) + 4 * h * -(-w // 32) + 3 * 4 * cap + 64)
 
 
-def find_blocks(pages):
+def skew_page_frame(w, h, vertical, cs):
+    """(L, M, stride) of a w x h page's frame bitmaps over the (c, s) of ``cs``: the most rows and columns a bitmap may have (the
+    search frame's axes swapped for a vertical page) and the most bins of its search frames."""
+    _, _, L, M = skew_frames(w, h, vertical, cs)
+    return (int(M.max()), int(L.max()), int(L.max())) if vertical else (int(L.max()), int(M.max()), int(L.max()))
+
+
+def skew_page_bytes(w, h, vertical, cs):
+    """Device bytes of one w x h page searched over ``cs`` in find_blocks: page_bytes of its largest frame, the search record
+    and table, and the per-angle scores and profiles of a search over more than one angle."""
+    L, M, stride = skew_page_frame(w, h, vertical, cs)
+    n = len(cs)
+    return page_bytes(M, L) + ctypes.sizeof(_lib.SkewBlock) + 16 * n + (8 * n + 4 * n * stride if n > 1 else 0) + 16
+
+
+def find_blocks(pages, scores=False):
     """Text pages split into blocks by a recursive XY-cut (mn_find_blocks_u8; DESIGN.md 7b, "Text pages"), every page of the call
     in 5 + 6 * 24 launches whatever the number of pages and nodes.  pages: list of (img, rect, vertical, polarity, gap_x, gap_y):
     img a uint8 [H, W, 3] CUDA view with dense pixels (any row stride) read in place, rect (x0, y0, x1, y1) a non-empty crop
     inside it with sides <= 32767, vertical a bool, polarity _lib.INK_AUTO / INK_DARK / INK_LIGHT, gap_x and gap_y positive
     integers or None for the default.  Returns (out, caps): out the uint8 CUDA tensor of the pages' mn_page_result records
     followed by each page's leaf table of caps[i] mn_page_node entries (read them back as ``page_result_dtype()`` and
-    ``page_node_dtype()``)."""
+    ``page_node_dtype()``).
+    skew, max_skew (DESIGN.md 7b, "Skewed pages"): as find_lines'.  A call with any skewed page goes through
+    mn_find_blocks_skewed_u8's 7 + 6 * 24 launches instead, every page of it; pages with skew None search the one-entry table
+    (1, 0) and keep their tables exactly.  out then starts with the n mn_skew_block records (``skew_block_dtype()``: the chosen
+    index and frame) and the leaves are in frame cells.  ``scores`` (tests): also return, per page, the int64 CUDA view of its
+    per-angle scores (None unless it searched)."""
     import numpy as np
     global LAUNCHES
     if not pages:
         raise ValueError("find_blocks: no pages")
     if len(pages) > 65535:
         raise ValueError("find_blocks: at most 65535 pages per launch")
+    if any(len(p) > 6 and p[6] is not None for p in pages):
+        return _find_blocks_skewed(pages, scores)
+    pages = [p[:6] for p in pages]
     dev = pages[0][0].device
     dims = []
     for i, (img, rect, vertical, polarity, *gaps) in enumerate(pages):
@@ -1802,7 +1912,96 @@ def find_blocks(pages):
     _lib.check(_lib.load().mn_find_blocks_u8(ctypes.c_void_p(base), ctypes.c_void_p(base + n * bsz), n, tiles,
                                              ctypes.c_void_p(base + out0), work0 + n_work - out0, _stream()), "mn_find_blocks_u8")
     LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS
-    return buf[out0:out0 + n_out], [d[4] for d in dims]
+    res = buf[out0:out0 + n_out], [d[4] for d in dims]
+    return res + ([None] * n,) if scores else res
+
+
+def _check_skew(skew, max_skew, vertical, what):
+    """The (c, s) table of skew / max_skew (find_lines' rules), or ValueError naming ``what``."""
+    if skew is None:
+        return [(1.0, 0.0)]
+    if not (skew == "auto" if isinstance(skew, str) else math.isfinite(skew) and abs(skew) < 45):
+        raise ValueError(f"{what}: bad skew {skew!r}")
+    if not (isinstance(skew, str) or max_skew == 10.0) or not 0 < max_skew <= 20:
+        raise ValueError(f"{what}: max_skew {max_skew!r} is outside (0, 20] or given without 'auto'")
+    return skew_cos_sin(skew_table(skew, max_skew, vertical))
+
+
+def _find_blocks_skewed(pages, want_scores):
+    """find_blocks for a call that holds a skewed page: mn_find_blocks_skewed_u8 over every page."""
+    import numpy as np
+    global LAUNCHES
+    dev = pages[0][0].device
+    n = len(pages)
+    rsz, bsz, psz, ssz, lsz = (ctypes.sizeof(t) for t in (_lib.PageResult, _lib.TextBlock, _lib.TextPage, _lib.SkewBlock,
+                                                           _lib.BlockLines))
+    dims, tables, keys, need = [], [], {}, 0
+    for i, pg in enumerate(pages):
+        img, rect, vertical, polarity, *gaps = pg[:6]
+        skew, max_skew = pg[6] if len(pg) > 6 else None, pg[7] if len(pg) > 7 else 10.0
+        _dense_u8(img, dev, 3, f"find_blocks: page {i}: img")
+        x0, y0, x1, y1 = (int(v) for v in rect)
+        if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
+            raise ValueError(f"find_blocks: page {i}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
+                             f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
+        if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or any(v is not None and not 1 <= v < 2 ** 31 for v in gaps):
+            raise ValueError(f"find_blocks: page {i}: bad polarity {polarity!r} or gap_x / gap_y {gaps!r}")
+        cs = _check_skew(skew, max_skew, vertical, f"find_blocks: page {i}")
+        need += skew_page_bytes(x1 - x0, y1 - y0, vertical, cs)
+        L, M, stride = skew_page_frame(x1 - x0, y1 - y0, vertical, cs)
+        if max(L, M) > 32767:
+            raise ValueError(f"find_blocks: page {i}: a frame side of {max(L, M)} exceeds 32767")
+        if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
+            raise ValueError(f"find_blocks: page {i}: {len(cs)} angles x {stride} bins exceed the {SKEW_MAX_PROFILE} profile "
+                             f"values a skewed page may use")
+        key = tuple(cs)
+        if key not in keys:
+            keys[key] = sum(len(t) for t in tables)
+            tables.append(cs)
+        dims.append((x0, y0, x1 - x0, y1 - y0, page_cap(M, L), L, M, len(cs), stride, keys[key]))
+    if need > PAGE_MAX_WORK:
+        raise ValueError(f"find_blocks: the pages need more than the {PAGE_MAX_WORK} bytes of work memory a call may use")
+    n_tab = sum(len(t) for t in tables)
+    pg0, tab0 = n * bsz, n * (bsz + psz)                 # records, tables and the skew records, then the results and leaves,
+    out0 = -(-(tab0 + 16 * n_tab + n * ssz) // 16) * 16  # then the work: the call zeroes everything from out0 on, and the
+    sk0 = out0 - n * ssz                                 # skew records come back with the results in one copy
+    n_out = n * rsz + 12 * sum(d[4] for d in dims)
+    work0 = out0 + -(-n_out // 16) * 16
+    per = [-(-(8 * (d[7] if d[7] > 1 else 0) + 4 * 256 + lsz + 4 * d[5] * -(-d[6] // 32) + 2 * 12 * d[4] + 3 * 4 * d[4]
+                + 4 * (d[7] * d[8] if d[7] > 1 else 0)) // 16) * 16 for d in dims]
+    buf = torch.empty(work0 + sum(per), dtype=torch.uint8, device=dev)
+    base = buf.data_ptr()
+    leaves, w, blocks, srecs, recs, views, tiles = base + out0 + n * rsz, base + work0, [], [], [], [], 0
+    for i, (pg, d, nb) in enumerate(zip(pages, dims, per)):
+        img, _, vertical, polarity, gap_x, gap_y = pg[:6]
+        x0, y0, bw, bh, cap, L, M, n_ang, stride, t = d
+        wp = -(-M // 32)
+        sc = w
+        hist = sc + 8 * (n_ang if n_ang > 1 else 0)
+        lines, bits = hist + 4 * 256, hist + 4 * 256 + lsz
+        lists = bits + 4 * L * wp
+        counts = lists + 2 * 12 * cap
+        prof = counts + 3 * 4 * cap
+        tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, 0, 0, 0, 0, hist, 0, 0, lines)
+        blocks.append(tb)
+        srecs.append(_lib.SkewBlock(tb, base + tab0 + 16 * t, sc if n_ang > 1 else 0, prof if n_ang > 1 else 0, n_ang, stride,
+                                    0, 0, 0, 0, 0.0, 0.0, 0.0, 0.0))
+        recs.append(_lib.TextPage(tb, bits, (ctypes.c_void_p * 2)(lists, lists + 12 * cap), leaves, counts, counts + 4 * cap,
+                                  counts + 8 * cap, base + out0 + i * rsz, wp, cap, gap_x or 0, gap_y or 0))
+        views.append(buf[sc - base:sc - base + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
+        leaves += 12 * cap
+        w += nb
+        tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
+    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.TextPage * n)(*recs)) + \
+        np.array([v for t in tables for p in t for v in p], np.float64).tobytes()
+    host += bytes(sk0 - len(host)) + bytes((_lib.SkewBlock * n)(*srecs))
+    buf[:out0].copy_(torch.from_numpy(np.frombuffer(host, dtype=np.uint8).copy()))
+    _lib.check(_lib.load().mn_find_blocks_skewed_u8(ctypes.c_void_p(base), ctypes.c_void_p(base + sk0), ctypes.c_void_p(base + pg0),
+                                                    n, tiles, ctypes.c_void_p(base + out0), work0 + sum(per) - out0, _stream()),
+               "mn_find_blocks_skewed_u8")
+    LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS
+    res = buf[sk0:out0 + n_out], [d[4] for d in dims]
+    return res + (views,) if want_scores else res
 
 
 def page_result_dtype():

@@ -1540,7 +1540,9 @@ class TextBlock(NamedTuple):
     minority side of the Otsu threshold is ink), "dark" or "light".  find_lines splits it into lines; restore_regions restores
     each line in its place.  ``skew`` (DESIGN.md 7b, "Skewed blocks"): None (level lines), a given angle in degrees with
     |skew| < 45, counter-clockwise on screen as OrientedRegion.from_rotated's, or "auto": the angle is searched on the device
-    within +-``max_skew`` degrees (in (0, 20], only with "auto") and the lines are OrientedRegions of that angle."""
+    within +-``max_skew`` degrees (in (0, 20], only with "auto") and the lines are OrientedRegions of that angle.
+    ``window`` (DESIGN.md 7b, "Skewed pages"; only with a given angle): an integer rectangle (c0, l0, c1, l1) of frame cells at
+    that angle; the block is then the pixels of ``rect`` whose cell lies in it.  find_blocks gives a tilted page's blocks so."""
     rect: object
     direction: str = "horizontal"
     min_ink: object = None
@@ -1549,6 +1551,7 @@ class TextBlock(NamedTuple):
     polarity: str = "auto"
     skew: object = None
     max_skew: float = 10.0
+    window: object = None
 
 
 _INK = {"auto": 0, "dark": 1, "light": 2}
@@ -1594,6 +1597,19 @@ def _check_block(blk, H, W, name):
         if len(table) > 1 and len(table) * stride > ops.SKEW_MAX_PROFILE:
             raise ValueError(f"{name}: the angle search needs {len(table)} angles x {stride} bins, over the "
                              f"{ops.SKEW_MAX_PROFILE} profile values a block may use (narrow max_skew or split the block)")
+    if blk.window is not None:
+        if sk is None or auto:
+            raise ValueError(f"{name}: a window is given, but skew is {sk!r}, not a given angle")
+        try:
+            c0, l0, c1, l1 = blk.window
+            if not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) for v in (c0, l0, c1, l1)):
+                raise ValueError
+        except (TypeError, ValueError):
+            raise ValueError(f"{name}: a window is four integers (c0, l0, c1, l1), got {blk.window!r}") from None
+        _, _, L, M = ops.skew_frames(x1 - x0, y1 - y0, vertical, ops.skew_cos_sin(table))
+        if not (0 <= c0 < c1 <= int(M[0]) and 0 <= l0 < l1 <= int(L[0])):
+            raise ValueError(f"{name}: window {(c0, l0, c1, l1)} is empty or outside the {int(M[0])}x{int(L[0])} frame of the "
+                             f"block at skew {sk!r}")
     return x0, y0, x1, y1
 
 
@@ -1602,31 +1618,60 @@ def _find_lines(dimg, items):
     copy and one synchronisation.  Returns per item dict(lines, threshold, ink), or the error message of a block with too many
     lines."""
     from . import ops
-    recs = ops.find_lines([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap, blk.min_height,
-                            blk.skew, blk.max_skew) for i, blk, rect in items])
-    host = _to_host(recs).numpy()
-    n_osz = len(items) * ops.block_lines_dtype().itemsize
-    table = host[:n_osz].view(ops.block_lines_dtype())
-    skew = host[n_osz:].view(ops.skew_block_dtype()) if len(host) > n_osz else [None] * len(items)
+    plain = [it for it in items if it[1].window is None]
+    wins = [it for it in items if it[1].window is not None]
+    parts = []
+    if plain:
+        parts.append(ops.find_lines([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap,
+                                      blk.min_height, blk.skew, blk.max_skew) for i, blk, rect in plain]))
+    if wins:
+        parts.append(ops.find_lines_window([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap,
+                                             blk.min_height, blk.skew, blk.window) for i, blk, rect in wins]))
+    host = _to_host(torch.cat(parts) if len(parts) > 1 else parts[0]).numpy()
+    ldt = ops.block_lines_dtype()
+    n_osz, n_wsz = len(plain) * ldt.itemsize, len(wins) * ldt.itemsize
+    table = host[:n_osz].view(ldt)
+    skew = host[n_osz:len(host) - n_wsz].view(ops.skew_block_dtype()) if len(host) > n_osz + n_wsz else [None] * len(plain)
+    found = dict(zip(map(id, plain), zip(table, skew)))
+    found.update((id(it), (t, None)) for it, t in zip(wins, host[len(host) - n_wsz:].view(ldt)))
     out = []
-    for (i, blk, rect), t, sk in zip(items, table, skew):
+    for it in items:
+        (i, blk, rect), (t, sk) = it, found[id(it)]
         n = int(t["n_lines"])
         if n < 0:
             out.append(f"{-n} lines exceed the {ops._lib.BLOCK_MAX_LINES} a text block may hold")
             continue
         lines = [tuple(int(v) for v in q) for q in t["rect"][:n]]
         vertical = blk.direction == "vertical"
-        if blk.skew is not None and sk["s"] != 0:
+        if blk.window is not None:
+            lines, sk = _window_lines(rect, vertical, blk.skew, blk.window, lines), None
+        elif blk.skew is not None and sk["s"] != 0:
             lines = skew_lines(rect, vertical, float(sk["c"]), float(sk["s"]), float(sk["u_min"]), float(sk["v_min"]), lines)
         elif vertical:
             lines = [VerticalRegion(q) for q in lines]
         res = dict(lines=lines, threshold=int(t["threshold"]), ink="dark" if t["ink"] == ops._lib.INK_DARK else "light")
         if blk.skew is not None:
             table_angles = ops.skew_table(blk.skew, blk.max_skew, vertical)
-            angle = table_angles[int(sk["chosen"])]
+            angle = table_angles[int(sk["chosen"])] if sk is not None else table_angles[0]
             res["skew"] = float(blk.skew) if not isinstance(blk.skew, str) else 0.0 - angle if vertical else angle
         out.append(res)
     return out
+
+
+def _window_lines(rect, vertical, skew, window, cells):
+    """The lines of a windowed block from its line table in window cells: offset by (c0, l0) into the block frame, then the
+    rectangles of skew 0 (VerticalRegions, right to left, for a vertical block) or skew_lines with the whole rect's frame."""
+    from . import ops
+    x0, y0, x1, y1 = rect
+    c0, l0 = window[0], window[1]
+    lines = [(c0 + a, l0 + b, c0 + e, l0 + f) for a, b, e, f in cells]
+    (c, s), = ops.skew_cos_sin(ops.skew_table(skew, 10.0, vertical))
+    if s != 0:
+        u_min, v_min, _, _ = (float(a[0]) for a in ops.skew_frames(x1 - x0, y1 - y0, vertical, [(c, s)]))
+        return skew_lines(rect, vertical, c, s, u_min, v_min, lines)
+    if vertical:
+        return [VerticalRegion((x0 + b, y0 + a, x0 + f, y0 + e)) for a, b, e, f in lines][::-1]
+    return [(x0 + a, y0 + b, x0 + e, y0 + f) for a, b, e, f in lines]
 
 
 def skew_lines(rect, vertical, c, s, u_min, v_min, frame_lines):
@@ -1777,12 +1822,15 @@ class TextPage(NamedTuple):
     ``rect``: None (the whole image) or an integer rectangle (x0, y0, x1, y1), as a TextBlock's.  ``direction``: "horizontal"
     (lines read left to right, blocks top to bottom) or "vertical" (columns read top to bottom, blocks right to left).
     ``polarity``: as a TextBlock's.  ``gap_x``, ``gap_y``: positive integers in place of the default cut thresholds.
-    find_blocks returns its blocks; restore_regions replaces it by them, and each of them by its lines."""
+    find_blocks returns its blocks; restore_regions replaces it by them, and each of them by its lines.  ``skew``, ``max_skew``
+    (DESIGN.md 7b, "Skewed pages"): as a TextBlock's; a tilted page's blocks are found in its rotated frame."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
     gap_x: object = None
     gap_y: object = None
+    skew: object = None
+    max_skew: float = 10.0
 
 
 def _check_page(pg, H, W, name):
@@ -1797,20 +1845,40 @@ def _check_page(pg, H, W, name):
             raise ValueError
     except (TypeError, ValueError):
         raise ValueError(f"{name}: a text page is None or an integer rectangle (x0, y0, x1, y1), got {pg.rect!r}") from None
-    _check_block(TextBlock((x0, y0, x1, y1), pg.direction, polarity=pg.polarity), H, W, name)
+    _check_block(TextBlock((x0, y0, x1, y1), pg.direction, polarity=pg.polarity, skew=pg.skew, max_skew=pg.max_skew), H, W, name)
     for what in ("gap_x", "gap_y"):
         v = getattr(pg, what)
         if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 1 <= v < 2 ** 31):
             raise ValueError(f"{name}: {what} must be a positive integer, got {v!r}")
-    if ops.page_bytes(x1 - x0, y1 - y0) > ops.PAGE_MAX_WORK:
+    if pg.skew is not None:
+        L, M, _ = ops.skew_page_frame(x1 - x0, y1 - y0, pg.direction == "vertical", _page_table(pg))
+        if max(L, M) > 32767:
+            raise ValueError(f"{name}: a side of the page's rotated frame reaches {max(L, M)} pixels, over 32767")
+    if _page_bytes(pg, (x0, y0, x1, y1), pg.skew is not None) > ops.PAGE_MAX_WORK:
         raise ValueError(f"{name}: the page needs more than the {ops.PAGE_MAX_WORK} bytes of work memory a call may use")
     return x0, y0, x1, y1
+
+
+def _page_table(pg):
+    """The (c, s) table of a skewed page's search."""
+    from . import ops
+    return ops.skew_cos_sin(ops.skew_table(pg.skew, pg.max_skew, pg.direction == "vertical"))
+
+
+def _page_bytes(pg, rect, skewed):
+    """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages."""
+    from . import ops
+    w, h = rect[2] - rect[0], rect[3] - rect[1]
+    if not skewed:
+        return ops.page_bytes(w, h)
+    return ops.skew_page_bytes(w, h, pg.direction == "vertical", _page_table(pg) if pg.skew is not None else [(1.0, 0.0)])
 
 
 def _check_page_work(items):
     """Refuse, before any launch, a call whose pages (image index, TextPage, rect) need more work memory than a call may use."""
     from . import ops
-    if sum(ops.page_bytes(r[2] - r[0], r[3] - r[1]) for _, _, r in items) > ops.PAGE_MAX_WORK:
+    skewed = any(pg.skew is not None for _, pg, _ in items)
+    if sum(_page_bytes(pg, r, skewed) for _, pg, r in items) > ops.PAGE_MAX_WORK:
         raise ValueError(f"the call's {len(items)} text pages need more than the {ops.PAGE_MAX_WORK} bytes of work memory a call "
                          f"may use (split the call)")
 
@@ -1821,13 +1889,16 @@ def _find_blocks(dimg, items):
     the error message of a page over a limit."""
     from . import ops
     lib = ops._lib
-    res_t, caps = ops.find_blocks([(dimg[i], rect, pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y)
-                                   for i, pg, rect in items])
+    res_t, caps = ops.find_blocks([(dimg[i], rect, pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y, pg.skew,
+                                    pg.max_skew) for i, pg, rect in items])
     host = _to_host(res_t).numpy()
-    rdt, ndt = ops.page_result_dtype(), ops.page_node_dtype()
-    res = host[:len(items) * rdt.itemsize].view(rdt)
-    o, out = len(items) * rdt.itemsize, []
-    for (i, pg, rect), r, cap in zip(items, res, caps):
+    rdt, ndt, sdt = ops.page_result_dtype(), ops.page_node_dtype(), ops.skew_block_dtype()
+    skewed = any(pg.skew is not None for _, pg, _ in items)
+    o = len(items) * sdt.itemsize if skewed else 0
+    skew = host[:o].view(sdt) if skewed else [None] * len(items)
+    res = host[o:o + len(items) * rdt.itemsize].view(rdt)
+    o, out = o + len(items) * rdt.itemsize, []
+    for (i, pg, rect), r, cap, sk in zip(items, res, caps, skew):
         leaves = host[o:o + cap * ndt.itemsize].view(ndt)[:int(r["n_leaves"])]
         o += cap * ndt.itemsize
         if r["error"] == lib.PAGE_ERR_NODES:
@@ -1837,13 +1908,27 @@ def _find_blocks(dimg, items):
             out.append(f"{int(r['n_blocks'])} blocks exceed the {lib.PAGE_MAX_BLOCKS} a text page may hold")
             continue
         X0, Y0 = rect[:2]
+        vertical = pg.direction == "vertical"
+        tilted = pg.skew is not None and sk["s"] != 0
         blocks, rejected = [], []
         for q in leaves:
-            box = (X0 + int(q["x0"]), Y0 + int(q["y0"]), X0 + int(q["x1"]), Y0 + int(q["y1"]))
+            x0, y0, x1, y1 = (int(q[f]) for f in ("x0", "y0", "x1", "y1"))
+            if not tilted:
+                box = (X0 + x0, Y0 + y0, X0 + x1, Y0 + y1)
+            else:                                       # a window of the block frame: a vertical page's bitmap is its transpose
+                box = (y0, x0, y1, x1) if vertical else (x0, y0, x1, y1)
             (rejected if q["st"] & lib.PAGE_REJECTED else blocks).append(box)
-        out.append(dict(blocks=[TextBlock(b, pg.direction, polarity=pg.polarity) for b in blocks], rejected=rejected,
-                        threshold=int(r["threshold"]), ink="dark" if r["ink"] == lib.INK_DARK else "light",
-                        text_size=int(r["text_size"]), gap_x=int(r["gap_x"]), gap_y=int(r["gap_y"])))
+        res = dict(threshold=int(r["threshold"]), ink="dark" if r["ink"] == lib.INK_DARK else "light",
+                   text_size=int(r["text_size"]), gap_x=int(r["gap_x"]), gap_y=int(r["gap_y"]))
+        if pg.skew is None:
+            res.update(blocks=[TextBlock(b, pg.direction, polarity=pg.polarity) for b in blocks], rejected=rejected)
+        else:
+            angle = ops.skew_table(pg.skew, pg.max_skew, vertical)[int(sk["chosen"])]
+            res["skew"] = float(pg.skew) if not isinstance(pg.skew, str) else 0.0 - angle if vertical else angle
+            res["blocks"] = [TextBlock(tuple(rect), pg.direction, polarity=pg.polarity, skew=res["skew"], window=b) if tilted
+                             else TextBlock(b, pg.direction, polarity=pg.polarity) for b in blocks]
+            res["rejected"] = rejected
+        out.append(dict(blocks=res.pop("blocks"), rejected=res.pop("rejected"), **res))
     return out
 
 
@@ -1859,7 +1944,11 @@ def find_blocks(images, pages):
     polarity, each one a region restore_regions takes; rejected, the rectangles of leaves that are not text; threshold and ink
     as find_lines'; text_size S; gap_x and gap_y, the thresholds used (all three 0 when the page has no text).  Raises
     ValueError naming the image and the page, before any launch, for a page restore_regions would reject, and after the
-    XY-cut for a page over its node or block limit."""
+    XY-cut for a page over its node or block limit.
+    A page with ``skew`` (DESIGN.md 7b, "Skewed pages") has its angle searched (or given) on the device and is cut in its
+    rotated frame; a call that holds one runs every page through ops.find_blocks' 151 launches.  Its dict gains ``skew``, the
+    angle used, and its blocks (and rejected leaves) are windows of that frame, TextBlock(page rect, skew=angle, window=...),
+    or the blocks of skew=None when the angle is exactly 0."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
@@ -2168,7 +2257,8 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     A TextPage (DESIGN.md 7b, "Text pages") is split into blocks on the uploaded images first (find_blocks: every page of the
     call in the same launches, one pinned copy and one synchronisation), its TextBlocks take its place, and each of them is then
     replaced by its lines as above, so the result is byte for byte that of the call given the found blocks.  No labels or boxes
-    may be given for a page.  Its entry is dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y, regions), regions one
+    may be given for a page; a tilted page (``skew``) gives windowed TextBlocks, which are split as any other.  Its entry is
+    dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, skew], regions), regions one
     block entry per block; a page over its node or block limit, or one of whose blocks fails, raises, or is dict(error=...)
     with ``skip_invalid``, and then none of its blocks is restored."""
     from . import ops

@@ -1,6 +1,6 @@
 """Text pages (DESIGN.md section 7b, "Text pages"): the layout analysis alone and restore_regions with pages.
 
-    MN_MODULE_GRAPHS=0 python tools/bench_pages.py [--pages 4] [--passes 3] [--iters 100] [--scale 2]
+    MN_MODULE_GRAPHS=0 python tools/bench_pages.py [--pages 4] [--passes 3] [--iters 100] [--scale 2] [--skew]
 
 The pages are seeded 1600 x 1200 pages: a heading over two or three columns of capital-letter lines drawn with cv2.putText
 (Hershey DUPLEX) on a light, slightly noisy background, one TextPage each.  Prints one JSON line each for:
@@ -8,6 +8,9 @@ The pages are seeded 1600 x 1200 pages: a heading over two or three columns of c
     CUDA events over --iters calls, per call and per page;
   - restore_regions with the pages against the same call given the found blocks, host uint8 in and out, pages/s; the arms
     alternate pass by pass and must give the same bytes.
+With --skew (DESIGN.md section 7b, "Skewed pages") the pages are turned by seeded angles within +-7.5 degrees and searched with
+TextPage(skew="auto"): the layout line times mn_find_blocks_skewed_u8 against the level pages in the same run, and the
+restore_regions arms are the tilted pages against the call given the found lines.
 Every line carries the card's name and power limit, read in the same run.  Not part of the product path.
 """
 import argparse
@@ -68,6 +71,7 @@ def main():
     ap.add_argument("--passes", type=int, default=3)
     ap.add_argument("--iters", type=int, default=100)
     ap.add_argument("--scale", type=int, default=2)
+    ap.add_argument("--skew", action="store_true")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_pages.py needs a CUDA device")
@@ -78,21 +82,34 @@ def main():
     card = _card()
     pages, cols = make_pages(args.pages)
 
-    dpages = [torch.from_numpy(p).to(dev) for p in pages]
-    items = [(d, (0, 0, d.shape[1], d.shape[0]), False, _lib.INK_AUTO, None, None) for d in dpages]
-    for _ in range(5):
-        ops.find_blocks(items)
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0.record()
-    for _ in range(args.iters):
-        ops.find_blocks(items)
-    t1.record()
-    t1.synchronize()
-    ms = t0.elapsed_time(t1) / args.iters
-    found = pipeline.find_blocks(pages, [[pipeline.TextPage()] for _ in pages])
+    level = pages
+    angles = [round(float(a), 2) for a in np.random.default_rng(1).uniform(-7.5, 7.5, len(pages))] if args.skew else None
+    if args.skew:
+        pages = [cv2.warpAffine(p, cv2.getRotationMatrix2D((p.shape[1] / 2, p.shape[0] / 2), a, 1.0), (p.shape[1], p.shape[0]),
+                                flags=cv2.INTER_LINEAR, borderMode=cv2.BORDER_REPLICATE) for p, a in zip(pages, angles)]
+    page = pipeline.TextPage(skew="auto") if args.skew else pipeline.TextPage()
+
+    def layout_ms(imgs, skew):
+        d = [torch.from_numpy(p).to(dev) for p in imgs]
+        items = [(x, (0, 0, x.shape[1], x.shape[0]), False, _lib.INK_AUTO, None, None, skew) for x in d]
+        for _ in range(5):
+            ops.find_blocks(items)
+        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0.record()
+        for _ in range(args.iters):
+            ops.find_blocks(items)
+        t1.record()
+        t1.synchronize()
+        return t0.elapsed_time(t1) / args.iters
+
+    ms = layout_ms(pages, "auto" if args.skew else None)
+    found = pipeline.find_blocks(pages, [[page] for _ in pages])
+    extra = {}
+    if args.skew:
+        extra = dict(angles=angles, found=[f[0]["skew"] for f in found], level_ms_per_call=round(layout_ms(level, None), 4))
     print(json.dumps(dict(card, what="layout", pages=len(pages), megapixels=sum(p.shape[0] * p.shape[1] for p in pages) / 1e6,
                           columns=cols, blocks=[len(f[0]["blocks"]) for f in found], text_size=[f[0]["text_size"] for f in found],
-                          ms_per_call=round(ms, 4), ms_per_page=round(ms / len(pages), 4))), flush=True)
+                          ms_per_call=round(ms, 4), ms_per_page=round(ms / len(pages), 4), **extra)), flush=True)
 
     sds = synth.make_checkpoints(0)
     m = []
@@ -102,8 +119,12 @@ def main():
         m.append(net.eval().to(dev))
     blocks = [f[0]["blocks"] for f in found]
     kw = dict(scale=args.scale, skip_invalid=True, to_host=True)
-    arms = {"pages": lambda: pipeline.restore_regions(*m, pages, [[pipeline.TextPage()] for _ in pages], **kw),
-            "found blocks": lambda: pipeline.restore_regions(*m, pages, blocks, **kw)}
+    if args.skew:
+        lines = [[q for r in f for q in r["lines"]] for f in pipeline.find_lines(pages, blocks)]
+        base = ("found lines", lambda: pipeline.restore_regions(*m, pages, lines, **kw))
+    else:
+        base = ("found blocks", lambda: pipeline.restore_regions(*m, pages, blocks, **kw))
+    arms = {"pages": lambda: pipeline.restore_regions(*m, pages, [[page] for _ in pages], **kw), base[0]: base[1]}
     outs = {name: fn() for name, fn in arms.items()}          # warm-up of every shape
     times = {name: [] for name in arms}
     for _ in range(args.passes):
@@ -112,9 +133,9 @@ def main():
             t = time.perf_counter()
             outs[name] = fn()
             times[name].append(time.perf_counter() - t)
-    for a, b in zip(outs["pages"], outs["found blocks"]):
+    for a, b in zip(outs["pages"], outs[base[0]]):
         assert np.array_equal(a["image"], b["image"]), "the arms differ"
-    n_lines = sum(len(e["lines"]) for f in outs["found blocks"] for e in f["regions"] if "lines" in e)
+    n_lines = sum(len(e["lines"]) for f in outs["pages"] for p in f["regions"] for e in p.get("regions", []) if "lines" in e)
     for name, ts in times.items():
         med = float(np.median(ts))
         print(json.dumps(dict(card, what=f"restore_regions with {name}", pages=len(pages), lines=n_lines, scale=args.scale,
