@@ -1067,6 +1067,16 @@ int page_levels(mn_text_page* pages, int n, cudaStream_t st) {
     return MN_OK;
 }
 
+// 1-2 of every text-block entry: the zeroed work, then each crop's histogram and Otsu threshold.
+int block_threshold(const mn_text_block* blocks, int n, long long max_tiles, void* work, long long work_bytes, cudaStream_t st) {
+    MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
+    MN_CUDA_CHECK((mn_launch(block_hist_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, blocks)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(block_threshold_kernel, dim3(mn_cdiv(n, 128)), dim3(128), 0, st, blocks, n)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
 }  // namespace
 
 extern "C" int mn_find_lines_u8(const mn_text_block* blocks, int n, long long max_tiles, void* work, long long work_bytes,
@@ -1074,11 +1084,8 @@ extern "C" int mn_find_lines_u8(const mn_text_block* blocks, int n, long long ma
     MN_REQUIRE(blocks && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
                "mn_find_lines_u8: bad args");
     cudaStream_t st = (cudaStream_t)stream;
-    MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
-    MN_CUDA_CHECK((mn_launch(block_hist_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, blocks)));
-    MN_LAUNCH_CHECK();
-    MN_CUDA_CHECK((mn_launch(block_threshold_kernel, dim3(mn_cdiv(n, 128)), dim3(128), 0, st, blocks, n)));
-    MN_LAUNCH_CHECK();
+    const int rc = block_threshold(blocks, n, max_tiles, work, work_bytes, st);
+    if (rc != MN_OK) return rc;
     MN_CUDA_CHECK((mn_launch(block_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, blocks)));
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(block_lines_kernel, dim3(n), dim3(kSegThreads), 0, st, blocks)));
@@ -1091,20 +1098,15 @@ extern "C" int mn_find_lines_skewed_u8(mn_text_block* blocks, mn_skew_block* ske
     MN_REQUIRE(blocks && skew && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
                "mn_find_lines_skewed_u8: bad args");
     cudaStream_t st = (cudaStream_t)stream;
-    const mn_text_block* cblocks = blocks;
-    const mn_skew_block* cskew = skew;
-    MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
-    MN_CUDA_CHECK((mn_launch(block_hist_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cblocks)));
-    MN_LAUNCH_CHECK();
-    MN_CUDA_CHECK((mn_launch(block_threshold_kernel, dim3(mn_cdiv(n, 128)), dim3(128), 0, st, cblocks, n)));
-    MN_LAUNCH_CHECK();
-    MN_CUDA_CHECK((mn_launch(skew_angle_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cskew)));
+    const int rc = block_threshold(blocks, n, max_tiles, work, work_bytes, st);
+    if (rc != MN_OK) return rc;
+    MN_CUDA_CHECK((mn_launch(skew_angle_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, skew)));
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(skew_score_kernel, dim3(n), dim3(kScoreThreads), 0, st, blocks, skew)));
     MN_LAUNCH_CHECK();
-    MN_CUDA_CHECK((mn_launch(skew_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cskew)));
+    MN_CUDA_CHECK((mn_launch(skew_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, skew)));
     MN_LAUNCH_CHECK();
-    MN_CUDA_CHECK((mn_launch(block_lines_kernel, dim3(n), dim3(kSegThreads), 0, st, cblocks)));
+    MN_CUDA_CHECK((mn_launch(block_lines_kernel, dim3(n), dim3(kSegThreads), 0, st, blocks)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }
@@ -1114,11 +1116,8 @@ extern "C" int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* page
     MN_REQUIRE(blocks && pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
                "mn_find_blocks_u8: bad args");
     cudaStream_t st = (cudaStream_t)stream;
-    MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
-    MN_CUDA_CHECK((mn_launch(block_hist_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, blocks)));
-    MN_LAUNCH_CHECK();
-    MN_CUDA_CHECK((mn_launch(block_threshold_kernel, dim3(mn_cdiv(n, 128)), dim3(128), 0, st, blocks, n)));
-    MN_LAUNCH_CHECK();
+    const int rc = block_threshold(blocks, n, max_tiles, work, work_bytes, st);
+    if (rc != MN_OK) return rc;
     MN_CUDA_CHECK((mn_launch(page_bits_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, pages)));
     MN_LAUNCH_CHECK();
     return page_levels(pages, n, st);
@@ -1129,18 +1128,13 @@ extern "C" int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* sk
     MN_REQUIRE(blocks && skew && pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
                "mn_find_blocks_skewed_u8: bad args");
     cudaStream_t st = (cudaStream_t)stream;
-    const mn_text_block* cblocks = blocks;
-    const mn_skew_block* cskew = skew;
-    MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
-    MN_CUDA_CHECK((mn_launch(block_hist_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cblocks)));
-    MN_LAUNCH_CHECK();
-    MN_CUDA_CHECK((mn_launch(block_threshold_kernel, dim3(mn_cdiv(n, 128)), dim3(128), 0, st, cblocks, n)));
-    MN_LAUNCH_CHECK();
-    MN_CUDA_CHECK((mn_launch(skew_angle_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, cskew)));
+    const int rc = block_threshold(blocks, n, max_tiles, work, work_bytes, st);
+    if (rc != MN_OK) return rc;
+    MN_CUDA_CHECK((mn_launch(skew_angle_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, skew)));
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(skew_score_kernel, dim3(n), dim3(kScoreThreads), 0, st, blocks, skew)));
     MN_LAUNCH_CHECK();
-    MN_CUDA_CHECK((mn_launch(page_frame_bits_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, pages, cskew)));
+    MN_CUDA_CHECK((mn_launch(page_frame_bits_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, pages, skew)));
     MN_LAUNCH_CHECK();
     return page_levels(pages, n, st);
 }

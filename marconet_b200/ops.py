@@ -1621,6 +1621,71 @@ def skew_block_dtype():
                      ("u_min", "<f8"), ("v_min", "<f8"), ("c", "<f8"), ("s", "<f8")])
 
 
+def _check_items(items, what, noun):
+    """The device of a layout call's items, after checking their number (one launch holds 1 to 65535)."""
+    if not items:
+        raise ValueError(f"{what}: no {noun}s")
+    if len(items) > 65535:
+        raise ValueError(f"{what}: at most 65535 {noun}s per launch")
+    return items[0][0].device
+
+
+def _check_crop(item, dev, what, knob_names):
+    """(x0, y0, w, h) of a layout item (img, rect, vertical, polarity, *knobs), validated as find_lines and find_blocks describe
+    it.  Raises naming ``what``."""
+    img, rect, _, polarity, *knobs = item
+    _dense_u8(img, dev, 3, f"{what}: img")
+    x0, y0, x1, y1 = (int(v) for v in rect)
+    if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
+        raise ValueError(f"{what}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
+                         f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
+    if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or any(v is not None and not 1 <= v < 2 ** 31 for v in knobs):
+        raise ValueError(f"{what}: bad polarity {polarity!r} or {knob_names} {knobs!r}")
+    return x0, y0, x1 - x0, y1 - y0
+
+
+def _check_skew(skew, max_skew, vertical, what):
+    """The (c, s) table of skew / max_skew (find_lines' rules), or ValueError naming ``what``."""
+    if skew is None:
+        return [(1.0, 0.0)]
+    if not (skew == "auto" if isinstance(skew, str) else math.isfinite(skew) and abs(skew) < 45):
+        raise ValueError(f"{what}: bad skew {skew!r}")
+    if not (isinstance(skew, str) or max_skew == 10.0) or not 0 < max_skew <= 20:
+        raise ValueError(f"{what}: max_skew {max_skew!r} is outside (0, 20] or given without 'auto'")
+    return skew_cos_sin(skew_table(skew, max_skew, vertical))
+
+
+def _angle_tables(tables):
+    """The fp64 (c, s) bytes of the distinct tables among ``tables``, and the offset of each one in (c, s) entries."""
+    import numpy as np
+    keys, offs, n = {}, [], 0
+    for cs in tables:
+        key = tuple(cs)
+        if key not in keys:
+            keys[key], n = n, n + len(cs)
+        offs.append(keys[key])
+    return np.array([v for key in keys for p in key for v in p], np.float64).tobytes(), offs
+
+
+def _skew_block(tb, table, scores, profiles, n_ang, stride):
+    """The mn_skew_block record of the crop ``tb`` over the n_ang (c, s) at ``table``; only a search (n_ang > 1) has per-angle
+    scores and profiles."""
+    return _lib.SkewBlock(tb, table, scores if n_ang > 1 else 0, profiles if n_ang > 1 else 0, n_ang, stride)
+
+
+def _line_areas(sizes):
+    """The int32 areas of the line kernels for blocks of ``sizes`` (L bins, extra values) each: every block's work (a 256-bin
+    histogram, 3 L profile values, then the extra values), which the call zeroes, followed by every block's scratch of 2 L + 4
+    values.  Returns per block the byte offsets (hist, prof, scratch), the bytes of the work and those of the whole."""
+    n_work = sum(256 + 3 * L + e for L, e in sizes)
+    out, w, s = [], 0, n_work
+    for L, e in sizes:
+        out.append((4 * w, 4 * (w + 256), 4 * s))
+        w += 256 + 3 * L + e
+        s += 2 * L + 4
+    return out, 4 * n_work, 4 * s
+
+
 def find_lines(blocks, scores=False):
     """Text blocks split into lines, every block in four launches whatever their number (mn_find_lines_u8; DESIGN.md 7b, "Text
     blocks").  blocks: list of (img, rect, vertical, polarity, min_ink, gap, min_height[, skew, max_skew]): img a uint8 [H, W, 3]
@@ -1630,119 +1695,57 @@ def find_lines(blocks, scores=False):
     ``block_lines_dtype()``).
     skew (DESIGN.md 7b, "Skewed blocks"): None, "auto" (search +-max_skew degrees) or a given angle in degrees, |skew| < 45.  A
     call with any skewed block goes through mn_find_lines_skewed_u8's six launches instead, every block of it, whatever their
-    number; blocks with skew None keep their mn_block_lines records exactly.  The tensor then holds the n mn_block_lines records
-    followed by the n mn_skew_block records (``skew_block_dtype()``: the chosen index and frame).  ``scores`` (tests): also
-    return, per block, the int64 CUDA view of its per-angle scores (None unless it searched)."""
-    import numpy as np
+    number; blocks with skew None search the one-entry table (1, 0), which keeps their mn_block_lines records exactly.  The
+    tensor then holds the n mn_block_lines records followed by the n mn_skew_block records (``skew_block_dtype()``: the chosen
+    index and frame).  ``scores`` (tests): also return, per block, the int64 CUDA view of its per-angle scores (None unless it
+    searched)."""
     global LAUNCHES
-    if not blocks:
-        raise ValueError("find_lines: no blocks")
-    if len(blocks) > 65535:
-        raise ValueError("find_lines: at most 65535 blocks per launch")
-    if any(len(b) > 7 and b[7] is not None for b in blocks):
-        return _find_lines_skewed(blocks, scores)
-    blocks = [b[:7] for b in blocks]
-    dev = blocks[0][0].device
-    osz, rsz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.TextBlock)
-    dims = []
-    for i, (img, rect, vertical, polarity, *knobs) in enumerate(blocks):
-        _dense_u8(img, dev, 3, f"find_lines: block {i}: img")
-        x0, y0, x1, y1 = (int(v) for v in rect)
-        if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
-            raise ValueError(f"find_lines: block {i}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
-                             f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
-        if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or \
-                any(v is not None and not 1 <= v < 2 ** 31 for v in knobs):
-            raise ValueError(f"find_lines: block {i}: bad polarity {polarity!r} or min_ink / gap / min_height {knobs!r}")
-        dims.append((x0, y0, x1 - x0, y1 - y0, y1 - y0 if not vertical else x1 - x0))
-    n_work = sum(256 + 3 * d[4] for d in dims)
-    n_scratch = sum(2 * d[4] + 4 for d in dims)
-    head = len(blocks) * (osz + rsz)
-    buf = torch.empty(head + 4 * (n_work + n_scratch), dtype=torch.uint8, device=dev)
-    out, work = buf.data_ptr(), buf.data_ptr() + head
-    scratch, w, s, recs, tiles = work + 4 * n_work, 0, 0, [], 0
-    for i, ((img, _, vertical, polarity, min_ink, gap, min_height), (x0, y0, bw, bh, L)) in enumerate(zip(blocks, dims)):
-        recs.append(_lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, min_ink or 0,
-                                   gap or 0, min_height or 0, 0, work + 4 * w, work + 4 * (w + 256), scratch + 4 * s, out + i * osz))
-        w += 256 + 3 * L
-        s += 2 * L + 4
-        tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
-    rec = buf[len(blocks) * osz:head]
-    rec.copy_(torch.from_numpy(np.frombuffer(bytes((_lib.TextBlock * len(recs))(*recs)), dtype=np.uint8).copy()))
-    _lib.check(_lib.load().mn_find_lines_u8(_ptr(rec), len(recs), tiles, work, 4 * n_work, _stream()), "mn_find_lines_u8")
-    LAUNCHES += 4
-    out = buf[:len(blocks) * osz]
-    return (out, [None] * len(blocks)) if scores else out
-
-
-def _find_lines_skewed(blocks, want_scores):
-    """find_lines for a call that holds a skewed block: mn_find_lines_skewed_u8 over every block.  A block without skew searches
-    the one-entry table (1, 0), which leaves its crop record and so its mn_block_lines record as mn_find_lines_u8 writes it."""
-    import numpy as np
-    global LAUNCHES
-    dev = blocks[0][0].device
+    dev = _check_items(blocks, "find_lines", "block")
+    skewed = any(len(b) > 7 and b[7] is not None for b in blocks)
     n = len(blocks)
-    osz, ssz, rsz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.SkewBlock), ctypes.sizeof(_lib.TextBlock)
-    dims, tables, keys = [], [], {}
+    osz, rsz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.TextBlock)
+    ssz = ctypes.sizeof(_lib.SkewBlock) if skewed else 0
+    dims, tables = [], []
     for i, blk in enumerate(blocks):
-        img, rect, vertical, polarity, *knobs = blk[:7]
-        skew, max_skew = blk[7] if len(blk) > 7 else None, blk[8] if len(blk) > 8 else 10.0
-        _dense_u8(img, dev, 3, f"find_lines: block {i}: img")
-        x0, y0, x1, y1 = (int(v) for v in rect)
-        if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
-            raise ValueError(f"find_lines: block {i}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
-                             f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
-        if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or \
-                any(v is not None and not 1 <= v < 2 ** 31 for v in knobs):
-            raise ValueError(f"find_lines: block {i}: bad polarity {polarity!r} or min_ink / gap / min_height {knobs!r}")
-        if skew is None:
-            cs = [(1.0, 0.0)]
-        elif skew == "auto" if isinstance(skew, str) else math.isfinite(skew) and abs(skew) < 45:
-            if not (isinstance(skew, str) or max_skew == 10.0) or not 0 < max_skew <= 20:
-                raise ValueError(f"find_lines: block {i}: max_skew {max_skew!r} is outside (0, 20] or given without 'auto'")
-            cs = skew_cos_sin(skew_table(skew, max_skew, vertical))
-        else:
-            raise ValueError(f"find_lines: block {i}: bad skew {skew!r}")
-        stride = skew_stride(x1 - x0, y1 - y0, vertical, cs)
+        what = f"find_lines: block {i}"
+        x0, y0, bw, bh = _check_crop(blk[:7], dev, what, "min_ink / gap / min_height")
+        vertical, skew, max_skew = blk[2], blk[7] if len(blk) > 7 else None, blk[8] if len(blk) > 8 else 10.0
+        cs = _check_skew(skew, max_skew, vertical, what)
+        stride = (bw if vertical else bh) if skew is None else skew_stride(bw, bh, vertical, cs)
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
-            raise ValueError(f"find_lines: block {i}: {len(cs)} angles x {stride} bins exceed the {SKEW_MAX_PROFILE} profile "
-                             f"values a skewed block may use")
-        key = tuple(cs)
-        if key not in keys:
-            keys[key] = sum(len(t) for t in tables)
-            tables.append(cs)
-        dims.append((x0, y0, x1 - x0, y1 - y0, len(cs), stride, keys[key]))
-    n_tab = sum(len(t) for t in tables)
+            raise ValueError(f"{what}: {len(cs)} angles x {stride} bins exceed the {SKEW_MAX_PROFILE} profile values a skewed "
+                             f"block may use")
+        tables.append(cs)
+        dims.append((x0, y0, bw, bh, len(cs), stride))
+    tab, t_offs = _angle_tables(tables) if skewed else (b"", [0] * n)
     n_scores = sum(d[4] for d in dims if d[4] > 1)
-    n_work = sum(256 + 3 * d[5] + (d[4] * d[5] if d[4] > 1 else 0) for d in dims)
-    n_scratch = sum(2 * d[5] + 4 for d in dims)
-    head = n * (osz + ssz + rsz) + 16 * n_tab
-    buf = torch.empty(head + 8 * n_scores + 4 * (n_work + n_scratch), dtype=torch.uint8, device=dev)
-    out, sk, seg = buf.data_ptr(), buf.data_ptr() + n * osz, buf.data_ptr() + n * (osz + ssz)
-    tab, work = seg + n * rsz, buf.data_ptr() + head
-    w32, scratch = work + 8 * n_scores, work + 8 * n_scores + 4 * n_work
-    recs, srecs, views, w, s, o, tiles = [], [], [], 0, 0, 0, 0
-    for i, (blk, (x0, y0, bw, bh, n_ang, stride, t)) in enumerate(zip(blocks, dims)):
+    areas, n_work, n_areas = _line_areas([(d[5], d[4] * d[5] if d[4] > 1 else 0) for d in dims])
+    head = n * (osz + ssz + rsz) + len(tab)             # results, skew records, crop records, tables; scores; work; scratch
+    buf = torch.empty(head + 8 * n_scores + n_areas, dtype=torch.uint8, device=dev)
+    base = buf.data_ptr()
+    sk, seg, w32 = base + n * osz, base + n * (osz + ssz), base + head + 8 * n_scores
+    recs, srecs, views, o, tiles = [], [], [], 0, 0
+    for i, (blk, (x0, y0, bw, bh, n_ang, stride), (hist, prof, scr), t) in enumerate(zip(blocks, dims, areas, t_offs)):
         img, _, vertical, polarity, min_ink, gap, min_height = blk[:7]
-        prof = w32 + 4 * (w + 256)
         tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, min_ink or 0, gap or 0,
-                            min_height or 0, 0, w32 + 4 * w, prof, scratch + 4 * s, out + i * osz)
+                            min_height or 0, 0, w32 + hist, w32 + prof, w32 + scr, base + i * osz)
         recs.append(tb)
-        srecs.append(_lib.SkewBlock(tb, tab + 16 * t, work + 8 * o if n_ang > 1 else 0, prof + 4 * 3 * stride if n_ang > 1 else 0,
-                                    n_ang, stride, 0, 0, 0, 0, 0.0, 0.0, 0.0, 0.0))
+        if skewed:
+            srecs.append(_skew_block(tb, seg + n * rsz + 16 * t, base + head + 8 * o, w32 + prof + 4 * 3 * stride, n_ang, stride))
         views.append(buf[head + 8 * o:head + 8 * (o + n_ang)].view(torch.int64) if n_ang > 1 else None)
         o += n_ang if n_ang > 1 else 0
-        w += 256 + 3 * stride + (n_ang * stride if n_ang > 1 else 0)
-        s += 2 * stride + 4
         tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
-    host = bytes((_lib.SkewBlock * n)(*srecs)) + bytes((_lib.TextBlock * n)(*recs)) + \
-        np.array([v for t in tables for p in t for v in p], np.float64).tobytes()
-    buf[n * osz:head].copy_(torch.from_numpy(np.frombuffer(host, dtype=np.uint8).copy()))
-    _lib.check(_lib.load().mn_find_lines_skewed_u8(ctypes.c_void_p(seg), ctypes.c_void_p(sk), n, tiles, work,
-                                                   8 * n_scores + 4 * n_work, _stream()), "mn_find_lines_skewed_u8")
-    LAUNCHES += 6
+    host = bytes((_lib.SkewBlock * len(srecs))(*srecs)) + bytes((_lib.TextBlock * n)(*recs)) + tab
+    buf[n * osz:head].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    if skewed:
+        _lib.check(_lib.load().mn_find_lines_skewed_u8(seg, sk, n, tiles, base + head, 8 * n_scores + n_work, _stream()),
+                   "mn_find_lines_skewed_u8")
+        LAUNCHES += 6
+    else:
+        _lib.check(_lib.load().mn_find_lines_u8(seg, n, tiles, base + head, n_work, _stream()), "mn_find_lines_u8")
+        LAUNCHES += 4
     res = buf[:n * (osz + ssz)]
-    return (res, views) if want_scores else res
+    return (res, views) if scores else res
 
 
 def window_footprint(w, h, vertical, c, s, u_min, v_min, window):
@@ -1766,55 +1769,41 @@ def find_lines_window(blocks):
     find_lines', skew a given finite angle and window (c0, l0, c1, l1) a non-empty integer rectangle inside the crop's frame at
     that angle (the transposed crop at the negated angle for a vertical block).  Returns the uint8 CUDA tensor of the blocks'
     mn_block_lines records, in order, whose rectangles are (c0', l0', c1', l1') in cells of the window."""
-    import numpy as np
     global LAUNCHES
-    if not blocks:
-        raise ValueError("find_lines_window: no blocks")
-    if len(blocks) > 65535:
-        raise ValueError("find_lines_window: at most 65535 blocks per launch")
-    dev = blocks[0][0].device
+    dev = _check_items(blocks, "find_lines_window", "block")
     n = len(blocks)
     osz, rsz, wsz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.TextBlock), ctypes.sizeof(_lib.WindowBlock)
     dims = []
-    for i, (img, rect, vertical, polarity, min_ink, gap, min_height, skew, window) in enumerate(blocks):
-        _dense_u8(img, dev, 3, f"find_lines: block {i}: img")
-        x0, y0, x1, y1 = (int(v) for v in rect)
-        if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
-            raise ValueError(f"find_lines: block {i}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
-                             f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
-        if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or \
-                any(v is not None and not 1 <= v < 2 ** 31 for v in (min_ink, gap, min_height)):
-            raise ValueError(f"find_lines: block {i}: bad polarity {polarity!r} or min_ink / gap / min_height")
+    for i, blk in enumerate(blocks):
+        what = f"find_lines: block {i}"
+        img, rect, vertical, polarity, min_ink, gap, min_height, skew, window = blk
+        x0, y0, bw, bh = _check_crop(blk[:7], dev, what, "min_ink / gap / min_height")
         if isinstance(skew, str) or skew is None or not math.isfinite(skew) or abs(skew) >= 45:
-            raise ValueError(f"find_lines: block {i}: a window needs a given finite angle, got skew {skew!r}")
-        (c, s), = skew_cos_sin(skew_table(skew, 10.0, vertical))
-        u_min, v_min, L, M = (float(a[0]) for a in skew_frames(x1 - x0, y1 - y0, vertical, [(c, s)]))
+            raise ValueError(f"{what}: a window needs a given finite angle, got skew {skew!r}")
+        (c, s), = _check_skew(skew, 10.0, vertical, what)
+        u_min, v_min, L, M = (float(a[0]) for a in skew_frames(bw, bh, vertical, [(c, s)]))
         c0, l0, c1, l1 = (int(v) for v in window)
         if not (0 <= c0 < c1 <= M and 0 <= l0 < l1 <= L):
-            raise ValueError(f"find_lines: block {i}: window {(c0, l0, c1, l1)} is empty or outside the {int(M)}x{int(L)} frame")
-        fp = window_footprint(x1 - x0, y1 - y0, vertical, c, s, u_min, v_min, (c0, l0, c1, l1))
-        dims.append((x0, y0, x1 - x0, y1 - y0, c, s, (c0, l0, c1, l1), fp))
-    n_work = sum(256 + 3 * (d[6][3] - d[6][1]) for d in dims)
-    n_scratch = sum(2 * (d[6][3] - d[6][1]) + 4 for d in dims)
+            raise ValueError(f"{what}: window {(c0, l0, c1, l1)} is empty or outside the {int(M)}x{int(L)} frame")
+        fp = window_footprint(bw, bh, vertical, c, s, u_min, v_min, (c0, l0, c1, l1))
+        dims.append((x0, y0, bw, bh, c, s, (c0, l0, c1, l1), fp))
+    areas, n_work, n_areas = _line_areas([(d[6][3] - d[6][1], 0) for d in dims])
     head = n * (osz + rsz + wsz)
-    buf = torch.empty(head + 4 * (n_work + n_scratch), dtype=torch.uint8, device=dev)
+    buf = torch.empty(head + n_areas, dtype=torch.uint8, device=dev)
     out, seg, wrec = buf.data_ptr(), buf.data_ptr() + n * osz, buf.data_ptr() + n * (osz + rsz)
     work = buf.data_ptr() + head
-    scratch, w, sc, recs, wrecs, tiles = work + 4 * n_work, 0, 0, [], [], 0
-    for i, (blk, (x0, y0, bw, bh, c, s, (c0, l0, c1, l1), (px0, py0, px1, py1))) in enumerate(zip(blocks, dims)):
+    recs, wrecs, tiles = [], [], 0
+    for i, (blk, (x0, y0, bw, bh, c, s, (c0, l0, c1, l1), (px0, py0, px1, py1)), (hist, prof, scr)) in \
+            enumerate(zip(blocks, dims, areas)):
         img, _, vertical, polarity, min_ink, gap, min_height = blk[:7]
-        hist, prof, scr = work + 4 * w, work + 4 * (w + 256), scratch + 4 * sc
-        knobs = (polarity, min_ink or 0, gap or 0, min_height or 0, 0, hist, prof, scr, out + i * osz)
+        knobs = (polarity, min_ink or 0, gap or 0, min_height or 0, 0, work + hist, work + prof, work + scr, out + i * osz)
         recs.append(_lib.TextBlock(img.data_ptr(), img.stride(0), 0, 0, c1 - c0, l1 - l0, 0, *knobs))
         crop = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), *knobs)
         wrecs.append(_lib.WindowBlock(crop, c, s, c0, l0, c1, l1, px0, py0, px1 - px0, py1 - py0))
-        w += 256 + 3 * (l1 - l0)
-        sc += 2 * (l1 - l0) + 4
         tiles = max(tiles, 1, -(-(px1 - px0) // 32) * -(-(py1 - py0) // 32))
     host = bytes((_lib.TextBlock * n)(*recs)) + bytes((_lib.WindowBlock * n)(*wrecs))
-    buf[n * osz:head].copy_(torch.from_numpy(np.frombuffer(host, dtype=np.uint8).copy()))
-    _lib.check(_lib.load().mn_find_lines_window_u8(ctypes.c_void_p(seg), ctypes.c_void_p(wrec), n, tiles, work, 4 * n_work,
-                                                   _stream()), "mn_find_lines_window_u8")
+    buf[n * osz:head].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    _lib.check(_lib.load().mn_find_lines_window_u8(seg, wrec, n, tiles, work, n_work, _stream()), "mn_find_lines_window_u8")
     LAUNCHES += 4
     return buf[:n * osz]
 
@@ -1864,106 +1853,32 @@ def find_blocks(pages, scores=False):
     (1, 0) and keep their tables exactly.  out then starts with the n mn_skew_block records (``skew_block_dtype()``: the chosen
     index and frame) and the leaves are in frame cells.  ``scores`` (tests): also return, per page, the int64 CUDA view of its
     per-angle scores (None unless it searched)."""
-    import numpy as np
     global LAUNCHES
-    if not pages:
-        raise ValueError("find_blocks: no pages")
-    if len(pages) > 65535:
-        raise ValueError("find_blocks: at most 65535 pages per launch")
-    if any(len(p) > 6 and p[6] is not None for p in pages):
-        return _find_blocks_skewed(pages, scores)
-    pages = [p[:6] for p in pages]
-    dev = pages[0][0].device
-    dims = []
-    for i, (img, rect, vertical, polarity, *gaps) in enumerate(pages):
-        _dense_u8(img, dev, 3, f"find_blocks: page {i}: img")
-        x0, y0, x1, y1 = (int(v) for v in rect)
-        if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
-            raise ValueError(f"find_blocks: page {i}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
-                             f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
-        if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or any(v is not None and not 1 <= v < 2 ** 31 for v in gaps):
-            raise ValueError(f"find_blocks: page {i}: bad polarity {polarity!r} or gap_x / gap_y {gaps!r}")
-        dims.append((x0, y0, x1 - x0, y1 - y0, page_cap(x1 - x0, y1 - y0)))
-    if sum(page_bytes(d[2], d[3]) for d in dims) > PAGE_MAX_WORK:
-        raise ValueError(f"find_blocks: the pages need more than the {PAGE_MAX_WORK} bytes of work memory a call may use")
+    dev = _check_items(pages, "find_blocks", "page")
+    skewed = any(len(p) > 6 and p[6] is not None for p in pages)
     n = len(pages)
     rsz, bsz, psz, lsz = (ctypes.sizeof(t) for t in (_lib.PageResult, _lib.TextBlock, _lib.TextPage, _lib.BlockLines))
-    out0 = n * (bsz + psz)                               # records, then the results and leaves, then the work: the call zeroes
-    n_out = n * rsz + 12 * sum(d[4] for d in dims)       # everything from out0 on
-    work0 = out0 + -(-n_out // 16) * 16
-    n_work = sum(4 * 256 + lsz + 4 * d[3] * -(-d[2] // 32) + 2 * 12 * d[4] + 3 * 4 * d[4] for d in dims)
-    buf = torch.empty(work0 + n_work, dtype=torch.uint8, device=dev)
-    base = buf.data_ptr()
-    leaves, w, blocks, recs, tiles = base + out0 + n * rsz, base + work0, [], [], 0
-    for i, ((img, _, vertical, polarity, gap_x, gap_y), (x0, y0, bw, bh, cap)) in enumerate(zip(pages, dims)):
-        wp = -(-bw // 32)
-        hist, lines, bits = w, w + 4 * 256, w + 4 * 256 + lsz
-        lists = bits + 4 * bh * wp
-        counts = lists + 2 * 12 * cap
-        w = counts + 3 * 4 * cap
-        tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, 0, 0, 0, 0, hist, 0, 0, lines)
-        blocks.append(tb)
-        recs.append(_lib.TextPage(tb, bits, (ctypes.c_void_p * 2)(lists, lists + 12 * cap), leaves, counts, counts + 4 * cap,
-                                  counts + 8 * cap, base + out0 + i * rsz, wp, cap, gap_x or 0, gap_y or 0))
-        leaves += 12 * cap
-        tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
-    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.TextPage * n)(*recs))
-    buf[:out0].copy_(torch.from_numpy(np.frombuffer(host, dtype=np.uint8).copy()))
-    _lib.check(_lib.load().mn_find_blocks_u8(ctypes.c_void_p(base), ctypes.c_void_p(base + n * bsz), n, tiles,
-                                             ctypes.c_void_p(base + out0), work0 + n_work - out0, _stream()), "mn_find_blocks_u8")
-    LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS
-    res = buf[out0:out0 + n_out], [d[4] for d in dims]
-    return res + ([None] * n,) if scores else res
-
-
-def _check_skew(skew, max_skew, vertical, what):
-    """The (c, s) table of skew / max_skew (find_lines' rules), or ValueError naming ``what``."""
-    if skew is None:
-        return [(1.0, 0.0)]
-    if not (skew == "auto" if isinstance(skew, str) else math.isfinite(skew) and abs(skew) < 45):
-        raise ValueError(f"{what}: bad skew {skew!r}")
-    if not (isinstance(skew, str) or max_skew == 10.0) or not 0 < max_skew <= 20:
-        raise ValueError(f"{what}: max_skew {max_skew!r} is outside (0, 20] or given without 'auto'")
-    return skew_cos_sin(skew_table(skew, max_skew, vertical))
-
-
-def _find_blocks_skewed(pages, want_scores):
-    """find_blocks for a call that holds a skewed page: mn_find_blocks_skewed_u8 over every page."""
-    import numpy as np
-    global LAUNCHES
-    dev = pages[0][0].device
-    n = len(pages)
-    rsz, bsz, psz, ssz, lsz = (ctypes.sizeof(t) for t in (_lib.PageResult, _lib.TextBlock, _lib.TextPage, _lib.SkewBlock,
-                                                           _lib.BlockLines))
-    dims, tables, keys, need = [], [], {}, 0
+    ssz = ctypes.sizeof(_lib.SkewBlock) if skewed else 0
+    dims, tables, need = [], [], 0
     for i, pg in enumerate(pages):
-        img, rect, vertical, polarity, *gaps = pg[:6]
-        skew, max_skew = pg[6] if len(pg) > 6 else None, pg[7] if len(pg) > 7 else 10.0
-        _dense_u8(img, dev, 3, f"find_blocks: page {i}: img")
-        x0, y0, x1, y1 = (int(v) for v in rect)
-        if not (0 <= x0 < x1 <= img.shape[1] and 0 <= y0 < y1 <= img.shape[0]) or max(x1 - x0, y1 - y0) > 32767:
-            raise ValueError(f"find_blocks: page {i}: rectangle {(x0, y0, x1, y1)} is empty, outside the "
-                             f"{img.shape[1]}x{img.shape[0]} image or has a side over 32767")
-        if polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT) or any(v is not None and not 1 <= v < 2 ** 31 for v in gaps):
-            raise ValueError(f"find_blocks: page {i}: bad polarity {polarity!r} or gap_x / gap_y {gaps!r}")
-        cs = _check_skew(skew, max_skew, vertical, f"find_blocks: page {i}")
-        need += skew_page_bytes(x1 - x0, y1 - y0, vertical, cs)
-        L, M, stride = skew_page_frame(x1 - x0, y1 - y0, vertical, cs)
+        what = f"find_blocks: page {i}"
+        x0, y0, bw, bh = _check_crop(pg[:6], dev, what, "gap_x / gap_y")
+        vertical, skew, max_skew = pg[2], pg[6] if len(pg) > 6 else None, pg[7] if len(pg) > 7 else 10.0
+        cs = _check_skew(skew, max_skew, vertical, what)
+        L, M, stride = (bh, bw, bw if vertical else bh) if skew is None else skew_page_frame(bw, bh, vertical, cs)
+        need += skew_page_bytes(bw, bh, vertical, cs) if skewed else page_bytes(bw, bh)
         if max(L, M) > 32767:
-            raise ValueError(f"find_blocks: page {i}: a frame side of {max(L, M)} exceeds 32767")
+            raise ValueError(f"{what}: a frame side of {max(L, M)} exceeds 32767")
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
-            raise ValueError(f"find_blocks: page {i}: {len(cs)} angles x {stride} bins exceed the {SKEW_MAX_PROFILE} profile "
-                             f"values a skewed page may use")
-        key = tuple(cs)
-        if key not in keys:
-            keys[key] = sum(len(t) for t in tables)
-            tables.append(cs)
-        dims.append((x0, y0, x1 - x0, y1 - y0, page_cap(M, L), L, M, len(cs), stride, keys[key]))
+            raise ValueError(f"{what}: {len(cs)} angles x {stride} bins exceed the {SKEW_MAX_PROFILE} profile values a skewed "
+                             f"page may use")
+        tables.append(cs)
+        dims.append((x0, y0, bw, bh, page_cap(M, L), L, M, len(cs), stride))
     if need > PAGE_MAX_WORK:
         raise ValueError(f"find_blocks: the pages need more than the {PAGE_MAX_WORK} bytes of work memory a call may use")
-    n_tab = sum(len(t) for t in tables)
+    tab, t_offs = _angle_tables(tables) if skewed else (b"", [0] * n)
     pg0, tab0 = n * bsz, n * (bsz + psz)                 # records, tables and the skew records, then the results and leaves,
-    out0 = -(-(tab0 + 16 * n_tab + n * ssz) // 16) * 16  # then the work: the call zeroes everything from out0 on, and the
+    out0 = -(-(tab0 + len(tab) + n * ssz) // 16) * 16    # then the work: the call zeroes everything from out0 on, and the
     sk0 = out0 - n * ssz                                 # skew records come back with the results in one copy
     n_out = n * rsz + 12 * sum(d[4] for d in dims)
     work0 = out0 + -(-n_out // 16) * 16
@@ -1972,36 +1887,37 @@ def _find_blocks_skewed(pages, want_scores):
     buf = torch.empty(work0 + sum(per), dtype=torch.uint8, device=dev)
     base = buf.data_ptr()
     leaves, w, blocks, srecs, recs, views, tiles = base + out0 + n * rsz, base + work0, [], [], [], [], 0
-    for i, (pg, d, nb) in enumerate(zip(pages, dims, per)):
+    for i, (pg, d, nb, t) in enumerate(zip(pages, dims, per, t_offs)):
         img, _, vertical, polarity, gap_x, gap_y = pg[:6]
-        x0, y0, bw, bh, cap, L, M, n_ang, stride, t = d
+        x0, y0, bw, bh, cap, L, M, n_ang, stride = d
         wp = -(-M // 32)
-        sc = w
-        hist = sc + 8 * (n_ang if n_ang > 1 else 0)
+        hist = w + 8 * (n_ang if n_ang > 1 else 0)       # after the page's per-angle scores
         lines, bits = hist + 4 * 256, hist + 4 * 256 + lsz
         lists = bits + 4 * L * wp
         counts = lists + 2 * 12 * cap
-        prof = counts + 3 * 4 * cap
         tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, 0, 0, 0, 0, hist, 0, 0, lines)
         blocks.append(tb)
-        srecs.append(_lib.SkewBlock(tb, base + tab0 + 16 * t, sc if n_ang > 1 else 0, prof if n_ang > 1 else 0, n_ang, stride,
-                                    0, 0, 0, 0, 0.0, 0.0, 0.0, 0.0))
+        if skewed:
+            srecs.append(_skew_block(tb, base + tab0 + 16 * t, w, counts + 3 * 4 * cap, n_ang, stride))
         recs.append(_lib.TextPage(tb, bits, (ctypes.c_void_p * 2)(lists, lists + 12 * cap), leaves, counts, counts + 4 * cap,
                                   counts + 8 * cap, base + out0 + i * rsz, wp, cap, gap_x or 0, gap_y or 0))
-        views.append(buf[sc - base:sc - base + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
+        views.append(buf[w - base:w - base + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         leaves += 12 * cap
         w += nb
         tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
-    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.TextPage * n)(*recs)) + \
-        np.array([v for t in tables for p in t for v in p], np.float64).tobytes()
-    host += bytes(sk0 - len(host)) + bytes((_lib.SkewBlock * n)(*srecs))
-    buf[:out0].copy_(torch.from_numpy(np.frombuffer(host, dtype=np.uint8).copy()))
-    _lib.check(_lib.load().mn_find_blocks_skewed_u8(ctypes.c_void_p(base), ctypes.c_void_p(base + sk0), ctypes.c_void_p(base + pg0),
-                                                    n, tiles, ctypes.c_void_p(base + out0), work0 + sum(per) - out0, _stream()),
-               "mn_find_blocks_skewed_u8")
-    LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS
+    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.TextPage * n)(*recs)) + tab
+    host += bytes(sk0 - len(host)) + bytes((_lib.SkewBlock * len(srecs))(*srecs))
+    buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    if skewed:
+        _lib.check(_lib.load().mn_find_blocks_skewed_u8(base, base + sk0, base + pg0, n, tiles, base + out0,
+                                                        work0 + sum(per) - out0, _stream()), "mn_find_blocks_skewed_u8")
+        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS
+    else:
+        _lib.check(_lib.load().mn_find_blocks_u8(base, base + pg0, n, tiles, base + out0, work0 + sum(per) - out0, _stream()),
+                   "mn_find_blocks_u8")
+        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS
     res = buf[sk0:out0 + n_out], [d[4] for d in dims]
-    return res + (views,) if want_scores else res
+    return res + (views,) if scores else res
 
 
 def page_result_dtype():

@@ -1613,6 +1613,17 @@ def _check_block(blk, H, W, name):
     return x0, y0, x1, y1
 
 
+def _skew_used(item, sk):
+    """The angle in degrees a TextBlock or TextPage with ``skew`` was split at: the given one, or the angle of the search table
+    that its mn_skew_block record ``sk`` chose (negated back for a vertical item, whose frame is the transposed crop)."""
+    from . import ops
+    if not isinstance(item.skew, str):
+        return float(item.skew)
+    vertical = item.direction == "vertical"
+    angle = ops.skew_table(item.skew, item.max_skew, vertical)[int(sk["chosen"])]
+    return 0.0 - angle if vertical else angle
+
+
 def _find_lines(dimg, items):
     """ops.find_lines over items (image index, TextBlock, rect) of the uploaded images ``dimg``, its table back through one pinned
     copy and one synchronisation.  Returns per item dict(lines, threshold, ink), or the error message of a block with too many
@@ -1651,9 +1662,7 @@ def _find_lines(dimg, items):
             lines = [VerticalRegion(q) for q in lines]
         res = dict(lines=lines, threshold=int(t["threshold"]), ink="dark" if t["ink"] == ops._lib.INK_DARK else "light")
         if blk.skew is not None:
-            table_angles = ops.skew_table(blk.skew, blk.max_skew, vertical)
-            angle = table_angles[int(sk["chosen"])] if sk is not None else table_angles[0]
-            res["skew"] = float(blk.skew) if not isinstance(blk.skew, str) else 0.0 - angle if vertical else angle
+            res["skew"] = _skew_used(blk, sk)
         out.append(res)
     return out
 
@@ -1731,36 +1740,42 @@ def find_lines(images, blocks):
     return out
 
 
-def _plan_blocks(shapes, regions, labels, boxes):
-    """restore_regions' text blocks, validated before any launch: [(image, region index, TextBlock, rect)], and the region lists
-    with each block in place of its rectangle (plan_regions validates the other regions on them)."""
+def _plan_items(shapes, regions, labels, boxes, kind, check, why):
+    """restore_regions' regions of type ``kind`` (TextBlock or TextPage), each validated by ``check`` before any launch:
+    [(image, region index, item, rect)], and the region lists with each item's rectangle in its place.  Labels or boxes given
+    for an item raise ValueError, ``why`` saying where its lines come from."""
     n = len(shapes)
     regions, labels, boxes = (_per_image(v, n, f"{what} (one list per image)") for v, what in
                               ((regions, "regions"), (labels, "labels"), (boxes, "boxes")))
-    blocks, stand_in = [], []
+    noun = "text block" if kind is TextBlock else "text page"
+    items, stand_in = [], []
     for i, (H, W) in enumerate(shapes):
         rects = list(regions[i] or [])
         labs = _per_image(labels[i], len(rects), f"image {i}: labels (one entry per region)")
         bxs = _per_image(boxes[i], len(rects), f"image {i}: boxes (one entry per region)")
         for r, reg in enumerate(rects):
-            if isinstance(reg, TextBlock):
-                name = f"image {i}, region {r} (a text block)"
+            if isinstance(reg, kind):
+                name = f"image {i}, region {r} (a {noun})"
                 if labs[r] is not None or bxs[r] is not None:
-                    raise ValueError(f"{name}: labels or boxes are given, but its lines are only found on the device (call "
-                                     f"find_lines and give the lines with their labels)")
-                rects[r] = _check_block(reg, H, W, name)
-                blocks.append((i, r, reg, rects[r]))
+                    raise ValueError(f"{name}: labels or boxes are given, but {why}")
+                rects[r] = check(reg, H, W, name)
+                items.append((i, r, reg, rects[r]))
         stand_in.append(rects)
-    return blocks, stand_in
+    return items, stand_in
 
 
-def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid, shapes=None, scale=4, feather=None, names=None):
-    """The region, label and box lists with each text block replaced in place by its lines, and per image the layout of its given
-    regions: None for a region, the block's find_lines result (or dict(error=...) under ``skip_invalid``) for a block.  A block
-    with too many lines, a vertical line that vertical_plan rejects, or an oriented line of a skewed block that plan_regions
-    rejects (on the image of ``shapes`` at ``scale`` and ``feather``) raises ValueError without ``skip_invalid``.  ``names``: the
-    name of the block at (image, position) when it is not "image i, region r (a text block)"."""
-    found = {(i, r): res for (i, r, _, _), res in zip(blocks, found)}
+def _plan_blocks(shapes, regions, labels, boxes):
+    """restore_regions' text blocks, validated before any launch: [(image, region index, TextBlock, rect)], and the region lists
+    with each block in place of its rectangle (plan_regions validates the other regions on them)."""
+    return _plan_items(shapes, regions, labels, boxes, TextBlock, _check_block,
+                       "its lines are only found on the device (call find_lines and give the lines with their labels)")
+
+
+def _splice(regions, labels, boxes, items, found, expand):
+    """The region, label and box lists with each item (image, region index, ...) of ``items`` replaced in place by its children,
+    and per image the layout of its given regions: None for a region, [entry, k] for an item of k children.  ``expand(i, r,
+    res)`` gives the (entry, children) of the item at (i, r) from its result ``res`` in ``found``."""
+    found = {(i, r): res for (i, r, *_), res in zip(items, found)}
     n = len(regions)
     labels, boxes = _per_image(labels, n, "labels"), _per_image(boxes, n, "boxes")
     out_r, out_l, out_b, layout = [], [], [], []
@@ -1769,32 +1784,14 @@ def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid, shapes=N
         labs, bxs = _per_image(labels[i], len(rects), "labels"), _per_image(boxes[i], len(rects), "boxes")
         rs, ls, bs, lay = [], [], [], []
         for r, reg in enumerate(rects):
-            res = found.get((i, r))
-            if res is None:
+            if (i, r) not in found:
                 rs.append(reg), ls.append(labs[r]), bs.append(bxs[r]), lay.append(None)
                 continue
-            name = (names or {}).get((i, r), f"image {i}, region {r} (a text block)")
-            err = f"{name}: {res}" if isinstance(res, str) else None
-            try:
-                for k, q in enumerate(res["lines"] if err is None else []):
-                    if isinstance(q, OrientedRegion) or isinstance(q, VerticalRegion) and isinstance(q.shape, OrientedRegion):
-                        try:
-                            plan_regions([shapes[i]], [[q]], None, None, scale, feather)
-                        except ValueError as e:
-                            raise ValueError(f"{name}, line {k}: {str(e).split(': ', 1)[-1]}") from None
-                    elif isinstance(q, VerticalRegion):
-                        vertical_plan(q.shape[2] - q.shape[0], q.shape[3] - q.shape[1], name=f"{name}, line {k}")
-            except ValueError as e:
-                err = str(e)
-            if err is not None:
-                if not skip_invalid:
-                    raise ValueError(err)
-                lay.append(dict(error=err))
-                continue
-            rs += res["lines"]
-            ls += [None] * len(res["lines"])
-            bs += [None] * len(res["lines"])
-            lay.append(res)
+            entry, children = expand(i, r, found[(i, r)])
+            rs += children
+            ls += [None] * len(children)
+            bs += [None] * len(children)
+            lay.append([entry, len(children)])
         out_r.append(rs)
         out_l.append(None if labels[i] is None else ls)
         out_b.append(None if boxes[i] is None else bs)
@@ -1802,19 +1799,47 @@ def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid, shapes=N
     return out_r, out_l, out_b, layout
 
 
-def _regroup_blocks(out, layout):
-    """restore_regions' result with each block's line entries gathered into the block's own entry, in place."""
+def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid, shapes=None, scale=4, feather=None, names=None):
+    """The region, label and box lists with each text block replaced in place by its lines, and per image the layout of its given
+    regions: None for a region, [entry, k] for a block of k lines, entry its find_lines result (or dict(error=...) and no lines
+    under ``skip_invalid``).  A block with too many lines, a vertical line that vertical_plan rejects, or an oriented line of a
+    skewed block that plan_regions rejects (on the image of ``shapes`` at ``scale`` and ``feather``) raises ValueError without
+    ``skip_invalid``.  ``names``: the name of the block at (image, position) when it is not "image i, region r (a text
+    block)"."""
+    def expand(i, r, res):
+        name = (names or {}).get((i, r), f"image {i}, region {r} (a text block)")
+        err = f"{name}: {res}" if isinstance(res, str) else None
+        try:
+            for k, q in enumerate(res["lines"] if err is None else []):
+                if isinstance(q, OrientedRegion) or isinstance(q, VerticalRegion) and isinstance(q.shape, OrientedRegion):
+                    try:
+                        plan_regions([shapes[i]], [[q]], None, None, scale, feather)
+                    except ValueError as e:
+                        raise ValueError(f"{name}, line {k}: {str(e).split(': ', 1)[-1]}") from None
+                elif isinstance(q, VerticalRegion):
+                    vertical_plan(q.shape[2] - q.shape[0], q.shape[3] - q.shape[1], name=f"{name}, line {k}")
+        except ValueError as e:
+            err = str(e)
+        if err is None:
+            return res, res["lines"]
+        if not skip_invalid:
+            raise ValueError(err)
+        return dict(error=err), []
+    return _splice(regions, labels, boxes, blocks, found, expand)
+
+
+def _regroup(out, layout):
+    """restore_regions' result with each block's (page's) child entries gathered into its own entry, in place."""
     for img, lay in zip(out, layout):
         flat, o, img["regions"] = img["regions"], 0, []
-        for res in lay:
-            if res is None:
+        for e in lay:
+            if e is None:
                 img["regions"].append(flat[o])
                 o += 1
-            elif "error" in res:
-                img["regions"].append(res)
-            else:
-                img["regions"].append(dict(res, regions=flat[o:o + len(res["lines"])]))
-                o += len(res["lines"])
+                continue
+            res, k = e
+            img["regions"].append(res if "error" in res else dict(res, regions=flat[o:o + k]))
+            o += k
 
 
 class TextPage(NamedTuple):
@@ -1923,8 +1948,7 @@ def _find_blocks(dimg, items):
         if pg.skew is None:
             res.update(blocks=[TextBlock(b, pg.direction, polarity=pg.polarity) for b in blocks], rejected=rejected)
         else:
-            angle = ops.skew_table(pg.skew, pg.max_skew, vertical)[int(sk["chosen"])]
-            res["skew"] = float(pg.skew) if not isinstance(pg.skew, str) else 0.0 - angle if vertical else angle
+            res["skew"] = _skew_used(pg, sk)
             res["blocks"] = [TextBlock(tuple(rect), pg.direction, polarity=pg.polarity, skew=res["skew"], window=b) if tilted
                              else TextBlock(b, pg.direction, polarity=pg.polarity) for b in blocks]
             res["rejected"] = rejected
@@ -1975,23 +1999,9 @@ def find_blocks(images, pages):
 def _plan_pages(shapes, regions, labels, boxes):
     """restore_regions' text pages, validated before any launch: [(image, region index, TextPage, rect)], and the region lists
     with each page's rectangle in its place."""
-    n = len(shapes)
-    regions, labels, boxes = (_per_image(v, n, f"{what} (one list per image)") for v, what in
-                              ((regions, "regions"), (labels, "labels"), (boxes, "boxes")))
-    pages, stand_in = [], []
-    for i, (H, W) in enumerate(shapes):
-        rects = list(regions[i] or [])
-        labs = _per_image(labels[i], len(rects), f"image {i}: labels (one entry per region)")
-        bxs = _per_image(boxes[i], len(rects), f"image {i}: boxes (one entry per region)")
-        for r, reg in enumerate(rects):
-            if isinstance(reg, TextPage):
-                name = f"image {i}, region {r} (a text page)"
-                if labs[r] is not None or bxs[r] is not None:
-                    raise ValueError(f"{name}: labels or boxes are given, but its blocks and lines are only found on the device "
-                                     f"(call find_blocks and find_lines and give the lines with their labels)")
-                rects[r] = _check_page(reg, H, W, name)
-                pages.append((i, r, reg, rects[r]))
-        stand_in.append(rects)
+    pages, stand_in = _plan_items(shapes, regions, labels, boxes, TextPage, _check_page,
+                                  "its blocks and lines are only found on the device (call find_blocks and find_lines and give "
+                                  "the lines with their labels)")
     if pages:
         _check_page_work([(i, pg, rect) for i, _, pg, rect in pages])
     return pages, stand_in
@@ -2001,36 +2011,23 @@ def _expand_pages(regions, labels, boxes, pages, found, skip_invalid):
     """The region, label and box lists with each text page replaced in place by its TextBlocks; the names of every TextBlock of
     the new lists by (image, position); and per image the layout of its given regions: None for a region, [entry, k] for a page
     of k blocks, entry its find_blocks result or dict(error=...) under ``skip_invalid`` for a page over a limit."""
-    found = {(i, r): res for (i, r, _, _), res in zip(pages, found)}
-    n = len(regions)
-    labels, boxes = _per_image(labels, n, "labels"), _per_image(boxes, n, "boxes")
-    out_r, out_l, out_b, names, layout = [], [], [], {}, []
-    for i in range(n):
-        rects = list(regions[i] or [])
-        labs, bxs = _per_image(labels[i], len(rects), "labels"), _per_image(boxes[i], len(rects), "boxes")
-        rs, ls, bs, lay = [], [], [], []
-        for r, reg in enumerate(rects):
-            res = found.get((i, r))
-            if res is None:
-                if isinstance(reg, TextBlock):
-                    names[(i, len(rs))] = f"image {i}, region {r} (a text block)"
-                rs.append(reg), ls.append(labs[r]), bs.append(bxs[r]), lay.append(None)
-                continue
-            name = f"image {i}, region {r} (a text page)"
-            if isinstance(res, str):
-                if not skip_invalid:
-                    raise ValueError(f"{name}: {res}")
-                lay.append([dict(error=f"{name}: {res}"), 0])
-                continue
-            for k, blk in enumerate(res["blocks"]):
-                names[(i, len(rs))] = f"{name}, block {k}"
-                rs.append(blk), ls.append(None), bs.append(None)
-            lay.append([res, len(res["blocks"])])
-        out_r.append(rs)
-        out_l.append(None if labels[i] is None else ls)
-        out_b.append(None if boxes[i] is None else bs)
-        layout.append(lay)
-    return out_r, out_l, out_b, names, layout
+    def expand(i, r, res):
+        if not isinstance(res, str):
+            return res, res["blocks"]
+        err = f"image {i}, region {r} (a text page): {res}"
+        if not skip_invalid:
+            raise ValueError(err)
+        return dict(error=err), []
+    regions, labels, boxes, layout = _splice(regions, labels, boxes, pages, found, expand)
+    names = {}
+    for i, lay in enumerate(layout):
+        at = [(r, k) for r, e in enumerate(lay) for k in ([None] if e is None else range(e[1]))]
+        for o, (r, k) in enumerate(at):
+            if k is not None:
+                names[(i, o)] = f"image {i}, region {r} (a text page), block {k}"
+            elif isinstance(regions[i][o], TextBlock):
+                names[(i, o)] = f"image {i}, region {r} (a text block)"
+    return regions, labels, boxes, names, layout
 
 
 def _failed_pages(page_layout, block_layout):
@@ -2043,26 +2040,12 @@ def _failed_pages(page_layout, block_layout):
             if e is None:
                 o += 1
                 continue
-            errs = [b["error"] for b in blays[o:o + e[1]] if b is not None and "error" in b]
+            errs = [b[0]["error"] for b in blays[o:o + e[1]] if b is not None and "error" in b[0]]
             if errs and "error" not in e[0]:
                 e[0] = dict(error=errs[0])
                 drop.update((i, o + k) for k in range(e[1]))
             o += e[1]
     return drop
-
-
-def _regroup_pages(out, layout):
-    """restore_regions' result with each page's block entries gathered into the page's own entry, in place."""
-    for img, lay in zip(out, layout):
-        flat, o, img["regions"] = img["regions"], 0, []
-        for e in lay:
-            if e is None:
-                img["regions"].append(flat[o])
-                o += 1
-                continue
-            res, k = e
-            img["regions"].append(res if "error" in res else dict(res, regions=flat[o:o + k]))
-            o += k
 
 
 def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None):
@@ -2375,9 +2358,9 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
             entry.update(size=p.size)
         out[p.image]["regions"].append(entry)
     if blocks:
-        _regroup_blocks(out, layout)
+        _regroup(out, layout)
     if text_pages:
-        _regroup_pages(out, page_layout)
+        _regroup(out, page_layout)
     return out
 
 
