@@ -818,6 +818,41 @@ typedef struct {
 int mn_find_lines_window_u8(const mn_text_block* blocks, const mn_window_block* wins, int n, long long max_tiles, void* work,
                             long long work_bytes, void* stream);
 
+/* Page corners (DESIGN.md section 7b, "Perspective pages").  Page i is the whole image of blocks[i] (x0 = y0 = 0, w x h, its
+ * polarity); pages[i].b is the same record.  mn_find_page_quads_u8 issues 8 launches for every page of a call:
+ *   1, 2. mn_find_lines_u8's histogram and threshold over blocks[] (Otsu's t into b.out);
+ *   3. per 32 x 32 tile, the 4-connected components of the paper mask (grey > t; grey <= t for MN_INK_LIGHT) merged in
+ *      shared memory: label[y w + x] = the raster index of the tile-local root, -1 off the paper;
+ *   4. the merge across tile borders, by union-find with atomicMin;
+ *   5. path compression (label = the component's smallest raster index) and each component's pixels into count[label];
+ *   6. the page: the most pixels, ties to the smallest label, into *best as (count << 32) | ~label (0: no paper);
+ *   7. each row's extent of the page, ext[2 y] = max(w - x), ext[2 y + 1] = max(x + 1) (0: none);
+ *   8. one CTA per page: the monotone-chain hull of the rows' pixel-square corners into hull (x, y pairs, cross products in
+ *      int64, collinear points dropped) and the four hull vertices of the largest doubled area, ties to the smallest index
+ *      tuple, ordered clockwise on screen from tl (the smallest x + y, then y) into res.
+ * label and count hold h w values, ext 2 h, hull 2 (4 h + 8); every one of them, best and res lie in work (work_bytes, zeroed
+ * by the call).  blocks, pages: DEVICE arrays (validated by the caller: 1 <= w, h <= 32767). */
+typedef struct {
+    int32_t threshold;          /* Otsu's t of the image */
+    int32_t label;              /* the page's label (its smallest raster index), -1 when no pixel is paper */
+    int32_t size;               /* its pixels */
+    int32_t n_hull;             /* hull vertices */
+    int64_t area2;              /* the quad's doubled area */
+    int32_t idx[4];             /* the quad's hull vertices, i < a < j < b */
+    int32_t quad[8];            /* tl, tr, br, bl as (x, y) pixel-square corners */
+} mn_page_quad;
+typedef struct {
+    mn_text_block b;
+    int32_t* label;
+    int32_t* count;
+    int32_t* ext;
+    unsigned long long* best;
+    int32_t* hull;
+    mn_page_quad* res;
+} mn_quad_page;
+int mn_find_page_quads_u8(const mn_text_block* blocks, const mn_quad_page* pages, int n, long long max_tiles, void* work,
+                          long long work_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -199,6 +199,16 @@ class TextPage(Structure):
                 ("gy", c_int32), ("pad", c_int32), ("n", c_int32 * 2)]
 
 
+class PageQuad(Structure):
+    _fields_ = [("threshold", c_int32), ("label", c_int32), ("size", c_int32), ("n_hull", c_int32), ("area2", c_int64),
+                ("idx", c_int32 * 4), ("quad", c_int32 * 8)]
+
+
+class QuadPage(Structure):
+    _fields_ = [("b", TextBlock), ("label", c_void_p), ("count", c_void_p), ("ext", c_void_p), ("best", c_void_p),
+                ("hull", c_void_p), ("res", c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -263,6 +273,7 @@ SYMBOLS = {
     "mn_find_blocks_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_blocks_skewed_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_window_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
+    "mn_find_page_quads_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

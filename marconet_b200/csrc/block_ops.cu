@@ -4,7 +4,8 @@
 // rest is integer arithmetic.  Skewed blocks (DESIGN.md 7b, "Skewed blocks") add an angle search and a rotated profile around
 // the same kernels, in six launches.  Text pages (DESIGN.md 7b, "Text pages") reuse the histogram and threshold kernels and find
 // blocks by a level-synchronous XY-cut over an ink bitmap.  Skewed pages (DESIGN.md 7b, "Skewed pages") run the same XY-cut on a
-// bitmap of rotated-frame cells, and their blocks are windows of that frame.
+// bitmap of rotated-frame cells, and their blocks are windows of that frame.  Perspective pages (DESIGN.md 7b, "Perspective
+// pages") find a photographed page's corners: the paper's largest 4-connected component, its hull and the largest quad on it.
 #include "mn_common.cuh"
 
 namespace {
@@ -1044,6 +1045,274 @@ __global__ void __launch_bounds__(kTileThreads) window_profile_kernel(const mn_w
     }
 }
 
+// Page corners (DESIGN.md 7b, "Perspective pages"): the paper's 4-connected components by label-equivalence union-find, whose
+// roots are always the smallest index of their set (a union links the larger root under the smaller one), so the labels do
+// not depend on scheduling; then the largest component's hull and its largest inscribed quad, exact in integers.
+constexpr int kHullThreads = 1024;
+
+__device__ __forceinline__ bool paper_at(const mn_text_block& b, int t, int x, int y) {
+    const int g = block_grey(b, x, y);
+    return b.polarity == MN_INK_LIGHT ? g <= t : g > t;
+}
+
+__device__ __forceinline__ int uf_find(const int* L, int x) {
+    const volatile int* v = L;                          // other threads link and compress while this one walks
+    for (int p = v[x]; p != x; p = v[x]) x = p;
+    return x;
+}
+
+__device__ void uf_union(int* L, int a, int b) {
+    for (;;) {
+        a = uf_find(L, a);
+        b = uf_find(L, b);
+        if (a == b) return;
+        if (a > b) {
+            const int t = a;
+            a = b;
+            b = t;
+        }
+        const int old = atomicMin(&L[b], a);
+        if (old == b) return;
+        b = old;                                        // b was linked meanwhile: join its new root too
+    }
+}
+
+__global__ void __launch_bounds__(kTileThreads) quad_label_local_kernel(const mn_quad_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    __shared__ int s_l[kTile * kTile];
+    const mn_text_block b = pages[blockIdx.y].b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    const int t = b.out->threshold, lx = threadIdx.x & 31;
+    for (int r = threadIdx.x >> 5; r < kTile; r += 8) {
+        const int x = tx + lx, y = ty + r;
+        s_l[r * kTile + lx] = x < b.w && y < b.h && paper_at(b, t, x, y) ? r * kTile + lx : -1;
+    }
+    __syncthreads();
+    for (int r = threadIdx.x >> 5; r < kTile; r += 8) {
+        const int k = r * kTile + lx;
+        if (s_l[k] < 0) continue;
+        if (lx > 0 && s_l[k - 1] >= 0) uf_union(s_l, k - 1, k);
+        if (r > 0 && s_l[k - kTile] >= 0) uf_union(s_l, k - kTile, k);
+    }
+    __syncthreads();
+    int* label = pages[blockIdx.y].label;
+    for (int r = threadIdx.x >> 5; r < kTile; r += 8) {
+        const int x = tx + lx, y = ty + r;
+        if (x >= b.w || y >= b.h) continue;
+        int v = -1;
+        if (s_l[r * kTile + lx] >= 0) {
+            const int root = uf_find(s_l, r * kTile + lx);
+            v = (ty + root / kTile) * b.w + tx + root % kTile;
+        }
+        label[(long long)y * b.w + x] = v;
+    }
+}
+
+// Thread k < 32 joins row k of the tile's left column to its left neighbour, thread 32 + k column k of its top row to the
+// pixel above.
+__global__ void __launch_bounds__(64) quad_label_border_kernel(const mn_quad_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    const mn_text_block b = pages[blockIdx.y].b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    const bool left = threadIdx.x < 32;
+    const int k = threadIdx.x & 31, x = left ? tx : tx + k, y = left ? ty + k : ty;
+    if ((left ? tx : ty) == 0 || x >= b.w || y >= b.h) return;
+    int* label = pages[blockIdx.y].label;
+    const int p = y * b.w + x, q = left ? p - 1 : p - b.w;
+    if (label[p] >= 0 && label[q] >= 0) uf_union(label, q, p);
+}
+
+// Path compression, and each component's pixels counted at its root with one atomic per label and warp row.
+__global__ void __launch_bounds__(kTileThreads) quad_label_count_kernel(const mn_quad_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    const mn_text_block b = pages[blockIdx.y].b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    int* label = pages[blockIdx.y].label;
+    int* count = pages[blockIdx.y].count;
+    const int x = tx + (threadIdx.x & 31);
+    for (int y = ty + (threadIdx.x >> 5); y < ty + kTile; y += 8) {
+        int r = -1;
+        if (x < b.w && y < b.h) {
+            const int p = y * b.w + x;
+            if (label[p] >= 0) {
+                r = uf_find(label, p);
+                label[p] = r;
+            }
+        }
+        const unsigned same = __match_any_sync(0xffffffffu, r);
+        if (r >= 0 && (int)(threadIdx.x & 31) == __ffs(same) - 1) atomicAdd(&count[r], __popc(same));
+    }
+}
+
+__global__ void __launch_bounds__(kTileThreads) quad_pick_kernel(const mn_quad_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    const mn_text_block b = pages[blockIdx.y].b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    const int* label = pages[blockIdx.y].label;
+    const int* count = pages[blockIdx.y].count;
+    const int x = tx + (threadIdx.x & 31);
+    unsigned long long key = 0;
+    for (int y = ty + (threadIdx.x >> 5); y < min(ty + kTile, b.h) && x < b.w; y += 8) {
+        const int p = y * b.w + x;
+        if (label[p] == p) key = max(key, (unsigned long long)count[p] << 32 | (unsigned)~p);
+    }
+    for (int o = 16; o; o >>= 1) key = max(key, __shfl_xor_sync(0xffffffffu, key, o));
+    if ((threadIdx.x & 31) == 0 && key) atomicMax(pages[blockIdx.y].best, key);
+}
+
+__global__ void __launch_bounds__(kTileThreads) quad_rows_kernel(const mn_quad_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    const mn_text_block b = pages[blockIdx.y].b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    const unsigned long long best = *pages[blockIdx.y].best;
+    if (!best) return;
+    const int page = (int)~(unsigned)best;
+    const int* label = pages[blockIdx.y].label;
+    int* ext = pages[blockIdx.y].ext;
+    const int x = tx + (threadIdx.x & 31);
+    for (int y = ty + (threadIdx.x >> 5); y < min(ty + kTile, b.h); y += 8) {
+        const bool in = x < b.w && label[y * b.w + x] == page;
+        const unsigned lo = __reduce_max_sync(0xffffffffu, in ? (unsigned)(b.w - x) : 0u);
+        const unsigned hi = __reduce_max_sync(0xffffffffu, in ? (unsigned)(x + 1) : 0u);
+        if ((threadIdx.x & 31) == 0 && hi) {
+            atomicMax(&ext[2 * y], (int)lo);
+            atomicMax(&ext[2 * y + 1], (int)hi);
+        }
+    }
+}
+
+__device__ __forceinline__ long long cross3(int2 o, int2 a, int2 c) {
+    return (long long)(a.x - o.x) * (c.y - o.y) - (long long)(a.y - o.y) * (c.x - o.x);
+}
+
+__device__ __forceinline__ long long tri2(const int2* v, int i, int m, int j) {
+    const long long c = cross3(v[i], v[m], v[j]);
+    return c < 0 ? -c : c;
+}
+
+// Point i of the rows' pixel-square corners, sorted by (y, x): y = y0 + i / 2, the left end (even i) or the right end (odd i)
+// of rows y - 1 and y.
+__device__ __forceinline__ int2 row_point(const int* ext, int w, int y0, int y1, int i) {
+    const int y = y0 + (i >> 1);
+    int v = 0;
+    for (int r = max(y - 1, y0); r <= min(y, y1); ++r) v = max(v, ext[2 * r + (i & 1)]);
+    return make_int2((i & 1) ? v : w - v, y);
+}
+
+__device__ __forceinline__ bool quad_before(long long a, int4 ia, long long b, int4 ib) {
+    if (a != b) return a > b;
+    if (ia.x != ib.x) return ia.x < ib.x;
+    if (ia.y != ib.y) return ia.y < ib.y;
+    if (ia.z != ib.z) return ia.z < ib.z;
+    return ia.w < ib.w;
+}
+
+// One CTA per page: the monotone chain on one thread, then the O(k^2) quad search over the first index, each thread with two
+// rotating apex pointers (on a strictly convex polygon the smallest apex of the largest triangle over a diagonal i-j moves
+// forward with j), and a tree reduction.
+__global__ void __launch_bounds__(kHullThreads) quad_hull_kernel(const mn_quad_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    __shared__ long long s_area[kHullThreads];
+    __shared__ int4 s_idx[kHullThreads];
+    __shared__ int s_y0, s_y1, s_k;
+    const mn_quad_page& pg = pages[blockIdx.x];
+    const mn_text_block b = pg.b;
+    mn_page_quad* res = pg.res;
+    const unsigned long long best = *pg.best;
+    const int* ext = pg.ext;
+    int2* hull = reinterpret_cast<int2*>(pg.hull);
+    if (threadIdx.x == 0) {
+        s_y0 = b.h;
+        s_y1 = -1;
+        res->threshold = b.out->threshold;
+        res->label = best ? (int)~(unsigned)best : -1;
+        res->size = (int)(best >> 32);
+    }
+    __syncthreads();
+    if (!best) return;
+    for (int y = threadIdx.x; y < b.h; y += blockDim.x) {
+        if (ext[2 * y + 1]) {
+            atomicMin(&s_y0, y);
+            atomicMax(&s_y1, y);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const int y0 = s_y0, y1 = s_y1, n = 2 * (y1 - y0 + 2);
+        int k = 0;
+        for (int i = 0; i < n; ++i) {
+            const int2 p = row_point(ext, b.w, y0, y1, i);
+            while (k >= 2 && cross3(hull[k - 2], hull[k - 1], p) <= 0) --k;
+            hull[k++] = p;
+        }
+        for (int i = n - 2, lo = k + 1; i >= 0; --i) {
+            const int2 p = row_point(ext, b.w, y0, y1, i);
+            while (k >= lo && cross3(hull[k - 2], hull[k - 1], p) <= 0) --k;
+            hull[k++] = p;
+        }
+        s_k = k - 1;
+        res->n_hull = k - 1;
+    }
+    __syncthreads();
+    const int k = s_k;
+    long long area = -1;
+    int4 id = make_int4(0, 0, 0, 0);
+    for (int i = threadIdx.x; i + 3 < k; i += blockDim.x) {
+        int a = i + 1, c = i + 3;
+        for (int j = i + 2; j + 1 < k; ++j) {
+            while (a + 1 < j && tri2(hull, i, a + 1, j) > tri2(hull, i, a, j)) ++a;
+            c = max(c, j + 1);
+            while (c + 1 < k && tri2(hull, j, c + 1, i) > tri2(hull, j, c, i)) ++c;
+            const long long s = tri2(hull, i, a, j) + tri2(hull, j, c, i);
+            if (s > area) {
+                area = s;
+                id = make_int4(i, a, j, c);
+            }
+        }
+    }
+    s_area[threadIdx.x] = area;
+    s_idx[threadIdx.x] = id;
+    __syncthreads();
+    for (int h = blockDim.x / 2; h; h >>= 1) {
+        if (threadIdx.x < h && quad_before(s_area[threadIdx.x + h], s_idx[threadIdx.x + h], s_area[threadIdx.x], s_idx[threadIdx.x])) {
+            s_area[threadIdx.x] = s_area[threadIdx.x + h];
+            s_idx[threadIdx.x] = s_idx[threadIdx.x + h];
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        const int4 q = s_idx[0];
+        const bool cw = cross3(hull[q.x], hull[q.y], hull[q.z]) > 0;   // clockwise on screen (y down)
+        int2 c[4] = {hull[q.x], hull[cw ? q.y : q.w], hull[q.z], hull[cw ? q.w : q.y]};
+        int s = 0, sx = c[0].x, sy = c[0].y;
+#pragma unroll
+        for (int m = 1; m < 4; ++m) {
+            const int d = (c[m].x + c[m].y) - (sx + sy);
+            if (d < 0 || (d == 0 && c[m].y < sy)) {
+                s = m;
+                sx = c[m].x;
+                sy = c[m].y;
+            }
+        }
+        res->area2 = s_area[0];
+        res->idx[0] = q.x;
+        res->idx[1] = q.y;
+        res->idx[2] = q.z;
+        res->idx[3] = q.w;
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+            const int2 p = s == 0 ? c[m] : s == 1 ? c[(m + 1) & 3] : s == 2 ? c[(m + 2) & 3] : c[(m + 3) & 3];
+            res->quad[2 * m] = p.x;
+            res->quad[2 * m + 1] = p.y;
+        }
+    }
+}
+
 // 4-11 of the XY-cut: both passes of levels, the text size between them and the leaves, on pages whose bitmap and root are
 // written.
 int page_levels(mn_text_page* pages, int n, cudaStream_t st) {
@@ -1152,6 +1421,29 @@ extern "C" int mn_find_lines_window_u8(const mn_text_block* blocks, const mn_win
     MN_CUDA_CHECK((mn_launch(window_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, wins)));
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(block_lines_kernel, dim3(n), dim3(kSegThreads), 0, st, blocks)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_find_page_quads_u8(const mn_text_block* blocks, const mn_quad_page* pages, int n, long long max_tiles, void* work,
+                                     long long work_bytes, void* stream) {
+    MN_REQUIRE(blocks && pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
+               "mn_find_page_quads_u8: bad args");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int rc = block_threshold(blocks, n, max_tiles, work, work_bytes, st);
+    if (rc != MN_OK) return rc;
+    const dim3 grid((unsigned)max_tiles, n);
+    MN_CUDA_CHECK((mn_launch(quad_label_local_kernel, grid, dim3(kTileThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(quad_label_border_kernel, grid, dim3(64), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(quad_label_count_kernel, grid, dim3(kTileThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(quad_pick_kernel, grid, dim3(kTileThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(quad_rows_kernel, grid, dim3(kTileThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(quad_hull_kernel, dim3(n), dim3(kHullThreads), 0, st, pages)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -7,6 +7,7 @@ slices of a concatenation buffer).
 """
 import ctypes
 import functools
+import itertools
 import math
 from typing import NamedTuple
 
@@ -1930,6 +1931,65 @@ def page_node_dtype():
     """numpy view of an mn_page_node record (x0, y0, x1, y1 in the page's crop, st)."""
     import numpy as np
     return np.dtype([("x0", "<i2"), ("y0", "<i2"), ("x1", "<i2"), ("y1", "<i2"), ("st", "<i4")])
+
+
+def _quad_areas(w, h):
+    """Byte sizes of one w x h image's areas in find_page_quads: histogram, threshold record, page key, row extents (2 h),
+    labels and counts (h w each) and the hull stack (4 h + 8 points), each rounded to 16 bytes."""
+    sizes = (4 * 256, ctypes.sizeof(_lib.BlockLines), 8, 8 * h, 4 * h * w, 4 * h * w, 8 * (4 * h + 8))
+    return [-(-s // 16) * 16 for s in sizes]
+
+
+def quad_page_bytes(w, h):
+    """Device bytes of one w x h image in find_page_quads: its records, its result and its areas."""
+    return (ctypes.sizeof(_lib.TextBlock) + ctypes.sizeof(_lib.QuadPage) + ctypes.sizeof(_lib.PageQuad) + 32
+            + sum(_quad_areas(w, h)))
+
+
+def find_page_quads(pages, hulls=False):
+    """Page corners (mn_find_page_quads_u8; DESIGN.md 7b, "Perspective pages"), every image of the call in 8 launches whatever
+    their number.  pages: list of (img, polarity): img a uint8 [H, W, 3] CUDA view with dense pixels (any row stride), H, W <=
+    32767, read in place whole; polarity _lib.INK_AUTO / INK_DARK / INK_LIGHT (paper is grey <= t for INK_LIGHT, else grey > t).
+    Returns the uint8 CUDA tensor of the pages' mn_page_quad records, in order (read it back as ``page_quad_dtype()``).
+    ``hulls`` (tests): also return, per page, the int32 [4 H + 8, 2] CUDA view of its hull stack, whose first n_hull rows are
+    the hull."""
+    global LAUNCHES
+    dev = _check_items(pages, "find_page_quads", "page")
+    n = len(pages)
+    bsz, psz, rsz = (ctypes.sizeof(t) for t in (_lib.TextBlock, _lib.QuadPage, _lib.PageQuad))
+    for i, (img, polarity) in enumerate(pages):
+        _check_crop((img, (0, 0, img.shape[1], img.shape[0]), False, polarity), dev, f"find_page_quads: page {i}", "")
+    if sum(quad_page_bytes(img.shape[1], img.shape[0]) for img, _ in pages) > PAGE_MAX_WORK:
+        raise ValueError(f"find_page_quads: the pages need more than the {PAGE_MAX_WORK} bytes of work memory a call may use")
+    out0 = -(-n * (bsz + psz) // 16) * 16                # records, then the results and the work, which the call zeroes
+    work0 = out0 + -(-n * rsz // 16) * 16
+    areas = [_quad_areas(img.shape[1], img.shape[0]) for img, _ in pages]
+    buf = torch.empty(work0 + sum(map(sum, areas)), dtype=torch.uint8, device=dev)
+    base = buf.data_ptr()
+    blocks, recs, views, w, tiles = [], [], [], base + work0, 0
+    for i, ((img, polarity), sizes) in enumerate(zip(pages, areas)):
+        h_, w_ = img.shape[:2]
+        hist, lines, best, ext, label, count, hull = itertools.accumulate([w] + sizes[:-1])
+        tb = _lib.TextBlock(img.data_ptr(), img.stride(0), 0, 0, w_, h_, 0, polarity, 0, 0, 0, 0, hist, 0, 0, lines)
+        blocks.append(tb)
+        recs.append(_lib.QuadPage(tb, label, count, ext, best, hull, base + out0 + i * rsz))
+        views.append(buf[hull - base:hull - base + sizes[-1]].view(torch.int32).view(-1, 2))
+        w += sum(sizes)
+        tiles = max(tiles, -(-w_ // 32) * -(-h_ // 32))
+    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.QuadPage * n)(*recs))
+    buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    _lib.check(_lib.load().mn_find_page_quads_u8(base, base + n * bsz, n, tiles, base + out0, len(buf) - out0, _stream()),
+               "mn_find_page_quads_u8")
+    LAUNCHES += 8
+    res = buf[out0:out0 + n * rsz]
+    return (res, views) if hulls else res
+
+
+def page_quad_dtype():
+    """numpy view of an mn_page_quad record."""
+    import numpy as np
+    return np.dtype([("threshold", "<i4"), ("label", "<i4"), ("size", "<i4"), ("n_hull", "<i4"), ("area2", "<i8"),
+                     ("idx", "<i4", (4,)), ("quad", "<i4", (8,))])
 
 
 def vertical_unlayout(items):

@@ -1192,9 +1192,16 @@ def _plan_quad(reg, H, W, scale, name, column=None):
     reach = max(abs(n[r][0] * x + n[r][1] * y + n[r][2]) for r in range(2) for x, y in corners)
     if 32 * reach / min(dens) >= 2.0 ** 30:
         raise ValueError(f"{name}: the map onto its {out} output box exceeds OpenCV's 32-bit fixed-point coordinates")
+    return maps, _quad_box(pts, (H, W)), out
+
+
+def _quad_box(pts, shape=None):
+    """The integer pixel box (x0, y0, x1, y1) of a quad's corners, clipped to an image of ``shape`` (H, W) when given, else at 0."""
     xs, ys = [p[0] for p in pts], [p[1] for p in pts]
-    rect = (max(0, math.floor(min(xs))), max(0, math.floor(min(ys))), min(W, math.ceil(max(xs))), min(H, math.ceil(max(ys))))
-    return maps, rect, out
+    x1, y1 = math.ceil(max(xs)), math.ceil(max(ys))
+    if shape is not None:
+        x1, y1 = min(shape[1], x1), min(shape[0], y1)
+    return max(0, math.floor(min(xs))), max(0, math.floor(min(ys))), x1, y1
 
 
 class CurvedRegion(NamedTuple):
@@ -1542,7 +1549,10 @@ class TextBlock(NamedTuple):
     |skew| < 45, counter-clockwise on screen as OrientedRegion.from_rotated's, or "auto": the angle is searched on the device
     within +-``max_skew`` degrees (in (0, 20], only with "auto") and the lines are OrientedRegions of that angle.
     ``window`` (DESIGN.md 7b, "Skewed pages"; only with a given angle): an integer rectangle (c0, l0, c1, l1) of frame cells at
-    that angle; the block is then the pixels of ``rect`` whose cell lies in it.  find_blocks gives a tilted page's blocks so."""
+    that angle; the block is then the pixels of ``rect`` whose cell lies in it.  find_blocks gives a tilted page's blocks so.
+    ``quad`` (DESIGN.md 7b, "Perspective pages"): a QuadRegion, a block seen in perspective whose lines are found on the quad's
+    rectified crop R (quad_maps' w_r x h_r) and come back as QuadRegions; ``rect`` is then the quad's pixel box (build the
+    block with from_quad), ``skew`` is None and ``window``, if given, is an integer rectangle (x0, y0, x1, y1) of R."""
     rect: object
     direction: str = "horizontal"
     min_ink: object = None
@@ -1552,6 +1562,14 @@ class TextBlock(NamedTuple):
     skew: object = None
     max_skew: float = 10.0
     window: object = None
+    quad: object = None
+
+    @classmethod
+    def from_quad(cls, quad, shape=None, **kw):
+        """The TextBlock of a QuadRegion ``quad``: ``rect`` its integer pixel box as _plan_quad computes it, clipped to an image of
+        ``shape`` (H, W) (needed when a corner lies past the image's right or bottom side); other fields as keywords."""
+        q = QuadRegion(*((float(p[0]), float(p[1])) for p in quad))
+        return cls(_quad_box(q, shape), quad=q, **kw)
 
 
 _INK = {"auto": 0, "dark": 1, "light": 2}
@@ -1572,6 +1590,10 @@ def _check_block(blk, H, W, name):
         raise ValueError(f"{name}: rectangle {(x0, y0, x1, y1)} is empty or outside the {W}x{H} image")
     if max(x1 - x0, y1 - y0) > 32767:
         raise ValueError(f"{name}: a side of rectangle {(x0, y0, x1, y1)} exceeds 32767 pixels")
+    size = _check_quad(blk.quad, blk.skew, H, W, name) if blk.quad is not None else None
+    if size is not None and (x0, y0, x1, y1) != _quad_box(blk.quad, (H, W)):
+        raise ValueError(f"{name}: rectangle {(x0, y0, x1, y1)} is not the quad's pixel box {_quad_box(blk.quad, (H, W))} "
+                         f"(build the block with TextBlock.from_quad)")
     if blk.direction not in ("horizontal", "vertical"):
         raise ValueError(f"{name}: direction must be 'horizontal' or 'vertical', got {blk.direction!r}")
     if blk.polarity not in _INK:
@@ -1597,7 +1619,17 @@ def _check_block(blk, H, W, name):
         if len(table) > 1 and len(table) * stride > ops.SKEW_MAX_PROFILE:
             raise ValueError(f"{name}: the angle search needs {len(table)} angles x {stride} bins, over the "
                              f"{ops.SKEW_MAX_PROFILE} profile values a block may use (narrow max_skew or split the block)")
-    if blk.window is not None:
+    if blk.window is not None and size is not None:
+        try:
+            wx0, wy0, wx1, wy1 = blk.window
+            if not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) for v in (wx0, wy0, wx1, wy1)):
+                raise ValueError
+        except (TypeError, ValueError):
+            raise ValueError(f"{name}: a window is four integers (x0, y0, x1, y1), got {blk.window!r}") from None
+        if not (0 <= wx0 < wx1 <= size[0] and 0 <= wy0 < wy1 <= size[1]):
+            raise ValueError(f"{name}: window {(wx0, wy0, wx1, wy1)} is empty or outside the {size[0]}x{size[1]} rectified crop "
+                             f"of the quad")
+    elif blk.window is not None:
         if sk is None or auto:
             raise ValueError(f"{name}: a window is given, but skew is {sk!r}, not a given angle")
         try:
@@ -1613,6 +1645,47 @@ def _check_block(blk, H, W, name):
     return x0, y0, x1, y1
 
 
+def _check_quad(quad, skew, H, W, name):
+    """The rectified size (w_r, h_r) of the QuadRegion ``quad`` of a TextBlock or TextPage of an H x W image, validated under
+    _plan_quad's rules (at scale 1) with no ``skew``.  Raises ValueError naming ``name``."""
+    if not isinstance(quad, QuadRegion):
+        raise ValueError(f"{name}: quad must be a QuadRegion, got {quad!r}")
+    if skew is not None:
+        raise ValueError(f"{name}: skew and quad are both given (skew together with perspective is not supported)")
+    return _plan_quad(quad, H, W, 1, name)[0].size
+
+
+def _quad_key(i, quad):
+    """The key of a quad's rectified crop of image i."""
+    return i, tuple((float(p[0]), float(p[1])) for p in quad)
+
+
+def _rectify(dimg, keys):
+    """The rectified crop R of every distinct (image index, quad) of ``keys`` (_quad_key), ops.warp_perspective of quad_maps(quad,
+    1), all in one launch: {key: uint8 [h_r, w_r, 3] CUDA view}.  No launch without keys."""
+    from . import ops
+    keys = list(dict.fromkeys(keys))
+    if not keys:
+        return {}
+    maps = [quad_maps(q, 1) for _, q in keys]
+    views = _flat_views([m.size[::-1] for m in maps], dimg[keys[0][0]].device)
+    ops.warp_perspective([(dimg[i], v, m.matrix) for (i, _), v, m in zip(keys, views, maps)])
+    return dict(zip(keys, views))
+
+
+def _line_quad(quad, size, rect):
+    """A line rectangle (x0, y0, x1, y1) of a quad's rectified crop of ``size`` (w_r, h_r) -> QuadRegion(H(x0 / w_r, y0 / h_r),
+    H(x1 / w_r, y0 / h_r), H(x1 / w_r, y1 / h_r), H(x0 / w_r, y1 / h_r)), H the quad's unit-square homography, in fp64."""
+    (a, b, c), (d, e, f), (g, h, _) = _quad_homography([(float(p[0]), float(p[1])) for p in quad])
+    w_r, h_r = size
+    x0, y0, x1, y1 = rect
+
+    def at(u, v):
+        w = g * u + h * v + 1.0
+        return ((a * u + b * v + c) / w, (d * u + e * v + f) / w)
+    return QuadRegion(at(x0 / w_r, y0 / h_r), at(x1 / w_r, y0 / h_r), at(x1 / w_r, y1 / h_r), at(x0 / w_r, y1 / h_r))
+
+
 def _skew_used(item, sk):
     """The angle in degrees a TextBlock or TextPage with ``skew`` was split at: the given one, or the angle of the search table
     that its mn_skew_block record ``sk`` chose (negated back for a vertical item, whose frame is the transposed crop)."""
@@ -1624,16 +1697,22 @@ def _skew_used(item, sk):
     return 0.0 - angle if vertical else angle
 
 
-def _find_lines(dimg, items):
+def _find_lines(dimg, items, rq=None):
     """ops.find_lines over items (image index, TextBlock, rect) of the uploaded images ``dimg``, its table back through one pinned
-    copy and one synchronisation.  Returns per item dict(lines, threshold, ink), or the error message of a block with too many
-    lines."""
+    copy and one synchronisation; a quad block is a level block on the window of its rectified crop in ``rq`` (_rectify).
+    Returns per item dict(lines, threshold, ink), or the error message of a block with too many lines."""
     from . import ops
-    plain = [it for it in items if it[1].window is None]
-    wins = [it for it in items if it[1].window is not None]
+    plain = [it for it in items if it[1].window is None or it[1].quad is not None]
+    wins = [it for it in items if it[1].window is not None and it[1].quad is None]
+
+    def src(i, blk, rect):
+        if blk.quad is None:
+            return dimg[i], rect
+        r = rq[_quad_key(i, blk.quad)]
+        return r, blk.window or (0, 0, r.shape[1], r.shape[0])
     parts = []
     if plain:
-        parts.append(ops.find_lines([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap,
+        parts.append(ops.find_lines([(*src(i, blk, rect), blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap,
                                       blk.min_height, blk.skew, blk.max_skew) for i, blk, rect in plain]))
     if wins:
         parts.append(ops.find_lines_window([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap,
@@ -1654,7 +1733,11 @@ def _find_lines(dimg, items):
             continue
         lines = [tuple(int(v) for v in q) for q in t["rect"][:n]]
         vertical = blk.direction == "vertical"
-        if blk.window is not None:
+        if blk.quad is not None:
+            r = rq[_quad_key(i, blk.quad)]
+            lines = [_line_quad(blk.quad, (r.shape[1], r.shape[0]), q) for q in lines]
+            lines = [VerticalRegion(q) for q in lines] if vertical else lines
+        elif blk.window is not None:
             lines, sk = _window_lines(rect, vertical, blk.skew, blk.window, lines), None
         elif blk.skew is not None and sk["s"] != 0:
             lines = skew_lines(rect, vertical, float(sk["c"]), float(sk["s"]), float(sk["u_min"]), float(sk["v_min"]), lines)
@@ -1717,7 +1800,9 @@ def find_lines(images, blocks):
     A block with ``skew`` (DESIGN.md 7b, "Skewed blocks") has its angle searched (or given) on the device and is split in the
     rotated frame; a call that holds one runs every block through ops.find_lines' six launches.  Its dict gains ``skew``, the
     angle used in degrees, and its lines are OrientedRegions (VerticalRegions of OrientedRegions for a vertical block), or the
-    rectangles of skew=None when the angle is exactly 0."""
+    rectangles of skew=None when the angle is exactly 0.  A block with ``quad`` (DESIGN.md 7b, "Perspective pages") is split
+    as a level block on its window of the quad's rectified crop (every distinct quad of the call warped in one launch), and its
+    lines are QuadRegions (VerticalRegions of QuadRegions for a vertical block)."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     blocks = _per_image(blocks, len(imgs), "blocks (one list per image)")
     items, names = [], []
@@ -1732,7 +1817,8 @@ def find_lines(images, blocks):
         return out
     dev = next((im.device for im in imgs if im.is_cuda), torch.device("cuda", torch.cuda.current_device()))
     with torch.cuda.device(dev):
-        res = _find_lines(_device_images(sorted({i for i, _, _ in items}), imgs, dev), items)
+        dimg = _device_images(sorted({i for i, _, _ in items}), imgs, dev)
+        res = _find_lines(dimg, items, _rectify(dimg, [_quad_key(i, blk.quad) for i, blk, _ in items if blk.quad is not None]))
     for (i, _, _), name, r in zip(items, names, res):
         if isinstance(r, str):
             raise ValueError(f"{name}: {r}")
@@ -1811,7 +1897,8 @@ def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid, shapes=N
         err = f"{name}: {res}" if isinstance(res, str) else None
         try:
             for k, q in enumerate(res["lines"] if err is None else []):
-                if isinstance(q, OrientedRegion) or isinstance(q, VerticalRegion) and isinstance(q.shape, OrientedRegion):
+                if isinstance(q, (OrientedRegion, QuadRegion)) or isinstance(q, VerticalRegion) and \
+                        isinstance(q.shape, (OrientedRegion, QuadRegion)):
                     try:
                         plan_regions([shapes[i]], [[q]], None, None, scale, feather)
                     except ValueError as e:
@@ -1848,7 +1935,10 @@ class TextPage(NamedTuple):
     (lines read left to right, blocks top to bottom) or "vertical" (columns read top to bottom, blocks right to left).
     ``polarity``: as a TextBlock's.  ``gap_x``, ``gap_y``: positive integers in place of the default cut thresholds.
     find_blocks returns its blocks; restore_regions replaces it by them, and each of them by its lines.  ``skew``, ``max_skew``
-    (DESIGN.md 7b, "Skewed pages"): as a TextBlock's; a tilted page's blocks are found in its rotated frame."""
+    (DESIGN.md 7b, "Skewed pages"): as a TextBlock's; a tilted page's blocks are found in its rotated frame.  ``quad``
+    (DESIGN.md 7b, "Perspective pages"): None, a QuadRegion (the page's corners tl, tr, br, bl as it is read) or "auto" (the
+    corners are found on the device); its blocks are found on the quad's rectified crop R and are TextBlock.from_quad(quad,
+    window=...) windows of R.  With a quad, ``rect`` and ``skew`` are None."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
@@ -1856,12 +1946,21 @@ class TextPage(NamedTuple):
     gap_y: object = None
     skew: object = None
     max_skew: float = 10.0
+    quad: object = None
 
 
 def _check_page(pg, H, W, name):
     """The rectangle (x0, y0, x1, y1) of the TextPage ``pg`` of an H x W image, validated.  Raises ValueError naming ``name``."""
     from . import ops
     rect = (0, 0, W, H) if pg.rect is None else pg.rect
+    if pg.quad is not None:
+        if pg.rect is not None:
+            raise ValueError(f"{name}: rect and quad are both given (a page in perspective is its quad: give rect=None)")
+        if not (isinstance(pg.quad, str) and pg.quad == "auto"):
+            _check_quad(pg.quad, pg.skew, H, W, name)
+            rect = _quad_box(pg.quad, (H, W))
+        elif pg.skew is not None:
+            raise ValueError(f"{name}: skew and quad are both given (skew together with perspective is not supported)")
     try:
         if isinstance(rect, (OrientedRegion, QuadRegion, CurvedRegion, VerticalRegion)):
             raise ValueError
@@ -1891,9 +1990,15 @@ def _page_table(pg):
 
 
 def _page_bytes(pg, rect, skewed):
-    """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages."""
+    """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages: a quad page's rectified crop and
+    its page, or an auto page's corner search on the image ``rect``."""
     from . import ops
     w, h = rect[2] - rect[0], rect[3] - rect[1]
+    if isinstance(pg.quad, str):
+        return ops.quad_page_bytes(w, h)
+    if pg.quad is not None:
+        w_r, h_r = quad_maps(pg.quad, 1).size
+        return 3 * w_r * h_r + _page_bytes(pg._replace(quad=None), (0, 0, w_r, h_r), skewed)
     if not skewed:
         return ops.page_bytes(w, h)
     return ops.skew_page_bytes(w, h, pg.direction == "vertical", _page_table(pg) if pg.skew is not None else [(1.0, 0.0)])
@@ -1908,14 +2013,61 @@ def _check_page_work(items):
                          f"may use (split the call)")
 
 
-def _find_blocks(dimg, items):
+def _page_quads(dimg, items):
+    """items (image index, TextPage, rect) with each TextPage(quad="auto") given the corners ops.find_page_quads finds (one
+    pinned copy and one synchronisation), or replaced by its error message when they are not a page: no paper, a quad under a
+    quarter of the image, or one _plan_quad or the work limit rejects.  No launch without such pages."""
+    from . import ops
+    items = list(items)
+    auto = [k for k, it in enumerate(items) if isinstance(it[1].quad, str)]
+    if not auto:
+        return items
+    host = _to_host(ops.find_page_quads([(dimg[items[k][0]], _INK[items[k][1].polarity]) for k in auto])).numpy()
+    for k, r in zip(auto, host.view(ops.page_quad_dtype())):
+        i, pg, _ = items[k]
+        H, W = dimg[i].shape[:2]
+        if r["label"] < 0:
+            items[k] = "no page found: no pixel is paper"
+            continue
+        if 2 * int(r["area2"]) < H * W:
+            items[k] = (f"no page found: the largest quad on the paper covers {int(r['area2']) / 2:g} pixels, under a "
+                             f"quarter of the {W}x{H} image")
+            continue
+        pq = pg._replace(quad=QuadRegion(*((float(r["quad"][2 * m]), float(r["quad"][2 * m + 1])) for m in range(4))))
+        try:
+            _check_page(pq, H, W, "page")
+        except ValueError as e:
+            items[k] = f"no page found: the quad {tuple(pq.quad)} is rejected ({str(e).split(': ', 1)[-1]})"
+            continue
+        items[k] = (i, pq, _quad_box(pq.quad, (H, W)))
+    return items
+
+
+def _find_pages(dimg, items, keys=()):
+    """_page_quads, _rectify and _find_blocks over items (image index, TextPage, rect): per item the _find_blocks result or an
+    error message, and the rectified crops of every quad page and of ``keys`` (warped in one launch)."""
+    items = _page_quads(dimg, items)
+    ok = [it for it in items if not isinstance(it, str)]
+    rq = _rectify(dimg, [_quad_key(i, pg.quad) for i, pg, _ in ok if pg.quad is not None] + list(keys))
+    found = iter(_find_blocks(dimg, ok, rq) if ok else [])
+    return [it if isinstance(it, str) else next(found) for it in items], rq
+
+
+def _find_blocks(dimg, items, rq=None):
     """ops.find_blocks over items (image index, TextPage, rect) of the uploaded images ``dimg``, its tables back through one
-    pinned copy and one synchronisation.  Returns per item dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y), or
-    the error message of a page over a limit."""
+    pinned copy and one synchronisation; a quad page (its corners given) is a level page on all of its rectified crop in ``rq``
+    (_rectify).  Returns per item dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y), or the error message of a
+    page over a limit."""
     from . import ops
     lib = ops._lib
-    res_t, caps = ops.find_blocks([(dimg[i], rect, pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y, pg.skew,
-                                    pg.max_skew) for i, pg, rect in items])
+
+    def src(i, pg, rect):
+        if pg.quad is None:
+            return dimg[i], rect
+        r = rq[_quad_key(i, pg.quad)]
+        return r, (0, 0, r.shape[1], r.shape[0])
+    res_t, caps = ops.find_blocks([(*src(i, pg, rect), pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y,
+                                    pg.skew, pg.max_skew) for i, pg, rect in items])
     host = _to_host(res_t).numpy()
     rdt, ndt, sdt = ops.page_result_dtype(), ops.page_node_dtype(), ops.skew_block_dtype()
     skewed = any(pg.skew is not None for _, pg, _ in items)
@@ -1932,7 +2084,7 @@ def _find_blocks(dimg, items):
         if r["error"] == lib.PAGE_ERR_BLOCKS:
             out.append(f"{int(r['n_blocks'])} blocks exceed the {lib.PAGE_MAX_BLOCKS} a text page may hold")
             continue
-        X0, Y0 = rect[:2]
+        X0, Y0 = (0, 0) if pg.quad is not None else rect[:2]
         vertical = pg.direction == "vertical"
         tilted = pg.skew is not None and sk["s"] != 0
         blocks, rejected = [], []
@@ -1945,7 +2097,11 @@ def _find_blocks(dimg, items):
             (rejected if q["st"] & lib.PAGE_REJECTED else blocks).append(box)
         res = dict(threshold=int(r["threshold"]), ink="dark" if r["ink"] == lib.INK_DARK else "light",
                    text_size=int(r["text_size"]), gap_x=int(r["gap_x"]), gap_y=int(r["gap_y"]))
-        if pg.skew is None:
+        if pg.quad is not None:
+            shape = dimg[i].shape[:2]
+            res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=pg.direction, polarity=pg.polarity, window=b) for b in blocks],
+                       rejected=rejected, quad=_quad_key(i, pg.quad)[1], size=tuple(src(i, pg, rect)[1][2:]))
+        elif pg.skew is None:
             res.update(blocks=[TextBlock(b, pg.direction, polarity=pg.polarity) for b in blocks], rejected=rejected)
         else:
             res["skew"] = _skew_used(pg, sk)
@@ -1972,7 +2128,11 @@ def find_blocks(images, pages):
     A page with ``skew`` (DESIGN.md 7b, "Skewed pages") has its angle searched (or given) on the device and is cut in its
     rotated frame; a call that holds one runs every page through ops.find_blocks' 151 launches.  Its dict gains ``skew``, the
     angle used, and its blocks (and rejected leaves) are windows of that frame, TextBlock(page rect, skew=angle, window=...),
-    or the blocks of skew=None when the angle is exactly 0."""
+    or the blocks of skew=None when the angle is exactly 0.
+    A page with ``quad`` (DESIGN.md 7b, "Perspective pages") is cut as a level page on its rectified crop R (every distinct quad
+    warped in one launch); under "auto" its corners are found first (ops.find_page_quads: 8 launches for every such page, one
+    more pinned copy and synchronisation), and a page without one raises "no page found".  Its dict gains ``quad`` (the corners
+    used) and ``size`` (R's w_r, h_r), and its blocks are TextBlock.from_quad(quad, window=...) windows of R."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
@@ -1988,7 +2148,7 @@ def find_blocks(images, pages):
     _check_page_work(items)
     dev = next((im.device for im in imgs if im.is_cuda), torch.device("cuda", torch.cuda.current_device()))
     with torch.cuda.device(dev):
-        res = _find_blocks(_device_images(sorted({i for i, _, _ in items}), imgs, dev), items)
+        res, _ = _find_pages(_device_images(sorted({i for i, _, _ in items}), imgs, dev), items)
     for (i, _, _), name, r in zip(items, names, res):
         if isinstance(r, str):
             raise ValueError(f"{name}: {r}")
@@ -2243,7 +2403,9 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     may be given for a page; a tilted page (``skew``) gives windowed TextBlocks, which are split as any other.  Its entry is
     dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, skew], regions), regions one
     block entry per block; a page over its node or block limit, or one of whose blocks fails, raises, or is dict(error=...)
-    with ``skip_invalid``, and then none of its blocks is restored."""
+    with ``skip_invalid``, and then none of its blocks is restored.  A quad page or block (DESIGN.md 7b, "Perspective pages")
+    is laid out on its rectified crop (TextPage(quad="auto") after the device's corner search), every distinct quad of the call
+    warped in one launch, and gives QuadRegion lines; a page without a quad found is its error."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     shapes = [im.shape[:2] for im in imgs]
@@ -2257,12 +2419,16 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     names = None
     with torch.cuda.device(dev):
         dimg = _device_images(range(len(imgs)), imgs, dev)
+        rq = {}
         if text_pages:                                   # every page's blocks take its place in the region list
-            found = _find_blocks(dimg, [(i, pg, rect) for i, _, pg, rect in text_pages])
+            found, rq = _find_pages(dimg, [(i, pg, rect) for i, _, pg, rect in text_pages],
+                                    [_quad_key(i, blk.quad) for i, _, blk, _ in blocks if blk.quad is not None])
             regions, labels, boxes, names, page_layout = _expand_pages(regions, labels, boxes, text_pages, found, skip_invalid)
             blocks, _ = _plan_blocks(shapes, regions, labels, boxes)
+        elif any(blk.quad is not None for _, _, blk, _ in blocks):
+            rq = _rectify(dimg, [_quad_key(i, blk.quad) for i, _, blk, _ in blocks if blk.quad is not None])
         if blocks:                                       # every block's lines take its place in the region list
-            found = _find_lines(dimg, [(i, blk, rect) for i, _, blk, rect in blocks])
+            found = _find_lines(dimg, [(i, blk, rect) for i, _, blk, rect in blocks], rq)
             expand = (regions, labels, boxes, blocks)
             regions, labels, boxes, layout = _expand_blocks(*expand, found, skip_invalid, shapes, scale, feather, names)
             drop = _failed_pages(page_layout, layout) if text_pages else None

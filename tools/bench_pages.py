@@ -1,6 +1,6 @@
 """Text pages (DESIGN.md section 7b, "Text pages"): the layout analysis alone and restore_regions with pages.
 
-    MN_MODULE_GRAPHS=0 python tools/bench_pages.py [--pages 4] [--passes 3] [--iters 100] [--scale 2] [--skew]
+    MN_MODULE_GRAPHS=0 python tools/bench_pages.py [--pages 4] [--passes 3] [--iters 100] [--scale 2] [--skew | --quad]
 
 The pages are seeded 1600 x 1200 pages: a heading over two or three columns of capital-letter lines drawn with cv2.putText
 (Hershey DUPLEX) on a light, slightly noisy background, one TextPage each.  Prints one JSON line each for:
@@ -11,6 +11,11 @@ The pages are seeded 1600 x 1200 pages: a heading over two or three columns of c
 With --skew (DESIGN.md section 7b, "Skewed pages") the pages are turned by seeded angles within +-7.5 degrees and searched with
 TextPage(skew="auto"): the layout line times mn_find_blocks_skewed_u8 against the level pages in the same run, and the
 restore_regions arms are the tilted pages against the call given the found lines.
+With --quad (DESIGN.md section 7b, "Perspective pages") each page is photographed: warped by a seeded homography (each corner
+pulled inwards by up to 10% of the page's sides) onto a canvas 120 pixels wider on every side, over a darker textured background,
+and found with TextPage(quad="auto"): the layout line times the corner search (mn_find_page_quads_u8), the warp of the found
+quads and the XY-cut of the rectified crops apart and together (with the host copy of the corners between them), and the
+restore_regions arms are the photographed pages against the call given the found lines.
 Every line carries the card's name and power limit, read in the same run.  Not part of the product path.
 """
 import argparse
@@ -58,6 +63,25 @@ def make_pages(n_pages, seed=0):
     return pages, cols
 
 
+def photograph(pages, seed=2, margin=120):
+    """The pages warped by seeded homographies over darker textured backgrounds: (images, corners tl, tr, br, bl)."""
+    rng = np.random.default_rng(seed)
+    out, corners = [], []
+    for p in pages:
+        h, w = p.shape[:2]
+        a = rng.uniform(0, 0.1, 8) * np.array([w, h] * 4)
+        c = np.float32([[margin + a[0], margin + a[1]], [margin + w - a[2], margin + a[3]],
+                        [margin + w - a[4], margin + h - a[5]], [margin + a[6], margin + h - a[7]]])
+        M = cv2.getPerspectiveTransform(np.float32([[0, 0], [w, 0], [w, h], [0, h]]) - 0.5, c - 0.5)
+        size = (w + 2 * margin, h + 2 * margin)
+        warped = cv2.warpPerspective(p, M, size, flags=cv2.INTER_LINEAR)
+        cover = cv2.warpPerspective(np.full((h, w), 255, np.uint8), M, size, flags=cv2.INTER_NEAREST) > 0
+        bg = cv2.GaussianBlur(rng.integers(80, 150, size[::-1]).astype(np.uint8), (7, 7), 0)[..., None].repeat(3, axis=2)
+        out.append(np.where(cover[..., None], warped, bg))
+        corners.append([[round(float(x), 2), round(float(y), 2)] for x, y in c])
+    return out, corners
+
+
 def _card():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
                        text=True)
@@ -72,6 +96,7 @@ def main():
     ap.add_argument("--iters", type=int, default=100)
     ap.add_argument("--scale", type=int, default=2)
     ap.add_argument("--skew", action="store_true")
+    ap.add_argument("--quad", action="store_true")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_pages.py needs a CUDA device")
@@ -87,7 +112,32 @@ def main():
     if args.skew:
         pages = [cv2.warpAffine(p, cv2.getRotationMatrix2D((p.shape[1] / 2, p.shape[0] / 2), a, 1.0), (p.shape[1], p.shape[0]),
                                 flags=cv2.INTER_LINEAR, borderMode=cv2.BORDER_REPLICATE) for p, a in zip(pages, angles)]
-    page = pipeline.TextPage(skew="auto") if args.skew else pipeline.TextPage()
+    if args.quad:
+        pages, drawn = photograph(pages)
+    page = pipeline.TextPage(skew="auto") if args.skew else pipeline.TextPage(quad="auto") if args.quad else pipeline.TextPage()
+
+    def events_ms(fn):
+        for _ in range(5):
+            fn()
+        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0.record()
+        for _ in range(args.iters):
+            fn()
+        t1.record()
+        t1.synchronize()
+        return t0.elapsed_time(t1) / args.iters
+
+    def quad_layout():
+        d = dict(enumerate(torch.from_numpy(p).to(dev) for p in pages))
+        items = [(i, page, (0, 0, x.shape[1], x.shape[0])) for i, x in d.items()]
+        found = pipeline._page_quads(d, items)
+        keys = [pipeline._quad_key(i, pg.quad) for i, pg, _ in found]
+        rq = pipeline._rectify(d, keys)
+        crops = [(rq[k], (0, 0, rq[k].shape[1], rq[k].shape[0]), False, _lib.INK_AUTO, None, None) for k in keys]
+        times = dict(search_ms=events_ms(lambda: ops.find_page_quads([(x, _lib.INK_AUTO) for x in d.values()])),
+                     warp_ms=events_ms(lambda: pipeline._rectify(d, keys)), xy_cut_ms=events_ms(lambda: ops.find_blocks(crops)),
+                     ms_per_call=events_ms(lambda: pipeline._find_pages(d, items)))
+        return {k: round(v, 4) for k, v in times.items()}, [[list(p) for p in pg.quad] for _, pg, _ in found]
 
     def layout_ms(imgs, skew):
         d = [torch.from_numpy(p).to(dev) for p in imgs]
@@ -102,9 +152,14 @@ def main():
         t1.synchronize()
         return t0.elapsed_time(t1) / args.iters
 
-    ms = layout_ms(pages, "auto" if args.skew else None)
-    found = pipeline.find_blocks(pages, [[page] for _ in pages])
     extra = {}
+    if args.quad:
+        extra, quads = quad_layout()
+        ms = extra.pop("ms_per_call")
+        extra.update(drawn=drawn, found=quads)
+    else:
+        ms = layout_ms(pages, "auto" if args.skew else None)
+    found = pipeline.find_blocks(pages, [[page] for _ in pages])
     if args.skew:
         extra = dict(angles=angles, found=[f[0]["skew"] for f in found], level_ms_per_call=round(layout_ms(level, None), 4))
     print(json.dumps(dict(card, what="layout", pages=len(pages), megapixels=sum(p.shape[0] * p.shape[1] for p in pages) / 1e6,
@@ -119,7 +174,7 @@ def main():
         m.append(net.eval().to(dev))
     blocks = [f[0]["blocks"] for f in found]
     kw = dict(scale=args.scale, skip_invalid=True, to_host=True)
-    if args.skew:
+    if args.skew or args.quad:
         lines = [[q for r in f for q in r["lines"]] for f in pipeline.find_lines(pages, blocks)]
         base = ("found lines", lambda: pipeline.restore_regions(*m, pages, lines, **kw))
     else:
