@@ -2208,13 +2208,17 @@ def _failed_pages(page_layout, block_layout):
     return drop
 
 
+MAX_REGIONS = 65535     # regions of one restore_regions call: each is one grid row (blockIdx.y) of the composite launch
+
+
 def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None):
     """restore_regions' host plan, validated before any launch.  shapes: (H, W) per image; regions: per image, a list of integer
     half-open rectangles (x0, y0, x1, y1) and OrientedRegions; labels / boxes: None, or per image None or a list with one entry
     per region (None: predicted, else the region's labels / its detector boxes [x1, y1, x2, y2], in IMAGE coordinates for a
     rectangle and in the rectified crop's frame for an oriented region).  Returns the RegionPlans of every region, image by
     image in region order.
-    Raises ValueError: scale not an integer in [1, 8], feather < 0, and, naming the image and the region, a rectangle that is
+    Raises ValueError: scale not an integer in [1, 8], feather < 0, more than MAX_REGIONS regions in the call (restore_regions
+    plans again once blocks and pages are split into lines, so lines count too, before any model runs), and, naming the image and the region, a rectangle that is
     empty or leaves the image, an oriented region with corners that are not finite, a side shorter than 1 pixel, mirrored or
     sheared past |e x f| < |e| |f| / 2, its centre outside the image, a crop, restored width or image side over 32767 pixels or
     a page map beyond OpenCV's fixed-point range, a label / box count mismatch, boxes without labels, a box outside the region's
@@ -2237,6 +2241,11 @@ def plan_regions(shapes, regions, labels=None, boxes=None, scale=4, feather=None
     n = len(shapes)
     regions, labels, boxes = (_per_image(v, n, f"{what} (one list per image)") for v, what in
                               ((regions, "regions"), (labels, "labels"), (boxes, "boxes")))
+    regions = [list(r or []) for r in regions]
+    total = sum(len(r) for r in regions)
+    if total > MAX_REGIONS:
+        raise ValueError(f"{total} regions in one call: one composite launch takes at most {MAX_REGIONS} (its grid's y "
+                         f"dimension); split the images over several calls")
     plan = []
     for i, (H, W) in enumerate(shapes):
         rects = list(regions[i] or [])

@@ -9,7 +9,7 @@ import numpy as np
 
 from .oriented_regions import oriented_patch
 from .quad_regions import quad_patch
-from .regions import alpha, background, blend, resized_region
+from .regions import alpha, background, blend, clip_box, compose_window_with, rect_patch, resized_region
 from .remap import remap_cubic_u8
 from .warp_affine import warp_sample_u8
 
@@ -123,7 +123,7 @@ def t_coords(maps, m, t, b, t_hw):
     return xq, yq
 
 
-def curved_footprint(t_shape, region, s, page_hw, feather):
+def curved_footprint(t_shape, region, s, page_hw, feather, window=None):
     """Where a curved region whose restored bytes have shape t_shape = (128, W_T, ...) lands on an image of page_hw = (H, W)
     output pixels at scale s: (box, xq, yq, mask, alpha) over pipeline.curved_footprint_box, with page pixel (X, Y) inverted at
     q = ((X + 0.5)/s, (Y + 0.5)/s), the footprint mask (a root accepted and -16 <= Xq < 32 W_T - 16, -16 <= Yq < 32 H_T - 16)
@@ -132,6 +132,10 @@ def curved_footprint(t_shape, region, s, page_hw, feather):
     th, tw = t_shape[:2]
     m = curved_maps(region, s, tw, th)
     box = curved_footprint_box(region, s, page_hw)
+    if window is not None:
+        box = clip_box(box, window)
+        if box is None:
+            return (None,) * 5
     xs, ys = np.arange(box[0], box[2], dtype=np.float64), np.arange(box[1], box[3], dtype=np.float64)
     qx = np.broadcast_to(((xs + 0.5) / s)[None, :], (len(ys), len(xs)))
     qy = np.broadcast_to(((ys + 0.5) / s)[:, None], (len(ys), len(xs)))
@@ -156,10 +160,12 @@ def feather_alpha(xq, yq, t_hw, kx, ky, feather):
     return np.minimum(f32(1), np.divide(np.minimum(du, dv), f32(feather), dtype=f32))
 
 
-def curved_patch(t, region, s, page_hw, feather):
+def curved_patch(t, region, s, page_hw, feather, window=None):
     """curved_footprint's (box, P, alpha, mask) for the restored bytes t (cv2.imwrite order), P = remap's cubic sample of
     t[..., ::-1] at the fixed-point T coordinates."""
-    box, xq, yq, mask, a = curved_footprint(t.shape, region, s, page_hw, feather)
+    box, xq, yq, mask, a = curved_footprint(t.shape, region, s, page_hw, feather, window)
+    if box is None:
+        return (None,) * 4
     return box, warp_sample_u8(np.ascontiguousarray(t[..., ::-1]), xq, yq), a, mask
 
 
@@ -185,3 +191,17 @@ def compose(img, rects, srs, s, feather):
         sl = out[r[1]:r[3], r[0]:r[2]]
         out[r[1]:r[3], r[0]:r[2]] = blend(sl, p, alpha(r, out.shape[:2], feather))
     return out
+
+
+def window_patch(t, rect, s, page_hw, feather, window):
+    """The (box, P, alpha, mask) of any region compose takes, inside ``window`` (oracle.regions.compose_window_with)."""
+    from marconet_b200.pipeline import CurvedRegion, OrientedRegion, QuadRegion
+    patch = curved_patch if isinstance(rect, CurvedRegion) else quad_patch if isinstance(rect, QuadRegion) else \
+        oriented_patch if isinstance(rect, OrientedRegion) else rect_patch
+    return patch(t, rect, s, page_hw, feather, window)
+
+
+def compose_window(background_window, origin, page_hw, rects, srs, s, feather):
+    """compose over one window of the page, every coordinate the page's own: background_window holds the page bytes at origin =
+    (column, row) of a page of page_hw = (H, W) output pixels (oracle.regions.compose_window_with)."""
+    return compose_window_with(window_patch, background_window, origin, page_hw, rects, srs, s, feather)

@@ -36,17 +36,19 @@ def cubic_coeffs(x):
     return np.array([c0, c1, c2, c3], dtype=np.float32)
 
 
+def taps_at(ds, scale):
+    """tap_tables for the destination indices ds only: (ofs, taps) int64 [n], [n, 4]."""
+    ds = np.asarray(ds, np.int64)
+    f = ((ds + 0.5) * scale - 0.5).astype(np.float32)       # double arithmetic, then (float)
+    s = np.floor(f)                                         # cvFloor
+    f = np.subtract(f, s, dtype=np.float32)
+    taps = np.rint(cubic_coeffs(f) * np.float32(COEF_SCALE)).astype(np.int64).T   # saturate_cast<short> = cvRound
+    return s.astype(np.int64), taps.reshape(len(ds), 4)
+
+
 def tap_tables(dst, scale):
     """Per destination index: first source index - 1 ... and the four 11-bit fixed-point taps (xofs/ialpha, yofs/ibeta)."""
-    ofs = np.zeros(dst, np.int64)
-    taps = np.zeros((dst, 4), np.int64)
-    for d in range(dst):
-        f = np.float32((d + 0.5) * scale - 0.5)            # double arithmetic, then (float)
-        s = int(np.floor(f))                                # cvFloor
-        f = np.float32(f - np.float32(s))
-        ofs[d] = s
-        taps[d] = np.rint(cubic_coeffs(f) * np.float32(COEF_SCALE)).astype(np.int64)   # saturate_cast<short> = cvRound
-    return ofs, taps
+    return taps_at(np.arange(dst), scale)
 
 
 def dsize_for(h, w, fx, fy):
@@ -81,6 +83,42 @@ def resize_cubic_u8(img, fx, fy):
     nvec = (dw * cn // SIMD_LANES) * SIMD_LANES
     out[:, :nvec] = vec.reshape(dh, dw * cn)[:, :nvec]
     return out.reshape(dh, dw, cn)
+
+
+def resize_cubic_rows(img, dsize, rows, cols=None, split_shift=0):
+    """Destination rows ``rows`` (and columns ``cols``, default all) of cv2.resize(img, dsize, interpolation=INTER_CUBIC) for a
+    uint8 HWC image, dsize = (dw, dh), computed without the rest of the destination: the dsize form's scales 1/((double)dw/w)
+    and 1/((double)dh/h), and the vector body / fixed-point tail split decided by the element's index in the full destination
+    row (the first floor(dw*cn/8)*8 elements are the vector body).  ``split_shift`` moves that split (negative controls only).
+    Returns uint8 [len(rows), len(cols), cn]."""
+    h, w, cn = img.shape
+    dw, dh = dsize
+    rows = np.asarray(rows, np.int64)
+    cols = np.arange(dw) if cols is None else np.asarray(cols, np.int64)
+    xo, xa = taps_at(cols, 1.0 / (dw / w))
+    yo, ya = taps_at(rows, 1.0 / (dh / h))
+    xi = [np.clip(xo + j - 1, 0, w - 1) for j in range(4)]
+    nvec = (dw * cn // SIMD_LANES) * SIMD_LANES + split_shift
+    vec_el = (cols[:, None] * cn + np.arange(cn)[None, :]) < nvec          # [len(cols), cn]
+    scale = np.float32(1.0) / np.float32(COEF_SCALE * COEF_SCALE)
+    out = np.empty((len(rows), len(cols), cn), np.uint8)
+    step = max(1, (1 << 22) // (4 * max(len(cols), w) * cn))               # rows per chunk: bounded int64 buffers
+    for r0 in range(0, len(rows), step):
+        sl = slice(r0, r0 + step)
+        yy = np.clip(yo[sl, None] + np.arange(4)[None, :] - 1, 0, h - 1)   # [n, 4] source rows
+        src = img[yy.reshape(-1)].astype(np.int64)                          # [n*4, w, cn]
+        hb = sum(src[:, xi[j], :] * xa[:, j][None, :, None] for j in range(4)).reshape(len(yy), 4, len(cols), cn)
+        beta = ya[sl]
+        fixed = sum(hb[:, j] * beta[:, j, None, None] for j in range(4))
+        fixed = np.clip((fixed + (1 << (2 * COEF_BITS - 1))) >> (2 * COEF_BITS), 0, 255)
+        bf = (beta.astype(np.float32) * scale)[:, :, None, None]
+        rf = hb.astype(np.float32)
+        acc = rf[:, 3] * bf[:, 3]
+        for k in (2, 1, 0):
+            acc = rf[:, k] * bf[:, k] + acc                                 # fp32 multiply, fp32 add (no FMA)
+        vec = np.clip(np.rint(acc), 0, 255)
+        out[sl] = np.where(vec_el[None], vec, fixed).astype(np.uint8)
+    return out
 
 
 def preprocess_lq(img, out_h=32, out_w=512):

@@ -5,7 +5,7 @@ all four sides; rectangles composed exactly as oracle.regions composes them.
 TEST INFRASTRUCTURE ONLY."""
 import numpy as np
 
-from .regions import alpha, background, blend, resized_region
+from .regions import alpha, background, blend, clip_box, compose_window_with, rect_patch, resized_region
 from .warp_affine import warp_affine_cubic_u8, warp_coords, warp_sample_u8
 
 
@@ -17,7 +17,7 @@ def rectify(img, region):
     return warp_affine_cubic_u8(img, m.matrix, m.size)
 
 
-def oriented_footprint(t_shape, region, s, page_hw, feather):
+def oriented_footprint(t_shape, region, s, page_hw, feather, window=None):
     """Where an oriented region whose restored bytes have shape t_shape = (128, W_T, ...) lands on an image of page_hw = (H, W)
     output pixels at scale s: (box, xq, yq, mask, alpha) over the footprint's bounding box (X0, Y0, X1, Y1) -- cv2.warpAffine's
     fixed-point T coordinates (xq, yq) of every pixel of the box under N, the footprint mask -16 <= Xq < 32 W_T - 16,
@@ -27,6 +27,10 @@ def oriented_footprint(t_shape, region, s, page_hw, feather):
     th, tw = t_shape[:2]
     m = oriented_maps(region, s, tw)
     box = footprint_box(region, m, s, page_hw)
+    if window is not None:
+        box = clip_box(box, window)
+        if box is None:
+            return (None,) * 5
     xq, yq = warp_coords(m.page_map, np.arange(box[0], box[2]), np.arange(box[1], box[3]))
     mask = (xq >= -16) & (xq < 32 * tw - 16) & (yq >= -16) & (yq < 32 * th - 16)
     if feather == 0:
@@ -39,10 +43,12 @@ def oriented_footprint(t_shape, region, s, page_hw, feather):
     return box, xq, yq, mask, np.minimum(f32(1), np.divide(np.minimum(du, dv), f32(feather), dtype=f32))
 
 
-def oriented_patch(t, region, s, page_hw, feather):
+def oriented_patch(t, region, s, page_hw, feather, window=None):
     """oriented_footprint's (box, P, alpha, mask) for the restored bytes t (cv2.imwrite order), with P = cv2.warpAffine(
     t[..., ::-1], N, (W, H), INTER_CUBIC | WARP_INVERSE_MAP, BORDER_REPLICATE) over the box."""
-    box, xq, yq, mask, a = oriented_footprint(t.shape, region, s, page_hw, feather)
+    box, xq, yq, mask, a = oriented_footprint(t.shape, region, s, page_hw, feather, window)
+    if box is None:
+        return (None,) * 4
     return box, warp_sample_u8(np.ascontiguousarray(t[..., ::-1]), xq, yq), a, mask
 
 
@@ -66,3 +72,16 @@ def compose(img, rects, srs, s, feather):
         sl = out[r[1]:r[3], r[0]:r[2]]
         out[r[1]:r[3], r[0]:r[2]] = blend(sl, p, alpha(r, out.shape[:2], feather))
     return out
+
+
+def window_patch(t, rect, s, page_hw, feather, window):
+    """The (box, P, alpha, mask) of any region compose takes, inside ``window`` (oracle.regions.compose_window_with)."""
+    from marconet_b200.pipeline import OrientedRegion
+    patch = oriented_patch if isinstance(rect, OrientedRegion) else rect_patch
+    return patch(t, rect, s, page_hw, feather, window)
+
+
+def compose_window(background_window, origin, page_hw, rects, srs, s, feather):
+    """compose over one window of the page, every coordinate the page's own: background_window holds the page bytes at origin =
+    (column, row) of a page of page_hw = (H, W) output pixels (oracle.regions.compose_window_with)."""
+    return compose_window_with(window_patch, background_window, origin, page_hw, rects, srs, s, feather)
