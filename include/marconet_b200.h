@@ -738,6 +738,49 @@ typedef struct {
 int mn_find_lines_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, int n, long long max_tiles, void* work, long long work_bytes,
                             void* stream);
 
+/* Curled text blocks (DESIGN.md section 7b, "Curled blocks").  Block i is a horizontal crop b (h x w) cut into n_strips column
+ * strips [x_j, x_{j+1}), x_j = j w / n_strips, each at least 32 pixels wide when n_strips > 1.  mn_find_lines_curved_u8 issues
+ * seven launches for every block of a call, whatever the number of blocks and strips:
+ *   1-4. mn_find_lines_u8's histogram, threshold, profile and segmentation over blocks[] (the lines of curve=None into b.out);
+ *   5. strip profiles over 32 x 32 tiles: sprof[(3 j + q) h + y], q = 0 the ink count of row y in strip j, q = 1 w - its least
+ *      ink column, q = 2 its largest ink column + 1 (0 where the row has no ink in the strip);
+ *   6. strip runs, one CTA per (strip, block): steps 1-3 of mn_find_lines_u8's segmentation on strip j's count with the strip's
+ *      width as M; the kept runs into runs[(j MN_CURVE_RUN_CAP + k) 4 ..] as (a, b, least ink column, largest ink column) and
+ *      their number into nruns[j] (minus it when it exceeds MN_CURVE_RUN_CAP, then no run is written);
+ *   7. link, one CTA per block: strip by strip, a run continues the line whose last run overlaps it most (rows
+ *      min(b, b') - max(a, a') > 0; ties to the least last a, then the least line) when that line's largest overlap in the strip
+ *      is this run (ties to the upper run); other runs start lines; a line whose last run lies more than MN_CURVE_MAX_GAP strips
+ *      back is closed.  Lines of fewer than (n_strips + 3) / 4 runs are dropped, the rest ordered by (their first run's a, line)
+ *      into cout: header = (status, n_lines, Hm, strip, count, 0, 0, 0), Hm the lower median of the kept runs' heights, and per
+ *      line (first strip, last strip, runs, least ink column, largest ink column, sample mask, 0, 0, then (a_j, b_j) for
+ *      j < MN_CURVE_MAX_STRIPS, (-1, -1) without a run); bit j of the mask is set when 2 (b_j - a_j) <= 3 Hm.  status is
+ *      MN_CURVE_ERR_RUNS (strip `strip` holds `count` runs) or MN_CURVE_ERR_LINES (`count` lines) over a limit.
+ * hist, b.prof, sprof and nruns lie in work (work_bytes, zeroed by the call); b.scratch (2 h + 4), sscratch (n_strips (2 h + 4)),
+ * runs and link (n_strips MN_CURVE_RUN_CAP 7 int32) need no zeroing.  max_tiles >= every block's tile count, max_strips >= every
+ * n_strips.  blocks[i] and curves[i].b are the same crop record (vertical = 0).  blocks, curves: DEVICE arrays. */
+#define MN_CURVE_MAX_STRIPS 32
+#define MN_CURVE_RUN_CAP 256
+#define MN_CURVE_MAX_GAP 2
+#define MN_CURVE_LINE_INTS (8 + 2 * MN_CURVE_MAX_STRIPS)
+#define MN_CURVE_ERR_RUNS 1
+#define MN_CURVE_ERR_LINES 2
+typedef struct {
+    int32_t header[8];
+    int32_t line[MN_BLOCK_MAX_LINES][MN_CURVE_LINE_INTS];
+} mn_curve_lines;
+typedef struct {
+    mn_text_block b;            /* the crop record: hist, prof, scratch and out as mn_find_lines_u8's */
+    int32_t* sprof;             /* 3 n_strips h */
+    int32_t* nruns;             /* n_strips */
+    int32_t* runs;              /* n_strips MN_CURVE_RUN_CAP 4 */
+    int32_t* sscratch;          /* n_strips (2 h + 4) */
+    int32_t* link;              /* n_strips MN_CURVE_RUN_CAP 7 */
+    mn_curve_lines* cout;
+    int32_t n_strips, pad;
+} mn_curve_block;
+int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* curves, int n, long long max_tiles, int max_strips,
+                            void* work, long long work_bytes, void* stream);
+
 /* Text pages: blocks found by a recursive XY-cut (DESIGN.md section 7b, "Text pages").  Page i is the crop of blocks[i] (h x w,
  * vertical = a vertical page) and pages[i] holds the same record in pages[i].b.  A node is a rectangle of the crop and the axis
  * it tries next; each level runs one attempt on every open node of every page.  mn_find_blocks_u8 issues

@@ -178,6 +178,20 @@ class WindowBlock(Structure):
                 ("l1", c_int32), ("px0", c_int32), ("py0", c_int32), ("pw", c_int32), ("ph", c_int32)]
 
 
+CURVE_MAX_STRIPS, CURVE_RUN_CAP, CURVE_MAX_GAP = 32, 256, 2        # MN_CURVE_MAX_STRIPS, MN_CURVE_RUN_CAP, MN_CURVE_MAX_GAP
+CURVE_LINE_INTS = 8 + 2 * CURVE_MAX_STRIPS
+CURVE_ERR_RUNS, CURVE_ERR_LINES = 1, 2
+
+
+class CurveLines(Structure):
+    _fields_ = [("header", c_int32 * 8), ("line", c_int32 * (BLOCK_MAX_LINES * CURVE_LINE_INTS))]
+
+
+class CurveBlock(Structure):
+    _fields_ = [("b", TextBlock), ("sprof", c_void_p), ("nruns", c_void_p), ("runs", c_void_p), ("sscratch", c_void_p),
+                ("link", c_void_p), ("cout", c_void_p), ("n_strips", c_int32), ("pad", c_int32)]
+
+
 PAGE_LEVELS, PAGE_MAX_BLOCKS, PAGE_MAX_NODES = 24, 1024, 65536    # MN_PAGE_LEVELS, MN_PAGE_MAX_BLOCKS, MN_PAGE_MAX_NODES
 PAGE_REJECTED = 8                                                  # MN_PAGE_REJECTED
 PAGE_ERR_NODES, PAGE_ERR_BLOCKS = 1, 2
@@ -273,6 +287,7 @@ SYMBOLS = {
     "mn_find_blocks_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_blocks_skewed_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_window_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
+    "mn_find_lines_curved_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_int, c_void_p, c_longlong, c_void_p]),
     "mn_find_page_quads_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),

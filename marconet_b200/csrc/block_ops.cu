@@ -6,6 +6,8 @@
 // blocks by a level-synchronous XY-cut over an ink bitmap.  Skewed pages (DESIGN.md 7b, "Skewed pages") run the same XY-cut on a
 // bitmap of rotated-frame cells, and their blocks are windows of that frame.  Perspective pages (DESIGN.md 7b, "Perspective
 // pages") find a photographed page's corners: the paper's largest 4-connected component, its hull and the largest quad on it.
+// Curled blocks (DESIGN.md 7b, "Curled blocks") trace each line across column strips: per-strip profiles and runs, and a
+// left-to-right link of the runs into lines, in seven launches.
 #include "mn_common.cuh"
 
 namespace {
@@ -137,7 +139,7 @@ __global__ void __launch_bounds__(kTileThreads) block_profile_kernel(const mn_te
 }
 
 // Exclusive prefix sum of v over the CTA; *total receives the sum.  s holds 32 ints.
-__device__ int cta_scan(int v, int* s, int* total) {
+__device__ __forceinline__ int cta_scan(int v, int* s, int* total) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
     int x = v;
 #pragma unroll
@@ -276,6 +278,311 @@ __global__ void __launch_bounds__(kSegThreads) block_lines_kernel(const mn_text_
         }
     }
     if (threadIdx.x == 0) b.out->n_lines = nk;
+}
+
+// ---- Curled blocks (DESIGN.md 7b, "Curled blocks") ----
+// Integer only, as the twin (oracle/curled_blocks.py).  A strip is at least 32 pixels wide (or the only one), so the 32 columns
+// of a tile fall in at most two strips.
+constexpr int kLinkThreads = 1024;
+constexpr int kLinkActive = (MN_CURVE_MAX_GAP + 1) * MN_CURVE_RUN_CAP;   // lines whose last run lies in the last 3 strips
+static_assert(kLinkActive + MN_CURVE_RUN_CAP <= kLinkThreads, "one link candidate per thread");
+
+__device__ __forceinline__ int strip_of(int x, int w, int n_s) { return ((x + 1) * n_s - 1) / w; }   // largest j, x_j <= x
+
+// Per tile and per row: the ink count, w - least ink column and largest ink column + 1 in each of the (at most) two strips the
+// tile's columns fall in, gathered in shared memory and added with one atomic per non-zero entry.
+__global__ void __launch_bounds__(kTileThreads) curve_profile_kernel(const mn_curve_block* __restrict__ curves) {
+    mn_pdl_prologue();
+    __shared__ int s_cnt[2][kTile], s_lo[2][kTile], s_hi[2][kTile];
+    const mn_curve_block cb = curves[blockIdx.y];
+    const mn_text_block& b = cb.b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    const int t = b.out->threshold;
+    const bool dark = b.out->ink == MN_INK_DARK;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int x = tx + lane, j0 = strip_of(tx, b.w, cb.n_strips);
+    const int q = x < b.w ? strip_of(x, b.w, cb.n_strips) - j0 : 0;
+    for (int r = 0; r < kTile / 8; ++r) {
+        const int y = ty + warp + 8 * r;
+        bool ink = false;
+        if (x < b.w && y < b.h) {
+            const int g = block_grey(b, x, y);
+            ink = dark ? g <= t : g > t;
+        }
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+            const bool in = ink && q == s;
+            const int c = __reduce_add_sync(0xffffffffu, in ? 1 : 0);
+            const unsigned l = __reduce_max_sync(0xffffffffu, in ? (unsigned)(b.w - x) : 0u);
+            const unsigned h = __reduce_max_sync(0xffffffffu, in ? (unsigned)(x + 1) : 0u);
+            if (lane == 0) {
+                s_cnt[s][warp + 8 * r] = c;
+                s_lo[s][warp + 8 * r] = (int)l;
+                s_hi[s][warp + 8 * r] = (int)h;
+            }
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < 2 * kTile) {
+        const int s = threadIdx.x / kTile, r = threadIdx.x % kTile;
+        if (s_cnt[s][r]) {
+            int* p = cb.sprof + (long long)3 * (j0 + s) * b.h + ty + r;
+            atomicAdd(p, s_cnt[s][r]);
+            atomicMax(p + b.h, s_lo[s][r]);
+            atomicMax(p + 2 * b.h, s_hi[s][r]);
+        }
+    }
+}
+
+// Steps 1-3 of block_lines_kernel on the row profile of strip blockIdx.x of block blockIdx.y; the kept runs, unpadded, with
+// their least and largest ink column.
+__global__ void __launch_bounds__(kSegThreads) curve_runs_kernel(const mn_curve_block* __restrict__ curves) {
+    mn_pdl_prologue();
+    __shared__ int s_scan[32];
+    __shared__ int s_a[MN_CURVE_RUN_CAP], s_b[MN_CURVE_RUN_CAP];
+    const mn_curve_block cb = curves[blockIdx.y];
+    const mn_text_block& b = cb.b;
+    const int j = blockIdx.x;
+    if (j >= cb.n_strips) return;
+    const int L = b.h, M = (j + 1) * b.w / cb.n_strips - j * b.w / cb.n_strips;
+    const int* cnt = cb.sprof + (long long)3 * j * L;
+    const int m = b.min_ink > 0 ? b.min_ink : max(1, M / 128);
+    const int half = (L + 2) / 2;
+    int* ra = cb.sscratch + (long long)j * (2 * L + 4);
+    int* rb = ra + half;
+    int* ma = rb + half;
+    int* mb = ma + half;
+    int total;
+    {
+        const int chunk = (L + blockDim.x - 1) / blockDim.x, l0 = threadIdx.x * chunk, l1 = min(L, l0 + chunk);
+        int c = 0;
+        for (int l = l0; l < l1; ++l) {
+            if (cnt[l] < m) continue;
+            c += (l == 0 || cnt[l - 1] < m) ? 1 : 0;
+            c += (l + 1 == L || cnt[l + 1] < m) ? 1 << 16 : 0;
+        }
+        int o = cta_scan(c, s_scan, &total);
+        int os = o & 0xffff, oe = o >> 16;
+        for (int l = l0; l < l1; ++l) {
+            if (cnt[l] < m) continue;
+            if (l == 0 || cnt[l - 1] < m) ra[os++] = l;
+            if (l + 1 == L || cnt[l + 1] < m) rb[oe++] = l + 1;
+        }
+    }
+    const int n = total & 0xffff;
+    if (n == 0) {
+        if (threadIdx.x == 0) cb.nruns[j] = 0;
+        return;
+    }
+    __syncthreads();
+    const int G = b.gap > 0 ? b.gap : max(1, cta_lower_median(ra, rb, n, L, s_scan) / 4);
+    int nm;
+    {
+        const int chunk = (n + blockDim.x - 1) / blockDim.x, j0 = threadIdx.x * chunk, j1 = min(n, j0 + chunk);
+        int c = 0;
+        for (int k = j0; k < j1; ++k) c += k == 0 || ra[k] - rb[k - 1] > G;
+        int g = cta_scan(c, s_scan, &nm) - 1;
+        for (int k = j0; k < j1; ++k) {
+            if (k == 0 || ra[k] - rb[k - 1] > G) ma[++g] = ra[k];
+            if (k + 1 == n || ra[k + 1] - rb[k] > G) mb[g] = rb[k];
+        }
+    }
+    __syncthreads();
+    const int mh = b.min_height > 0 ? b.min_height : max(2, cta_lower_median(ma, mb, nm, L, s_scan) / 3);
+    int nk;
+    {
+        const int chunk = (nm + blockDim.x - 1) / blockDim.x, j0 = threadIdx.x * chunk, j1 = min(nm, j0 + chunk);
+        int c = 0;
+        for (int k = j0; k < j1; ++k) c += mb[k] - ma[k] >= mh;
+        int k = cta_scan(c, s_scan, &nk);
+        if (nk > MN_CURVE_RUN_CAP) {
+            if (threadIdx.x == 0) cb.nruns[j] = -nk;
+            return;
+        }
+        for (int e = j0; e < j1; ++e) {
+            if (mb[e] - ma[e] < mh) continue;
+            s_a[k] = ma[e];
+            s_b[k++] = mb[e];
+        }
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int k = warp; k < nk; k += blockDim.x >> 5) {
+        int lo = 0, hi = 0;
+        for (int l = s_a[k] + lane; l < s_b[k]; l += 32) {
+            lo = max(lo, cnt[L + l]);
+            hi = max(hi, cnt[2 * L + l]);
+        }
+        lo = (int)__reduce_max_sync(0xffffffffu, (unsigned)lo);
+        hi = (int)__reduce_max_sync(0xffffffffu, (unsigned)hi);
+        if (lane == 0) {
+            int* r = cb.runs + ((long long)j * MN_CURVE_RUN_CAP + k) * 4;
+            r[0] = s_a[k]; r[1] = s_b[k]; r[2] = b.w - lo; r[3] = hi - 1;
+        }
+    }
+    if (threadIdx.x == 0) cb.nruns[j] = nk;
+}
+
+__device__ __forceinline__ int run_overlap(int a, int b, int a2, int b2) { return min(b, b2) - max(a, a2); }
+
+// The link of one block: strip by strip, every run of the strip and every open line in parallel (one thread each), the new
+// lines numbered in run order with a CTA scan; then the kept lines ranked, the median run height and the table.
+__global__ void __launch_bounds__(kLinkThreads) curve_link_kernel(const mn_curve_block* __restrict__ curves) {
+    mn_pdl_prologue();
+    __shared__ int s_scan[32];
+    __shared__ int s_act[kLinkActive];
+    __shared__ int s_best[MN_CURVE_RUN_CAP];
+    __shared__ int s_err;
+    const mn_curve_block& cb = curves[blockIdx.x];      // read in place: a copy would not fit the 64 registers of 1024 threads
+    const int n_s = cb.n_strips, cap = n_s * MN_CURVE_RUN_CAP, tid = threadIdx.x;
+    int* hd = cb.cout->header;
+    // per line: last strip, last run's a and b, runs, first run's a, its best run in the strip (then its rank, -1: dropped);
+    // per (strip, run): its line.  One base pointer: seven would not fit the 64 registers of 1024 threads.
+    int* lk = cb.link;
+#define last_j(l) lk[(l)]
+#define last_a(l) lk[cap + (l)]
+#define last_b(l) lk[2 * cap + (l)]
+#define count(l) lk[3 * cap + (l)]
+#define first_a(l) lk[4 * cap + (l)]
+#define rank(l) lk[5 * cap + (l)]
+#define run_line(e) lk[6 * cap + (e)]
+    if (tid == 0) {
+        s_err = -1;
+        for (int j = 0; j < n_s && s_err < 0; ++j) {
+            if (cb.nruns[j] < 0) s_err = j;
+        }
+        if (s_err >= 0) {
+            hd[0] = MN_CURVE_ERR_RUNS; hd[1] = 0; hd[2] = 0; hd[3] = s_err; hd[4] = -cb.nruns[s_err];
+            hd[5] = hd[6] = hd[7] = 0;
+        }
+    }
+    __syncthreads();
+    if (s_err >= 0) return;
+    int n_lines = 0, n_act = 0;
+    for (int j = 0; j < n_s; ++j) {
+        const int R = cb.nruns[j];
+        const int* runs = cb.runs + (long long)j * MN_CURVE_RUN_CAP * 4;
+        if (tid < R) {                                  // this run's line
+            const int a = runs[4 * tid], e = runs[4 * tid + 1];
+            int best = -1, bo = 0, ba = 0;
+            for (int q = 0; q < n_act; ++q) {
+                const int l = s_act[q], la = last_a(l), o = run_overlap(a, e, la, last_b(l));
+                if (o > bo || (o == bo && o > 0 && (la < ba || (la == ba && l < best)))) {
+                    best = l; bo = o; ba = la;
+                }
+            }
+            s_best[tid] = best;
+        }
+        if (tid < n_act) {                              // this line's run
+            const int l = s_act[tid], la = last_a(l), lb = last_b(l);
+            int best = -1, bo = 0;
+            for (int k = 0; k < R; ++k) {
+                const int o = run_overlap(runs[4 * k], runs[4 * k + 1], la, lb);
+                if (o > bo) { best = k; bo = o; }
+            }
+            rank(l) = best;
+        }
+        __syncthreads();
+        const int l = tid < R ? s_best[tid] : -1;
+        const bool cont = l >= 0 && rank(l) == tid;
+        int fresh;
+        const int id = n_lines + cta_scan(tid < R && !cont ? 1 : 0, s_scan, &fresh);
+        if (tid < R) {
+            const int a = runs[4 * tid], e = runs[4 * tid + 1], dst = cont ? l : id;
+            last_j(dst) = j; last_a(dst) = a; last_b(dst) = e;
+            count(dst) = cont ? count(dst) + 1 : 1;
+            if (!cont) first_a(dst) = a;
+            run_line(j * MN_CURVE_RUN_CAP + tid) = dst;
+        }
+        __syncthreads();
+        // the lines open for strip j + 1: the open ones, then the new ones, whose last run lies at most MN_CURVE_MAX_GAP back
+        const int cand = tid < n_act ? s_act[tid] : tid < n_act + fresh ? n_lines + tid - n_act : -1;
+        const bool keep = cand >= 0 && last_j(cand) >= j - MN_CURVE_MAX_GAP;
+        int n_next;
+        const int o = cta_scan(keep ? 1 : 0, s_scan, &n_next);
+        if (keep) s_act[o] = cand;
+        n_lines += fresh;
+        n_act = n_next;
+        __syncthreads();
+    }
+    // drop the short lines, rank the rest by (first run's a, line)
+    const int need = (n_s + 3) / 4;
+    int kept = 0;
+    for (int l = tid; l < n_lines; l += blockDim.x) {
+        if (count(l) < need) {
+            rank(l) = -1;
+            continue;
+        }
+        ++kept;
+        int r = 0;
+        for (int m = 0; m < n_lines; ++m) {
+            r += count(m) >= need && (first_a(m) < first_a(l) || (first_a(m) == first_a(l) && m < l));
+        }
+        rank(l) = r;
+    }
+    int n_kept;
+    cta_scan(kept, s_scan, &n_kept);
+    if (n_kept > MN_BLOCK_MAX_LINES) {
+        if (tid == 0) {
+            hd[0] = MN_CURVE_ERR_LINES; hd[1] = 0; hd[2] = 0; hd[3] = 0; hd[4] = n_kept;
+            hd[5] = hd[6] = hd[7] = 0;
+        }
+        return;
+    }
+    // Hm: the lower median of the kept runs' heights, by bisection over [1, h]
+    const int n_all = n_s * MN_CURVE_RUN_CAP;
+    int n_runs = 0;
+    for (int e = tid; e < n_all; e += blockDim.x) {
+        const int j = e / MN_CURVE_RUN_CAP, k = e % MN_CURVE_RUN_CAP;
+        n_runs += k < cb.nruns[j] && rank(run_line(e)) >= 0;
+    }
+    int total;
+    cta_scan(n_runs, s_scan, &total);
+    int lo = 1, hi = cb.b.h;
+    while (total && lo < hi) {
+        const int mid = lo + (hi - lo) / 2;
+        int c = 0, below;
+        for (int e = tid; e < n_all; e += blockDim.x) {
+            const int j = e / MN_CURVE_RUN_CAP, k = e % MN_CURVE_RUN_CAP;
+            if (k < cb.nruns[j] && rank(run_line(e)) >= 0) c += cb.runs[4 * e + 1] - cb.runs[4 * e] <= mid;
+        }
+        cta_scan(c, s_scan, &below);
+        if (below > (total - 1) / 2) hi = mid; else lo = mid + 1;
+    }
+    const int med = total ? lo : 0;
+    for (int e = tid; e < n_kept * MN_CURVE_LINE_INTS; e += blockDim.x) {
+        const int f = e % MN_CURVE_LINE_INTS;
+        cb.cout->line[e / MN_CURVE_LINE_INTS][f] = f == 0 ? MN_CURVE_MAX_STRIPS : f == 3 ? 0x7fffffff : f >= 6 && f < 8 ? 0 :
+                                                    f == 5 ? 0 : -1;
+    }
+    __syncthreads();
+    for (int l = tid; l < n_lines; l += blockDim.x) {
+        if (rank(l) >= 0) cb.cout->line[rank(l)][2] = count(l);
+    }
+    for (int e = tid; e < n_all; e += blockDim.x) {
+        const int j = e / MN_CURVE_RUN_CAP, k = e % MN_CURVE_RUN_CAP;
+        if (k >= cb.nruns[j] || rank(run_line(e)) < 0) continue;
+        const int* r = cb.runs + 4 * e;
+        int* row = cb.cout->line[rank(run_line(e))];
+        row[8 + 2 * j] = r[0];
+        row[9 + 2 * j] = r[1];
+        atomicMin(&row[0], j);
+        atomicMax(&row[1], j);
+        atomicMin(&row[3], r[2]);
+        atomicMax(&row[4], r[3]);
+        if (2 * (r[1] - r[0]) <= 3 * med) atomicOr(&row[5], 1 << j);
+    }
+    if (tid == 0) {
+        hd[0] = 0; hd[1] = n_kept; hd[2] = med; hd[3] = hd[4] = hd[5] = hd[6] = hd[7] = 0;
+    }
+#undef last_j
+#undef last_a
+#undef last_b
+#undef count
+#undef first_a
+#undef rank
+#undef run_line
 }
 
 // ---- Skewed blocks (DESIGN.md 7b, "Skewed blocks") ----
@@ -1444,6 +1751,26 @@ extern "C" int mn_find_page_quads_u8(const mn_text_block* blocks, const mn_quad_
     MN_CUDA_CHECK((mn_launch(quad_rows_kernel, grid, dim3(kTileThreads), 0, st, pages)));
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(quad_hull_kernel, dim3(n), dim3(kHullThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* curves, int n, long long max_tiles,
+                                       int max_strips, void* work, long long work_bytes, void* stream) {
+    MN_REQUIRE(blocks && curves && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && max_strips >= 1 &&
+               max_strips <= MN_CURVE_MAX_STRIPS && work && work_bytes > 0, "mn_find_lines_curved_u8: bad args");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int rc = block_threshold(blocks, n, max_tiles, work, work_bytes, st);
+    if (rc != MN_OK) return rc;
+    MN_CUDA_CHECK((mn_launch(block_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, blocks)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(block_lines_kernel, dim3(n), dim3(kSegThreads), 0, st, blocks)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(curve_profile_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, curves)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(curve_runs_kernel, dim3((unsigned)max_strips, n), dim3(kSegThreads), 0, st, curves)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(curve_link_kernel, dim3(n), dim3(kLinkThreads), 0, st, curves)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -1809,6 +1809,97 @@ def find_lines_window(blocks):
     return buf[:n * osz]
 
 
+CURVE_MAX_STRIPS = _lib.CURVE_MAX_STRIPS
+CURVE_MIN_STRIP = 32           # pixels of a strip when there are several: a 32-pixel tile then spans at most two strips
+CURVE_MAX_WORK = 1 << 30       # bytes of device memory the curled blocks of one find_lines call may use
+
+
+def curve_strips(w, strips=None):
+    """n_s of a curled block w pixels wide (DESIGN.md 7b, "Curled blocks"): ``strips``, or clamp(w // 48, 1, 32):
+    strips 48 to 95 pixels wide, in which a line that climbs one pixel in five still rises less than the gap between lines."""
+    return int(strips) if strips is not None else min(CURVE_MAX_STRIPS, max(1, w // 48))
+
+
+def _curve_ints(h, n_s):
+    """(work, scratch) int32 values of one curled block: the zeroed histogram, profile, strip profiles and run counts; then the
+    segmentation scratch of the block and of each strip, the run table and the link state."""
+    return 256 + 3 * h + 3 * n_s * h + n_s, (2 * h + 4) * (1 + n_s) + 11 * _lib.CURVE_RUN_CAP * n_s
+
+
+def curve_block_bytes(w, h, strips=None):
+    """Device bytes of one curled block of w x h pixels in a find_lines_curved call: its records, work and scratch."""
+    work, scratch = _curve_ints(h, curve_strips(w, strips))
+    return 4 * (work + scratch) + sum(ctypes.sizeof(t) for t in (_lib.BlockLines, _lib.CurveLines, _lib.TextBlock, _lib.CurveBlock))
+
+
+def curve_lines_dtype():
+    """numpy view of an mn_curve_lines record (the link table of mn_find_lines_curved_u8)."""
+    import numpy as np
+    return np.dtype([("header", "<i4", (8,)), ("lines", "<i4", (_lib.BLOCK_MAX_LINES, _lib.CURVE_LINE_INTS))])
+
+
+def find_lines_curved(blocks, tables=False):
+    """Curled text blocks traced line by line across column strips, every block in seven launches whatever the number of blocks
+    and strips (mn_find_lines_curved_u8; DESIGN.md 7b, "Curled blocks").  blocks: list of (img, rect, polarity, min_ink, gap,
+    min_height, strips): as find_lines' horizontal blocks, strips a positive integer or None for the default (curve_strips), at
+    most CURVE_MAX_STRIPS and each strip at least CURVE_MIN_STRIP pixels wide when there are several.  Returns the uint8 CUDA
+    tensor of the n mn_block_lines records (the lines of curve=None) followed by the n mn_curve_lines records
+    (``curve_lines_dtype()``).  ``tables`` (tests): also return per block dict(profiles, nruns, runs), int32 CUDA views of its strip
+    profiles [n_s, 3, h], run counts [n_s] and run table [n_s, CURVE_RUN_CAP, 4].  Raises ValueError naming the block, before
+    any launch, for a call whose blocks need more than CURVE_MAX_WORK bytes."""
+    global LAUNCHES
+    dev = _check_items(blocks, "find_lines_curved", "block")
+    n = len(blocks)
+    osz, csz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.CurveLines)
+    rsz, bsz = ctypes.sizeof(_lib.TextBlock), ctypes.sizeof(_lib.CurveBlock)
+    dims, total = [], 0
+    for i, blk in enumerate(blocks):
+        what = f"find_lines_curved: block {i}"
+        x0, y0, bw, bh = _check_crop((blk[0], blk[1], False, *blk[2:6]), dev, what, "min_ink / gap / min_height")
+        strips = blk[6]
+        n_s = curve_strips(bw, strips)
+        if not 1 <= n_s <= CURVE_MAX_STRIPS or (n_s > 1 and bw // n_s < CURVE_MIN_STRIP):
+            raise ValueError(f"{what}: {n_s} strips of a {bw}-pixel block: at most {CURVE_MAX_STRIPS}, each at least "
+                             f"{CURVE_MIN_STRIP} pixels wide")
+        total += curve_block_bytes(bw, bh, strips)
+        if total > CURVE_MAX_WORK:
+            raise ValueError(f"{what}: the blocks up to this one need {total} bytes, over the {CURVE_MAX_WORK} a call may use")
+        dims.append((x0, y0, bw, bh, n_s))
+    sizes = [_curve_ints(d[3], d[4]) for d in dims]
+    n_work, n_scr = sum(s[0] for s in sizes), sum(s[1] for s in sizes)
+    head = n * (osz + csz + rsz + bsz)
+    buf = torch.empty(head + 4 * (n_work + n_scr), dtype=torch.uint8, device=dev)
+    base = buf.data_ptr()
+    seg, crec, work = base + n * (osz + csz), base + n * (osz + csz + rsz), base + head
+    recs, crecs, views, w, s, tiles = [], [], [], 0, n_work, 0
+    cap = _lib.CURVE_RUN_CAP
+    for i, (blk, (x0, y0, bw, bh, n_s)) in enumerate(zip(blocks, dims)):
+        img, _, polarity, min_ink, gap, min_height, _ = blk
+        hist, prof, sprof, nruns = w, w + 256, w + 256 + 3 * bh, w + 256 + 3 * bh + 3 * n_s * bh
+        scr, sscr = s, s + 2 * bh + 4
+        runs = sscr + n_s * (2 * bh + 4)
+        link = runs + 4 * cap * n_s
+        tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, 0, polarity, min_ink or 0, gap or 0, min_height or 0,
+                            0, work + 4 * hist, work + 4 * prof, work + 4 * scr, base + i * osz)
+        recs.append(tb)
+        crecs.append(_lib.CurveBlock(tb, work + 4 * sprof, work + 4 * nruns, work + 4 * runs, work + 4 * sscr, work + 4 * link,
+                                     base + n * osz + i * csz, n_s))
+        if tables:
+            i32 = buf[head:].view(torch.int32)
+            views.append(dict(profiles=i32[sprof:sprof + 3 * n_s * bh].view(n_s, 3, bh), nruns=i32[nruns:nruns + n_s],
+                              runs=i32[runs:runs + 4 * cap * n_s].view(n_s, cap, 4)))
+        w += sizes[i][0]
+        s += sizes[i][1]
+        tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
+    host = bytes((_lib.TextBlock * n)(*recs)) + bytes((_lib.CurveBlock * n)(*crecs))
+    buf[n * (osz + csz):head].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    _lib.check(_lib.load().mn_find_lines_curved_u8(seg, crec, n, tiles, max(d[4] for d in dims), work, 4 * n_work, _stream()),
+               "mn_find_lines_curved_u8")
+    LAUNCHES += 7
+    res = buf[:n * (osz + csz)]
+    return (res, views) if tables else res
+
+
 PAGE_MAX_WORK = 1 << 30        # bytes of device memory one find_blocks call may use
 
 

@@ -1552,7 +1552,9 @@ class TextBlock(NamedTuple):
     that angle; the block is then the pixels of ``rect`` whose cell lies in it.  find_blocks gives a tilted page's blocks so.
     ``quad`` (DESIGN.md 7b, "Perspective pages"): a QuadRegion, a block seen in perspective whose lines are found on the quad's
     rectified crop R (quad_maps' w_r x h_r) and come back as QuadRegions; ``rect`` is then the quad's pixel box (build the
-    block with from_quad), ``skew`` is None and ``window``, if given, is an integer rectangle (x0, y0, x1, y1) of R."""
+    block with from_quad), ``skew`` is None and ``window``, if given, is an integer rectangle (x0, y0, x1, y1) of R.
+    ``curve`` (DESIGN.md 7b, "Curled blocks"): None, or "auto" to trace each line of a curled horizontal block across ``strips``
+    column strips (a positive integer, only with "auto"; default clamp(w // 48, 1, 32)) and return it as a CurvedRegion."""
     rect: object
     direction: str = "horizontal"
     min_ink: object = None
@@ -1563,6 +1565,8 @@ class TextBlock(NamedTuple):
     max_skew: float = 10.0
     window: object = None
     quad: object = None
+    curve: object = None
+    strips: object = None
 
     @classmethod
     def from_quad(cls, quad, shape=None, **kw):
@@ -1602,6 +1606,7 @@ def _check_block(blk, H, W, name):
         v = getattr(blk, what)
         if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 1 <= v < 2 ** 31):
             raise ValueError(f"{name}: {what} must be a positive integer, got {v!r}")
+    _check_curve(blk.curve, blk.strips, blk, x1 - x0, name)
     sk, ms = blk.skew, blk.max_skew
     auto = isinstance(sk, str) and sk == "auto"
     if not (sk is None or auto or (isinstance(sk, numbers.Real) and not isinstance(sk, bool) and math.isfinite(sk)
@@ -1643,6 +1648,44 @@ def _check_block(blk, H, W, name):
             raise ValueError(f"{name}: window {(c0, l0, c1, l1)} is empty or outside the {int(M[0])}x{int(L[0])} frame of the "
                              f"block at skew {sk!r}")
     return x0, y0, x1, y1
+
+
+def _check_curve(curve, strips, item, w, name):
+    """The curve knobs of a TextBlock or TextPage ``item`` of width w, validated (DESIGN.md 7b, "Curled blocks").  Raises
+    ValueError naming ``name``."""
+    from . import ops
+    auto = isinstance(curve, str) and curve == "auto"
+    if not (curve is None or auto):
+        raise ValueError(f"{name}: curve must be None or 'auto', got {curve!r}")
+    if strips is not None:
+        if isinstance(strips, bool) or not isinstance(strips, int) or strips < 1:
+            raise ValueError(f"{name}: strips must be a positive integer, got {strips!r}")
+        if not auto:
+            raise ValueError(f"{name}: strips is given, but curve is {curve!r}, not 'auto'")
+    if not auto:
+        return
+    for what in ("skew", "window", "quad"):
+        if getattr(item, what, None) is not None:
+            raise ValueError(f"{name}: curve and {what} are both given (curled blocks are level: {what} together with curve is "
+                             f"not supported)")
+    if item.direction == "vertical":
+        raise ValueError(f"{name}: curve is given for a vertical block (curled columns are not supported)")
+    if strips is not None and (strips > ops.CURVE_MAX_STRIPS or strips > 1 and w // strips < ops.CURVE_MIN_STRIP):
+        raise ValueError(f"{name}: {strips} strips of a {w}-pixel block: at most {ops.CURVE_MAX_STRIPS} strips, each at least "
+                         f"{ops.CURVE_MIN_STRIP} pixels wide")
+
+
+def _check_curve_work(items, names):
+    """Refuse, before any launch, curled blocks (image index, TextBlock, rect) whose work memory, added up in order, passes the
+    limit of one call: the error names the block that passes it."""
+    from . import ops
+    total = 0
+    for (_, blk, rect), name in zip(items, names):
+        if blk.curve is not None:
+            total += ops.curve_block_bytes(rect[2] - rect[0], rect[3] - rect[1], blk.strips)
+            if total > ops.CURVE_MAX_WORK:
+                raise ValueError(f"{name}: the call's curled blocks up to this one need {total} bytes of work memory, over the "
+                                 f"{ops.CURVE_MAX_WORK} a call may use (split the call)")
 
 
 def _check_quad(quad, skew, H, W, name):
@@ -1702,7 +1745,8 @@ def _find_lines(dimg, items, rq=None):
     copy and one synchronisation; a quad block is a level block on the window of its rectified crop in ``rq`` (_rectify).
     Returns per item dict(lines, threshold, ink), or the error message of a block with too many lines."""
     from . import ops
-    plain = [it for it in items if it[1].window is None or it[1].quad is not None]
+    curled = [it for it in items if it[1].curve is not None]
+    plain = [it for it in items if (it[1].window is None or it[1].quad is not None) and it[1].curve is None]
     wins = [it for it in items if it[1].window is not None and it[1].quad is None]
 
     def src(i, blk, rect):
@@ -1717,16 +1761,26 @@ def _find_lines(dimg, items, rq=None):
     if wins:
         parts.append(ops.find_lines_window([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap,
                                              blk.min_height, blk.skew, blk.window) for i, blk, rect in wins]))
+    if curled:
+        parts.append(ops.find_lines_curved([(dimg[i], rect, _INK[blk.polarity], blk.min_ink, blk.gap, blk.min_height, blk.strips)
+                                            for i, blk, rect in curled]))
     host = _to_host(torch.cat(parts) if len(parts) > 1 else parts[0]).numpy()
-    ldt = ops.block_lines_dtype()
+    ldt, cdt = ops.block_lines_dtype(), ops.curve_lines_dtype()
+    n_csz = len(curled) * (ldt.itemsize + cdt.itemsize)
+    host, chost = host[:len(host) - n_csz], host[len(host) - n_csz:]
     n_osz, n_wsz = len(plain) * ldt.itemsize, len(wins) * ldt.itemsize
     table = host[:n_osz].view(ldt)
     skew = host[n_osz:len(host) - n_wsz].view(ops.skew_block_dtype()) if len(host) > n_osz + n_wsz else [None] * len(plain)
     found = dict(zip(map(id, plain), zip(table, skew)))
     found.update((id(it), (t, None)) for it, t in zip(wins, host[len(host) - n_wsz:].view(ldt)))
+    ctab = chost[len(curled) * ldt.itemsize:].view(cdt)
+    found.update((id(it), (t, c)) for it, t, c in zip(curled, chost[:len(curled) * ldt.itemsize].view(ldt), ctab))
     out = []
     for it in items:
         (i, blk, rect), (t, sk) = it, found[id(it)]
+        if blk.curve is not None:
+            out.append(_curled_result(rect, blk, t, sk))
+            continue
         n = int(t["n_lines"])
         if n < 0:
             out.append(f"{-n} lines exceed the {ops._lib.BLOCK_MAX_LINES} a text block may hold")
@@ -1785,6 +1839,92 @@ def skew_lines(rect, vertical, c, s, u_min, v_min, frame_lines):
     return out[::-1] if vertical else out
 
 
+def _bezier_1d(p, t):
+    """De Casteljau's value of the cubic with control values p at t, every operation rounded on its own."""
+    s = 1.0 - t
+    a0, a1, a2 = s * p[0] + t * p[1], s * p[1] + t * p[2], s * p[2] + t * p[3]
+    b0, b1 = s * a0 + t * a1, s * a1 + t * a2
+    return s * b0 + t * b1
+
+
+def curve_lines(rect, strips, table, level_lines=None):
+    """The lines of a curled block (DESIGN.md 7b, "Curled blocks") from its link table (one row per line, as
+    mn_find_lines_curved_u8 writes it), in plain Python and numpy fp64; the numpy twin calls this function as it is.  Returns
+    (lines, curve): lines the CurvedRegions top to bottom, or ``level_lines`` (the rectangles of curve=None, or None when that
+    segmentation failed) when the block is level; curve = dict(strips=n_s, samples), samples per line the (x, a, b) it was
+    fitted to, x a strip centre and a, b the run's top and bottom edge, all in image coordinates.
+    The block is level when ``level_lines`` has as many lines as the table and rectangle k holds the rows of every run of line
+    k (integer comparisons only): curve=None already separates its lines.  Otherwise, per line, in this order: the samples are
+    the strips whose bit is set in the sample mask, or all of its strips when none is; H = the lower median of their heights
+    b - a, p = (H + 3) // 4; the span [X0, X1] = [max(0, xmin - p), min(w, xmax + 1 + p)]; t_j = ((x_j + x_{j+1}) / 2 - X0) /
+    (X1 - X0); the least-squares polynomial of degree d = min(3, n - 1) in t through the mid points (t_j, 0.5 (a_j + b_j))
+    (numpy.linalg.lstsq), zero-padded to four coefficients c and turned into Bernstein form m = (c0, c0 + c1 / 3,
+    c0 + 2 c1 / 3 + c2 / 3, c0 + c1 + c2 + c3); the top and bottom edges are m - H / 2 and m + H / 2 (a band of even height:
+    each strip's ascenders and descenders move its own a and b by a few pixels, its mid point by half as much).  Each edge
+    moves out by p, cut for each pair of neighbours to half the least gap between the upper line's bottom edge and the lower
+    line's top edge at 33 evenly spaced x over their common span (0 when they cross); the control points sit at
+    x = x0 + X0 + (X1 - X0) k / 3, k = 0 .. 3."""
+    import numpy as np
+    x0, y0, x1, _ = rect
+    w = x1 - x0
+    xb = [j * w // strips for j in range(strips + 1)]
+    fits, samples = [], []
+    for row in table:
+        js = [j for j in range(int(row[0]), int(row[1]) + 1) if row[8 + 2 * j] >= 0]
+        sj = [j for j in js if int(row[5]) >> j & 1] or js
+        a, b = [float(row[8 + 2 * j]) for j in sj], [float(row[9 + 2 * j]) for j in sj]
+        hs = sorted(int(row[9 + 2 * j]) - int(row[8 + 2 * j]) for j in sj)
+        p = (hs[(len(hs) - 1) // 2] + 3) // 4
+        X0, X1 = max(0, int(row[3]) - p), min(w, int(row[4]) + 1 + p)
+        t = np.array([((xb[j] + xb[j + 1]) / 2 - X0) / (X1 - X0) for j in sj], np.float64)
+        d = min(3, len(sj) - 1)
+        coef = np.zeros(4, np.float64)
+        coef[:d + 1] = np.linalg.lstsq(np.stack([t ** k for k in range(d + 1)], axis=1),
+                                       np.array([0.5 * (u + v) for u, v in zip(a, b)], np.float64), rcond=None)[0]
+        c0, c1, c2, c3 = (float(v) for v in coef)
+        mid = (c0, c0 + c1 / 3, c0 + 2 * c1 / 3 + c2 / 3, c0 + c1 + c2 + c3)
+        half = 0.5 * hs[(len(hs) - 1) // 2]
+        fits.append((X0, X1, tuple(v - half for v in mid), tuple(v + half for v in mid), p))
+        samples.append(tuple((x0 + (xb[j] + xb[j + 1]) / 2, y0 + a[k], y0 + b[k]) for k, j in enumerate(sj)))
+    curve = dict(strips=strips, samples=samples)
+    if level_lines is not None and len(level_lines) == len(table) and all(
+            level_lines[k][1] <= y0 + row[8 + 2 * j] and y0 + row[9 + 2 * j] <= level_lines[k][3]
+            for k, row in enumerate(table) for j in range(int(row[0]), int(row[1]) + 1) if row[8 + 2 * j] >= 0):
+        return list(level_lines), curve
+    pt, pb = [f[4] for f in fits], [f[4] for f in fits]
+    for k in range(len(fits) - 1):
+        (X0, X1, _, bot, _), (Y0, Y1, top, _, _) = fits[k], fits[k + 1]
+        lo, hi = max(X0, Y0), min(X1, Y1)
+        if lo >= hi:
+            continue
+        xs = [lo + (hi - lo) * i / 32 for i in range(33)]
+        g = min(_bezier_1d(top, (x - Y0) / (Y1 - Y0)) - _bezier_1d(bot, (x - X0) / (X1 - X0)) for x in xs)
+        cut = max(0.0, g / 2)
+        pb[k], pt[k + 1] = min(pb[k], cut), min(pt[k + 1], cut)
+    lines = []
+    for (X0, X1, top, bot, _), up, down in zip(fits, pt, pb):
+        xs = [x0 + X0 + (X1 - X0) * k / 3 for k in range(4)]
+        lines.append(CurvedRegion(tuple((x, y0 + v - up) for x, v in zip(xs, top)),
+                                  tuple((x, y0 + v + down) for x, v in zip(xs, bot))))
+    return lines, curve
+
+
+def _curled_result(rect, blk, t, c):
+    """find_lines' dict of a curled block from its mn_block_lines record ``t`` (the lines of curve=None) and its mn_curve_lines
+    record ``c``, or its error message."""
+    from . import ops
+    lib = ops._lib
+    hd = [int(v) for v in c["header"]]
+    if hd[0] == lib.CURVE_ERR_RUNS:
+        return f"strip {hd[3]} has {hd[4]} line runs, over the {lib.CURVE_RUN_CAP} a strip may hold"
+    if hd[0] == lib.CURVE_ERR_LINES:
+        return f"{hd[4]} lines exceed the {lib.BLOCK_MAX_LINES} a text block may hold"
+    n = int(t["n_lines"])
+    level = [tuple(int(v) for v in q) for q in t["rect"][:n]] if n >= 0 else None
+    lines, curve = curve_lines(rect, ops.curve_strips(rect[2] - rect[0], blk.strips), c["lines"][:hd[1]], level)
+    return dict(lines=lines, threshold=int(t["threshold"]), ink="dark" if t["ink"] == lib.INK_DARK else "light", curve=curve)
+
+
 @torch.no_grad()
 def find_lines(images, blocks):
     """The lines of text blocks (DESIGN.md 7b, "Text blocks"): Otsu's threshold of each block's grey crop, the ink's row profile
@@ -1802,7 +1942,10 @@ def find_lines(images, blocks):
     angle used in degrees, and its lines are OrientedRegions (VerticalRegions of OrientedRegions for a vertical block), or the
     rectangles of skew=None when the angle is exactly 0.  A block with ``quad`` (DESIGN.md 7b, "Perspective pages") is split
     as a level block on its window of the quad's rectified crop (every distinct quad of the call warped in one launch), and its
-    lines are QuadRegions (VerticalRegions of QuadRegions for a vertical block)."""
+    lines are QuadRegions (VerticalRegions of QuadRegions for a vertical block).  A block with ``curve="auto"`` (DESIGN.md 7b,
+    "Curled blocks") has each line traced across column strips on the device (every such block of the call in
+    ops.find_lines_curved's seven launches) and fitted on the host (curve_lines): its lines are CurvedRegions top to bottom, or
+    the rectangles of curve=None when every fitted edge is level, and its dict gains ``curve``."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     blocks = _per_image(blocks, len(imgs), "blocks (one list per image)")
     items, names = [], []
@@ -1812,6 +1955,7 @@ def find_lines(images, blocks):
             if not isinstance(blk, TextBlock):
                 raise ValueError(f"{names[-1]}: expected a TextBlock, got {blk!r}")
             items.append((i, blk, _check_block(blk, im.shape[0], im.shape[1], names[-1])))
+    _check_curve_work(items, names)
     out = [[] for _ in imgs]
     if not items:
         return out
@@ -1897,7 +2041,7 @@ def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid, shapes=N
         err = f"{name}: {res}" if isinstance(res, str) else None
         try:
             for k, q in enumerate(res["lines"] if err is None else []):
-                if isinstance(q, (OrientedRegion, QuadRegion)) or isinstance(q, VerticalRegion) and \
+                if isinstance(q, (OrientedRegion, QuadRegion, CurvedRegion)) or isinstance(q, VerticalRegion) and \
                         isinstance(q.shape, (OrientedRegion, QuadRegion)):
                     try:
                         plan_regions([shapes[i]], [[q]], None, None, scale, feather)
@@ -1938,7 +2082,8 @@ class TextPage(NamedTuple):
     (DESIGN.md 7b, "Skewed pages"): as a TextBlock's; a tilted page's blocks are found in its rotated frame.  ``quad``
     (DESIGN.md 7b, "Perspective pages"): None, a QuadRegion (the page's corners tl, tr, br, bl as it is read) or "auto" (the
     corners are found on the device); its blocks are found on the quad's rectified crop R and are TextBlock.from_quad(quad,
-    window=...) windows of R.  With a quad, ``rect`` and ``skew`` are None."""
+    window=...) windows of R.  With a quad, ``rect`` and ``skew`` are None.  ``curve`` (DESIGN.md 7b, "Curled blocks"): None, or
+    "auto" for a level horizontal page whose blocks are TextBlock(..., curve="auto"), each line traced as a CurvedRegion."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
@@ -1947,6 +2092,7 @@ class TextPage(NamedTuple):
     skew: object = None
     max_skew: float = 10.0
     quad: object = None
+    curve: object = None
 
 
 def _check_page(pg, H, W, name):
@@ -1970,6 +2116,7 @@ def _check_page(pg, H, W, name):
     except (TypeError, ValueError):
         raise ValueError(f"{name}: a text page is None or an integer rectangle (x0, y0, x1, y1), got {pg.rect!r}") from None
     _check_block(TextBlock((x0, y0, x1, y1), pg.direction, polarity=pg.polarity, skew=pg.skew, max_skew=pg.max_skew), H, W, name)
+    _check_curve(pg.curve, None, pg, x1 - x0, name)
     for what in ("gap_x", "gap_y"):
         v = getattr(pg, what)
         if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 1 <= v < 2 ** 31):
@@ -2102,7 +2249,7 @@ def _find_blocks(dimg, items, rq=None):
             res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=pg.direction, polarity=pg.polarity, window=b) for b in blocks],
                        rejected=rejected, quad=_quad_key(i, pg.quad)[1], size=tuple(src(i, pg, rect)[1][2:]))
         elif pg.skew is None:
-            res.update(blocks=[TextBlock(b, pg.direction, polarity=pg.polarity) for b in blocks], rejected=rejected)
+            res.update(blocks=[TextBlock(b, pg.direction, polarity=pg.polarity, curve=pg.curve) for b in blocks], rejected=rejected)
         else:
             res["skew"] = _skew_used(pg, sk)
             res["blocks"] = [TextBlock(tuple(rect), pg.direction, polarity=pg.polarity, skew=res["skew"], window=b) if tilted
@@ -2132,7 +2279,8 @@ def find_blocks(images, pages):
     A page with ``quad`` (DESIGN.md 7b, "Perspective pages") is cut as a level page on its rectified crop R (every distinct quad
     warped in one launch); under "auto" its corners are found first (ops.find_page_quads: 8 launches for every such page, one
     more pinned copy and synchronisation), and a page without one raises "no page found".  Its dict gains ``quad`` (the corners
-    used) and ``size`` (R's w_r, h_r), and its blocks are TextBlock.from_quad(quad, window=...) windows of R."""
+    used) and ``size`` (R's w_r, h_r), and its blocks are TextBlock.from_quad(quad, window=...) windows of R.  A page with
+    ``curve="auto"`` (DESIGN.md 7b, "Curled blocks") is cut as any level page, and its blocks are TextBlock(..., curve="auto")."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
@@ -2405,7 +2553,9 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     may be given for a block.  Its entry is dict(lines, threshold, ink, regions), regions one entry per line as above; a block
     of more than 256 lines, or with a vertical line vertical_plan rejects, raises, or is dict(error=...) with ``skip_invalid``.
     A skewed block (DESIGN.md 7b, "Skewed blocks") takes the place of its OrientedRegion lines alike, and its entry gains
-    ``skew``; a line plan_regions rejects makes the block's error.
+    ``skew``; a line plan_regions rejects makes the block's error.  A curled block (DESIGN.md 7b, "Curled blocks") takes the
+    place of its CurvedRegion lines alike (every curled block of the call in ops.find_lines_curved's seven launches), and its
+    entry gains ``curve``; a line plan_regions' curved rules reject makes the block's error.
     A TextPage (DESIGN.md 7b, "Text pages") is split into blocks on the uploaded images first (find_blocks: every page of the
     call in the same launches, one pinned copy and one synchronisation), its TextBlocks take its place, and each of them is then
     replaced by its lines as above, so the result is byte for byte that of the call given the found blocks.  No labels or boxes
@@ -2420,6 +2570,8 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     shapes = [im.shape[:2] for im in imgs]
     text_pages, given = _plan_pages(shapes, regions, labels, boxes)
     blocks, stand_in = _plan_blocks(shapes, given if text_pages else regions, labels, boxes)
+    _check_curve_work([(i, blk, rect) for i, _, blk, rect in blocks], [f"image {i}, region {r} (a text block)"
+                                                                       for i, r, _, _ in blocks])
     plan = plan_regions(shapes, stand_in if blocks or text_pages else regions, labels, boxes, scale, feather)
     feather = 2 * scale if feather is None else feather
     if not imgs:
@@ -2434,6 +2586,7 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
                                     [_quad_key(i, blk.quad) for i, _, blk, _ in blocks if blk.quad is not None])
             regions, labels, boxes, names, page_layout = _expand_pages(regions, labels, boxes, text_pages, found, skip_invalid)
             blocks, _ = _plan_blocks(shapes, regions, labels, boxes)
+            _check_curve_work([(i, blk, rect) for i, _, blk, rect in blocks], [names[(i, r)] for i, r, _, _ in blocks])
         elif any(blk.quad is not None for _, _, blk, _ in blocks):
             rq = _rectify(dimg, [_quad_key(i, blk.quad) for i, _, blk, _ in blocks if blk.quad is not None])
         if blocks:                                       # every block's lines take its place in the region list
