@@ -2037,13 +2037,15 @@ def quad_page_bytes(w, h):
             + sum(_quad_areas(w, h)))
 
 
-def find_page_quads(pages, hulls=False):
+def find_page_quads(pages, hulls=False, labels=False):
     """Page corners (mn_find_page_quads_u8; DESIGN.md 7b, "Perspective pages"), every image of the call in 8 launches whatever
     their number.  pages: list of (img, polarity): img a uint8 [H, W, 3] CUDA view with dense pixels (any row stride), H, W <=
     32767, read in place whole; polarity _lib.INK_AUTO / INK_DARK / INK_LIGHT (paper is grey <= t for INK_LIGHT, else grey > t).
     Returns the uint8 CUDA tensor of the pages' mn_page_quad records, in order (read it back as ``page_quad_dtype()``).
     ``hulls`` (tests): also return, per page, the int32 [4 H + 8, 2] CUDA view of its hull stack, whose first n_hull rows are
-    the hull."""
+    the hull.  ``labels`` (tests): also return, per page, the int32 CUDA views of its compressed labels [H, W] (each paper pixel's
+    component root, the smallest raster index y W + x of the component; -1 elsewhere) and pixel counts [H W] (a component's
+    size at its root, 0 elsewhere)."""
     global LAUNCHES
     dev = _check_items(pages, "find_page_quads", "page")
     n = len(pages)
@@ -2057,7 +2059,7 @@ def find_page_quads(pages, hulls=False):
     areas = [_quad_areas(img.shape[1], img.shape[0]) for img, _ in pages]
     buf = torch.empty(work0 + sum(map(sum, areas)), dtype=torch.uint8, device=dev)
     base = buf.data_ptr()
-    blocks, recs, views, w, tiles = [], [], [], base + work0, 0
+    blocks, recs, views, lviews, w, tiles = [], [], [], [], base + work0, 0
     for i, ((img, polarity), sizes) in enumerate(zip(pages, areas)):
         h_, w_ = img.shape[:2]
         hist, lines, best, ext, label, count, hull = itertools.accumulate([w] + sizes[:-1])
@@ -2065,6 +2067,8 @@ def find_page_quads(pages, hulls=False):
         blocks.append(tb)
         recs.append(_lib.QuadPage(tb, label, count, ext, best, hull, base + out0 + i * rsz))
         views.append(buf[hull - base:hull - base + sizes[-1]].view(torch.int32).view(-1, 2))
+        lviews.append((buf[label - base:label - base + 4 * h_ * w_].view(torch.int32).view(h_, w_),
+                       buf[count - base:count - base + 4 * h_ * w_].view(torch.int32)))
         w += sum(sizes)
         tiles = max(tiles, -(-w_ // 32) * -(-h_ // 32))
     host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.QuadPage * n)(*recs))
@@ -2073,7 +2077,8 @@ def find_page_quads(pages, hulls=False):
                "mn_find_page_quads_u8")
     LAUNCHES += 8
     res = buf[out0:out0 + n * rsz]
-    return (res, views) if hulls else res
+    out = (res,) + ((views,) if hulls else ()) + ((lviews,) if labels else ())
+    return out if len(out) > 1 else res
 
 
 def page_quad_dtype():

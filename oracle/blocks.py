@@ -17,7 +17,12 @@ def grey(crop):
 def otsu(g):
     """cv2.threshold(g, 0, 255, THRESH_BINARY | THRESH_OTSU)[0] for 8-bit values g: OpenCV's fp64 loop over the 256-bin
     histogram, every operation rounded on its own.  Returns an int."""
-    h = np.bincount(np.asarray(g, np.int64).reshape(-1), minlength=256).tolist()
+    return otsu_hist(np.bincount(np.asarray(g, np.int64).reshape(-1), minlength=256))
+
+
+def otsu_hist(hist):
+    """OpenCV's Otsu loop on a 256-bin histogram of pixel counts (any integer sequence): the threshold of the pixels it counts."""
+    h = [int(v) for v in hist]
     scale = 1.0 / float(sum(h))
     mu = 0.0
     for i in range(256):

@@ -98,6 +98,53 @@ def _segment(r, lo, hi, L, M, min_ink, gap, min_height):
     return out
 
 
+def find_lines_banded(band, h, w, origin=(0, 0), direction="horizontal", min_ink=None, gap=None, min_height=None,
+                      polarity="auto", rows=512):
+    """oracle/blocks.find_lines of an h x w block too large to hold as one int64 grey array (a 32767 x 32767 block on a device
+    page, say).  band(y0, y1) returns the block's rows [y0, y1) as a uint8 [y1 - y0, w, 3] array; origin is the block's (x0, y0)
+    in its image.  The histogram is built band by band, then Otsu's threshold and the polarity; then, band by band again, each
+    line's ink count r and its least and largest ink index along the line; steps 4 to 9 are _segment's.  Returns dict(lines,
+    threshold, ink) as blocks.find_lines does, or raises its ValueError."""
+    def grey(y0):
+        c = band(y0, min(h, y0 + rows)).astype(np.uint16)
+        return (c[..., 0] + c[..., 1] + c[..., 2] + 1) // 3
+    hist = np.zeros(256, np.int64)
+    for y0 in range(0, h, rows):
+        hist += np.bincount(grey(y0).reshape(-1), minlength=256)
+    t = B.otsu_hist(hist)
+    if polarity == "auto":
+        polarity = "dark" if 2 * int(hist[:t + 1].sum()) <= h * w else "light"
+    vertical = direction == "vertical"
+    L, M = (w, h) if vertical else (h, w)
+    r = np.zeros(L, np.int64)
+    lo = np.full(L, np.iinfo(np.int64).max)
+    hi = np.full(L, -1)
+    for y0 in range(0, h, rows):
+        g = grey(y0)
+        ink = g <= t if polarity == "dark" else g > t
+        ax = 0 if vertical else 1                     # the axis along the line
+        has = ink.any(axis=ax)
+        first = np.argmax(ink, axis=ax)
+        last = ink.shape[ax] - 1 - np.argmax(np.flip(ink, axis=ax), axis=ax)
+        if vertical:
+            first, last = first + y0, last + y0
+            r += ink.sum(axis=0)
+            lo = np.where(has, np.minimum(lo, first), lo)
+            hi = np.where(has, np.maximum(hi, last), hi)
+        else:
+            y1 = y0 + len(g)
+            r[y0:y1] = ink.sum(axis=1)
+            lo[y0:y1] = np.where(has, first, lo[y0:y1])
+            hi[y0:y1] = np.where(has, last, hi[y0:y1])
+    x0, y0 = origin
+    fl = _segment(r, lo, hi, L, M, min_ink, gap, min_height)
+    if vertical:
+        lines = [(x0 + l0, y0 + c0, x0 + l1, y0 + c1) for c0, l0, c1, l1 in fl][::-1]
+    else:
+        lines = [(x0 + c0, y0 + l0, x0 + c1, y0 + l1) for c0, l0, c1, l1 in fl]
+    return dict(lines=lines, threshold=t, ink=polarity)
+
+
 def corners(line, c, s, u_min, v_min, O):
     """Frame line (c0, l0, c1, l1) -> its (tl, tr, bl) in the crop's frame coordinates around O: a = u_min - 0.5 + c,
     b = v_min - 0.5 + l, e = (c, -s), f = (s, c), p = O + a e + b f, in fp64."""
