@@ -896,6 +896,44 @@ typedef struct {
 int mn_find_page_quads_u8(const mn_text_block* blocks, const mn_quad_page* pages, int n, long long max_tiles, void* work,
                           long long work_bytes, void* stream);
 
+/* Flat pages (DESIGN.md section 7b, "Flat pages"): the dewarp field of a curled page, built from its traced lines, composed with
+ * the page's frame and sampled from the photo.  A page's line table (built on the host, pipeline.flat_line_table) holds
+ * MN_FLAT_LINE_DOUBLES fp64 values per line, sorted by anchor Y (ties in reading order): xs, xe, mu_0 .. mu_3, Y, bx0, bx1.
+ * mn_flat_columns_batched: blockIdx.y = page, one thread per frame column x (centre xc = x + 0.5).  For every line k whose
+ * block holds x (bx0 <= x < bx1), in table order, it writes (Y_k, m_k(x)) to field[(x * stride + n) * 2 ..], n counting up,
+ * with m_k(x) the de Casteljau value of mu at t = clamp(fl(fl(xc - xs) / fl(xe - xs)), 0, 1); then cols[x] = n,
+ * cols[dw + x] = the nearest column left of x that some line's block holds (-1: none) and cols[2 dw + x] the nearest one right
+ * of it (-1: none).  The host sizes stride as the most lines any column meets (at most MN_FLAT_MAX_COLUMN_LINES).
+ * mn_flat_remap_u8_batched: blockIdx.y = page, one thread per pixel (x, y) of the [dh][dw][cn] flat page, yc = y + 0.5.  In a
+ * column with n > 0 lines, k = the last line with Y_k <= yc (a binary search): src = fl(yc + fl(M_0 - Y_0)) above the first line,
+ * fl(yc + fl(M_last - Y_last)) below the last, else fl(M_k + fl(fl(fl(yc - Y_k) fl(M_k+1 - M_k)) / fl(Y_k+1 - Y_k))).  A column
+ * without lines takes d = src - yc of its neighbours l < x < r at the same yc, fl(dl + fl(fl(fl(x - l) fl(dr - dl)) / fl(r - l)))
+ * (the one side's d when only one exists, 0 when none does), and src = fl(yc + d).  The frame point (xc, src) maps to the photo:
+ * MN_FLAT_RECT (m = x0, y0): (fl(x0 + xc), fl(y0 + src)); MN_FLAT_QUAD (m = H's a .. h): u = xc / dw, v = src / dh, w =
+ * fl(fl(fl(g u) + fl(h v)) + 1), X = fl(fl(fl(fl(a u) + fl(b v)) + c) / w), Y likewise with d, e, f.  Then mapx = fl(X - 0.5),
+ * mapy = fl(Y - 0.5), and remap's cubic sampler exactly as mn_remap_curved_u8_batched uses it.  Byte offsets are 64-bit.
+ * pages: DEVICE array of records whose tables point into device memory (validated by the caller). */
+#define MN_FLAT_LINE_DOUBLES 9
+#define MN_FLAT_MAX_COLUMN_LINES 256
+#define MN_FLAT_RECT 0
+#define MN_FLAT_QUAD 1
+typedef struct {
+    const uint8_t* src;         /* row 0 of the photo */
+    int64_t src_pitch;
+    int32_t h, w;
+    uint8_t* dst;               /* row 0 of the flat page */
+    int64_t dst_pitch;
+    int32_t dh, dw;
+    const double* lines;        /* the line table */
+    int32_t* cols;              /* [3][dw]: line counts, left and right neighbours */
+    double* field;              /* [dw][stride][2]: (Y, M) per column */
+    int32_t n_lines, stride;
+    int32_t kind, pad;          /* MN_FLAT_RECT or MN_FLAT_QUAD */
+    double m[8];
+} mn_flat_page;
+int mn_flat_columns_batched(const mn_flat_page* pages, int n, int max_width, void* stream);
+int mn_flat_remap_u8_batched(const mn_flat_page* pages, int n, int cn, long long max_pixels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

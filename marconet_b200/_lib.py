@@ -148,6 +148,17 @@ class RemapCurvedImage(Structure):
 REGION_CURVED = 3
 
 
+FLAT_LINE_DOUBLES = 9           # MN_FLAT_LINE_DOUBLES
+FLAT_MAX_COLUMN_LINES = 256     # MN_FLAT_MAX_COLUMN_LINES
+FLAT_RECT, FLAT_QUAD = 0, 1
+
+
+class FlatPage(Structure):
+    _fields_ = [("src", c_void_p), ("src_pitch", c_int64), ("h", c_int32), ("w", c_int32), ("dst", c_void_p), ("dst_pitch", c_int64),
+                ("dh", c_int32), ("dw", c_int32), ("lines", c_void_p), ("cols", c_void_p), ("field", c_void_p), ("n_lines", c_int32),
+                ("stride", c_int32), ("kind", c_int32), ("pad", c_int32), ("m", c_double * 8)]
+
+
 class RegionCurved(Structure):
     _fields_ = [("q", RegionQuad), ("curve", c_void_p), ("n_seg", c_int32), ("pad", c_int32)]
 
@@ -282,6 +293,8 @@ SYMBOLS = {
     "mn_vertical_unlayout_u8_batched": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_remap_curved_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
     "mn_composite_regions_curved_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
+    "mn_flat_columns_batched": (c_int, [c_void_p, c_int, c_int, c_void_p]),
+    "mn_flat_remap_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
     "mn_find_lines_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_skewed_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_blocks_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),

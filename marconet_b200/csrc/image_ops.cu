@@ -624,6 +624,90 @@ __global__ void vertical_gather_kernel(const mn_vertical_column* __restrict__ co
     o[2] = s[2];
 }
 
+// blockIdx.y = page; one thread per frame column of its line table (layout: mn_flat_page), those past its dw columns exit.
+__global__ void flat_columns_kernel(const mn_flat_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    const mn_flat_page pg = pages[blockIdx.y];
+    if (x >= pg.dw) return;
+    const double xc = __dadd_rn((double)x, 0.5);
+    double* f = pg.field + (long long)x * pg.stride * 2;
+    int n = 0, left = -1, right = -1;
+    for (int k = 0; k < pg.n_lines; ++k) {
+        const double* L = pg.lines + (long long)k * MN_FLAT_LINE_DOUBLES;
+        const int bx0 = (int)L[7], bx1 = (int)L[8];
+        if (bx1 <= x) { left = max(left, bx1 - 1); continue; }
+        if (bx0 > x) { right = right < 0 ? bx0 : min(right, bx0); continue; }
+        const double t = fmin(fmax(__ddiv_rn(__dsub_rn(xc, L[0]), __dsub_rn(L[1], L[0])), 0.0), 1.0);
+        const double s = __dsub_rn(1.0, t);
+        const double a0 = bez_lerp(L[2], L[3], s, t), a1 = bez_lerp(L[3], L[4], s, t), a2 = bez_lerp(L[4], L[5], s, t);
+        f[2 * n] = L[6];
+        f[2 * n + 1] = bez_lerp(bez_lerp(a0, a1, s, t), bez_lerp(a1, a2, s, t), s, t);
+        ++n;
+    }
+    pg.cols[x] = n;
+    pg.cols[pg.dw + x] = left;
+    pg.cols[2 * pg.dw + x] = right;
+}
+
+// The source row of row centre yc in a column of n >= 1 (Y, M) pairs sorted by Y.
+__device__ __forceinline__ double flat_row(const double* __restrict__ f, int n, double yc) {
+    int lo = -1, hi = n - 1;                              // the last k with Y_k <= yc, -1 when none
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (f[2 * mid] <= yc) lo = mid; else hi = mid - 1;
+    }
+    if (lo < 0) return __dadd_rn(yc, __dsub_rn(f[1], f[0]));
+    if (lo == n - 1) return __dadd_rn(yc, __dsub_rn(f[2 * lo + 1], f[2 * lo]));
+    const double* a = f + 2 * lo;
+    return __dadd_rn(a[1], __ddiv_rn(__dmul_rn(__dsub_rn(yc, a[0]), __dsub_rn(a[3], a[1])), __dsub_rn(a[2], a[0])));
+}
+
+// blockIdx.y = page; one thread per pixel of its [dh][dw][cn] flat page, those past its dh*dw pixels exit.
+__global__ void flat_remap_kernel(const mn_flat_page* __restrict__ pages, int cn) {
+    mn_pdl_prologue();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const mn_flat_page pg = pages[blockIdx.y];
+    if (idx >= (long long)pg.dh * pg.dw) return;
+    const int x = (int)(idx % pg.dw), y = (int)(idx / pg.dw);
+    const double xc = __dadd_rn((double)x, 0.5), yc = __dadd_rn((double)y, 0.5);
+    const long long st = 2ll * pg.stride;
+    double src;
+    const int n = pg.cols[x];
+    if (n > 0) {
+        src = flat_row(pg.field + x * st, n, yc);
+    } else {
+        const int l = pg.cols[pg.dw + x], r = pg.cols[2 * pg.dw + x];
+        double d = 0.0;
+        if (l >= 0 && r >= 0) {
+            const double dl = __dsub_rn(flat_row(pg.field + l * st, pg.cols[l], yc), yc);
+            const double dr = __dsub_rn(flat_row(pg.field + r * st, pg.cols[r], yc), yc);
+            d = __dadd_rn(dl, __ddiv_rn(__dmul_rn((double)(x - l), __dsub_rn(dr, dl)), (double)(r - l)));
+        } else if (l >= 0 || r >= 0) {
+            const int c = l >= 0 ? l : r;
+            d = __dsub_rn(flat_row(pg.field + c * st, pg.cols[c], yc), yc);
+        }
+        src = __dadd_rn(yc, d);
+    }
+    const double* m = pg.m;
+    double X, Y;
+    if (pg.kind == MN_FLAT_RECT) {
+        X = __dadd_rn(m[0], xc);
+        Y = __dadd_rn(m[1], src);
+    } else {
+        const double u = __ddiv_rn(xc, (double)pg.dw), v = __ddiv_rn(src, (double)pg.dh);
+        const double w = __dadd_rn(__dadd_rn(__dmul_rn(m[6], u), __dmul_rn(m[7], v)), 1.0);
+        X = __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(m[0], u), __dmul_rn(m[1], v)), m[2]), w);
+        Y = __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(m[3], u), __dmul_rn(m[4], v)), m[5]), w);
+    }
+    const WarpCoord wc = {__float2int_rn(__fmul_rn(__double2float_rn(__dsub_rn(X, 0.5)), 32.f)),
+                          __float2int_rn(__fmul_rn(__double2float_rn(__dsub_rn(Y, 0.5)), 32.f))};
+    int wt[16];
+    warp_taps(wc, wt);
+    uint8_t* o = pg.dst + (long long)y * pg.dst_pitch + (long long)x * cn;
+    for (int c = 0; c < cn; ++c) o[c] = (uint8_t)warp_cubic_u8(pg.src, pg.src_pitch, pg.h, pg.w, cn, c, wc, wt);
+}
+
 }  // namespace
 
 template <bool kUnlayout>
@@ -775,6 +859,23 @@ extern "C" int mn_prior_tiles_u8(const float* priors, long long stride_n, long l
     MN_REQUIRE(priors && tiles && n_rows > 0 && n_rows <= 65535, "mn_prior_tiles_u8: bad args");
     MN_CUDA_CHECK((mn_launch(prior_tiles_kernel, dim3(128 * 128 / 256, n_rows), dim3(256), 0, (cudaStream_t)stream, priors, stride_n,
                              stride_c, stride_h, stride_w, tiles)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_flat_columns_batched(const mn_flat_page* pages, int n, int max_width, void* stream) {
+    MN_REQUIRE(pages && n > 0 && n <= 65535 && max_width > 0, "mn_flat_columns_batched: bad args");
+    MN_CUDA_CHECK((mn_launch(flat_columns_kernel, dim3((unsigned)mn_cdiv64(max_width, 128), n), dim3(128), 0, (cudaStream_t)stream,
+                             pages)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_flat_remap_u8_batched(const mn_flat_page* pages, int n, int cn, long long max_pixels, void* stream) {
+    MN_REQUIRE(pages && n > 0 && n <= 65535 && cn > 0 && cn <= 4 && max_pixels > 0, "mn_flat_remap_u8_batched: bad args");
+    MN_REQUIRE(max_pixels < (1ll << 31) * 256, "mn_flat_remap_u8_batched: %lld pixels exceed the grid", max_pixels);
+    MN_CUDA_CHECK((mn_launch(flat_remap_kernel, dim3((unsigned)mn_cdiv64(max_pixels, 256), n), dim3(256), 0, (cudaStream_t)stream,
+                             pages, cn)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -1468,6 +1468,90 @@ def remap_curved(items):
     LAUNCHES += 1
 
 
+FLAT_MAX_COLUMN_LINES = _lib.FLAT_MAX_COLUMN_LINES
+
+
+def flat_column_lines(lines, width):
+    """The most lines of an fp64 line table (pipeline.flat_line_table) that one of ``width`` frame columns meets."""
+    import numpy as np
+    if len(lines) == 0:
+        return 0
+    d = np.zeros(width + 1, np.int64)
+    np.add.at(d, np.asarray(lines[:, 7], np.int64), 1)
+    np.add.at(d, np.asarray(lines[:, 8], np.int64), -1)
+    return int(np.cumsum(d).max())
+
+
+def flat_remap(items, tables=False):
+    """Curled pages flattened through their dewarp field, every page in two launches (mn_flat_columns_batched, then
+    mn_flat_remap_u8_batched; DESIGN.md 7b, "Flat pages").  items: list of (src, dst, kind, m, lines): src the uint8 [h, w, cn]
+    photo and dst the [dh, dw, cn] flat page, CUDA views with dense pixels (any row stride), h, w <= 32767; kind "rect" (m = (x0,
+    y0)) or "quad" (m = the unit-square homography's a .. h); lines the page's fp64 [n, 9] line table (pipeline.flat_line_table)
+    with block ranges inside [0, dw].  The records and line tables go up in one copy.  ``tables`` (tests): also return per page
+    the int32 CUDA view [3, dw] of its column counts and neighbours, and the fp64 view [dw, stride, 2] of its (Y, M) pairs.
+    Raises ValueError naming the page, before any launch, for a column met by more than FLAT_MAX_COLUMN_LINES lines."""
+    import numpy as np
+    global LAUNCHES
+    if not items:
+        raise ValueError("flat_remap: no pages")
+    if len(items) > 65535:
+        raise ValueError("flat_remap: at most 65535 pages per launch")
+    dev = items[0][0].device
+    cn = items[0][0].shape[2] if isinstance(items[0][0], torch.Tensor) and items[0][0].dim() == 3 else 3
+    if not 1 <= cn <= 4:
+        raise RuntimeError(f"flat_remap: {cn} channels (1 to 4)")
+    isz = ctypes.sizeof(_lib.FlatPage)
+    tabs, strides, o = [], [], _align8(len(items) * isz)
+    for i, (src, dst, kind, m, lines) in enumerate(items):
+        what = f"flat_remap: page {i}"
+        _dense_u8(src, dev, cn, f"{what}: src")
+        _dense_u8(dst, dev, cn, f"{what}: dst")
+        if max(src.shape[:2]) > 32767:
+            raise ValueError(f"{what}: a {src.shape[0]}x{src.shape[1]} source exceeds OpenCV's int16 source coordinates")
+        if kind not in ("rect", "quad") or len(m) != (2 if kind == "rect" else 8):
+            raise ValueError(f"{what}: expected kind 'rect' with (x0, y0) or 'quad' with H's eight values")
+        t = np.ascontiguousarray(lines, np.float64).reshape(-1, _lib.FLAT_LINE_DOUBLES)
+        dw = dst.shape[1]
+        if len(t) and not (np.all(t[:, 7] >= 0) and np.all(t[:, 7] < t[:, 8]) and np.all(t[:, 8] <= dw)
+                           and np.all(t[:, 7] == np.floor(t[:, 7])) and np.all(t[:, 8] == np.floor(t[:, 8]))):
+            raise ValueError(f"{what}: a line's block range is not an integer range inside the {dw} columns")
+        stride = flat_column_lines(t, dw)
+        if stride > FLAT_MAX_COLUMN_LINES:
+            raise ValueError(f"{what}: a column meets {stride} lines, over the {FLAT_MAX_COLUMN_LINES} a column may hold")
+        tabs.append(t)
+        strides.append(max(1, stride))
+    los = list(itertools.accumulate((8 * t.size for t in tabs), initial=o))     # the records, then every line table
+    o = _align8(los[-1])
+    offs = []
+    for (_, dst, *_), lo, stride in zip(items, los, strides):             # then each page's column table and (Y, M) pairs
+        dw = dst.shape[1]
+        co = o
+        fo = _align8(co + 12 * dw)
+        o = fo + 16 * dw * stride
+        offs.append((lo, co, fo))
+    buf = torch.empty(o, dtype=torch.uint8, device=dev)
+    base, recs, mx, mw = buf.data_ptr(), [], 0, 0
+    for (src, dst, kind, m, _), t, stride, (lo, co, fo) in zip(items, tabs, strides, offs):
+        (h, w), (dh, dw) = src.shape[:2], dst.shape[:2]
+        recs.append(_lib.FlatPage(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw, base + lo, base + co,
+                                  base + fo, len(t), stride, _lib.FLAT_RECT if kind == "rect" else _lib.FLAT_QUAD, 0,
+                                  (ctypes.c_double * 8)(*[float(v) for v in m])))
+        mx, mw = max(mx, dh * dw), max(mw, dw)
+    host = bytearray(los[0])
+    host[:len(items) * isz] = bytes((_lib.FlatPage * len(recs))(*recs))
+    host += b"".join(t.tobytes() for t in tabs)
+    buf[:len(host)].copy_(torch.frombuffer(host, dtype=torch.uint8))
+    lib = _lib.load()
+    _lib.check(lib.mn_flat_columns_batched(base, len(recs), mw, _stream()), "mn_flat_columns_batched")
+    _lib.check(lib.mn_flat_remap_u8_batched(base, len(recs), cn, mx, _stream()), "mn_flat_remap_u8_batched")
+    LAUNCHES += 2
+    if not tables:
+        return None
+    return [(buf[co:co + 12 * d.shape[1]].view(torch.int32).view(3, d.shape[1]),
+             buf[fo:fo + 16 * d.shape[1] * s].view(torch.float64).view(d.shape[1], s, 2))
+            for (_, d, *_), s, (_, co, fo) in zip(items, strides, offs)]
+
+
 def composite_regions_curved(regions, feather):
     """composite_regions_quad for pages that also hold curved regions (mn_composite_regions_curved_u8; DESIGN.md 7b, "Curved text
     regions"), one launch.  regions: list of (page, sr, rect, chain, maps) as composite_regions_quad takes them; maps may also be

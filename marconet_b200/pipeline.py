@@ -2356,6 +2356,265 @@ def _failed_pages(page_layout, block_layout):
     return drop
 
 
+class FlatPage(NamedTuple):
+    """A page of an image to flatten (DESIGN.md 7b, "Flat pages") in one of three frames: ``rect`` None (the whole image) or an
+    integer rectangle, whose frame is the crop; ``skew``, a given angle in degrees or "auto" (searched within +-``max_skew`` as a
+    TextPage's), whose frame is the crop rotated upright; or ``quad``, a QuadRegion or "auto" (found as a TextPage's), whose
+    frame is its rectified crop R.  ``curve="auto"`` (rect and quad frames, horizontal pages) straightens the page's curled lines
+    through a dewarp field built from them; each block of the frame is traced across ``strips`` column strips (default: a curled
+    block's), or as many as fit in the block when it is narrower.  ``direction``, ``polarity``, ``gap_x`` and ``gap_y`` are a
+    TextPage's, used wherever the page's blocks are searched."""
+    rect: object = None
+    quad: object = None
+    skew: object = None
+    max_skew: float = 10.0
+    curve: object = None
+    strips: object = None
+    direction: str = "horizontal"
+    polarity: str = "auto"
+    gap_x: object = None
+    gap_y: object = None
+
+
+FLAT_MAX_WORK = 1 << 31     # bytes of device memory the flat pages of one flatten_pages call may use
+
+
+def _flat_text_page(fp, **kw):
+    """The TextPage of a FlatPage's search (no curve)."""
+    return TextPage(fp.rect, fp.direction, fp.polarity, fp.gap_x, fp.gap_y, fp.skew, fp.max_skew, fp.quad)._replace(**kw)
+
+
+def _flat_frame(fp, rect):
+    """(w_f, h_f) of a FlatPage's frame: the crop, R, or the upright frame of a given angle (under "auto": the largest side over
+    the search table, for both sides); None for quad="auto" before its corners are found."""
+    from . import ops
+    w, h = rect[2] - rect[0], rect[3] - rect[1]
+    if fp.quad is not None:
+        return None if isinstance(fp.quad, str) else quad_maps(fp.quad, 1).size
+    if fp.skew is None:
+        return w, h
+    _, _, L, M = ops.skew_frames(w, h, False, ops.skew_cos_sin(ops.skew_table(fp.skew, fp.max_skew, False)))
+    return int(M.max()), int(L.max())
+
+
+def _check_flat(fp, H, W, name):
+    """The rectangle (x0, y0, x1, y1) of the FlatPage ``fp`` of an H x W image (the quad's pixel box for a given quad, the image
+    for quad="auto"), validated under _check_page's, _check_quad's and _check_curve's rules, curve with quad allowed.  Raises
+    ValueError naming ``name``."""
+    auto = isinstance(fp.curve, str) and fp.curve == "auto"
+    if auto and fp.skew is not None:
+        raise ValueError(f"{name}: curve and skew are both given (curl together with skew is not supported)")
+    if auto and fp.direction == "vertical":
+        raise ValueError(f"{name}: curve is given for a vertical page (curled columns are not supported)")
+    if fp.skew is not None and fp.quad is not None:
+        raise ValueError(f"{name}: skew and quad are both given (skew together with perspective is not supported)")
+    rect = _check_page(_flat_text_page(fp), H, W, name)
+    _check_curve(fp.curve, None, _flat_text_page(fp, quad=None), rect[2] - rect[0], name)
+    if fp.strips is not None:
+        from . import ops
+        if isinstance(fp.strips, bool) or not isinstance(fp.strips, int) or not 1 <= fp.strips <= ops.CURVE_MAX_STRIPS:
+            raise ValueError(f"{name}: strips must be an integer in [1, {ops.CURVE_MAX_STRIPS}], got {fp.strips!r}")
+        if not auto:
+            raise ValueError(f"{name}: strips is given, but curve is {fp.curve!r}, not 'auto'")
+    if auto and max(H, W) > 32767:
+        raise ValueError(f"{name}: a curled page is resampled from the whole {W}x{H} image, whose side exceeds 32767 pixels "
+                         f"(OpenCV's int16 source coordinates; crop the image first)")
+    size = _flat_frame(fp, rect)
+    if size is not None and max(size) > 32767:
+        raise ValueError(f"{name}: a side of the page's flat frame reaches {max(size)} pixels, over 32767")
+    return rect
+
+
+def _flat_bytes(fp, size):
+    """Device bytes of a flat page of frame ``size`` beyond its search: the flat page, and for a curled page its column table
+    at the column cap and the tracing of one block as large as the frame."""
+    from . import ops
+    w, h = size
+    n = 3 * w * h
+    if fp.curve is not None:
+        n += w * (12 + 16 * ops.FLAT_MAX_COLUMN_LINES) + ops.curve_block_bytes(w, h, fp.strips)
+    return n
+
+
+def _check_flat_work(items, names):
+    """Refuse, before any launch, flat pages (image index, FlatPage, rect) whose work memory, added up in order, passes
+    FLAT_MAX_WORK (a quad="auto" page counts its image until its corners are found), and a call whose searched pages pass the
+    page search's limit."""
+    total = 0
+    for (_, fp, rect), name in zip(items, names):
+        total += _flat_bytes(fp, _flat_frame(fp, rect) or (rect[2] - rect[0], rect[3] - rect[1]))
+        if total > FLAT_MAX_WORK:
+            raise ValueError(f"{name}: the call's flat pages up to this one need {total} bytes of work memory, over the "
+                             f"{FLAT_MAX_WORK} a call may use (split the call)")
+    searched = [(i, _flat_text_page(fp), rect) for i, fp, rect in items
+                if fp.curve is not None or isinstance(fp.skew, str) or isinstance(fp.quad, str)]
+    if searched:
+        _check_page_work(searched)
+
+
+def flat_strips(strips, w):
+    """The strip count of a curled block w pixels wide on a flat page: curve_strips', or ``strips`` cut to what the block
+    holds (strips of at least CURVE_MIN_STRIP pixels)."""
+    from . import ops
+    return None if strips is None else max(1, min(strips, w // ops.CURVE_MIN_STRIP))
+
+
+def skew_flat_matrix(w, h, c, s):
+    """(M, (w_f, h_f)): the 2 x 3 warpAffine map (WARP_INVERSE_MAP) of a w x h crop into its upright frame at (c, s), frame pixel
+    (i, j) -> crop pixel index O - 0.5 + (u_min + j) e + (v_min + i) f, O = (w / 2, h / 2), e = (c, -s), f = (s, c), and the
+    frame's size (M, L) from skew_frames."""
+    from . import ops
+    u_min, v_min, L, M = (a[0] for a in ops.skew_frames(w, h, False, [(c, s)]))
+    u_min, v_min = float(u_min), float(v_min)
+    m = ((c, s, w / 2 - 0.5 + u_min * c + v_min * s), (-s, c, h / 2 - 0.5 - u_min * s + v_min * c))
+    return m, (int(M), int(L))
+
+
+def flat_line_table(blocks):
+    """The fp64 [n, 9] line table of a curled page (DESIGN.md 7b, "Flat pages") from its blocks in reading order, each (rect,
+    lines) with rect (x0, y0, x1, y1) and its lines (CurvedRegions or integer rectangles) in frame coordinates.  Per line: xs,
+    xe (its first and last control points' x, or a rectangle's x0 and x1), mu_j = fl(0.5 fl(top_j.y + bottom_j.y)) (a
+    rectangle's (y0 + y1) / 2 four times), the anchor Y = fl(fl(fl(fl(mu_0 + mu_1) + mu_2) + mu_3) / 4) and its block's columns
+    bx0, bx1; rows sorted by Y, ties in reading order."""
+    import numpy as np
+    rows = []
+    for rect, lines in blocks:
+        for q in lines:
+            if isinstance(q, CurvedRegion):
+                xs, xe = float(q.top[0][0]), float(q.top[3][0])
+                mu = [0.5 * (float(t[1]) + float(b[1])) for t, b in zip(q.top, q.bottom)]
+            else:
+                xs, xe = float(q[0]), float(q[2])
+                mu = [(q[1] + q[3]) / 2] * 4
+            rows.append((xs, xe, *mu, (((mu[0] + mu[1]) + mu[2]) + mu[3]) / 4, float(rect[0]), float(rect[2])))
+    order = sorted(range(len(rows)), key=lambda k: (rows[k][6], k))
+    return np.array([rows[k] for k in order], np.float64).reshape(-1, 9)
+
+
+@torch.no_grad()
+def flatten_pages(images, pages, to_host=False):
+    """Flat, upright pages of photographed, tilted and curled pages (DESIGN.md 7b, "Flat pages").
+
+    images: uint8 [H, W, 3] numpy arrays or CPU / CUDA tensors; pages: per image, a list of FlatPages.  Returns per image a list
+    with one dict per page: ``image``, the flat page (uint8 [h_f, w_f, 3] CUDA tensor, or numpy through one pinned copy with
+    ``to_host``); ``kind``, "rect", "skew" or "quad"; ``size`` (w_f, h_f); ``quad`` (the corners used) or ``skew`` (the angle
+    used, in degrees); for a curled page ``lines``, the lines the field was built from in frame coordinates.
+    A rect page is its crop; a quad page is R (ops.warp_perspective of quad_maps(quad, 1)); a skewed page is its crop warped
+    upright, every one in one ops.warp_affine launch.  A curled page's blocks are found on its frame and traced (find_blocks'
+    and find_lines' stages), and every page with a curled line goes through ops.flat_remap's two launches; a page whose lines
+    all come back level is flattened as without curve.  Raises ValueError naming the image and the page, before any launch,
+    for a page its rules reject, and after the search for a page without a page found or over a limit."""
+    from . import ops
+    imgs = [_as_image(im, i) for i, im in enumerate(images)]
+    pages = _per_image(pages, len(imgs), "pages (one list per image)")
+    items, names = [], []
+    for i, im in enumerate(imgs):
+        for r, fp in enumerate(pages[i] or []):
+            names.append(f"image {i}, page {r}")
+            if not isinstance(fp, FlatPage):
+                raise ValueError(f"{names[-1]}: expected a FlatPage, got {fp!r}")
+            items.append((i, fp, _check_flat(fp, im.shape[0], im.shape[1], names[-1])))
+    _check_flat_work(items, names)
+    out = [[] for _ in imgs]
+    if not items:
+        return out
+    dev = next((im.device for im in imgs if im.is_cuda), torch.device("cuda", torch.cuda.current_device()))
+    with torch.cuda.device(dev):
+        dimg = _device_images(sorted({i for i, _, _ in items}), imgs, dev)
+        found = _page_quads(dimg, [(i, _flat_text_page(fp), rect) for i, fp, rect in items])
+        for k, (f, name) in enumerate(zip(found, names)):
+            if isinstance(f, str):
+                raise ValueError(f"{name}: {f}")
+            i, fp, _ = items[k]
+            if isinstance(fp.quad, str):
+                fp = fp._replace(quad=f[1].quad)
+                size = _flat_frame(fp, f[2])
+                if max(size) > 32767:
+                    raise ValueError(f"{name}: a side of the page's flat frame reaches {max(size)} pixels, over 32767")
+                items[k] = (i, fp, f[2])
+        _check_flat_work(items, names)
+        rq = _rectify(dimg, [_quad_key(i, fp.quad) for i, fp, _ in items if fp.quad is not None])
+        src, frames = dict(dimg), {}
+        for k, (i, fp, (x0, y0, x1, y1)) in enumerate(items):
+            if fp.quad is not None:
+                frames[k] = rq[_quad_key(i, fp.quad)]
+            elif fp.skew is None:
+                frames[k] = dimg[i][y0:y1, x0:x1]
+            if k in frames:
+                src[("frame", k)] = frames[k]
+        search = [k for k, (_, fp, _) in enumerate(items) if fp.curve is not None or isinstance(fp.skew, str)]
+        sitems = [(i, _flat_text_page(fp), rect) if fp.curve is None else
+                  (("frame", k), TextPage(None, fp.direction, fp.polarity, fp.gap_x, fp.gap_y),
+                   (0, 0, frames[k].shape[1], frames[k].shape[0])) for k, (i, fp, rect) in ((k, items[k]) for k in search)]
+        pres = dict(zip(search, _find_blocks(src, sitems) if sitems else []))
+        for k, r in pres.items():
+            if isinstance(r, str):
+                raise ValueError(f"{names[k]}: {r}")
+        angle = {k: r["skew"] if "skew" in r else 0.0 for k, r in pres.items() if items[k][1].curve is None}
+        bitems, bnames, bpage = [], [], []
+        for k in search:
+            fp = items[k][1]
+            if fp.curve is None:
+                continue
+            for b, blk in enumerate(pres[k]["blocks"]):
+                bw = blk.rect[2] - blk.rect[0]
+                bitems.append((("frame", k), blk._replace(curve="auto", strips=flat_strips(fp.strips, bw)), tuple(blk.rect)))
+                bnames.append(f"{names[k]}, block {b}")
+                bpage.append(k)
+        _check_curve_work(bitems, bnames)
+        lines = {k: [] for k in search if items[k][1].curve is not None}
+        for (_, blk, rect), name, k, r in zip(bitems, bnames, bpage, _find_lines(src, bitems) if bitems else []):
+            if isinstance(r, str):
+                raise ValueError(f"{name}: {r}")
+            lines[k].append((rect, r["lines"]))
+        sizes = []
+        for k, (i, fp, (x0, y0, x1, y1)) in enumerate(items):
+            if fp.skew is not None:
+                theta = float(fp.skew) if k not in angle else angle[k]
+                c, s = ops.skew_cos_sin([theta])[0]
+                m, size = skew_flat_matrix(x1 - x0, y1 - y0, c, s)
+                frames[k] = (theta, m)
+                sizes.append(size[::-1])
+            else:
+                sizes.append(tuple(frames[k].shape[:2]))
+        views = _flat_views(sizes, dev)
+        warps, remaps, res = [], [], []
+        for k, ((i, fp, (x0, y0, x1, y1)), dst) in enumerate(zip(items, views)):
+            d = dict(image=dst, kind="quad" if fp.quad is not None else "skew" if fp.skew is not None else "rect",
+                     size=(dst.shape[1], dst.shape[0]))
+            curled = k in lines and any(isinstance(q, CurvedRegion) for _, ls in lines[k] for q in ls)
+            table = flat_line_table(lines[k]) if curled else None
+            if curled and ops.flat_column_lines(table, dst.shape[1]) > ops.FLAT_MAX_COLUMN_LINES:
+                raise ValueError(f"{names[k]}: a column of the page meets {ops.flat_column_lines(table, dst.shape[1])} lines, "
+                                 f"over the {ops.FLAT_MAX_COLUMN_LINES} a column may hold")
+            if fp.skew is not None:
+                d["skew"] = frames[k][0]
+                warps.append((dimg[i][y0:y1, x0:x1], dst, frames[k][1]))
+            elif curled:
+                if fp.quad is not None:
+                    (a, b, c), (e, f, g), (h, j, _) = _quad_homography([(float(p[0]), float(p[1])) for p in fp.quad])
+                    remaps.append((dimg[i], dst, "quad", (a, b, c, e, f, g, h, j), table))
+                else:
+                    remaps.append((dimg[i], dst, "rect", (x0, y0), table))
+            else:
+                dst.copy_(frames[k])
+            if fp.quad is not None:
+                d["quad"] = _quad_key(i, fp.quad)[1]
+            if k in lines:
+                d["lines"] = [q for _, ls in lines[k] for q in ls]
+            res.append(d)
+        if warps:
+            ops.warp_affine(warps)
+        if remaps:
+            ops.flat_remap(remaps)
+        if to_host:
+            for d, v in zip(res, _to_host_all([d["image"] for d in res])):
+                d["image"] = v
+    for (i, _, _), d in zip(items, res):
+        out[i].append(d)
+    return out
+
+
 MAX_REGIONS = 65535     # regions of one restore_regions call: each is one grid row (blockIdx.y) of the composite launch
 
 
