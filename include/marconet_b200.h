@@ -934,6 +934,38 @@ typedef struct {
 int mn_flat_columns_batched(const mn_flat_page* pages, int n, int max_width, void* stream);
 int mn_flat_remap_u8_batched(const mn_flat_page* pages, int n, int cn, long long max_pixels, void* stream);
 
+/* Even lighting (DESIGN.md section 7b, "Even lighting"): page i (h x w, three channels, odd window k) is evened as
+ * E = rint(255 F / B) per channel (half to even, 0 where B = 0, at most 255), B the grey closing of F (the min over the k x k
+ * window cut to the page of the max over the k x k window cut to the page), computed as rintf(__fdiv_rn(255.f F, (float)B)).
+ * For light ink every byte is complemented on read and on write (v ^ 255), so E = 255 - E_dark(255 - F) on one code path.
+ * mn_even_light_u8 issues 6 launches for every page of a call (4 when `threshold` is 0), whatever their number:
+ *   1, 2. (threshold != 0) mn_find_lines_u8's histogram and threshold over blocks[] (blocks[i] and pages[i].b the same
+ *         record: the frame whose ink decides the polarity, b.polarity; MN_INK_AUTO: the minority side of Otsu's threshold),
+ *         the ink into b.out->ink;
+ *   3-6. a row max, a column max, a row min and a column min pass, the divide fused into the last; blockIdx.y = page.  Each pass
+ *        gives thread (line, s) the outputs i in [s k, s k + k) of its line and costs O(1) comparisons per pixel whatever k:
+ *        the van Herk / Gil-Werman suffix extrema of segment s and prefix extrema of segment s + 1 of the line padded by k / 2
+ *        identities (0 for max, 255 for min) at each end, the padding never read.
+ * ink is read from b.out->ink on the device: written by launch 2, or left there by an earlier call when `threshold` is 0.
+ * src and dst may be the same pixels (evened in place).  s1, s2: dense scratch planes of h w 3 bytes.  b.out needs only its
+ * first 16 bytes (threshold and ink), b.hist 256 int32 in work (work_bytes, zeroed by the call when `threshold` is set).
+ * max_tiles >= every frame's tile count, max_lines >= every page's h ceil(w / k) and w ceil(h / k).  Byte offsets are 64-bit.
+ * blocks, pages: DEVICE arrays (validated by the caller: 1 <= h, w <= 32767, k odd in [3, 32767]; blocks may be NULL when
+ * `threshold` is 0). */
+typedef struct {
+    mn_text_block b;            /* the frame whose ink is used */
+    const uint8_t* src;         /* row 0 of the page F */
+    int64_t src_pitch;
+    uint8_t* dst;               /* row 0 of the evened page */
+    int64_t dst_pitch;
+    int32_t h, w;
+    int32_t k, pad;             /* the window */
+    uint8_t* s1;                /* scratch planes */
+    uint8_t* s2;
+} mn_light_page;
+int mn_even_light_u8(const mn_text_block* blocks, const mn_light_page* pages, int n, int threshold, long long max_tiles,
+                     long long max_lines, void* work, long long work_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

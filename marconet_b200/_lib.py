@@ -178,6 +178,11 @@ class TextBlock(Structure):
                 ("pad", c_int32), ("hist", c_void_p), ("prof", c_void_p), ("scratch", c_void_p), ("out", c_void_p)]
 
 
+class LightPage(Structure):
+    _fields_ = [("b", TextBlock), ("src", c_void_p), ("src_pitch", c_int64), ("dst", c_void_p), ("dst_pitch", c_int64), ("h", c_int32),
+                ("w", c_int32), ("k", c_int32), ("pad", c_int32), ("s1", c_void_p), ("s2", c_void_p)]
+
+
 class SkewBlock(Structure):
     _fields_ = [("b", TextBlock), ("table", c_void_p), ("scores", c_void_p), ("profiles", c_void_p), ("n_ang", c_int32),
                 ("stride", c_int32), ("chosen", c_int32), ("L", c_int32), ("M", c_int32), ("pad", c_int32), ("u_min", c_double),
@@ -295,6 +300,7 @@ SYMBOLS = {
     "mn_composite_regions_curved_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_flat_columns_batched": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "mn_flat_remap_u8_batched": (c_int, [c_void_p, c_int, c_int, c_longlong, c_void_p]),
+    "mn_even_light_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_longlong, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_skewed_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_blocks_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),

@@ -1655,6 +1655,11 @@ int block_threshold(const mn_text_block* blocks, int n, long long max_tiles, voi
 
 }  // namespace
 
+// The histogram and threshold launches for the other files of the library (light_ops.cu).
+int mn_block_threshold(const mn_text_block* blocks, int n, long long max_tiles, void* work, long long work_bytes, cudaStream_t st) {
+    return block_threshold(blocks, n, max_tiles, work, work_bytes, st);
+}
+
 extern "C" int mn_find_lines_u8(const mn_text_block* blocks, int n, long long max_tiles, void* work, long long work_bytes,
                                 void* stream) {
     MN_REQUIRE(blocks && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,

@@ -1552,6 +1552,97 @@ def flat_remap(items, tables=False):
             for (_, d, *_), s, (_, co, fo) in zip(items, strides, offs)]
 
 
+LIGHT_MAX_WINDOW = 32767
+
+
+def light_window(w, h):
+    """The default evening window of a w x h frame (DESIGN.md 7b, "Even lighting"): max(3, 2 floor(min(w, h) / 40) + 1), a
+    heuristic that holds a line of ordinary text."""
+    return max(3, 2 * (min(w, h) // 40) + 1)
+
+
+def even_light(items, inks=None):
+    """Pages evened by their paper, every page in six launches (mn_even_light_u8; DESIGN.md 7b, "Even lighting"): E = rint(255 F
+    / B) per channel, B the grey closing of F with a k x k window cut to the page, complemented on read and write for light ink.
+    items: list of (frame, src, dst, k, polarity): src and dst uint8 [h, w, 3] CUDA views with dense pixels (any row stride) of
+    the same size, sides <= 32767 (dst may be src: evened in place); k an odd int in [3, 32767]; frame the [h_f, w_f, 3] view
+    whose histogram and Otsu threshold choose the ink under polarity _lib.INK_AUTO (else the polarity given).
+    ``inks``: None, or per item the int32 CUDA view of 4 values an earlier call returned: its ink is used as it is on the device,
+    frame and polarity are ignored and the call takes four launches.  Returns the int32 CUDA tensor [n, 4] of every page's
+    (0, threshold, ink, 0), whose rows an evening of the same pages may take as ``inks``; None when ``inks`` is given."""
+    global LAUNCHES
+    if not items:
+        raise ValueError("even_light: no pages")
+    if len(items) > 65535:
+        raise ValueError("even_light: at most 65535 pages per launch")
+    if inks is not None and len(inks) != len(items):
+        raise ValueError("even_light: one ink per page")
+    dev = items[0][1].device
+    n = len(items)
+    rsz, lsz = ctypes.sizeof(_lib.TextBlock), ctypes.sizeof(_lib.LightPage)
+    tiles, lines = 1, 1
+    for i, (frame, src, dst, k, polarity) in enumerate(items):
+        what = f"even_light: page {i}"
+        _dense_u8(src, dev, 3, f"{what}: src")
+        _dense_u8(dst, dev, 3, f"{what}: dst")
+        h, w = src.shape[:2]
+        if tuple(dst.shape) != tuple(src.shape) or max(h, w) > 32767:
+            raise ValueError(f"{what}: src {tuple(src.shape)} and dst {tuple(dst.shape)} differ or have a side over 32767")
+        if isinstance(k, bool) or not isinstance(k, int) or not 3 <= k <= LIGHT_MAX_WINDOW or k % 2 == 0:
+            raise ValueError(f"{what}: the window must be an odd int in [3, {LIGHT_MAX_WINDOW}], got {k!r}")
+        if inks is None:
+            _dense_u8(frame, dev, 3, f"{what}: frame")
+            if max(frame.shape[:2]) > 32767 or polarity not in (_lib.INK_AUTO, _lib.INK_DARK, _lib.INK_LIGHT):
+                raise ValueError(f"{what}: a frame side over 32767 or a bad polarity {polarity!r}")
+            tiles = max(tiles, -(-frame.shape[0] // 32) * -(-frame.shape[1] // 32))
+        elif not (isinstance(inks[i], torch.Tensor) and inks[i].device == dev and inks[i].dtype == torch.int32
+                  and inks[i].numel() == 4 and inks[i].is_contiguous()):
+            raise ValueError(f"{what}: an ink must be an int32 CUDA view of 4 values on {dev}")
+        lines = max(lines, h * -(-w // k), w * -(-h // k))
+    planes = [_align8(3 * src.shape[0] * src.shape[1]) for _, src, *_ in items]
+    o_rec = n * rsz
+    o_work = _align8(o_rec + n * lsz)
+    o_planes = o_work + (1024 * n if inks is None else 0)
+    buf = torch.empty(o_planes + 2 * sum(planes), dtype=torch.uint8, device=dev)
+    base = buf.data_ptr()
+    if inks is None:                # apart from the work, so that the scratch planes are freed with the call
+        table = torch.zeros(n, 4, dtype=torch.int32, device=dev)
+        inks, threshold = table.unbind(0), 1
+    else:
+        threshold = 0
+    blocks, recs, o = [], [], base + o_planes
+    for i, ((frame, src, dst, k, polarity), pl) in enumerate(zip(items, planes)):
+        if threshold:
+            fh, fw = frame.shape[:2]
+            tb = _lib.TextBlock(frame.data_ptr(), frame.stride(0), 0, 0, fw, fh, 0, polarity, 0, 0, 0, 0, base + o_work + 1024 * i,
+                                0, 0, inks[i].data_ptr())
+        else:
+            tb = _lib.TextBlock(0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, inks[i].data_ptr())
+        blocks.append(tb)
+        recs.append(_lib.LightPage(tb, src.data_ptr(), src.stride(0), dst.data_ptr(), dst.stride(0), src.shape[0], src.shape[1], k, 0,
+                                   o, o + pl))
+        o += 2 * pl
+    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.LightPage * n)(*recs))
+    buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    if threshold:
+        _lib.check(_lib.load().mn_even_light_u8(base, base + o_rec, n, 1, tiles, lines, base + o_work, 1024 * n, _stream()),
+                   "mn_even_light_u8")
+        LAUNCHES += 6
+        return table
+    _lib.check(_lib.load().mn_even_light_u8(0, base + o_rec, n, 0, 0, lines, 0, 0, _stream()), "mn_even_light_u8")
+    LAUNCHES += 4
+    return None
+
+
+def even_light_bytes(w, h, frame=None):
+    """Device bytes of evening a w x h page beyond the page itself: its two scratch planes and, when ``frame`` (w_f, h_f) is
+    given, the evened frame the page's searches read."""
+    n = 2 * _align8(3 * w * h) + 1024 + 16
+    if frame is not None:
+        n += 3 * frame[0] * frame[1]
+    return n
+
+
 def composite_regions_curved(regions, feather):
     """composite_regions_quad for pages that also hold curved regions (mn_composite_regions_curved_u8; DESIGN.md 7b, "Curved text
     regions"), one launch.  regions: list of (page, sr, rect, chain, maps) as composite_regions_quad takes them; maps may also be

@@ -2363,7 +2363,10 @@ class FlatPage(NamedTuple):
     frame is its rectified crop R.  ``curve="auto"`` (rect and quad frames, horizontal pages) straightens the page's curled lines
     through a dewarp field built from them; each block of the frame is traced across ``strips`` column strips (default: a curled
     block's), or as many as fit in the block when it is narrower.  ``direction``, ``polarity``, ``gap_x`` and ``gap_y`` are a
-    TextPage's, used wherever the page's blocks are searched."""
+    TextPage's, used wherever the page's blocks are searched.  ``light="even"`` (DESIGN.md 7b, "Even lighting") divides the
+    page by its paper, the grey closing of its frame with an odd ``light_window`` x ``light_window`` window (default
+    ops.light_window of the frame, a heuristic: darker features wider than the window are lightened); the page's searches then
+    run on the evened frame, and the flat page is evened with the same window and ink."""
     rect: object = None
     quad: object = None
     skew: object = None
@@ -2374,6 +2377,8 @@ class FlatPage(NamedTuple):
     polarity: str = "auto"
     gap_x: object = None
     gap_y: object = None
+    light: object = None
+    light_window: object = None
 
 
 FLAT_MAX_WORK = 1 << 31     # bytes of device memory the flat pages of one flatten_pages call may use
@@ -2401,6 +2406,15 @@ def _check_flat(fp, H, W, name):
     """The rectangle (x0, y0, x1, y1) of the FlatPage ``fp`` of an H x W image (the quad's pixel box for a given quad, the image
     for quad="auto"), validated under _check_page's, _check_quad's and _check_curve's rules, curve with quad allowed.  Raises
     ValueError naming ``name``."""
+    from . import ops
+    if fp.light is not None and not (isinstance(fp.light, str) and fp.light == "even"):
+        raise ValueError(f"{name}: light must be None or 'even', got {fp.light!r}")
+    if fp.light_window is not None:
+        if fp.light is None:
+            raise ValueError(f"{name}: light_window is given, but light is None, not 'even'")
+        k = fp.light_window
+        if isinstance(k, bool) or not isinstance(k, int) or not 3 <= k <= ops.LIGHT_MAX_WINDOW or k % 2 == 0:
+            raise ValueError(f"{name}: light_window must be an odd integer in [3, {ops.LIGHT_MAX_WINDOW}], got {k!r}")
     auto = isinstance(fp.curve, str) and fp.curve == "auto"
     if auto and fp.skew is not None:
         raise ValueError(f"{name}: curve and skew are both given (curl together with skew is not supported)")
@@ -2425,14 +2439,18 @@ def _check_flat(fp, H, W, name):
     return rect
 
 
-def _flat_bytes(fp, size):
-    """Device bytes of a flat page of frame ``size`` beyond its search: the flat page, and for a curled page its column table
-    at the column cap and the tracing of one block as large as the frame."""
+def _flat_bytes(fp, size, crop):
+    """Device bytes of a flat page of frame ``size`` beyond its search: the flat page, for a curled page its column table
+    at the column cap and the tracing of one block as large as the frame, and for an evened page the evened frame (the crop
+    ``crop`` of a skewed page) and the scratch of the evening."""
     from . import ops
     w, h = size
     n = 3 * w * h
     if fp.curve is not None:
         n += w * (12 + 16 * ops.FLAT_MAX_COLUMN_LINES) + ops.curve_block_bytes(w, h, fp.strips)
+    if fp.light is not None:
+        frame = crop if fp.skew is not None else size
+        n += ops.even_light_bytes(*max(size, frame, key=lambda s: s[0] * s[1]), frame)
     return n
 
 
@@ -2442,7 +2460,8 @@ def _check_flat_work(items, names):
     page search's limit."""
     total = 0
     for (_, fp, rect), name in zip(items, names):
-        total += _flat_bytes(fp, _flat_frame(fp, rect) or (rect[2] - rect[0], rect[3] - rect[1]))
+        crop = (rect[2] - rect[0], rect[3] - rect[1])
+        total += _flat_bytes(fp, _flat_frame(fp, rect) or crop, crop)
         if total > FLAT_MAX_WORK:
             raise ValueError(f"{name}: the call's flat pages up to this one need {total} bytes of work memory, over the "
                              f"{FLAT_MAX_WORK} a call may use (split the call)")
@@ -2503,7 +2522,12 @@ def flatten_pages(images, pages, to_host=False):
     upright, every one in one ops.warp_affine launch.  A curled page's blocks are found on its frame and traced (find_blocks'
     and find_lines' stages), and every page with a curled line goes through ops.flat_remap's two launches; a page whose lines
     all come back level is flattened as without curve.  Raises ValueError naming the image and the page, before any launch,
-    for a page its rules reject, and after the search for a page without a page found or over a limit."""
+    for a page its rules reject, and after the search for a page without a page found or over a limit.
+    A page with ``light="even"`` (DESIGN.md 7b, "Even lighting") has its frame evened first, every light page in one
+    ops.even_light call (six launches), and its searches after the corners' read the evened frame; a skewed or curled light
+    page is evened again after its warp or remap (four more launches for all of them).  Its dict gains ``light_window`` (the
+    k used) and ``ink`` ("dark" or "light").  The ink comes back with the call's first synchronisation after the evening; a
+    call with no search and no ``to_host`` waits once for it, and only when an ink is "auto"."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
@@ -2542,10 +2566,27 @@ def flatten_pages(images, pages, to_host=False):
                 frames[k] = dimg[i][y0:y1, x0:x1]
             if k in frames:
                 src[("frame", k)] = frames[k]
+        light = [k for k, (_, fp, _) in enumerate(items) if fp.light is not None]
+        win, inks = {}, {}
+        if light:                       # each page's frame evened, in one ops.even_light call; the searches read it
+            crops = [frames.get(k, dimg[i][y0:y1, x0:x1]) for k, (i, _, (x0, y0, x1, y1)) in ((k, items[k]) for k in light)]
+            evened = _flat_views([tuple(c.shape[:2]) for c in crops], dev)
+            for k, c in zip(light, crops):
+                win[k] = items[k][1].light_window or ops.light_window(c.shape[1], c.shape[0])
+            table = ops.even_light([(c, c, e, win[k], _INK[items[k][1].polarity]) for k, c, e in zip(light, crops, evened)])
+            inks = dict(zip(light, table.unbind(0)))
+            ink_host = torch.empty(len(light), 4, dtype=torch.int32, pin_memory=True)
+            ink_host.copy_(table, non_blocking=True)    # complete at the call's next synchronisation
+            for k, e in zip(light, evened):
+                if items[k][1].skew is None:
+                    frames[k] = src[("frame", k)] = e
+                else:
+                    src[("light", k)] = e
         search = [k for k, (_, fp, _) in enumerate(items) if fp.curve is not None or isinstance(fp.skew, str)]
-        sitems = [(i, _flat_text_page(fp), rect) if fp.curve is None else
-                  (("frame", k), TextPage(None, fp.direction, fp.polarity, fp.gap_x, fp.gap_y),
-                   (0, 0, frames[k].shape[1], frames[k].shape[0])) for k, (i, fp, rect) in ((k, items[k]) for k in search)]
+        sitems = [(i, _flat_text_page(fp), rect) if fp.curve is None and k not in inks else
+                  (("light", k), _flat_text_page(fp, rect=None), (0, 0, rect[2] - rect[0], rect[3] - rect[1])) if fp.curve is None
+                  else (("frame", k), TextPage(None, fp.direction, fp.polarity, fp.gap_x, fp.gap_y),
+                        (0, 0, frames[k].shape[1], frames[k].shape[0])) for k, (i, fp, rect) in ((k, items[k]) for k in search)]
         pres = dict(zip(search, _find_blocks(src, sitems) if sitems else []))
         for k, r in pres.items():
             if isinstance(r, str):
@@ -2578,7 +2619,7 @@ def flatten_pages(images, pages, to_host=False):
             else:
                 sizes.append(tuple(frames[k].shape[:2]))
         views = _flat_views(sizes, dev)
-        warps, remaps, res = [], [], []
+        warps, remaps, res, again = [], [], [], []
         for k, ((i, fp, (x0, y0, x1, y1)), dst) in enumerate(zip(items, views)):
             d = dict(image=dst, kind="quad" if fp.quad is not None else "skew" if fp.skew is not None else "rect",
                      size=(dst.shape[1], dst.shape[0]))
@@ -2602,14 +2643,28 @@ def flatten_pages(images, pages, to_host=False):
                 d["quad"] = _quad_key(i, fp.quad)[1]
             if k in lines:
                 d["lines"] = [q for _, ls in lines[k] for q in ls]
+            if k in inks:
+                d["light_window"] = win[k]
+                if fp.skew is not None or curled:
+                    again.append(k)
             res.append(d)
         if warps:
             ops.warp_affine(warps)
         if remaps:
             ops.flat_remap(remaps)
+        if again:                       # skewed and curled pages evened in place, with their frame's window and ink
+            ops.even_light([(None, views[k], views[k], win[k], None) for k in again], inks=[inks[k] for k in again])
         if to_host:
             for d, v in zip(res, _to_host_all([d["image"] for d in res])):
                 d["image"] = v
+        if light:
+            # The ink copy went out before every search and before the pages' copy back, so it has landed if either ran; a
+            # call with neither waits for it only when an ink is "auto".
+            if not (sitems or to_host) and any(items[k][1].polarity == "auto" for k in light):
+                torch.cuda.current_stream(dev).synchronize()
+            for j, k in enumerate(light):
+                pol = items[k][1].polarity
+                res[k]["ink"] = pol if pol != "auto" else "dark" if int(ink_host[j, 2]) == ops._lib.INK_DARK else "light"
     for (i, _, _), d in zip(items, res):
         out[i].append(d)
     return out
