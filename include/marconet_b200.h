@@ -797,7 +797,14 @@ int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* c
  * the page has more than MN_PAGE_MAX_BLOCKS blocks.  hist, bits, list[2], leaves, nch, nopen, off, b.out (threshold and ink)
  * and res are device memory inside work (work_bytes, zeroed by the call); list[k], leaves, nch, nopen and off hold cap entries, with
  * cap <= min(MN_PAGE_MAX_NODES, (h + 1) (w + 1) / 4).  The state fields are zero on entry.  blocks, pages: DEVICE arrays
- * (validated by the caller: 1 <= w, h <= 32767, the crop inside its image). */
+ * (validated by the caller: 1 <= w, h <= 32767, the crop inside its image).
+ * Ruled pages (DESIGN.md section 7b, "Ruled pages"): a page with rbits (inside work) has rule pixels U, the ink pixels in a
+ * maximal row or column run of at least rule_length.  A call with ruled != 0 issues 3 more launches after the bitmap, whatever
+ * the number of pages: the bitmap transposed into rbits' scratch, the long runs of every row of both planes, and the column
+ * runs transposed back into rbits, U cleared from bits and |U| counted into res->rule_pixels.  In such a page's XY-cut an index
+ * whose U count is at least half the node's extent is white, and a white run holding one cuts whatever its length; a block
+ * grows by q on each side only up to the nearest row (column) of its margin with U in its columns (rows).  Pages without
+ * rbits take the path of a call with ruled = 0, and a call with ruled = 0 issues exactly the launches above. */
 #define MN_PAGE_LEVELS 24
 #define MN_PAGE_MAX_BLOCKS 1024
 #define MN_PAGE_MAX_NODES 65536
@@ -814,6 +821,7 @@ typedef struct {
 typedef struct {
     int32_t error, n_leaves, n_blocks, text_size;
     int32_t gap_x, gap_y, threshold, ink;
+    int32_t rule_pixels, pad;   /* |U| of a ruled page (DESIGN.md section 7b, "Ruled pages"), else 0 */
 } mn_page_result;
 typedef struct {
     mn_text_block b;            /* the crop record (b.hist, b.out as mn_find_lines_u8's) */
@@ -826,9 +834,11 @@ typedef struct {
     mn_page_result* res;
     int32_t wpitch, cap, gap_x, gap_y;   /* gap_x, gap_y: 0 = the default */
     int32_t src, active, open, gx, gy, pad, n[2];   /* state, written by the call */
+    uint32_t* rbits;            /* null, or a ruled page's h x wpitch words of U followed by w x ceil(h / 32) words of scratch */
+    int32_t rule_length, pad2;  /* a ruled page's rule length, 2 <= rule_length <= 32767 */
 } mn_text_page;
-int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, void* work, long long work_bytes,
-                      void* stream);
+int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, int ruled, void* work,
+                      long long work_bytes, void* stream);
 
 /* Skewed pages (DESIGN.md section 7b, "Skewed pages").  Page i is searched as a skewed block on skew[i] (skew[i].b, blocks[i] and
  * pages[i].b the same crop record on entry; a page without skew the one-entry table (1, 0)), and the XY-cut of
@@ -838,11 +848,12 @@ int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, l
  *   5. the frame bitmap: bit j & 31 of bits[k wpitch + j / 32] is set iff an ink pixel has cell (k, j) in the frame at (c, s),
  *      or for a vertical page at (c, -s) on the untransposed crop (the transposed search frame with its axes swapped); the root
  *      node, and pages[i].b.w = M, pages[i].b.h = L;
- *   6-13. mn_find_blocks_u8's levels, text size and leaves, in frame cells.
+ *   6-13. mn_find_blocks_u8's levels, text size and leaves, in frame cells (after its 3 rule launches under ruled != 0; a
+ *         ruled page has skew None, so its frame bitmap is mn_find_blocks_u8's).
  * bits holds max L x wpitch words, wpitch >= max M / 32, and cap entries per list, max over the page's table; the angle
  * profiles and scores are as mn_find_lines_skewed_u8's (b.prof unused).  work (work_bytes) is zeroed by the call. */
-int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles, void* work,
-                             long long work_bytes, void* stream);
+int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles, int ruled,
+                             void* work, long long work_bytes, void* stream);
 
 /* Windowed blocks (DESIGN.md section 7b, "Skewed pages").  Block i is the set of pixels of the crop wins[i].b whose frame cell
  * (k, j) at (c, s) (the frame of "Skewed blocks", transposed crop for a vertical block) lies in [c0, c1) x [l0, l1).

@@ -219,14 +219,14 @@ class PageNode(Structure):
 
 class PageResult(Structure):
     _fields_ = [("error", c_int32), ("n_leaves", c_int32), ("n_blocks", c_int32), ("text_size", c_int32), ("gap_x", c_int32),
-                ("gap_y", c_int32), ("threshold", c_int32), ("ink", c_int32)]
+                ("gap_y", c_int32), ("threshold", c_int32), ("ink", c_int32), ("rule_pixels", c_int32), ("pad", c_int32)]
 
 
 class TextPage(Structure):
     _fields_ = [("b", TextBlock), ("bits", c_void_p), ("list", c_void_p * 2), ("leaves", c_void_p), ("nch", c_void_p),
                 ("nopen", c_void_p), ("off", c_void_p), ("res", c_void_p), ("wpitch", c_int32), ("cap", c_int32),
                 ("gap_x", c_int32), ("gap_y", c_int32), ("src", c_int32), ("active", c_int32), ("open", c_int32), ("gx", c_int32),
-                ("gy", c_int32), ("pad", c_int32), ("n", c_int32 * 2)]
+                ("gy", c_int32), ("pad", c_int32), ("n", c_int32 * 2), ("rbits", c_void_p), ("rule_length", c_int32), ("pad2", c_int32)]
 
 
 class PageQuad(Structure):
@@ -303,8 +303,8 @@ SYMBOLS = {
     "mn_even_light_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_longlong, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_skewed_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
-    "mn_find_blocks_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
-    "mn_find_blocks_skewed_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
+    "mn_find_blocks_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_int, c_void_p, c_longlong, c_void_p]),
+    "mn_find_blocks_skewed_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_int, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_window_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_curved_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_int, c_void_p, c_longlong, c_void_p]),
     "mn_find_page_quads_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),

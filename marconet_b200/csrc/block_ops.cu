@@ -7,7 +7,10 @@
 // bitmap of rotated-frame cells, and their blocks are windows of that frame.  Perspective pages (DESIGN.md 7b, "Perspective
 // pages") find a photographed page's corners: the paper's largest 4-connected component, its hull and the largest quad on it.
 // Curled blocks (DESIGN.md 7b, "Curled blocks") trace each line across column strips: per-strip profiles and runs, and a
-// left-to-right link of the runs into lines, in seven launches.
+// left-to-right link of the runs into lines, in seven launches.  Ruled pages (DESIGN.md 7b, "Ruled pages") find the ink runs of at
+// least a rule length in rows and columns in three more launches, take them out of the page's bitmap and let them cut.
+#include <climits>
+
 #include "mn_common.cuh"
 
 namespace {
@@ -855,8 +858,9 @@ constexpr int kSpanWords = 1024;                       // one bit per index of a
 constexpr int kScanThreads = 1024;
 
 struct page_smem {
-    int cnt[kChunk];
+    int cnt[kChunk];                                   // ink count, plus the U count << 16 on a ruled page
     unsigned nw[kSpanWords];                           // bit i: index lo + i of the node's span is not white
+    unsigned ru[kSpanWords];                           // bit i: index lo + i is a rule index (ruled pages only)
     int scan[32];
     int first;
 };
@@ -928,21 +932,30 @@ __device__ int cta_max_scan(int v, int* s, int* total) {
 }
 
 // The node's non-white indices along its axis into s.nw: index l is white iff its ink count < max(1, extent / 128), extent the
-// node's length on the other axis.  Ends with a barrier.
+// node's length on the other axis.  On a ruled page its rule indices (2 u >= extent, u the U count) go to s.ru and are white
+// too; counts fit 16 bits (<= 32767), so u rides in the high half of s.cnt.  Ends with a barrier.
 __device__ __forceinline__ void node_profile(const mn_text_page& p, const mn_page_node& nd, bool rows, page_smem& s) {
     const int lo = rows ? nd.y0 : nd.x0, L = (rows ? nd.y1 : nd.x1) - lo;
-    const int m = max(1, (rows ? nd.x1 - nd.x0 : nd.y1 - nd.y0) / 128);
+    const int ext = rows ? nd.x1 - nd.x0 : nd.y1 - nd.y0, m = max(1, ext / 128);
+    const bool ruled = p.rbits != nullptr;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
     __syncthreads();                                    // the previous node's readers of s are done
-    for (int j = threadIdx.x; j < kSpanWords; j += blockDim.x) s.nw[j] = 0u;
+    for (int j = threadIdx.x; j < kSpanWords; j += blockDim.x) {
+        s.nw[j] = 0u;
+        if (ruled) s.ru[j] = 0u;
+    }
     for (int c0 = 0; c0 < L; c0 += kChunk) {
         const int n = min(kChunk, L - c0);
         if (rows) {
             const int wx0 = nd.x0 >> 5, wx1 = (nd.x1 - 1) >> 5;
             for (int r = warp; r < n; r += n_warps) {
-                const uint32_t* row = p.bits + (long long)(lo + c0 + r) * p.wpitch;
+                const long long o = (long long)(lo + c0 + r) * p.wpitch;
                 int c = 0;
-                for (int wd = wx0 + lane; wd <= wx1; wd += 32) c += __popc(row[wd] & word_mask(wd, nd.x0, nd.x1));
+                for (int wd = wx0 + lane; wd <= wx1; wd += 32) {
+                    const unsigned mk = word_mask(wd, nd.x0, nd.x1);
+                    c += __popc(p.bits[o + wd] & mk);
+                    if (ruled) c += __popc(p.rbits[o + wd] & mk) << 16;
+                }
                 c = (int)__reduce_add_sync(0xffffffffu, (unsigned)c);
                 if (lane == 0) s.cnt[r] = c;
             }
@@ -955,13 +968,23 @@ __device__ __forceinline__ void node_profile(const mn_text_page& p, const mn_pag
                 const int y = nd.y0 + k / nwords, wd = w0 + k % nwords;
                 for (unsigned v = p.bits[(long long)y * p.wpitch + wd] & word_mask(wd, a, e); v; v &= v - 1u)
                     atomicAdd(&s.cnt[(wd << 5) + __ffs(v) - 1 - a], 1);
+                if (ruled) {
+                    for (unsigned v = p.rbits[(long long)y * p.wpitch + wd] & word_mask(wd, a, e); v; v &= v - 1u)
+                        atomicAdd(&s.cnt[(wd << 5) + __ffs(v) - 1 - a], 1 << 16);
+                }
             }
         }
         __syncthreads();
         for (int j = threadIdx.x; 32 * j < n; j += blockDim.x) {
-            unsigned v = 0u;
-            for (int t = 0; t < 32 && 32 * j + t < n; ++t) v |= (unsigned)(s.cnt[32 * j + t] >= m) << t;
+            unsigned v = 0u, r = 0u;
+            for (int t = 0; t < 32 && 32 * j + t < n; ++t) {
+                const int c = s.cnt[32 * j + t];
+                const bool rule = ruled && 2 * (c >> 16) >= ext;
+                v |= (unsigned)(!rule && (c & 0xffff) >= m) << t;
+                r |= (unsigned)rule << t;
+            }
             s.nw[(c0 >> 5) + j] = v;
+            if (ruled) s.ru[(c0 >> 5) + j] = r;
         }
         __syncthreads();
     }
@@ -980,39 +1003,51 @@ __device__ __forceinline__ void child_end(mn_page_node* c, bool rows, int e) {
     if (rows) c->y1 = (int16_t)e; else c->x1 = (int16_t)e;
 }
 
+// The last rule index before index b of word j (32 j <= b < 32 j + 32), lr the last one before word j (-1: none).
+__device__ __forceinline__ int rule_before(unsigned ru, int j, int b, int lr) {
+    const unsigned below = ru & ((1u << (b & 31)) - 1u);
+    return below ? 32 * j + 31 - __clz(below) : lr;
+}
+
 // One attempt on the open node nd (every thread of the CTA): returns its number of children (0: dropped) and, in *n_open, how
-// many of them stay open.  With kEmit, writes them into dst[0 ..) in reading order.
+// many of them stay open.  With kEmit, writes them into dst[0 ..) in reading order.  A white run between the non-white
+// indices prev and b cuts when it is at least g long or, on a ruled page, holds a rule index (the last one before b > prev).
 template <bool kEmit>
 __device__ __forceinline__ int page_attempt(const mn_text_page& p, const mn_page_node& nd, bool last_level, page_smem& s, mn_page_node* dst,
                             int* n_open) {
     const bool rows = nd.st & MN_PAGE_ROWS;
     const int lo = rows ? nd.y0 : nd.x0, g = rows ? p.gy : p.gx;
     const int o0 = rows ? nd.x0 : nd.y0, o1 = rows ? nd.x1 : nd.y1, failed = nd.st & MN_PAGE_FAILED;
+    const bool ruled = p.rbits != nullptr;
     if (threadIdx.x == 0) s.first = 1 << 30;
     node_profile(p, nd, rows, s);
     constexpr int kPer = kSpanWords / kPageThreads;
     const int j0 = threadIdx.x * kPer;
-    int my_first = 1 << 30, my_last = -1;
+    int my_first = 1 << 30, my_last = -1, my_rule = -1;
     for (int j = j0; j < j0 + kPer; ++j) {
         const unsigned v = s.nw[j];
         if (v) {
             my_first = min(my_first, 32 * j + __ffs(v) - 1);
             my_last = 32 * j + 31 - __clz(v);
         }
+        if (ruled && s.ru[j]) my_rule = 32 * j + 31 - __clz(s.ru[j]);
     }
     if (my_last >= 0) atomicMin(&s.first, my_first);
-    int last;
+    int last, any_rule;
     const int prev0 = cta_max_scan(my_last, s.scan, &last);
+    const int rule0 = ruled ? cta_max_scan(my_rule, s.scan, &any_rule) : -1;
     *n_open = 0;
     if (last < 0) return 0;
     const int first = s.first;
-    int c = 0, prev = prev0;
+    int c = 0, prev = prev0, lr = rule0;
     for (int j = j0; j < j0 + kPer; ++j) {
+        const unsigned ru = ruled ? s.ru[j] : 0u;
         for (unsigned v = s.nw[j]; v; v &= v - 1u) {
             const int b = 32 * j + __ffs(v) - 1;
-            c += prev >= 0 && b - prev - 1 >= g;
+            c += prev >= 0 && (b - prev - 1 >= g || rule_before(ru, j, b, lr) > prev);
             prev = b;
         }
+        if (ru) lr = 32 * j + 31 - __clz(ru);
     }
     int cuts;
     int k = cta_scan(c, s.scan, &cuts);
@@ -1029,16 +1064,19 @@ __device__ __forceinline__ int page_attempt(const mn_text_page& p, const mn_page
         const bool rev = !rows && p.b.vertical;          // columns of a vertical page read right to left
         const int st = (rows ? 0 : MN_PAGE_ROWS) | (last_level ? MN_PAGE_LEAF : 0);
         prev = prev0;
+        lr = rule0;
         for (int j = j0; j < j0 + kPer; ++j) {
+            const unsigned ru = ruled ? s.ru[j] : 0u;
             for (unsigned v = s.nw[j]; v; v &= v - 1u) {
                 const int b = 32 * j + __ffs(v) - 1;
-                if (prev >= 0 && b - prev - 1 >= g) {
+                if (prev >= 0 && (b - prev - 1 >= g || rule_before(ru, j, b, lr) > prev)) {
                     child_end(dst + (rev ? cuts - k : k), rows, lo + prev + 1);
                     child_start(dst + (rev ? cuts - k - 1 : k + 1), rows, lo + b, o0, o1, st);
                     ++k;
                 }
                 prev = b;
             }
+            if (ru) lr = 32 * j + 31 - __clz(ru);
         }
         if (threadIdx.x == 0) {
             child_start(dst + (rev ? cuts : 0), rows, lo + first, o0, o1, st);
@@ -1171,7 +1209,24 @@ __global__ void __launch_bounds__(kScanThreads) page_size_kernel(mn_text_page* p
     p.open = 1;
 }
 
-// 11. The leaves, one warp each: rejected when 2 ink > h w or min(h, w) < max(1, S / 3), else a block grown by q and clipped.
+// The greatest (kMin: least) row (kRows) or column of the rectangle [xa, xb) x [ya, yb) of a ruled page that holds a U pixel,
+// over the warp: -1 (kMin: 1 << 30) when there is none.
+template <bool kRows, bool kMin>
+__device__ int rule_edge(const mn_text_page& p, int xa, int ya, int xb, int yb) {
+    const int w0 = xa >> 5, nwords = xb > xa ? ((xb - 1) >> 5) - w0 + 1 : 0;
+    int best = kMin ? 1 << 30 : -1;
+    for (int k = threadIdx.x & 31; k < nwords * max(0, yb - ya); k += 32) {
+        const int y = ya + k / nwords, wd = w0 + k % nwords;
+        const unsigned m = p.rbits[(long long)y * p.wpitch + wd] & word_mask(wd, xa, xb);
+        if (!m) continue;
+        const int v = kRows ? y : kMin ? 32 * wd + __ffs(m) - 1 : 32 * wd + 31 - __clz(m);
+        best = kMin ? min(best, v) : max(best, v);
+    }
+    return kMin ? __reduce_min_sync(0xffffffffu, best) : __reduce_max_sync(0xffffffffu, best);
+}
+
+// 11. The leaves, one warp each: rejected when 2 ink > h w or min(h, w) < max(1, S / 3), else a block grown by q and clipped;
+// on a ruled page each side stops short of the nearest row (column) of its margin with U in the leaf's columns (rows).
 __global__ void __launch_bounds__(kScanThreads) page_blocks_kernel(mn_text_page* pages) {
     mn_pdl_prologue();
     __shared__ int s_blocks;
@@ -1199,12 +1254,23 @@ __global__ void __launch_bounds__(kScanThreads) page_blocks_kernel(mn_text_page*
 #pragma unroll
         for (int o = 16; o; o >>= 1) ink += __shfl_xor_sync(0xffffffffu, ink, o);
         const int h = nd.y1 - nd.y0, w = nd.x1 - nd.x0;
+        const bool reject = 2 * ink > (long long)h * w || min(h, w) < min_side;
+        int x0 = max(0, nd.x0 - q), y0 = max(0, nd.y0 - q), x1 = min(p.b.w, nd.x1 + q), y1 = min(p.b.h, nd.y1 + q);
+        if (!reject && p.rbits) {
+            const int top = rule_edge<true, false>(p, nd.x0, y0, nd.x1, nd.y0);
+            const int bottom = rule_edge<true, true>(p, nd.x0, nd.y1, nd.x1, y1);
+            const int left = rule_edge<false, false>(p, x0, nd.y0, nd.x0, nd.y1);
+            const int right = rule_edge<false, true>(p, nd.x1, nd.y0, x1, nd.y1);
+            y0 = top >= 0 ? top + 1 : y0;
+            y1 = min(y1, bottom);
+            x0 = left >= 0 ? left + 1 : x0;
+            x1 = min(x1, right);
+        }
         if (lane != 0) continue;
-        if (2 * ink > (long long)h * w || min(h, w) < min_side) {
+        if (reject) {
             nd.st |= MN_PAGE_REJECTED;
         } else {
-            nd.x0 = (int16_t)max(0, nd.x0 - q); nd.y0 = (int16_t)max(0, nd.y0 - q);
-            nd.x1 = (int16_t)min(p.b.w, nd.x1 + q); nd.y1 = (int16_t)min(p.b.h, nd.y1 + q);
+            nd.x0 = (int16_t)x0; nd.y0 = (int16_t)y0; nd.x1 = (int16_t)x1; nd.y1 = (int16_t)y1;
             atomicAdd(&s_blocks, 1);
         }
         p.leaves[i] = nd;
@@ -1217,6 +1283,147 @@ __global__ void __launch_bounds__(kScanThreads) page_blocks_kernel(mn_text_page*
     }
 }
 
+// ---- Ruled pages (DESIGN.md 7b, "Ruled pages") ----
+// U, the ink pixels in a maximal row or column run of at least rule_length, for every ruled page of a call in three launches:
+// the bitmap transposed into the scratch plane after rbits (w rows of ceil(h / 32) words, so that columns are rows), the long
+// runs of every row of both planes, and the column runs transposed back, OR'd into rbits and cleared from bits.  A row of up to
+// 1024 words is one warp's: per-iteration summaries of its zeros and two warp scans give each word the ink runs that continue
+// past its ends, so the work is O(1) per word for any rule length.  Pages without rbits return at once.
+constexpr int kRuleThreads = 256;
+
+__device__ __forceinline__ uint32_t* rule_plane(const mn_text_page& p) { return p.rbits + (long long)p.b.h * p.wpitch; }
+
+// A 32 x 32 bit transpose across the warp: lane r holds row r; returns column `lane` (bit r = row r's bit lane).
+__device__ __forceinline__ unsigned warp_transpose(unsigned v) {
+    unsigned out = 0u;
+#pragma unroll
+    for (int c = 0; c < 32; ++c) {
+        const unsigned t = __ballot_sync(0xffffffffu, (v >> c) & 1u);
+        if ((threadIdx.x & 31) == c) out = t;
+    }
+    return out;
+}
+
+// Max of v over the lanes below this one (INT_MIN for lane 0), and min over the lanes above (INT_MAX for lane 31).
+__device__ __forceinline__ int warp_max_below(int v) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v = max(v, y);
+    }
+    const int e = __shfl_up_sync(0xffffffffu, v, 1);
+    return lane ? e : INT_MIN;
+}
+__device__ __forceinline__ int warp_min_above(int v) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_down_sync(0xffffffffu, v, o);
+        if (lane + o < 32) v = min(v, y);
+    }
+    const int e = __shfl_down_sync(0xffffffffu, v, 1);
+    return lane < 31 ? e : INT_MAX;
+}
+
+// The bits of the word v in runs of ones at least l long, the run at bit 0 continuing `before` ones below the word and the run
+// at bit 31 `after` ones above it.
+__device__ __forceinline__ unsigned long_runs(unsigned v, int before, int after, int l) {
+    unsigned out = 0u;
+    while (v) {
+        const int a = __ffs(v) - 1;
+        const unsigned rest = ~(v >> a);                // zero only for a = 0 and v all ones
+        const int len = rest ? __ffs(rest) - 1 : 32;
+        const unsigned run = (len == 32 ? ~0u : (1u << len) - 1u) << a;
+        if (len + (a == 0 ? before : 0) + (a + len == 32 ? after : 0) >= l) out |= run;
+        v &= ~run;
+    }
+    return out;
+}
+
+// One line of n bits in words src[0 .. ceil(n / 32)) (bits past n zero; outside the line is paper) by the warp: dst[k] = the
+// bits of src[k] in maximal runs of at least l ones.  dst may be src.
+__device__ __forceinline__ void line_runs(const uint32_t* src, uint32_t* dst, int n, int l) {
+    const int lane = threadIdx.x & 31, nwords = (n + 31) >> 5, nit = (nwords + 31) >> 5;
+    int lz = -1, fz = INT_MAX;                          // lane `it`: the last and first zero of iteration it's 32 words
+    for (int it = 0; it < nit; ++it) {
+        const int k = 32 * it + lane;
+        const unsigned z = ~(k < nwords ? src[k] : 0u);
+        const int a = __reduce_max_sync(0xffffffffu, z ? 32 * k + 31 - __clz(z) : -1);
+        const int b = __reduce_min_sync(0xffffffffu, z ? 32 * k + __ffs(z) - 1 : INT_MAX);
+        if (lane == it) {
+            lz = a;
+            fz = b;
+        }
+    }
+    const int lz_before = max(-1, warp_max_below(lz)), fz_after = min(32 * nwords, warp_min_above(fz));
+    for (int it = 0; it < nit; ++it) {
+        const int k = 32 * it + lane;
+        const unsigned v = k < nwords ? src[k] : 0u, z = ~v;
+        const int zb = max(__shfl_sync(0xffffffffu, lz_before, it), warp_max_below(z ? 32 * k + 31 - __clz(z) : -1));
+        const int za = min(__shfl_sync(0xffffffffu, fz_after, it), warp_min_above(z ? 32 * k + __ffs(z) - 1 : INT_MAX));
+        const unsigned m = long_runs(v, 32 * k - zb - 1, za - 32 * k - 32, l);
+        if (k < nwords) dst[k] = m;
+    }
+}
+
+// R1. The bitmap's 32 x 32 tiles transposed into the scratch plane, one warp per tile.
+__global__ void __launch_bounds__(kRuleThreads) rule_transpose_kernel(mn_text_page* pages) {
+    mn_pdl_prologue();
+    const mn_text_page& p = pages[blockIdx.y];
+    if (!p.rbits) return;
+    const int w = p.b.w, h = p.b.h, nw = (w + 31) >> 5, th = (h + 31) >> 5, lane = threadIdx.x & 31;
+    constexpr int kWarps = kRuleThreads / 32;
+    uint32_t* tp = rule_plane(p);
+    for (long long t = (long long)blockIdx.x * kWarps + (threadIdx.x >> 5); t < (long long)nw * th; t += (long long)gridDim.x * kWarps) {
+        const int ty = (int)(t % th), wd = (int)(t / th), y = 32 * ty + lane, x = 32 * wd + lane;
+        const unsigned c = warp_transpose(y < h ? p.bits[(long long)y * p.wpitch + wd] : 0u);
+        if (x < w) tp[(long long)x * th + ty] = c;
+    }
+}
+
+// R2. The long runs of the h rows of bits into rbits, and of the w rows of the scratch plane in place, one warp per row.
+__global__ void __launch_bounds__(kRuleThreads, 1) rule_runs_kernel(mn_text_page* pages) {
+    mn_pdl_prologue();
+    const mn_text_page& p = pages[blockIdx.y];
+    if (!p.rbits) return;
+    const int w = p.b.w, h = p.b.h, th = (h + 31) >> 5;
+    constexpr int kWarps = kRuleThreads / 32;
+    uint32_t* tp = rule_plane(p);
+    for (int i = blockIdx.x * kWarps + (threadIdx.x >> 5); i < h + w; i += gridDim.x * kWarps) {
+        if (i < h) line_runs(p.bits + (long long)i * p.wpitch, p.rbits + (long long)i * p.wpitch, w, p.rule_length);
+        else line_runs(tp + (long long)(i - h) * th, tp + (long long)(i - h) * th, h, p.rule_length);
+    }
+}
+
+// R3. The column runs transposed back and OR'd into rbits (U), U cleared from bits (I' = I and not U), |U| into res.
+__global__ void __launch_bounds__(kRuleThreads) rule_merge_kernel(mn_text_page* pages) {
+    mn_pdl_prologue();
+    __shared__ int s_count;
+    const mn_text_page& p = pages[blockIdx.y];
+    if (!p.rbits) return;
+    const int w = p.b.w, h = p.b.h, nw = (w + 31) >> 5, th = (h + 31) >> 5, lane = threadIdx.x & 31;
+    constexpr int kWarps = kRuleThreads / 32;
+    const uint32_t* tp = rule_plane(p);
+    if (threadIdx.x == 0) s_count = 0;
+    __syncthreads();
+    int count = 0;
+    for (long long t = (long long)blockIdx.x * kWarps + (threadIdx.x >> 5); t < (long long)nw * th; t += (long long)gridDim.x * kWarps) {
+        const int ty = (int)(t % th), wd = (int)(t / th), y = 32 * ty + lane, x = 32 * wd + lane;
+        const unsigned r = warp_transpose(x < w ? tp[(long long)x * th + ty] : 0u);
+        if (y < h) {
+            const long long o = (long long)y * p.wpitch + wd;
+            const unsigned u = p.rbits[o] | r;
+            p.rbits[o] = u;
+            p.bits[o] &= ~u;
+            count += __popc(u);
+        }
+    }
+    count = (int)__reduce_add_sync(0xffffffffu, (unsigned)count);
+    if (lane == 0 && count) atomicAdd(&s_count, count);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_count) atomicAdd(&p.res->rule_pixels, s_count);
+}
 
 // ---- Skewed pages (DESIGN.md 7b, "Skewed pages") ----
 // The page's angle is searched by the skewed-block kernels on its mn_skew_block record; the XY-cut then runs unchanged on a
@@ -1621,8 +1828,17 @@ __global__ void __launch_bounds__(kHullThreads) quad_hull_kernel(const mn_quad_p
 }
 
 // 4-11 of the XY-cut: both passes of levels, the text size between them and the leaves, on pages whose bitmap and root are
-// written.
-int page_levels(mn_text_page* pages, int n, cudaStream_t st) {
+// written; under `ruled`, the three rule launches first.
+int page_levels(mn_text_page* pages, int n, long long max_tiles, int ruled, cudaStream_t st) {
+    if (ruled) {
+        const dim3 rgrid((unsigned)mn_cdiv64(max_tiles, kRuleThreads / 32), (unsigned)n);
+        MN_CUDA_CHECK((mn_launch(rule_transpose_kernel, rgrid, dim3(kRuleThreads), 0, st, pages)));
+        MN_LAUNCH_CHECK();
+        MN_CUDA_CHECK((mn_launch(rule_runs_kernel, rgrid, dim3(kRuleThreads), 0, st, pages)));
+        MN_LAUNCH_CHECK();
+        MN_CUDA_CHECK((mn_launch(rule_merge_kernel, rgrid, dim3(kRuleThreads), 0, st, pages)));
+        MN_LAUNCH_CHECK();
+    }
     const dim3 grid((unsigned)max(1, 4 * mn_num_sms() / n), (unsigned)n);   // about four CTAs per SM over all pages
     for (int pass = 0; pass < 2; ++pass) {
         for (int level = 0; level < MN_PAGE_LEVELS; ++level) {
@@ -1692,7 +1908,7 @@ extern "C" int mn_find_lines_skewed_u8(mn_text_block* blocks, mn_skew_block* ske
     return MN_OK;
 }
 
-extern "C" int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, void* work,
+extern "C" int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, int ruled, void* work,
                                  long long work_bytes, void* stream) {
     MN_REQUIRE(blocks && pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
                "mn_find_blocks_u8: bad args");
@@ -1701,11 +1917,11 @@ extern "C" int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* page
     if (rc != MN_OK) return rc;
     MN_CUDA_CHECK((mn_launch(page_bits_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, pages)));
     MN_LAUNCH_CHECK();
-    return page_levels(pages, n, st);
+    return page_levels(pages, n, max_tiles, ruled, st);
 }
 
 extern "C" int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles,
-                                        void* work, long long work_bytes, void* stream) {
+                                        int ruled, void* work, long long work_bytes, void* stream) {
     MN_REQUIRE(blocks && skew && pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
                "mn_find_blocks_skewed_u8: bad args");
     cudaStream_t st = (cudaStream_t)stream;
@@ -1717,7 +1933,7 @@ extern "C" int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* sk
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(page_frame_bits_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, pages, skew)));
     MN_LAUNCH_CHECK();
-    return page_levels(pages, n, st);
+    return page_levels(pages, n, max_tiles, ruled, st);
 }
 
 extern "C" int mn_find_lines_window_u8(const mn_text_block* blocks, const mn_window_block* wins, int n, long long max_tiles,

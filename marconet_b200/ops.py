@@ -2092,6 +2092,18 @@ def page_bytes(w, h):
             + ctypes.sizeof(_lib.BlockLines) + 4 * h * -(-w // 32) + 3 * 4 * cap + 64)
 
 
+def rule_length(w, h):
+    """The default rule length of a w x h page frame (DESIGN.md 7b, "Ruled pages"): max(32, min(w, h) // 16).  A heuristic: a
+    glyph stroke at least this long counts as a rule."""
+    return max(32, min(w, h) // 16)
+
+
+def rule_page_bytes(w, h):
+    """Device bytes a w x h page adds to find_blocks when it has rules (DESIGN.md 7b, "Ruled pages"): its U bitmap (h rows of
+    ceil(w / 32) words) and the transposed bitmap's scratch (w rows of ceil(h / 32) words)."""
+    return 4 * (h * -(-w // 32) + w * -(-h // 32))
+
+
 def skew_page_frame(w, h, vertical, cs):
     """(L, M, stride) of a w x h page's frame bitmaps over the (c, s) of ``cs``: the most rows and columns a bitmap may have (the
     search frame's axes swapped for a vertical page) and the most bins of its search frames."""
@@ -2119,10 +2131,15 @@ def find_blocks(pages, scores=False):
     mn_find_blocks_skewed_u8's 7 + 6 * 24 launches instead, every page of it; pages with skew None search the one-entry table
     (1, 0) and keep their tables exactly.  out then starts with the n mn_skew_block records (``skew_block_dtype()``: the chosen
     index and frame) and the leaves are in frame cells.  ``scores`` (tests): also return, per page, the int64 CUDA view of its
-    per-angle scores (None unless it searched)."""
+    per-angle scores (None unless it searched).
+    rule_length (DESIGN.md 7b, "Ruled pages"), a ninth entry after skew and max_skew: None, or an integer in [2, 32767] on a
+    page with skew None, whose ink pixels in a maximal row or column run of at least that many pixels are its rules U.  A call
+    with such a page issues 3 more launches whatever the number of pages; its records gain rule_pixels (|U|), and the other
+    pages' tables are those of a call without it."""
     global LAUNCHES
     dev = _check_items(pages, "find_blocks", "page")
     skewed = any(len(p) > 6 and p[6] is not None for p in pages)
+    rules = [p[8] if len(p) > 8 else None for p in pages]
     n = len(pages)
     rsz, bsz, psz, lsz = (ctypes.sizeof(t) for t in (_lib.PageResult, _lib.TextBlock, _lib.TextPage, _lib.BlockLines))
     ssz = ctypes.sizeof(_lib.SkewBlock) if skewed else 0
@@ -2132,8 +2149,12 @@ def find_blocks(pages, scores=False):
         x0, y0, bw, bh = _check_crop(pg[:6], dev, what, "gap_x / gap_y")
         vertical, skew, max_skew = pg[2], pg[6] if len(pg) > 6 else None, pg[7] if len(pg) > 7 else 10.0
         cs = _check_skew(skew, max_skew, vertical, what)
+        rl = rules[i]
+        if rl is not None and (isinstance(rl, bool) or not isinstance(rl, int) or not 2 <= rl <= 32767 or skew is not None):
+            raise ValueError(f"{what}: rule_length {rl!r} is not an integer in [2, 32767] on a page with skew None")
         L, M, stride = (bh, bw, bw if vertical else bh) if skew is None else skew_page_frame(bw, bh, vertical, cs)
         need += skew_page_bytes(bw, bh, vertical, cs) if skewed else page_bytes(bw, bh)
+        need += rule_page_bytes(bw, bh) if rl is not None else 0
         if max(L, M) > 32767:
             raise ValueError(f"{what}: a frame side of {max(L, M)} exceeds 32767")
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
@@ -2150,7 +2171,8 @@ def find_blocks(pages, scores=False):
     n_out = n * rsz + 12 * sum(d[4] for d in dims)
     work0 = out0 + -(-n_out // 16) * 16
     per = [-(-(8 * (d[7] if d[7] > 1 else 0) + 4 * 256 + lsz + 4 * d[5] * -(-d[6] // 32) + 2 * 12 * d[4] + 3 * 4 * d[4]
-                + 4 * (d[7] * d[8] if d[7] > 1 else 0)) // 16) * 16 for d in dims]
+                + 4 * (d[7] * d[8] if d[7] > 1 else 0) + (rule_page_bytes(d[6], d[5]) if rl is not None else 0)) // 16) * 16
+           for d, rl in zip(dims, rules)]
     buf = torch.empty(work0 + sum(per), dtype=torch.uint8, device=dev)
     base = buf.data_ptr()
     leaves, w, blocks, srecs, recs, views, tiles = base + out0 + n * rsz, base + work0, [], [], [], [], 0
@@ -2162,12 +2184,14 @@ def find_blocks(pages, scores=False):
         lines, bits = hist + 4 * 256, hist + 4 * 256 + lsz
         lists = bits + 4 * L * wp
         counts = lists + 2 * 12 * cap
+        rbits = counts + 3 * 4 * cap + 4 * (n_ang * stride if n_ang > 1 else 0)
         tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, 0, 0, 0, 0, hist, 0, 0, lines)
         blocks.append(tb)
         if skewed:
             srecs.append(_skew_block(tb, base + tab0 + 16 * t, w, counts + 3 * 4 * cap, n_ang, stride))
         recs.append(_lib.TextPage(tb, bits, (ctypes.c_void_p * 2)(lists, lists + 12 * cap), leaves, counts, counts + 4 * cap,
-                                  counts + 8 * cap, base + out0 + i * rsz, wp, cap, gap_x or 0, gap_y or 0))
+                                  counts + 8 * cap, base + out0 + i * rsz, wp, cap, gap_x or 0, gap_y or 0,
+                                  rbits=rbits if rules[i] is not None else None, rule_length=rules[i] or 0))
         views.append(buf[w - base:w - base + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         leaves += 12 * cap
         w += nb
@@ -2175,14 +2199,15 @@ def find_blocks(pages, scores=False):
     host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.TextPage * n)(*recs)) + tab
     host += bytes(sk0 - len(host)) + bytes((_lib.SkewBlock * len(srecs))(*srecs))
     buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    ruled = int(any(rl is not None for rl in rules))
     if skewed:
-        _lib.check(_lib.load().mn_find_blocks_skewed_u8(base, base + sk0, base + pg0, n, tiles, base + out0,
+        _lib.check(_lib.load().mn_find_blocks_skewed_u8(base, base + sk0, base + pg0, n, tiles, ruled, base + out0,
                                                         work0 + sum(per) - out0, _stream()), "mn_find_blocks_skewed_u8")
-        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS
+        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS + 3 * ruled
     else:
-        _lib.check(_lib.load().mn_find_blocks_u8(base, base + pg0, n, tiles, base + out0, work0 + sum(per) - out0, _stream()),
-                   "mn_find_blocks_u8")
-        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS
+        _lib.check(_lib.load().mn_find_blocks_u8(base, base + pg0, n, tiles, ruled, base + out0, work0 + sum(per) - out0,
+                                                 _stream()), "mn_find_blocks_u8")
+        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS + 3 * ruled
     res = buf[sk0:out0 + n_out], [d[4] for d in dims]
     return res + (views,) if scores else res
 

@@ -2083,7 +2083,11 @@ class TextPage(NamedTuple):
     (DESIGN.md 7b, "Perspective pages"): None, a QuadRegion (the page's corners tl, tr, br, bl as it is read) or "auto" (the
     corners are found on the device); its blocks are found on the quad's rectified crop R and are TextBlock.from_quad(quad,
     window=...) windows of R.  With a quad, ``rect`` and ``skew`` are None.  ``curve`` (DESIGN.md 7b, "Curled blocks"): None, or
-    "auto" for a level horizontal page whose blocks are TextBlock(..., curve="auto"), each line traced as a CurvedRegion."""
+    "auto" for a level horizontal page whose blocks are TextBlock(..., curve="auto"), each line traced as a CurvedRegion.
+    ``rules`` (DESIGN.md 7b, "Ruled pages"): None, or "auto" for a page whose tables, forms and frames are drawn with ruling
+    lines: ink runs at least ``rule_length`` pixels long in a row or a column (an integer in [2, 32767]; default
+    max(32, min(w, h) // 16) of the crop, or of R for a quad page, a heuristic) are rules, which cut the page into cells and stop
+    its blocks.  Not with skew or curve: flatten such a page with flatten_pages first."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
@@ -2093,12 +2097,25 @@ class TextPage(NamedTuple):
     max_skew: float = 10.0
     quad: object = None
     curve: object = None
+    rules: object = None
+    rule_length: object = None
 
 
 def _check_page(pg, H, W, name):
     """The rectangle (x0, y0, x1, y1) of the TextPage ``pg`` of an H x W image, validated.  Raises ValueError naming ``name``."""
     from . import ops
     rect = (0, 0, W, H) if pg.rect is None else pg.rect
+    if pg.rules is not None and not (isinstance(pg.rules, str) and pg.rules == "auto"):
+        raise ValueError(f"{name}: rules must be None or 'auto', got {pg.rules!r}")
+    v = pg.rule_length
+    if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 2 <= v <= 32767):
+        raise ValueError(f"{name}: rule_length must be an integer in [2, 32767], got {v!r}")
+    if v is not None and pg.rules is None:
+        raise ValueError(f"{name}: rule_length is given, but rules is None, not 'auto'")
+    for what in ("skew", "curve"):
+        if pg.rules is not None and getattr(pg, what) is not None:
+            raise ValueError(f"{name}: rules and {what} are both given (a ruled page is level and flat: flatten a tilted or "
+                             f"curled page with flatten_pages first)")
     if pg.quad is not None:
         if pg.rect is not None:
             raise ValueError(f"{name}: rect and quad are both given (a page in perspective is its quad: give rect=None)")
@@ -2137,8 +2154,8 @@ def _page_table(pg):
 
 
 def _page_bytes(pg, rect, skewed):
-    """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages: a quad page's rectified crop and
-    its page, or an auto page's corner search on the image ``rect``."""
+    """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages, with a ruled page's two extra
+    bitmaps: a quad page's rectified crop and its page, or an auto page's corner search on the image ``rect``."""
     from . import ops
     w, h = rect[2] - rect[0], rect[3] - rect[1]
     if isinstance(pg.quad, str):
@@ -2146,9 +2163,11 @@ def _page_bytes(pg, rect, skewed):
     if pg.quad is not None:
         w_r, h_r = quad_maps(pg.quad, 1).size
         return 3 * w_r * h_r + _page_bytes(pg._replace(quad=None), (0, 0, w_r, h_r), skewed)
+    rules = ops.rule_page_bytes(w, h) if pg.rules is not None else 0
     if not skewed:
-        return ops.page_bytes(w, h)
-    return ops.skew_page_bytes(w, h, pg.direction == "vertical", _page_table(pg) if pg.skew is not None else [(1.0, 0.0)])
+        return ops.page_bytes(w, h) + rules
+    return rules + ops.skew_page_bytes(w, h, pg.direction == "vertical",
+                                       _page_table(pg) if pg.skew is not None else [(1.0, 0.0)])
 
 
 def _check_page_work(items):
@@ -2203,8 +2222,8 @@ def _find_pages(dimg, items, keys=()):
 def _find_blocks(dimg, items, rq=None):
     """ops.find_blocks over items (image index, TextPage, rect) of the uploaded images ``dimg``, its tables back through one
     pinned copy and one synchronisation; a quad page (its corners given) is a level page on all of its rectified crop in ``rq``
-    (_rectify).  Returns per item dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y), or the error message of a
-    page over a limit."""
+    (_rectify).  Returns per item dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, rule_length, rule_pixels]), or
+    the error message of a page over a limit."""
     from . import ops
     lib = ops._lib
 
@@ -2213,8 +2232,13 @@ def _find_blocks(dimg, items, rq=None):
             return dimg[i], rect
         r = rq[_quad_key(i, pg.quad)]
         return r, (0, 0, r.shape[1], r.shape[0])
+
+    def rule_length(i, pg, rect):                       # of the crop, or of R for a quad page
+        _, (x0, y0, x1, y1) = src(i, pg, rect)
+        return None if pg.rules is None else pg.rule_length or ops.rule_length(x1 - x0, y1 - y0)
+    rls = [rule_length(*it) for it in items]
     res_t, caps = ops.find_blocks([(*src(i, pg, rect), pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y,
-                                    pg.skew, pg.max_skew) for i, pg, rect in items])
+                                    pg.skew, pg.max_skew, rl) for (i, pg, rect), rl in zip(items, rls)])
     host = _to_host(res_t).numpy()
     rdt, ndt, sdt = ops.page_result_dtype(), ops.page_node_dtype(), ops.skew_block_dtype()
     skewed = any(pg.skew is not None for _, pg, _ in items)
@@ -2222,7 +2246,7 @@ def _find_blocks(dimg, items, rq=None):
     skew = host[:o].view(sdt) if skewed else [None] * len(items)
     res = host[o:o + len(items) * rdt.itemsize].view(rdt)
     o, out = o + len(items) * rdt.itemsize, []
-    for (i, pg, rect), r, cap, sk in zip(items, res, caps, skew):
+    for (i, pg, rect), r, cap, sk, rl in zip(items, res, caps, skew, rls):
         leaves = host[o:o + cap * ndt.itemsize].view(ndt)[:int(r["n_leaves"])]
         o += cap * ndt.itemsize
         if r["error"] == lib.PAGE_ERR_NODES:
@@ -2244,6 +2268,8 @@ def _find_blocks(dimg, items, rq=None):
             (rejected if q["st"] & lib.PAGE_REJECTED else blocks).append(box)
         res = dict(threshold=int(r["threshold"]), ink="dark" if r["ink"] == lib.INK_DARK else "light",
                    text_size=int(r["text_size"]), gap_x=int(r["gap_x"]), gap_y=int(r["gap_y"]))
+        if rl is not None:
+            res.update(rule_length=rl, rule_pixels=int(r["rule_pixels"]))
         if pg.quad is not None:
             shape = dimg[i].shape[:2]
             res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=pg.direction, polarity=pg.polarity, window=b) for b in blocks],
@@ -2280,7 +2306,11 @@ def find_blocks(images, pages):
     warped in one launch); under "auto" its corners are found first (ops.find_page_quads: 8 launches for every such page, one
     more pinned copy and synchronisation), and a page without one raises "no page found".  Its dict gains ``quad`` (the corners
     used) and ``size`` (R's w_r, h_r), and its blocks are TextBlock.from_quad(quad, window=...) windows of R.  A page with
-    ``curve="auto"`` (DESIGN.md 7b, "Curled blocks") is cut as any level page, and its blocks are TextBlock(..., curve="auto")."""
+    ``curve="auto"`` (DESIGN.md 7b, "Curled blocks") is cut as any level page, and its blocks are TextBlock(..., curve="auto").
+    A page with ``rules="auto"`` (DESIGN.md 7b, "Ruled pages") has its rules U, the ink runs of at least its rule length in a row
+    or a column, found on the device (3 more launches for all such pages of the call) and taken out of its ink; a row or column
+    of a node that is at least half U is white and cuts, and each block stops growing at the nearest rule.  Its dict gains
+    ``rule_length`` (the length used) and ``rule_pixels`` (|U|); its blocks are those of a page without rules."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
