@@ -804,7 +804,19 @@ int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* c
  * runs transposed back into rbits, U cleared from bits and |U| counted into res->rule_pixels.  In such a page's XY-cut an index
  * whose U count is at least half the node's extent is white, and a white run holding one cuts whatever its length; a block
  * grows by q on each side only up to the nearest row (column) of its margin with U in its columns (rows).  Pages without
- * rbits take the path of a call with ruled = 0, and a call with ruled = 0 issues exactly the launches above. */
+ * rbits take the path of a call with ruled = 0, and a call with ruled = 0 issues exactly the launches above.
+ * Figures (DESIGN.md section 7b, "Figures"): `ruled` is a flags word, MN_PAGE_RULES | MN_PAGE_FIGURES (0 and 1 keep their
+ * meaning).  A page with fbits (inside work) has figures: at 7, its pass-1 leaves whose shorter side is at least f go, in leaf
+ * order, into figs (MN_PAGE_MAX_FIGURES entries; st = the rows of the figures before it), with f = figure_size, or 3 S when
+ * figure_size is 0; res->figure_size = f and res->n_figures = their number, or res->error = MN_PAGE_ERR_FIGURES over the limit.
+ * A call with MN_PAGE_FIGURES issues 1 more launch after 7, whatever the number of pages: each figure row of every figure page
+ * painted into fbits (F, the union of the figure rectangles) and cleared from bits, so that pass 2 and the leaf rules see
+ * I'' = I' and not F.  F takes no part in the rule-index cut; a block's growth stops at U or F as it does at U alone.  The rule
+ * launches skip a page with fbits and no rbits, the figure launch a page without fbits, and a call without MN_PAGE_FIGURES
+ * issues exactly the launches above. */
+#define MN_PAGE_RULES 1
+#define MN_PAGE_FIGURES 2
+#define MN_PAGE_MAX_FIGURES 1024
 #define MN_PAGE_LEVELS 24
 #define MN_PAGE_MAX_BLOCKS 1024
 #define MN_PAGE_MAX_NODES 65536
@@ -814,6 +826,7 @@ int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* c
 #define MN_PAGE_REJECTED 8      /* node st: a leaf that is not text */
 #define MN_PAGE_ERR_NODES 1
 #define MN_PAGE_ERR_BLOCKS 2
+#define MN_PAGE_ERR_FIGURES 3
 typedef struct {
     int16_t x0, y0, x1, y1;     /* in the crop */
     int32_t st;
@@ -821,7 +834,8 @@ typedef struct {
 typedef struct {
     int32_t error, n_leaves, n_blocks, text_size;
     int32_t gap_x, gap_y, threshold, ink;
-    int32_t rule_pixels, pad;   /* |U| of a ruled page (DESIGN.md section 7b, "Ruled pages"), else 0 */
+    int32_t rule_pixels;        /* |U| of a ruled page (DESIGN.md section 7b, "Ruled pages"), else 0 */
+    int32_t figure_size, n_figures, pad;   /* f and the number of figures of a figure page with a text size, else 0 */
 } mn_page_result;
 typedef struct {
     mn_text_block b;            /* the crop record (b.hist, b.out as mn_find_lines_u8's) */
@@ -836,6 +850,10 @@ typedef struct {
     int32_t src, active, open, gx, gy, pad, n[2];   /* state, written by the call */
     uint32_t* rbits;            /* null, or a ruled page's h x wpitch words of U followed by w x ceil(h / 32) words of scratch */
     int32_t rule_length, pad2;  /* a ruled page's rule length, 2 <= rule_length <= 32767 */
+    uint32_t* fbits;            /* null, or a figure page's h x wpitch words of F */
+    mn_page_node* figs;         /* a figure page's table of MN_PAGE_MAX_FIGURES figures */
+    int32_t figure_size;        /* a figure page's f in [2, 32767], or 0 for 3 S */
+    int32_t frows;              /* state: the rows of all of its figures */
 } mn_text_page;
 int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, int ruled, void* work,
                       long long work_bytes, void* stream);
@@ -848,8 +866,9 @@ int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, l
  *   5. the frame bitmap: bit j & 31 of bits[k wpitch + j / 32] is set iff an ink pixel has cell (k, j) in the frame at (c, s),
  *      or for a vertical page at (c, -s) on the untransposed crop (the transposed search frame with its axes swapped); the root
  *      node, and pages[i].b.w = M, pages[i].b.h = L;
- *   6-13. mn_find_blocks_u8's levels, text size and leaves, in frame cells (after its 3 rule launches under ruled != 0; a
- *         ruled page has skew None, so its frame bitmap is mn_find_blocks_u8's).
+ *   6-13. mn_find_blocks_u8's levels, text size and leaves, in frame cells (with its 3 rule launches under MN_PAGE_RULES and
+ *         its figure launch under MN_PAGE_FIGURES; a ruled or figure page has skew None, so its frame bitmap is
+ *         mn_find_blocks_u8's).
  * bits holds max L x wpitch words, wpitch >= max M / 32, and cap entries per list, max over the page's table; the angle
  * profiles and scores are as mn_find_lines_skewed_u8's (b.prof unused).  work (work_bytes) is zeroed by the call. */
 int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles, int ruled,

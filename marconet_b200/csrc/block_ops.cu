@@ -8,7 +8,9 @@
 // pages") find a photographed page's corners: the paper's largest 4-connected component, its hull and the largest quad on it.
 // Curled blocks (DESIGN.md 7b, "Curled blocks") trace each line across column strips: per-strip profiles and runs, and a
 // left-to-right link of the runs into lines, in seven launches.  Ruled pages (DESIGN.md 7b, "Ruled pages") find the ink runs of at
-// least a rule length in rows and columns in three more launches, take them out of the page's bitmap and let them cut.
+// least a rule length in rows and columns in three more launches, take them out of the page's bitmap and let them cut.  Figures
+// (DESIGN.md 7b, "Figures") are the pass-1 leaves of at least a figure size, selected with the text size and painted out of the
+// bitmap in one more launch before pass 2.
 #include <climits>
 
 #include "mn_common.cuh"
@@ -1163,8 +1165,42 @@ __global__ void __launch_bounds__(kPageThreads, 1) page_emit_kernel(mn_text_page
     }
 }
 
+// The figures of a figure page (DESIGN.md 7b, "Figures"), by the CTA: its pass-1 leaves list[0 .. n) whose shorter side is at
+// least f, in leaf order, into p.figs (st: the rows of the figures before it), their rows into p.frows and f and their number
+// into res; over MN_PAGE_MAX_FIGURES the page error.  Returns false on that error.  Ends with a barrier.
+__device__ bool page_figures(mn_text_page& p, const mn_page_node* list, int n, int S, int* s_scan) {
+    const int f = p.figure_size > 0 ? p.figure_size : 3 * S;
+    const int chunk = (n + blockDim.x - 1) / blockDim.x, i0 = threadIdx.x * chunk, i1 = min(n, i0 + chunk);
+    auto figure = [&](int i) { return min(list[i].x1 - list[i].x0, list[i].y1 - list[i].y0) >= f; };
+    int c = 0, r = 0, total, rows;
+    for (int i = i0; i < i1; ++i) {
+        if (!figure(i)) continue;
+        ++c;
+        r += list[i].y1 - list[i].y0;
+    }
+    int k = cta_scan(c, s_scan, &total);
+    r = cta_scan(r, s_scan, &rows);                     // disjoint, sides >= 2: at most w h / 2 rows
+    if (total <= MN_PAGE_MAX_FIGURES) {
+        for (int i = i0; i < i1; ++i) {
+            if (!figure(i)) continue;
+            mn_page_node g = list[i];
+            g.st = r;
+            p.figs[k++] = g;
+            r += g.y1 - g.y0;
+        }
+    }
+    __syncthreads();                                    // list is read before the root overwrites it
+    if (threadIdx.x == 0) {
+        p.res->figure_size = f;
+        p.res->n_figures = total;
+        if (total > MN_PAGE_MAX_FIGURES) p.res->error = MN_PAGE_ERR_FIGURES;
+        else p.frows = rows;
+    }
+    return total <= MN_PAGE_MAX_FIGURES;
+}
+
 // 7. Text size S: the lower median of max(h, w) over the leaves with max(h, w) >= 2, by bisection over counts; the gaps of
-// pass 2 and its root.  A page without such a leaf has no blocks.
+// pass 2 and its root.  A page without such a leaf has no blocks; a figure page's figures are selected first.
 __global__ void __launch_bounds__(kScanThreads) page_size_kernel(mn_text_page* pages) {
     mn_pdl_prologue();
     __shared__ int s_scan[32];
@@ -1188,9 +1224,10 @@ __global__ void __launch_bounds__(kScanThreads) page_size_kernel(mn_text_page* p
         cta_scan(k, s_scan, &t);
         if (t > (n2 - 1) / 2) hi = mid; else lo = mid + 1;
     }
+    const bool ok = n2 == 0 || !p.fbits || page_figures(p, list, n, lo, s_scan);
     if (threadIdx.x != 0) return;
     p.src = 0;
-    if (n2 == 0) {
+    if (n2 == 0 || !ok) {
         p.n[0] = 0;
         p.open = 0;
         return;
@@ -1209,15 +1246,16 @@ __global__ void __launch_bounds__(kScanThreads) page_size_kernel(mn_text_page* p
     p.open = 1;
 }
 
-// The greatest (kMin: least) row (kRows) or column of the rectangle [xa, xb) x [ya, yb) of a ruled page that holds a U pixel,
-// over the warp: -1 (kMin: 1 << 30) when there is none.
+// The greatest (kMin: least) row (kRows) or column of the rectangle [xa, xb) x [ya, yb) of a ruled or figure page that holds a
+// pixel of U or F, over the warp: -1 (kMin: 1 << 30) when there is none.
 template <bool kRows, bool kMin>
 __device__ int rule_edge(const mn_text_page& p, int xa, int ya, int xb, int yb) {
     const int w0 = xa >> 5, nwords = xb > xa ? ((xb - 1) >> 5) - w0 + 1 : 0;
     int best = kMin ? 1 << 30 : -1;
     for (int k = threadIdx.x & 31; k < nwords * max(0, yb - ya); k += 32) {
         const int y = ya + k / nwords, wd = w0 + k % nwords;
-        const unsigned m = p.rbits[(long long)y * p.wpitch + wd] & word_mask(wd, xa, xb);
+        const long long o = (long long)y * p.wpitch + wd;
+        const unsigned m = ((p.rbits ? p.rbits[o] : 0u) | (p.fbits ? p.fbits[o] : 0u)) & word_mask(wd, xa, xb);
         if (!m) continue;
         const int v = kRows ? y : kMin ? 32 * wd + __ffs(m) - 1 : 32 * wd + 31 - __clz(m);
         best = kMin ? min(best, v) : max(best, v);
@@ -1226,7 +1264,8 @@ __device__ int rule_edge(const mn_text_page& p, int xa, int ya, int xb, int yb) 
 }
 
 // 11. The leaves, one warp each: rejected when 2 ink > h w or min(h, w) < max(1, S / 3), else a block grown by q and clipped;
-// on a ruled page each side stops short of the nearest row (column) of its margin with U in the leaf's columns (rows).
+// on a ruled or figure page each side stops short of the nearest row (column) of its margin with U or F in the leaf's columns
+// (rows).
 __global__ void __launch_bounds__(kScanThreads) page_blocks_kernel(mn_text_page* pages) {
     mn_pdl_prologue();
     __shared__ int s_blocks;
@@ -1256,7 +1295,7 @@ __global__ void __launch_bounds__(kScanThreads) page_blocks_kernel(mn_text_page*
         const int h = nd.y1 - nd.y0, w = nd.x1 - nd.x0;
         const bool reject = 2 * ink > (long long)h * w || min(h, w) < min_side;
         int x0 = max(0, nd.x0 - q), y0 = max(0, nd.y0 - q), x1 = min(p.b.w, nd.x1 + q), y1 = min(p.b.h, nd.y1 + q);
-        if (!reject && p.rbits) {
+        if (!reject && (p.rbits || p.fbits)) {
             const int top = rule_edge<true, false>(p, nd.x0, y0, nd.x1, nd.y0);
             const int bottom = rule_edge<true, true>(p, nd.x0, nd.y1, nd.x1, y1);
             const int left = rule_edge<false, false>(p, x0, nd.y0, nd.x0, nd.y1);
@@ -1423,6 +1462,34 @@ __global__ void __launch_bounds__(kRuleThreads) rule_merge_kernel(mn_text_page* 
     if (lane == 0 && count) atomicAdd(&s_count, count);
     __syncthreads();
     if (threadIdx.x == 0 && s_count) atomicAdd(&p.res->rule_pixels, s_count);
+}
+
+// ---- Figures (DESIGN.md 7b, "Figures") ----
+// F1. Every row of every figure of a figure page (page_figures' table), one warp each: its words OR'd into fbits (F) and cleared
+// from bits (I'' = I' and not F).  Figures may share a word at their ends, hence the atomics.  Pages without fbits, and pages
+// with an error, return at once.
+constexpr int kFigureThreads = 256;
+
+__global__ void __launch_bounds__(kFigureThreads) figure_paint_kernel(mn_text_page* pages) {
+    mn_pdl_prologue();
+    const mn_text_page& p = pages[blockIdx.y];
+    if (!p.fbits || p.res->error) return;
+    const int nf = p.res->n_figures, lane = threadIdx.x & 31;
+    constexpr int kWarps = kFigureThreads / 32;
+    for (int t = blockIdx.x * kWarps + (threadIdx.x >> 5); t < p.frows; t += gridDim.x * kWarps) {
+        int lo = 0, hi = nf - 1;                        // the last figure whose first row index is <= t
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (p.figs[mid].st <= t) lo = mid; else hi = mid - 1;
+        }
+        const mn_page_node g = p.figs[lo];
+        const long long o = (long long)(g.y0 + t - g.st) * p.wpitch;
+        for (int wd = (g.x0 >> 5) + lane; wd <= (g.x1 - 1) >> 5; wd += 32) {
+            const unsigned m = word_mask(wd, g.x0, g.x1);
+            atomicOr(p.fbits + o + wd, m);
+            atomicAnd(p.bits + o + wd, ~m);
+        }
+    }
 }
 
 // ---- Skewed pages (DESIGN.md 7b, "Skewed pages") ----
@@ -1828,10 +1895,10 @@ __global__ void __launch_bounds__(kHullThreads) quad_hull_kernel(const mn_quad_p
 }
 
 // 4-11 of the XY-cut: both passes of levels, the text size between them and the leaves, on pages whose bitmap and root are
-// written; under `ruled`, the three rule launches first.
-int page_levels(mn_text_page* pages, int n, long long max_tiles, int ruled, cudaStream_t st) {
-    if (ruled) {
-        const dim3 rgrid((unsigned)mn_cdiv64(max_tiles, kRuleThreads / 32), (unsigned)n);
+// written; under MN_PAGE_RULES, the three rule launches first, and under MN_PAGE_FIGURES the figure launch after the text size.
+int page_levels(mn_text_page* pages, int n, long long max_tiles, int flags, cudaStream_t st) {
+    const dim3 rgrid((unsigned)mn_cdiv64(max_tiles, kRuleThreads / 32), (unsigned)n);
+    if (flags & MN_PAGE_RULES) {
         MN_CUDA_CHECK((mn_launch(rule_transpose_kernel, rgrid, dim3(kRuleThreads), 0, st, pages)));
         MN_LAUNCH_CHECK();
         MN_CUDA_CHECK((mn_launch(rule_runs_kernel, rgrid, dim3(kRuleThreads), 0, st, pages)));
@@ -1852,6 +1919,10 @@ int page_levels(mn_text_page* pages, int n, long long max_tiles, int ruled, cuda
         if (pass == 0) {
             MN_CUDA_CHECK((mn_launch(page_size_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
             MN_LAUNCH_CHECK();
+            if (flags & MN_PAGE_FIGURES) {
+                MN_CUDA_CHECK((mn_launch(figure_paint_kernel, rgrid, dim3(kFigureThreads), 0, st, pages)));
+                MN_LAUNCH_CHECK();
+            }
         }
     }
     MN_CUDA_CHECK((mn_launch(page_blocks_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
@@ -1908,7 +1979,7 @@ extern "C" int mn_find_lines_skewed_u8(mn_text_block* blocks, mn_skew_block* ske
     return MN_OK;
 }
 
-extern "C" int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, int ruled, void* work,
+extern "C" int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, int flags, void* work,
                                  long long work_bytes, void* stream) {
     MN_REQUIRE(blocks && pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
                "mn_find_blocks_u8: bad args");
@@ -1917,11 +1988,11 @@ extern "C" int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* page
     if (rc != MN_OK) return rc;
     MN_CUDA_CHECK((mn_launch(page_bits_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, pages)));
     MN_LAUNCH_CHECK();
-    return page_levels(pages, n, max_tiles, ruled, st);
+    return page_levels(pages, n, max_tiles, flags, st);
 }
 
 extern "C" int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles,
-                                        int ruled, void* work, long long work_bytes, void* stream) {
+                                        int flags, void* work, long long work_bytes, void* stream) {
     MN_REQUIRE(blocks && skew && pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && work && work_bytes > 0,
                "mn_find_blocks_skewed_u8: bad args");
     cudaStream_t st = (cudaStream_t)stream;
@@ -1933,7 +2004,7 @@ extern "C" int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* sk
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(page_frame_bits_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, pages, skew)));
     MN_LAUNCH_CHECK();
-    return page_levels(pages, n, max_tiles, ruled, st);
+    return page_levels(pages, n, max_tiles, flags, st);
 }
 
 extern "C" int mn_find_lines_window_u8(const mn_text_block* blocks, const mn_window_block* wins, int n, long long max_tiles,

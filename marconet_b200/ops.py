@@ -2104,6 +2104,12 @@ def rule_page_bytes(w, h):
     return 4 * (h * -(-w // 32) + w * -(-h // 32))
 
 
+def figure_page_bytes(w, h):
+    """Device bytes a w x h page adds to find_blocks when it has figures (DESIGN.md 7b, "Figures"): its F bitmap (h rows of
+    ceil(w / 32) words) and its figure table of PAGE_MAX_FIGURES page nodes."""
+    return 4 * h * -(-w // 32) + 12 * _lib.PAGE_MAX_FIGURES
+
+
 def skew_page_frame(w, h, vertical, cs):
     """(L, M, stride) of a w x h page's frame bitmaps over the (c, s) of ``cs``: the most rows and columns a bitmap may have (the
     search frame's axes swapped for a vertical page) and the most bins of its search frames."""
@@ -2135,11 +2141,17 @@ def find_blocks(pages, scores=False):
     rule_length (DESIGN.md 7b, "Ruled pages"), a ninth entry after skew and max_skew: None, or an integer in [2, 32767] on a
     page with skew None, whose ink pixels in a maximal row or column run of at least that many pixels are its rules U.  A call
     with such a page issues 3 more launches whatever the number of pages; its records gain rule_pixels (|U|), and the other
-    pages' tables are those of a call without it."""
+    pages' tables are those of a call without it.
+    figure_size (DESIGN.md 7b, "Figures"), a tenth entry: None, or on a page with skew None 0 (the figure size 3 S) or an
+    integer f in [2, 32767]: its pass-1 leaves whose shorter side is at least f are its figures, taken out of its ink before
+    pass 2.  A call with such a page issues 1 more launch whatever the number of pages; its records gain figure_size and
+    n_figures, and out ends with each such page's table of _lib.PAGE_MAX_FIGURES mn_page_node figures, in the order of the
+    pages.  The other pages' tables are those of a call without it."""
     global LAUNCHES
     dev = _check_items(pages, "find_blocks", "page")
     skewed = any(len(p) > 6 and p[6] is not None for p in pages)
     rules = [p[8] if len(p) > 8 else None for p in pages]
+    figs = [p[9] if len(p) > 9 else None for p in pages]
     n = len(pages)
     rsz, bsz, psz, lsz = (ctypes.sizeof(t) for t in (_lib.PageResult, _lib.TextBlock, _lib.TextPage, _lib.BlockLines))
     ssz = ctypes.sizeof(_lib.SkewBlock) if skewed else 0
@@ -2152,9 +2164,14 @@ def find_blocks(pages, scores=False):
         rl = rules[i]
         if rl is not None and (isinstance(rl, bool) or not isinstance(rl, int) or not 2 <= rl <= 32767 or skew is not None):
             raise ValueError(f"{what}: rule_length {rl!r} is not an integer in [2, 32767] on a page with skew None")
+        fs = figs[i]
+        if fs is not None and (isinstance(fs, bool) or not isinstance(fs, int) or not (fs == 0 or 2 <= fs <= 32767)
+                               or skew is not None):
+            raise ValueError(f"{what}: figure_size {fs!r} is not 0 or an integer in [2, 32767] on a page with skew None")
         L, M, stride = (bh, bw, bw if vertical else bh) if skew is None else skew_page_frame(bw, bh, vertical, cs)
         need += skew_page_bytes(bw, bh, vertical, cs) if skewed else page_bytes(bw, bh)
         need += rule_page_bytes(bw, bh) if rl is not None else 0
+        need += figure_page_bytes(bw, bh) if fs is not None else 0
         if max(L, M) > 32767:
             raise ValueError(f"{what}: a frame side of {max(L, M)} exceeds 32767")
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
@@ -2168,14 +2185,17 @@ def find_blocks(pages, scores=False):
     pg0, tab0 = n * bsz, n * (bsz + psz)                 # records, tables and the skew records, then the results and leaves,
     out0 = -(-(tab0 + len(tab) + n * ssz) // 16) * 16    # then the work: the call zeroes everything from out0 on, and the
     sk0 = out0 - n * ssz                                 # skew records come back with the results in one copy
-    n_out = n * rsz + 12 * sum(d[4] for d in dims)
+    n_leaves = n * rsz + 12 * sum(d[4] for d in dims)
+    n_out = n_leaves + 12 * _lib.PAGE_MAX_FIGURES * sum(fs is not None for fs in figs)
     work0 = out0 + -(-n_out // 16) * 16
     per = [-(-(8 * (d[7] if d[7] > 1 else 0) + 4 * 256 + lsz + 4 * d[5] * -(-d[6] // 32) + 2 * 12 * d[4] + 3 * 4 * d[4]
-                + 4 * (d[7] * d[8] if d[7] > 1 else 0) + (rule_page_bytes(d[6], d[5]) if rl is not None else 0)) // 16) * 16
-           for d, rl in zip(dims, rules)]
+                + 4 * (d[7] * d[8] if d[7] > 1 else 0) + (rule_page_bytes(d[6], d[5]) if rl is not None else 0)
+                + (4 * d[5] * -(-d[6] // 32) if fs is not None else 0)) // 16) * 16
+           for d, rl, fs in zip(dims, rules, figs)]
     buf = torch.empty(work0 + sum(per), dtype=torch.uint8, device=dev)
     base = buf.data_ptr()
     leaves, w, blocks, srecs, recs, views, tiles = base + out0 + n * rsz, base + work0, [], [], [], [], 0
+    ftab = base + out0 + n_leaves
     for i, (pg, d, nb, t) in enumerate(zip(pages, dims, per, t_offs)):
         img, _, vertical, polarity, gap_x, gap_y = pg[:6]
         x0, y0, bw, bh, cap, L, M, n_ang, stride = d
@@ -2185,13 +2205,17 @@ def find_blocks(pages, scores=False):
         lists = bits + 4 * L * wp
         counts = lists + 2 * 12 * cap
         rbits = counts + 3 * 4 * cap + 4 * (n_ang * stride if n_ang > 1 else 0)
+        fbits = rbits + (rule_page_bytes(M, L) if rules[i] is not None else 0)
         tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, 0, 0, 0, 0, hist, 0, 0, lines)
         blocks.append(tb)
         if skewed:
             srecs.append(_skew_block(tb, base + tab0 + 16 * t, w, counts + 3 * 4 * cap, n_ang, stride))
         recs.append(_lib.TextPage(tb, bits, (ctypes.c_void_p * 2)(lists, lists + 12 * cap), leaves, counts, counts + 4 * cap,
                                   counts + 8 * cap, base + out0 + i * rsz, wp, cap, gap_x or 0, gap_y or 0,
-                                  rbits=rbits if rules[i] is not None else None, rule_length=rules[i] or 0))
+                                  rbits=rbits if rules[i] is not None else None, rule_length=rules[i] or 0,
+                                  fbits=fbits if figs[i] is not None else None, figs=ftab if figs[i] is not None else None,
+                                  figure_size=figs[i] or 0))
+        ftab += 12 * _lib.PAGE_MAX_FIGURES if figs[i] is not None else 0
         views.append(buf[w - base:w - base + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         leaves += 12 * cap
         w += nb
@@ -2199,15 +2223,16 @@ def find_blocks(pages, scores=False):
     host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.TextPage * n)(*recs)) + tab
     host += bytes(sk0 - len(host)) + bytes((_lib.SkewBlock * len(srecs))(*srecs))
     buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
-    ruled = int(any(rl is not None for rl in rules))
+    ruled, figured = any(rl is not None for rl in rules), any(fs is not None for fs in figs)
+    flags = (_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0)
     if skewed:
-        _lib.check(_lib.load().mn_find_blocks_skewed_u8(base, base + sk0, base + pg0, n, tiles, ruled, base + out0,
+        _lib.check(_lib.load().mn_find_blocks_skewed_u8(base, base + sk0, base + pg0, n, tiles, flags, base + out0,
                                                         work0 + sum(per) - out0, _stream()), "mn_find_blocks_skewed_u8")
-        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS + 3 * ruled
+        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured
     else:
-        _lib.check(_lib.load().mn_find_blocks_u8(base, base + pg0, n, tiles, ruled, base + out0, work0 + sum(per) - out0,
+        _lib.check(_lib.load().mn_find_blocks_u8(base, base + pg0, n, tiles, flags, base + out0, work0 + sum(per) - out0,
                                                  _stream()), "mn_find_blocks_u8")
-        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS + 3 * ruled
+        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured
     res = buf[sk0:out0 + n_out], [d[4] for d in dims]
     return res + (views,) if scores else res
 

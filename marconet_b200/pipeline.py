@@ -2087,7 +2087,12 @@ class TextPage(NamedTuple):
     ``rules`` (DESIGN.md 7b, "Ruled pages"): None, or "auto" for a page whose tables, forms and frames are drawn with ruling
     lines: ink runs at least ``rule_length`` pixels long in a row or a column (an integer in [2, 32767]; default
     max(32, min(w, h) // 16) of the crop, or of R for a quad page, a heuristic) are rules, which cut the page into cells and stop
-    its blocks.  Not with skew or curve: flatten such a page with flatten_pages first."""
+    its blocks.  Not with skew or curve: flatten such a page with flatten_pages first.
+    ``figures`` (DESIGN.md 7b, "Figures"): None, or "auto" for a page with photos, charts or drawings: the pieces of the page
+    (leaves of the unit-gap XY-cut) whose shorter side is at least ``figure_size`` (an integer in [2, 32767]; default 3 times
+    the text size, a heuristic) are figures, taken out of the ink before the blocks are cut; blocks stop growing at them, and a
+    figure is never restored as a block of its own (a block whose rectangle spans one can restore lines over it).  Not with skew
+    or curve: flatten such a page with flatten_pages first."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
@@ -2099,6 +2104,8 @@ class TextPage(NamedTuple):
     curve: object = None
     rules: object = None
     rule_length: object = None
+    figures: object = None
+    figure_size: object = None
 
 
 def _check_page(pg, H, W, name):
@@ -2116,6 +2123,17 @@ def _check_page(pg, H, W, name):
         if pg.rules is not None and getattr(pg, what) is not None:
             raise ValueError(f"{name}: rules and {what} are both given (a ruled page is level and flat: flatten a tilted or "
                              f"curled page with flatten_pages first)")
+    if pg.figures is not None and not (isinstance(pg.figures, str) and pg.figures == "auto"):
+        raise ValueError(f"{name}: figures must be None or 'auto', got {pg.figures!r}")
+    v = pg.figure_size
+    if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 2 <= v <= 32767):
+        raise ValueError(f"{name}: figure_size must be an integer in [2, 32767], got {v!r}")
+    if v is not None and pg.figures is None:
+        raise ValueError(f"{name}: figure_size is given, but figures is None, not 'auto'")
+    for what in ("skew", "curve"):
+        if pg.figures is not None and getattr(pg, what) is not None:
+            raise ValueError(f"{name}: figures and {what} are both given (a page with figures is level and flat: flatten a "
+                             f"tilted or curled page with flatten_pages first)")
     if pg.quad is not None:
         if pg.rect is not None:
             raise ValueError(f"{name}: rect and quad are both given (a page in perspective is its quad: give rect=None)")
@@ -2155,7 +2173,8 @@ def _page_table(pg):
 
 def _page_bytes(pg, rect, skewed):
     """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages, with a ruled page's two extra
-    bitmaps: a quad page's rectified crop and its page, or an auto page's corner search on the image ``rect``."""
+    bitmaps and a figure page's bitmap and table: a quad page's rectified crop and its page, or an auto page's corner search on
+    the image ``rect``."""
     from . import ops
     w, h = rect[2] - rect[0], rect[3] - rect[1]
     if isinstance(pg.quad, str):
@@ -2164,6 +2183,7 @@ def _page_bytes(pg, rect, skewed):
         w_r, h_r = quad_maps(pg.quad, 1).size
         return 3 * w_r * h_r + _page_bytes(pg._replace(quad=None), (0, 0, w_r, h_r), skewed)
     rules = ops.rule_page_bytes(w, h) if pg.rules is not None else 0
+    rules += ops.figure_page_bytes(w, h) if pg.figures is not None else 0
     if not skewed:
         return ops.page_bytes(w, h) + rules
     return rules + ops.skew_page_bytes(w, h, pg.direction == "vertical",
@@ -2222,8 +2242,8 @@ def _find_pages(dimg, items, keys=()):
 def _find_blocks(dimg, items, rq=None):
     """ops.find_blocks over items (image index, TextPage, rect) of the uploaded images ``dimg``, its tables back through one
     pinned copy and one synchronisation; a quad page (its corners given) is a level page on all of its rectified crop in ``rq``
-    (_rectify).  Returns per item dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, rule_length, rule_pixels]), or
-    the error message of a page over a limit."""
+    (_rectify).  Returns per item dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, rule_length, rule_pixels]
+    [, figure_size, figures]), or the error message of a page over a limit."""
     from . import ops
     lib = ops._lib
 
@@ -2237,8 +2257,9 @@ def _find_blocks(dimg, items, rq=None):
         _, (x0, y0, x1, y1) = src(i, pg, rect)
         return None if pg.rules is None else pg.rule_length or ops.rule_length(x1 - x0, y1 - y0)
     rls = [rule_length(*it) for it in items]
+    fss = [None if pg.figures is None else pg.figure_size or 0 for _, pg, _ in items]
     res_t, caps = ops.find_blocks([(*src(i, pg, rect), pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y,
-                                    pg.skew, pg.max_skew, rl) for (i, pg, rect), rl in zip(items, rls)])
+                                    pg.skew, pg.max_skew, rl, fs) for (i, pg, rect), rl, fs in zip(items, rls, fss)])
     host = _to_host(res_t).numpy()
     rdt, ndt, sdt = ops.page_result_dtype(), ops.page_node_dtype(), ops.skew_block_dtype()
     skewed = any(pg.skew is not None for _, pg, _ in items)
@@ -2246,14 +2267,21 @@ def _find_blocks(dimg, items, rq=None):
     skew = host[:o].view(sdt) if skewed else [None] * len(items)
     res = host[o:o + len(items) * rdt.itemsize].view(rdt)
     o, out = o + len(items) * rdt.itemsize, []
-    for (i, pg, rect), r, cap, sk, rl in zip(items, res, caps, skew, rls):
+    ft = o + sum(caps) * ndt.itemsize                   # the figure pages' tables, after every leaf table
+    for (i, pg, rect), r, cap, sk, rl, fs in zip(items, res, caps, skew, rls, fss):
         leaves = host[o:o + cap * ndt.itemsize].view(ndt)[:int(r["n_leaves"])]
         o += cap * ndt.itemsize
+        if fs is not None:
+            figs = host[ft:ft + lib.PAGE_MAX_FIGURES * ndt.itemsize].view(ndt)[:int(r["n_figures"])]
+            ft += lib.PAGE_MAX_FIGURES * ndt.itemsize
         if r["error"] == lib.PAGE_ERR_NODES:
             out.append(f"more than {lib.PAGE_MAX_NODES} nodes in one level of the XY-cut")
             continue
         if r["error"] == lib.PAGE_ERR_BLOCKS:
             out.append(f"{int(r['n_blocks'])} blocks exceed the {lib.PAGE_MAX_BLOCKS} a text page may hold")
+            continue
+        if r["error"] == lib.PAGE_ERR_FIGURES:
+            out.append(f"{int(r['n_figures'])} figures exceed the {lib.PAGE_MAX_FIGURES} a text page may hold")
             continue
         X0, Y0 = (0, 0) if pg.quad is not None else rect[:2]
         vertical = pg.direction == "vertical"
@@ -2270,6 +2298,9 @@ def _find_blocks(dimg, items, rq=None):
                    text_size=int(r["text_size"]), gap_x=int(r["gap_x"]), gap_y=int(r["gap_y"]))
         if rl is not None:
             res.update(rule_length=rl, rule_pixels=int(r["rule_pixels"]))
+        if fs is not None:                              # in image coordinates, or rectangles of R on a quad page
+            res.update(figure_size=int(r["figure_size"]),
+                       figures=[(X0 + int(q["x0"]), Y0 + int(q["y0"]), X0 + int(q["x1"]), Y0 + int(q["y1"])) for q in figs])
         if pg.quad is not None:
             shape = dimg[i].shape[:2]
             res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=pg.direction, polarity=pg.polarity, window=b) for b in blocks],
@@ -2310,7 +2341,12 @@ def find_blocks(images, pages):
     A page with ``rules="auto"`` (DESIGN.md 7b, "Ruled pages") has its rules U, the ink runs of at least its rule length in a row
     or a column, found on the device (3 more launches for all such pages of the call) and taken out of its ink; a row or column
     of a node that is at least half U is white and cuts, and each block stops growing at the nearest rule.  Its dict gains
-    ``rule_length`` (the length used) and ``rule_pixels`` (|U|); its blocks are those of a page without rules."""
+    ``rule_length`` (the length used) and ``rule_pixels`` (|U|); its blocks are those of a page without rules.
+    A page with ``figures="auto"`` (DESIGN.md 7b, "Figures") has its figures, the leaves of the unit-gap XY-cut whose shorter
+    side is at least its figure size f, selected on the device with the text size and taken out of its ink before the second
+    XY-cut (1 more launch for all such pages of the call); each block stops growing at a figure as at a rule.  Its dict gains
+    ``figure_size`` (the f used, 0 without a text size) and ``figures``, their rectangles in leaf order (as ``rejected``: in
+    image coordinates, or rectangles of R on a quad page).  A page over 1024 figures raises, as one over its block limit."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
@@ -2904,7 +2940,7 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     call in the same launches, one pinned copy and one synchronisation), its TextBlocks take its place, and each of them is then
     replaced by its lines as above, so the result is byte for byte that of the call given the found blocks.  No labels or boxes
     may be given for a page; a tilted page (``skew``) gives windowed TextBlocks, which are split as any other.  Its entry is
-    dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, skew], regions), regions one
+    dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, skew][, figure_size, figures], regions), regions one
     block entry per block; a page over its node or block limit, or one of whose blocks fails, raises, or is dict(error=...)
     with ``skip_invalid``, and then none of its blocks is restored.  A quad page or block (DESIGN.md 7b, "Perspective pages")
     is laid out on its rectified crop (TextPage(quad="auto") after the device's corner search), every distinct quad of the call
