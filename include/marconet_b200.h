@@ -813,9 +813,15 @@ int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* c
  * painted into fbits (F, the union of the figure rectangles) and cleared from bits, so that pass 2 and the leaf rules see
  * I'' = I' and not F.  F takes no part in the rule-index cut; a block's growth stops at U or F as it does at U alone.  The rule
  * launches skip a page with fbits and no rbits, the figure launch a page without fbits, and a call without MN_PAGE_FIGURES
- * issues exactly the launches above. */
+ * issues exactly the launches above.
+ * Mixed directions (DESIGN.md section 7b, "Mixed directions"): a page with dirs != 0 has its blocks' directions tested.  A call
+ * with MN_PAGE_DIRECTIONS issues 1 more launch after 11, whatever the number of pages: every kept leaf of such a page (its
+ * ungrown rectangle in list[src]) has its row and column bands counted and its leaves[] entry marked MN_PAGE_VERTICAL when
+ * its direction is vertical, and MN_PAGE_UNDECIDED (with the page's direction) when the test is undecided.  The launch skips
+ * pages without dirs and pages with an error; a call without MN_PAGE_DIRECTIONS issues exactly the launches above. */
 #define MN_PAGE_RULES 1
 #define MN_PAGE_FIGURES 2
+#define MN_PAGE_DIRECTIONS 4
 #define MN_PAGE_MAX_FIGURES 1024
 #define MN_PAGE_LEVELS 24
 #define MN_PAGE_MAX_BLOCKS 1024
@@ -824,6 +830,8 @@ int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* c
 #define MN_PAGE_FAILED 2        /* node st: its previous attempt made no cut */
 #define MN_PAGE_LEAF 4          /* node st: closed */
 #define MN_PAGE_REJECTED 8      /* node st: a leaf that is not text */
+#define MN_PAGE_VERTICAL 16     /* leaf st: a block of a direction page whose direction is vertical */
+#define MN_PAGE_UNDECIDED 32    /* leaf st: a block of a direction page that took the page's direction, its test undecided */
 #define MN_PAGE_ERR_NODES 1
 #define MN_PAGE_ERR_BLOCKS 2
 #define MN_PAGE_ERR_FIGURES 3
@@ -849,7 +857,8 @@ typedef struct {
     int32_t wpitch, cap, gap_x, gap_y;   /* gap_x, gap_y: 0 = the default */
     int32_t src, active, open, gx, gy, pad, n[2];   /* state, written by the call */
     uint32_t* rbits;            /* null, or a ruled page's h x wpitch words of U followed by w x ceil(h / 32) words of scratch */
-    int32_t rule_length, pad2;  /* a ruled page's rule length, 2 <= rule_length <= 32767 */
+    int32_t rule_length;        /* a ruled page's rule length, 2 <= rule_length <= 32767 */
+    int32_t dirs;               /* 1: a direction page, its blocks' directions tested; else 0 */
     uint32_t* fbits;            /* null, or a figure page's h x wpitch words of F */
     mn_page_node* figs;         /* a figure page's table of MN_PAGE_MAX_FIGURES figures */
     int32_t figure_size;        /* a figure page's f in [2, 32767], or 0 for 3 S */
@@ -866,9 +875,9 @@ int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, l
  *   5. the frame bitmap: bit j & 31 of bits[k wpitch + j / 32] is set iff an ink pixel has cell (k, j) in the frame at (c, s),
  *      or for a vertical page at (c, -s) on the untransposed crop (the transposed search frame with its axes swapped); the root
  *      node, and pages[i].b.w = M, pages[i].b.h = L;
- *   6-13. mn_find_blocks_u8's levels, text size and leaves, in frame cells (with its 3 rule launches under MN_PAGE_RULES and
- *         its figure launch under MN_PAGE_FIGURES; a ruled or figure page has skew None, so its frame bitmap is
- *         mn_find_blocks_u8's).
+ *   6-13. mn_find_blocks_u8's levels, text size and leaves, in frame cells (with its 3 rule launches under MN_PAGE_RULES,
+ *         its figure launch under MN_PAGE_FIGURES and its direction launch under MN_PAGE_DIRECTIONS; a ruled, figure or
+ *         direction page has skew None, so its frame bitmap is mn_find_blocks_u8's).
  * bits holds max L x wpitch words, wpitch >= max M / 32, and cap entries per list, max over the page's table; the angle
  * profiles and scores are as mn_find_lines_skewed_u8's (b.prof unused).  work (work_bytes) is zeroed by the call. */
 int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles, int ruled,

@@ -212,6 +212,7 @@ PAGE_LEVELS, PAGE_MAX_BLOCKS, PAGE_MAX_NODES = 24, 1024, 65536    # MN_PAGE_LEVE
 PAGE_REJECTED = 8                                                  # MN_PAGE_REJECTED
 PAGE_ERR_NODES, PAGE_ERR_BLOCKS, PAGE_ERR_FIGURES = 1, 2, 3
 PAGE_RULES, PAGE_FIGURES, PAGE_MAX_FIGURES = 1, 2, 1024           # MN_PAGE_RULES, MN_PAGE_FIGURES, MN_PAGE_MAX_FIGURES
+PAGE_DIRECTIONS, PAGE_VERTICAL, PAGE_UNDECIDED = 4, 16, 32         # MN_PAGE_DIRECTIONS, MN_PAGE_VERTICAL, MN_PAGE_UNDECIDED
 
 
 class PageNode(Structure):
@@ -228,7 +229,7 @@ class TextPage(Structure):
     _fields_ = [("b", TextBlock), ("bits", c_void_p), ("list", c_void_p * 2), ("leaves", c_void_p), ("nch", c_void_p),
                 ("nopen", c_void_p), ("off", c_void_p), ("res", c_void_p), ("wpitch", c_int32), ("cap", c_int32),
                 ("gap_x", c_int32), ("gap_y", c_int32), ("src", c_int32), ("active", c_int32), ("open", c_int32), ("gx", c_int32),
-                ("gy", c_int32), ("pad", c_int32), ("n", c_int32 * 2), ("rbits", c_void_p), ("rule_length", c_int32), ("pad2", c_int32),
+                ("gy", c_int32), ("pad", c_int32), ("n", c_int32 * 2), ("rbits", c_void_p), ("rule_length", c_int32), ("dirs", c_int32),
                 ("fbits", c_void_p), ("figs", c_void_p), ("figure_size", c_int32), ("frows", c_int32)]
 
 

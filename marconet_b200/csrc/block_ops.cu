@@ -10,7 +10,8 @@
 // left-to-right link of the runs into lines, in seven launches.  Ruled pages (DESIGN.md 7b, "Ruled pages") find the ink runs of at
 // least a rule length in rows and columns in three more launches, take them out of the page's bitmap and let them cut.  Figures
 // (DESIGN.md 7b, "Figures") are the pass-1 leaves of at least a figure size, selected with the text size and painted out of the
-// bitmap in one more launch before pass 2.
+// bitmap in one more launch before pass 2.  Mixed directions (DESIGN.md 7b, "Mixed directions") test each kept leaf's row and
+// column bands for its own direction in one more launch after the leaves.
 #include <climits>
 
 #include "mn_common.cuh"
@@ -1492,6 +1493,71 @@ __global__ void __launch_bounds__(kFigureThreads) figure_paint_kernel(mn_text_pa
     }
 }
 
+// ---- Mixed directions (DESIGN.md 7b, "Mixed directions") ----
+// The bands of a leaf along rows (or columns), by the CTA from node_profile's non-white bits: *n the number of maximal runs
+// of non-white indices, *b the longest and *g the white indices between the first and the last non-white one.  A run's
+// length at each of its indices is its distance to the last white index before it, carried across threads by a max-scan.
+__device__ void leaf_bands(const mn_text_page& p, const mn_page_node& nd, bool rows, page_smem& s, int* n, int* b, int* g) {
+    node_profile(p, nd, rows, s);
+    constexpr int kPer = kSpanWords / kPageThreads;
+    const int j0 = threadIdx.x * kPer;
+    int my_n = 0, my_set = 0, my_first = -1, my_last = -1, my_white = -1, t;
+    for (int j = j0; j < j0 + kPer; ++j) {
+        const unsigned v = s.nw[j], carry = j ? s.nw[j - 1] >> 31 : 0u;
+        my_n += __popc(v & ~((v << 1) | carry));         // the indices that start a band
+        my_set += __popc(v);
+        if (v && my_first < 0) my_first = 32 * j + __ffs(v) - 1;
+        if (v) my_last = 32 * j + 31 - __clz(v);
+        if (~v) my_white = 32 * j + 31 - __clz(~v);
+    }
+    int white = cta_max_scan(my_white, s.scan, &t), best = 0;
+    for (int j = j0; j < j0 + kPer; ++j) {
+        for (unsigned v = s.nw[j]; v; v &= v - 1u) {
+            const int i = 32 * j + __ffs(v) - 1;
+            if (i == 0 || !((s.nw[(i - 1) >> 5] >> ((i - 1) & 31)) & 1u)) white = i - 1;
+            best = max(best, i - white);
+        }
+    }
+    int set, first, last;
+    cta_scan(my_n, s.scan, n);
+    cta_scan(my_set, s.scan, &set);
+    cta_max_scan(my_first < 0 ? -1 : kSpanWords * 32 - my_first, s.scan, &first);
+    cta_max_scan(my_last, s.scan, &last);
+    cta_max_scan(best, s.scan, b);
+    *g = last < 0 ? 0 : last - (kSpanWords * 32 - first) + 1 - set;
+}
+
+// D1. The direction of every kept leaf of a direction page, one CTA per leaf (grid-stride over blockIdx.x): with its row bands
+// (n_r, b_r, G_y) and column bands (n_c, b_c, G_x) on its ungrown h x w rectangle, horizontal iff A > B and vertical iff
+// A < B for (A, B) = (w, h) when n_r = n_c = 1, (2 b_c, h) when n_r = 1 < n_c, (w, 2 b_r) when n_c = 1 < n_r and
+// (G_y (n_c - 1), G_x (n_r - 1)) when both exceed 1 (the mean gaps between row bands and between column bands); otherwise
+// (A = B, or no band) undecided, and the page's direction.  Pages without dirs, and pages with an error, return at once.
+__global__ void __launch_bounds__(kPageThreads) page_direction_kernel(mn_text_page* pages) {
+    mn_pdl_prologue();
+    __shared__ page_smem s;
+    const mn_text_page& p = pages[blockIdx.y];
+    if (!p.dirs || p.res->error) return;
+    const mn_page_node* list = p.list[p.src];
+    const int n = p.res->n_leaves;
+    for (int i = blockIdx.x; i < n; i += gridDim.x) {
+        const int st = p.leaves[i].st;
+        if (st & MN_PAGE_REJECTED) continue;
+        const mn_page_node nd = list[i];
+        int nr, br, gy, nc, bc, gx;
+        leaf_bands(p, nd, true, s, &nr, &br, &gy);
+        leaf_bands(p, nd, false, s, &nc, &bc, &gx);
+        const long long h = nd.y1 - nd.y0, w = nd.x1 - nd.x0;
+        long long a = 0, b = 0;
+        if (nr == 1 && nc == 1) { a = w; b = h; }
+        else if (nr == 1 && nc > 1) { a = 2ll * bc; b = h; }
+        else if (nc == 1 && nr > 1) { a = w; b = 2ll * br; }
+        else if (nr > 1 && nc > 1) { a = (long long)gy * (nc - 1); b = (long long)gx * (nr - 1); }
+        if (threadIdx.x != 0) continue;
+        const bool vertical = a == b ? p.b.vertical != 0 : a < b;
+        p.leaves[i].st = st | (vertical ? MN_PAGE_VERTICAL : 0) | (a == b ? MN_PAGE_UNDECIDED : 0);
+    }
+}
+
 // ---- Skewed pages (DESIGN.md 7b, "Skewed pages") ----
 // The page's angle is searched by the skewed-block kernels on its mn_skew_block record; the XY-cut then runs unchanged on a
 // bitmap of frame cells, whose sides the page record takes.  A vertical page's bitmap is of the untransposed frame at the
@@ -1895,7 +1961,8 @@ __global__ void __launch_bounds__(kHullThreads) quad_hull_kernel(const mn_quad_p
 }
 
 // 4-11 of the XY-cut: both passes of levels, the text size between them and the leaves, on pages whose bitmap and root are
-// written; under MN_PAGE_RULES, the three rule launches first, and under MN_PAGE_FIGURES the figure launch after the text size.
+// written; under MN_PAGE_RULES, the three rule launches first, under MN_PAGE_FIGURES the figure launch after the text size, and
+// under MN_PAGE_DIRECTIONS the direction launch after the leaves.
 int page_levels(mn_text_page* pages, int n, long long max_tiles, int flags, cudaStream_t st) {
     const dim3 rgrid((unsigned)mn_cdiv64(max_tiles, kRuleThreads / 32), (unsigned)n);
     if (flags & MN_PAGE_RULES) {
@@ -1927,6 +1994,10 @@ int page_levels(mn_text_page* pages, int n, long long max_tiles, int flags, cuda
     }
     MN_CUDA_CHECK((mn_launch(page_blocks_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
     MN_LAUNCH_CHECK();
+    if (flags & MN_PAGE_DIRECTIONS) {
+        MN_CUDA_CHECK((mn_launch(page_direction_kernel, grid, dim3(kPageThreads), 0, st, pages)));
+        MN_LAUNCH_CHECK();
+    }
     return MN_OK;
 }
 

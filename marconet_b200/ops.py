@@ -2146,12 +2146,18 @@ def find_blocks(pages, scores=False):
     integer f in [2, 32767]: its pass-1 leaves whose shorter side is at least f are its figures, taken out of its ink before
     pass 2.  A call with such a page issues 1 more launch whatever the number of pages; its records gain figure_size and
     n_figures, and out ends with each such page's table of _lib.PAGE_MAX_FIGURES mn_page_node figures, in the order of the
-    pages.  The other pages' tables are those of a call without it."""
+    pages.  The other pages' tables are those of a call without it.
+    directions (DESIGN.md 7b, "Mixed directions"), an eleventh entry: None or False, or True on a page with skew None: each of
+    its kept leaves has its own direction tested, _lib.PAGE_VERTICAL set in its st when it is vertical and
+    _lib.PAGE_UNDECIDED when the test is undecided (it then takes the page's direction).  A call with such a page issues 1
+    more launch whatever the number of pages and needs no more memory; the other pages' tables are those of a call without
+    it."""
     global LAUNCHES
     dev = _check_items(pages, "find_blocks", "page")
     skewed = any(len(p) > 6 and p[6] is not None for p in pages)
     rules = [p[8] if len(p) > 8 else None for p in pages]
     figs = [p[9] if len(p) > 9 else None for p in pages]
+    dirs = [p[10] if len(p) > 10 else None for p in pages]
     n = len(pages)
     rsz, bsz, psz, lsz = (ctypes.sizeof(t) for t in (_lib.PageResult, _lib.TextBlock, _lib.TextPage, _lib.BlockLines))
     ssz = ctypes.sizeof(_lib.SkewBlock) if skewed else 0
@@ -2168,6 +2174,8 @@ def find_blocks(pages, scores=False):
         if fs is not None and (isinstance(fs, bool) or not isinstance(fs, int) or not (fs == 0 or 2 <= fs <= 32767)
                                or skew is not None):
             raise ValueError(f"{what}: figure_size {fs!r} is not 0 or an integer in [2, 32767] on a page with skew None")
+        if (dirs[i] is not None and not isinstance(dirs[i], bool)) or (dirs[i] and skew is not None):
+            raise ValueError(f"{what}: directions {dirs[i]!r} is not None, False or True on a page with skew None")
         L, M, stride = (bh, bw, bw if vertical else bh) if skew is None else skew_page_frame(bw, bh, vertical, cs)
         need += skew_page_bytes(bw, bh, vertical, cs) if skewed else page_bytes(bw, bh)
         need += rule_page_bytes(bw, bh) if rl is not None else 0
@@ -2214,7 +2222,7 @@ def find_blocks(pages, scores=False):
                                   counts + 8 * cap, base + out0 + i * rsz, wp, cap, gap_x or 0, gap_y or 0,
                                   rbits=rbits if rules[i] is not None else None, rule_length=rules[i] or 0,
                                   fbits=fbits if figs[i] is not None else None, figs=ftab if figs[i] is not None else None,
-                                  figure_size=figs[i] or 0))
+                                  figure_size=figs[i] or 0, dirs=int(bool(dirs[i]))))
         ftab += 12 * _lib.PAGE_MAX_FIGURES if figs[i] is not None else 0
         views.append(buf[w - base:w - base + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         leaves += 12 * cap
@@ -2224,15 +2232,16 @@ def find_blocks(pages, scores=False):
     host += bytes(sk0 - len(host)) + bytes((_lib.SkewBlock * len(srecs))(*srecs))
     buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
     ruled, figured = any(rl is not None for rl in rules), any(fs is not None for fs in figs)
-    flags = (_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0)
+    directed = any(bool(d) for d in dirs)
+    flags = (_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0) | (_lib.PAGE_DIRECTIONS if directed else 0)
     if skewed:
         _lib.check(_lib.load().mn_find_blocks_skewed_u8(base, base + sk0, base + pg0, n, tiles, flags, base + out0,
                                                         work0 + sum(per) - out0, _stream()), "mn_find_blocks_skewed_u8")
-        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured
+        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed
     else:
         _lib.check(_lib.load().mn_find_blocks_u8(base, base + pg0, n, tiles, flags, base + out0, work0 + sum(per) - out0,
                                                  _stream()), "mn_find_blocks_u8")
-        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured
+        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed
     res = buf[sk0:out0 + n_out], [d[4] for d in dims]
     return res + (views,) if scores else res
 

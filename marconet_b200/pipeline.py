@@ -2092,7 +2092,12 @@ class TextPage(NamedTuple):
     (leaves of the unit-gap XY-cut) whose shorter side is at least ``figure_size`` (an integer in [2, 32767]; default 3 times
     the text size, a heuristic) are figures, taken out of the ink before the blocks are cut; blocks stop growing at them, and a
     figure is never restored as a block of its own (a block whose rectangle spans one can restore lines over it).  Not with skew
-    or curve: flatten such a page with flatten_pages first."""
+    or curve: flatten such a page with flatten_pages first.
+    ``block_direction`` (DESIGN.md 7b, "Mixed directions"): None (every block takes ``direction``), or "auto" for a page that
+    mixes horizontal and vertical text: each block found gets its own direction, "horizontal" or "vertical", from its row and
+    column ink bands, and takes ``direction`` when that test is undecided.  ``direction`` keeps its role for the cut and the
+    reading order of the blocks.  TextPage(rect, block_direction="auto") is one rectangle of unknown direction when it holds
+    one block.  Not with skew or curve: flatten such a page with flatten_pages first."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
@@ -2106,6 +2111,7 @@ class TextPage(NamedTuple):
     rule_length: object = None
     figures: object = None
     figure_size: object = None
+    block_direction: object = None
 
 
 def _check_page(pg, H, W, name):
@@ -2134,6 +2140,12 @@ def _check_page(pg, H, W, name):
         if pg.figures is not None and getattr(pg, what) is not None:
             raise ValueError(f"{name}: figures and {what} are both given (a page with figures is level and flat: flatten a "
                              f"tilted or curled page with flatten_pages first)")
+    if pg.block_direction is not None and not (isinstance(pg.block_direction, str) and pg.block_direction == "auto"):
+        raise ValueError(f"{name}: block_direction must be None or 'auto', got {pg.block_direction!r}")
+    for what in ("skew", "curve"):
+        if pg.block_direction is not None and getattr(pg, what) is not None:
+            raise ValueError(f"{name}: block_direction and {what} are both given (a page whose blocks' directions are found is "
+                             f"level and flat: flatten a tilted or curled page with flatten_pages first)")
     if pg.quad is not None:
         if pg.rect is not None:
             raise ValueError(f"{name}: rect and quad are both given (a page in perspective is its quad: give rect=None)")
@@ -2243,7 +2255,7 @@ def _find_blocks(dimg, items, rq=None):
     """ops.find_blocks over items (image index, TextPage, rect) of the uploaded images ``dimg``, its tables back through one
     pinned copy and one synchronisation; a quad page (its corners given) is a level page on all of its rectified crop in ``rq``
     (_rectify).  Returns per item dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, rule_length, rule_pixels]
-    [, figure_size, figures]), or the error message of a page over a limit."""
+    [, figure_size, figures][, block_direction, undecided]), or the error message of a page over a limit."""
     from . import ops
     lib = ops._lib
 
@@ -2259,7 +2271,8 @@ def _find_blocks(dimg, items, rq=None):
     rls = [rule_length(*it) for it in items]
     fss = [None if pg.figures is None else pg.figure_size or 0 for _, pg, _ in items]
     res_t, caps = ops.find_blocks([(*src(i, pg, rect), pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y,
-                                    pg.skew, pg.max_skew, rl, fs) for (i, pg, rect), rl, fs in zip(items, rls, fss)])
+                                    pg.skew, pg.max_skew, rl, fs, pg.block_direction is not None)
+                                   for (i, pg, rect), rl, fs in zip(items, rls, fss)])
     host = _to_host(res_t).numpy()
     rdt, ndt, sdt = ops.page_result_dtype(), ops.page_node_dtype(), ops.skew_block_dtype()
     skewed = any(pg.skew is not None for _, pg, _ in items)
@@ -2286,14 +2299,23 @@ def _find_blocks(dimg, items, rq=None):
         X0, Y0 = (0, 0) if pg.quad is not None else rect[:2]
         vertical = pg.direction == "vertical"
         tilted = pg.skew is not None and sk["s"] != 0
-        blocks, rejected = [], []
+        blocks, rejected, dirs, undecided = [], [], [], []
         for q in leaves:
             x0, y0, x1, y1 = (int(q[f]) for f in ("x0", "y0", "x1", "y1"))
             if not tilted:
                 box = (X0 + x0, Y0 + y0, X0 + x1, Y0 + y1)
             else:                                       # a window of the block frame: a vertical page's bitmap is its transpose
                 box = (y0, x0, y1, x1) if vertical else (x0, y0, x1, y1)
-            (rejected if q["st"] & lib.PAGE_REJECTED else blocks).append(box)
+            if q["st"] & lib.PAGE_REJECTED:
+                rejected.append(box)
+                continue
+            if pg.block_direction is None:
+                dirs.append(pg.direction)
+            else:                                       # the leaf's own direction, or the page's when its test is undecided
+                dirs.append("vertical" if q["st"] & lib.PAGE_VERTICAL else "horizontal")
+                if q["st"] & lib.PAGE_UNDECIDED:
+                    undecided.append(len(blocks))
+            blocks.append(box)
         res = dict(threshold=int(r["threshold"]), ink="dark" if r["ink"] == lib.INK_DARK else "light",
                    text_size=int(r["text_size"]), gap_x=int(r["gap_x"]), gap_y=int(r["gap_y"]))
         if rl is not None:
@@ -2301,12 +2323,16 @@ def _find_blocks(dimg, items, rq=None):
         if fs is not None:                              # in image coordinates, or rectangles of R on a quad page
             res.update(figure_size=int(r["figure_size"]),
                        figures=[(X0 + int(q["x0"]), Y0 + int(q["y0"]), X0 + int(q["x1"]), Y0 + int(q["y1"])) for q in figs])
+        if pg.block_direction is not None:
+            res.update(block_direction=pg.block_direction, undecided=undecided)
         if pg.quad is not None:
             shape = dimg[i].shape[:2]
-            res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=pg.direction, polarity=pg.polarity, window=b) for b in blocks],
+            res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=d, polarity=pg.polarity, window=b)
+                               for b, d in zip(blocks, dirs)],
                        rejected=rejected, quad=_quad_key(i, pg.quad)[1], size=tuple(src(i, pg, rect)[1][2:]))
         elif pg.skew is None:
-            res.update(blocks=[TextBlock(b, pg.direction, polarity=pg.polarity, curve=pg.curve) for b in blocks], rejected=rejected)
+            res.update(blocks=[TextBlock(b, d, polarity=pg.polarity, curve=pg.curve) for b, d in zip(blocks, dirs)],
+                       rejected=rejected)
         else:
             res["skew"] = _skew_used(pg, sk)
             res["blocks"] = [TextBlock(tuple(rect), pg.direction, polarity=pg.polarity, skew=res["skew"], window=b) if tilted
@@ -2346,7 +2372,12 @@ def find_blocks(images, pages):
     side is at least its figure size f, selected on the device with the text size and taken out of its ink before the second
     XY-cut (1 more launch for all such pages of the call); each block stops growing at a figure as at a rule.  Its dict gains
     ``figure_size`` (the f used, 0 without a text size) and ``figures``, their rectangles in leaf order (as ``rejected``: in
-    image coordinates, or rectangles of R on a quad page).  A page over 1024 figures raises, as one over its block limit."""
+    image coordinates, or rectangles of R on a quad page).  A page over 1024 figures raises, as one over its block limit.
+    A page with ``block_direction="auto"`` (DESIGN.md 7b, "Mixed directions") is cut as before with its ``direction``, and each
+    of its blocks then has its own direction tested on the device from the row and column bands of its ink (1 more launch for
+    all such pages of the call, and no more memory): its TextBlocks (or from_quad windows) are "horizontal" or "vertical",
+    each restored as such.  Its dict gains ``block_direction`` ("auto") and ``undecided``, the indices of the blocks whose test
+    was undecided and which took the page's direction."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
@@ -2940,7 +2971,8 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     call in the same launches, one pinned copy and one synchronisation), its TextBlocks take its place, and each of them is then
     replaced by its lines as above, so the result is byte for byte that of the call given the found blocks.  No labels or boxes
     may be given for a page; a tilted page (``skew``) gives windowed TextBlocks, which are split as any other.  Its entry is
-    dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, skew][, figure_size, figures], regions), regions one
+    dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, skew][, figure_size, figures][, block_direction,
+    undecided], regions), regions one
     block entry per block; a page over its node or block limit, or one of whose blocks fails, raises, or is dict(error=...)
     with ``skip_invalid``, and then none of its blocks is restored.  A quad page or block (DESIGN.md 7b, "Perspective pages")
     is laid out on its rectified crop (TextPage(quad="auto") after the device's corner search), every distinct quad of the call
