@@ -818,11 +818,25 @@ int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* c
  * with MN_PAGE_DIRECTIONS issues 1 more launch after 11, whatever the number of pages: every kept leaf of such a page (its
  * ungrown rectangle in list[src]) has its row and column bands counted and its leaves[] entry marked MN_PAGE_VERTICAL when
  * its direction is vertical, and MN_PAGE_UNDECIDED (with the page's direction) when the test is undecided.  The launch skips
- * pages without dirs and pages with an error; a call without MN_PAGE_DIRECTIONS issues exactly the launches above. */
+ * pages without dirs and pages with an error; a call without MN_PAGE_DIRECTIONS issues exactly the launches above.
+ * Reversed panels (DESIGN.md section 7b, "Reversed panels"): a page with pans (inside work) has panels, and rbits (U's plane,
+ * h x wpitch words, with its scratch only when rule_length != 0) even without rules; the rule launches skip a page with
+ * rule_length 0.  At 7, such a page keeps its pass-1 leaves (no root yet) with p = panel_size, or S when it is 0, in
+ * res->panel_size.  A call with MN_PAGE_PANELS issues 2 more launches after 7, whatever the number of pages:
+ *   a. the panel test, one CTA per pass-1 leaf whose shorter side is at least p: a panel iff 2 |I' & leaf| > h w and more than
+ *      half of its pixels have a grey within 8 of its modal grey (ties to the smaller); such a leaf's st gains MN_PAGE_PANEL.
+ *      The last CTA of each page lists the panels in leaf order in pans (MN_PAGE_MAX_PANELS entries; st = the rows of the
+ *      panels before it; res->n_panels, or res->error = MN_PAGE_ERR_PANELS over the limit), selects the figures among the other
+ *      leaves and writes the root of pass 2;
+ *   b. every panel row painted, one warp per row: the interior inverted in bits (J = not I), the 1-pixel outline cleared from
+ *      bits and OR'd into rbits, so that the rule-index cut and the growth stops see it as a rule.
+ * A call without MN_PAGE_PANELS issues exactly the launches above. */
 #define MN_PAGE_RULES 1
 #define MN_PAGE_FIGURES 2
 #define MN_PAGE_DIRECTIONS 4
+#define MN_PAGE_PANELS 8
 #define MN_PAGE_MAX_FIGURES 1024
+#define MN_PAGE_MAX_PANELS 1024
 #define MN_PAGE_LEVELS 24
 #define MN_PAGE_MAX_BLOCKS 1024
 #define MN_PAGE_MAX_NODES 65536
@@ -832,9 +846,11 @@ int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* c
 #define MN_PAGE_REJECTED 8      /* node st: a leaf that is not text */
 #define MN_PAGE_VERTICAL 16     /* leaf st: a block of a direction page whose direction is vertical */
 #define MN_PAGE_UNDECIDED 32    /* leaf st: a block of a direction page that took the page's direction, its test undecided */
+#define MN_PAGE_PANEL 64        /* pass-1 leaf st: a panel of a panel page */
 #define MN_PAGE_ERR_NODES 1
 #define MN_PAGE_ERR_BLOCKS 2
 #define MN_PAGE_ERR_FIGURES 3
+#define MN_PAGE_ERR_PANELS 4
 typedef struct {
     int16_t x0, y0, x1, y1;     /* in the crop */
     int32_t st;
@@ -843,7 +859,8 @@ typedef struct {
     int32_t error, n_leaves, n_blocks, text_size;
     int32_t gap_x, gap_y, threshold, ink;
     int32_t rule_pixels;        /* |U| of a ruled page (DESIGN.md section 7b, "Ruled pages"), else 0 */
-    int32_t figure_size, n_figures, pad;   /* f and the number of figures of a figure page with a text size, else 0 */
+    int32_t figure_size, n_figures;        /* f and the number of figures of a figure page with a text size, else 0 */
+    int32_t panel_size, n_panels, pad;     /* p and the number of panels of a panel page with a text size, else 0 */
 } mn_page_result;
 typedef struct {
     mn_text_block b;            /* the crop record (b.hist, b.out as mn_find_lines_u8's) */
@@ -863,6 +880,10 @@ typedef struct {
     mn_page_node* figs;         /* a figure page's table of MN_PAGE_MAX_FIGURES figures */
     int32_t figure_size;        /* a figure page's f in [2, 32767], or 0 for 3 S */
     int32_t frows;              /* state: the rows of all of its figures */
+    mn_page_node* pans;         /* null, or a panel page's table of MN_PAGE_MAX_PANELS panels */
+    int32_t panel_size;         /* a panel page's p in [2, 32767], or 0 for S */
+    int32_t prows;              /* state: the rows of all of its panels */
+    int32_t pdone, pad3;        /* state: the panel test's CTAs done with the page */
 } mn_text_page;
 int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, int ruled, void* work,
                       long long work_bytes, void* stream);
@@ -876,8 +897,9 @@ int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, l
  *      or for a vertical page at (c, -s) on the untransposed crop (the transposed search frame with its axes swapped); the root
  *      node, and pages[i].b.w = M, pages[i].b.h = L;
  *   6-13. mn_find_blocks_u8's levels, text size and leaves, in frame cells (with its 3 rule launches under MN_PAGE_RULES,
- *         its figure launch under MN_PAGE_FIGURES and its direction launch under MN_PAGE_DIRECTIONS; a ruled, figure or
- *         direction page has skew None, so its frame bitmap is mn_find_blocks_u8's).
+ *         its figure launch under MN_PAGE_FIGURES, its direction launch under MN_PAGE_DIRECTIONS and its 2 panel launches
+ *         under MN_PAGE_PANELS; a ruled, figure, direction or panel page has skew None, so its frame bitmap is
+ *         mn_find_blocks_u8's).
  * bits holds max L x wpitch words, wpitch >= max M / 32, and cap entries per list, max over the page's table; the angle
  * profiles and scores are as mn_find_lines_skewed_u8's (b.prof unused).  work (work_bytes) is zeroed by the call. */
 int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles, int ruled,

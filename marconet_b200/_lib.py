@@ -210,9 +210,10 @@ class CurveBlock(Structure):
 
 PAGE_LEVELS, PAGE_MAX_BLOCKS, PAGE_MAX_NODES = 24, 1024, 65536    # MN_PAGE_LEVELS, MN_PAGE_MAX_BLOCKS, MN_PAGE_MAX_NODES
 PAGE_REJECTED = 8                                                  # MN_PAGE_REJECTED
-PAGE_ERR_NODES, PAGE_ERR_BLOCKS, PAGE_ERR_FIGURES = 1, 2, 3
+PAGE_ERR_NODES, PAGE_ERR_BLOCKS, PAGE_ERR_FIGURES, PAGE_ERR_PANELS = 1, 2, 3, 4
 PAGE_RULES, PAGE_FIGURES, PAGE_MAX_FIGURES = 1, 2, 1024           # MN_PAGE_RULES, MN_PAGE_FIGURES, MN_PAGE_MAX_FIGURES
 PAGE_DIRECTIONS, PAGE_VERTICAL, PAGE_UNDECIDED = 4, 16, 32         # MN_PAGE_DIRECTIONS, MN_PAGE_VERTICAL, MN_PAGE_UNDECIDED
+PAGE_PANELS, PAGE_MAX_PANELS = 8, 1024                             # MN_PAGE_PANELS, MN_PAGE_MAX_PANELS
 
 
 class PageNode(Structure):
@@ -222,7 +223,7 @@ class PageNode(Structure):
 class PageResult(Structure):
     _fields_ = [("error", c_int32), ("n_leaves", c_int32), ("n_blocks", c_int32), ("text_size", c_int32), ("gap_x", c_int32),
                 ("gap_y", c_int32), ("threshold", c_int32), ("ink", c_int32), ("rule_pixels", c_int32), ("figure_size", c_int32),
-                ("n_figures", c_int32), ("pad", c_int32)]
+                ("n_figures", c_int32), ("panel_size", c_int32), ("n_panels", c_int32), ("pad", c_int32)]
 
 
 class TextPage(Structure):
@@ -230,7 +231,8 @@ class TextPage(Structure):
                 ("nopen", c_void_p), ("off", c_void_p), ("res", c_void_p), ("wpitch", c_int32), ("cap", c_int32),
                 ("gap_x", c_int32), ("gap_y", c_int32), ("src", c_int32), ("active", c_int32), ("open", c_int32), ("gx", c_int32),
                 ("gy", c_int32), ("pad", c_int32), ("n", c_int32 * 2), ("rbits", c_void_p), ("rule_length", c_int32), ("dirs", c_int32),
-                ("fbits", c_void_p), ("figs", c_void_p), ("figure_size", c_int32), ("frows", c_int32)]
+                ("fbits", c_void_p), ("figs", c_void_p), ("figure_size", c_int32), ("frows", c_int32), ("pans", c_void_p),
+                ("panel_size", c_int32), ("prows", c_int32), ("pdone", c_int32), ("pad3", c_int32)]
 
 
 class PageQuad(Structure):

@@ -11,7 +11,9 @@
 // least a rule length in rows and columns in three more launches, take them out of the page's bitmap and let them cut.  Figures
 // (DESIGN.md 7b, "Figures") are the pass-1 leaves of at least a figure size, selected with the text size and painted out of the
 // bitmap in one more launch before pass 2.  Mixed directions (DESIGN.md 7b, "Mixed directions") test each kept leaf's row and
-// column bands for its own direction in one more launch after the leaves.
+// column bands for its own direction in one more launch after the leaves.  Reversed panels (DESIGN.md 7b, "Reversed panels")
+// are the flat-filled pass-1 leaves of over half ink, tested and painted as paper-coloured ink inside a rule outline in two more
+// launches before pass 2.
 #include <climits>
 
 #include "mn_common.cuh"
@@ -1166,31 +1168,53 @@ __global__ void __launch_bounds__(kPageThreads, 1) page_emit_kernel(mn_text_page
     }
 }
 
-// The figures of a figure page (DESIGN.md 7b, "Figures"), by the CTA: its pass-1 leaves list[0 .. n) whose shorter side is at
-// least f, in leaf order, into p.figs (st: the rows of the figures before it), their rows into p.frows and f and their number
-// into res; over MN_PAGE_MAX_FIGURES the page error.  Returns false on that error.  Ends with a barrier.
-__device__ bool page_figures(mn_text_page& p, const mn_page_node* list, int n, int S, int* s_scan) {
-    const int f = p.figure_size > 0 ? p.figure_size : 3 * S;
+// A page node read through L2: the panel test's last CTA reads nodes other CTAs have just marked.
+__device__ __forceinline__ mn_page_node load_node(const mn_page_node* a) {
+    const int* q = reinterpret_cast<const int*>(a);
+    const int v0 = __ldcg(q), v1 = __ldcg(q + 1), v2 = __ldcg(q + 2);
+    mn_page_node g;
+    g.x0 = (int16_t)(v0 & 0xffff); g.y0 = (int16_t)(v0 >> 16); g.x1 = (int16_t)(v1 & 0xffff); g.y1 = (int16_t)(v1 >> 16);
+    g.st = v2;
+    return g;
+}
+
+// The pass-1 leaves list[0 .. n) for which keep(leaf) holds, by the CTA, in leaf order into table (st: the rows of the entries
+// before it), unless they are more than max: returns their number, and their rows in *rows.  Ends with a barrier.
+template <class Keep>
+__device__ int page_table(const mn_page_node* list, int n, Keep keep, mn_page_node* table, int max, int* s_scan, int* rows) {
     const int chunk = (n + blockDim.x - 1) / blockDim.x, i0 = threadIdx.x * chunk, i1 = min(n, i0 + chunk);
-    auto figure = [&](int i) { return min(list[i].x1 - list[i].x0, list[i].y1 - list[i].y0) >= f; };
-    int c = 0, r = 0, total, rows;
+    int c = 0, r = 0, total;
     for (int i = i0; i < i1; ++i) {
-        if (!figure(i)) continue;
+        const mn_page_node g = load_node(list + i);
+        if (!keep(g)) continue;
         ++c;
-        r += list[i].y1 - list[i].y0;
+        r += g.y1 - g.y0;
     }
     int k = cta_scan(c, s_scan, &total);
-    r = cta_scan(r, s_scan, &rows);                     // disjoint, sides >= 2: at most w h / 2 rows
-    if (total <= MN_PAGE_MAX_FIGURES) {
+    r = cta_scan(r, s_scan, rows);                      // disjoint, sides >= 2: at most w h / 2 rows
+    if (total <= max) {
         for (int i = i0; i < i1; ++i) {
-            if (!figure(i)) continue;
-            mn_page_node g = list[i];
+            mn_page_node g = load_node(list + i);
+            if (!keep(g)) continue;
             g.st = r;
-            p.figs[k++] = g;
+            table[k++] = g;
             r += g.y1 - g.y0;
         }
     }
     __syncthreads();                                    // list is read before the root overwrites it
+    return total;
+}
+
+// The figures of a figure page (DESIGN.md 7b, "Figures"), by the CTA: its pass-1 leaves that are not panels and whose shorter
+// side is at least f, into p.figs (page_table), their rows into p.frows and f and their number into res; over
+// MN_PAGE_MAX_FIGURES the page error.  Returns false on that error.  Ends with a barrier.
+__device__ bool page_figures(mn_text_page& p, const mn_page_node* list, int n, int S, int* s_scan) {
+    const int f = p.figure_size > 0 ? p.figure_size : 3 * S;
+    auto figure = [f](const mn_page_node& g) {          // a panel is never a figure
+        return !(g.st & MN_PAGE_PANEL) && min(g.x1 - g.x0, g.y1 - g.y0) >= f;
+    };
+    int rows;
+    const int total = page_table(list, n, figure, p.figs, MN_PAGE_MAX_FIGURES, s_scan, &rows);
     if (threadIdx.x == 0) {
         p.res->figure_size = f;
         p.res->n_figures = total;
@@ -1200,8 +1224,27 @@ __device__ bool page_figures(mn_text_page& p, const mn_page_node* list, int n, i
     return total <= MN_PAGE_MAX_FIGURES;
 }
 
+// The gaps of pass 2 for the text size S, and its root (thread 0).
+__device__ void page_root(mn_text_page& p, int S) {
+    const int wide = S, narrow = max(1, S / 2);
+    p.src = 0;
+    p.gx = p.gap_x > 0 ? p.gap_x : p.b.vertical ? narrow : wide;
+    p.gy = p.gap_y > 0 ? p.gap_y : p.b.vertical ? wide : narrow;
+    p.res->text_size = S;
+    p.res->gap_x = p.gx;
+    p.res->gap_y = p.gy;
+    mn_page_node r;
+    r.x0 = 0; r.y0 = 0; r.x1 = (int16_t)p.b.w; r.y1 = (int16_t)p.b.h;
+    r.st = p.b.vertical ? 0 : MN_PAGE_ROWS;
+    p.list[0][0] = r;
+    p.n[0] = 1;
+    p.open = 1;
+}
+
 // 7. Text size S: the lower median of max(h, w) over the leaves with max(h, w) >= 2, by bisection over counts; the gaps of
-// pass 2 and its root.  A page without such a leaf has no blocks; a figure page's figures are selected first.
+// pass 2 and its root.  A page without such a leaf has no blocks; a figure page's figures are selected first.  A panel page
+// with such a leaf keeps its pass-1 leaves: S and p go to res, and the panel test selects its panels and figures and writes
+// the root.
 __global__ void __launch_bounds__(kScanThreads) page_size_kernel(mn_text_page* pages) {
     mn_pdl_prologue();
     __shared__ int s_scan[32];
@@ -1225,26 +1268,22 @@ __global__ void __launch_bounds__(kScanThreads) page_size_kernel(mn_text_page* p
         cta_scan(k, s_scan, &t);
         if (t > (n2 - 1) / 2) hi = mid; else lo = mid + 1;
     }
+    if (n2 > 0 && p.pans) {
+        if (threadIdx.x == 0) {
+            p.res->text_size = lo;
+            p.res->panel_size = p.panel_size > 0 ? p.panel_size : lo;
+        }
+        return;
+    }
     const bool ok = n2 == 0 || !p.fbits || page_figures(p, list, n, lo, s_scan);
     if (threadIdx.x != 0) return;
-    p.src = 0;
     if (n2 == 0 || !ok) {
+        p.src = 0;
         p.n[0] = 0;
         p.open = 0;
         return;
     }
-    const int S = lo, wide = S, narrow = max(1, S / 2);
-    p.gx = p.gap_x > 0 ? p.gap_x : p.b.vertical ? narrow : wide;
-    p.gy = p.gap_y > 0 ? p.gap_y : p.b.vertical ? wide : narrow;
-    p.res->text_size = S;
-    p.res->gap_x = p.gx;
-    p.res->gap_y = p.gy;
-    mn_page_node r;
-    r.x0 = 0; r.y0 = 0; r.x1 = (int16_t)p.b.w; r.y1 = (int16_t)p.b.h;
-    r.st = p.b.vertical ? 0 : MN_PAGE_ROWS;
-    p.list[0][0] = r;
-    p.n[0] = 1;
-    p.open = 1;
+    page_root(p, lo);
 }
 
 // The greatest (kMin: least) row (kRows) or column of the rectangle [xa, xb) x [ya, yb) of a ruled or figure page that holds a
@@ -1411,7 +1450,7 @@ __device__ __forceinline__ void line_runs(const uint32_t* src, uint32_t* dst, in
 __global__ void __launch_bounds__(kRuleThreads) rule_transpose_kernel(mn_text_page* pages) {
     mn_pdl_prologue();
     const mn_text_page& p = pages[blockIdx.y];
-    if (!p.rbits) return;
+    if (!p.rbits || !p.rule_length) return;
     const int w = p.b.w, h = p.b.h, nw = (w + 31) >> 5, th = (h + 31) >> 5, lane = threadIdx.x & 31;
     constexpr int kWarps = kRuleThreads / 32;
     uint32_t* tp = rule_plane(p);
@@ -1426,7 +1465,7 @@ __global__ void __launch_bounds__(kRuleThreads) rule_transpose_kernel(mn_text_pa
 __global__ void __launch_bounds__(kRuleThreads, 1) rule_runs_kernel(mn_text_page* pages) {
     mn_pdl_prologue();
     const mn_text_page& p = pages[blockIdx.y];
-    if (!p.rbits) return;
+    if (!p.rbits || !p.rule_length) return;
     const int w = p.b.w, h = p.b.h, th = (h + 31) >> 5;
     constexpr int kWarps = kRuleThreads / 32;
     uint32_t* tp = rule_plane(p);
@@ -1441,7 +1480,7 @@ __global__ void __launch_bounds__(kRuleThreads) rule_merge_kernel(mn_text_page* 
     mn_pdl_prologue();
     __shared__ int s_count;
     const mn_text_page& p = pages[blockIdx.y];
-    if (!p.rbits) return;
+    if (!p.rbits || !p.rule_length) return;
     const int w = p.b.w, h = p.b.h, nw = (w + 31) >> 5, th = (h + 31) >> 5, lane = threadIdx.x & 31;
     constexpr int kWarps = kRuleThreads / 32;
     const uint32_t* tp = rule_plane(p);
@@ -1489,6 +1528,151 @@ __global__ void __launch_bounds__(kFigureThreads) figure_paint_kernel(mn_text_pa
             const unsigned m = word_mask(wd, g.x0, g.x1);
             atomicOr(p.fbits + o + wd, m);
             atomicAnd(p.bits + o + wd, ~m);
+        }
+    }
+}
+
+// ---- Reversed panels (DESIGN.md 7b, "Reversed panels") ----
+// P1. The panel test of every pass-1 leaf of a panel page whose shorter side is at least p, one CTA per leaf (grid-stride over
+// blockIdx.x): its ink count |I' & leaf| and, when that is over half the rectangle, the 256-bin histogram of its greys, the
+// mode m (ties to the smaller grey) and the flat count of greys in [m - 8, m + 8]; a panel iff the flat count is over half, and
+// its st gains MN_PAGE_PANEL.  The last CTA of each page then lists its panels (st: the rows of the panels before it), selects
+// its figures among the other leaves and writes the root of pass 2.  Pages without pans, without a text size or with an error
+// return at once.
+constexpr int kPanelFlat = 8;
+constexpr int kPanelThreads = 1024;                   // 32 warps: the pixel loads of one large leaf in flight
+constexpr int kPanelWarps = kPanelThreads / 32;
+constexpr int kPanelUnroll = 8;
+
+__device__ __forceinline__ long long cta_sum64(long long v, long long* s) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();
+    if (lane == 0) s[warp] = v;
+    __syncthreads();
+    long long t = 0;
+    for (int k = 0; k < (int)(blockDim.x >> 5); ++k) t += s[k];
+    return t;
+}
+
+__global__ void __launch_bounds__(kPanelThreads) panel_test_kernel(mn_text_page* pages) {
+    mn_pdl_prologue();
+    __shared__ int s_hist[kPanelWarps * 256];
+    __shared__ long long s_sum[kPanelWarps];
+    __shared__ unsigned long long s_best[8];
+    __shared__ int s_scan[32];
+    __shared__ bool s_last;
+    mn_text_page& p = pages[blockIdx.y];
+    if (!p.pans || p.res->error || p.res->panel_size == 0) return;
+    mn_page_node* list = p.list[p.src];
+    const mn_text_block b = p.b;                        // the crop record in registers for the pixel loop
+    const int n = p.n[p.src], P = p.res->panel_size, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int i = blockIdx.x; i < n; i += gridDim.x) {
+        const mn_page_node nd = list[i];
+        const int h = nd.y1 - nd.y0, w = nd.x1 - nd.x0;
+        if (min(h, w) < P) continue;
+        const int wx0 = nd.x0 >> 5, nwords = ((nd.x1 - 1) >> 5) - wx0 + 1;
+        long long ink = 0;                              // one warp per row
+        for (int y = nd.y0 + warp; y < nd.y1; y += kPanelWarps) {
+            for (int wd = wx0 + lane; wd < wx0 + nwords; wd += 32)
+                ink += __popc(p.bits[(long long)y * p.wpitch + wd] & word_mask(wd, nd.x0, nd.x1));
+        }
+        const long long area = (long long)h * w;
+        if (2 * cta_sum64(ink, s_sum) <= area) continue;
+        for (int k = threadIdx.x; k < kPanelWarps * 256; k += blockDim.x) s_hist[k] = 0;
+        __syncthreads();
+        int* hist = s_hist + 256 * warp;                // one histogram per warp; each thread counts runs of its greys
+        int cur = -1, run = 0;
+        for (int y = nd.y0 + warp; y < nd.y1; y += kPanelWarps) {
+            for (int x0 = nd.x0 + lane; x0 < nd.x1; x0 += 32 * kPanelUnroll) {
+                int g[kPanelUnroll];                    // the loads of kPanelUnroll pixels in flight together
+#pragma unroll
+                for (int u = 0; u < kPanelUnroll; ++u) g[u] = x0 + 32 * u < nd.x1 ? block_grey(b, x0 + 32 * u, y) : -1;
+#pragma unroll
+                for (int u = 0; u < kPanelUnroll; ++u) {
+                    if (g[u] < 0 || g[u] == cur) {
+                        run += g[u] >= 0;
+                        continue;
+                    }
+                    if (run) atomicAdd(hist + cur, run);
+                    cur = g[u];
+                    run = 1;
+                }
+            }
+        }
+        if (run) atomicAdd(hist + cur, run);
+        __syncthreads();
+        const int t = threadIdx.x;                      // threads 0 .. 255: the bins
+        int v = 0;
+        for (int k = 0; k < kPanelWarps && t < 256; ++k) v += s_hist[256 * k + t];
+        __syncthreads();
+        if (t < 256) s_hist[t] = v;
+        __syncthreads();
+        unsigned long long key = t < 256 ? ((unsigned long long)v << 8) | (255u - t) : 0ull;
+#pragma unroll
+        for (int o = 16; o; o >>= 1) key = max(key, __shfl_xor_sync(0xffffffffu, key, o));
+        if (lane == 0 && warp < 8) s_best[warp] = key;
+        __syncthreads();
+        unsigned long long best = 0;
+        for (int k = 0; k < 8; ++k) best = max(best, s_best[k]);
+        const int m = 255 - (int)(best & 255u);
+        const long long flat = cta_sum64(t < 256 && abs(t - m) <= kPanelFlat ? v : 0, s_sum);
+        if (threadIdx.x == 0 && 2 * flat > area) list[i].st = nd.st | MN_PAGE_PANEL;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();                                // this CTA's marks before its ticket
+        s_last = atomicAdd(&p.pdone, 1) == (int)gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    int rows;
+    auto panel = [](const mn_page_node& g) { return (g.st & MN_PAGE_PANEL) != 0; };
+    const int total = page_table(list, n, panel, p.pans, MN_PAGE_MAX_PANELS, s_scan, &rows);
+    const bool ok = total <= MN_PAGE_MAX_PANELS && (!p.fbits || page_figures(p, list, n, p.res->text_size, s_scan));
+    if (threadIdx.x != 0) return;
+    p.res->n_panels = total;
+    if (total > MN_PAGE_MAX_PANELS) p.res->error = MN_PAGE_ERR_PANELS;
+    if (!ok) {
+        p.src = 0;
+        p.n[0] = 0;
+        p.open = 0;
+        return;
+    }
+    p.prows = rows;
+    page_root(p, p.res->text_size);
+}
+
+// P2. Every row of every panel of a panel page (panel_test_kernel's table), one warp each: its interior (the rectangle less its
+// 1-pixel outline) inverted in bits, which holds I' = I and not U, to J = not I (its U pixels stay clear), and its outline
+// cleared from bits and OR'd into rbits.  Panels may share a word at their ends, hence the atomics.  Pages without pans, and
+// pages with an error, return at once.
+__global__ void __launch_bounds__(kFigureThreads) panel_paint_kernel(mn_text_page* pages) {
+    mn_pdl_prologue();
+    const mn_text_page& p = pages[blockIdx.y];
+    if (!p.pans || p.res->error) return;
+    const int np = p.res->n_panels, lane = threadIdx.x & 31;
+    constexpr int kWarps = kFigureThreads / 32;
+    for (int t = blockIdx.x * kWarps + (threadIdx.x >> 5); t < p.prows; t += gridDim.x * kWarps) {
+        int lo = 0, hi = np - 1;                        // the last panel whose first row index is <= t
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (p.pans[mid].st <= t) lo = mid; else hi = mid - 1;
+        }
+        const mn_page_node g = p.pans[lo];
+        const int y = g.y0 + t - g.st;
+        const bool edge_row = y == g.y0 || y == g.y1 - 1;
+        const long long o = (long long)y * p.wpitch;
+        for (int wd = (g.x0 >> 5) + lane; wd <= (g.x1 - 1) >> 5; wd += 32) {
+            const unsigned all = word_mask(wd, g.x0, g.x1);
+            const unsigned inner = edge_row ? 0u : word_mask(wd, g.x0 + 1, g.x1 - 1), edge = all & ~inner;
+            if (inner) atomicXor(p.bits + o + wd, inner & ~p.rbits[o + wd]);
+            if (edge) {
+                atomicOr(p.rbits + o + wd, edge);
+                atomicAnd(p.bits + o + wd, ~edge);
+            }
         }
     }
 }
@@ -1961,8 +2145,8 @@ __global__ void __launch_bounds__(kHullThreads) quad_hull_kernel(const mn_quad_p
 }
 
 // 4-11 of the XY-cut: both passes of levels, the text size between them and the leaves, on pages whose bitmap and root are
-// written; under MN_PAGE_RULES, the three rule launches first, under MN_PAGE_FIGURES the figure launch after the text size, and
-// under MN_PAGE_DIRECTIONS the direction launch after the leaves.
+// written; under MN_PAGE_RULES, the three rule launches first, under MN_PAGE_PANELS the panel test and paint after the text
+// size, under MN_PAGE_FIGURES the figure launch after those, and under MN_PAGE_DIRECTIONS the direction launch after the leaves.
 int page_levels(mn_text_page* pages, int n, long long max_tiles, int flags, cudaStream_t st) {
     const dim3 rgrid((unsigned)mn_cdiv64(max_tiles, kRuleThreads / 32), (unsigned)n);
     if (flags & MN_PAGE_RULES) {
@@ -1986,6 +2170,12 @@ int page_levels(mn_text_page* pages, int n, long long max_tiles, int flags, cuda
         if (pass == 0) {
             MN_CUDA_CHECK((mn_launch(page_size_kernel, dim3(n), dim3(kScanThreads), 0, st, pages)));
             MN_LAUNCH_CHECK();
+            if (flags & MN_PAGE_PANELS) {
+                MN_CUDA_CHECK((mn_launch(panel_test_kernel, grid, dim3(kPanelThreads), 0, st, pages)));
+                MN_LAUNCH_CHECK();
+                MN_CUDA_CHECK((mn_launch(panel_paint_kernel, rgrid, dim3(kFigureThreads), 0, st, pages)));
+                MN_LAUNCH_CHECK();
+            }
             if (flags & MN_PAGE_FIGURES) {
                 MN_CUDA_CHECK((mn_launch(figure_paint_kernel, rgrid, dim3(kFigureThreads), 0, st, pages)));
                 MN_LAUNCH_CHECK();

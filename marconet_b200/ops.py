@@ -2110,6 +2110,13 @@ def figure_page_bytes(w, h):
     return 4 * h * -(-w // 32) + 12 * _lib.PAGE_MAX_FIGURES
 
 
+def panel_page_bytes(w, h, ruled):
+    """Device bytes a w x h page adds to find_blocks when it has panels (DESIGN.md 7b, "Reversed panels"): the plane of U that
+    takes the panels' outlines (h rows of ceil(w / 32) words) unless the page is ``ruled`` and has one, and its panel table of
+    PAGE_MAX_PANELS page nodes."""
+    return (0 if ruled else 4 * h * -(-w // 32)) + 12 * _lib.PAGE_MAX_PANELS
+
+
 def skew_page_frame(w, h, vertical, cs):
     """(L, M, stride) of a w x h page's frame bitmaps over the (c, s) of ``cs``: the most rows and columns a bitmap may have (the
     search frame's axes swapped for a vertical page) and the most bins of its search frames."""
@@ -2151,13 +2158,21 @@ def find_blocks(pages, scores=False):
     its kept leaves has its own direction tested, _lib.PAGE_VERTICAL set in its st when it is vertical and
     _lib.PAGE_UNDECIDED when the test is undecided (it then takes the page's direction).  A call with such a page issues 1
     more launch whatever the number of pages and needs no more memory; the other pages' tables are those of a call without
-    it."""
+    it.
+    panel_size (DESIGN.md 7b, "Reversed panels"), a twelfth entry: None, or on a page with skew None 0 (the panel size S) or
+    an integer p in [2, 32767]: its pass-1 leaves of shorter side at least p that are over half ink and flat-filled are its
+    panels, whose insides are cut as ink of the other polarity inside a rule outline (with rule_length, after the rules U
+    have left the ink: a fill with runs of at least rule_length is no panel).  A call with such a page issues 2 more
+    launches whatever the number of pages; its records gain panel_size and n_panels, and out ends, after the figure tables,
+    with each such page's table of _lib.PAGE_MAX_PANELS mn_page_node panels, in the order of the pages.  The other pages'
+    tables are those of a call without it."""
     global LAUNCHES
     dev = _check_items(pages, "find_blocks", "page")
     skewed = any(len(p) > 6 and p[6] is not None for p in pages)
     rules = [p[8] if len(p) > 8 else None for p in pages]
     figs = [p[9] if len(p) > 9 else None for p in pages]
     dirs = [p[10] if len(p) > 10 else None for p in pages]
+    pans = [p[11] if len(p) > 11 else None for p in pages]
     n = len(pages)
     rsz, bsz, psz, lsz = (ctypes.sizeof(t) for t in (_lib.PageResult, _lib.TextBlock, _lib.TextPage, _lib.BlockLines))
     ssz = ctypes.sizeof(_lib.SkewBlock) if skewed else 0
@@ -2176,10 +2191,15 @@ def find_blocks(pages, scores=False):
             raise ValueError(f"{what}: figure_size {fs!r} is not 0 or an integer in [2, 32767] on a page with skew None")
         if (dirs[i] is not None and not isinstance(dirs[i], bool)) or (dirs[i] and skew is not None):
             raise ValueError(f"{what}: directions {dirs[i]!r} is not None, False or True on a page with skew None")
+        ps = pans[i]
+        if ps is not None and (isinstance(ps, bool) or not isinstance(ps, int) or not (ps == 0 or 2 <= ps <= 32767)
+                               or skew is not None):
+            raise ValueError(f"{what}: panel_size {ps!r} is not 0 or an integer in [2, 32767] on a page with skew None")
         L, M, stride = (bh, bw, bw if vertical else bh) if skew is None else skew_page_frame(bw, bh, vertical, cs)
         need += skew_page_bytes(bw, bh, vertical, cs) if skewed else page_bytes(bw, bh)
         need += rule_page_bytes(bw, bh) if rl is not None else 0
         need += figure_page_bytes(bw, bh) if fs is not None else 0
+        need += panel_page_bytes(bw, bh, rl is not None) if ps is not None else 0
         if max(L, M) > 32767:
             raise ValueError(f"{what}: a frame side of {max(L, M)} exceeds 32767")
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
@@ -2194,16 +2214,18 @@ def find_blocks(pages, scores=False):
     out0 = -(-(tab0 + len(tab) + n * ssz) // 16) * 16    # then the work: the call zeroes everything from out0 on, and the
     sk0 = out0 - n * ssz                                 # skew records come back with the results in one copy
     n_leaves = n * rsz + 12 * sum(d[4] for d in dims)
-    n_out = n_leaves + 12 * _lib.PAGE_MAX_FIGURES * sum(fs is not None for fs in figs)
+    n_figs = n_leaves + 12 * _lib.PAGE_MAX_FIGURES * sum(fs is not None for fs in figs)
+    n_out = n_figs + 12 * _lib.PAGE_MAX_PANELS * sum(ps is not None for ps in pans)
     work0 = out0 + -(-n_out // 16) * 16
     per = [-(-(8 * (d[7] if d[7] > 1 else 0) + 4 * 256 + lsz + 4 * d[5] * -(-d[6] // 32) + 2 * 12 * d[4] + 3 * 4 * d[4]
                 + 4 * (d[7] * d[8] if d[7] > 1 else 0) + (rule_page_bytes(d[6], d[5]) if rl is not None else 0)
-                + (4 * d[5] * -(-d[6] // 32) if fs is not None else 0)) // 16) * 16
-           for d, rl, fs in zip(dims, rules, figs)]
+                + (4 * d[5] * -(-d[6] // 32) if fs is not None else 0)
+                + (4 * d[5] * -(-d[6] // 32) if ps is not None and rl is None else 0)) // 16) * 16
+           for d, rl, fs, ps in zip(dims, rules, figs, pans)]
     buf = torch.empty(work0 + sum(per), dtype=torch.uint8, device=dev)
     base = buf.data_ptr()
     leaves, w, blocks, srecs, recs, views, tiles = base + out0 + n * rsz, base + work0, [], [], [], [], 0
-    ftab = base + out0 + n_leaves
+    ftab, ptab = base + out0 + n_leaves, base + out0 + n_figs
     for i, (pg, d, nb, t) in enumerate(zip(pages, dims, per, t_offs)):
         img, _, vertical, polarity, gap_x, gap_y = pg[:6]
         x0, y0, bw, bh, cap, L, M, n_ang, stride = d
@@ -2214,16 +2236,20 @@ def find_blocks(pages, scores=False):
         counts = lists + 2 * 12 * cap
         rbits = counts + 3 * 4 * cap + 4 * (n_ang * stride if n_ang > 1 else 0)
         fbits = rbits + (rule_page_bytes(M, L) if rules[i] is not None else 0)
+        pbits = fbits + (4 * L * wp if figs[i] is not None else 0)   # a panel page's U plane when it has no rules
+        ubits = rbits if rules[i] is not None else pbits if pans[i] is not None else None
         tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, 0, 0, 0, 0, hist, 0, 0, lines)
         blocks.append(tb)
         if skewed:
             srecs.append(_skew_block(tb, base + tab0 + 16 * t, w, counts + 3 * 4 * cap, n_ang, stride))
         recs.append(_lib.TextPage(tb, bits, (ctypes.c_void_p * 2)(lists, lists + 12 * cap), leaves, counts, counts + 4 * cap,
                                   counts + 8 * cap, base + out0 + i * rsz, wp, cap, gap_x or 0, gap_y or 0,
-                                  rbits=rbits if rules[i] is not None else None, rule_length=rules[i] or 0,
+                                  rbits=ubits, rule_length=rules[i] or 0,
                                   fbits=fbits if figs[i] is not None else None, figs=ftab if figs[i] is not None else None,
-                                  figure_size=figs[i] or 0, dirs=int(bool(dirs[i]))))
+                                  figure_size=figs[i] or 0, dirs=int(bool(dirs[i])),
+                                  pans=ptab if pans[i] is not None else None, panel_size=pans[i] or 0))
         ftab += 12 * _lib.PAGE_MAX_FIGURES if figs[i] is not None else 0
+        ptab += 12 * _lib.PAGE_MAX_PANELS if pans[i] is not None else 0
         views.append(buf[w - base:w - base + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         leaves += 12 * cap
         w += nb
@@ -2232,16 +2258,17 @@ def find_blocks(pages, scores=False):
     host += bytes(sk0 - len(host)) + bytes((_lib.SkewBlock * len(srecs))(*srecs))
     buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
     ruled, figured = any(rl is not None for rl in rules), any(fs is not None for fs in figs)
-    directed = any(bool(d) for d in dirs)
+    directed, paneled = any(bool(d) for d in dirs), any(ps is not None for ps in pans)
     flags = (_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0) | (_lib.PAGE_DIRECTIONS if directed else 0)
+    flags |= _lib.PAGE_PANELS if paneled else 0
     if skewed:
         _lib.check(_lib.load().mn_find_blocks_skewed_u8(base, base + sk0, base + pg0, n, tiles, flags, base + out0,
                                                         work0 + sum(per) - out0, _stream()), "mn_find_blocks_skewed_u8")
-        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed
+        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed + 2 * paneled
     else:
         _lib.check(_lib.load().mn_find_blocks_u8(base, base + pg0, n, tiles, flags, base + out0, work0 + sum(per) - out0,
                                                  _stream()), "mn_find_blocks_u8")
-        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed
+        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed + 2 * paneled
     res = buf[sk0:out0 + n_out], [d[4] for d in dims]
     return res + (views,) if scores else res
 

@@ -2097,7 +2097,14 @@ class TextPage(NamedTuple):
     mixes horizontal and vertical text: each block found gets its own direction, "horizontal" or "vertical", from its row and
     column ink bands, and takes ``direction`` when that test is undecided.  ``direction`` keeps its role for the cut and the
     reading order of the blocks.  TextPage(rect, block_direction="auto") is one rectangle of unknown direction when it holds
-    one block.  Not with skew or curve: flatten such a page with flatten_pages first."""
+    one block.  Not with skew or curve: flatten such a page with flatten_pages first.
+    ``panels`` (DESIGN.md 7b, "Reversed panels"): None, or "auto" for a page with reversed text (light on a dark fill: banners,
+    shaded table headers, sidebars, buttons): the pieces of the page (leaves of the unit-gap XY-cut) whose shorter side is at
+    least ``panel_size`` (an integer in [2, 32767]; default the text size, a heuristic), over half ink and filled flat (more
+    than half of their greys within 8 of the modal grey) are panels.  A panel's inside is cut as text of the opposite
+    polarity inside a rule outline, and its blocks are TextBlocks of that polarity, restored line by line.  A panel is never a
+    figure.  With ``rules``, a fill whose rows or columns are at least ``rule_length`` long is rules, not a panel: give a
+    ``rule_length`` above the panels' sides.  Not with skew or curve: flatten such a page with flatten_pages first."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
@@ -2112,6 +2119,8 @@ class TextPage(NamedTuple):
     figures: object = None
     figure_size: object = None
     block_direction: object = None
+    panels: object = None
+    panel_size: object = None
 
 
 def _check_page(pg, H, W, name):
@@ -2146,6 +2155,17 @@ def _check_page(pg, H, W, name):
         if pg.block_direction is not None and getattr(pg, what) is not None:
             raise ValueError(f"{name}: block_direction and {what} are both given (a page whose blocks' directions are found is "
                              f"level and flat: flatten a tilted or curled page with flatten_pages first)")
+    if pg.panels is not None and not (isinstance(pg.panels, str) and pg.panels == "auto"):
+        raise ValueError(f"{name}: panels must be None or 'auto', got {pg.panels!r}")
+    v = pg.panel_size
+    if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 2 <= v <= 32767):
+        raise ValueError(f"{name}: panel_size must be an integer in [2, 32767], got {v!r}")
+    if v is not None and pg.panels is None:
+        raise ValueError(f"{name}: panel_size is given, but panels is None, not 'auto'")
+    for what in ("skew", "curve"):
+        if pg.panels is not None and getattr(pg, what) is not None:
+            raise ValueError(f"{name}: panels and {what} are both given (a page with panels is level and flat: flatten a "
+                             f"tilted or curled page with flatten_pages first)")
     if pg.quad is not None:
         if pg.rect is not None:
             raise ValueError(f"{name}: rect and quad are both given (a page in perspective is its quad: give rect=None)")
@@ -2185,8 +2205,8 @@ def _page_table(pg):
 
 def _page_bytes(pg, rect, skewed):
     """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages, with a ruled page's two extra
-    bitmaps and a figure page's bitmap and table: a quad page's rectified crop and its page, or an auto page's corner search on
-    the image ``rect``."""
+    bitmaps, a figure page's bitmap and table and a panel page's table (and outline bitmap without rules): a quad page's
+    rectified crop and its page, or an auto page's corner search on the image ``rect``."""
     from . import ops
     w, h = rect[2] - rect[0], rect[3] - rect[1]
     if isinstance(pg.quad, str):
@@ -2196,6 +2216,7 @@ def _page_bytes(pg, rect, skewed):
         return 3 * w_r * h_r + _page_bytes(pg._replace(quad=None), (0, 0, w_r, h_r), skewed)
     rules = ops.rule_page_bytes(w, h) if pg.rules is not None else 0
     rules += ops.figure_page_bytes(w, h) if pg.figures is not None else 0
+    rules += ops.panel_page_bytes(w, h, pg.rules is not None) if pg.panels is not None else 0
     if not skewed:
         return ops.page_bytes(w, h) + rules
     return rules + ops.skew_page_bytes(w, h, pg.direction == "vertical",
@@ -2255,7 +2276,8 @@ def _find_blocks(dimg, items, rq=None):
     """ops.find_blocks over items (image index, TextPage, rect) of the uploaded images ``dimg``, its tables back through one
     pinned copy and one synchronisation; a quad page (its corners given) is a level page on all of its rectified crop in ``rq``
     (_rectify).  Returns per item dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, rule_length, rule_pixels]
-    [, figure_size, figures][, block_direction, undecided]), or the error message of a page over a limit."""
+    [, figure_size, figures][, block_direction, undecided][, panel_size, panels]), or the error message of a page over a
+    limit."""
     from . import ops
     lib = ops._lib
 
@@ -2270,9 +2292,10 @@ def _find_blocks(dimg, items, rq=None):
         return None if pg.rules is None else pg.rule_length or ops.rule_length(x1 - x0, y1 - y0)
     rls = [rule_length(*it) for it in items]
     fss = [None if pg.figures is None else pg.figure_size or 0 for _, pg, _ in items]
+    pss = [None if pg.panels is None else pg.panel_size or 0 for _, pg, _ in items]
     res_t, caps = ops.find_blocks([(*src(i, pg, rect), pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y,
-                                    pg.skew, pg.max_skew, rl, fs, pg.block_direction is not None)
-                                   for (i, pg, rect), rl, fs in zip(items, rls, fss)])
+                                    pg.skew, pg.max_skew, rl, fs, pg.block_direction is not None, ps)
+                                   for (i, pg, rect), rl, fs, ps in zip(items, rls, fss, pss)])
     host = _to_host(res_t).numpy()
     rdt, ndt, sdt = ops.page_result_dtype(), ops.page_node_dtype(), ops.skew_block_dtype()
     skewed = any(pg.skew is not None for _, pg, _ in items)
@@ -2281,12 +2304,16 @@ def _find_blocks(dimg, items, rq=None):
     res = host[o:o + len(items) * rdt.itemsize].view(rdt)
     o, out = o + len(items) * rdt.itemsize, []
     ft = o + sum(caps) * ndt.itemsize                   # the figure pages' tables, after every leaf table
-    for (i, pg, rect), r, cap, sk, rl, fs in zip(items, res, caps, skew, rls, fss):
+    pt = ft + lib.PAGE_MAX_FIGURES * ndt.itemsize * sum(fs is not None for fs in fss)   # then the panel pages' tables
+    for (i, pg, rect), r, cap, sk, rl, fs, ps in zip(items, res, caps, skew, rls, fss, pss):
         leaves = host[o:o + cap * ndt.itemsize].view(ndt)[:int(r["n_leaves"])]
         o += cap * ndt.itemsize
         if fs is not None:
             figs = host[ft:ft + lib.PAGE_MAX_FIGURES * ndt.itemsize].view(ndt)[:int(r["n_figures"])]
             ft += lib.PAGE_MAX_FIGURES * ndt.itemsize
+        if ps is not None:
+            pans = host[pt:pt + lib.PAGE_MAX_PANELS * ndt.itemsize].view(ndt)[:int(r["n_panels"])]
+            pt += lib.PAGE_MAX_PANELS * ndt.itemsize
         if r["error"] == lib.PAGE_ERR_NODES:
             out.append(f"more than {lib.PAGE_MAX_NODES} nodes in one level of the XY-cut")
             continue
@@ -2296,10 +2323,18 @@ def _find_blocks(dimg, items, rq=None):
         if r["error"] == lib.PAGE_ERR_FIGURES:
             out.append(f"{int(r['n_figures'])} figures exceed the {lib.PAGE_MAX_FIGURES} a text page may hold")
             continue
+        if r["error"] == lib.PAGE_ERR_PANELS:
+            out.append(f"{int(r['n_panels'])} panels exceed the {lib.PAGE_MAX_PANELS} a text page may hold")
+            continue
         X0, Y0 = (0, 0) if pg.quad is not None else rect[:2]
         vertical = pg.direction == "vertical"
         tilted = pg.skew is not None and sk["s"] != 0
-        blocks, rejected, dirs, undecided = [], [], [], []
+        ink = "dark" if r["ink"] == lib.INK_DARK else "light"
+        # A block grown inside a panel's outline is a panel block, of the opposite polarity: growth stops at the outline, so
+        # a grown block lies inside a panel exactly when its leaf does.
+        boxes = [] if ps is None else [tuple(int(q[f]) for f in ("x0", "y0", "x1", "y1")) for q in pans]
+        opposite = "light" if ink == "dark" else "dark"
+        blocks, rejected, dirs, undecided, pols = [], [], [], [], []
         for q in leaves:
             x0, y0, x1, y1 = (int(q[f]) for f in ("x0", "y0", "x1", "y1"))
             if not tilted:
@@ -2315,9 +2350,11 @@ def _find_blocks(dimg, items, rq=None):
                 dirs.append("vertical" if q["st"] & lib.PAGE_VERTICAL else "horizontal")
                 if q["st"] & lib.PAGE_UNDECIDED:
                     undecided.append(len(blocks))
+            inside = any(a <= x0 and b <= y0 and x1 <= c and y1 <= e for a, b, c, e in boxes)
+            pols.append(opposite if inside else pg.polarity)
             blocks.append(box)
-        res = dict(threshold=int(r["threshold"]), ink="dark" if r["ink"] == lib.INK_DARK else "light",
-                   text_size=int(r["text_size"]), gap_x=int(r["gap_x"]), gap_y=int(r["gap_y"]))
+        res = dict(threshold=int(r["threshold"]), ink=ink, text_size=int(r["text_size"]), gap_x=int(r["gap_x"]),
+                   gap_y=int(r["gap_y"]))
         if rl is not None:
             res.update(rule_length=rl, rule_pixels=int(r["rule_pixels"]))
         if fs is not None:                              # in image coordinates, or rectangles of R on a quad page
@@ -2325,13 +2362,15 @@ def _find_blocks(dimg, items, rq=None):
                        figures=[(X0 + int(q["x0"]), Y0 + int(q["y0"]), X0 + int(q["x1"]), Y0 + int(q["y1"])) for q in figs])
         if pg.block_direction is not None:
             res.update(block_direction=pg.block_direction, undecided=undecided)
+        if ps is not None:                              # in image coordinates, or rectangles of R on a quad page
+            res.update(panel_size=int(r["panel_size"]), panels=[(X0 + a, Y0 + b, X0 + c, Y0 + e) for a, b, c, e in boxes])
         if pg.quad is not None:
             shape = dimg[i].shape[:2]
-            res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=d, polarity=pg.polarity, window=b)
-                               for b, d in zip(blocks, dirs)],
+            res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=d, polarity=pl, window=b)
+                               for b, d, pl in zip(blocks, dirs, pols)],
                        rejected=rejected, quad=_quad_key(i, pg.quad)[1], size=tuple(src(i, pg, rect)[1][2:]))
         elif pg.skew is None:
-            res.update(blocks=[TextBlock(b, d, polarity=pg.polarity, curve=pg.curve) for b, d in zip(blocks, dirs)],
+            res.update(blocks=[TextBlock(b, d, polarity=pl, curve=pg.curve) for b, d, pl in zip(blocks, dirs, pols)],
                        rejected=rejected)
         else:
             res["skew"] = _skew_used(pg, sk)
@@ -2377,7 +2416,15 @@ def find_blocks(images, pages):
     of its blocks then has its own direction tested on the device from the row and column bands of its ink (1 more launch for
     all such pages of the call, and no more memory): its TextBlocks (or from_quad windows) are "horizontal" or "vertical",
     each restored as such.  Its dict gains ``block_direction`` ("auto") and ``undecided``, the indices of the blocks whose test
-    was undecided and which took the page's direction."""
+    was undecided and which took the page's direction.
+    A page with ``panels="auto"`` (DESIGN.md 7b, "Reversed panels") has its panels, the leaves of the unit-gap XY-cut of
+    shorter side at least its panel size p that are over half ink and flat-filled, tested on the device (2 more launches for
+    all such pages of the call); inside each, the ink is the page's paper less the panel's 1-pixel outline, which stops the
+    cut and the growth as a rule.  The blocks inside a panel are TextBlocks (or from_quad windows) of the polarity opposite
+    to the page's ink; the others keep the page's.  Its dict gains ``panel_size`` (the p used, 0 without a text size) and
+    ``panels``, their rectangles in leaf order (as ``figures``).  A page over 1024 panels raises, as one over its figure
+    limit.  With ``rules="auto"`` the rules are taken out of the ink first, so a fill whose rows or columns reach the rule
+    length is no panel: give a ``rule_length`` above the panels' sides."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
@@ -2972,7 +3019,7 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     replaced by its lines as above, so the result is byte for byte that of the call given the found blocks.  No labels or boxes
     may be given for a page; a tilted page (``skew``) gives windowed TextBlocks, which are split as any other.  Its entry is
     dict(blocks, rejected, threshold, ink, text_size, gap_x, gap_y[, skew][, figure_size, figures][, block_direction,
-    undecided], regions), regions one
+    undecided][, panel_size, panels], regions), regions one
     block entry per block; a page over its node or block limit, or one of whose blocks fails, raises, or is dict(error=...)
     with ``skip_invalid``, and then none of its blocks is restored.  A quad page or block (DESIGN.md 7b, "Perspective pages")
     is laid out on its rectified crop (TextPage(quad="auto") after the device's corner search), every distinct quad of the call
