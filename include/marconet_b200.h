@@ -799,16 +799,18 @@ int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* c
  * cap <= min(MN_PAGE_MAX_NODES, (h + 1) (w + 1) / 4).  The state fields are zero on entry.  blocks, pages: DEVICE arrays
  * (validated by the caller: 1 <= w, h <= 32767, the crop inside its image).
  * Ruled pages (DESIGN.md section 7b, "Ruled pages"): a page with rbits (inside work) has rule pixels U, the ink pixels in a
- * maximal row or column run of at least rule_length.  A call with ruled != 0 issues 3 more launches after the bitmap, whatever
- * the number of pages: the bitmap transposed into rbits' scratch, the long runs of every row of both planes, and the column
- * runs transposed back into rbits, U cleared from bits and |U| counted into res->rule_pixels.  In such a page's XY-cut an index
- * whose U count is at least half the node's extent is white, and a white run holding one cuts whatever its length; a block
- * grows by q on each side only up to the nearest row (column) of its margin with U in its columns (rows).  Pages without
- * rbits take the path of a call with ruled = 0, and a call with ruled = 0 issues exactly the launches above.
- * Figures (DESIGN.md section 7b, "Figures"): `ruled` is a flags word, MN_PAGE_RULES | MN_PAGE_FIGURES (0 and 1 keep their
- * meaning).  A page with fbits (inside work) has figures: at 7, its pass-1 leaves whose shorter side is at least f go, in leaf
- * order, into figs (MN_PAGE_MAX_FIGURES entries; st = the rows of the figures before it), with f = figure_size, or 3 S when
- * figure_size is 0; res->figure_size = f and res->n_figures = their number, or res->error = MN_PAGE_ERR_FIGURES over the limit.
+ * maximal row or column run of at least rule_length.  flags holds MN_PAGE_RULES, MN_PAGE_FIGURES, MN_PAGE_DIRECTIONS and
+ * MN_PAGE_PANELS for the options below that some page of the call has.  A call with MN_PAGE_RULES issues 3 more launches
+ * after the bitmap, whatever the number of pages: the bitmap transposed into rbits' scratch, the long runs of every row of
+ * both planes, and the column runs transposed back into rbits, U cleared from bits and |U| counted into res->rule_pixels.
+ * In such a page's XY-cut an index whose U count is at least half the node's extent is white, and a white run holding one
+ * cuts whatever its length; a block grows by q on each side only up to the nearest row (column) of its margin with U in its
+ * columns (rows).  Pages without rbits take the path of a call without MN_PAGE_RULES, and a call without it issues exactly
+ * the launches above.
+ * Figures (DESIGN.md section 7b, "Figures"): a page with fbits (inside work) has figures: at 7, its pass-1 leaves whose
+ * shorter side is at least f go, in leaf order, into figs (MN_PAGE_MAX_FIGURES entries; st = the rows of the figures before
+ * it), with f = figure_size, or 3 S when figure_size is 0; res->figure_size = f and res->n_figures = their number, or
+ * res->error = MN_PAGE_ERR_FIGURES over the limit.
  * A call with MN_PAGE_FIGURES issues 1 more launch after 7, whatever the number of pages: each figure row of every figure page
  * painted into fbits (F, the union of the figure rectangles) and cleared from bits, so that pass 2 and the leaf rules see
  * I'' = I' and not F.  F takes no part in the rule-index cut; a block's growth stops at U or F as it does at U alone.  The rule
@@ -885,7 +887,7 @@ typedef struct {
     int32_t prows;              /* state: the rows of all of its panels */
     int32_t pdone, pad3;        /* state: the panel test's CTAs done with the page */
 } mn_text_page;
-int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, int ruled, void* work,
+int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, long long max_tiles, int flags, void* work,
                       long long work_bytes, void* stream);
 
 /* Skewed pages (DESIGN.md section 7b, "Skewed pages").  Page i is searched as a skewed block on skew[i] (skew[i].b, blocks[i] and
@@ -902,7 +904,7 @@ int mn_find_blocks_u8(const mn_text_block* blocks, mn_text_page* pages, int n, l
  *         mn_find_blocks_u8's).
  * bits holds max L x wpitch words, wpitch >= max M / 32, and cap entries per list, max over the page's table; the angle
  * profiles and scores are as mn_find_lines_skewed_u8's (b.prof unused).  work (work_bytes) is zeroed by the call. */
-int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles, int ruled,
+int mn_find_blocks_skewed_u8(mn_text_block* blocks, mn_skew_block* skew, mn_text_page* pages, int n, long long max_tiles, int flags,
                              void* work, long long work_bytes, void* stream);
 
 /* Windowed blocks (DESIGN.md section 7b, "Skewed pages").  Block i is the set of pixels of the crop wins[i].b whose frame cell

@@ -2078,18 +2078,26 @@ def find_lines_curved(blocks, tables=False):
 PAGE_MAX_WORK = 1 << 30        # bytes of device memory one find_blocks call may use
 
 
+class PageItem(NamedTuple):
+    """One page of a find_blocks call (its docstring gives the fields' meaning)."""
+    img: object
+    rect: object
+    vertical: bool
+    polarity: int
+    gap_x: object = None
+    gap_y: object = None
+    skew: object = None
+    max_skew: float = 10.0
+    rule_length: object = None
+    figure_size: object = None
+    directions: bool = False
+    panel_size: object = None
+
+
 def page_cap(w, h):
     """Nodes one level of a w x h page may hold: disjoint rectangles with ink, pairwise apart by a white pixel, so at most
     (h + 1) (w + 1) / 4, and at most the node limit."""
     return min(_lib.PAGE_MAX_NODES, (h + 1) * (w + 1) // 4)
-
-
-def page_bytes(w, h):
-    """Device bytes of one w x h page in find_blocks: records, result, leaves, histogram, threshold record, ink bitmap, two
-    level lists and three per-node counts."""
-    cap = page_cap(w, h)
-    return (ctypes.sizeof(_lib.PageResult) + ctypes.sizeof(_lib.TextBlock) + ctypes.sizeof(_lib.TextPage) + 3 * 12 * cap + 4 * 256
-            + ctypes.sizeof(_lib.BlockLines) + 4 * h * -(-w // 32) + 3 * 4 * cap + 64)
 
 
 def rule_length(w, h):
@@ -2098,158 +2106,168 @@ def rule_length(w, h):
     return max(32, min(w, h) // 16)
 
 
-def rule_page_bytes(w, h):
-    """Device bytes a w x h page adds to find_blocks when it has rules (DESIGN.md 7b, "Ruled pages"): its U bitmap (h rows of
-    ceil(w / 32) words) and the transposed bitmap's scratch (w rows of ceil(h / 32) words)."""
-    return 4 * (h * -(-w // 32) + w * -(-h // 32))
-
-
-def figure_page_bytes(w, h):
-    """Device bytes a w x h page adds to find_blocks when it has figures (DESIGN.md 7b, "Figures"): its F bitmap (h rows of
-    ceil(w / 32) words) and its figure table of PAGE_MAX_FIGURES page nodes."""
-    return 4 * h * -(-w // 32) + 12 * _lib.PAGE_MAX_FIGURES
-
-
-def panel_page_bytes(w, h, ruled):
-    """Device bytes a w x h page adds to find_blocks when it has panels (DESIGN.md 7b, "Reversed panels"): the plane of U that
-    takes the panels' outlines (h rows of ceil(w / 32) words) unless the page is ``ruled`` and has one, and its panel table of
-    PAGE_MAX_PANELS page nodes."""
-    return (0 if ruled else 4 * h * -(-w // 32)) + 12 * _lib.PAGE_MAX_PANELS
-
-
 def skew_page_frame(w, h, vertical, cs):
     """(L, M, stride) of a w x h page's frame bitmaps over the (c, s) of ``cs``: the most rows and columns a bitmap may have (the
-    search frame's axes swapped for a vertical page) and the most bins of its search frames."""
+    search frame's axes swapped for a vertical page) and the most bins of its search frames.  The one-entry table (1, 0) gives
+    the crop's own (h, w) and its bins."""
+    if cs == [(1.0, 0.0)]:
+        return h, w, w if vertical else h
     _, _, L, M = skew_frames(w, h, vertical, cs)
     return (int(M.max()), int(L.max()), int(L.max())) if vertical else (int(L.max()), int(M.max()), int(L.max()))
 
 
+def _page_areas(L, M, cap, n_ang, stride, rules, figures, panels):
+    """Byte sizes of one page's work areas in find_blocks, in their order: the per-angle scores of a search (n_ang > 1), the
+    histogram, the threshold record, the ink bitmap (L rows of ceil(M / 32) words), two level lists and three per-node counts
+    of cap nodes, the angle profiles of a search, a ruled page's U plane (as the ink bitmap) and the transposed bitmap's
+    scratch (M rows of ceil(L / 32) words), a figure page's F plane, and a panel page's U plane when it has no rules (the
+    panels' outlines join the rules' plane when it has)."""
+    plane, search = 4 * L * -(-M // 32), n_ang > 1
+    return [8 * n_ang if search else 0, 4 * 256, ctypes.sizeof(_lib.BlockLines), plane, 2 * 12 * cap, 3 * 4 * cap,
+            4 * n_ang * stride if search else 0, plane + 4 * M * -(-L // 32) if rules else 0, plane if figures else 0,
+            plane if panels and not rules else 0]
+
+
+def page_bytes(w, h, vertical=False, cs=None, rules=False, figures=False, panels=False):
+    """Device bytes of one w x h page in find_blocks, with or without ``rules``, ``figures`` and ``panels``: its records,
+    result and leaf table, a figure page's table of PAGE_MAX_FIGURES and a panel page's table of PAGE_MAX_PANELS page nodes,
+    its work areas and 64 bytes for the call's 16-byte alignments.  ``cs``: None in a call without skewed pages, else the
+    (c, s) table the page searches ([(1.0, 0.0)] for a page with skew None), which adds the search record, the table and 16
+    bytes for its alignment; the page's bitmaps are then those of its largest frame."""
+    n_ang = len(cs) if cs else 1
+    L, M, stride = skew_page_frame(w, h, vertical, cs or [(1.0, 0.0)])
+    cap = page_cap(M, L)
+    tables = 12 * (cap + (_lib.PAGE_MAX_FIGURES if figures else 0) + (_lib.PAGE_MAX_PANELS if panels else 0))
+    search = ctypes.sizeof(_lib.SkewBlock) + 16 * n_ang + 16 if cs else 0
+    return (ctypes.sizeof(_lib.PageResult) + ctypes.sizeof(_lib.TextBlock) + ctypes.sizeof(_lib.TextPage) + tables + search
+            + sum(_page_areas(L, M, cap, n_ang, stride, rules, figures, panels)) + 64)
+
+
+def rule_page_bytes(w, h):
+    """Device bytes a w x h page adds to find_blocks when it has rules (page_bytes): its U plane and the transposed bitmap's
+    scratch."""
+    return page_bytes(w, h, rules=True) - page_bytes(w, h)
+
+
+def figure_page_bytes(w, h):
+    """Device bytes a w x h page adds to find_blocks when it has figures (page_bytes): its F plane and figure table."""
+    return page_bytes(w, h, figures=True) - page_bytes(w, h)
+
+
+def panel_page_bytes(w, h, ruled):
+    """Device bytes a w x h page adds to find_blocks when it has panels (page_bytes): its panel table, and the plane of U
+    that takes the panels' outlines unless the page is ``ruled`` and has one."""
+    return page_bytes(w, h, rules=ruled, panels=True) - page_bytes(w, h, rules=ruled)
+
+
 def skew_page_bytes(w, h, vertical, cs):
-    """Device bytes of one w x h page searched over ``cs`` in find_blocks: page_bytes of its largest frame, the search record
-    and table, and the per-angle scores and profiles of a search over more than one angle."""
-    L, M, stride = skew_page_frame(w, h, vertical, cs)
-    n = len(cs)
-    return page_bytes(M, L) + ctypes.sizeof(_lib.SkewBlock) + 16 * n + (8 * n + 4 * n * stride if n > 1 else 0) + 16
+    """Device bytes of one w x h page searched over ``cs`` in a find_blocks call with skewed pages (page_bytes)."""
+    return page_bytes(w, h, vertical, cs)
+
+
+def _check_page_options(page, what):
+    """Refuses, naming ``what``, a PageItem's rule_length, figure_size or panel_size that is not None or an integer in
+    [2, 32767] (figure_size and panel_size may be 0, their default) and its directions that is not None, False or True, or
+    any of them set on a page with skew.  They are checked in their field order."""
+    for knob, zero in (("rule_length", False), ("figure_size", True), ("directions", None), ("panel_size", True)):
+        v = getattr(page, knob)
+        if zero is None:                                # directions: a bool
+            bad, want = (v is not None and not isinstance(v, bool)) or (v and page.skew is not None), "None, False or True"
+        else:
+            bad = v is not None and (isinstance(v, bool) or not isinstance(v, int) or not (zero and v == 0 or 2 <= v <= 32767)
+                                     or page.skew is not None)
+            want = f"{'0 or ' if zero else ''}an integer in [2, 32767]"
+        if bad:
+            raise ValueError(f"{what}: {knob} {v!r} is not {want} on a page with skew None")
 
 
 def find_blocks(pages, scores=False):
     """Text pages split into blocks by a recursive XY-cut (mn_find_blocks_u8; DESIGN.md 7b, "Text pages"), every page of the call
-    in 5 + 6 * 24 launches whatever the number of pages and nodes.  pages: list of (img, rect, vertical, polarity, gap_x, gap_y):
-    img a uint8 [H, W, 3] CUDA view with dense pixels (any row stride) read in place, rect (x0, y0, x1, y1) a non-empty crop
-    inside it with sides <= 32767, vertical a bool, polarity _lib.INK_AUTO / INK_DARK / INK_LIGHT, gap_x and gap_y positive
-    integers or None for the default.  Returns (out, caps): out the uint8 CUDA tensor of the pages' mn_page_result records
-    followed by each page's leaf table of caps[i] mn_page_node entries (read them back as ``page_result_dtype()`` and
-    ``page_node_dtype()``).
+    in 5 + 6 * 24 launches whatever the number of pages and nodes.  pages: list of PageItem records, or of tuples of their
+    leading fields in order.  img: a uint8 [H, W, 3] CUDA view with dense pixels (any row stride) read in place.  rect:
+    (x0, y0, x1, y1), a non-empty crop inside it with sides <= 32767.  vertical: a bool.  polarity: _lib.INK_AUTO / INK_DARK /
+    INK_LIGHT.  gap_x, gap_y: positive integers, or None for the default.  Returns (out, caps): out the uint8 CUDA tensor of the pages' mn_page_result records followed by each
+    page's leaf table of caps[i] mn_page_node entries; page_tables reads its host copy back.
     skew, max_skew (DESIGN.md 7b, "Skewed pages"): as find_lines'.  A call with any skewed page goes through
     mn_find_blocks_skewed_u8's 7 + 6 * 24 launches instead, every page of it; pages with skew None search the one-entry table
-    (1, 0) and keep their tables exactly.  out then starts with the n mn_skew_block records (``skew_block_dtype()``: the chosen
-    index and frame) and the leaves are in frame cells.  ``scores`` (tests): also return, per page, the int64 CUDA view of its
-    per-angle scores (None unless it searched).
-    rule_length (DESIGN.md 7b, "Ruled pages"), a ninth entry after skew and max_skew: None, or an integer in [2, 32767] on a
-    page with skew None, whose ink pixels in a maximal row or column run of at least that many pixels are its rules U.  A call
-    with such a page issues 3 more launches whatever the number of pages; its records gain rule_pixels (|U|), and the other
-    pages' tables are those of a call without it.
-    figure_size (DESIGN.md 7b, "Figures"), a tenth entry: None, or on a page with skew None 0 (the figure size 3 S) or an
-    integer f in [2, 32767]: its pass-1 leaves whose shorter side is at least f are its figures, taken out of its ink before
-    pass 2.  A call with such a page issues 1 more launch whatever the number of pages; its records gain figure_size and
-    n_figures, and out ends with each such page's table of _lib.PAGE_MAX_FIGURES mn_page_node figures, in the order of the
-    pages.  The other pages' tables are those of a call without it.
-    directions (DESIGN.md 7b, "Mixed directions"), an eleventh entry: None or False, or True on a page with skew None: each of
-    its kept leaves has its own direction tested, _lib.PAGE_VERTICAL set in its st when it is vertical and
-    _lib.PAGE_UNDECIDED when the test is undecided (it then takes the page's direction).  A call with such a page issues 1
-    more launch whatever the number of pages and needs no more memory; the other pages' tables are those of a call without
-    it.
-    panel_size (DESIGN.md 7b, "Reversed panels"), a twelfth entry: None, or on a page with skew None 0 (the panel size S) or
-    an integer p in [2, 32767]: its pass-1 leaves of shorter side at least p that are over half ink and flat-filled are its
-    panels, whose insides are cut as ink of the other polarity inside a rule outline (with rule_length, after the rules U
-    have left the ink: a fill with runs of at least rule_length is no panel).  A call with such a page issues 2 more
-    launches whatever the number of pages; its records gain panel_size and n_panels, and out ends, after the figure tables,
-    with each such page's table of _lib.PAGE_MAX_PANELS mn_page_node panels, in the order of the pages.  The other pages'
-    tables are those of a call without it."""
+    (1, 0) and keep their tables exactly.  out then starts with the n mn_skew_block records (the chosen index and frame) and
+    the leaves are in frame cells.  ``scores`` (tests): also return, per page, the int64 CUDA view of its per-angle scores
+    (None unless it searched).
+    rule_length (DESIGN.md 7b, "Ruled pages"): None, or an integer in [2, 32767] on a page with skew None, whose ink pixels in
+    a maximal row or column run of at least that many pixels are its rules U.  A call with such a page issues 3 more launches
+    whatever the number of pages; its records gain rule_pixels (|U|).
+    figure_size (DESIGN.md 7b, "Figures"): None, or on a page with skew None 0 (the figure size 3 S) or an integer f in
+    [2, 32767]: its pass-1 leaves whose shorter side is at least f are its figures, taken out of its ink before pass 2.  A call
+    with such a page issues 1 more launch whatever the number of pages; its records gain figure_size and n_figures, and out
+    ends with each such page's table of _lib.PAGE_MAX_FIGURES mn_page_node figures, in the order of the pages.
+    directions (DESIGN.md 7b, "Mixed directions"): False (or None), or True on a page with skew None: each of its kept leaves
+    has its own direction tested, _lib.PAGE_VERTICAL set in its st when it is vertical and _lib.PAGE_UNDECIDED when the test is
+    undecided (it then takes the page's direction).  A call with such a page issues 1 more launch whatever the number of
+    pages and needs no more memory.
+    panel_size (DESIGN.md 7b, "Reversed panels"): None, or on a page with skew None 0 (the panel size S) or an integer p in
+    [2, 32767]: its pass-1 leaves of shorter side at least p that are over half ink and flat-filled are its panels, whose
+    insides are cut as ink of the other polarity inside a rule outline (with rule_length, after the rules U have left the
+    ink: a fill with runs of at least rule_length is no panel).  A call with such a page issues 2 more launches whatever the
+    number of pages; its records gain panel_size and n_panels, and out ends, after the figure tables, with each such page's
+    table of _lib.PAGE_MAX_PANELS mn_page_node panels, in the order of the pages.
+    A page without one of these options gets the tables of a call without it."""
     global LAUNCHES
     dev = _check_items(pages, "find_blocks", "page")
-    skewed = any(len(p) > 6 and p[6] is not None for p in pages)
-    rules = [p[8] if len(p) > 8 else None for p in pages]
-    figs = [p[9] if len(p) > 9 else None for p in pages]
-    dirs = [p[10] if len(p) > 10 else None for p in pages]
-    pans = [p[11] if len(p) > 11 else None for p in pages]
+    pages = [PageItem(*p) for p in pages]
+    skewed = any(p.skew is not None for p in pages)
     n = len(pages)
-    rsz, bsz, psz, lsz = (ctypes.sizeof(t) for t in (_lib.PageResult, _lib.TextBlock, _lib.TextPage, _lib.BlockLines))
+    rsz, bsz, psz = (ctypes.sizeof(t) for t in (_lib.PageResult, _lib.TextBlock, _lib.TextPage))
     ssz = ctypes.sizeof(_lib.SkewBlock) if skewed else 0
-    dims, tables, need = [], [], 0
-    for i, pg in enumerate(pages):
+    dims, tables, areas, need = [], [], [], 0
+    for i, p in enumerate(pages):
         what = f"find_blocks: page {i}"
-        x0, y0, bw, bh = _check_crop(pg[:6], dev, what, "gap_x / gap_y")
-        vertical, skew, max_skew = pg[2], pg[6] if len(pg) > 6 else None, pg[7] if len(pg) > 7 else 10.0
-        cs = _check_skew(skew, max_skew, vertical, what)
-        rl = rules[i]
-        if rl is not None and (isinstance(rl, bool) or not isinstance(rl, int) or not 2 <= rl <= 32767 or skew is not None):
-            raise ValueError(f"{what}: rule_length {rl!r} is not an integer in [2, 32767] on a page with skew None")
-        fs = figs[i]
-        if fs is not None and (isinstance(fs, bool) or not isinstance(fs, int) or not (fs == 0 or 2 <= fs <= 32767)
-                               or skew is not None):
-            raise ValueError(f"{what}: figure_size {fs!r} is not 0 or an integer in [2, 32767] on a page with skew None")
-        if (dirs[i] is not None and not isinstance(dirs[i], bool)) or (dirs[i] and skew is not None):
-            raise ValueError(f"{what}: directions {dirs[i]!r} is not None, False or True on a page with skew None")
-        ps = pans[i]
-        if ps is not None and (isinstance(ps, bool) or not isinstance(ps, int) or not (ps == 0 or 2 <= ps <= 32767)
-                               or skew is not None):
-            raise ValueError(f"{what}: panel_size {ps!r} is not 0 or an integer in [2, 32767] on a page with skew None")
-        L, M, stride = (bh, bw, bw if vertical else bh) if skew is None else skew_page_frame(bw, bh, vertical, cs)
-        need += skew_page_bytes(bw, bh, vertical, cs) if skewed else page_bytes(bw, bh)
-        need += rule_page_bytes(bw, bh) if rl is not None else 0
-        need += figure_page_bytes(bw, bh) if fs is not None else 0
-        need += panel_page_bytes(bw, bh, rl is not None) if ps is not None else 0
+        x0, y0, bw, bh = _check_crop(p[:6], dev, what, "gap_x / gap_y")
+        cs = _check_skew(p.skew, p.max_skew, p.vertical, what)
+        _check_page_options(p, what)
+        opts = (p.rule_length is not None, p.figure_size is not None, p.panel_size is not None)   # rules, figures, panels
+        L, M, stride = skew_page_frame(bw, bh, p.vertical, cs)
+        need += page_bytes(bw, bh, p.vertical, cs if skewed else None, *opts)
         if max(L, M) > 32767:
             raise ValueError(f"{what}: a frame side of {max(L, M)} exceeds 32767")
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
             raise ValueError(f"{what}: {len(cs)} angles x {stride} bins exceed the {SKEW_MAX_PROFILE} profile values a skewed "
                              f"page may use")
+        cap = page_cap(M, L)
         tables.append(cs)
-        dims.append((x0, y0, bw, bh, page_cap(M, L), L, M, len(cs), stride))
+        dims.append((x0, y0, bw, bh, cap, M, len(cs), stride, opts))
+        areas.append(_page_areas(L, M, cap, len(cs), stride, *opts))
     if need > PAGE_MAX_WORK:
         raise ValueError(f"find_blocks: the pages need more than the {PAGE_MAX_WORK} bytes of work memory a call may use")
     tab, t_offs = _angle_tables(tables) if skewed else (b"", [0] * n)
     pg0, tab0 = n * bsz, n * (bsz + psz)                 # records, tables and the skew records, then the results and leaves,
     out0 = -(-(tab0 + len(tab) + n * ssz) // 16) * 16    # then the work: the call zeroes everything from out0 on, and the
     sk0 = out0 - n * ssz                                 # skew records come back with the results in one copy
-    n_leaves = n * rsz + 12 * sum(d[4] for d in dims)
-    n_figs = n_leaves + 12 * _lib.PAGE_MAX_FIGURES * sum(fs is not None for fs in figs)
-    n_out = n_figs + 12 * _lib.PAGE_MAX_PANELS * sum(ps is not None for ps in pans)
+    n_figs = sum(p.figure_size is not None for p in pages)
+    n_pans = sum(p.panel_size is not None for p in pages)
+    n_out = n * rsz + 12 * (sum(d[4] for d in dims) + _lib.PAGE_MAX_FIGURES * n_figs + _lib.PAGE_MAX_PANELS * n_pans)
     work0 = out0 + -(-n_out // 16) * 16
-    per = [-(-(8 * (d[7] if d[7] > 1 else 0) + 4 * 256 + lsz + 4 * d[5] * -(-d[6] // 32) + 2 * 12 * d[4] + 3 * 4 * d[4]
-                + 4 * (d[7] * d[8] if d[7] > 1 else 0) + (rule_page_bytes(d[6], d[5]) if rl is not None else 0)
-                + (4 * d[5] * -(-d[6] // 32) if fs is not None else 0)
-                + (4 * d[5] * -(-d[6] // 32) if ps is not None and rl is None else 0)) // 16) * 16
-           for d, rl, fs, ps in zip(dims, rules, figs, pans)]
+    per = [-(-sum(a) // 16) * 16 for a in areas]
     buf = torch.empty(work0 + sum(per), dtype=torch.uint8, device=dev)
     base = buf.data_ptr()
     leaves, w, blocks, srecs, recs, views, tiles = base + out0 + n * rsz, base + work0, [], [], [], [], 0
-    ftab, ptab = base + out0 + n_leaves, base + out0 + n_figs
-    for i, (pg, d, nb, t) in enumerate(zip(pages, dims, per, t_offs)):
-        img, _, vertical, polarity, gap_x, gap_y = pg[:6]
-        x0, y0, bw, bh, cap, L, M, n_ang, stride = d
-        wp = -(-M // 32)
-        hist = w + 8 * (n_ang if n_ang > 1 else 0)       # after the page's per-angle scores
-        lines, bits = hist + 4 * 256, hist + 4 * 256 + lsz
-        lists = bits + 4 * L * wp
-        counts = lists + 2 * 12 * cap
-        rbits = counts + 3 * 4 * cap + 4 * (n_ang * stride if n_ang > 1 else 0)
-        fbits = rbits + (rule_page_bytes(M, L) if rules[i] is not None else 0)
-        pbits = fbits + (4 * L * wp if figs[i] is not None else 0)   # a panel page's U plane when it has no rules
-        ubits = rbits if rules[i] is not None else pbits if pans[i] is not None else None
-        tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, 0, 0, 0, 0, hist, 0, 0, lines)
+    ftab = leaves + 12 * sum(d[4] for d in dims)         # the figure pages' tables follow every leaf table,
+    ptab = ftab + 12 * _lib.PAGE_MAX_FIGURES * n_figs    # and the panel pages' tables follow those
+    for i, (p, (x0, y0, bw, bh, cap, M, n_ang, stride, (rules, figures, panels)), a, nb, t) in \
+            enumerate(zip(pages, dims, areas, per, t_offs)):
+        _, hist, lines, bits, lists, counts, prof, rbits, fbits, pbits = itertools.accumulate([w] + a[:-1])
+        tb = _lib.TextBlock(p.img.data_ptr(), p.img.stride(0), x0, y0, bw, bh, int(bool(p.vertical)), p.polarity, 0, 0, 0, 0, hist,
+                            0, 0, lines)
         blocks.append(tb)
         if skewed:
-            srecs.append(_skew_block(tb, base + tab0 + 16 * t, w, counts + 3 * 4 * cap, n_ang, stride))
+            srecs.append(_skew_block(tb, base + tab0 + 16 * t, w, prof, n_ang, stride))
         recs.append(_lib.TextPage(tb, bits, (ctypes.c_void_p * 2)(lists, lists + 12 * cap), leaves, counts, counts + 4 * cap,
-                                  counts + 8 * cap, base + out0 + i * rsz, wp, cap, gap_x or 0, gap_y or 0,
-                                  rbits=ubits, rule_length=rules[i] or 0,
-                                  fbits=fbits if figs[i] is not None else None, figs=ftab if figs[i] is not None else None,
-                                  figure_size=figs[i] or 0, dirs=int(bool(dirs[i])),
-                                  pans=ptab if pans[i] is not None else None, panel_size=pans[i] or 0))
-        ftab += 12 * _lib.PAGE_MAX_FIGURES if figs[i] is not None else 0
-        ptab += 12 * _lib.PAGE_MAX_PANELS if pans[i] is not None else 0
+                                  counts + 8 * cap, base + out0 + i * rsz, -(-M // 32), cap, p.gap_x or 0, p.gap_y or 0,
+                                  rbits=rbits if rules else pbits if panels else None, rule_length=p.rule_length or 0,
+                                  fbits=fbits if figures else None, figs=ftab if figures else None,
+                                  figure_size=p.figure_size or 0, dirs=int(bool(p.directions)),
+                                  pans=ptab if panels else None, panel_size=p.panel_size or 0))
+        ftab += 12 * _lib.PAGE_MAX_FIGURES if figures else 0
+        ptab += 12 * _lib.PAGE_MAX_PANELS if panels else 0
         views.append(buf[w - base:w - base + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         leaves += 12 * cap
         w += nb
@@ -2257,20 +2275,39 @@ def find_blocks(pages, scores=False):
     host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.TextPage * n)(*recs)) + tab
     host += bytes(sk0 - len(host)) + bytes((_lib.SkewBlock * len(srecs))(*srecs))
     buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
-    ruled, figured = any(rl is not None for rl in rules), any(fs is not None for fs in figs)
-    directed, paneled = any(bool(d) for d in dirs), any(ps is not None for ps in pans)
-    flags = (_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0) | (_lib.PAGE_DIRECTIONS if directed else 0)
-    flags |= _lib.PAGE_PANELS if paneled else 0
-    if skewed:
-        _lib.check(_lib.load().mn_find_blocks_skewed_u8(base, base + sk0, base + pg0, n, tiles, flags, base + out0,
-                                                        work0 + sum(per) - out0, _stream()), "mn_find_blocks_skewed_u8")
-        LAUNCHES += 7 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed + 2 * paneled
-    else:
-        _lib.check(_lib.load().mn_find_blocks_u8(base, base + pg0, n, tiles, flags, base + out0, work0 + sum(per) - out0,
-                                                 _stream()), "mn_find_blocks_u8")
-        LAUNCHES += 5 + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed + 2 * paneled
+    ruled, figured, directed, paneled = (any(p.rule_length is not None for p in pages), n_figs > 0,
+                                         any(p.directions for p in pages), n_pans > 0)
+    flags = ((_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0) | (_lib.PAGE_DIRECTIONS if directed else 0)
+             | (_lib.PAGE_PANELS if paneled else 0))
+    entry, head = ("mn_find_blocks_skewed_u8", (base, base + sk0)) if skewed else ("mn_find_blocks_u8", (base,))
+    _lib.check(getattr(_lib.load(), entry)(*head, base + pg0, n, tiles, flags, base + out0, len(buf) - out0, _stream()), entry)
+    LAUNCHES += (7 if skewed else 5) + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed + 2 * paneled
     res = buf[sk0:out0 + n_out], [d[4] for d in dims]
     return res + (views,) if scores else res
+
+
+def page_tables(host, pages, caps):
+    """Per page of a find_blocks call, numpy views of its tables in ``host``, the uint8 host copy of the call's out:
+    (skew, res, leaves, figures, panels).  skew is its mn_skew_block record (None in a call without skewed pages), res its
+    mn_page_result record, and leaves, figures and panels its mn_page_node entries, as many as res counts; figures is None
+    unless the page has a figure_size, panels None unless it has a panel_size."""
+    sdt, rdt, ndt = skew_block_dtype(), page_result_dtype(), page_node_dtype()
+    n = len(pages)
+    o = n * sdt.itemsize if any(p.skew is not None for p in pages) else 0
+    skews = host[:o].view(sdt) if o else [None] * n
+    res = host[o:o + n * rdt.itemsize].view(rdt)
+    nodes = host[o + n * rdt.itemsize:].view(ndt)       # every leaf table, then the figure pages' tables, then the panel pages'
+    f = sum(caps)
+    t = f + _lib.PAGE_MAX_FIGURES * sum(p.figure_size is not None for p in pages)
+    out = []
+    for p, sk, r, l0, cap in zip(pages, skews, res, itertools.accumulate(caps, initial=0), caps):
+        figs = pans = None
+        if p.figure_size is not None:
+            figs, f = nodes[f:f + _lib.PAGE_MAX_FIGURES][:int(r["n_figures"])], f + _lib.PAGE_MAX_FIGURES
+        if p.panel_size is not None:
+            pans, t = nodes[t:t + _lib.PAGE_MAX_PANELS][:int(r["n_panels"])], t + _lib.PAGE_MAX_PANELS
+        out.append((sk, r, nodes[l0:l0 + cap][:int(r["n_leaves"])], figs, pans))
+    return out
 
 
 def page_result_dtype():

@@ -2127,45 +2127,18 @@ def _check_page(pg, H, W, name):
     """The rectangle (x0, y0, x1, y1) of the TextPage ``pg`` of an H x W image, validated.  Raises ValueError naming ``name``."""
     from . import ops
     rect = (0, 0, W, H) if pg.rect is None else pg.rect
-    if pg.rules is not None and not (isinstance(pg.rules, str) and pg.rules == "auto"):
-        raise ValueError(f"{name}: rules must be None or 'auto', got {pg.rules!r}")
-    v = pg.rule_length
-    if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 2 <= v <= 32767):
-        raise ValueError(f"{name}: rule_length must be an integer in [2, 32767], got {v!r}")
-    if v is not None and pg.rules is None:
-        raise ValueError(f"{name}: rule_length is given, but rules is None, not 'auto'")
-    for what in ("skew", "curve"):
-        if pg.rules is not None and getattr(pg, what) is not None:
-            raise ValueError(f"{name}: rules and {what} are both given (a ruled page is level and flat: flatten a tilted or "
-                             f"curled page with flatten_pages first)")
-    if pg.figures is not None and not (isinstance(pg.figures, str) and pg.figures == "auto"):
-        raise ValueError(f"{name}: figures must be None or 'auto', got {pg.figures!r}")
-    v = pg.figure_size
-    if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 2 <= v <= 32767):
-        raise ValueError(f"{name}: figure_size must be an integer in [2, 32767], got {v!r}")
-    if v is not None and pg.figures is None:
-        raise ValueError(f"{name}: figure_size is given, but figures is None, not 'auto'")
-    for what in ("skew", "curve"):
-        if pg.figures is not None and getattr(pg, what) is not None:
-            raise ValueError(f"{name}: figures and {what} are both given (a page with figures is level and flat: flatten a "
-                             f"tilted or curled page with flatten_pages first)")
-    if pg.block_direction is not None and not (isinstance(pg.block_direction, str) and pg.block_direction == "auto"):
-        raise ValueError(f"{name}: block_direction must be None or 'auto', got {pg.block_direction!r}")
-    for what in ("skew", "curve"):
-        if pg.block_direction is not None and getattr(pg, what) is not None:
-            raise ValueError(f"{name}: block_direction and {what} are both given (a page whose blocks' directions are found is "
-                             f"level and flat: flatten a tilted or curled page with flatten_pages first)")
-    if pg.panels is not None and not (isinstance(pg.panels, str) and pg.panels == "auto"):
-        raise ValueError(f"{name}: panels must be None or 'auto', got {pg.panels!r}")
-    v = pg.panel_size
-    if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 2 <= v <= 32767):
-        raise ValueError(f"{name}: panel_size must be an integer in [2, 32767], got {v!r}")
-    if v is not None and pg.panels is None:
-        raise ValueError(f"{name}: panel_size is given, but panels is None, not 'auto'")
-    for what in ("skew", "curve"):
-        if pg.panels is not None and getattr(pg, what) is not None:
-            raise ValueError(f"{name}: panels and {what} are both given (a page with panels is level and flat: flatten a "
-                             f"tilted or curled page with flatten_pages first)")
+    for switch, knob in (("rules", "rule_length"), ("figures", "figure_size"), ("block_direction", None), ("panels", "panel_size")):
+        on, v = getattr(pg, switch), None if knob is None else getattr(pg, knob)
+        if on is not None and not (isinstance(on, str) and on == "auto"):
+            raise ValueError(f"{name}: {switch} must be None or 'auto', got {on!r}")
+        if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 2 <= v <= 32767):
+            raise ValueError(f"{name}: {knob} must be an integer in [2, 32767], got {v!r}")
+        if v is not None and on is None:
+            raise ValueError(f"{name}: {knob} is given, but {switch} is None, not 'auto'")
+        for what in ("skew", "curve"):
+            if on is not None and getattr(pg, what) is not None:
+                raise ValueError(f"{name}: {switch} and {what} are both given (a page with {switch}='auto' is level and flat: "
+                                 f"flatten a tilted or curled page with flatten_pages first)")
     if pg.quad is not None:
         if pg.rect is not None:
             raise ValueError(f"{name}: rect and quad are both given (a page in perspective is its quad: give rect=None)")
@@ -2204,8 +2177,7 @@ def _page_table(pg):
 
 
 def _page_bytes(pg, rect, skewed):
-    """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages, with a ruled page's two extra
-    bitmaps, a figure page's bitmap and table and a panel page's table (and outline bitmap without rules): a quad page's
+    """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages (ops.page_bytes): a quad page's
     rectified crop and its page, or an auto page's corner search on the image ``rect``."""
     from . import ops
     w, h = rect[2] - rect[0], rect[3] - rect[1]
@@ -2214,13 +2186,9 @@ def _page_bytes(pg, rect, skewed):
     if pg.quad is not None:
         w_r, h_r = quad_maps(pg.quad, 1).size
         return 3 * w_r * h_r + _page_bytes(pg._replace(quad=None), (0, 0, w_r, h_r), skewed)
-    rules = ops.rule_page_bytes(w, h) if pg.rules is not None else 0
-    rules += ops.figure_page_bytes(w, h) if pg.figures is not None else 0
-    rules += ops.panel_page_bytes(w, h, pg.rules is not None) if pg.panels is not None else 0
-    if not skewed:
-        return ops.page_bytes(w, h) + rules
-    return rules + ops.skew_page_bytes(w, h, pg.direction == "vertical",
-                                       _page_table(pg) if pg.skew is not None else [(1.0, 0.0)])
+    cs = (_page_table(pg) if pg.skew is not None else [(1.0, 0.0)]) if skewed else None
+    return ops.page_bytes(w, h, pg.direction == "vertical", cs, rules=pg.rules is not None, figures=pg.figures is not None,
+                          panels=pg.panels is not None)
 
 
 def _check_page_work(items):
@@ -2272,6 +2240,11 @@ def _find_pages(dimg, items, keys=()):
     return [it if isinstance(it, str) else next(found) for it in items], rq
 
 
+def _node_rects(nodes, x0=0, y0=0):
+    """The rectangles of mn_page_node entries, shifted by (x0, y0)."""
+    return [(x0 + int(q["x0"]), y0 + int(q["y0"]), x0 + int(q["x1"]), y0 + int(q["y1"])) for q in nodes]
+
+
 def _find_blocks(dimg, items, rq=None):
     """ops.find_blocks over items (image index, TextPage, rect) of the uploaded images ``dimg``, its tables back through one
     pinned copy and one synchronisation; a quad page (its corners given) is a level page on all of its rectified crop in ``rq``
@@ -2287,44 +2260,26 @@ def _find_blocks(dimg, items, rq=None):
         r = rq[_quad_key(i, pg.quad)]
         return r, (0, 0, r.shape[1], r.shape[0])
 
-    def rule_length(i, pg, rect):                       # of the crop, or of R for a quad page
-        _, (x0, y0, x1, y1) = src(i, pg, rect)
-        return None if pg.rules is None else pg.rule_length or ops.rule_length(x1 - x0, y1 - y0)
-    rls = [rule_length(*it) for it in items]
-    fss = [None if pg.figures is None else pg.figure_size or 0 for _, pg, _ in items]
-    pss = [None if pg.panels is None else pg.panel_size or 0 for _, pg, _ in items]
-    res_t, caps = ops.find_blocks([(*src(i, pg, rect), pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y,
-                                    pg.skew, pg.max_skew, rl, fs, pg.block_direction is not None, ps)
-                                   for (i, pg, rect), rl, fs, ps in zip(items, rls, fss, pss)])
-    host = _to_host(res_t).numpy()
-    rdt, ndt, sdt = ops.page_result_dtype(), ops.page_node_dtype(), ops.skew_block_dtype()
-    skewed = any(pg.skew is not None for _, pg, _ in items)
-    o = len(items) * sdt.itemsize if skewed else 0
-    skew = host[:o].view(sdt) if skewed else [None] * len(items)
-    res = host[o:o + len(items) * rdt.itemsize].view(rdt)
-    o, out = o + len(items) * rdt.itemsize, []
-    ft = o + sum(caps) * ndt.itemsize                   # the figure pages' tables, after every leaf table
-    pt = ft + lib.PAGE_MAX_FIGURES * ndt.itemsize * sum(fs is not None for fs in fss)   # then the panel pages' tables
-    for (i, pg, rect), r, cap, sk, rl, fs, ps in zip(items, res, caps, skew, rls, fss, pss):
-        leaves = host[o:o + cap * ndt.itemsize].view(ndt)[:int(r["n_leaves"])]
-        o += cap * ndt.itemsize
-        if fs is not None:
-            figs = host[ft:ft + lib.PAGE_MAX_FIGURES * ndt.itemsize].view(ndt)[:int(r["n_figures"])]
-            ft += lib.PAGE_MAX_FIGURES * ndt.itemsize
-        if ps is not None:
-            pans = host[pt:pt + lib.PAGE_MAX_PANELS * ndt.itemsize].view(ndt)[:int(r["n_panels"])]
-            pt += lib.PAGE_MAX_PANELS * ndt.itemsize
+    def page(i, pg, rect):
+        img, crop = src(i, pg, rect)                    # the default rule length is the crop's, or R's on a quad page
+        rl = None if pg.rules is None else pg.rule_length or ops.rule_length(crop[2] - crop[0], crop[3] - crop[1])
+        return ops.PageItem(img, crop, pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y, pg.skew, pg.max_skew,
+                            rule_length=rl,
+                            figure_size=None if pg.figures is None else pg.figure_size or 0,
+                            directions=pg.block_direction is not None,
+                            panel_size=None if pg.panels is None else pg.panel_size or 0)
+    pages = [page(*it) for it in items]
+    res_t, caps = ops.find_blocks(pages)
+    limits = {lib.PAGE_ERR_BLOCKS: ("blocks", lib.PAGE_MAX_BLOCKS), lib.PAGE_ERR_FIGURES: ("figures", lib.PAGE_MAX_FIGURES),
+              lib.PAGE_ERR_PANELS: ("panels", lib.PAGE_MAX_PANELS)}
+    out = []
+    for (i, pg, rect), p, (sk, r, leaves, figs, pans) in zip(items, pages, ops.page_tables(_to_host(res_t).numpy(), pages, caps)):
         if r["error"] == lib.PAGE_ERR_NODES:
             out.append(f"more than {lib.PAGE_MAX_NODES} nodes in one level of the XY-cut")
             continue
-        if r["error"] == lib.PAGE_ERR_BLOCKS:
-            out.append(f"{int(r['n_blocks'])} blocks exceed the {lib.PAGE_MAX_BLOCKS} a text page may hold")
-            continue
-        if r["error"] == lib.PAGE_ERR_FIGURES:
-            out.append(f"{int(r['n_figures'])} figures exceed the {lib.PAGE_MAX_FIGURES} a text page may hold")
-            continue
-        if r["error"] == lib.PAGE_ERR_PANELS:
-            out.append(f"{int(r['n_panels'])} panels exceed the {lib.PAGE_MAX_PANELS} a text page may hold")
+        if r["error"]:                                  # a table over its limit
+            noun, limit = limits[int(r["error"])]
+            out.append(f"{int(r['n_' + noun])} {noun} exceed the {limit} a text page may hold")
             continue
         X0, Y0 = (0, 0) if pg.quad is not None else rect[:2]
         vertical = pg.direction == "vertical"
@@ -2332,7 +2287,7 @@ def _find_blocks(dimg, items, rq=None):
         ink = "dark" if r["ink"] == lib.INK_DARK else "light"
         # A block grown inside a panel's outline is a panel block, of the opposite polarity: growth stops at the outline, so
         # a grown block lies inside a panel exactly when its leaf does.
-        boxes = [] if ps is None else [tuple(int(q[f]) for f in ("x0", "y0", "x1", "y1")) for q in pans]
+        boxes = [] if pans is None else _node_rects(pans)
         opposite = "light" if ink == "dark" else "dark"
         blocks, rejected, dirs, undecided, pols = [], [], [], [], []
         for q in leaves:
@@ -2355,20 +2310,19 @@ def _find_blocks(dimg, items, rq=None):
             blocks.append(box)
         res = dict(threshold=int(r["threshold"]), ink=ink, text_size=int(r["text_size"]), gap_x=int(r["gap_x"]),
                    gap_y=int(r["gap_y"]))
-        if rl is not None:
-            res.update(rule_length=rl, rule_pixels=int(r["rule_pixels"]))
-        if fs is not None:                              # in image coordinates, or rectangles of R on a quad page
-            res.update(figure_size=int(r["figure_size"]),
-                       figures=[(X0 + int(q["x0"]), Y0 + int(q["y0"]), X0 + int(q["x1"]), Y0 + int(q["y1"])) for q in figs])
+        if p.rule_length is not None:
+            res.update(rule_length=p.rule_length, rule_pixels=int(r["rule_pixels"]))
+        if figs is not None:                            # in image coordinates, or rectangles of R on a quad page
+            res.update(figure_size=int(r["figure_size"]), figures=_node_rects(figs, X0, Y0))
         if pg.block_direction is not None:
             res.update(block_direction=pg.block_direction, undecided=undecided)
-        if ps is not None:                              # in image coordinates, or rectangles of R on a quad page
-            res.update(panel_size=int(r["panel_size"]), panels=[(X0 + a, Y0 + b, X0 + c, Y0 + e) for a, b, c, e in boxes])
+        if pans is not None:                            # in image coordinates, or rectangles of R on a quad page
+            res.update(panel_size=int(r["panel_size"]), panels=_node_rects(pans, X0, Y0))
         if pg.quad is not None:
             shape = dimg[i].shape[:2]
             res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=d, polarity=pl, window=b)
                                for b, d, pl in zip(blocks, dirs, pols)],
-                       rejected=rejected, quad=_quad_key(i, pg.quad)[1], size=tuple(src(i, pg, rect)[1][2:]))
+                       rejected=rejected, quad=_quad_key(i, pg.quad)[1], size=tuple(p.rect[2:]))
         elif pg.skew is None:
             res.update(blocks=[TextBlock(b, d, polarity=pl, curve=pg.curve) for b, d, pl in zip(blocks, dirs, pols)],
                        rejected=rejected)

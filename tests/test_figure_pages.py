@@ -404,7 +404,7 @@ def test_ops_refuses_a_bad_figure_size():
     img = torch.zeros((8, 8, 3), dtype=torch.uint8)
     for bad, skew in ((1, None), (32768, None), (True, None), (-1, None), (40, 2.0), (0, 2.0)):
         with pytest.raises(ValueError, match="find_blocks: page 0: figure_size"):
-            ops.find_blocks([(img, (0, 0, 8, 8), False, 0, None, None, skew, 10.0, None, bad)])
+            ops.find_blocks([ops.PageItem(img, (0, 0, 8, 8), False, 0, skew=skew, figure_size=bad)])
 
 
 def test_kernels_build_without_spills(tmp_path):

@@ -405,7 +405,7 @@ def test_pages_32767_wide_and_skewed_frame_sides():
     SEEN["find_blocks_skewed"]["frame side 32767"] += 1
     n0 = ops.LAUNCHES
     with pytest.raises(ValueError, match="a frame side of 32768 exceeds 32767"):
-        ops.find_blocks([(_up(tall), (0, 0, w + 1, h), False, _lib.INK_AUTO, None, None, 2.0)])
+        ops.find_blocks([ops.PageItem(_up(tall), (0, 0, w + 1, h), False, _lib.INK_AUTO, skew=2.0)])
     assert ops.LAUNCHES == n0
     SEEN["find_blocks_skewed"]["frame side 32768"] += 1
 

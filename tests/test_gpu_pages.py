@@ -91,7 +91,7 @@ def test_page_tables_equal_twin():
     dimgs = [torch.from_numpy(im).to(DEV) for im in imgs]
     rects = [r if r is not None else (0, 0, imgs[i].shape[1], imgs[i].shape[0]) for i, r, *_ in items]
     pol = dict(auto=_lib.INK_AUTO, dark=_lib.INK_DARK, light=_lib.INK_LIGHT)
-    args = [(dimgs[i], rect, v, pol[p], *g) for (i, _, v, p, g), rect in zip(items, rects)]
+    args = [ops.PageItem(dimgs[i], rect, v, pol[p], *g) for (i, _, v, p, g), rect in zip(items, rects)]
     n0 = ops.LAUNCHES
     ops.find_blocks(args[:1])
     one = ops.LAUNCHES - n0

@@ -390,7 +390,7 @@ def test_ops_refuses_bad_directions():
     img = torch.zeros((8, 8, 3), dtype=torch.uint8)
     for bad, skew in ((1, None), ("auto", None), (True, 2.0)):
         with pytest.raises(ValueError, match="find_blocks: page 0: directions"):
-            ops.find_blocks([(img, (0, 0, 8, 8), False, 0, None, None, skew, 10.0, None, None, bad)])
+            ops.find_blocks([ops.PageItem(img, (0, 0, 8, 8), False, 0, skew=skew, directions=bad)])
 
 
 def test_work_memory_is_unchanged():

@@ -443,7 +443,7 @@ def test_ops_refuses_a_bad_panel_size():
     img = torch.zeros((8, 8, 3), dtype=torch.uint8)
     for bad, skew in ((1, None), (32768, None), (True, None), (-1, None), (40, 2.0), (0, 2.0)):
         with pytest.raises(ValueError, match="find_blocks: page 0: panel_size"):
-            ops.find_blocks([(img, (0, 0, 8, 8), False, 0, None, None, skew, 10.0, None, None, None, bad)])
+            ops.find_blocks([ops.PageItem(img, (0, 0, 8, 8), False, 0, skew=skew, panel_size=bad)])
 
 
 def test_constants_match_the_header():

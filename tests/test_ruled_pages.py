@@ -327,7 +327,7 @@ def test_ops_refuses_a_bad_rule_length():
     img = torch.zeros((8, 8, 3), dtype=torch.uint8)
     for bad, skew in ((1, None), (32768, None), (True, None), (40, 2.0)):
         with pytest.raises(ValueError, match="find_blocks: page 0: rule_length"):
-            ops.find_blocks([(img, (0, 0, 8, 8), False, 0, None, None, skew, 10.0, bad)])
+            ops.find_blocks([ops.PageItem(img, (0, 0, 8, 8), False, 0, skew=skew, rule_length=bad)])
 
 
 def test_kernels_build_without_spills(tmp_path):

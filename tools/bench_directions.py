@@ -129,8 +129,8 @@ def main():
     drawn = make_pages()
     pages = [p for p, _, _ in drawn]
     d = [torch.from_numpy(p).to(dev) for p in pages]
-    plain = [(x, (0, 0, x.shape[1], x.shape[0]), dr == "vertical", _lib.INK_AUTO, None, None) for x, (_, dr, _) in zip(d, drawn)]
-    auto = [r + (None, 10.0, None, None, True) for r in plain]
+    plain = [ops.PageItem(x, (0, 0, x.shape[1], x.shape[0]), dr == "vertical", _lib.INK_AUTO) for x, (_, dr, _) in zip(d, drawn)]
+    auto = [r._replace(directions=True) for r in plain]
 
     if args.profile:
         from torch.profiler import ProfilerActivity, profile

@@ -133,7 +133,7 @@ def main():
         found = pipeline._page_quads(d, items)
         keys = [pipeline._quad_key(i, pg.quad) for i, pg, _ in found]
         rq = pipeline._rectify(d, keys)
-        crops = [(rq[k], (0, 0, rq[k].shape[1], rq[k].shape[0]), False, _lib.INK_AUTO, None, None) for k in keys]
+        crops = [ops.PageItem(rq[k], (0, 0, rq[k].shape[1], rq[k].shape[0]), False, _lib.INK_AUTO) for k in keys]
         times = dict(search_ms=events_ms(lambda: ops.find_page_quads([(x, _lib.INK_AUTO) for x in d.values()])),
                      warp_ms=events_ms(lambda: pipeline._rectify(d, keys)), xy_cut_ms=events_ms(lambda: ops.find_blocks(crops)),
                      ms_per_call=events_ms(lambda: pipeline._find_pages(d, items)))
@@ -141,7 +141,7 @@ def main():
 
     def layout_ms(imgs, skew):
         d = [torch.from_numpy(p).to(dev) for p in imgs]
-        items = [(x, (0, 0, x.shape[1], x.shape[0]), False, _lib.INK_AUTO, None, None, skew) for x in d]
+        items = [ops.PageItem(x, (0, 0, x.shape[1], x.shape[0]), False, _lib.INK_AUTO, skew=skew) for x in d]
         for _ in range(5):
             ops.find_blocks(items)
         t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -114,8 +114,8 @@ def main():
     drawn = make_pages()
     pages = [p for p, _ in drawn]
     d = [torch.from_numpy(p).to(dev) for p in pages]
-    plain = [(x, (0, 0, x.shape[1], x.shape[0]), False, _lib.INK_AUTO, None, None) for x in d]
-    panels = [r + (None, 10.0, None, None, None, 0) for r in plain]
+    plain = [ops.PageItem(x, (0, 0, x.shape[1], x.shape[0]), False, _lib.INK_AUTO) for x in d]
+    panels = [r._replace(panel_size=0) for r in plain]
 
     if args.profile:
         from torch.profiler import ProfilerActivity, profile

@@ -91,9 +91,8 @@ def main():
     card = _card()
     pages = make_pages(args.pages)
     d = [torch.from_numpy(p).to(dev) for p in pages]
-    ruled = [(x, (0, 0, x.shape[1], x.shape[0]), False, _lib.INK_AUTO, None, None, None, 10.0,
-              ops.rule_length(x.shape[1], x.shape[0])) for x in d]
-    plain = [r[:6] for r in ruled]
+    plain = [ops.PageItem(x, (0, 0, x.shape[1], x.shape[0]), False, _lib.INK_AUTO) for x in d]
+    ruled = [r._replace(rule_length=ops.rule_length(x.shape[1], x.shape[0])) for r, x in zip(plain, d)]
 
     if args.profile:
         from torch.profiler import ProfilerActivity, profile
