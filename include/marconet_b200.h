@@ -959,6 +959,30 @@ typedef struct {
 int mn_find_page_quads_u8(const mn_text_block* blocks, const mn_quad_page* pages, int n, long long max_tiles, void* work,
                           long long work_bytes, void* stream);
 
+/* Book spreads (DESIGN.md section 7b, "Book spreads"): the spine of an open book, searched on the page component and corners
+ * that mn_find_page_quads_u8 left in its work, on the same stream, before that work is freed.  spines[i].page points to the
+ * mn_quad_page record of the spread's image.  mn_find_page_spines_u8 issues 2 launches for every spread of a call:
+ *   1. per 32 x 32 tile, each column's extent of the page component: cols[x] = max(h - y), cols[w + x] = max(y + 1) over the
+ *      component's pixels of column x (0: none), so cols[x] = h - t(x) and cols[w + x] = b(x);
+ *   2. one CTA per spread: over the columns with 4 (x - tl.x) >= tr.x - tl.x and 4 (tr.x - x) >= tr.x - tl.x, the top point
+ *      T_x = (x, t(x)) of the largest D_x = cross(tr - tl, T_x - tl), ties to the smallest x; over bl.x .. br.x likewise the
+ *      bottom point B_x = (x, b(x)) of the largest E_x = cross(B_x - bl, br - bl); found when D, E > 0, D^2 >= 4 |tr - tl|^2,
+ *      100 D >= |tr - tl|^2 and the same for E against |br - bl|.  All in int64.
+ * cols holds 2 w int32 in zeroed memory (mn_find_page_quads_u8's work); res is written whole.  spines: DEVICE array. */
+typedef struct {
+    int32_t found;              /* 1 when both notches are deep enough */
+    int32_t st[2];              /* the top spine point (x, t(x)); (-1, -1) when no column lies in the range */
+    int32_t sb[2];              /* the bottom spine point (x, b(x)); (-1, -1) likewise */
+    int32_t pad;
+    int64_t D, E;               /* the largest top and bottom depths, doubled-area units (INT64_MIN: no column) */
+} mn_page_spine;
+typedef struct {
+    const mn_quad_page* page;
+    int32_t* cols;
+    mn_page_spine* res;
+} mn_spine_page;
+int mn_find_page_spines_u8(const mn_spine_page* spines, int n, long long max_tiles, void* stream);
+
 /* Flat pages (DESIGN.md section 7b, "Flat pages"): the dewarp field of a curled page, built from its traced lines, composed with
  * the page's frame and sampled from the photo.  A page's line table (built on the host, pipeline.flat_line_table) holds
  * MN_FLAT_LINE_DOUBLES fp64 values per line, sorted by anchor Y (ties in reading order): xs, xe, mu_0 .. mu_3, Y, bx0, bx1.

@@ -245,6 +245,14 @@ class QuadPage(Structure):
                 ("hull", c_void_p), ("res", c_void_p)]
 
 
+class PageSpine(Structure):
+    _fields_ = [("found", c_int32), ("st", c_int32 * 2), ("sb", c_int32 * 2), ("pad", c_int32), ("D", c_int64), ("E", c_int64)]
+
+
+class SpinePage(Structure):
+    _fields_ = [("page", c_void_p), ("cols", c_void_p), ("res", c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -314,6 +322,7 @@ SYMBOLS = {
     "mn_find_lines_window_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_lines_curved_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_int, c_void_p, c_longlong, c_void_p]),
     "mn_find_page_quads_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
+    "mn_find_page_spines_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

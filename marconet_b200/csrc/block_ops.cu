@@ -2144,6 +2144,103 @@ __global__ void __launch_bounds__(kHullThreads) quad_hull_kernel(const mn_quad_p
     }
 }
 
+// Book spreads (DESIGN.md 7b, "Book spreads"): each column's first row t(x) and last row + 1 b(x) of the page component, as
+// h - t(x) and b(x) by atomicMax into zeroed memory (0: the column holds none of it); each warp takes rows w + 8 j of the
+// tile, and warp 0 folds the eight and issues one pair of atomics per column.
+__global__ void __launch_bounds__(kTileThreads) spine_cols_kernel(const mn_spine_page* __restrict__ spines) {
+    mn_pdl_prologue();
+    __shared__ int s_top[kTileThreads / 32][kTile], s_bot[kTileThreads / 32][kTile];
+    const mn_spine_page sp = spines[blockIdx.y];
+    const mn_quad_page* pg = sp.page;
+    const mn_text_block b = pg->b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    const unsigned long long best = *pg->best;
+    if (!best) return;
+    const int page = (int)~(unsigned)best, lx = threadIdx.x & 31, wp = threadIdx.x >> 5, x = tx + lx;
+    const int* label = pg->label;
+    int top = 0, bot = 0;
+    for (int y = ty + wp; x < b.w && y < min(ty + kTile, b.h); y += kTileThreads / 32) {
+        if (label[(long long)y * b.w + x] == page) {
+            top = max(top, b.h - y);
+            bot = y + 1;
+        }
+    }
+    s_top[wp][lx] = top;
+    s_bot[wp][lx] = bot;
+    __syncthreads();
+    if (wp == 0) {
+#pragma unroll
+        for (int k = 1; k < kTileThreads / 32; ++k) {
+            top = max(top, s_top[k][lx]);
+            bot = max(bot, s_bot[k][lx]);
+        }
+        if (bot) {
+            atomicMax(&sp.cols[x], top);
+            atomicMax(&sp.cols[b.w + x], bot);
+        }
+    }
+}
+
+// (depth, x) as one int64 that orders by depth, then by the smaller x: |depth| < 2^31 (sides up to 32767), so it cannot wrap.
+__device__ __forceinline__ long long spine_key(long long d, int x) {
+    return d * 4294967296ll + (long long)(0xffffffffu - (unsigned)x);
+}
+
+__device__ __forceinline__ bool spine_deep(long long d, int2 a, int2 c) {
+    const long long l2 = (long long)(c.x - a.x) * (c.x - a.x) + (long long)(c.y - a.y) * (c.y - a.y);
+    return d > 0 && d * d >= 4 * l2 && 100 * d >= l2;
+}
+
+// One CTA per spread: the keyed max of D over the top edge's middle half and of E over the bottom edge's, then the test.
+__global__ void __launch_bounds__(kHullThreads) spine_kernel(const mn_spine_page* __restrict__ spines) {
+    mn_pdl_prologue();
+    __shared__ long long s_key[2][kHullThreads / 32];
+    const mn_spine_page sp = spines[blockIdx.x];
+    const mn_quad_page* pg = sp.page;
+    const int w = pg->b.w, h = pg->b.h;
+    const int* q = pg->res->quad;
+    const int2 tl = make_int2(q[0], q[1]), tr = make_int2(q[2], q[3]), br = make_int2(q[4], q[5]), bl = make_int2(q[6], q[7]);
+    long long kt = LLONG_MIN, kb = LLONG_MIN;
+    for (int x = threadIdx.x; x < w; x += blockDim.x) {
+        const int top = sp.cols[x];
+        if (!top) continue;
+        if (4ll * (x - tl.x) >= tr.x - tl.x && 4ll * (tr.x - x) >= tr.x - tl.x)
+            kt = max(kt, spine_key(cross3(tl, tr, make_int2(x, h - top)), x));
+        if (4ll * (x - bl.x) >= br.x - bl.x && 4ll * (br.x - x) >= br.x - bl.x)
+            kb = max(kb, spine_key(-cross3(bl, br, make_int2(x, sp.cols[w + x])), x));
+    }
+    for (int o = 16; o; o >>= 1) {
+        kt = max(kt, (long long)__shfl_xor_sync(0xffffffffu, kt, o));
+        kb = max(kb, (long long)__shfl_xor_sync(0xffffffffu, kb, o));
+    }
+    if ((threadIdx.x & 31) == 0) {
+        s_key[0][threadIdx.x >> 5] = kt;
+        s_key[1][threadIdx.x >> 5] = kb;
+    }
+    __syncthreads();
+    if (threadIdx.x >= 32) return;
+    kt = threadIdx.x < blockDim.x / 32 ? s_key[0][threadIdx.x] : LLONG_MIN;
+    kb = threadIdx.x < blockDim.x / 32 ? s_key[1][threadIdx.x] : LLONG_MIN;
+    for (int o = 16; o; o >>= 1) {
+        kt = max(kt, (long long)__shfl_xor_sync(0xffffffffu, kt, o));
+        kb = max(kb, (long long)__shfl_xor_sync(0xffffffffu, kb, o));
+    }
+    if (threadIdx.x) return;
+    mn_page_spine* res = sp.res;
+    const int xt = kt == LLONG_MIN ? -1 : (int)(0xffffffffu - (unsigned)(kt & 0xffffffffll));
+    const int xb = kb == LLONG_MIN ? -1 : (int)(0xffffffffu - (unsigned)(kb & 0xffffffffll));
+    const long long D = kt == LLONG_MIN ? LLONG_MIN : kt >> 32, E = kb == LLONG_MIN ? LLONG_MIN : kb >> 32;
+    res->st[0] = xt;
+    res->st[1] = xt < 0 ? -1 : h - sp.cols[xt];
+    res->sb[0] = xb;
+    res->sb[1] = xb < 0 ? -1 : sp.cols[w + xb];
+    res->pad = 0;
+    res->D = D;
+    res->E = E;
+    res->found = xt >= 0 && xb >= 0 && spine_deep(D, tl, tr) && spine_deep(E, bl, br);
+}
+
 // 4-11 of the XY-cut: both passes of levels, the text size between them and the leaves, on pages whose bitmap and root are
 // written; under MN_PAGE_RULES, the three rule launches first, under MN_PAGE_PANELS the panel test and paint after the text
 // size, under MN_PAGE_FIGURES the figure launch after those, and under MN_PAGE_DIRECTIONS the direction launch after the leaves.
@@ -2304,6 +2401,16 @@ extern "C" int mn_find_page_quads_u8(const mn_text_block* blocks, const mn_quad_
     MN_CUDA_CHECK((mn_launch(quad_rows_kernel, grid, dim3(kTileThreads), 0, st, pages)));
     MN_LAUNCH_CHECK();
     MN_CUDA_CHECK((mn_launch(quad_hull_kernel, dim3(n), dim3(kHullThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_find_page_spines_u8(const mn_spine_page* spines, int n, long long max_tiles, void* stream) {
+    MN_REQUIRE(spines && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31), "mn_find_page_spines_u8: bad args");
+    cudaStream_t st = (cudaStream_t)stream;
+    MN_CUDA_CHECK((mn_launch(spine_cols_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, st, spines)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(spine_kernel, dim3(n), dim3(kHullThreads), 0, st, spines)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

@@ -2335,11 +2335,21 @@ def quad_page_bytes(w, h):
             + sum(_quad_areas(w, h)))
 
 
-def find_page_quads(pages, hulls=False, labels=False):
+def spine_page_bytes(w):
+    """Device bytes of one w pixels wide spread in find_page_quads beyond its image's (DESIGN.md 7b, "Book spreads"): its record,
+    its result and its column extents (2 w int32)."""
+    return ctypes.sizeof(_lib.SpinePage) + ctypes.sizeof(_lib.PageSpine) + 32 + -(-8 * w // 16) * 16
+
+
+def find_page_quads(pages, hulls=False, labels=False, spreads=()):
     """Page corners (mn_find_page_quads_u8; DESIGN.md 7b, "Perspective pages"), every image of the call in 8 launches whatever
     their number.  pages: list of (img, polarity): img a uint8 [H, W, 3] CUDA view with dense pixels (any row stride), H, W <=
     32767, read in place whole; polarity _lib.INK_AUTO / INK_DARK / INK_LIGHT (paper is grey <= t for INK_LIGHT, else grey > t).
     Returns the uint8 CUDA tensor of the pages' mn_page_quad records, in order (read it back as ``page_quad_dtype()``).
+    ``spreads`` (DESIGN.md 7b, "Book spreads"): the indices of the pages whose spine is searched too, on their component and
+    corners, by mn_find_page_spines_u8's 2 more launches whatever their number; the call then returns (quads, spines), spines
+    the uint8 CUDA tensor of their mn_page_spine records in the order given (``page_spine_dtype()``), in a table of its own
+    after the quads'.  Without spreads the call is exactly the one before: no spine memory and no more launches.
     ``hulls`` (tests): also return, per page, the int32 [4 H + 8, 2] CUDA view of its hull stack, whose first n_hull rows are
     the hull.  ``labels`` (tests): also return, per page, the int32 CUDA views of its compressed labels [H, W] (each paper pixel's
     component root, the smallest raster index y W + x of the component; -1 elsewhere) and pixel counts [H W] (a component's
@@ -2347,15 +2357,22 @@ def find_page_quads(pages, hulls=False, labels=False):
     global LAUNCHES
     dev = _check_items(pages, "find_page_quads", "page")
     n = len(pages)
+    spreads = [int(k) for k in spreads]
+    if any(not 0 <= k < n for k in spreads) or len(set(spreads)) != len(spreads):
+        raise ValueError(f"find_page_quads: spreads must be distinct page indices in [0, {n}), got {spreads!r}")
+    m = len(spreads)
     bsz, psz, rsz = (ctypes.sizeof(t) for t in (_lib.TextBlock, _lib.QuadPage, _lib.PageQuad))
+    ssz, spsz = ctypes.sizeof(_lib.SpinePage), ctypes.sizeof(_lib.PageSpine)
     for i, (img, polarity) in enumerate(pages):
         _check_crop((img, (0, 0, img.shape[1], img.shape[0]), False, polarity), dev, f"find_page_quads: page {i}", "")
-    if sum(quad_page_bytes(img.shape[1], img.shape[0]) for img, _ in pages) > PAGE_MAX_WORK:
+    if (sum(quad_page_bytes(img.shape[1], img.shape[0]) for img, _ in pages)
+            + sum(spine_page_bytes(pages[k][0].shape[1]) for k in spreads) > PAGE_MAX_WORK):
         raise ValueError(f"find_page_quads: the pages need more than the {PAGE_MAX_WORK} bytes of work memory a call may use")
-    out0 = -(-n * (bsz + psz) // 16) * 16                # records, then the results and the work, which the call zeroes
-    work0 = out0 + -(-n * rsz // 16) * 16
+    out0 = -(-(n * (bsz + psz) + m * ssz) // 16) * 16     # records, then the results and the work, which the call zeroes
+    work0 = out0 + -(-(n * rsz + m * spsz) // 16) * 16
     areas = [_quad_areas(img.shape[1], img.shape[0]) for img, _ in pages]
-    buf = torch.empty(work0 + sum(map(sum, areas)), dtype=torch.uint8, device=dev)
+    cols = [-(-8 * pages[k][0].shape[1] // 16) * 16 for k in spreads]
+    buf = torch.empty(work0 + sum(map(sum, areas)) + sum(cols), dtype=torch.uint8, device=dev)
     base = buf.data_ptr()
     blocks, recs, views, lviews, w, tiles = [], [], [], [], base + work0, 0
     for i, ((img, polarity), sizes) in enumerate(zip(pages, areas)):
@@ -2369,14 +2386,23 @@ def find_page_quads(pages, hulls=False, labels=False):
                        buf[count - base:count - base + 4 * h_ * w_].view(torch.int32)))
         w += sum(sizes)
         tiles = max(tiles, -(-w_ // 32) * -(-h_ // 32))
-    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.QuadPage * n)(*recs))
+    spines = [_lib.SpinePage(base + n * bsz + k * psz, c, base + out0 + n * rsz + j * spsz)
+              for j, (k, c) in enumerate(zip(spreads, itertools.accumulate([w] + cols[:-1])))]
+    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.QuadPage * n)(*recs)) + bytes((_lib.SpinePage * m)(*spines))
     buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
     _lib.check(_lib.load().mn_find_page_quads_u8(base, base + n * bsz, n, tiles, base + out0, len(buf) - out0, _stream()),
                "mn_find_page_quads_u8")
     LAUNCHES += 8
     res = buf[out0:out0 + n * rsz]
-    out = (res,) + ((views,) if hulls else ()) + ((lviews,) if labels else ())
-    return out if len(out) > 1 else res
+    if spreads:
+        stiles = max(-(-pages[k][0].shape[1] // 32) * -(-pages[k][0].shape[0] // 32) for k in spreads)
+        _lib.check(_lib.load().mn_find_page_spines_u8(base + n * (bsz + psz), m, stiles, _stream()), "mn_find_page_spines_u8")
+        LAUNCHES += 2
+        res = (res, buf[out0 + n * rsz:out0 + n * rsz + m * spsz])
+    else:
+        res = (res,)
+    out = res + ((views,) if hulls else ()) + ((lviews,) if labels else ())
+    return out if len(out) > 1 else res[0]
 
 
 def page_quad_dtype():
@@ -2384,6 +2410,12 @@ def page_quad_dtype():
     import numpy as np
     return np.dtype([("threshold", "<i4"), ("label", "<i4"), ("size", "<i4"), ("n_hull", "<i4"), ("area2", "<i8"),
                      ("idx", "<i4", (4,)), ("quad", "<i4", (8,))])
+
+
+def page_spine_dtype():
+    """numpy view of an mn_page_spine record."""
+    import numpy as np
+    return np.dtype([("found", "<i4"), ("st", "<i4", (2,)), ("sb", "<i4", (2,)), ("pad", "<i4"), ("D", "<i8"), ("E", "<i8")])
 
 
 def vertical_unlayout(items):

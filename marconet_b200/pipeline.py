@@ -2191,25 +2191,35 @@ def _page_bytes(pg, rect, skewed):
                           panels=pg.panels is not None)
 
 
-def _check_page_work(items):
-    """Refuse, before any launch, a call whose pages (image index, TextPage, rect) need more work memory than a call may use."""
+def _check_page_work(items, extra=0):
+    """Refuse, before any launch, a call whose pages (image index, TextPage, rect) need more work memory than a call may use,
+    ``extra`` bytes (the spines' of flat spreads) included."""
     from . import ops
     skewed = any(pg.skew is not None for _, pg, _ in items)
-    if sum(_page_bytes(pg, r, skewed) for _, pg, r in items) > ops.PAGE_MAX_WORK:
+    if sum(_page_bytes(pg, r, skewed) for _, pg, r in items) + extra > ops.PAGE_MAX_WORK:
         raise ValueError(f"the call's {len(items)} text pages need more than the {ops.PAGE_MAX_WORK} bytes of work memory a call "
                          f"may use (split the call)")
 
 
-def _page_quads(dimg, items):
+def _page_quads(dimg, items, spreads=()):
     """items (image index, TextPage, rect) with each TextPage(quad="auto") given the corners ops.find_page_quads finds (one
     pinned copy and one synchronisation), or replaced by its error message when they are not a page: no paper, a quad under a
-    quarter of the image, or one _plan_quad or the work limit rejects.  No launch without such pages."""
+    quarter of the image, or one _plan_quad or the work limit rejects.  No launch without such pages.  The items of indices
+    ``spreads`` (quad="auto" pages) also have their spine searched (DESIGN.md 7b, "Book spreads"), its records back in the same
+    synchronisation, and become (image index, TextPage, rect, mn_page_spine record) once their corners are a page."""
     from . import ops
     items = list(items)
     auto = [k for k, it in enumerate(items) if isinstance(it[1].quad, str)]
     if not auto:
         return items
-    host = _to_host(ops.find_page_quads([(dimg[items[k][0]], _INK[items[k][1].polarity]) for k in auto])).numpy()
+    quads = ops.find_page_quads([(dimg[items[k][0]], _INK[items[k][1].polarity]) for k in auto],
+                                spreads=[auto.index(k) for k in spreads])
+    spines = {}
+    if spreads:
+        host, sp = _to_host_all(list(quads))
+        spines = dict(zip(spreads, sp.view(ops.page_spine_dtype())))
+    else:
+        host = _to_host(quads).numpy()
     for k, r in zip(auto, host.view(ops.page_quad_dtype())):
         i, pg, _ = items[k]
         H, W = dimg[i].shape[:2]
@@ -2226,7 +2236,7 @@ def _page_quads(dimg, items):
         except ValueError as e:
             items[k] = f"no page found: the quad {tuple(pq.quad)} is rejected ({str(e).split(': ', 1)[-1]})"
             continue
-        items[k] = (i, pq, _quad_box(pq.quad, (H, W)))
+        items[k] = (i, pq, _quad_box(pq.quad, (H, W))) + ((spines[k],) if k in spines else ())
     return items
 
 
@@ -2464,7 +2474,9 @@ class FlatPage(NamedTuple):
     TextPage's, used wherever the page's blocks are searched.  ``light="even"`` (DESIGN.md 7b, "Even lighting") divides the
     page by its paper, the grey closing of its frame with an odd ``light_window`` x ``light_window`` window (default
     ops.light_window of the frame, a heuristic: darker features wider than the window are lightened); the page's searches then
-    run on the evened frame, and the flat page is evened with the same window and ink."""
+    run on the evened frame, and the flat page is evened with the same window and ink.  ``spread="auto"`` (DESIGN.md 7b, "Book
+    spreads"; with quad="auto") takes the page for an open book: the spine is searched on the paper the corners are found on,
+    and the spread's two pages are each flattened as a FlatPage with its half of the quad given."""
     rect: object = None
     quad: object = None
     skew: object = None
@@ -2477,6 +2489,7 @@ class FlatPage(NamedTuple):
     gap_y: object = None
     light: object = None
     light_window: object = None
+    spread: object = None
 
 
 FLAT_MAX_WORK = 1 << 31     # bytes of device memory the flat pages of one flatten_pages call may use
@@ -2505,6 +2518,15 @@ def _check_flat(fp, H, W, name):
     for quad="auto"), validated under _check_page's, _check_quad's and _check_curve's rules, curve with quad allowed.  Raises
     ValueError naming ``name``."""
     from . import ops
+    if fp.spread is not None:
+        if not (isinstance(fp.spread, str) and fp.spread == "auto"):
+            raise ValueError(f"{name}: spread must be None or 'auto', got {fp.spread!r}")
+        if not (isinstance(fp.quad, str) and fp.quad == "auto"):
+            raise ValueError(f"{name}: spread='auto' needs quad='auto' (the spine is searched on the paper the corner search "
+                             f"finds), got quad={fp.quad!r}")
+        for what in ("rect", "skew"):
+            if getattr(fp, what) is not None:
+                raise ValueError(f"{name}: spread and {what} are both given (a spread is its found quad, cut at the spine)")
     if fp.light is not None and not (isinstance(fp.light, str) and fp.light == "even"):
         raise ValueError(f"{name}: light must be None or 'even', got {fp.light!r}")
     if fp.light_window is not None:
@@ -2563,10 +2585,39 @@ def _check_flat_work(items, names):
         if total > FLAT_MAX_WORK:
             raise ValueError(f"{name}: the call's flat pages up to this one need {total} bytes of work memory, over the "
                              f"{FLAT_MAX_WORK} a call may use (split the call)")
+    from . import ops
     searched = [(i, _flat_text_page(fp), rect) for i, fp, rect in items
                 if fp.curve is not None or isinstance(fp.skew, str) or isinstance(fp.quad, str)]
     if searched:
-        _check_page_work(searched)
+        _check_page_work(searched, sum(ops.spine_page_bytes(rect[2] - rect[0]) for _, fp, rect in items if fp.spread is not None))
+
+
+def _spread_halves(fp, sp, shape, name):
+    """(spine, depth, halves) of a spread page ``fp`` (its quad found) with its mn_page_spine record ``sp`` (DESIGN.md 7b, "Book
+    spreads"): the spine points ((x_t, y_t), (x_b, y_b)), the notch depths in pixels and, in reading order, (side, FlatPage of the
+    half's quad, rect) with the half validated as a FlatPage.  Raises ValueError naming ``name`` for no spine found or a half
+    _check_flat rejects."""
+    tl, tr, br, bl = ((int(p[0]), int(p[1])) for p in fp.quad)
+    lt, lb = math.hypot(tr[0] - tl[0], tr[1] - tl[1]), math.hypot(br[0] - bl[0], br[1] - bl[1])
+    if not sp["found"]:
+        if sp["st"][0] < 0 or sp["sb"][0] < 0:
+            raise ValueError(f"{name}: no spread found: no column of the page lies in the middle half of its top or bottom edge")
+        raise ValueError(f"{name}: no spread found: the top and bottom notches are {int(sp['D']) / lt:.2f} and "
+                         f"{int(sp['E']) / lb:.2f} pixels deep, where {max(2.0, lt / 100):.2f} and {max(2.0, lb / 100):.2f} "
+                         f"are needed")
+    st, sb = tuple(int(v) for v in sp["st"]), tuple(int(v) for v in sp["sb"])
+    halves = []
+    for side, q in (("left", (tl, st, sb, bl)), ("right", (st, tr, br, sb))):
+        half = fp._replace(quad=QuadRegion(*((float(x), float(y)) for x, y in q)), spread=None)
+        try:
+            rect = _check_flat(half, *shape, "page")
+        except ValueError as e:
+            raise ValueError(f"{name}: the {side} page {tuple(half.quad)} of the spread is rejected "
+                             f"({str(e).split(': ', 1)[-1]})") from None
+        halves.append((side, half, rect))
+    if fp.direction == "vertical":                      # bound on the right: the right page is read first
+        halves.reverse()
+    return (st, sb), (int(sp["D"]) / lt, int(sp["E"]) / lb), halves
 
 
 def flat_strips(strips, w):
@@ -2621,6 +2672,14 @@ def flatten_pages(images, pages, to_host=False):
     and find_lines' stages), and every page with a curled line goes through ops.flat_remap's two launches; a page whose lines
     all come back level is flattened as without curve.  Raises ValueError naming the image and the page, before any launch,
     for a page its rules reject, and after the search for a page without a page found or over a limit.
+    A page with ``spread="auto"`` (DESIGN.md 7b, "Book spreads") is an open book: its spine, the deepest notch in the middle half
+    of the found quad's top edge and of its bottom edge, is searched on the device in the corner search's call (2 more launches
+    for all such pages of the call, and its records back in the same synchronisation as the corners), and the spread is cut
+    into the quads (tl, st, sb, bl) and (st, tr, br, sb).  Its dict is kind "spread", ``quad`` (the outer corners), ``spine``
+    ((x_t, y_t), (x_b, y_b)), ``depth`` (the top and bottom notch depths, in pixels) and ``pages``: the two halves' dicts in
+    reading order (left, right; right, left for a vertical page), each exactly the dict of FlatPage(quad=half) with the page's
+    other fields, plus ``side`` ("left" or "right").  A spread without notches deep enough raises "no spread found" after the
+    search, naming the image and the page, as does a half the quad rules reject.
     A page with ``light="even"`` (DESIGN.md 7b, "Even lighting") has its frame evened first, every light page in one
     ops.even_light call (six launches), and its searches after the corners' read the evened frame; a skewed or curled light
     page is evened again after its warp or remap (four more launches for all of them).  Its dict gains ``light_window`` (the
@@ -2643,17 +2702,34 @@ def flatten_pages(images, pages, to_host=False):
     dev = next((im.device for im in imgs if im.is_cuda), torch.device("cuda", torch.cuda.current_device()))
     with torch.cuda.device(dev):
         dimg = _device_images(sorted({i for i, _, _ in items}), imgs, dev)
-        found = _page_quads(dimg, [(i, _flat_text_page(fp), rect) for i, fp, rect in items])
+        found = _page_quads(dimg, [(i, _flat_text_page(fp), rect) for i, fp, rect in items],
+                            [k for k, (_, fp, _) in enumerate(items) if fp.spread is not None])
+        # Each spread becomes its two halves, quads given; ``groups`` folds their dicts back into the spread's afterwards.
+        given, groups, flat_names = items, [], []
+        items = []
         for k, (f, name) in enumerate(zip(found, names)):
             if isinstance(f, str):
                 raise ValueError(f"{name}: {f}")
-            i, fp, _ = items[k]
+            i, fp, _ = given[k]
+            if fp.spread is not None:
+                fp = fp._replace(quad=f[1].quad)
+                spine, depth, halves = _spread_halves(fp, f[3], dimg[i].shape[:2], name)
+                groups.append((dict(kind="spread", quad=_quad_key(i, fp.quad)[1], spine=spine, depth=depth),
+                               [(len(items) + j, side) for j, (side, _, _) in enumerate(halves)]))
+                for side, half, rect in halves:
+                    items.append((i, half, rect))
+                    flat_names.append(f"{name}, {side} page")
+                continue
             if isinstance(fp.quad, str):
                 fp = fp._replace(quad=f[1].quad)
                 size = _flat_frame(fp, f[2])
                 if max(size) > 32767:
                     raise ValueError(f"{name}: a side of the page's flat frame reaches {max(size)} pixels, over 32767")
-                items[k] = (i, fp, f[2])
+                given[k] = (i, fp, f[2])
+            groups.append(len(items))
+            items.append(given[k])
+            flat_names.append(name)
+        names = flat_names
         _check_flat_work(items, names)
         rq = _rectify(dimg, [_quad_key(i, fp.quad) for i, fp, _ in items if fp.quad is not None])
         src, frames = dict(dimg), {}
@@ -2763,8 +2839,8 @@ def flatten_pages(images, pages, to_host=False):
             for j, k in enumerate(light):
                 pol = items[k][1].polarity
                 res[k]["ink"] = pol if pol != "auto" else "dark" if int(ink_host[j, 2]) == ops._lib.INK_DARK else "light"
-    for (i, _, _), d in zip(items, res):
-        out[i].append(d)
+    for (i, _, _), g in zip(given, groups):
+        out[i].append(res[g] if isinstance(g, int) else dict(g[0], pages=[dict(res[k], side=side) for k, side in g[1]]))
     return out
 
 
