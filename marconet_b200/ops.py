@@ -942,11 +942,61 @@ def postprocess_sr(sr):
     return out
 
 
-def _table(ctype, records, device):
-    """Host-built array of C records -> device byte tensor (the kernels read their descriptors from device memory)."""
-    import numpy as np
-    arr = (ctype * len(records))(*records)
-    return torch.from_numpy(np.frombuffer(bytes(arr), dtype=np.uint8).copy()).to(device)
+class _Pack:
+    """The one uint8 device buffer of a batched call, which the kernels read their records and tables from.  ``area`` places
+    its areas in order, each at the next multiple of its alignment; ``alloc`` allocates it, its length a multiple of the
+    largest alignment (as a C struct's), and returns its address, to which the records' pointers add the areas' offsets;
+    ``upload`` copies the host bytes of the areas that have them in one host-to-device copy."""
+
+    def __init__(self):
+        self.end, self.align = 0, 1
+
+    def area(self, nbytes, align=1):
+        """The offset of ``nbytes`` new bytes at the next multiple of ``align``."""
+        o = -(-self.end // align) * align
+        self.end, self.align = o + nbytes, max(self.align, align)
+        return o
+
+    def alloc(self, device):
+        self.buf = torch.empty(-(-self.end // self.align) * self.align, dtype=torch.uint8, device=device)
+        return self.buf.data_ptr()
+
+    def upload(self, *areas):
+        """Copies (offset, bytes) areas, in increasing order, as the one range from the first area to the end of the last, with
+        zeros between them.  Returns the buffer."""
+        lo = areas[0][0]
+        host = bytearray(areas[-1][0] + len(areas[-1][1]) - lo)
+        for o, b in areas:
+            host[o - lo:o - lo + len(b)] = b
+        self.buf[lo:lo + len(host)].copy_(torch.frombuffer(host, dtype=torch.uint8))
+        return self.buf
+
+    @classmethod
+    def of(cls, ctype, recs, device):
+        """The buffer of one table of C records (which point outside it), allocated and uploaded."""
+        pack = cls()
+        pack.area(len(recs) * ctypes.sizeof(ctype))
+        pack.alloc(device)
+        return pack.upload((0, bytes((ctype * len(recs))(*recs))))
+
+
+def _check_items(items, what, noun, field=0):
+    """The device of a batched call's items, that of field ``field`` of the first one, after checking their number (one launch
+    holds 1 to 65535)."""
+    if not items:
+        raise ValueError(f"{what}: no {noun}s")
+    if len(items) > 65535:
+        raise ValueError(f"{what}: at most 65535 {noun}s per launch")
+    return items[0][field].device
+
+
+def _check_channels(items, what):
+    """The channel count cn of a batched image call, that of its first source (3 unless that is a 3-D tensor), 1 to 4."""
+    src = items[0][0]
+    cn = src.shape[2] if isinstance(src, torch.Tensor) and src.dim() == 3 else 3
+    if not 1 <= cn <= 4:
+        raise RuntimeError(f"{what}: {cn} channels (1 to 4)")
+    return cn
 
 
 def preprocess_lq_crops(crops, out_h=32, out_w=512):
@@ -982,7 +1032,7 @@ def preprocess_lq_crops(crops, out_h=32, out_w=512):
         recs.append(_lib.LqCrop(img.data_ptr() + x0 * cn, img.stride(0), h, x1 - x0, cn, fx, fy, dh, dw))
         widths.append(dw)
     dev = crops[0][0].device
-    table = _table(_lib.LqCrop, recs, dev)
+    table = _Pack.of(_lib.LqCrop, recs, dev)
     lq = torch.empty((len(recs), cn, out_h, out_w), dtype=torch.float32, device=dev)
     _lib.check(_lib.load().mn_preprocess_lq_u8_batched(_ptr(table), len(recs), cn, _ptr(lq), out_h, out_w, _stream()),
                "mn_preprocess_lq_u8_batched")
@@ -1015,7 +1065,7 @@ def postprocess_sr_pieces(sr, pieces):
             raise ValueError(f"postprocess_sr_pieces: piece {i}: line {line}, columns [{x0}, {x0 + width}) outside the [{b}, {w}] SR output")
         recs.append(_lib.SrPiece(line, x0, width, dst.data_ptr(), dst.stride(0)))
         mx = max(mx, width)
-    table = _table(_lib.SrPiece, recs, sr.device)
+    table = _Pack.of(_lib.SrPiece, recs, sr.device)
     sn, sc, sh, sw = sr.stride()
     _lib.check(_lib.load().mn_postprocess_sr_u8_pieces(_ptr(sr), sn, sc, sh, sw, c, h, w, _ptr(table), len(recs), mx, _stream()),
                "mn_postprocess_sr_u8_pieces")
@@ -1032,23 +1082,17 @@ def figure_panels(items):
       priors  non-empty list of fp32 [3, 128, 128] CUDA views (any strides), the characters' generator images in label order."""
     import numpy as np
     global LAUNCHES
-    if not items:
-        raise ValueError("figure_panels: no images")
-    if len(items) > 65535:
-        raise ValueError("figure_panels: at most 65535 images per launch")
-    dev = items[0][1].device
-    n_prior = sum(len(it[4]) for it in items)
-    n_marks = sum(len(it[2]) + len(it[3]) for it in items)
-    isz, psz = ctypes.sizeof(_lib.FigureImage), ctypes.sizeof(_lib.FigurePrior)
-    buf = torch.empty(len(items) * isz + n_prior * psz + 8 * max(1, n_marks), dtype=torch.uint8, device=dev)
-    base = buf.data_ptr()
-    p_off, m_off = len(items) * isz, len(items) * isz + n_prior * psz
+    dev = _check_items(items, "figure_panels", "image", 1)
+    psz = ctypes.sizeof(_lib.FigurePrior)
+    pack = _Pack()
+    pack.area(len(items) * ctypes.sizeof(_lib.FigureImage))
+    p_off = pack.area(sum(len(it[4]) for it in items) * psz)
+    m_off = pack.area(8 * max(1, sum(len(it[2]) + len(it[3]) for it in items)))
+    base = pack.alloc(dev)
     recs, prs, marks, mx = [], [], [], 0
     for i, (img, fig, top, bot, priors) in enumerate(items):
-        for name, t in (("img", img), ("fig", fig)):
-            if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3 \
-                    or t.stride(2) != 1 or t.stride(1) != 3 or t.stride(0) < 3 * t.shape[1]:
-                raise RuntimeError(f"figure_panels: image {i}: {name} must be a uint8 [., ., 3] tensor with dense pixels on {dev}")
+        _dense_u8(img, dev, 3, f"figure_panels: image {i}: img")
+        _dense_u8(fig, dev, 3, f"figure_panels: image {i}: fig")
         h, w = img.shape[:2]
         S = round_half_even(w * (128 / h))
         W = fig.shape[1]
@@ -1067,9 +1111,8 @@ def figure_panels(items):
                 raise RuntimeError(f"figure_panels: image {i}, character {k}: prior must be an fp32 [3, 128, 128] tensor on {dev}")
             prs.append(_lib.FigurePrior(p.data_ptr(), *p.stride()))
         mx = max(mx, W)
-    host = bytes((_lib.FigureImage * len(recs))(*recs)) + bytes((_lib.FigurePrior * len(prs))(*prs)) + \
-        np.asarray(marks or [(0, 0)], dtype=np.int32).tobytes()
-    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    buf = pack.upload((0, bytes((_lib.FigureImage * len(recs))(*recs))), (p_off, bytes((_lib.FigurePrior * len(prs))(*prs))),
+                      (m_off, np.asarray(marks or [(0, 0)], dtype=np.int32).tobytes()))
     _lib.check(_lib.load().mn_figure_u8(_ptr(buf), len(recs), mx, _stream()), "mn_figure_u8")
     LAUNCHES += 1
 
@@ -1098,7 +1141,7 @@ def prediction_table(windows, device, out=None):
     elif out.dtype != torch.uint8 or out.device != torch.device(device) or out.numel() < len(windows) * isz or out.data_ptr() % 8:
         raise ValueError(f"prediction_table: out must be an 8-byte aligned uint8 buffer of >= {len(windows) * isz} bytes on {device}")
     recs = [_lib.PredRow(float(a), float(s), float(lo), float(hi), out.data_ptr() + r * isz) for r, (a, s, lo, hi) in enumerate(windows)]
-    return _table(_lib.PredRow, recs, device), out
+    return _Pack.of(_lib.PredRow, recs, device), out
 
 
 def decode_predictions(logits, locs_lr, rows, first=0, n_alphabet=6735):
@@ -1229,14 +1272,8 @@ def resize_cubic(items):
     pixels (any row stride; dst may exceed 2^31 bytes).  The scales are the dsize form's 1/((double)dw/w) and 1/((double)dh/h);
     for dw = s*w, dh = s*h they equal 1/s, so dst is also cv2.resize(src, (0, 0), fx=s, fy=s, interpolation=INTER_CUBIC)."""
     global LAUNCHES
-    if not items:
-        raise ValueError("resize_cubic: no images")
-    if len(items) > 65535:
-        raise ValueError("resize_cubic: at most 65535 images per launch")
-    dev = items[0][0].device
-    cn = items[0][0].shape[2] if isinstance(items[0][0], torch.Tensor) and items[0][0].dim() == 3 else 3
-    if not 1 <= cn <= 4:
-        raise RuntimeError(f"resize_cubic: {cn} channels (1 to 4)")
+    dev = _check_items(items, "resize_cubic", "image")
+    cn = _check_channels(items, "resize_cubic")
     recs, mx = [], 0
     for i, (src, dst) in enumerate(items):
         _dense_u8(src, dev, cn, f"resize_cubic: image {i}: src")
@@ -1245,25 +1282,24 @@ def resize_cubic(items):
         recs.append(_lib.ResizeImage(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw,
                                      1.0 / (dw / w), 1.0 / (dh / h)))
         mx = max(mx, dh * dw)
-    table = _table(_lib.ResizeImage, recs, dev)
+    table = _Pack.of(_lib.ResizeImage, recs, dev)
     _lib.check(_lib.load().mn_resize_cubic_u8_batched(_ptr(table), len(recs), cn, mx, _stream()), "mn_resize_cubic_u8_batched")
     LAUNCHES += 1
 
 
-def _region_records(regions, feather, what, record, extra=0):
-    """Validated mn_region records of composite_regions' (page, sr, rect, chain, ...) tuples, their chains, the largest rectangle's
-    pixel count and a device buffer for the ``record``-type table followed by the chains (and ``extra`` bytes after them)."""
-    if not regions:
-        raise ValueError(f"{what}: no regions")
-    if len(regions) > 65535:
-        raise ValueError(f"{what}: at most 65535 regions per launch")
+def _region_records(regions, feather, what, record, tables=None):
+    """Validated mn_region records of composite_regions' (page, sr, rect, chain, ...) tuples, the largest rectangle's pixel
+    count, the call's allocated buffer, the (offset, bytes) of the chains in it and the offset of its ``tables`` bytes of curve
+    tables (None without them).  The buffer holds the ``record``-type table, the chains, then the 8-byte aligned tables."""
+    import numpy as np
+    dev = _check_items(regions, what, "region")
     if feather < 0:
         raise ValueError(f"{what}: feather {feather} < 0")
-    dev = regions[0][0].device
-    n_chain = sum(len(r[3]) for r in regions)
-    isz = ctypes.sizeof(record)
-    buf = torch.empty(len(regions) * isz + 4 * max(1, n_chain) + extra, dtype=torch.uint8, device=dev)
-    c_base = buf.data_ptr() + len(regions) * isz
+    pack = _Pack()
+    pack.area(len(regions) * ctypes.sizeof(record))
+    c_off = pack.area(4 * max(1, sum(len(r[3]) for r in regions)))
+    t_off = None if tables is None else pack.area(tables, 8)
+    c_base = pack.alloc(dev) + c_off
     recs, chains, mx = [], [], 0
     for i, (page, sr, rect, chain) in enumerate(r[:4] for r in regions):
         _dense_u8(page, dev, 3, f"{what}: region {i}: page")
@@ -1281,13 +1317,7 @@ def _region_records(regions, feather, what, record, extra=0):
                                 sr.shape[0], sr.shape[1], x0, y0, x1, y1, feather, len(chain)))
         chains += chain
         mx = max(mx, (x1 - x0) * (y1 - y0))
-    return recs, chains, mx, buf
-
-
-def _upload_records(buf, recs, chains):
-    import numpy as np
-    host = bytes((type(recs[0]) * len(recs))(*recs)) + np.asarray(chains or [0], dtype=np.int32).tobytes()
-    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    return recs, mx, pack, (c_off, np.asarray(chains or [0], dtype=np.int32).tobytes()), t_off
 
 
 def composite_regions(regions, feather):
@@ -1301,8 +1331,8 @@ def composite_regions(regions, feather):
     back) is blended over the page with weight a = min(1, fl((float)d + 0.5)/F), d the distance to the nearest side not on the
     page border; regions later in the list compose over earlier ones, and each pixel is written once."""
     global LAUNCHES
-    recs, chains, mx, buf = _region_records(regions, int(feather), "composite_regions", _lib.Region)
-    _upload_records(buf, recs, chains)
+    recs, mx, pack, chains, _ = _region_records(regions, int(feather), "composite_regions", _lib.Region)
+    buf = pack.upload((0, bytes((_lib.Region * len(recs))(*recs))), chains)
     _lib.check(_lib.load().mn_composite_regions_u8(_ptr(buf), len(recs), mx, _stream()), "mn_composite_regions_u8")
     LAUNCHES += 1
 
@@ -1328,14 +1358,8 @@ def warp_perspective(items):
 def _warp(items, what, rows, record, symbol):
     """One launch of ``symbol`` over warp_affine's / warp_perspective's items, M ``rows`` x 3."""
     global LAUNCHES
-    if not items:
-        raise ValueError(f"{what}: no images")
-    if len(items) > 65535:
-        raise ValueError(f"{what}: at most 65535 images per launch")
-    dev = items[0][0].device
-    cn = items[0][0].shape[2] if isinstance(items[0][0], torch.Tensor) and items[0][0].dim() == 3 else 3
-    if not 1 <= cn <= 4:
-        raise RuntimeError(f"{what}: {cn} channels (1 to 4)")
+    dev = _check_items(items, what, "image")
+    cn = _check_channels(items, what)
     recs, mx = [], 0
     for i, (src, dst, m) in enumerate(items):
         _dense_u8(src, dev, cn, f"{what}: image {i}: src")
@@ -1348,7 +1372,7 @@ def _warp(items, what, rows, record, symbol):
             raise ValueError(f"{what}: image {i}: M must be {rows} x 3")
         recs.append(record(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw, (ctypes.c_double * (3 * rows))(*m)))
         mx = max(mx, dh * dw)
-    table = _table(record, recs, dev)
+    table = _Pack.of(record, recs, dev)
     _lib.check(getattr(_lib.load(), symbol)(_ptr(table), len(recs), cn, mx, _stream()), symbol)
     LAUNCHES += 1
 
@@ -1361,7 +1385,7 @@ def composite_regions_affine(regions, feather):
     (pipeline.oriented_maps).  A page pixel belongs to an oriented region where its fixed-point sr coordinates fall in
     [-1/2, w - 1/2) x [-1/2, h - 1/2)."""
     global LAUNCHES
-    recs, chains, mx, buf = _region_records(regions, int(feather), "composite_regions_affine", _lib.RegionAffine)
+    recs, mx, pack, chains, _ = _region_records(regions, int(feather), "composite_regions_affine", _lib.RegionAffine)
     out = []
     for i, (r, rec) in enumerate(zip(regions, recs)):
         maps = r[4]
@@ -1373,7 +1397,7 @@ def composite_regions_affine(regions, feather):
         if len(n) != 6 or not (kx > 0 and ky > 0):
             raise ValueError(f"composite_regions_affine: region {i}: expected (N 2 x 3, kx > 0, ky > 0)")
         out.append(_lib.RegionAffine(rec, _lib.REGION_AFFINE, kx, ky, 0, (ctypes.c_double * 6)(*n)))
-    _upload_records(buf, out, chains)
+    buf = pack.upload((0, bytes((_lib.RegionAffine * len(out))(*out))), chains)
     _lib.check(_lib.load().mn_composite_regions_affine_u8(_ptr(buf), len(out), mx, _stream()), "mn_composite_regions_affine_u8")
     LAUNCHES += 1
 
@@ -1385,7 +1409,7 @@ def composite_regions_quad(regions, feather):
     denominator over rect, the bounding box of its footprint in page pixels (pipeline.quad_maps).  The footprint test is the
     affine one on its fixed-point sr coordinates."""
     global LAUNCHES
-    recs, chains, mx, buf = _region_records(regions, int(feather), "composite_regions_quad", _lib.RegionQuad)
+    recs, mx, pack, chains, _ = _region_records(regions, int(feather), "composite_regions_quad", _lib.RegionQuad)
     out = []
     for i, (r, rec) in enumerate(zip(regions, recs)):
         maps = r[4]
@@ -1398,7 +1422,7 @@ def composite_regions_quad(regions, feather):
             raise ValueError(f"composite_regions_quad: region {i}: expected (N 2 x 3 or 3 x 3, kx > 0, ky > 0)")
         kind = _lib.REGION_AFFINE if len(n) == 6 else _lib.REGION_PERSPECTIVE
         out.append(_lib.RegionQuad(rec, kind, kx, ky, 0, (ctypes.c_double * 9)(*n)))
-    _upload_records(buf, out, chains)
+    buf = pack.upload((0, bytes((_lib.RegionQuad * len(out))(*out))), chains)
     _lib.check(_lib.load().mn_composite_regions_quad_u8(_ptr(buf), len(out), mx, _stream()), "mn_composite_regions_quad_u8")
     LAUNCHES += 1
 
@@ -1424,26 +1448,15 @@ class CurveTable(NamedTuple):
         return np.concatenate([[float(self.scale)], np.asarray(self.c, np.float64), top, bottom]), k
 
 
-def _align8(n):
-    return (n + 7) & ~7
-
-
 def remap_curved(items):
     """Curved text regions rectified, every crop in one launch (mn_remap_curved_u8_batched; DESIGN.md 7b, "Curved text regions"):
     cv2.remap(src, mapx, mapy, INTER_CUBIC, borderMode=BORDER_REPLICATE) with the fp32 crop maps of each region's curves, OpenCV's
     own 8-bit path (IPP off).  items: list of (src, dst, curve): uint8 [h, w, cn] and [h_r, w_r, cn] CUDA views with dense pixels
     (any row stride), h, w <= 32767, and curve a CurveTable whose crop map stays below 2^14 pixels in magnitude
     (pipeline.plan_regions keeps it so).  The curve tables go up with the records in one copy."""
-    import numpy as np
     global LAUNCHES
-    if not items:
-        raise ValueError("remap_curved: no images")
-    if len(items) > 65535:
-        raise ValueError("remap_curved: at most 65535 images per launch")
-    dev = items[0][0].device
-    cn = items[0][0].shape[2] if isinstance(items[0][0], torch.Tensor) and items[0][0].dim() == 3 else 3
-    if not 1 <= cn <= 4:
-        raise RuntimeError(f"remap_curved: {cn} channels (1 to 4)")
+    dev = _check_items(items, "remap_curved", "image")
+    cn = _check_channels(items, "remap_curved")
     tables = []
     for i, (src, dst, curve) in enumerate(items):
         _dense_u8(src, dev, cn, f"remap_curved: image {i}: src")
@@ -1452,18 +1465,17 @@ def remap_curved(items):
             raise ValueError(f"remap_curved: image {i}: a {src.shape[0]}x{src.shape[1]} source exceeds OpenCV's int16 source "
                              f"coordinates")
         tables.append(curve.values(f"remap_curved: image {i}"))
-    isz = ctypes.sizeof(_lib.RemapCurvedImage)
-    n_tab = sum(t.size for t, _ in tables)
-    buf = torch.empty(len(items) * isz + 8 * n_tab, dtype=torch.uint8, device=dev)
-    base, o, recs, mx = buf.data_ptr() + len(items) * isz, 0, [], 0
+    pack = _Pack()
+    pack.area(len(items) * ctypes.sizeof(_lib.RemapCurvedImage))
+    t_off = pack.area(8 * sum(t.size for t, _ in tables))
+    base, o, recs, mx = pack.alloc(dev) + t_off, 0, [], 0
     for (src, dst, _), (t, k) in zip(items, tables):
         (h, w), (dh, dw) = src.shape[:2], dst.shape[:2]
         recs.append(_lib.RemapCurvedImage(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw, base + 8 * o,
                                           k, 0))
         o += t.size
         mx = max(mx, dh * dw)
-    host = bytes((_lib.RemapCurvedImage * len(recs))(*recs)) + np.concatenate([t for t, _ in tables]).tobytes()
-    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    buf = pack.upload((0, bytes((_lib.RemapCurvedImage * len(recs))(*recs))), (t_off, b"".join(t.tobytes() for t, _ in tables)))
     _lib.check(_lib.load().mn_remap_curved_u8_batched(_ptr(buf), len(recs), cn, mx, _stream()), "mn_remap_curved_u8_batched")
     LAUNCHES += 1
 
@@ -1492,16 +1504,9 @@ def flat_remap(items, tables=False):
     Raises ValueError naming the page, before any launch, for a column met by more than FLAT_MAX_COLUMN_LINES lines."""
     import numpy as np
     global LAUNCHES
-    if not items:
-        raise ValueError("flat_remap: no pages")
-    if len(items) > 65535:
-        raise ValueError("flat_remap: at most 65535 pages per launch")
-    dev = items[0][0].device
-    cn = items[0][0].shape[2] if isinstance(items[0][0], torch.Tensor) and items[0][0].dim() == 3 else 3
-    if not 1 <= cn <= 4:
-        raise RuntimeError(f"flat_remap: {cn} channels (1 to 4)")
-    isz = ctypes.sizeof(_lib.FlatPage)
-    tabs, strides, o = [], [], _align8(len(items) * isz)
+    dev = _check_items(items, "flat_remap", "page")
+    cn = _check_channels(items, "flat_remap")
+    tabs, strides = [], []
     for i, (src, dst, kind, m, lines) in enumerate(items):
         what = f"flat_remap: page {i}"
         _dense_u8(src, dev, cn, f"{what}: src")
@@ -1520,27 +1525,19 @@ def flat_remap(items, tables=False):
             raise ValueError(f"{what}: a column meets {stride} lines, over the {FLAT_MAX_COLUMN_LINES} a column may hold")
         tabs.append(t)
         strides.append(max(1, stride))
-    los = list(itertools.accumulate((8 * t.size for t in tabs), initial=o))     # the records, then every line table
-    o = _align8(los[-1])
-    offs = []
-    for (_, dst, *_), lo, stride in zip(items, los, strides):             # then each page's column table and (Y, M) pairs
-        dw = dst.shape[1]
-        co = o
-        fo = _align8(co + 12 * dw)
-        o = fo + 16 * dw * stride
-        offs.append((lo, co, fo))
-    buf = torch.empty(o, dtype=torch.uint8, device=dev)
-    base, recs, mx, mw = buf.data_ptr(), [], 0, 0
+    pack = _Pack()                  # the records, then every line table, then each page's column table and (Y, M) pairs
+    pack.area(len(items) * ctypes.sizeof(_lib.FlatPage))
+    los = [pack.area(8 * t.size, 8) for t in tabs]
+    offs = [(lo, pack.area(12 * d.shape[1], 8), pack.area(16 * d.shape[1] * stride, 8))
+            for (_, d, *_), lo, stride in zip(items, los, strides)]
+    base, recs, mx, mw = pack.alloc(dev), [], 0, 0
     for (src, dst, kind, m, _), t, stride, (lo, co, fo) in zip(items, tabs, strides, offs):
         (h, w), (dh, dw) = src.shape[:2], dst.shape[:2]
         recs.append(_lib.FlatPage(src.data_ptr(), src.stride(0), h, w, dst.data_ptr(), dst.stride(0), dh, dw, base + lo, base + co,
                                   base + fo, len(t), stride, _lib.FLAT_RECT if kind == "rect" else _lib.FLAT_QUAD, 0,
                                   (ctypes.c_double * 8)(*[float(v) for v in m])))
         mx, mw = max(mx, dh * dw), max(mw, dw)
-    host = bytearray(los[0])
-    host[:len(items) * isz] = bytes((_lib.FlatPage * len(recs))(*recs))
-    host += b"".join(t.tobytes() for t in tabs)
-    buf[:len(host)].copy_(torch.frombuffer(host, dtype=torch.uint8))
+    buf = pack.upload((0, bytes((_lib.FlatPage * len(recs))(*recs))), (los[0], b"".join(t.tobytes() for t in tabs)))
     lib = _lib.load()
     _lib.check(lib.mn_flat_columns_batched(base, len(recs), mw, _stream()), "mn_flat_columns_batched")
     _lib.check(lib.mn_flat_remap_u8_batched(base, len(recs), cn, mx, _stream()), "mn_flat_remap_u8_batched")
@@ -1571,15 +1568,10 @@ def even_light(items, inks=None):
     frame and polarity are ignored and the call takes four launches.  Returns the int32 CUDA tensor [n, 4] of every page's
     (0, threshold, ink, 0), whose rows an evening of the same pages may take as ``inks``; None when ``inks`` is given."""
     global LAUNCHES
-    if not items:
-        raise ValueError("even_light: no pages")
-    if len(items) > 65535:
-        raise ValueError("even_light: at most 65535 pages per launch")
+    dev = _check_items(items, "even_light", "page", 1)
     if inks is not None and len(inks) != len(items):
         raise ValueError("even_light: one ink per page")
-    dev = items[0][1].device
     n = len(items)
-    rsz, lsz = ctypes.sizeof(_lib.TextBlock), ctypes.sizeof(_lib.LightPage)
     tiles, lines = 1, 1
     for i, (frame, src, dst, k, polarity) in enumerate(items):
         what = f"even_light: page {i}"
@@ -1599,18 +1591,18 @@ def even_light(items, inks=None):
                   and inks[i].numel() == 4 and inks[i].is_contiguous()):
             raise ValueError(f"{what}: an ink must be an int32 CUDA view of 4 values on {dev}")
         lines = max(lines, h * -(-w // k), w * -(-h // k))
-    planes = [_align8(3 * src.shape[0] * src.shape[1]) for _, src, *_ in items]
-    o_rec = n * rsz
-    o_work = _align8(o_rec + n * lsz)
-    o_planes = o_work + (1024 * n if inks is None else 0)
-    buf = torch.empty(o_planes + 2 * sum(planes), dtype=torch.uint8, device=dev)
-    base = buf.data_ptr()
+    pack = _Pack()                  # the crop records, the page records, the threshold work, then each page's two planes
+    pack.area(n * ctypes.sizeof(_lib.TextBlock))
+    o_rec = pack.area(n * ctypes.sizeof(_lib.LightPage))
+    o_work = pack.area(1024 * n if inks is None else 0, 8)
+    planes = [[pack.area(3 * src.shape[0] * src.shape[1], 8) for _ in range(2)] for _, src, *_ in items]
+    base = pack.alloc(dev)
     if inks is None:                # apart from the work, so that the scratch planes are freed with the call
         table = torch.zeros(n, 4, dtype=torch.int32, device=dev)
         inks, threshold = table.unbind(0), 1
     else:
         threshold = 0
-    blocks, recs, o = [], [], base + o_planes
+    blocks, recs = [], []
     for i, ((frame, src, dst, k, polarity), pl) in enumerate(zip(items, planes)):
         if threshold:
             fh, fw = frame.shape[:2]
@@ -1620,10 +1612,8 @@ def even_light(items, inks=None):
             tb = _lib.TextBlock(0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, inks[i].data_ptr())
         blocks.append(tb)
         recs.append(_lib.LightPage(tb, src.data_ptr(), src.stride(0), dst.data_ptr(), dst.stride(0), src.shape[0], src.shape[1], k, 0,
-                                   o, o + pl))
-        o += 2 * pl
-    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.LightPage * n)(*recs))
-    buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+                                   base + pl[0], base + pl[1]))
+    pack.upload((0, bytes((_lib.TextBlock * n)(*blocks))), (o_rec, bytes((_lib.LightPage * n)(*recs))))
     if threshold:
         _lib.check(_lib.load().mn_even_light_u8(base, base + o_rec, n, 1, tiles, lines, base + o_work, 1024 * n, _stream()),
                    "mn_even_light_u8")
@@ -1637,7 +1627,7 @@ def even_light(items, inks=None):
 def even_light_bytes(w, h, frame=None):
     """Device bytes of evening a w x h page beyond the page itself: its two scratch planes and, when ``frame`` (w_f, h_f) is
     given, the evened frame the page's searches read."""
-    n = 2 * _align8(3 * w * h) + 1024 + 16
+    n = 2 * (-(-3 * w * h // 8) * 8) + 1024 + 16
     if frame is not None:
         n += 3 * frame[0] * frame[1]
     return n
@@ -1658,12 +1648,8 @@ def composite_regions_curved(regions, feather):
             if not t[0] >= 1:
                 raise ValueError(f"composite_regions_curved: region {i}: scale {t[0]} < 1")
             tables[i] = (t, k)
-    n_tab = sum(t.size for t, _ in tables.values())
-    recs, chains, mx, buf = _region_records(regions, int(feather), "composite_regions_curved", _lib.RegionCurved,
-                                            extra=8 + 8 * n_tab)
-    isz = ctypes.sizeof(_lib.RegionCurved)
-    head = len(regions) * isz + 4 * max(1, len(chains))
-    t_off = _align8(buf.data_ptr() + head) - buf.data_ptr()
+    recs, mx, pack, chains, t_off = _region_records(regions, int(feather), "composite_regions_curved", _lib.RegionCurved,
+                                                    tables=8 * sum(t.size for t, _ in tables.values()))
     out, o = [], 0
     for i, (r, rec) in enumerate(zip(regions, recs)):
         maps = r[4]
@@ -1676,7 +1662,7 @@ def composite_regions_curved(regions, feather):
         if i in tables:
             t, k = tables[i]
             out.append(_lib.RegionCurved(_lib.RegionQuad(rec, _lib.REGION_CURVED, kx, ky, 0, (ctypes.c_double * 9)()),
-                                         buf.data_ptr() + t_off + 8 * o, k, 0))
+                                         pack.buf.data_ptr() + t_off + 8 * o, k, 0))
             o += t.size
             continue
         n = [float(v) for row in n for v in row]
@@ -1684,11 +1670,8 @@ def composite_regions_curved(regions, feather):
             raise ValueError(f"composite_regions_curved: region {i}: expected (N 2 x 3 or 3 x 3, kx, ky) or (CurveTable, kx, ky)")
         kind = _lib.REGION_AFFINE if len(n) == 6 else _lib.REGION_PERSPECTIVE
         out.append(_lib.RegionCurved(_lib.RegionQuad(rec, kind, kx, ky, 0, (ctypes.c_double * 9)(*n)), None, 0, 0))
-    host = bytes((_lib.RegionCurved * len(out))(*out)) + np.asarray(chains or [0], dtype=np.int32).tobytes()
-    host += bytes(t_off - head)
-    if tables:
-        host += np.concatenate([tables[i][0] for i in sorted(tables)]).tobytes()
-    buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    buf = pack.upload((0, bytes((_lib.RegionCurved * len(out))(*out))), chains,
+                      (t_off, b"".join(tables[i][0].tobytes() for i in sorted(tables))))
     _lib.check(_lib.load().mn_composite_regions_curved_u8(_ptr(buf), len(out), mx, _stream()), "mn_composite_regions_curved_u8")
     LAUNCHES += 1
 
@@ -1697,11 +1680,7 @@ def _vertical_gather(items, what, width, symbol):
     """One launch of ``symbol`` over vertical_layout's / vertical_unlayout's items, ``width`` int32 values per cell."""
     import numpy as np
     global LAUNCHES
-    if not items:
-        raise ValueError(f"{what}: no columns")
-    if len(items) > 65535:
-        raise ValueError(f"{what}: at most 65535 columns per launch")
-    dev = items[0][0].device
+    dev = _check_items(items, what, "column")
     tables = []
     for i, (src, dst, cells) in enumerate(items):
         _dense_u8(src, dev, 3, f"{what}: column {i}: src")
@@ -1718,18 +1697,17 @@ def _vertical_gather(items, what, width, symbol):
         if not ok or t.max() >= 2 ** 31:
             raise ValueError(f"{what}: column {i}: its cell table reads outside the {sh}x{sw} source")
         tables.append(t.astype(np.int32))
-    isz = ctypes.sizeof(_lib.VerticalColumn)
-    n_int = sum(t.size for t in tables)
-    buf = torch.empty(len(items) * isz + 4 * n_int, dtype=torch.uint8, device=dev)
-    base, o, recs, mx = buf.data_ptr() + len(items) * isz, 0, [], 0
+    pack = _Pack()
+    pack.area(len(items) * ctypes.sizeof(_lib.VerticalColumn))
+    t_off = pack.area(4 * sum(t.size for t in tables))
+    base, o, recs, mx = pack.alloc(dev) + t_off, 0, [], 0
     for (src, dst, _), t in zip(items, tables):
         dh, dw = dst.shape[:2]
         recs.append(_lib.VerticalColumn(src.data_ptr(), src.stride(0), dst.data_ptr(), dst.stride(0), base + 4 * o, dh, dw, len(t),
                                         dw // len(t) if width == 3 else 0))
         o += t.size
         mx = max(mx, dh * dw)
-    host = bytes((_lib.VerticalColumn * len(recs))(*recs)) + b"".join(t.tobytes() for t in tables)
-    buf.copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    buf = pack.upload((0, bytes((_lib.VerticalColumn * len(recs))(*recs))), (t_off, b"".join(t.tobytes() for t in tables)))
     _lib.check(getattr(_lib.load(), symbol)(_ptr(buf), len(recs), mx, _stream()), symbol)
     LAUNCHES += 1
 
@@ -1797,15 +1775,6 @@ def skew_block_dtype():
                      ("u_min", "<f8"), ("v_min", "<f8"), ("c", "<f8"), ("s", "<f8")])
 
 
-def _check_items(items, what, noun):
-    """The device of a layout call's items, after checking their number (one launch holds 1 to 65535)."""
-    if not items:
-        raise ValueError(f"{what}: no {noun}s")
-    if len(items) > 65535:
-        raise ValueError(f"{what}: at most 65535 {noun}s per launch")
-    return items[0][0].device
-
-
 def _check_crop(item, dev, what, knob_names):
     """(x0, y0, w, h) of a layout item (img, rect, vertical, polarity, *knobs), validated as find_lines and find_blocks describe
     it.  Raises naming ``what``."""
@@ -1849,19 +1818,6 @@ def _skew_block(tb, table, scores, profiles, n_ang, stride):
     return _lib.SkewBlock(tb, table, scores if n_ang > 1 else 0, profiles if n_ang > 1 else 0, n_ang, stride)
 
 
-def _line_areas(sizes):
-    """The int32 areas of the line kernels for blocks of ``sizes`` (L bins, extra values) each: every block's work (a 256-bin
-    histogram, 3 L profile values, then the extra values), which the call zeroes, followed by every block's scratch of 2 L + 4
-    values.  Returns per block the byte offsets (hist, prof, scratch), the bytes of the work and those of the whole."""
-    n_work = sum(256 + 3 * L + e for L, e in sizes)
-    out, w, s = [], 0, n_work
-    for L, e in sizes:
-        out.append((4 * w, 4 * (w + 256), 4 * s))
-        w += 256 + 3 * L + e
-        s += 2 * L + 4
-    return out, 4 * n_work, 4 * s
-
-
 def find_lines(blocks, scores=False):
     """Text blocks split into lines, every block in four launches whatever their number (mn_find_lines_u8; DESIGN.md 7b, "Text
     blocks").  blocks: list of (img, rect, vertical, polarity, min_ink, gap, min_height[, skew, max_skew]): img a uint8 [H, W, 3]
@@ -1894,33 +1850,35 @@ def find_lines(blocks, scores=False):
         tables.append(cs)
         dims.append((x0, y0, bw, bh, len(cs), stride))
     tab, t_offs = _angle_tables(tables) if skewed else (b"", [0] * n)
-    n_scores = sum(d[4] for d in dims if d[4] > 1)
-    areas, n_work, n_areas = _line_areas([(d[5], d[4] * d[5] if d[4] > 1 else 0) for d in dims])
-    head = n * (osz + ssz + rsz) + len(tab)             # results, skew records, crop records, tables; scores; work; scratch
-    buf = torch.empty(head + 8 * n_scores + n_areas, dtype=torch.uint8, device=dev)
-    base = buf.data_ptr()
-    sk, seg, w32 = base + n * osz, base + n * (osz + ssz), base + head + 8 * n_scores
-    recs, srecs, views, o, tiles = [], [], [], 0, 0
-    for i, (blk, (x0, y0, bw, bh, n_ang, stride), (hist, prof, scr), t) in enumerate(zip(blocks, dims, areas, t_offs)):
+    pack = _Pack()                  # results, skew records, crop records, tables; scores, work (zeroed); scratch
+    pack.area(n * osz)
+    sk, seg, t_off = pack.area(n * ssz), pack.area(n * rsz), pack.area(len(tab))
+    score = [pack.area(8 * n_ang if n_ang > 1 else 0) for *_, n_ang, _ in dims]
+    work = [(pack.area(4 * 256), pack.area(4 * 3 * L), pack.area(4 * n_ang * L if n_ang > 1 else 0)) for *_, n_ang, L in dims]
+    w_end = pack.end
+    scratch = [pack.area(4 * (2 * L + 4)) for *_, L in dims]
+    base = pack.alloc(dev)
+    recs, srecs, views, tiles = [], [], [], 0
+    for i, (blk, (x0, y0, bw, bh, n_ang, stride), sc, (hist, prof, ext), scr, t) in \
+            enumerate(zip(blocks, dims, score, work, scratch, t_offs)):
         img, _, vertical, polarity, min_ink, gap, min_height = blk[:7]
         tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, min_ink or 0, gap or 0,
-                            min_height or 0, 0, w32 + hist, w32 + prof, w32 + scr, base + i * osz)
+                            min_height or 0, 0, base + hist, base + prof, base + scr, base + i * osz)
         recs.append(tb)
         if skewed:
-            srecs.append(_skew_block(tb, seg + n * rsz + 16 * t, base + head + 8 * o, w32 + prof + 4 * 3 * stride, n_ang, stride))
-        views.append(buf[head + 8 * o:head + 8 * (o + n_ang)].view(torch.int64) if n_ang > 1 else None)
-        o += n_ang if n_ang > 1 else 0
+            srecs.append(_skew_block(tb, base + t_off + 16 * t, base + sc, base + ext, n_ang, stride))
+        views.append(pack.buf[sc:sc + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
-    host = bytes((_lib.SkewBlock * len(srecs))(*srecs)) + bytes((_lib.TextBlock * n)(*recs)) + tab
-    buf[n * osz:head].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
+    pack.upload((sk, bytes((_lib.SkewBlock * len(srecs))(*srecs))), (seg, bytes((_lib.TextBlock * n)(*recs))), (t_off, tab))
     if skewed:
-        _lib.check(_lib.load().mn_find_lines_skewed_u8(seg, sk, n, tiles, base + head, 8 * n_scores + n_work, _stream()),
-                   "mn_find_lines_skewed_u8")
+        _lib.check(_lib.load().mn_find_lines_skewed_u8(base + seg, base + sk, n, tiles, base + score[0], w_end - score[0],
+                                                       _stream()), "mn_find_lines_skewed_u8")
         LAUNCHES += 6
     else:
-        _lib.check(_lib.load().mn_find_lines_u8(seg, n, tiles, base + head, n_work, _stream()), "mn_find_lines_u8")
+        _lib.check(_lib.load().mn_find_lines_u8(base + seg, n, tiles, base + score[0], w_end - score[0], _stream()),
+                   "mn_find_lines_u8")
         LAUNCHES += 4
-    res = buf[:n * (osz + ssz)]
+    res = pack.buf[:n * (osz + ssz)]
     return (res, views) if scores else res
 
 
@@ -1963,23 +1921,25 @@ def find_lines_window(blocks):
             raise ValueError(f"{what}: window {(c0, l0, c1, l1)} is empty or outside the {int(M)}x{int(L)} frame")
         fp = window_footprint(bw, bh, vertical, c, s, u_min, v_min, (c0, l0, c1, l1))
         dims.append((x0, y0, bw, bh, c, s, (c0, l0, c1, l1), fp))
-    areas, n_work, n_areas = _line_areas([(d[6][3] - d[6][1], 0) for d in dims])
-    head = n * (osz + rsz + wsz)
-    buf = torch.empty(head + n_areas, dtype=torch.uint8, device=dev)
-    out, seg, wrec = buf.data_ptr(), buf.data_ptr() + n * osz, buf.data_ptr() + n * (osz + rsz)
-    work = buf.data_ptr() + head
+    pack = _Pack()                  # results, line records, window records; work (zeroed); scratch
+    pack.area(n * osz)
+    seg, wrec = pack.area(n * rsz), pack.area(n * wsz)
+    work = [(pack.area(4 * 256), pack.area(4 * 3 * (d[6][3] - d[6][1]))) for d in dims]
+    w_end = pack.end
+    scratch = [pack.area(4 * (2 * (d[6][3] - d[6][1]) + 4)) for d in dims]
+    base = pack.alloc(dev)
     recs, wrecs, tiles = [], [], 0
-    for i, (blk, (x0, y0, bw, bh, c, s, (c0, l0, c1, l1), (px0, py0, px1, py1)), (hist, prof, scr)) in \
-            enumerate(zip(blocks, dims, areas)):
+    for i, (blk, (x0, y0, bw, bh, c, s, (c0, l0, c1, l1), (px0, py0, px1, py1)), (hist, prof), scr) in \
+            enumerate(zip(blocks, dims, work, scratch)):
         img, _, vertical, polarity, min_ink, gap, min_height = blk[:7]
-        knobs = (polarity, min_ink or 0, gap or 0, min_height or 0, 0, work + hist, work + prof, work + scr, out + i * osz)
+        knobs = (polarity, min_ink or 0, gap or 0, min_height or 0, 0, base + hist, base + prof, base + scr, base + i * osz)
         recs.append(_lib.TextBlock(img.data_ptr(), img.stride(0), 0, 0, c1 - c0, l1 - l0, 0, *knobs))
         crop = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), *knobs)
         wrecs.append(_lib.WindowBlock(crop, c, s, c0, l0, c1, l1, px0, py0, px1 - px0, py1 - py0))
         tiles = max(tiles, 1, -(-(px1 - px0) // 32) * -(-(py1 - py0) // 32))
-    host = bytes((_lib.TextBlock * n)(*recs)) + bytes((_lib.WindowBlock * n)(*wrecs))
-    buf[n * osz:head].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
-    _lib.check(_lib.load().mn_find_lines_window_u8(seg, wrec, n, tiles, work, n_work, _stream()), "mn_find_lines_window_u8")
+    buf = pack.upload((seg, bytes((_lib.TextBlock * n)(*recs))), (wrec, bytes((_lib.WindowBlock * n)(*wrecs))))
+    _lib.check(_lib.load().mn_find_lines_window_u8(base + seg, base + wrec, n, tiles, base + work[0][0], w_end - work[0][0],
+                                                   _stream()), "mn_find_lines_window_u8")
     LAUNCHES += 4
     return buf[:n * osz]
 
@@ -1995,16 +1955,17 @@ def curve_strips(w, strips=None):
     return int(strips) if strips is not None else min(CURVE_MAX_STRIPS, max(1, w // 48))
 
 
-def _curve_ints(h, n_s):
-    """(work, scratch) int32 values of one curled block: the zeroed histogram, profile, strip profiles and run counts; then the
-    segmentation scratch of the block and of each strip, the run table and the link state."""
-    return 256 + 3 * h + 3 * n_s * h + n_s, (2 * h + 4) * (1 + n_s) + 11 * _lib.CURVE_RUN_CAP * n_s
+def _curve_areas(h, n_s):
+    """Byte sizes of one curled block's int32 areas: its work (histogram, profile, strip profiles, run counts), which the call
+    zeroes, and its scratch (segmentation scratch of the block and of its strips, run table, link state)."""
+    cap = _lib.CURVE_RUN_CAP
+    return [4 * 256, 4 * 3 * h, 4 * 3 * n_s * h, 4 * n_s], [4 * (2 * h + 4), 4 * n_s * (2 * h + 4), 4 * 4 * cap * n_s, 4 * 7 * cap * n_s]
 
 
 def curve_block_bytes(w, h, strips=None):
     """Device bytes of one curled block of w x h pixels in a find_lines_curved call: its records, work and scratch."""
-    work, scratch = _curve_ints(h, curve_strips(w, strips))
-    return 4 * (work + scratch) + sum(ctypes.sizeof(t) for t in (_lib.BlockLines, _lib.CurveLines, _lib.TextBlock, _lib.CurveBlock))
+    work, scratch = _curve_areas(h, curve_strips(w, strips))
+    return sum(work + scratch) + sum(ctypes.sizeof(t) for t in (_lib.BlockLines, _lib.CurveLines, _lib.TextBlock, _lib.CurveBlock))
 
 
 def curve_lines_dtype():
@@ -2040,38 +2001,35 @@ def find_lines_curved(blocks, tables=False):
         if total > CURVE_MAX_WORK:
             raise ValueError(f"{what}: the blocks up to this one need {total} bytes, over the {CURVE_MAX_WORK} a call may use")
         dims.append((x0, y0, bw, bh, n_s))
-    sizes = [_curve_ints(d[3], d[4]) for d in dims]
-    n_work, n_scr = sum(s[0] for s in sizes), sum(s[1] for s in sizes)
-    head = n * (osz + csz + rsz + bsz)
-    buf = torch.empty(head + 4 * (n_work + n_scr), dtype=torch.uint8, device=dev)
-    base = buf.data_ptr()
-    seg, crec, work = base + n * (osz + csz), base + n * (osz + csz + rsz), base + head
-    recs, crecs, views, w, s, tiles = [], [], [], 0, n_work, 0
+    pack = _Pack()                  # results, link tables, line records, curve records; work (zeroed); scratch
+    pack.area(n * osz)
+    pack.area(n * csz)
+    seg, crec = pack.area(n * rsz), pack.area(n * bsz)
+    areas = [_curve_areas(d[3], d[4]) for d in dims]
+    work = [[pack.area(a) for a in w] for w, _ in areas]
+    w_end = pack.end
+    scratch = [[pack.area(a) for a in s] for _, s in areas]
+    base = pack.alloc(dev)
+    recs, crecs, views, tiles = [], [], [], 0
     cap = _lib.CURVE_RUN_CAP
-    for i, (blk, (x0, y0, bw, bh, n_s)) in enumerate(zip(blocks, dims)):
+    for i, (blk, (x0, y0, bw, bh, n_s), (hist, prof, sprof, nruns), (scr, sscr, runs, link)) in \
+            enumerate(zip(blocks, dims, work, scratch)):
         img, _, polarity, min_ink, gap, min_height, _ = blk
-        hist, prof, sprof, nruns = w, w + 256, w + 256 + 3 * bh, w + 256 + 3 * bh + 3 * n_s * bh
-        scr, sscr = s, s + 2 * bh + 4
-        runs = sscr + n_s * (2 * bh + 4)
-        link = runs + 4 * cap * n_s
         tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, 0, polarity, min_ink or 0, gap or 0, min_height or 0,
-                            0, work + 4 * hist, work + 4 * prof, work + 4 * scr, base + i * osz)
+                            0, base + hist, base + prof, base + scr, base + i * osz)
         recs.append(tb)
-        crecs.append(_lib.CurveBlock(tb, work + 4 * sprof, work + 4 * nruns, work + 4 * runs, work + 4 * sscr, work + 4 * link,
+        crecs.append(_lib.CurveBlock(tb, base + sprof, base + nruns, base + runs, base + sscr, base + link,
                                      base + n * osz + i * csz, n_s))
         if tables:
-            i32 = buf[head:].view(torch.int32)
-            views.append(dict(profiles=i32[sprof:sprof + 3 * n_s * bh].view(n_s, 3, bh), nruns=i32[nruns:nruns + n_s],
-                              runs=i32[runs:runs + 4 * cap * n_s].view(n_s, cap, 4)))
-        w += sizes[i][0]
-        s += sizes[i][1]
+            views.append(dict(profiles=pack.buf[sprof:sprof + 12 * n_s * bh].view(torch.int32).view(n_s, 3, bh),
+                              nruns=pack.buf[nruns:nruns + 4 * n_s].view(torch.int32),
+                              runs=pack.buf[runs:runs + 16 * cap * n_s].view(torch.int32).view(n_s, cap, 4)))
         tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
-    host = bytes((_lib.TextBlock * n)(*recs)) + bytes((_lib.CurveBlock * n)(*crecs))
-    buf[n * (osz + csz):head].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
-    _lib.check(_lib.load().mn_find_lines_curved_u8(seg, crec, n, tiles, max(d[4] for d in dims), work, 4 * n_work, _stream()),
-               "mn_find_lines_curved_u8")
+    pack.upload((seg, bytes((_lib.TextBlock * n)(*recs))), (crec, bytes((_lib.CurveBlock * n)(*crecs))))
+    _lib.check(_lib.load().mn_find_lines_curved_u8(base + seg, base + crec, n, tiles, max(d[4] for d in dims), base + work[0][0],
+                                                   w_end - work[0][0], _stream()), "mn_find_lines_curved_u8")
     LAUNCHES += 7
-    res = buf[:n * (osz + csz)]
+    res = pack.buf[:n * (osz + csz)]
     return (res, views) if tables else res
 
 
@@ -2239,50 +2197,45 @@ def find_blocks(pages, scores=False):
     if need > PAGE_MAX_WORK:
         raise ValueError(f"find_blocks: the pages need more than the {PAGE_MAX_WORK} bytes of work memory a call may use")
     tab, t_offs = _angle_tables(tables) if skewed else (b"", [0] * n)
-    pg0, tab0 = n * bsz, n * (bsz + psz)                 # records, tables and the skew records, then the results and leaves,
-    out0 = -(-(tab0 + len(tab) + n * ssz) // 16) * 16    # then the work: the call zeroes everything from out0 on, and the
-    sk0 = out0 - n * ssz                                 # skew records come back with the results in one copy
-    n_figs = sum(p.figure_size is not None for p in pages)
-    n_pans = sum(p.panel_size is not None for p in pages)
-    n_out = n * rsz + 12 * (sum(d[4] for d in dims) + _lib.PAGE_MAX_FIGURES * n_figs + _lib.PAGE_MAX_PANELS * n_pans)
-    work0 = out0 + -(-n_out // 16) * 16
-    per = [-(-sum(a) // 16) * 16 for a in areas]
-    buf = torch.empty(work0 + sum(per), dtype=torch.uint8, device=dev)
-    base = buf.data_ptr()
-    leaves, w, blocks, srecs, recs, views, tiles = base + out0 + n * rsz, base + work0, [], [], [], [], 0
-    ftab = leaves + 12 * sum(d[4] for d in dims)         # the figure pages' tables follow every leaf table,
-    ptab = ftab + 12 * _lib.PAGE_MAX_FIGURES * n_figs    # and the panel pages' tables follow those
-    for i, (p, (x0, y0, bw, bh, cap, M, n_ang, stride, (rules, figures, panels)), a, nb, t) in \
-            enumerate(zip(pages, dims, areas, per, t_offs)):
-        _, hist, lines, bits, lists, counts, prof, rbits, fbits, pbits = itertools.accumulate([w] + a[:-1])
-        tb = _lib.TextBlock(p.img.data_ptr(), p.img.stride(0), x0, y0, bw, bh, int(bool(p.vertical)), p.polarity, 0, 0, 0, 0, hist,
-                            0, 0, lines)
+    pack = _Pack()                  # records, tables and the skew records, which come back with the results in one copy; then
+    pack.area(n * bsz)              # the results, leaves, figure and panel tables and each page's work, which the call zeroes
+    pg, t_off = pack.area(n * psz), pack.area(len(tab))
+    pack.area(n * ssz)
+    out0 = pack.area(n * rsz, 16)
+    sk0 = out0 - n * ssz            # the skew records end where the results begin
+    leaves = [pack.area(12 * d[4]) for d in dims]
+    figs = [pack.area(12 * _lib.PAGE_MAX_FIGURES) if d[8][1] else None for d in dims]
+    pans = [pack.area(12 * _lib.PAGE_MAX_PANELS) if d[8][2] else None for d in dims]
+    out1 = pack.end
+    work = [[pack.area(a[0], 16)] + [pack.area(s) for s in a[1:]] for a in areas]
+    base = pack.alloc(dev)
+    blocks, srecs, recs, views, tiles = [], [], [], [], 0
+    for i, (p, (x0, y0, bw, bh, cap, M, n_ang, stride, (rules, figures, panels)), wk, lv, f, pn, t) in \
+            enumerate(zip(pages, dims, work, leaves, figs, pans, t_offs)):
+        sc, hist, lines, bits, lists, counts, prof, rbits, fbits, pbits = (base + o for o in wk)
+        tb = _lib.TextBlock(p.img.data_ptr(), p.img.stride(0), x0, y0, bw, bh, int(bool(p.vertical)), p.polarity, 0, 0, 0, 0,
+                            hist, 0, 0, lines)
         blocks.append(tb)
         if skewed:
-            srecs.append(_skew_block(tb, base + tab0 + 16 * t, w, prof, n_ang, stride))
-        recs.append(_lib.TextPage(tb, bits, (ctypes.c_void_p * 2)(lists, lists + 12 * cap), leaves, counts, counts + 4 * cap,
+            srecs.append(_skew_block(tb, base + t_off + 16 * t, sc, prof, n_ang, stride))
+        recs.append(_lib.TextPage(tb, bits, (ctypes.c_void_p * 2)(lists, lists + 12 * cap), base + lv, counts, counts + 4 * cap,
                                   counts + 8 * cap, base + out0 + i * rsz, -(-M // 32), cap, p.gap_x or 0, p.gap_y or 0,
                                   rbits=rbits if rules else pbits if panels else None, rule_length=p.rule_length or 0,
-                                  fbits=fbits if figures else None, figs=ftab if figures else None,
+                                  fbits=fbits if figures else None, figs=base + f if figures else None,
                                   figure_size=p.figure_size or 0, dirs=int(bool(p.directions)),
-                                  pans=ptab if panels else None, panel_size=p.panel_size or 0))
-        ftab += 12 * _lib.PAGE_MAX_FIGURES if figures else 0
-        ptab += 12 * _lib.PAGE_MAX_PANELS if panels else 0
-        views.append(buf[w - base:w - base + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
-        leaves += 12 * cap
-        w += nb
+                                  pans=base + pn if panels else None, panel_size=p.panel_size or 0))
+        views.append(pack.buf[wk[0]:wk[0] + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
-    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.TextPage * n)(*recs)) + tab
-    host += bytes(sk0 - len(host)) + bytes((_lib.SkewBlock * len(srecs))(*srecs))
-    buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
-    ruled, figured, directed, paneled = (any(p.rule_length is not None for p in pages), n_figs > 0,
-                                         any(p.directions for p in pages), n_pans > 0)
+    buf = pack.upload((0, bytes((_lib.TextBlock * n)(*blocks))), (pg, bytes((_lib.TextPage * n)(*recs))), (t_off, tab),
+                      (sk0, bytes((_lib.SkewBlock * len(srecs))(*srecs))))
+    ruled, figured, directed, paneled = (any(p.rule_length is not None for p in pages), any(f is not None for f in figs),
+                                         any(p.directions for p in pages), any(pn is not None for pn in pans))
     flags = ((_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0) | (_lib.PAGE_DIRECTIONS if directed else 0)
              | (_lib.PAGE_PANELS if paneled else 0))
     entry, head = ("mn_find_blocks_skewed_u8", (base, base + sk0)) if skewed else ("mn_find_blocks_u8", (base,))
-    _lib.check(getattr(_lib.load(), entry)(*head, base + pg0, n, tiles, flags, base + out0, len(buf) - out0, _stream()), entry)
+    _lib.check(getattr(_lib.load(), entry)(*head, base + pg, n, tiles, flags, base + out0, len(buf) - out0, _stream()), entry)
     LAUNCHES += (7 if skewed else 5) + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed + 2 * paneled
-    res = buf[sk0:out0 + n_out], [d[4] for d in dims]
+    res = buf[sk0:out1], [d[4] for d in dims]
     return res + (views,) if scores else res
 
 
@@ -2368,37 +2321,35 @@ def find_page_quads(pages, hulls=False, labels=False, spreads=()):
     if (sum(quad_page_bytes(img.shape[1], img.shape[0]) for img, _ in pages)
             + sum(spine_page_bytes(pages[k][0].shape[1]) for k in spreads) > PAGE_MAX_WORK):
         raise ValueError(f"find_page_quads: the pages need more than the {PAGE_MAX_WORK} bytes of work memory a call may use")
-    out0 = -(-(n * (bsz + psz) + m * ssz) // 16) * 16     # records, then the results and the work, which the call zeroes
-    work0 = out0 + -(-(n * rsz + m * spsz) // 16) * 16
-    areas = [_quad_areas(img.shape[1], img.shape[0]) for img, _ in pages]
-    cols = [-(-8 * pages[k][0].shape[1] // 16) * 16 for k in spreads]
-    buf = torch.empty(work0 + sum(map(sum, areas)) + sum(cols), dtype=torch.uint8, device=dev)
-    base = buf.data_ptr()
-    blocks, recs, views, lviews, w, tiles = [], [], [], [], base + work0, 0
-    for i, ((img, polarity), sizes) in enumerate(zip(pages, areas)):
+    pack = _Pack()                  # records; then the results and the work, which the call zeroes
+    pack.area(n * bsz)
+    qp, sp = pack.area(n * psz), pack.area(m * ssz)
+    out0, sres = pack.area(n * rsz, 16), pack.area(m * spsz)
+    work = [[pack.area(s, 16) for s in _quad_areas(img.shape[1], img.shape[0])] for img, _ in pages]
+    cols = [pack.area(8 * pages[k][0].shape[1], 16) for k in spreads]
+    base = pack.alloc(dev)
+    blocks, recs, views, lviews, tiles = [], [], [], [], 0
+    for i, ((img, polarity), (hist, lines, best, ext, label, count, hull)) in enumerate(zip(pages, work)):
         h_, w_ = img.shape[:2]
-        hist, lines, best, ext, label, count, hull = itertools.accumulate([w] + sizes[:-1])
-        tb = _lib.TextBlock(img.data_ptr(), img.stride(0), 0, 0, w_, h_, 0, polarity, 0, 0, 0, 0, hist, 0, 0, lines)
+        tb = _lib.TextBlock(img.data_ptr(), img.stride(0), 0, 0, w_, h_, 0, polarity, 0, 0, 0, 0, base + hist, 0, 0, base + lines)
         blocks.append(tb)
-        recs.append(_lib.QuadPage(tb, label, count, ext, best, hull, base + out0 + i * rsz))
-        views.append(buf[hull - base:hull - base + sizes[-1]].view(torch.int32).view(-1, 2))
-        lviews.append((buf[label - base:label - base + 4 * h_ * w_].view(torch.int32).view(h_, w_),
-                       buf[count - base:count - base + 4 * h_ * w_].view(torch.int32)))
-        w += sum(sizes)
+        recs.append(_lib.QuadPage(tb, base + label, base + count, base + ext, base + best, base + hull, base + out0 + i * rsz))
+        views.append(pack.buf[hull:hull + 8 * (4 * h_ + 8)].view(torch.int32).view(-1, 2))
+        lviews.append((pack.buf[label:label + 4 * h_ * w_].view(torch.int32).view(h_, w_),
+                       pack.buf[count:count + 4 * h_ * w_].view(torch.int32)))
         tiles = max(tiles, -(-w_ // 32) * -(-h_ // 32))
-    spines = [_lib.SpinePage(base + n * bsz + k * psz, c, base + out0 + n * rsz + j * spsz)
-              for j, (k, c) in enumerate(zip(spreads, itertools.accumulate([w] + cols[:-1])))]
-    host = bytes((_lib.TextBlock * n)(*blocks)) + bytes((_lib.QuadPage * n)(*recs)) + bytes((_lib.SpinePage * m)(*spines))
-    buf[:len(host)].copy_(torch.frombuffer(bytearray(host), dtype=torch.uint8))
-    _lib.check(_lib.load().mn_find_page_quads_u8(base, base + n * bsz, n, tiles, base + out0, len(buf) - out0, _stream()),
+    spines = [_lib.SpinePage(base + qp + k * psz, base + c, base + sres + j * spsz) for j, (k, c) in enumerate(zip(spreads, cols))]
+    buf = pack.upload((0, bytes((_lib.TextBlock * n)(*blocks))), (qp, bytes((_lib.QuadPage * n)(*recs))),
+                      (sp, bytes((_lib.SpinePage * m)(*spines))))
+    _lib.check(_lib.load().mn_find_page_quads_u8(base, base + qp, n, tiles, base + out0, len(buf) - out0, _stream()),
                "mn_find_page_quads_u8")
     LAUNCHES += 8
     res = buf[out0:out0 + n * rsz]
     if spreads:
         stiles = max(-(-pages[k][0].shape[1] // 32) * -(-pages[k][0].shape[0] // 32) for k in spreads)
-        _lib.check(_lib.load().mn_find_page_spines_u8(base + n * (bsz + psz), m, stiles, _stream()), "mn_find_page_spines_u8")
+        _lib.check(_lib.load().mn_find_page_spines_u8(base + sp, m, stiles, _stream()), "mn_find_page_spines_u8")
         LAUNCHES += 2
-        res = (res, buf[out0 + n * rsz:out0 + n * rsz + m * spsz])
+        res = (res, buf[sres:sres + m * spsz])
     else:
         res = (res,)
     out = res + ((views,) if hulls else ()) + ((lviews,) if labels else ())
