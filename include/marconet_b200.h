@@ -983,6 +983,93 @@ typedef struct {
 } mn_spine_page;
 int mn_find_page_spines_u8(const mn_spine_page* spines, int n, long long max_tiles, void* stream);
 
+/* Seals (DESIGN.md section 7b, "Seals"): round and oval stamps found by colour and shape on a level page crop b (w x h, 3
+ * channels), kept out of its layout and described for restoration.  A pixel is seal-coloured when max(c) - min(c) >=
+ * MN_SEAL_CHROMA over its three channels (any channel order).  The crop is cut into MN_SEAL_CELL x MN_SEAL_CELL cells (cell
+ * (cx, cy) = pixels [4 cx, 4 cx + 4) x [4 cy, 4 cy + 4) of the crop, index cy cw + cx, cw = ceil(w / 4), ch = ceil(h / 4)); a
+ * cell is on when it holds at least MN_SEAL_CELL_MIN seal-coloured pixels.  A candidate is an 8-connected component of on cells
+ * whose seal-coloured pixels' box (x0, y0, x1, y1) (crop pixels, end exclusive) has sides A = x1 - x0, B = y1 - y0 in
+ * [seal_size, MN_SEAL_MAX_SIDE] and 2 max(A, B) <= 3 min(A, B).  For a pixel (x, y), X = 2 x + 1 - (x0 + x1),
+ * Y = 2 y + 1 - (y0 + y1); its radial bin is k = floor(32 rho), rho^2 = (X / A)^2 + (Y / B)^2, the largest k with
+ * k^2 A^2 B^2 <= 1024 (X^2 B^2 + Y^2 A^2) in int64, and only k < MN_SEAL_BINS counts (rho < 33 / 32); its sector s in
+ * [0, 72) is the 5-degree sector of (X B, -Y A) between the directions d_s and d_s+1 of MN_SEAL_DIRS (d_s+36 = -d_s): for p in
+ * the upper half plane (p.y > 0, or p.y = 0 < p.x) the largest s < 36 with cross(d_s, p) >= 0, else 36 + that of -p; p = 0 is
+ * sector 0.  Per candidate, ink[k][s] counts the seal-coloured pixels and area[k] all pixels of the box in each bin:
+ *   ring = the sectors with ink at k in [MN_SEAL_RING_K, 32]; a seal when ring >= MN_SEAL_RING_SECTORS.
+ *   band: from k = 32 inward, the first run of bins with 4 ink_k >= area_k (the ring), then the bins with 32 ink_k >= area_k
+ *   (its edge), then at least one bin with 32 ink_k < area_k (the gap), then the run of bins with 32 ink_k >= area_k down to
+ *   k = MN_SEAL_BAND_MIN_K at most: k_top its first bin and k_bottom its last; no gap or no such run is MN_SEAL_NO_BAND.
+ *   arc: per sector the ink of the band's bins; a sector is empty when 720 ink < max(720, band_ink); the gap [g0, g0 + n) is the
+ *   longest circular run of empty sectors, ties to the smallest g0 (n = 72, g0 = 0 when all are empty); MN_SEAL_NO_GAP when
+ *   n < MN_SEAL_MIN_GAP, MN_SEAL_SHORT when 72 - n < MN_SEAL_MIN_TEXT.
+ * mn_find_seals_u8 issues 6 launches for every page of a call, whatever the number of pages and candidates:
+ *   1. per cell, its seal-coloured count and their box: label[c] = c for an on cell, else -1; box[4 c ..] the on cell's box;
+ *   2. per on cell, union with its on neighbours W, NW, N and NE (uf_union: a root is the smallest index of its set);
+ *   3. per on cell, path compression and its box folded into its root's by atomicMin / atomicMax;
+ *   4. per root, the size test, and the candidate (box, root) appended to cand (out->n_cand counts them all);
+ *   5. one CTA per candidate slot (MN_PAGE_MAX_SEALS per page): the histograms in shared memory and the ring, band and arc
+ *      into out->seal[r], r the candidate's rank by (y0, x0, root); out->n_seals counts the seals.  A page with more than
+ *      MN_PAGE_MAX_SEALS candidates gets out->error = MN_SEAL_ERR_SEALS and no seal;
+ *   6. the layout copy (mn_seal_layout_u8's launch).
+ * mn_seal_layout_u8 issues that one launch: copy (h x 3 w bytes, pitch 3 w) = the crop, with every seal-coloured pixel at
+ * rho < 33 / 32 of a seal of out (the out->n_cand entries with found != 0, boxes in crop pixels) set to (255, 255, 255).
+ * label and box hold cw ch and 4 cw ch int32, cand MN_PAGE_MAX_SEALS 8 int32; out tables lie in work (work_bytes, zeroed by
+ * mn_find_seals_u8); the copy is written whole.  pages: DEVICE array, every crop at most 32767 on a side. */
+#define MN_PAGE_SEALS 16
+#define MN_PAGE_MAX_SEALS 64
+#define MN_SEAL_CHROMA 64
+#define MN_SEAL_CELL 4
+#define MN_SEAL_CELL_MIN 2
+#define MN_SEAL_MAX_SIDE 4096
+#define MN_SEAL_BINS 33
+#define MN_SEAL_SECTORS 72
+#define MN_SEAL_RING_K 26
+#define MN_SEAL_RING_SECTORS 54
+#define MN_SEAL_RING_DENSITY 4
+#define MN_SEAL_BAND_DENSITY 32
+#define MN_SEAL_BAND_MIN_K 10
+#define MN_SEAL_EMPTY_DIV 720
+#define MN_SEAL_MIN_GAP 2
+#define MN_SEAL_MIN_TEXT 9
+#define MN_SEAL_NO_BAND 1
+#define MN_SEAL_NO_GAP 2
+#define MN_SEAL_SHORT 3
+#define MN_SEAL_ERR_SEALS 1
+/* d_s = (round(2^20 cos 5s), round(2^20 sin 5s)) for s < 36 */
+#define MN_SEAL_DIRS {{1048576, 0}, {1044586, 91389}, {1032646, 182083}, {1012847, 271391}, {985339, 358634}, {950333, 443147}, \
+    {908093, 524288}, {858943, 601438}, {803256, 674012}, {741455, 741455}, {674012, 803256}, {601438, 858943}, {524288, 908093}, \
+    {443147, 950333}, {358634, 985339}, {271391, 1012847}, {182083, 1032646}, {91389, 1044586}, {0, 1048576}, {-91389, 1044586}, \
+    {-182083, 1032646}, {-271391, 1012847}, {-358634, 985339}, {-443147, 950333}, {-524288, 908093}, {-601438, 858943}, \
+    {-674012, 803256}, {-741455, 741455}, {-803256, 674012}, {-858943, 601438}, {-908093, 524288}, {-950333, 443147}, \
+    {-985339, 358634}, {-1012847, 271391}, {-1032646, 182083}, {-1044586, 91389}}
+typedef struct {
+    int32_t x0, y0, x1, y1;     /* the box, in crop pixels */
+    int32_t root;               /* the component's smallest cell index */
+    int32_t ring;               /* sectors hit at k >= MN_SEAL_RING_K */
+    int32_t found;              /* 1: a seal */
+    int32_t k_bottom, k_top;    /* the band, or -1 */
+    int32_t g0, n_gap;          /* the arc's gap, or -1 */
+    int32_t why;                /* 0, MN_SEAL_NO_BAND, MN_SEAL_NO_GAP or MN_SEAL_SHORT; 0 for a candidate that is no seal */
+    int32_t band_ink;           /* the band's seal-coloured pixels */
+    int32_t pad[3];
+} mn_seal;
+typedef struct {
+    int32_t error, n_cand, n_seals, pad;
+    mn_seal seal[MN_PAGE_MAX_SEALS];   /* the candidates by (y0, x0, root) */
+} mn_seal_table;
+typedef struct {
+    mn_text_block b;            /* the crop record (img, pitch, x0, y0, w, h) */
+    uint8_t* copy;              /* the layout copy */
+    int32_t* label;
+    int32_t* box;
+    int32_t* cand;
+    mn_seal_table* out;
+    int32_t seal_size, pad;
+} mn_seal_page;
+int mn_find_seals_u8(const mn_seal_page* pages, int n, long long max_tiles, long long max_cell_tiles, void* work,
+                     long long work_bytes, void* stream);
+int mn_seal_layout_u8(const mn_seal_page* pages, int n, long long max_tiles, void* stream);
+
 /* Flat pages (DESIGN.md section 7b, "Flat pages"): the dewarp field of a curled page, built from its traced lines, composed with
  * the page's frame and sampled from the photo.  A page's line table (built on the host, pipeline.flat_line_table) holds
  * MN_FLAT_LINE_DOUBLES fp64 values per line, sorted by anchor Y (ties in reading order): xs, xe, mu_0 .. mu_3, Y, bx0, bx1.

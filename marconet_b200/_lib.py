@@ -253,6 +253,25 @@ class SpinePage(Structure):
     _fields_ = [("page", c_void_p), ("cols", c_void_p), ("res", c_void_p)]
 
 
+PAGE_SEALS, PAGE_MAX_SEALS = 16, 64                                # MN_PAGE_SEALS, MN_PAGE_MAX_SEALS
+SEAL_ERR_SEALS = 1                                                 # MN_SEAL_ERR_SEALS
+SEAL_NO_BAND, SEAL_NO_GAP, SEAL_SHORT = 1, 2, 3                    # MN_SEAL_NO_BAND, MN_SEAL_NO_GAP, MN_SEAL_SHORT
+
+
+class Seal(Structure):
+    _fields_ = [(f, c_int32) for f in ("x0", "y0", "x1", "y1", "root", "ring", "found", "k_bottom", "k_top", "g0", "n_gap", "why",
+                                       "band_ink")] + [("pad", c_int32 * 3)]
+
+
+class SealTable(Structure):
+    _fields_ = [("error", c_int32), ("n_cand", c_int32), ("n_seals", c_int32), ("pad", c_int32), ("seal", Seal * PAGE_MAX_SEALS)]
+
+
+class SealPage(Structure):
+    _fields_ = [("b", TextBlock), ("copy", c_void_p), ("label", c_void_p), ("box", c_void_p), ("cand", c_void_p), ("out", c_void_p),
+                ("seal_size", c_int32), ("pad", c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -323,6 +342,8 @@ SYMBOLS = {
     "mn_find_lines_curved_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_int, c_void_p, c_longlong, c_void_p]),
     "mn_find_page_quads_u8": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_find_page_spines_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
+    "mn_find_seals_u8": (c_int, [c_void_p, c_int, c_longlong, c_longlong, c_void_p, c_longlong, c_void_p]),
+    "mn_seal_layout_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -2241,6 +2241,288 @@ __global__ void __launch_bounds__(kHullThreads) spine_kernel(const mn_spine_page
     res->found = xt >= 0 && xb >= 0 && spine_deep(D, tl, tr) && spine_deep(E, bl, br);
 }
 
+// Seals (DESIGN.md 7b, "Seals"): cells of seal-coloured pixels, their 8-connected components by union-find on the cell grid,
+// the components' boxes, then one CTA per candidate with its radial x sector histogram in shared memory, all in integers.
+constexpr int kSealCellsX = 32, kSealCellsY = 8;      // a cell tile: one thread per cell, a warp per cell row
+constexpr int kSealThreads = 512;
+__constant__ int2 c_seal_dirs[MN_SEAL_SECTORS / 2] = MN_SEAL_DIRS;
+
+__device__ __forceinline__ bool seal_coloured(const uint8_t* p) {
+    const int a = p[0], b = p[1], c = p[2];
+    return max(a, max(b, c)) - min(a, min(b, c)) >= MN_SEAL_CHROMA;
+}
+
+__device__ __forceinline__ const uint8_t* crop_px(const mn_text_block& b, int x, int y) {
+    return b.img + (long long)(b.y0 + y) * b.pitch + (long long)(b.x0 + x) * 3;
+}
+
+__device__ __forceinline__ bool cell_origin(const mn_text_block& b, int& cx, int& cy, int& cw, int& ch) {
+    cw = (b.w + MN_SEAL_CELL - 1) / MN_SEAL_CELL;
+    ch = (b.h + MN_SEAL_CELL - 1) / MN_SEAL_CELL;
+    const int tiles_x = (cw + kSealCellsX - 1) / kSealCellsX, tiles_y = (ch + kSealCellsY - 1) / kSealCellsY;
+    if ((long long)blockIdx.x >= (long long)tiles_x * tiles_y) return false;
+    cx = (int)(blockIdx.x % tiles_x) * kSealCellsX + (threadIdx.x & 31);
+    cy = (int)(blockIdx.x / tiles_x) * kSealCellsY + (threadIdx.x >> 5);
+    return cx < cw && cy < ch;
+}
+
+// 1: each cell's count of seal-coloured pixels and their box.
+__global__ void __launch_bounds__(kTileThreads) seal_cells_kernel(const mn_seal_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    const mn_seal_page sp = pages[blockIdx.y];
+    const mn_text_block b = sp.b;
+    int cx, cy, cw, ch;
+    if (!cell_origin(b, cx, cy, cw, ch)) return;
+    int n = 0, x0 = INT_MAX, y0 = INT_MAX, x1 = 0, y1 = 0;
+    for (int y = cy * MN_SEAL_CELL; y < min(cy * MN_SEAL_CELL + MN_SEAL_CELL, b.h); ++y) {
+        for (int x = cx * MN_SEAL_CELL; x < min(cx * MN_SEAL_CELL + MN_SEAL_CELL, b.w); ++x) {
+            if (!seal_coloured(crop_px(b, x, y))) continue;
+            ++n;
+            x0 = min(x0, x);
+            y0 = min(y0, y);
+            x1 = max(x1, x + 1);
+            y1 = y + 1;
+        }
+    }
+    const int c = cy * cw + cx;
+    const bool on = n >= MN_SEAL_CELL_MIN;
+    sp.label[c] = on ? c : -1;
+    if (on) reinterpret_cast<int4*>(sp.box)[c] = make_int4(x0, y0, x1, y1);
+}
+
+// 2: each on cell joined to its on neighbours W, NW, N and NE.
+__global__ void __launch_bounds__(kTileThreads) seal_union_kernel(const mn_seal_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    const mn_seal_page sp = pages[blockIdx.y];
+    int cx, cy, cw, ch;
+    if (!cell_origin(sp.b, cx, cy, cw, ch)) return;
+    int* label = sp.label;
+    const int c = cy * cw + cx;
+    if (label[c] < 0) return;
+    if (cx > 0 && label[c - 1] >= 0) uf_union(label, c - 1, c);
+    if (cy > 0) {
+        for (int d = -1; d <= 1; ++d) {
+            if (cx + d >= 0 && cx + d < cw && label[c - cw + d] >= 0) uf_union(label, c - cw + d, c);
+        }
+    }
+}
+
+// 3: path compression and each on cell's box folded into its root's.
+__global__ void __launch_bounds__(kTileThreads) seal_box_kernel(const mn_seal_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    const mn_seal_page sp = pages[blockIdx.y];
+    int cx, cy, cw, ch;
+    if (!cell_origin(sp.b, cx, cy, cw, ch)) return;
+    const int c = cy * cw + cx;
+    if (sp.label[c] < 0) return;
+    const int r = uf_find(sp.label, c);
+    sp.label[c] = r;
+    if (r == c) return;
+    const int4 bx = reinterpret_cast<const int4*>(sp.box)[c];
+    atomicMin(&sp.box[4 * r], bx.x);
+    atomicMin(&sp.box[4 * r + 1], bx.y);
+    atomicMax(&sp.box[4 * r + 2], bx.z);
+    atomicMax(&sp.box[4 * r + 3], bx.w);
+}
+
+// 4: each root whose box passes the size test appended as a candidate.
+__global__ void __launch_bounds__(kTileThreads) seal_cand_kernel(const mn_seal_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    const mn_seal_page sp = pages[blockIdx.y];
+    int cx, cy, cw, ch;
+    if (!cell_origin(sp.b, cx, cy, cw, ch)) return;
+    const int c = cy * cw + cx;
+    if (sp.label[c] != c) return;
+    const int4 bx = reinterpret_cast<const int4*>(sp.box)[c];
+    const int A = bx.z - bx.x, B = bx.w - bx.y, lo = min(A, B), hi = max(A, B);
+    if (lo < sp.seal_size || hi > MN_SEAL_MAX_SIDE || 2 * hi > 3 * lo) return;
+    const int slot = atomicAdd(&sp.out->n_cand, 1);
+    if (slot >= MN_PAGE_MAX_SEALS) return;
+    int* e = sp.cand + 8 * slot;
+    e[0] = bx.x;
+    e[1] = bx.y;
+    e[2] = bx.z;
+    e[3] = bx.w;
+    e[4] = c;
+}
+
+// The radial bin k = floor(32 rho) of (X, Y) in an A x B box, exact: q = floor(1024 (X^2 B^2 + Y^2 A^2) / (A^2 B^2)) <= 2048,
+// and floor(sqrt(q)) = floor(32 rho).
+__device__ __forceinline__ int seal_bin(long long X, long long Y, long long A, long long B) {
+    const long long q = 1024 * (X * X * B * B + Y * Y * A * A) / (A * A * B * B);
+    int k = (int)sqrtf((float)q);
+    while ((long long)k * k > q) --k;
+    while ((long long)(k + 1) * (k + 1) <= q) ++k;
+    return k;
+}
+
+__device__ __forceinline__ int seal_half_sector(long long px, long long py) {
+    int lo = 0, hi = MN_SEAL_SECTORS / 2 - 1;                   // the largest s < 36 with cross(d_s, p) >= 0; s = 0 holds
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        const int2 d = c_seal_dirs[mid];
+        if ((long long)d.x * py - (long long)d.y * px >= 0) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+__device__ __forceinline__ int seal_sector(long long px, long long py) {
+    if (px == 0 && py == 0) return 0;
+    if (py > 0 || (py == 0 && px > 0)) return seal_half_sector(px, py);
+    return MN_SEAL_SECTORS / 2 + seal_half_sector(-px, -py);
+}
+
+// 5: one CTA per candidate slot: the histograms, then thread 0 reads the ring, band and arc off them.
+__global__ void __launch_bounds__(kSealThreads) seal_test_kernel(const mn_seal_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    __shared__ int s_ink[MN_SEAL_BINS][MN_SEAL_SECTORS];
+    __shared__ int s_area[MN_SEAL_BINS];
+    __shared__ int s_sum[MN_SEAL_BINS + MN_SEAL_SECTORS];     // ink_k, then the ring's sectors hit
+    __shared__ int s_sec[MN_SEAL_SECTORS];
+    __shared__ int s_rank;
+    const mn_seal_page sp = pages[blockIdx.y];
+    mn_seal_table* out = sp.out;
+    const int n_cand = out->n_cand, slot = blockIdx.x;
+    if (n_cand > MN_PAGE_MAX_SEALS) {
+        if (slot == 0 && threadIdx.x == 0) out->error = MN_SEAL_ERR_SEALS;
+        return;
+    }
+    if (slot >= n_cand) return;
+    const int* e = sp.cand + 8 * slot;
+    const int x0 = e[0], y0 = e[1], x1 = e[2], y1 = e[3], root = e[4];
+    for (int i = threadIdx.x; i < MN_SEAL_BINS * MN_SEAL_SECTORS; i += blockDim.x) (&s_ink[0][0])[i] = 0;
+    if (threadIdx.x < MN_SEAL_BINS) s_area[threadIdx.x] = 0;
+    if (threadIdx.x == 0) s_rank = 0;
+    __syncthreads();
+    const mn_text_block b = sp.b;
+    const long long A = x1 - x0, B = y1 - y0;
+    const long long n_px = A * B;
+    for (long long i = threadIdx.x; i < n_px; i += blockDim.x) {
+        const int x = x0 + (int)(i % A), y = y0 + (int)(i / A);
+        const long long X = 2 * x + 1 - (x0 + x1), Y = 2 * y + 1 - (y0 + y1);
+        const int k = seal_bin(X, Y, A, B);
+        if (k >= MN_SEAL_BINS) continue;
+        atomicAdd(&s_area[k], 1);
+        if (seal_coloured(crop_px(b, x, y))) atomicAdd(&s_ink[k][seal_sector(X * B, -Y * A)], 1);
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < MN_SEAL_BINS + MN_SEAL_SECTORS; j += blockDim.x) {
+        int t = 0;
+        if (j < MN_SEAL_BINS) {                                  // ink_k
+            for (int s = 0; s < MN_SEAL_SECTORS; ++s) t += s_ink[j][s];
+        } else {                                                 // a sector hit by the ring
+            for (int k = MN_SEAL_RING_K; k < MN_SEAL_BINS; ++k) t |= s_ink[k][j - MN_SEAL_BINS];
+            t = t != 0;
+        }
+        s_sum[j] = t;
+    }
+    int rank = 0;                                                // by (y0, x0, root) among the page's candidates
+    for (int j = threadIdx.x; j < n_cand; j += blockDim.x) {
+        const int* f = sp.cand + 8 * j;
+        rank += f[1] < y0 || (f[1] == y0 && (f[0] < x0 || (f[0] == x0 && f[4] < root)));
+    }
+    if (rank) atomicAdd(&s_rank, rank);
+    __syncthreads();
+    if (threadIdx.x) return;
+    const int* ink = s_sum;
+    int ring = 0;
+    for (int s = 0; s < MN_SEAL_SECTORS; ++s) ring += s_sum[MN_SEAL_BINS + s];
+    mn_seal r;
+    r.x0 = x0, r.y0 = y0, r.x1 = x1, r.y1 = y1, r.root = root, r.ring = ring;
+    r.found = ring >= MN_SEAL_RING_SECTORS;
+    r.k_bottom = r.k_top = r.g0 = r.n_gap = -1;
+    r.why = 0, r.band_ink = 0, r.pad[0] = r.pad[1] = r.pad[2] = 0;
+    if (r.found) {
+        int k = MN_SEAL_BINS - 1;
+        while (k >= 0 && MN_SEAL_RING_DENSITY * ink[k] < s_area[k]) --k;                       // the ring's outer bin
+        while (k >= 0 && MN_SEAL_RING_DENSITY * ink[k] >= s_area[k]) --k;                      // the ring run
+        while (k >= 0 && MN_SEAL_BAND_DENSITY * ink[k] >= s_area[k]) --k;                      // its edge
+        const int gap_top = k;
+        while (k >= MN_SEAL_BAND_MIN_K && MN_SEAL_BAND_DENSITY * ink[k] < s_area[k]) --k;      // the gap
+        if (gap_top >= MN_SEAL_BAND_MIN_K && k < gap_top && k >= MN_SEAL_BAND_MIN_K) {
+            r.k_top = k;
+            while (k >= MN_SEAL_BAND_MIN_K && MN_SEAL_BAND_DENSITY * ink[k] >= s_area[k]) --k;
+            r.k_bottom = k + 1;
+        }
+        if (r.k_top < 0) {
+            r.why = MN_SEAL_NO_BAND;
+        } else {
+            int* sec = s_sec;
+            int band = 0;
+            for (int s = 0; s < MN_SEAL_SECTORS; ++s) {
+                int t = 0;
+                for (int kk = r.k_bottom; kk <= r.k_top; ++kk) t += s_ink[kk][s];
+                sec[s] = t;
+                band += t;
+            }
+            r.band_ink = band;
+            const int lim = max(MN_SEAL_EMPTY_DIV, band);
+            int g0 = 0, n = 0, all = 1;
+            for (int s = 0; s < MN_SEAL_SECTORS; ++s) all &= MN_SEAL_EMPTY_DIV * sec[s] < lim;
+            if (all) {
+                n = MN_SEAL_SECTORS;
+            } else {
+                for (int s = 0; s < MN_SEAL_SECTORS; ++s) {   // runs start at an empty sector after a non-empty one
+                    const int prev = (s + MN_SEAL_SECTORS - 1) % MN_SEAL_SECTORS;
+                    if (!(MN_SEAL_EMPTY_DIV * sec[s] < lim) || MN_SEAL_EMPTY_DIV * sec[prev] < lim) continue;
+                    int m = 0;
+                    while (MN_SEAL_EMPTY_DIV * sec[(s + m) % MN_SEAL_SECTORS] < lim) ++m;
+                    if (m > n) g0 = s, n = m;
+                }
+            }
+            r.g0 = g0, r.n_gap = n;
+            r.why = n < MN_SEAL_MIN_GAP ? MN_SEAL_NO_GAP : MN_SEAL_SECTORS - n < MN_SEAL_MIN_TEXT ? MN_SEAL_SHORT : 0;
+        }
+    }
+    out->seal[s_rank] = r;
+    if (r.found) atomicAdd(&out->n_seals, 1);
+}
+
+// 6: the layout copy, the seals' own ink set to paper.
+__global__ void __launch_bounds__(kTileThreads) seal_copy_kernel(const mn_seal_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    __shared__ int4 s_box[MN_PAGE_MAX_SEALS];
+    __shared__ int s_n;
+    const mn_seal_page sp = pages[blockIdx.y];
+    const mn_text_block b = sp.b;
+    int tx, ty;
+    if (!tile_origin(b, tx, ty)) return;
+    if (threadIdx.x == 0) {
+        const mn_seal_table* t = sp.out;
+        int n = 0;
+        if (!t->error) {
+            for (int j = 0; j < min(t->n_cand, MN_PAGE_MAX_SEALS); ++j) {
+                const mn_seal& s = t->seal[j];
+                if (s.found && s.x0 < tx + kTile && tx < s.x1 && s.y0 < ty + kTile && ty < s.y1)
+                    s_box[n++] = make_int4(s.x0, s.y0, s.x1, s.y1);
+            }
+        }
+        s_n = n;
+    }
+    __syncthreads();
+    const int x = tx + (threadIdx.x & 31), n = s_n;
+    if (x >= b.w) return;
+    for (int y = ty + (threadIdx.x >> 5); y < min(ty + kTile, b.h); y += 8) {
+        const uint8_t* p = crop_px(b, x, y);
+        uint8_t v0 = p[0], v1 = p[1], v2 = p[2];
+        if (n && seal_coloured(p)) {
+            for (int j = 0; j < n; ++j) {
+                const int4 s = s_box[j];
+                if (x < s.x || x >= s.z || y < s.y || y >= s.w) continue;
+                const long long A = s.z - s.x, B = s.w - s.y, X = 2 * x + 1 - (s.x + s.z), Y = 2 * y + 1 - (s.y + s.w);
+                if (1024 * (X * X * B * B + Y * Y * A * A) < (long long)MN_SEAL_BINS * MN_SEAL_BINS * A * A * B * B) {
+                    v0 = v1 = v2 = 255;
+                    break;
+                }
+            }
+        }
+        uint8_t* q = sp.copy + (long long)y * 3 * b.w + (long long)x * 3;
+        q[0] = v0;
+        q[1] = v1;
+        q[2] = v2;
+    }
+}
+
 // 4-11 of the XY-cut: both passes of levels, the text size between them and the leaves, on pages whose bitmap and root are
 // written; under MN_PAGE_RULES, the three rule launches first, under MN_PAGE_PANELS the panel test and paint after the text
 // size, under MN_PAGE_FIGURES the figure launch after those, and under MN_PAGE_DIRECTIONS the direction launch after the leaves.
@@ -2413,6 +2695,33 @@ extern "C" int mn_find_page_spines_u8(const mn_spine_page* spines, int n, long l
     MN_CUDA_CHECK((mn_launch(spine_kernel, dim3(n), dim3(kHullThreads), 0, st, spines)));
     MN_LAUNCH_CHECK();
     return MN_OK;
+}
+
+extern "C" int mn_seal_layout_u8(const mn_seal_page* pages, int n, long long max_tiles, void* stream) {
+    MN_REQUIRE(pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31), "mn_seal_layout_u8: bad args");
+    MN_CUDA_CHECK((mn_launch(seal_copy_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, (cudaStream_t)stream, pages)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_find_seals_u8(const mn_seal_page* pages, int n, long long max_tiles, long long max_cell_tiles, void* work,
+                                long long work_bytes, void* stream) {
+    MN_REQUIRE(pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31) && max_cell_tiles > 0 &&
+               max_cell_tiles < (1ll << 31) && work && work_bytes > 0, "mn_find_seals_u8: bad args");
+    cudaStream_t st = (cudaStream_t)stream;
+    MN_CUDA_CHECK(cudaMemsetAsync(work, 0, (size_t)work_bytes, st));
+    const dim3 grid((unsigned)max_cell_tiles, n);
+    MN_CUDA_CHECK((mn_launch(seal_cells_kernel, grid, dim3(kTileThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(seal_union_kernel, grid, dim3(kTileThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(seal_box_kernel, grid, dim3(kTileThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(seal_cand_kernel, grid, dim3(kTileThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    MN_CUDA_CHECK((mn_launch(seal_test_kernel, dim3(MN_PAGE_MAX_SEALS, n), dim3(kSealThreads), 0, st, pages)));
+    MN_LAUNCH_CHECK();
+    return mn_seal_layout_u8(pages, n, max_tiles, stream);
 }
 
 extern "C" int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* curves, int n, long long max_tiles,

@@ -1830,19 +1830,31 @@ def find_lines(blocks, scores=False):
     number; blocks with skew None search the one-entry table (1, 0), which keeps their mn_block_lines records exactly.  The
     tensor then holds the n mn_block_lines records followed by the n mn_skew_block records (``skew_block_dtype()``: the chosen
     index and frame).  ``scores`` (tests): also return, per block, the int64 CUDA view of its per-angle scores (None unless it
-    searched)."""
+    searched).
+    seals (DESIGN.md 7b, "Seals"; index 9, blocks with skew None only): None or a list of at most PAGE_MAX_SEALS seal boxes
+    (x0, y0, x1, y1) in image pixels.  Such a block is split on its layout copy, the crop with every seal-coloured pixel inside
+    a box's inscribed ellipse (rho < 33 / 32) set to paper, made by one more launch (mn_seal_layout_u8) for all sealed blocks
+    of the call; a call with skewed blocks reads the copies through its skew records alike.  The copies (seal_block_bytes)
+    may use PAGE_MAX_WORK bytes per call."""
     global LAUNCHES
     dev = _check_items(blocks, "find_lines", "block")
     skewed = any(len(b) > 7 and b[7] is not None for b in blocks)
     n = len(blocks)
     osz, rsz = ctypes.sizeof(_lib.BlockLines), ctypes.sizeof(_lib.TextBlock)
     ssz = ctypes.sizeof(_lib.SkewBlock) if skewed else 0
-    dims, tables = [], []
+    dims, tables, copies = [], [], 0
     for i, blk in enumerate(blocks):
         what = f"find_lines: block {i}"
         x0, y0, bw, bh = _check_crop(blk[:7], dev, what, "min_ink / gap / min_height")
         vertical, skew, max_skew = blk[2], blk[7] if len(blk) > 7 else None, blk[8] if len(blk) > 8 else 10.0
         cs = _check_skew(skew, max_skew, vertical, what)
+        if len(blk) > 9 and blk[9]:
+            if skew is not None or len(blk[9]) > _lib.PAGE_MAX_SEALS:
+                raise ValueError(f"{what}: a sealed block is level (skew None) and has at most {_lib.PAGE_MAX_SEALS} seals")
+            copies += seal_block_bytes(bw, bh)
+            if copies > PAGE_MAX_WORK:
+                raise ValueError(f"{what}: the sealed blocks up to this one need {copies} bytes of layout copies, over the "
+                                 f"{PAGE_MAX_WORK} a call may use")
         stride = (bw if vertical else bh) if skew is None else skew_stride(bw, bh, vertical, cs)
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
             raise ValueError(f"{what}: {len(cs)} angles x {stride} bins exceed the {SKEW_MAX_PROFILE} profile values a skewed "
@@ -1850,26 +1862,41 @@ def find_lines(blocks, scores=False):
         tables.append(cs)
         dims.append((x0, y0, bw, bh, len(cs), stride))
     tab, t_offs = _angle_tables(tables) if skewed else (b"", [0] * n)
-    pack = _Pack()                  # results, skew records, crop records, tables; scores, work (zeroed); scratch
-    pack.area(n * osz)
+    sealed = [i for i, blk in enumerate(blocks) if len(blk) > 9 and blk[9]]
+    m, tsz, spsz = len(sealed), ctypes.sizeof(_lib.SealTable), ctypes.sizeof(_lib.SealPage)
+    pack = _Pack()                  # results, skew records, crop records, tables; scores, work (zeroed); scratch; seal records,
+    pack.area(n * osz)              # tables and layout copies
     sk, seg, t_off = pack.area(n * ssz), pack.area(n * rsz), pack.area(len(tab))
     score = [pack.area(8 * n_ang if n_ang > 1 else 0) for *_, n_ang, _ in dims]
     work = [(pack.area(4 * 256), pack.area(4 * 3 * L), pack.area(4 * n_ang * L if n_ang > 1 else 0)) for *_, n_ang, L in dims]
     w_end = pack.end
     scratch = [pack.area(4 * (2 * L + 4)) for *_, L in dims]
+    sp, st = (pack.area(m * spsz, 16), pack.area(m * tsz, 16)) if sealed else (0, 0)
+    copies = {i: pack.area(3 * dims[i][2] * dims[i][3], 16) for i in sealed}
     base = pack.alloc(dev)
-    recs, srecs, views, tiles = [], [], [], 0
+    recs, srecs, views, tiles, seal_recs, seal_tabs = [], [], [], 0, [], []
     for i, (blk, (x0, y0, bw, bh, n_ang, stride), sc, (hist, prof, ext), scr, t) in \
             enumerate(zip(blocks, dims, score, work, scratch, t_offs)):
         img, _, vertical, polarity, min_ink, gap, min_height = blk[:7]
-        tb = _lib.TextBlock(img.data_ptr(), img.stride(0), x0, y0, bw, bh, int(bool(vertical)), polarity, min_ink or 0, gap or 0,
+        src, pitch = img.data_ptr(), img.stride(0)
+        if i in copies:             # the block reads its layout copy through its own crop offsets
+            crop = _lib.TextBlock(src, pitch, x0, y0, bw, bh)
+            src, pitch = (base + copies[i] - y0 * 3 * bw - 3 * x0) % (1 << 64), 3 * bw
+            seal_recs.append(_lib.SealPage(crop, base + copies[i], 0, 0, 0, base + st + len(seal_tabs) * tsz))
+            seal_tabs.append(seal_table(blk[9], x0, y0))
+        tb = _lib.TextBlock(src, pitch, x0, y0, bw, bh, int(bool(vertical)), polarity, min_ink or 0, gap or 0,
                             min_height or 0, 0, base + hist, base + prof, base + scr, base + i * osz)
         recs.append(tb)
         if skewed:
             srecs.append(_skew_block(tb, base + t_off + 16 * t, base + sc, base + ext, n_ang, stride))
         views.append(pack.buf[sc:sc + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
-    pack.upload((sk, bytes((_lib.SkewBlock * len(srecs))(*srecs))), (seg, bytes((_lib.TextBlock * n)(*recs))), (t_off, tab))
+    pack.upload((sk, bytes((_lib.SkewBlock * len(srecs))(*srecs))), (seg, bytes((_lib.TextBlock * n)(*recs))), (t_off, tab),
+                *(((sp, bytes((_lib.SealPage * m)(*seal_recs))), (st, b"".join(seal_tabs))) if sealed else ()))
+    if sealed:
+        _lib.check(_lib.load().mn_seal_layout_u8(base + sp, m, max(-(-dims[i][2] // 32) * -(-dims[i][3] // 32) for i in sealed),
+                                                 _stream()), "mn_seal_layout_u8")
+        LAUNCHES += 1
     if skewed:
         _lib.check(_lib.load().mn_find_lines_skewed_u8(base + seg, base + sk, n, tiles, base + score[0], w_end - score[0],
                                                        _stream()), "mn_find_lines_skewed_u8")
@@ -1880,6 +1907,35 @@ def find_lines(blocks, scores=False):
         LAUNCHES += 4
     res = pack.buf[:n * (osz + ssz)]
     return (res, views) if scores else res
+
+
+def seal_table(boxes, x0=0, y0=0):
+    """The bytes of the mn_seal_table of given seal ``boxes`` (x0, y0, x1, y1) of a crop at (x0, y0): each box in crop pixels,
+    a found seal, in the order given."""
+    t = _lib.SealTable(0, len(boxes), len(boxes))
+    for j, (a, b, c, d) in enumerate(boxes):
+        t.seal[j] = _lib.Seal(a - x0, b - y0, c - x0, d - y0, -1, 0, 1, -1, -1, -1, -1, 0, 0)
+    return bytes(t)
+
+
+def seal_block_bytes(w, h):
+    """Device bytes a sealed w x h block adds to find_lines (DESIGN.md 7b, "Seals"): its layout copy (3 w h), record and seal
+    table, with 16 bytes for each area's alignment.  A call's sealed blocks may use PAGE_MAX_WORK bytes in all."""
+    return 3 * w * h + ctypes.sizeof(_lib.SealPage) + ctypes.sizeof(_lib.SealTable) + 3 * 16
+
+
+def _seal_areas(w, h):
+    """Byte sizes of one seal page's areas after the results in find_blocks: its layout copy, cell labels, cell boxes and
+    candidate list."""
+    cells = -(-w // 4) * -(-h // 4)
+    return [3 * w * h, 4 * cells, 16 * cells, 32 * _lib.PAGE_MAX_SEALS]
+
+
+def seal_bytes(w, h):
+    """Device bytes a w x h page adds to find_blocks when its seals are found (DESIGN.md 7b, "Seals"): its record, seal table,
+    candidate list, cell labels and boxes (one int32 and four per 4 x 4 cell) and its layout copy (3 w h), with 16 bytes for
+    each area's alignment."""
+    return ctypes.sizeof(_lib.SealPage) + ctypes.sizeof(_lib.SealTable) + sum(_seal_areas(w, h)) + 6 * 16
 
 
 def window_footprint(w, h, vertical, c, s, u_min, v_min, window):
@@ -2050,6 +2106,7 @@ class PageItem(NamedTuple):
     figure_size: object = None
     directions: bool = False
     panel_size: object = None
+    seal_size: object = None
 
 
 def page_cap(w, h):
@@ -2086,19 +2143,19 @@ def _page_areas(L, M, cap, n_ang, stride, rules, figures, panels):
             plane if panels and not rules else 0]
 
 
-def page_bytes(w, h, vertical=False, cs=None, rules=False, figures=False, panels=False):
+def page_bytes(w, h, vertical=False, cs=None, rules=False, figures=False, panels=False, seals=False):
     """Device bytes of one w x h page in find_blocks, with or without ``rules``, ``figures`` and ``panels``: its records,
     result and leaf table, a figure page's table of PAGE_MAX_FIGURES and a panel page's table of PAGE_MAX_PANELS page nodes,
     its work areas and 64 bytes for the call's 16-byte alignments.  ``cs``: None in a call without skewed pages, else the
     (c, s) table the page searches ([(1.0, 0.0)] for a page with skew None), which adds the search record, the table and 16
-    bytes for its alignment; the page's bitmaps are then those of its largest frame."""
+    bytes for its alignment; the page's bitmaps are then those of its largest frame.  ``seals``: with seal_bytes."""
     n_ang = len(cs) if cs else 1
     L, M, stride = skew_page_frame(w, h, vertical, cs or [(1.0, 0.0)])
     cap = page_cap(M, L)
     tables = 12 * (cap + (_lib.PAGE_MAX_FIGURES if figures else 0) + (_lib.PAGE_MAX_PANELS if panels else 0))
     search = ctypes.sizeof(_lib.SkewBlock) + 16 * n_ang + 16 if cs else 0
     return (ctypes.sizeof(_lib.PageResult) + ctypes.sizeof(_lib.TextBlock) + ctypes.sizeof(_lib.TextPage) + tables + search
-            + sum(_page_areas(L, M, cap, n_ang, stride, rules, figures, panels)) + 64)
+            + sum(_page_areas(L, M, cap, n_ang, stride, rules, figures, panels)) + 64 + (seal_bytes(w, h) if seals else 0))
 
 
 def rule_page_bytes(w, h):
@@ -2137,6 +2194,9 @@ def _check_page_options(page, what):
             want = f"{'0 or ' if zero else ''}an integer in [2, 32767]"
         if bad:
             raise ValueError(f"{what}: {knob} {v!r} is not {want} on a page with skew None")
+    v = page.seal_size
+    if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 8 <= v <= 4096 or page.skew is not None):
+        raise ValueError(f"{what}: seal_size {v!r} is not an integer in [8, 4096] on a page with skew None")
 
 
 def find_blocks(pages, scores=False):
@@ -2168,6 +2228,10 @@ def find_blocks(pages, scores=False):
     ink: a fill with runs of at least rule_length is no panel).  A call with such a page issues 2 more launches whatever the
     number of pages; its records gain panel_size and n_panels, and out ends, after the figure tables, with each such page's
     table of _lib.PAGE_MAX_PANELS mn_page_node panels, in the order of the pages.
+    seal_size (DESIGN.md 7b, "Seals"): None, or on a page with skew None an integer in [8, 4096]: the page's seals are found
+    (mn_find_seals_u8's 6 launches for all such pages of the call, before the layout) and its layout runs on its layout copy,
+    the crop with the seals' own ink set to paper.  out then starts with each such page's mn_seal_table, in the order of the
+    pages (seal_tables reads them back).
     A page without one of these options gets the tables of a call without it."""
     global LAUNCHES
     dev = _check_items(pages, "find_blocks", "page")
@@ -2184,7 +2248,7 @@ def find_blocks(pages, scores=False):
         _check_page_options(p, what)
         opts = (p.rule_length is not None, p.figure_size is not None, p.panel_size is not None)   # rules, figures, panels
         L, M, stride = skew_page_frame(bw, bh, p.vertical, cs)
-        need += page_bytes(bw, bh, p.vertical, cs if skewed else None, *opts)
+        need += page_bytes(bw, bh, p.vertical, cs if skewed else None, *opts, seals=p.seal_size is not None)
         if max(L, M) > 32767:
             raise ValueError(f"{what}: a frame side of {max(L, M)} exceeds 32767")
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
@@ -2197,24 +2261,39 @@ def find_blocks(pages, scores=False):
     if need > PAGE_MAX_WORK:
         raise ValueError(f"find_blocks: the pages need more than the {PAGE_MAX_WORK} bytes of work memory a call may use")
     tab, t_offs = _angle_tables(tables) if skewed else (b"", [0] * n)
-    pack = _Pack()                  # records, tables and the skew records, which come back with the results in one copy; then
-    pack.area(n * bsz)              # the results, leaves, figure and panel tables and each page's work, which the call zeroes
-    pg, t_off = pack.area(n * psz), pack.area(len(tab))
+    sealed = [i for i, p in enumerate(pages) if p.seal_size is not None]
+    m, spsz, tsz = len(sealed), ctypes.sizeof(_lib.SealPage), ctypes.sizeof(_lib.SealTable)
+    pack = _Pack()                  # records, tables, the seal tables and the skew records, which come back with the results in
+    pack.area(n * bsz)              # one copy; then the results, leaves, figure and panel tables and each page's work, which
+    pg, t_off = pack.area(n * psz), pack.area(len(tab))     # the call zeroes; then the seal pages' cells and layout copies
+    if sealed:
+        sp = pack.area(m * spsz, 16)
+        pack.area(m * tsz, 16)
     pack.area(n * ssz)
     out0 = pack.area(n * rsz, 16)
-    sk0 = out0 - n * ssz            # the skew records end where the results begin
+    sk0 = out0 - n * ssz            # the skew records end where the results begin, and the seal tables where they begin
+    st0 = sk0 - m * tsz
     leaves = [pack.area(12 * d[4]) for d in dims]
     figs = [pack.area(12 * _lib.PAGE_MAX_FIGURES) if d[8][1] else None for d in dims]
     pans = [pack.area(12 * _lib.PAGE_MAX_PANELS) if d[8][2] else None for d in dims]
     out1 = pack.end
     work = [[pack.area(a[0], 16)] + [pack.area(s) for s in a[1:]] for a in areas]
+    w_end = pack.end
+    scells = {i: [pack.area(a, 16) for a in _seal_areas(dims[i][2], dims[i][3])] for i in sealed}
     base = pack.alloc(dev)
-    blocks, srecs, recs, views, tiles = [], [], [], [], 0
+    blocks, srecs, recs, views, tiles, seal_recs, stiles, ctiles = [], [], [], [], 0, [], 0, 0
     for i, (p, (x0, y0, bw, bh, cap, M, n_ang, stride, (rules, figures, panels)), wk, lv, f, pn, t) in \
             enumerate(zip(pages, dims, work, leaves, figs, pans, t_offs)):
         sc, hist, lines, bits, lists, counts, prof, rbits, fbits, pbits = (base + o for o in wk)
-        tb = _lib.TextBlock(p.img.data_ptr(), p.img.stride(0), x0, y0, bw, bh, int(bool(p.vertical)), p.polarity, 0, 0, 0, 0,
-                            hist, 0, 0, lines)
+        src, pitch = p.img.data_ptr(), p.img.stride(0)
+        if i in scells:             # the page's layout reads its copy through its own crop offsets
+            copy, label, box, cand = (base + o for o in scells[i])
+            seal_recs.append(_lib.SealPage(_lib.TextBlock(src, pitch, x0, y0, bw, bh), copy, label, box, cand,
+                                           base + st0 + len(seal_recs) * tsz, p.seal_size))
+            src, pitch = (copy - y0 * 3 * bw - 3 * x0) % (1 << 64), 3 * bw
+            stiles = max(stiles, -(-bw // 32) * -(-bh // 32))
+            ctiles = max(ctiles, -(-bw // (4 * 32)) * -(-bh // (4 * 8)))
+        tb = _lib.TextBlock(src, pitch, x0, y0, bw, bh, int(bool(p.vertical)), p.polarity, 0, 0, 0, 0, hist, 0, 0, lines)
         blocks.append(tb)
         if skewed:
             srecs.append(_skew_block(tb, base + t_off + 16 * t, sc, prof, n_ang, stride))
@@ -2227,15 +2306,20 @@ def find_blocks(pages, scores=False):
         views.append(pack.buf[wk[0]:wk[0] + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
     buf = pack.upload((0, bytes((_lib.TextBlock * n)(*blocks))), (pg, bytes((_lib.TextPage * n)(*recs))), (t_off, tab),
+                      *(((sp, bytes((_lib.SealPage * m)(*seal_recs))),) if sealed else ()),
                       (sk0, bytes((_lib.SkewBlock * len(srecs))(*srecs))))
+    if sealed:
+        _lib.check(_lib.load().mn_find_seals_u8(base + sp, m, stiles, ctiles, base + st0, m * tsz, _stream()), "mn_find_seals_u8")
+        LAUNCHES += 6
     ruled, figured, directed, paneled = (any(p.rule_length is not None for p in pages), any(f is not None for f in figs),
                                          any(p.directions for p in pages), any(pn is not None for pn in pans))
     flags = ((_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0) | (_lib.PAGE_DIRECTIONS if directed else 0)
              | (_lib.PAGE_PANELS if paneled else 0))
     entry, head = ("mn_find_blocks_skewed_u8", (base, base + sk0)) if skewed else ("mn_find_blocks_u8", (base,))
-    _lib.check(getattr(_lib.load(), entry)(*head, base + pg, n, tiles, flags, base + out0, len(buf) - out0, _stream()), entry)
+    w_bytes = (w_end if sealed else len(buf)) - out0
+    _lib.check(getattr(_lib.load(), entry)(*head, base + pg, n, tiles, flags, base + out0, w_bytes, _stream()), entry)
     LAUNCHES += (7 if skewed else 5) + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed + 2 * paneled
-    res = buf[sk0:out1], [d[4] for d in dims]
+    res = buf[st0:out1], [d[4] for d in dims]
     return res + (views,) if scores else res
 
 
@@ -2246,6 +2330,7 @@ def page_tables(host, pages, caps):
     unless the page has a figure_size, panels None unless it has a panel_size."""
     sdt, rdt, ndt = skew_block_dtype(), page_result_dtype(), page_node_dtype()
     n = len(pages)
+    host = host[ctypes.sizeof(_lib.SealTable) * sum(p.seal_size is not None for p in pages):]
     o = n * sdt.itemsize if any(p.skew is not None for p in pages) else 0
     skews = host[:o].view(sdt) if o else [None] * n
     res = host[o:o + n * rdt.itemsize].view(rdt)
@@ -2261,6 +2346,22 @@ def page_tables(host, pages, caps):
             pans, t = nodes[t:t + _lib.PAGE_MAX_PANELS][:int(r["n_panels"])], t + _lib.PAGE_MAX_PANELS
         out.append((sk, r, nodes[l0:l0 + cap][:int(r["n_leaves"])], figs, pans))
     return out
+
+
+def seal_tables(host, pages):
+    """Per page of a find_blocks call, the numpy view of its mn_seal_table in ``host`` (seal_table_dtype()), or None for a page
+    without seal_size."""
+    tdt = seal_table_dtype()
+    tabs = iter(host[:tdt.itemsize * sum(p.seal_size is not None for p in pages)].view(tdt))
+    return [None if p.seal_size is None else next(tabs) for p in pages]
+
+
+def seal_table_dtype():
+    """numpy view of an mn_seal_table record."""
+    import numpy as np
+    seal = np.dtype([(f, "<i4") for f, _ in _lib.Seal._fields_[:-1]] + [("pad", "<i4", (3,))])
+    return np.dtype([("error", "<i4"), ("n_cand", "<i4"), ("n_seals", "<i4"), ("pad", "<i4"),
+                     ("seal", seal, (_lib.PAGE_MAX_SEALS,))])
 
 
 def page_result_dtype():

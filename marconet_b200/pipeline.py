@@ -1214,30 +1214,55 @@ class CurvedRegion(NamedTuple):
     bottom: tuple
 
     @classmethod
-    def from_arc(cls, cx, cy, r_top, r_bottom, start, end):
+    def from_arc(cls, cx, cy, r_top, r_bottom, start, end, segments=None):
         """Text on a circle centred at (cx, cy): the top edge at radius r_top, the bottom edge at r_bottom, read from angle
         ``start`` to ``end`` (degrees, counter-clockwise on screen: a point is (cx + r cos a, cy - r sin a)), 0 < |end - start| <
         360.  The top of a seal read left to right is start 150, end 30, r_top > r_bottom.  The arc is split into
         k = ceil(|end - start| / 90) equal segments whose handles lie along the tangents at r (4/3) tan(phi/4), phi the segment's
-        signed span."""
+        signed span.  A radius may also be a pair (rx, ry), for an oval seal: a point is then (cx + rx cos a, cy - ry sin a) and
+        its handles are scaled alike, the affine image of the circle's curve; r means (r, r) and gives the same points.
+        ``segments``: k in place of ceil(|end - start| / 90), an integer in [that, 8] (arc_segments gives one that restore_regions
+        accepts for an oval)."""
         span = float(end) - float(start)
         if not 0 < abs(span) < 360:
             raise ValueError(f"from_arc: the span end - start = {span:g} degrees must satisfy 0 < |span| < 360")
         k = math.ceil(abs(span) / 90)
+        if segments is not None:
+            if isinstance(segments, bool) or not isinstance(segments, int) or not k <= segments <= 8:
+                raise ValueError(f"from_arc: segments must be an integer in [{k}, 8], got {segments!r}")
+            k = segments
         h = 4 / 3 * math.tan(math.radians(span / k) / 4)
 
         def curve(r):
+            rx, ry = (float(r[0]), float(r[1])) if isinstance(r, (tuple, list)) else (float(r), float(r))
             pts = []
             for m in range(k):
                 a0, a1 = math.radians(start + span * m / k), math.radians(start + span * (m + 1) / k)
-                p0 = (cx + r * math.cos(a0), cy - r * math.sin(a0))
-                p3 = (cx + r * math.cos(a1), cy - r * math.sin(a1))
+                p0 = (cx + rx * math.cos(a0), cy - ry * math.sin(a0))
+                p3 = (cx + rx * math.cos(a1), cy - ry * math.sin(a1))
                 if m == 0:
                     pts.append(p0)
-                pts += [(p0[0] - h * r * math.sin(a0), p0[1] - h * r * math.cos(a0)),       # p0 + h dP/da(a0)
-                        (p3[0] + h * r * math.sin(a1), p3[1] + h * r * math.cos(a1)), p3]    # p3 - h dP/da(a1)
+                pts += [(p0[0] - h * rx * math.sin(a0), p0[1] - h * ry * math.cos(a0)),       # p0 + h dP/da(a0)
+                        (p3[0] + h * rx * math.sin(a1), p3[1] + h * ry * math.cos(a1)), p3]    # p3 - h dP/da(a1)
             return tuple(pts)
-        return cls(curve(float(r_top)), curve(float(r_bottom)))
+        return cls(curve(r_top), curve(r_bottom))
+
+
+def arc_segments(rx, ry, start, end, max_turn=80.0):
+    """The fewest equal segments k >= ceil(|end - start| / 90) of the arc from ``start`` to ``end`` (degrees) on the ellipse of
+    semi-axes (rx, ry) within each of which its ruling direction (rx cos a, -ry sin a) turns by at most ``max_turn`` degrees, or
+    None when 8 segments are not enough.  On a circle the ruling turns as a does; on an oval it turns faster near the ends of
+    the long axis, and restore_regions refuses a segment whose ruling turns by more than 90 degrees."""
+    def phi(a):                                         # the ruling's angle, unwrapped: it lies within 90 degrees of a
+        a = math.radians(a)
+        p = math.atan2(ry * math.sin(a), rx * math.cos(a))
+        return p + 2 * math.pi * round((a - p) / (2 * math.pi))
+    span = float(end) - float(start)
+    for k in range(math.ceil(abs(span) / 90), 9):
+        edges = [phi(start + span * m / k) for m in range(k + 1)]
+        if all(abs(b - a) <= math.radians(max_turn) for a, b in zip(edges, edges[1:])):
+            return k
+    return None
 
 
 class CurvedMaps(NamedTuple):
@@ -1554,7 +1579,11 @@ class TextBlock(NamedTuple):
     rectified crop R (quad_maps' w_r x h_r) and come back as QuadRegions; ``rect`` is then the quad's pixel box (build the
     block with from_quad), ``skew`` is None and ``window``, if given, is an integer rectangle (x0, y0, x1, y1) of R.
     ``curve`` (DESIGN.md 7b, "Curled blocks"): None, or "auto" to trace each line of a curled horizontal block across ``strips``
-    column strips (a positive integer, only with "auto"; default clamp(w // 48, 1, 32)) and return it as a CurvedRegion."""
+    column strips (a positive integer, only with "auto"; default clamp(w // 48, 1, 32)) and return it as a CurvedRegion.
+    ``seals`` (DESIGN.md 7b, "Seals"): a tuple of integer seal boxes (x0, y0, x1, y1) in image pixels, sides in [1, 4096],
+    inside the image, at most 64.  Inside each box's inscribed ellipse, seal-coloured pixels (max(c) - min(c) >= 64) are paper
+    when the block is split into lines; black text under a stamp stays ink.  Only on a level block: no skew, curve, quad or
+    window, and no polarity "light".  find_blocks gives each block of a TextPage(seals="auto") the seals that meet it."""
     rect: object
     direction: str = "horizontal"
     min_ink: object = None
@@ -1567,6 +1596,7 @@ class TextBlock(NamedTuple):
     quad: object = None
     curve: object = None
     strips: object = None
+    seals: tuple = ()
 
     @classmethod
     def from_quad(cls, quad, shape=None, **kw):
@@ -1607,6 +1637,7 @@ def _check_block(blk, H, W, name):
         if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 1 <= v < 2 ** 31):
             raise ValueError(f"{name}: {what} must be a positive integer, got {v!r}")
     _check_curve(blk.curve, blk.strips, blk, x1 - x0, name)
+    _check_seals(blk, H, W, name)
     sk, ms = blk.skew, blk.max_skew
     auto = isinstance(sk, str) and sk == "auto"
     if not (sk is None or auto or (isinstance(sk, numbers.Real) and not isinstance(sk, bool) and math.isfinite(sk)
@@ -1650,6 +1681,32 @@ def _check_block(blk, H, W, name):
     return x0, y0, x1, y1
 
 
+def _check_seals(blk, H, W, name):
+    """The seal boxes of a TextBlock ``blk`` of an H x W image, validated (DESIGN.md 7b, "Seals").  Raises ValueError naming
+    ``name``."""
+    from . import ops
+    try:
+        boxes = tuple(blk.seals)
+        if not all(len(b) == 4 and all(isinstance(v, numbers.Integral) and not isinstance(v, bool) for v in b) for b in boxes):
+            raise ValueError
+    except (TypeError, ValueError):
+        raise ValueError(f"{name}: seals must be a tuple of integer boxes (x0, y0, x1, y1), got {blk.seals!r}") from None
+    if not boxes:
+        return
+    if len(boxes) > ops._lib.PAGE_MAX_SEALS:
+        raise ValueError(f"{name}: {len(boxes)} seals exceed the {ops._lib.PAGE_MAX_SEALS} a text block may hold")
+    for b in boxes:
+        x0, y0, x1, y1 = b
+        if not (0 <= x0 < x1 <= W and 0 <= y0 < y1 <= H) or max(x1 - x0, y1 - y0) > 4096:
+            raise ValueError(f"{name}: seal box {tuple(b)} is empty, outside the {W}x{H} image or has a side over 4096")
+    for what in ("skew", "curve", "quad", "window"):
+        if getattr(blk, what) is not None:
+            raise ValueError(f"{name}: seals and {what} are both given (a sealed block is level and flat: flatten a tilted, "
+                             f"curled or photographed page with flatten_pages first)")
+    if blk.polarity == "light":
+        raise ValueError(f"{name}: seals are given for a block of polarity 'light' (seals are dark stamps on paper)")
+
+
 def _check_curve(curve, strips, item, w, name):
     """The curve knobs of a TextBlock or TextPage ``item`` of width w, validated (DESIGN.md 7b, "Curled blocks").  Raises
     ValueError naming ``name``."""
@@ -1675,17 +1732,22 @@ def _check_curve(curve, strips, item, w, name):
                          f"{ops.CURVE_MIN_STRIP} pixels wide")
 
 
-def _check_curve_work(items, names):
-    """Refuse, before any launch, curled blocks (image index, TextBlock, rect) whose work memory, added up in order, passes the
-    limit of one call: the error names the block that passes it."""
+def _check_block_work(items, names):
+    """Refuse, before any launch, curled blocks (image index, TextBlock, rect) whose work memory, or sealed blocks whose layout
+    copies, added up in order, pass the limit of one call: the error names the block that passes it."""
     from . import ops
-    total = 0
+    total = copies = 0
     for (_, blk, rect), name in zip(items, names):
         if blk.curve is not None:
             total += ops.curve_block_bytes(rect[2] - rect[0], rect[3] - rect[1], blk.strips)
             if total > ops.CURVE_MAX_WORK:
                 raise ValueError(f"{name}: the call's curled blocks up to this one need {total} bytes of work memory, over the "
                                  f"{ops.CURVE_MAX_WORK} a call may use (split the call)")
+        if blk.seals:
+            copies += ops.seal_block_bytes(rect[2] - rect[0], rect[3] - rect[1])
+            if copies > ops.PAGE_MAX_WORK:
+                raise ValueError(f"{name}: the call's sealed blocks up to this one need {copies} bytes of layout copies, over the "
+                                 f"{ops.PAGE_MAX_WORK} a call may use (split the call)")
 
 
 def _check_quad(quad, skew, H, W, name):
@@ -1757,7 +1819,7 @@ def _find_lines(dimg, items, rq=None):
     parts = []
     if plain:
         parts.append(ops.find_lines([(*src(i, blk, rect), blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap,
-                                      blk.min_height, blk.skew, blk.max_skew) for i, blk, rect in plain]))
+                                      blk.min_height, blk.skew, blk.max_skew, blk.seals) for i, blk, rect in plain]))
     if wins:
         parts.append(ops.find_lines_window([(dimg[i], rect, blk.direction == "vertical", _INK[blk.polarity], blk.min_ink, blk.gap,
                                              blk.min_height, blk.skew, blk.window) for i, blk, rect in wins]))
@@ -1955,7 +2017,7 @@ def find_lines(images, blocks):
             if not isinstance(blk, TextBlock):
                 raise ValueError(f"{names[-1]}: expected a TextBlock, got {blk!r}")
             items.append((i, blk, _check_block(blk, im.shape[0], im.shape[1], names[-1])))
-    _check_curve_work(items, names)
+    _check_block_work(items, names)
     out = [[] for _ in imgs]
     if not items:
         return out
@@ -2059,8 +2121,14 @@ def _expand_blocks(regions, labels, boxes, blocks, found, skip_invalid, shapes=N
     return _splice(regions, labels, boxes, blocks, found, expand)
 
 
+def _n_arcs(res):
+    """The number of seal arcs a page's find_blocks result ``res`` puts before its blocks (0 for any other entry)."""
+    return sum(s["region"] is not None for s in res.get("seals", ())) if isinstance(res, dict) else 0
+
+
 def _regroup(out, layout):
-    """restore_regions' result with each block's (page's) child entries gathered into its own entry, in place."""
+    """restore_regions' result with each block's (page's) child entries gathered into its own entry, in place; a page's seal
+    arcs go into its ``seal_regions``."""
     for img, lay in zip(out, layout):
         flat, o, img["regions"] = img["regions"], 0, []
         for e in lay:
@@ -2069,7 +2137,9 @@ def _regroup(out, layout):
                 o += 1
                 continue
             res, k = e
-            img["regions"].append(res if "error" in res else dict(res, regions=flat[o:o + k]))
+            a = _n_arcs(res) if "seals" in res else 0
+            extra = dict(seal_regions=flat[o:o + a]) if "seals" in res else {}
+            img["regions"].append(res if "error" in res else dict(res, **extra, regions=flat[o + a:o + k]))
             o += k
 
 
@@ -2104,7 +2174,13 @@ class TextPage(NamedTuple):
     than half of their greys within 8 of the modal grey) are panels.  A panel's inside is cut as text of the opposite
     polarity inside a rule outline, and its blocks are TextBlocks of that polarity, restored line by line.  A panel is never a
     figure.  With ``rules``, a fill whose rows or columns are at least ``rule_length`` long is rules, not a panel: give a
-    ``rule_length`` above the panels' sides.  Not with skew or curve: flatten such a page with flatten_pages first."""
+    ``rule_length`` above the panels' sides.  Not with skew or curve: flatten such a page with flatten_pages first.
+    ``seals`` (DESIGN.md 7b, "Seals"): None, or "auto" for a page with round or oval stamps (red or blue seals): components of
+    seal-coloured 4 x 4 cells whose box has sides in [``seal_size``, 4096] and at most a 3:2 ratio, with a ring of colour along
+    its inscribed ellipse, are seals.  Their own ink is taken out of the layout (black text under a stamp stays ink), each
+    block gets the seals that meet it, and the text along a seal's upper arc is found and restored as a CurvedRegion.
+    ``seal_size`` is an integer in [8, 4096], default max(24, min(w, h) // 12) of the crop, a heuristic.  Only on a level,
+    flat page of dark ink: not with skew, curve or quad (flatten such a page with flatten_pages first) or polarity "light"."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
@@ -2121,6 +2197,8 @@ class TextPage(NamedTuple):
     block_direction: object = None
     panels: object = None
     panel_size: object = None
+    seals: object = None
+    seal_size: object = None
 
 
 def _check_page(pg, H, W, name):
@@ -2139,6 +2217,20 @@ def _check_page(pg, H, W, name):
             if on is not None and getattr(pg, what) is not None:
                 raise ValueError(f"{name}: {switch} and {what} are both given (a page with {switch}='auto' is level and flat: "
                                  f"flatten a tilted or curled page with flatten_pages first)")
+    if pg.seals is not None and not (isinstance(pg.seals, str) and pg.seals == "auto"):
+        raise ValueError(f"{name}: seals must be None or 'auto', got {pg.seals!r}")
+    v = pg.seal_size
+    if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 8 <= v <= 4096):
+        raise ValueError(f"{name}: seal_size must be an integer in [8, 4096], got {v!r}")
+    if v is not None and pg.seals is None:
+        raise ValueError(f"{name}: seal_size is given, but seals is None, not 'auto'")
+    if pg.seals is not None:
+        for what in ("skew", "curve", "quad"):
+            if getattr(pg, what) is not None:
+                raise ValueError(f"{name}: seals and {what} are both given (a page with seals='auto' is level and flat: "
+                                 f"flatten a tilted, curled or photographed page with flatten_pages first)")
+        if pg.polarity == "light":
+            raise ValueError(f"{name}: seals are asked for on a page of polarity 'light' (seals are dark stamps on paper)")
     if pg.quad is not None:
         if pg.rect is not None:
             raise ValueError(f"{name}: rect and quad are both given (a page in perspective is its quad: give rect=None)")
@@ -2188,7 +2280,7 @@ def _page_bytes(pg, rect, skewed):
         return 3 * w_r * h_r + _page_bytes(pg._replace(quad=None), (0, 0, w_r, h_r), skewed)
     cs = (_page_table(pg) if pg.skew is not None else [(1.0, 0.0)]) if skewed else None
     return ops.page_bytes(w, h, pg.direction == "vertical", cs, rules=pg.rules is not None, figures=pg.figures is not None,
-                          panels=pg.panels is not None)
+                          panels=pg.panels is not None, seals=pg.seals is not None)
 
 
 def _check_page_work(items, extra=0):
@@ -2250,6 +2342,54 @@ def _find_pages(dimg, items, keys=()):
     return [it if isinstance(it, str) else next(found) for it in items], rq
 
 
+def seal_size(w, h):
+    """The default seal size of a w x h page crop (DESIGN.md 7b, "Seals"): max(24, min(w, h) // 12).  A heuristic: a stamp is
+    rarely under a twelfth of the page's shorter side."""
+    return max(24, min(w, h) // 12)
+
+
+_SEAL_WHY = {1: "no arc text", 2: "no gap in the arc text", 3: "the arc text spans under 45 degrees"}
+
+
+def _seal_entries(stab, X0, Y0, shape):
+    """The seals of a page's mn_seal_table, in image coordinates: per seal dict(box, ring, band, arc, region[, why]).  A seal's
+    arc is split into arc_segments' segments, and its region is kept only when restore_regions' curved rules accept it on the
+    image of ``shape`` (H, W); otherwise arc and region are None and why says why."""
+    out = []
+    for s in stab["seal"][:min(int(stab["n_cand"]), len(stab["seal"]))]:
+        if not s["found"]:
+            continue
+        x0, y0, x1, y1 = (int(s[f]) for f in ("x0", "y0", "x1", "y1"))
+        box = (X0 + x0, Y0 + y0, X0 + x1, Y0 + y1)
+        e = dict(box=box, ring=int(s["ring"]), band=None if s["k_top"] < 0 else (int(s["k_bottom"]), int(s["k_top"])), arc=None,
+                 region=None)
+        if s["why"]:
+            e["why"] = _SEAL_WHY[int(s["why"])]
+        else:
+            start = 5 * int(s["g0"])
+            end = start - 5 * (72 - int(s["n_gap"]))
+            a, b = (x1 - x0) / 2, (y1 - y0) / 2
+            kb, kt = e["band"]
+            k = arc_segments(a, b, start, end)
+            try:
+                if k is None:
+                    raise ValueError(f"seal: its arc of {start - end} degrees needs more than 8 segments")
+                reg = CurvedRegion.from_arc((box[0] + box[2]) / 2, (box[1] + box[3]) / 2, ((kt + 1) / 32 * a, (kt + 1) / 32 * b),
+                                            (kb / 32 * a, kb / 32 * b), start, end, segments=k)
+                _plan_curved(reg, *shape, 1, "seal")
+                e.update(arc=(start, end), region=reg)
+            except ValueError as err:
+                e["why"] = f"the arc region is rejected ({str(err).split(': ', 1)[-1]})"
+        out.append(e)
+    return out
+
+
+def _meeting(seals, rect):
+    """The boxes of ``seals`` that meet the rectangle ``rect`` (share a pixel with it), as a tuple."""
+    x0, y0, x1, y1 = rect
+    return tuple(s["box"] for s in seals if s["box"][0] < x1 and x0 < s["box"][2] and s["box"][1] < y1 and y0 < s["box"][3])
+
+
 def _node_rects(nodes, x0=0, y0=0):
     """The rectangles of mn_page_node entries, shifted by (x0, y0)."""
     return [(x0 + int(q["x0"]), y0 + int(q["y0"]), x0 + int(q["x1"]), y0 + int(q["y1"])) for q in nodes]
@@ -2277,13 +2417,19 @@ def _find_blocks(dimg, items, rq=None):
                             rule_length=rl,
                             figure_size=None if pg.figures is None else pg.figure_size or 0,
                             directions=pg.block_direction is not None,
-                            panel_size=None if pg.panels is None else pg.panel_size or 0)
+                            panel_size=None if pg.panels is None else pg.panel_size or 0,
+                            seal_size=None if pg.seals is None else pg.seal_size or seal_size(crop[2] - crop[0], crop[3] - crop[1]))
     pages = [page(*it) for it in items]
     res_t, caps = ops.find_blocks(pages)
+    host = _to_host(res_t).numpy()
+    stabs = ops.seal_tables(host, pages)
     limits = {lib.PAGE_ERR_BLOCKS: ("blocks", lib.PAGE_MAX_BLOCKS), lib.PAGE_ERR_FIGURES: ("figures", lib.PAGE_MAX_FIGURES),
               lib.PAGE_ERR_PANELS: ("panels", lib.PAGE_MAX_PANELS)}
     out = []
-    for (i, pg, rect), p, (sk, r, leaves, figs, pans) in zip(items, pages, ops.page_tables(_to_host(res_t).numpy(), pages, caps)):
+    for (i, pg, rect), p, (sk, r, leaves, figs, pans), stab in zip(items, pages, ops.page_tables(host, pages, caps), stabs):
+        if stab is not None and stab["error"]:
+            out.append(f"{int(stab['n_cand'])} seal candidates exceed the {lib.PAGE_MAX_SEALS} a text page may hold")
+            continue
         if r["error"] == lib.PAGE_ERR_NODES:
             out.append(f"more than {lib.PAGE_MAX_NODES} nodes in one level of the XY-cut")
             continue
@@ -2334,8 +2480,11 @@ def _find_blocks(dimg, items, rq=None):
                                for b, d, pl in zip(blocks, dirs, pols)],
                        rejected=rejected, quad=_quad_key(i, pg.quad)[1], size=tuple(p.rect[2:]))
         elif pg.skew is None:
-            res.update(blocks=[TextBlock(b, d, polarity=pl, curve=pg.curve) for b, d, pl in zip(blocks, dirs, pols)],
-                       rejected=rejected)
+            seals = [] if stab is None else _seal_entries(stab, X0, Y0, dimg[i].shape[:2])
+            res.update(blocks=[TextBlock(b, d, polarity=pl, curve=pg.curve, seals=_meeting(seals, b))
+                               for b, d, pl in zip(blocks, dirs, pols)], rejected=rejected)
+            if stab is not None:
+                res.update(seal_size=p.seal_size, seals=seals)
         else:
             res["skew"] = _skew_used(pg, sk)
             res["blocks"] = [TextBlock(tuple(rect), pg.direction, polarity=pg.polarity, skew=res["skew"], window=b) if tilted
@@ -2388,7 +2537,13 @@ def find_blocks(images, pages):
     to the page's ink; the others keep the page's.  Its dict gains ``panel_size`` (the p used, 0 without a text size) and
     ``panels``, their rectangles in leaf order (as ``figures``).  A page over 1024 panels raises, as one over its figure
     limit.  With ``rules="auto"`` the rules are taken out of the ink first, so a fill whose rows or columns reach the rule
-    length is no panel: give a ``rule_length`` above the panels' sides."""
+    length is no panel: give a ``rule_length`` above the panels' sides.
+    A page with ``seals="auto"`` (DESIGN.md 7b, "Seals") has its stamps found on the device (6 more launches for all such pages
+    of the call, their tables back in the same copy) and is cut on its layout copy, in which the seals' own seal-coloured ink
+    is paper.  Its dict gains ``seal_size`` (the size used) and ``seals``, one dict per seal ordered by box (y0, then x0): box
+    (image pixels), ring (the sectors hit), band ((k_bottom, k_top) or None), arc ((start, end) in degrees or None), region
+    (the arc text's CurvedRegion or None) and, when arc is None, why.  Each of its blocks is TextBlock(..., seals=...) with the
+    boxes of the seals that meet it.  A page over 64 seal candidates raises, as one over its figure limit."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
@@ -2423,24 +2578,34 @@ def _plan_pages(shapes, regions, labels, boxes):
     return pages, stand_in
 
 
-def _expand_pages(regions, labels, boxes, pages, found, skip_invalid):
-    """The region, label and box lists with each text page replaced in place by its TextBlocks; the names of every TextBlock of
-    the new lists by (image, position); and per image the layout of its given regions: None for a region, [entry, k] for a page
-    of k blocks, entry its find_blocks result or dict(error=...) under ``skip_invalid`` for a page over a limit."""
+def _expand_pages(regions, labels, boxes, pages, found, skip_invalid, shapes, scale, feather):
+    """The region, label and box lists with each text page replaced in place by its seal arcs and TextBlocks; the names of every
+    TextBlock and seal arc of the new lists by (image, position); and per image the layout of its given regions: None for a
+    region, [entry, k] for a page of k arcs and blocks, entry its find_blocks result or dict(error=...) under ``skip_invalid``
+    for a page over a limit or with an arc plan_regions rejects on the image of ``shapes`` at ``scale`` and ``feather``."""
     def expand(i, r, res):
-        if not isinstance(res, str):
-            return res, res["blocks"]
-        err = f"image {i}, region {r} (a text page): {res}"
+        err = None if not isinstance(res, str) else f"image {i}, region {r} (a text page): {res}"
+        arcs = [] if err else [s["region"] for s in res.get("seals", ()) if s["region"] is not None]
+        for j, arc in enumerate(arcs):
+            try:
+                plan_regions([shapes[i]], [[arc]], None, None, scale, feather)
+            except ValueError as e:
+                err = f"image {i}, region {r} (a text page), seal {j}: {str(e).split(': ', 1)[-1]}"
+                break
+        if err is None:                                 # a page's seal arcs compose before its blocks
+            return res, arcs + res["blocks"]
         if not skip_invalid:
             raise ValueError(err)
         return dict(error=err), []
     regions, labels, boxes, layout = _splice(regions, labels, boxes, pages, found, expand)
     names = {}
     for i, lay in enumerate(layout):
-        at = [(r, k) for r, e in enumerate(lay) for k in ([None] if e is None else range(e[1]))]
+        at = [(r, k if e is None else k - _n_arcs(e[0])) for r, e in enumerate(lay) for k in ([None] if e is None else range(e[1]))]
         for o, (r, k) in enumerate(at):
-            if k is not None:
+            if k is not None and k >= 0:
                 names[(i, o)] = f"image {i}, region {r} (a text page), block {k}"
+            elif k is not None:                         # the arcs, seal 0 first
+                names[(i, o)] = f"image {i}, region {r} (a text page), seal {k + _n_arcs(lay[r][0])}"
             elif isinstance(regions[i][o], TextBlock):
                 names[(i, o)] = f"image {i}, region {r} (a text block)"
     return regions, labels, boxes, names, layout
@@ -2776,7 +2941,7 @@ def flatten_pages(images, pages, to_host=False):
                 bitems.append((("frame", k), blk._replace(curve="auto", strips=flat_strips(fp.strips, bw)), tuple(blk.rect)))
                 bnames.append(f"{names[k]}, block {b}")
                 bpage.append(k)
-        _check_curve_work(bitems, bnames)
+        _check_block_work(bitems, bnames)
         lines = {k: [] for k in search if items[k][1].curve is not None}
         for (_, blk, rect), name, k, r in zip(bitems, bnames, bpage, _find_lines(src, bitems) if bitems else []):
             if isinstance(r, str):
@@ -3053,13 +3218,16 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     block entry per block; a page over its node or block limit, or one of whose blocks fails, raises, or is dict(error=...)
     with ``skip_invalid``, and then none of its blocks is restored.  A quad page or block (DESIGN.md 7b, "Perspective pages")
     is laid out on its rectified crop (TextPage(quad="auto") after the device's corner search), every distinct quad of the call
-    warped in one launch, and gives QuadRegion lines; a page without a quad found is its error."""
+    warped in one launch, and gives QuadRegion lines; a page without a quad found is its error.  A page with
+    ``seals="auto"`` (DESIGN.md 7b, "Seals") puts the CurvedRegion of each seal's arc text in the region list before its
+    blocks, so where a printed line crosses a stamp the line's restoration is composed last; its entry's ``regions`` stays one
+    block entry per block and ``seal_regions`` holds one curved-region entry per arc.  The seal's centre keeps the background."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     shapes = [im.shape[:2] for im in imgs]
     text_pages, given = _plan_pages(shapes, regions, labels, boxes)
     blocks, stand_in = _plan_blocks(shapes, given if text_pages else regions, labels, boxes)
-    _check_curve_work([(i, blk, rect) for i, _, blk, rect in blocks], [f"image {i}, region {r} (a text block)"
+    _check_block_work([(i, blk, rect) for i, _, blk, rect in blocks], [f"image {i}, region {r} (a text block)"
                                                                        for i, r, _, _ in blocks])
     plan = plan_regions(shapes, stand_in if blocks or text_pages else regions, labels, boxes, scale, feather)
     feather = 2 * scale if feather is None else feather
@@ -3073,9 +3241,10 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
         if text_pages:                                   # every page's blocks take its place in the region list
             found, rq = _find_pages(dimg, [(i, pg, rect) for i, _, pg, rect in text_pages],
                                     [_quad_key(i, blk.quad) for i, _, blk, _ in blocks if blk.quad is not None])
-            regions, labels, boxes, names, page_layout = _expand_pages(regions, labels, boxes, text_pages, found, skip_invalid)
+            regions, labels, boxes, names, page_layout = _expand_pages(regions, labels, boxes, text_pages, found, skip_invalid,
+                                                                       shapes, scale, feather)
             blocks, _ = _plan_blocks(shapes, regions, labels, boxes)
-            _check_curve_work([(i, blk, rect) for i, _, blk, rect in blocks], [names[(i, r)] for i, r, _, _ in blocks])
+            _check_block_work([(i, blk, rect) for i, _, blk, rect in blocks], [names[(i, r)] for i, r, _, _ in blocks])
         elif any(blk.quad is not None for _, _, blk, _ in blocks):
             rq = _rectify(dimg, [_quad_key(i, blk.quad) for i, _, blk, _ in blocks if blk.quad is not None])
         if blocks:                                       # every block's lines take its place in the region list
