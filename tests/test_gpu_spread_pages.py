@@ -45,7 +45,11 @@ def _masks():
             notched(w, h, top=[(hi + 1, 40, 0), (hi, 20, 0), (100, 10, 1)], bottom=[(hi + 1, 30, 0), (hi, 6, 0)]),
             notched(1000, 60, top=[(500, 10, 1)], bottom=[(503, 9, 1)]),
             notched(1000, 60, top=[(500, 10, 1)], bottom=[(503, 10, 1)]),
-            notched(150, 50, top=[(75, 2, 1)], bottom=[(70, 2, 1)])]
+            notched(150, 50, top=[(75, 2, 1)], bottom=[(70, 2, 1)]),
+            notched(120, 60, top=[(60, 8, 1)], bottom=[(50, 5, 2)], pad=0),     # cols[w - 1] set and b(x) = h
+            *[notched(m, h, top=[(c + e, 40, 0), (c, 20, 0)], bottom=[(c + e, 30, 0), (c, 6, 0)])
+              for m in (201, 203) for c, e in ((-(-m // 4), -1), (m - -(-m // 4), 1))],    # tr.x - tl.x = 1, 3 mod 4
+            np.pad(np.ones((48, 1), bool), 6)]                                   # one column wide: none in range
 
 
 def test_device_spines_equal_the_twin_beside_other_pages():
