@@ -1070,6 +1070,65 @@ int mn_find_seals_u8(const mn_seal_page* pages, int n, long long max_tiles, long
                      long long work_bytes, void* stream);
 int mn_seal_layout_u8(const mn_seal_page* pages, int n, long long max_tiles, void* stream);
 
+/* Seal centre lines (DESIGN.md section 7b, "Seal centre lines"): the horizontal text across a found seal's centre, and the
+ * seal's turn.  Per found seal j of a page's mn_seal_table, with its box, A x B, and histograms as mn_find_seals_u8 defines them:
+ *   head: with a band whose k_top >= MN_SEAL_HEAD_MIN_K, sec[s] = the ink of bins [k_top - MN_SEAL_HEAD_BINS + 1, k_top] in sector s, and (g0, n)
+ *   its gap by the arc rule; why = MN_SEAL_NO_GAP / MN_SEAL_SHORT / 0 as for the arc.  The turn t = 2 g0 + n - 108 in
+ *   2.5-degree steps, normalised to (-72, 72], counter-clockwise on screen; t = 0 when why != 0.  A seal without such a
+ *   band gets why = MN_SEAL_NO_BAND, t = 0, no gap and no band (-1).
+ *   arc band: the arc sectors are all but [g0, g0 + n); ink'_k their ink in bin k.  From k = k_top inward, k_bottom is the last
+ *   bin of the run with 32 * 72 * ink'_k >= area_k (72 - n), down to MN_SEAL_BAND_MIN_K; k_top is always in it.
+ *   interior: the seal-coloured pixels at k < k_in, k_in = k_bottom, and those at k < k_gap = max(k_bottom, k_top -
+ *   MN_SEAL_HEAD_BINS + 1) in the gap's sectors less MN_SEAL_GAP_MARGIN at each end, (s - g0 - margin) mod 72 < n - 2 margin.
+ *   Without a band, k_in = k_gap = the first bin inside the ring's edge of the band walk (gap_top; 0 when negative).
+ *   rows: a pixel's (X, Y) turned by -t with (c, s) = MN_SEAL_TURNS[t mod 36] turned by (t mod 144) / 36 quarter turns
+ *   ((c, s) -> (-s, c)): u = (X c - Y s) >> 21, v = (X s + Y c) >> 21 (floor).  Per row v, the min and max u of its ink.
+ *   lines: runs of ink rows whose gaps are under MN_SEAL_LINE_GAP rows; a run h rows high and w = u_max - u_min + 1 wide is a
+ *   line when h >= max(MN_SEAL_LINE_MIN_H, (A + B) / MN_SEAL_LINE_H_DIV) and w >= MN_SEAL_LINE_RATIO h.  Its box (u0, v0, u1,
+ *   v1), end exclusive, is padded by p = max(MN_SEAL_LINE_PAD, h / MN_SEAL_LINE_PAD_DIV) and clipped to [-R - 1, R + 1],
+ *   R = k_gap max(A, B) / 64.  n_found counts the lines, the first MN_SEAL_MAX_LINES from the top are kept.
+ * mn_find_seal_lines_u8 issues 1 launch: one CTA per seal slot (MN_PAGE_MAX_SEALS per page) writes the slot's record of
+ * page->lines.  It rebuilds the seal's histograms and the row extents (at most MN_SEAL_MAX_SIDE + 4 rows) in shared memory.  A
+ * slot that is no found seal, and every slot of a table with an error, gets a zero record.  It reads the tables
+ * mn_find_seals_u8 wrote before it on the same stream.  pages: DEVICE array. */
+#define MN_SEAL_HEAD_BINS 4
+#define MN_SEAL_HEAD_MIN_K 16
+#define MN_SEAL_GAP_MARGIN 2
+#define MN_SEAL_LINE_GAP 3
+#define MN_SEAL_LINE_MIN_H 4
+#define MN_SEAL_LINE_H_DIV 64
+#define MN_SEAL_LINE_RATIO 2
+#define MN_SEAL_LINE_PAD 2
+#define MN_SEAL_LINE_PAD_DIV 8
+#define MN_SEAL_MAX_LINES 4
+#define MN_SEAL_TURN_STEPS 144
+/* (round(2^20 cos 2.5 j), round(2^20 sin 2.5 j)) for j < 36 */
+#define MN_SEAL_TURNS {{1048576, 0}, {1047578, 45738}, {1044586, 91389}, {1039605, 136867}, {1032646, 182083}, {1023721, 226953}, \
+    {1012847, 271391}, {1000045, 315313}, {985339, 358634}, {968758, 401273}, {950333, 443147}, {930098, 484179}, \
+    {908093, 524288}, {884360, 563399}, {858943, 601438}, {831891, 638333}, {803256, 674012}, {773091, 708408}, \
+    {741455, 741455}, {708408, 773091}, {674012, 803256}, {638333, 831891}, {601438, 858943}, {563399, 884360}, \
+    {524288, 908093}, {484179, 930098}, {443147, 950333}, {401273, 968758}, {358634, 985339}, {315313, 1000045}, \
+    {271391, 1012847}, {226953, 1023721}, {182083, 1032646}, {136867, 1039605}, {91389, 1044586}, {45738, 1047578}}
+typedef struct {
+    int32_t turn;               /* t, 2.5-degree steps */
+    int32_t g0, n_gap;          /* the head gap, or -1 */
+    int32_t k_bottom, k_top;    /* the arc band, or -1 */
+    int32_t why;                /* 0, MN_SEAL_NO_BAND, MN_SEAL_NO_GAP or MN_SEAL_SHORT */
+    int32_t k_in, k_gap;        /* the interior's bins, and in the head gap */
+    int32_t n_found, n_lines;   /* the lines found, and kept */
+    int32_t pad[2];
+    int32_t box[MN_SEAL_MAX_LINES][4];  /* (u0, v0, u1, v1) in the stamp frame, pixels from the box centre */
+} mn_seal_lines;
+typedef struct {
+    mn_seal_lines seal[MN_PAGE_MAX_SEALS];   /* slot j describes the table's seal[j] */
+} mn_seal_line_table;
+typedef struct {
+    mn_text_block b;            /* the crop record, as in the page's mn_seal_page */
+    const mn_seal_table* seals;
+    mn_seal_line_table* lines;
+} mn_centre_page;
+int mn_find_seal_lines_u8(const mn_centre_page* pages, int n, void* stream);
+
 /* Flat pages (DESIGN.md section 7b, "Flat pages"): the dewarp field of a curled page, built from its traced lines, composed with
  * the page's frame and sampled from the photo.  A page's line table (built on the host, pipeline.flat_line_table) holds
  * MN_FLAT_LINE_DOUBLES fp64 values per line, sorted by anchor Y (ties in reading order): xs, xe, mu_0 .. mu_3, Y, bx0, bx1.

@@ -272,6 +272,22 @@ class SealPage(Structure):
                 ("seal_size", c_int32), ("pad", c_int32)]
 
 
+SEAL_MAX_LINES = 4                                                 # MN_SEAL_MAX_LINES
+
+
+class SealLines(Structure):
+    _fields_ = [(f, c_int32) for f in ("turn", "g0", "n_gap", "k_bottom", "k_top", "why", "k_in", "k_gap", "n_found",
+                                       "n_lines")] + [("pad", c_int32 * 2), ("box", (c_int32 * 4) * SEAL_MAX_LINES)]
+
+
+class SealLineTable(Structure):
+    _fields_ = [("seal", SealLines * PAGE_MAX_SEALS)]
+
+
+class CentrePage(Structure):
+    _fields_ = [("b", TextBlock), ("seals", c_void_p), ("lines", c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/marconet_b200.h declares
 SYMBOLS = {
     "mn_last_error": (c_char_p, []),
@@ -344,6 +360,7 @@ SYMBOLS = {
     "mn_find_page_spines_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
     "mn_find_seals_u8": (c_int, [c_void_p, c_int, c_longlong, c_longlong, c_void_p, c_longlong, c_void_p]),
     "mn_seal_layout_u8": (c_int, [c_void_p, c_int, c_longlong, c_void_p]),
+    "mn_find_seal_lines_u8": (c_int, [c_void_p, c_int, c_void_p]),
     "mn_token_mix": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mn_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -2372,6 +2372,35 @@ __device__ __forceinline__ int seal_sector(long long px, long long py) {
     return MN_SEAL_SECTORS / 2 + seal_half_sector(-px, -py);
 }
 
+// The band walk's first bin inside the ring's edge: from k = 32 inward past the ring's outer bins, the ring run and its edge.
+__device__ __forceinline__ int seal_gap_top(const int* ink, const int* area) {
+    int k = MN_SEAL_BINS - 1;
+    while (k >= 0 && MN_SEAL_RING_DENSITY * ink[k] < area[k]) --k;                         // the ring's outer bin
+    while (k >= 0 && MN_SEAL_RING_DENSITY * ink[k] >= area[k]) --k;                        // the ring run
+    while (k >= 0 && MN_SEAL_BAND_DENSITY * ink[k] >= area[k]) --k;                        // its edge
+    return k;
+}
+
+// The gap (g0, n) of per-sector ink sec, band its sum: the longest circular run of empty sectors; returns the arc's why.
+__device__ __forceinline__ int seal_arc_gap(const int* sec, int band, int& g0, int& n) {
+    const int lim = max(MN_SEAL_EMPTY_DIV, band);
+    int all = 1;
+    g0 = 0, n = 0;
+    for (int s = 0; s < MN_SEAL_SECTORS; ++s) all &= MN_SEAL_EMPTY_DIV * sec[s] < lim;
+    if (all) {
+        n = MN_SEAL_SECTORS;
+    } else {
+        for (int s = 0; s < MN_SEAL_SECTORS; ++s) {           // runs start at an empty sector after a non-empty one
+            const int prev = (s + MN_SEAL_SECTORS - 1) % MN_SEAL_SECTORS;
+            if (!(MN_SEAL_EMPTY_DIV * sec[s] < lim) || MN_SEAL_EMPTY_DIV * sec[prev] < lim) continue;
+            int m = 0;
+            while (MN_SEAL_EMPTY_DIV * sec[(s + m) % MN_SEAL_SECTORS] < lim) ++m;
+            if (m > n) g0 = s, n = m;
+        }
+    }
+    return n < MN_SEAL_MIN_GAP ? MN_SEAL_NO_GAP : MN_SEAL_SECTORS - n < MN_SEAL_MIN_TEXT ? MN_SEAL_SHORT : 0;
+}
+
 // 5: one CTA per candidate slot: the histograms, then thread 0 reads the ring, band and arc off them.
 __global__ void __launch_bounds__(kSealThreads) seal_test_kernel(const mn_seal_page* __restrict__ pages) {
     mn_pdl_prologue();
@@ -2433,11 +2462,8 @@ __global__ void __launch_bounds__(kSealThreads) seal_test_kernel(const mn_seal_p
     r.k_bottom = r.k_top = r.g0 = r.n_gap = -1;
     r.why = 0, r.band_ink = 0, r.pad[0] = r.pad[1] = r.pad[2] = 0;
     if (r.found) {
-        int k = MN_SEAL_BINS - 1;
-        while (k >= 0 && MN_SEAL_RING_DENSITY * ink[k] < s_area[k]) --k;                       // the ring's outer bin
-        while (k >= 0 && MN_SEAL_RING_DENSITY * ink[k] >= s_area[k]) --k;                      // the ring run
-        while (k >= 0 && MN_SEAL_BAND_DENSITY * ink[k] >= s_area[k]) --k;                      // its edge
-        const int gap_top = k;
+        const int gap_top = seal_gap_top(ink, s_area);
+        int k = gap_top;
         while (k >= MN_SEAL_BAND_MIN_K && MN_SEAL_BAND_DENSITY * ink[k] < s_area[k]) --k;      // the gap
         if (gap_top >= MN_SEAL_BAND_MIN_K && k < gap_top && k >= MN_SEAL_BAND_MIN_K) {
             r.k_top = k;
@@ -2456,22 +2482,7 @@ __global__ void __launch_bounds__(kSealThreads) seal_test_kernel(const mn_seal_p
                 band += t;
             }
             r.band_ink = band;
-            const int lim = max(MN_SEAL_EMPTY_DIV, band);
-            int g0 = 0, n = 0, all = 1;
-            for (int s = 0; s < MN_SEAL_SECTORS; ++s) all &= MN_SEAL_EMPTY_DIV * sec[s] < lim;
-            if (all) {
-                n = MN_SEAL_SECTORS;
-            } else {
-                for (int s = 0; s < MN_SEAL_SECTORS; ++s) {   // runs start at an empty sector after a non-empty one
-                    const int prev = (s + MN_SEAL_SECTORS - 1) % MN_SEAL_SECTORS;
-                    if (!(MN_SEAL_EMPTY_DIV * sec[s] < lim) || MN_SEAL_EMPTY_DIV * sec[prev] < lim) continue;
-                    int m = 0;
-                    while (MN_SEAL_EMPTY_DIV * sec[(s + m) % MN_SEAL_SECTORS] < lim) ++m;
-                    if (m > n) g0 = s, n = m;
-                }
-            }
-            r.g0 = g0, r.n_gap = n;
-            r.why = n < MN_SEAL_MIN_GAP ? MN_SEAL_NO_GAP : MN_SEAL_SECTORS - n < MN_SEAL_MIN_TEXT ? MN_SEAL_SHORT : 0;
+            r.why = seal_arc_gap(sec, band, r.g0, r.n_gap);
         }
     }
     out->seal[s_rank] = r;
@@ -2521,6 +2532,134 @@ __global__ void __launch_bounds__(kTileThreads) seal_copy_kernel(const mn_seal_p
         q[1] = v1;
         q[2] = v2;
     }
+}
+
+// Seal centre lines (DESIGN.md 7b, "Seal centre lines"): one CTA per seal slot rebuilds the seal's histograms, reads its head
+// gap, turn and arc band off them (thread 0), then the min and max u of each interior row in the stamp frame.
+constexpr int kCentreRows = MN_SEAL_MAX_SIDE + 4;     // v in [-M / 2 - 1, M / 2] for M = max(A, B): row v at v + M / 2 + 2
+__constant__ int2 c_seal_turns[MN_SEAL_TURN_STEPS / 4] = MN_SEAL_TURNS;
+
+__global__ void __launch_bounds__(kSealThreads) centre_lines_kernel(const mn_centre_page* __restrict__ pages) {
+    mn_pdl_prologue();
+    __shared__ int s_ink[MN_SEAL_BINS][MN_SEAL_SECTORS];
+    __shared__ int s_area[MN_SEAL_BINS];
+    __shared__ int s_sum[MN_SEAL_BINS];
+    __shared__ int s_sec[MN_SEAL_SECTORS];
+    __shared__ int s_lo[kCentreRows], s_hi[kCentreRows];
+    __shared__ int s_k_in, s_k_gap, s_g0, s_n, s_c, s_s, s_vlo, s_vhi;
+    __shared__ mn_seal_lines s_rec;
+    const mn_centre_page cp = pages[blockIdx.y];
+    const mn_seal_table* t = cp.seals;
+    const int slot = blockIdx.x;
+    if (t->error || slot >= min(t->n_cand, MN_PAGE_MAX_SEALS) || !t->seal[slot].found) {     // a zero record
+        int* z = reinterpret_cast<int*>(&cp.lines->seal[slot]);
+        for (int i = threadIdx.x; i < (int)(sizeof(mn_seal_lines) / 4); i += blockDim.x) z[i] = 0;
+        return;
+    }
+    const mn_seal sl = t->seal[slot];
+    const int x0 = sl.x0, y0 = sl.y0, x1 = sl.x1, y1 = sl.y1;
+    const long long A = x1 - x0, B = y1 - y0, n_px = A * B;
+    const int off = (int)(max(A, B) / 2) + 2;
+    for (int i = threadIdx.x; i < MN_SEAL_BINS * MN_SEAL_SECTORS; i += blockDim.x) (&s_ink[0][0])[i] = 0;
+    for (int i = threadIdx.x; i < kCentreRows; i += blockDim.x) s_lo[i] = INT_MAX, s_hi[i] = INT_MIN;
+    if (threadIdx.x < MN_SEAL_BINS) s_area[threadIdx.x] = 0;
+    if (threadIdx.x == 0) s_vlo = INT_MAX, s_vhi = INT_MIN;
+    __syncthreads();
+    const mn_text_block b = cp.b;
+    for (long long i = threadIdx.x; i < n_px; i += blockDim.x) {
+        const int x = x0 + (int)(i % A), y = y0 + (int)(i / A);
+        const long long X = 2 * x + 1 - (x0 + x1), Y = 2 * y + 1 - (y0 + y1);
+        const int k = seal_bin(X, Y, A, B);
+        if (k >= MN_SEAL_BINS) continue;
+        atomicAdd(&s_area[k], 1);
+        if (seal_coloured(crop_px(b, x, y))) atomicAdd(&s_ink[k][seal_sector(X * B, -Y * A)], 1);
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < MN_SEAL_BINS; k += blockDim.x) {
+        int v = 0;
+        for (int s = 0; s < MN_SEAL_SECTORS; ++s) v += s_ink[k][s];
+        s_sum[k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        mn_seal_lines& r = s_rec;
+        r.turn = 0, r.g0 = r.n_gap = r.k_bottom = r.k_top = -1, r.why = MN_SEAL_NO_BAND;
+        r.k_in = r.k_gap = max(seal_gap_top(s_sum, s_area), 0);
+        r.n_found = r.n_lines = 0, r.pad[0] = r.pad[1] = 0;
+        for (int j = 0; j < MN_SEAL_MAX_LINES; ++j) r.box[j][0] = r.box[j][1] = r.box[j][2] = r.box[j][3] = 0;
+        if (sl.k_top >= MN_SEAL_HEAD_MIN_K) {
+            const int kt = sl.k_top;
+            int head = 0;
+            for (int s = 0; s < MN_SEAL_SECTORS; ++s) {
+                int v = 0;
+                for (int k = kt - MN_SEAL_HEAD_BINS + 1; k <= kt; ++k) v += s_ink[k][s];
+                s_sec[s] = v;
+                head += v;
+            }
+            int g0, n;
+            r.why = seal_arc_gap(s_sec, head, g0, n);
+            int turn = (2 * g0 + n - 108 + MN_SEAL_TURN_STEPS) % MN_SEAL_TURN_STEPS;
+            if (turn > MN_SEAL_TURN_STEPS / 2) turn -= MN_SEAL_TURN_STEPS;
+            int k = kt;                                          // the walk over the arc sectors [g0 + n, g0 + 72)
+            for (; k - 1 >= MN_SEAL_BAND_MIN_K; --k) {
+                long long arc = 0;
+                for (int m = n; m < MN_SEAL_SECTORS; ++m) arc += s_ink[k - 1][(g0 + m) % MN_SEAL_SECTORS];
+                if ((long long)MN_SEAL_BAND_DENSITY * MN_SEAL_SECTORS * arc < (long long)s_area[k - 1] * (MN_SEAL_SECTORS - n)) break;
+            }
+            r.turn = r.why ? 0 : turn, r.g0 = g0, r.n_gap = n, r.k_bottom = k, r.k_top = kt, r.k_in = k;
+            r.k_gap = max(k, kt - MN_SEAL_HEAD_BINS + 1);
+        }
+        const int j = (r.turn % MN_SEAL_TURN_STEPS + MN_SEAL_TURN_STEPS) % MN_SEAL_TURN_STEPS;
+        int c = c_seal_turns[j % (MN_SEAL_TURN_STEPS / 4)].x, s = c_seal_turns[j % (MN_SEAL_TURN_STEPS / 4)].y;
+        for (int q = 0; q < j / (MN_SEAL_TURN_STEPS / 4); ++q) {
+            const int c0 = c;
+            c = -s, s = c0;
+        }
+        s_k_in = r.k_in, s_k_gap = r.k_gap, s_g0 = r.g0, s_n = r.n_gap, s_c = c, s_s = s;
+    }
+    __syncthreads();
+    const int k_in = s_k_in, k_gap = s_k_gap, g0 = s_g0 + MN_SEAL_GAP_MARGIN, n_in = s_n - 2 * MN_SEAL_GAP_MARGIN;
+    const long long c = s_c, s = s_s;
+    for (long long i = threadIdx.x; i < n_px; i += blockDim.x) {
+        const int x = x0 + (int)(i % A), y = y0 + (int)(i / A);
+        const long long X = 2 * x + 1 - (x0 + x1), Y = 2 * y + 1 - (y0 + y1);
+        const int k = seal_bin(X, Y, A, B);                     // the interior: k < k_in, or k < k_gap inside the head gap
+        if (k >= k_gap || !seal_coloured(crop_px(b, x, y))) continue;
+        if (k >= k_in && (seal_sector(X * B, -Y * A) - g0 + 2 * MN_SEAL_SECTORS) % MN_SEAL_SECTORS >= n_in) continue;
+        const int u = (int)((X * c - Y * s) >> 21), v = (int)((X * s + Y * c) >> 21);
+        atomicMin(&s_lo[v + off], u);
+        atomicMax(&s_hi[v + off], u);
+        atomicMin(&s_vlo, v);
+        atomicMax(&s_vhi, v);
+    }
+    __syncthreads();
+    if (threadIdx.x) return;
+    mn_seal_lines& r = s_rec;
+    const int min_h = max(MN_SEAL_LINE_MIN_H, (int)((A + B) / MN_SEAL_LINE_H_DIV)), R = (int)(k_gap * max(A, B) / 64);
+    int u0 = 0, u1 = 0, v0 = 0, last = INT_MIN / 2;
+    auto close = [&]() {                                         // the run [v0, last] ends
+        const int h = last - v0 + 1;
+        if (h < min_h || u1 - u0 + 1 < MN_SEAL_LINE_RATIO * h) return;
+        if (r.n_found < MN_SEAL_MAX_LINES) {
+            const int p = max(MN_SEAL_LINE_PAD, h / MN_SEAL_LINE_PAD_DIV);
+            int* o = r.box[r.n_found];
+            o[0] = max(u0 - p, -R - 1), o[1] = max(v0 - p, -R - 1), o[2] = min(u1 + 1 + p, R + 1), o[3] = min(last + 1 + p, R + 1);
+        }
+        ++r.n_found;
+    };
+    for (int v = s_vlo; v <= s_vhi; ++v) {
+        const int lo = s_lo[v + off], hi = s_hi[v + off];
+        if (lo > hi) continue;
+        if (v > s_vlo && v - last - 1 < MN_SEAL_LINE_GAP) {
+            u0 = min(u0, lo), u1 = max(u1, hi), last = v;
+            continue;
+        }
+        if (v > s_vlo) close();
+        u0 = lo, u1 = hi, v0 = last = v;
+    }
+    if (s_vlo <= s_vhi) close();
+    r.n_lines = min(r.n_found, MN_SEAL_MAX_LINES);
+    cp.lines->seal[slot] = r;
 }
 
 // 4-11 of the XY-cut: both passes of levels, the text size between them and the leaves, on pages whose bitmap and root are
@@ -2700,6 +2839,13 @@ extern "C" int mn_find_page_spines_u8(const mn_spine_page* spines, int n, long l
 extern "C" int mn_seal_layout_u8(const mn_seal_page* pages, int n, long long max_tiles, void* stream) {
     MN_REQUIRE(pages && n > 0 && n <= 65535 && max_tiles > 0 && max_tiles < (1ll << 31), "mn_seal_layout_u8: bad args");
     MN_CUDA_CHECK((mn_launch(seal_copy_kernel, dim3((unsigned)max_tiles, n), dim3(kTileThreads), 0, (cudaStream_t)stream, pages)));
+    MN_LAUNCH_CHECK();
+    return MN_OK;
+}
+
+extern "C" int mn_find_seal_lines_u8(const mn_centre_page* pages, int n, void* stream) {
+    MN_REQUIRE(pages && n > 0 && n <= 65535, "mn_find_seal_lines_u8: bad args");
+    MN_CUDA_CHECK((mn_launch(centre_lines_kernel, dim3(MN_PAGE_MAX_SEALS, n), dim3(kSealThreads), 0, (cudaStream_t)stream, pages)));
     MN_LAUNCH_CHECK();
     return MN_OK;
 }

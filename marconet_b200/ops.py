@@ -2107,6 +2107,7 @@ class PageItem(NamedTuple):
     directions: bool = False
     panel_size: object = None
     seal_size: object = None
+    seal_lines: bool = False
 
 
 def page_cap(w, h):
@@ -2143,19 +2144,27 @@ def _page_areas(L, M, cap, n_ang, stride, rules, figures, panels):
             plane if panels and not rules else 0]
 
 
-def page_bytes(w, h, vertical=False, cs=None, rules=False, figures=False, panels=False, seals=False):
+def page_bytes(w, h, vertical=False, cs=None, rules=False, figures=False, panels=False, seals=False, seal_lines=False):
     """Device bytes of one w x h page in find_blocks, with or without ``rules``, ``figures`` and ``panels``: its records,
     result and leaf table, a figure page's table of PAGE_MAX_FIGURES and a panel page's table of PAGE_MAX_PANELS page nodes,
     its work areas and 64 bytes for the call's 16-byte alignments.  ``cs``: None in a call without skewed pages, else the
     (c, s) table the page searches ([(1.0, 0.0)] for a page with skew None), which adds the search record, the table and 16
-    bytes for its alignment; the page's bitmaps are then those of its largest frame.  ``seals``: with seal_bytes."""
+    bytes for its alignment; the page's bitmaps are then those of its largest frame.  ``seals``: with seal_bytes, and
+    ``seal_lines`` with seal_line_bytes."""
     n_ang = len(cs) if cs else 1
     L, M, stride = skew_page_frame(w, h, vertical, cs or [(1.0, 0.0)])
     cap = page_cap(M, L)
     tables = 12 * (cap + (_lib.PAGE_MAX_FIGURES if figures else 0) + (_lib.PAGE_MAX_PANELS if panels else 0))
     search = ctypes.sizeof(_lib.SkewBlock) + 16 * n_ang + 16 if cs else 0
     return (ctypes.sizeof(_lib.PageResult) + ctypes.sizeof(_lib.TextBlock) + ctypes.sizeof(_lib.TextPage) + tables + search
-            + sum(_page_areas(L, M, cap, n_ang, stride, rules, figures, panels)) + 64 + (seal_bytes(w, h) if seals else 0))
+            + sum(_page_areas(L, M, cap, n_ang, stride, rules, figures, panels)) + 64 + (seal_bytes(w, h) if seals else 0)
+            + (seal_line_bytes() if seal_lines else 0))
+
+
+def seal_line_bytes():
+    """Device bytes a page with seal_lines adds to find_blocks (DESIGN.md 7b, "Seal centre lines"): its record and line table,
+    with 16 bytes for each area's alignment.  The rows of the line search live in shared memory."""
+    return ctypes.sizeof(_lib.CentrePage) + ctypes.sizeof(_lib.SealLineTable) + 2 * 16
 
 
 def rule_page_bytes(w, h):
@@ -2197,6 +2206,9 @@ def _check_page_options(page, what):
     v = page.seal_size
     if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 8 <= v <= 4096 or page.skew is not None):
         raise ValueError(f"{what}: seal_size {v!r} is not an integer in [8, 4096] on a page with skew None")
+    v = page.seal_lines
+    if not isinstance(v, bool) or (v and page.seal_size is None):
+        raise ValueError(f"{what}: seal_lines {v!r} is not False, or True on a page with a seal_size")
 
 
 def find_blocks(pages, scores=False):
@@ -2232,6 +2244,10 @@ def find_blocks(pages, scores=False):
     (mn_find_seals_u8's 6 launches for all such pages of the call, before the layout) and its layout runs on its layout copy,
     the crop with the seals' own ink set to paper.  out then starts with each such page's mn_seal_table, in the order of the
     pages (seal_tables reads them back).
+    seal_lines (DESIGN.md 7b, "Seal centre lines"): False, or True on a page with a seal_size: each found seal's turn, arc band
+    and centre lines are found (mn_find_seal_lines_u8's 1 launch for all such pages of the call, after mn_find_seals_u8).  out
+    then has, after the seal tables, each such page's mn_seal_line_table, in the order of the pages (seal_line_tables reads
+    them back).
     A page without one of these options gets the tables of a call without it."""
     global LAUNCHES
     dev = _check_items(pages, "find_blocks", "page")
@@ -2248,7 +2264,8 @@ def find_blocks(pages, scores=False):
         _check_page_options(p, what)
         opts = (p.rule_length is not None, p.figure_size is not None, p.panel_size is not None)   # rules, figures, panels
         L, M, stride = skew_page_frame(bw, bh, p.vertical, cs)
-        need += page_bytes(bw, bh, p.vertical, cs if skewed else None, *opts, seals=p.seal_size is not None)
+        need += page_bytes(bw, bh, p.vertical, cs if skewed else None, *opts, seals=p.seal_size is not None,
+                           seal_lines=p.seal_lines)
         if max(L, M) > 32767:
             raise ValueError(f"{what}: a frame side of {max(L, M)} exceeds 32767")
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
@@ -2263,16 +2280,21 @@ def find_blocks(pages, scores=False):
     tab, t_offs = _angle_tables(tables) if skewed else (b"", [0] * n)
     sealed = [i for i, p in enumerate(pages) if p.seal_size is not None]
     m, spsz, tsz = len(sealed), ctypes.sizeof(_lib.SealPage), ctypes.sizeof(_lib.SealTable)
-    pack = _Pack()                  # records, tables, the seal tables and the skew records, which come back with the results in
-    pack.area(n * bsz)              # one copy; then the results, leaves, figure and panel tables and each page's work, which
-    pg, t_off = pack.area(n * psz), pack.area(len(tab))     # the call zeroes; then the seal pages' cells and layout copies
+    lined = [i for i in sealed if pages[i].seal_lines]
+    ml, cpsz, lsz = len(lined), ctypes.sizeof(_lib.CentrePage), ctypes.sizeof(_lib.SealLineTable)
+    pack = _Pack()                  # records, tables, the seal and line tables and the skew records, which come back with the
+    pack.area(n * bsz)              # results in one copy; then the results, leaves, figure and panel tables and each page's
+    pg, t_off = pack.area(n * psz), pack.area(len(tab))     # work, which the call zeroes; then the seal pages' cells and copies
     if sealed:
         sp = pack.area(m * spsz, 16)
+        cp = pack.area(ml * cpsz, 16)
         pack.area(m * tsz, 16)
+        pack.area(ml * lsz, 16)
     pack.area(n * ssz)
     out0 = pack.area(n * rsz, 16)
-    sk0 = out0 - n * ssz            # the skew records end where the results begin, and the seal tables where they begin
-    st0 = sk0 - m * tsz
+    sk0 = out0 - n * ssz            # the skew records end where the results begin, the line tables where they begin and the
+    lt0 = sk0 - ml * lsz            # seal tables where those begin
+    st0 = lt0 - m * tsz
     leaves = [pack.area(12 * d[4]) for d in dims]
     figs = [pack.area(12 * _lib.PAGE_MAX_FIGURES) if d[8][1] else None for d in dims]
     pans = [pack.area(12 * _lib.PAGE_MAX_PANELS) if d[8][2] else None for d in dims]
@@ -2281,7 +2303,7 @@ def find_blocks(pages, scores=False):
     w_end = pack.end
     scells = {i: [pack.area(a, 16) for a in _seal_areas(dims[i][2], dims[i][3])] for i in sealed}
     base = pack.alloc(dev)
-    blocks, srecs, recs, views, tiles, seal_recs, stiles, ctiles = [], [], [], [], 0, [], 0, 0
+    blocks, srecs, recs, views, tiles, seal_recs, centre_recs, stiles, ctiles = [], [], [], [], 0, [], [], 0, 0
     for i, (p, (x0, y0, bw, bh, cap, M, n_ang, stride, (rules, figures, panels)), wk, lv, f, pn, t) in \
             enumerate(zip(pages, dims, work, leaves, figs, pans, t_offs)):
         sc, hist, lines, bits, lists, counts, prof, rbits, fbits, pbits = (base + o for o in wk)
@@ -2290,6 +2312,8 @@ def find_blocks(pages, scores=False):
             copy, label, box, cand = (base + o for o in scells[i])
             seal_recs.append(_lib.SealPage(_lib.TextBlock(src, pitch, x0, y0, bw, bh), copy, label, box, cand,
                                            base + st0 + len(seal_recs) * tsz, p.seal_size))
+            if p.seal_lines:
+                centre_recs.append(_lib.CentrePage(seal_recs[-1].b, seal_recs[-1].out, base + lt0 + len(centre_recs) * lsz))
             src, pitch = (copy - y0 * 3 * bw - 3 * x0) % (1 << 64), 3 * bw
             stiles = max(stiles, -(-bw // 32) * -(-bh // 32))
             ctiles = max(ctiles, -(-bw // (4 * 32)) * -(-bh // (4 * 8)))
@@ -2307,10 +2331,14 @@ def find_blocks(pages, scores=False):
         tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
     buf = pack.upload((0, bytes((_lib.TextBlock * n)(*blocks))), (pg, bytes((_lib.TextPage * n)(*recs))), (t_off, tab),
                       *(((sp, bytes((_lib.SealPage * m)(*seal_recs))),) if sealed else ()),
+                      *(((cp, bytes((_lib.CentrePage * ml)(*centre_recs))),) if lined else ()),
                       (sk0, bytes((_lib.SkewBlock * len(srecs))(*srecs))))
     if sealed:
         _lib.check(_lib.load().mn_find_seals_u8(base + sp, m, stiles, ctiles, base + st0, m * tsz, _stream()), "mn_find_seals_u8")
         LAUNCHES += 6
+    if lined:
+        _lib.check(_lib.load().mn_find_seal_lines_u8(base + cp, ml, _stream()), "mn_find_seal_lines_u8")
+        LAUNCHES += 1
     ruled, figured, directed, paneled = (any(p.rule_length is not None for p in pages), any(f is not None for f in figs),
                                          any(p.directions for p in pages), any(pn is not None for pn in pans))
     flags = ((_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0) | (_lib.PAGE_DIRECTIONS if directed else 0)
@@ -2330,7 +2358,8 @@ def page_tables(host, pages, caps):
     unless the page has a figure_size, panels None unless it has a panel_size."""
     sdt, rdt, ndt = skew_block_dtype(), page_result_dtype(), page_node_dtype()
     n = len(pages)
-    host = host[ctypes.sizeof(_lib.SealTable) * sum(p.seal_size is not None for p in pages):]
+    host = host[ctypes.sizeof(_lib.SealTable) * sum(p.seal_size is not None for p in pages)
+                + ctypes.sizeof(_lib.SealLineTable) * sum(p.seal_lines for p in pages):]
     o = n * sdt.itemsize if any(p.skew is not None for p in pages) else 0
     skews = host[:o].view(sdt) if o else [None] * n
     res = host[o:o + n * rdt.itemsize].view(rdt)
@@ -2354,6 +2383,22 @@ def seal_tables(host, pages):
     tdt = seal_table_dtype()
     tabs = iter(host[:tdt.itemsize * sum(p.seal_size is not None for p in pages)].view(tdt))
     return [None if p.seal_size is None else next(tabs) for p in pages]
+
+
+def seal_line_tables(host, pages):
+    """Per page of a find_blocks call, the numpy view of its mn_seal_line_table in ``host`` (seal_line_table_dtype()), or None
+    for a page without seal_lines."""
+    ldt, o = seal_line_table_dtype(), ctypes.sizeof(_lib.SealTable) * sum(p.seal_size is not None for p in pages)
+    tabs = iter(host[o:o + ldt.itemsize * sum(p.seal_lines for p in pages)].view(ldt))
+    return [next(tabs) if p.seal_lines else None for p in pages]
+
+
+def seal_line_table_dtype():
+    """numpy view of an mn_seal_line_table record."""
+    import numpy as np
+    rec = np.dtype([(f, "<i4") for f, _ in _lib.SealLines._fields_[:-2]] + [("pad", "<i4", (2,)),
+                                                                            ("box", "<i4", (_lib.SEAL_MAX_LINES, 4))])
+    return np.dtype([("seal", rec, (_lib.PAGE_MAX_SEALS,))])
 
 
 def seal_table_dtype():

@@ -2126,9 +2126,16 @@ def _n_arcs(res):
     return sum(s["region"] is not None for s in res.get("seals", ())) if isinstance(res, dict) else 0
 
 
+def _line_names(res):
+    """(seal j, line m) of each seal centre line a page's find_blocks result ``res`` puts after its arcs, in order (none for any
+    other entry)."""
+    seals = res.get("seals", ()) if isinstance(res, dict) else ()
+    return [(j, m) for j, s in enumerate(seals) for m, ln in enumerate(s.get("lines", ())) if ln["region"] is not None]
+
+
 def _regroup(out, layout):
     """restore_regions' result with each block's (page's) child entries gathered into its own entry, in place; a page's seal
-    arcs go into its ``seal_regions``."""
+    arcs go into its ``seal_regions`` and, with seal_lines, its seal centre lines into its ``seal_line_regions``."""
     for img, lay in zip(out, layout):
         flat, o, img["regions"] = img["regions"], 0, []
         for e in lay:
@@ -2138,8 +2145,11 @@ def _regroup(out, layout):
                 continue
             res, k = e
             a = _n_arcs(res) if "seals" in res else 0
+            c = a + len(_line_names(res))
             extra = dict(seal_regions=flat[o:o + a]) if "seals" in res else {}
-            img["regions"].append(res if "error" in res else dict(res, **extra, regions=flat[o + a:o + k]))
+            if "seal_lines" in res:
+                extra["seal_line_regions"] = flat[o + a:o + c]
+            img["regions"].append(res if "error" in res else dict(res, **extra, regions=flat[o + c:o + k]))
             o += k
 
 
@@ -2180,7 +2190,11 @@ class TextPage(NamedTuple):
     its inscribed ellipse, are seals.  Their own ink is taken out of the layout (black text under a stamp stays ink), each
     block gets the seals that meet it, and the text along a seal's upper arc is found and restored as a CurvedRegion.
     ``seal_size`` is an integer in [8, 4096], default max(24, min(w, h) // 12) of the crop, a heuristic.  Only on a level,
-    flat page of dark ink: not with skew, curve or quad (flatten such a page with flatten_pages first) or polarity "light"."""
+    flat page of dark ink: not with skew, curve or quad (flatten such a page with flatten_pages first) or polarity "light".
+    ``seal_lines`` (DESIGN.md 7b, "Seal centre lines"): None, or "auto" with seals="auto": each seal's turn is read off the gap
+    of its arc text's outer bins, its arc band stops where the arc sectors thin out, and the horizontal lines of text across
+    its centre (合同专用章 under a star, an invoice seal's number) are found in the stamp's frame and restored as rectangles or
+    OrientedRegions.  The arc, band and why then follow that definition."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
@@ -2199,6 +2213,7 @@ class TextPage(NamedTuple):
     panel_size: object = None
     seals: object = None
     seal_size: object = None
+    seal_lines: object = None
 
 
 def _check_page(pg, H, W, name):
@@ -2231,6 +2246,10 @@ def _check_page(pg, H, W, name):
                                  f"flatten a tilted, curled or photographed page with flatten_pages first)")
         if pg.polarity == "light":
             raise ValueError(f"{name}: seals are asked for on a page of polarity 'light' (seals are dark stamps on paper)")
+    if pg.seal_lines is not None and not (isinstance(pg.seal_lines, str) and pg.seal_lines == "auto"):
+        raise ValueError(f"{name}: seal_lines must be None or 'auto', got {pg.seal_lines!r}")
+    if pg.seal_lines is not None and pg.seals is None:
+        raise ValueError(f"{name}: seal_lines is given, but seals is None, not 'auto'")
     if pg.quad is not None:
         if pg.rect is not None:
             raise ValueError(f"{name}: rect and quad are both given (a page in perspective is its quad: give rect=None)")
@@ -2280,7 +2299,7 @@ def _page_bytes(pg, rect, skewed):
         return 3 * w_r * h_r + _page_bytes(pg._replace(quad=None), (0, 0, w_r, h_r), skewed)
     cs = (_page_table(pg) if pg.skew is not None else [(1.0, 0.0)]) if skewed else None
     return ops.page_bytes(w, h, pg.direction == "vertical", cs, rules=pg.rules is not None, figures=pg.figures is not None,
-                          panels=pg.panels is not None, seals=pg.seals is not None)
+                          panels=pg.panels is not None, seals=pg.seals is not None, seal_lines=pg.seal_lines is not None)
 
 
 def _check_page_work(items, extra=0):
@@ -2351,30 +2370,56 @@ def seal_size(w, h):
 _SEAL_WHY = {1: "no arc text", 2: "no gap in the arc text", 3: "the arc text spans under 45 degrees"}
 
 
-def _seal_entries(stab, X0, Y0, shape):
+def _seal_line(cx, cy, box, turn, shape):
+    """A seal centre line's dict(box, region[, why]): ``box`` (u0, v0, u1, v1) in the frame of a seal centred at (cx, cy) and
+    turned ``turn`` degrees.  Its region is the rectangle of the box when turn is 0, else the OrientedRegion of the box turned
+    about the seal's centre; it is kept only when restore_regions accepts it on the image of ``shape`` (H, W) at scale 1."""
+    u0, v0, u1, v1 = box
+    if turn == 0:
+        reg = (math.floor(cx + u0), math.floor(cy + v0), math.ceil(cx + u1), math.ceil(cy + v1))
+    else:
+        a, uc, vc = math.radians(turn), (u0 + u1) / 2, (v0 + v1) / 2
+        reg = OrientedRegion.from_rotated(cx + uc * math.cos(a) + vc * math.sin(a), cy - uc * math.sin(a) + vc * math.cos(a),
+                                          u1 - u0, v1 - v0, turn)
+    e = dict(box=box, region=reg)
+    try:
+        plan_regions([shape], [[reg]], None, None, 1)
+    except ValueError as err:
+        e.update(region=None, why=f"the line region is rejected ({str(err).split(': ', 1)[-1]})")
+    return e
+
+
+def _seal_entries(stab, X0, Y0, shape, ltab=None):
     """The seals of a page's mn_seal_table, in image coordinates: per seal dict(box, ring, band, arc, region[, why]).  A seal's
     arc is split into arc_segments' segments, and its region is kept only when restore_regions' curved rules accept it on the
-    image of ``shape`` (H, W); otherwise arc and region are None and why says why."""
+    image of ``shape`` (H, W); otherwise arc and region are None and why says why.  With the page's mn_seal_line_table
+    ``ltab`` (DESIGN.md 7b, "Seal centre lines"), the band, arc and why are the line table's and each seal gains turn (degrees,
+    counter-clockwise on screen) and lines, one _seal_line dict per centre line, top to bottom."""
     out = []
-    for s in stab["seal"][:min(int(stab["n_cand"]), len(stab["seal"]))]:
+    for j, s in enumerate(stab["seal"][:min(int(stab["n_cand"]), len(stab["seal"]))]):
         if not s["found"]:
             continue
         x0, y0, x1, y1 = (int(s[f]) for f in ("x0", "y0", "x1", "y1"))
         box = (X0 + x0, Y0 + y0, X0 + x1, Y0 + y1)
-        e = dict(box=box, ring=int(s["ring"]), band=None if s["k_top"] < 0 else (int(s["k_bottom"]), int(s["k_top"])), arc=None,
+        cx, cy = (box[0] + box[2]) / 2, (box[1] + box[3]) / 2
+        t = s if ltab is None else ltab["seal"][j]
+        e = dict(box=box, ring=int(s["ring"]), band=None if t["k_top"] < 0 else (int(t["k_bottom"]), int(t["k_top"])), arc=None,
                  region=None)
-        if s["why"]:
-            e["why"] = _SEAL_WHY[int(s["why"])]
+        if ltab is not None:
+            e["turn"] = 2.5 * int(t["turn"])
+            e["lines"] = [_seal_line(cx, cy, tuple(int(v) for v in b), e["turn"], shape) for b in t["box"][:int(t["n_lines"])]]
+        if t["why"]:
+            e["why"] = _SEAL_WHY[int(t["why"])]
         else:
-            start = 5 * int(s["g0"])
-            end = start - 5 * (72 - int(s["n_gap"]))
+            start = 5 * int(t["g0"])
+            end = start - 5 * (72 - int(t["n_gap"]))
             a, b = (x1 - x0) / 2, (y1 - y0) / 2
             kb, kt = e["band"]
             k = arc_segments(a, b, start, end)
             try:
                 if k is None:
                     raise ValueError(f"seal: its arc of {start - end} degrees needs more than 8 segments")
-                reg = CurvedRegion.from_arc((box[0] + box[2]) / 2, (box[1] + box[3]) / 2, ((kt + 1) / 32 * a, (kt + 1) / 32 * b),
+                reg = CurvedRegion.from_arc(cx, cy, ((kt + 1) / 32 * a, (kt + 1) / 32 * b),
                                             (kb / 32 * a, kb / 32 * b), start, end, segments=k)
                 _plan_curved(reg, *shape, 1, "seal")
                 e.update(arc=(start, end), region=reg)
@@ -2418,15 +2463,17 @@ def _find_blocks(dimg, items, rq=None):
                             figure_size=None if pg.figures is None else pg.figure_size or 0,
                             directions=pg.block_direction is not None,
                             panel_size=None if pg.panels is None else pg.panel_size or 0,
-                            seal_size=None if pg.seals is None else pg.seal_size or seal_size(crop[2] - crop[0], crop[3] - crop[1]))
+                            seal_size=None if pg.seals is None else pg.seal_size or seal_size(crop[2] - crop[0], crop[3] - crop[1]),
+                            seal_lines=pg.seal_lines is not None)
     pages = [page(*it) for it in items]
     res_t, caps = ops.find_blocks(pages)
     host = _to_host(res_t).numpy()
-    stabs = ops.seal_tables(host, pages)
+    stabs, ltabs = ops.seal_tables(host, pages), ops.seal_line_tables(host, pages)
     limits = {lib.PAGE_ERR_BLOCKS: ("blocks", lib.PAGE_MAX_BLOCKS), lib.PAGE_ERR_FIGURES: ("figures", lib.PAGE_MAX_FIGURES),
               lib.PAGE_ERR_PANELS: ("panels", lib.PAGE_MAX_PANELS)}
     out = []
-    for (i, pg, rect), p, (sk, r, leaves, figs, pans), stab in zip(items, pages, ops.page_tables(host, pages, caps), stabs):
+    for (i, pg, rect), p, (sk, r, leaves, figs, pans), stab, ltab in zip(items, pages, ops.page_tables(host, pages, caps), stabs,
+                                                                        ltabs):
         if stab is not None and stab["error"]:
             out.append(f"{int(stab['n_cand'])} seal candidates exceed the {lib.PAGE_MAX_SEALS} a text page may hold")
             continue
@@ -2480,11 +2527,13 @@ def _find_blocks(dimg, items, rq=None):
                                for b, d, pl in zip(blocks, dirs, pols)],
                        rejected=rejected, quad=_quad_key(i, pg.quad)[1], size=tuple(p.rect[2:]))
         elif pg.skew is None:
-            seals = [] if stab is None else _seal_entries(stab, X0, Y0, dimg[i].shape[:2])
+            seals = [] if stab is None else _seal_entries(stab, X0, Y0, dimg[i].shape[:2], ltab)
             res.update(blocks=[TextBlock(b, d, polarity=pl, curve=pg.curve, seals=_meeting(seals, b))
                                for b, d, pl in zip(blocks, dirs, pols)], rejected=rejected)
             if stab is not None:
                 res.update(seal_size=p.seal_size, seals=seals)
+            if ltab is not None:
+                res.update(seal_lines=pg.seal_lines)
         else:
             res["skew"] = _skew_used(pg, sk)
             res["blocks"] = [TextBlock(tuple(rect), pg.direction, polarity=pg.polarity, skew=res["skew"], window=b) if tilted
@@ -2543,7 +2592,14 @@ def find_blocks(images, pages):
     is paper.  Its dict gains ``seal_size`` (the size used) and ``seals``, one dict per seal ordered by box (y0, then x0): box
     (image pixels), ring (the sectors hit), band ((k_bottom, k_top) or None), arc ((start, end) in degrees or None), region
     (the arc text's CurvedRegion or None) and, when arc is None, why.  Each of its blocks is TextBlock(..., seals=...) with the
-    boxes of the seals that meet it.  A page over 64 seal candidates raises, as one over its figure limit."""
+    boxes of the seals that meet it.  A page over 64 seal candidates raises, as one over its figure limit.
+    A page with ``seal_lines="auto"`` (DESIGN.md 7b, "Seal centre lines") has the centre lines of its seals found on the device
+    (1 more launch for all such pages of the call, their tables back in the same copy).  Its dict gains ``seal_lines``
+    ("auto"), and each seal gains ``turn`` (degrees, counter-clockwise on screen, a multiple of 2.5) and ``lines``, one dict
+    per centre line top to bottom in the stamp's frame: box ((u0, v0, u1, v1), pixels from the seal box's centre in the
+    stamp's frame), region (a rectangle when turn is 0, else an OrientedRegion; None when restore_regions rejects it) and, when
+    region is None, why.  The seal's band, arc, region and why follow the centre-line definition: its turn and arc come from
+    the gap of the arc text's outer 4 bins, and its band stops where the arc sectors thin out."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
@@ -2579,33 +2635,39 @@ def _plan_pages(shapes, regions, labels, boxes):
 
 
 def _expand_pages(regions, labels, boxes, pages, found, skip_invalid, shapes, scale, feather):
-    """The region, label and box lists with each text page replaced in place by its seal arcs and TextBlocks; the names of every
-    TextBlock and seal arc of the new lists by (image, position); and per image the layout of its given regions: None for a
-    region, [entry, k] for a page of k arcs and blocks, entry its find_blocks result or dict(error=...) under ``skip_invalid``
-    for a page over a limit or with an arc plan_regions rejects on the image of ``shapes`` at ``scale`` and ``feather``."""
+    """The region, label and box lists with each text page replaced in place by its seal arcs, seal centre lines and TextBlocks;
+    the names of every TextBlock, seal arc and centre line of the new lists by (image, position); and per image the layout of
+    its given regions: None for a region, [entry, k] for a page of k arcs, lines and blocks, entry its find_blocks result or
+    dict(error=...) under ``skip_invalid`` for a page over a limit or with an arc or line plan_regions rejects on the image of
+    ``shapes`` at ``scale`` and ``feather``."""
     def expand(i, r, res):
         err = None if not isinstance(res, str) else f"image {i}, region {r} (a text page): {res}"
         arcs = [] if err else [s["region"] for s in res.get("seals", ()) if s["region"] is not None]
-        for j, arc in enumerate(arcs):
+        lines = [] if err else [(f"seal {j}, line {m}", res["seals"][j]["lines"][m]["region"]) for j, m in _line_names(res)]
+        for what, reg in [(f"seal {j}", arc) for j, arc in enumerate(arcs)] + lines:
             try:
-                plan_regions([shapes[i]], [[arc]], None, None, scale, feather)
+                plan_regions([shapes[i]], [[reg]], None, None, scale, feather)
             except ValueError as e:
-                err = f"image {i}, region {r} (a text page), seal {j}: {str(e).split(': ', 1)[-1]}"
+                err = f"image {i}, region {r} (a text page), {what}: {str(e).split(': ', 1)[-1]}"
                 break
-        if err is None:                                 # a page's seal arcs compose before its blocks
-            return res, arcs + res["blocks"]
+        if err is None:                                 # a page's seal arcs, then its centre lines, compose before its blocks
+            return res, arcs + [reg for _, reg in lines] + res["blocks"]
         if not skip_invalid:
             raise ValueError(err)
         return dict(error=err), []
     regions, labels, boxes, layout = _splice(regions, labels, boxes, pages, found, expand)
     names = {}
     for i, lay in enumerate(layout):
-        at = [(r, k if e is None else k - _n_arcs(e[0])) for r, e in enumerate(lay) for k in ([None] if e is None else range(e[1]))]
+        at = [(r, k if e is None else k - _n_arcs(e[0]) - len(_line_names(e[0]))) for r, e in enumerate(lay)
+              for k in ([None] if e is None else range(e[1]))]
         for o, (r, k) in enumerate(at):
             if k is not None and k >= 0:
                 names[(i, o)] = f"image {i}, region {r} (a text page), block {k}"
+            elif k is not None and k >= -len(_line_names(lay[r][0])):      # the centre lines, after the arcs
+                j, m = _line_names(lay[r][0])[k]
+                names[(i, o)] = f"image {i}, region {r} (a text page), seal {j}, line {m}"
             elif k is not None:                         # the arcs, seal 0 first
-                names[(i, o)] = f"image {i}, region {r} (a text page), seal {k + _n_arcs(lay[r][0])}"
+                names[(i, o)] = f"image {i}, region {r} (a text page), seal {k + _n_arcs(lay[r][0]) + len(_line_names(lay[r][0]))}"
             elif isinstance(regions[i][o], TextBlock):
                 names[(i, o)] = f"image {i}, region {r} (a text block)"
     return regions, labels, boxes, names, layout
@@ -3221,7 +3283,10 @@ def restore_regions(encoder, tspgan, sr, images, regions, labels=None, boxes=Non
     warped in one launch, and gives QuadRegion lines; a page without a quad found is its error.  A page with
     ``seals="auto"`` (DESIGN.md 7b, "Seals") puts the CurvedRegion of each seal's arc text in the region list before its
     blocks, so where a printed line crosses a stamp the line's restoration is composed last; its entry's ``regions`` stays one
-    block entry per block and ``seal_regions`` holds one curved-region entry per arc.  The seal's centre keeps the background."""
+    block entry per block and ``seal_regions`` holds one curved-region entry per arc.  The seal's centre keeps the background,
+    unless the page has ``seal_lines="auto"`` (DESIGN.md 7b, "Seal centre lines"): each seal's centre lines then follow the
+    arcs, before the blocks, and its entry's ``seal_line_regions`` holds one region entry per line.  A line plan_regions
+    rejects at the call's scale is named "seal j, line m" of its page and fails the page, as an arc does."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     shapes = [im.shape[:2] for im in imgs]
