@@ -832,11 +832,25 @@ int mn_find_lines_curved_u8(const mn_text_block* blocks, const mn_curve_block* c
  *      leaves and writes the root of pass 2;
  *   b. every panel row painted, one warp per row: the interior inverted in bits (J = not I), the 1-pixel outline cleared from
  *      bits and OR'd into rbits, so that the rule-index cut and the growth stops see it as a rule.
- * A call without MN_PAGE_PANELS issues exactly the launches above. */
+ * A call without MN_PAGE_PANELS issues exactly the launches above.
+ * Page turns (DESIGN.md section 7b, "Page turns"): a page with dirs & MN_PAGE_DIRS_TURN (and dirs & 1: its blocks' directions
+ * are tested) has a vote table of cap mn_page_turn entries inside work, at the first 16-byte boundary after its leaves table.
+ * A call with MN_PAGE_TURNS (and MN_PAGE_DIRECTIONS) issues 1 more launch after the direction launch, whatever the number of
+ * pages: every kept leaf i of such a page writes entry i, from the bands along its direction (rows when its leaves[] st lacks
+ * MN_PAGE_VERTICAL, else columns), the maximal runs of non-white indices of the direction test: n_bands, e_lo = the sum over
+ * bands of lo_k - min lo and e_hi = the sum of max hi - hi_k, lo_k and hi_k the least and largest index across of an ink bit
+ * of band k's rows (columns) inside the leaf; all 0 without a band.  Rejected leaves keep a zero entry.  The launch skips pages
+ * without the table and pages with an error; a call without MN_PAGE_TURNS issues exactly the launches above. */
 #define MN_PAGE_RULES 1
 #define MN_PAGE_FIGURES 2
 #define MN_PAGE_DIRECTIONS 4
 #define MN_PAGE_PANELS 8
+#define MN_PAGE_TURNS 16
+#define MN_PAGE_DIRS_TURN 2     /* dirs bit: a turn page, with a vote table */
+typedef struct {
+    int32_t n_bands, pad;
+    int64_t e_lo, e_hi;
+} mn_page_turn;
 #define MN_PAGE_MAX_FIGURES 1024
 #define MN_PAGE_MAX_PANELS 1024
 #define MN_PAGE_LEVELS 24
@@ -877,7 +891,7 @@ typedef struct {
     int32_t src, active, open, gx, gy, pad, n[2];   /* state, written by the call */
     uint32_t* rbits;            /* null, or a ruled page's h x wpitch words of U followed by w x ceil(h / 32) words of scratch */
     int32_t rule_length;        /* a ruled page's rule length, 2 <= rule_length <= 32767 */
-    int32_t dirs;               /* 1: a direction page, its blocks' directions tested; else 0 */
+    int32_t dirs;               /* 1: a direction page, its blocks' directions tested; else 0.  | MN_PAGE_DIRS_TURN: a turn page */
     uint32_t* fbits;            /* null, or a figure page's h x wpitch words of F */
     mn_page_node* figs;         /* a figure page's table of MN_PAGE_MAX_FIGURES figures */
     int32_t figure_size;        /* a figure page's f in [2, 32767], or 0 for 3 S */

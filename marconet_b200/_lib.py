@@ -214,6 +214,7 @@ PAGE_ERR_NODES, PAGE_ERR_BLOCKS, PAGE_ERR_FIGURES, PAGE_ERR_PANELS = 1, 2, 3, 4
 PAGE_RULES, PAGE_FIGURES, PAGE_MAX_FIGURES = 1, 2, 1024           # MN_PAGE_RULES, MN_PAGE_FIGURES, MN_PAGE_MAX_FIGURES
 PAGE_DIRECTIONS, PAGE_VERTICAL, PAGE_UNDECIDED = 4, 16, 32         # MN_PAGE_DIRECTIONS, MN_PAGE_VERTICAL, MN_PAGE_UNDECIDED
 PAGE_PANELS, PAGE_MAX_PANELS = 8, 1024                             # MN_PAGE_PANELS, MN_PAGE_MAX_PANELS
+PAGE_TURNS, PAGE_DIRS_TURN = 16, 2                                 # MN_PAGE_TURNS, MN_PAGE_DIRS_TURN
 
 
 class PageNode(Structure):
@@ -233,6 +234,10 @@ class TextPage(Structure):
                 ("gy", c_int32), ("pad", c_int32), ("n", c_int32 * 2), ("rbits", c_void_p), ("rule_length", c_int32), ("dirs", c_int32),
                 ("fbits", c_void_p), ("figs", c_void_p), ("figure_size", c_int32), ("frows", c_int32), ("pans", c_void_p),
                 ("panel_size", c_int32), ("prows", c_int32), ("pdone", c_int32), ("pad3", c_int32)]
+
+
+class PageTurn(Structure):
+    _fields_ = [("n_bands", c_int32), ("pad", c_int32), ("e_lo", c_int64), ("e_hi", c_int64)]
 
 
 class PageQuad(Structure):

@@ -1742,6 +1742,172 @@ __global__ void __launch_bounds__(kPageThreads) page_direction_kernel(mn_text_pa
     }
 }
 
+// ---- Page turns (DESIGN.md 7b, "Page turns") ----
+// A turn page's vote table: cap mn_page_turn entries at the first 16-byte boundary after its leaf table.
+__device__ __forceinline__ mn_page_turn* turn_table(const mn_text_page& p) {
+    return reinterpret_cast<mn_page_turn*>((reinterpret_cast<uintptr_t>(p.leaves + p.cap) + 15) & ~(uintptr_t)15);
+}
+
+// Exclusive max-scan of v over the CTA (0 before the first thread); *total receives the maximum.  s holds 32 values.
+__device__ unsigned long long cta_max_scan64(unsigned long long v, unsigned long long* s, unsigned long long* total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+    unsigned long long x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x = max(x, y);
+    }
+    const unsigned long long before = __shfl_up_sync(0xffffffffu, x, 1);
+    if (lane == 31) s[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        unsigned long long w = lane < n_warps ? s[lane] : 0ull;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= o) w = max(w, y);
+        }
+        s[lane] = w;
+    }
+    __syncthreads();
+    const unsigned long long pre = max(warp ? s[warp - 1] : 0ull, lane ? before : 0ull);
+    *total = s[n_warps - 1];
+    __syncthreads();
+    return pre;
+}
+
+// T1. The vote statistics of every kept leaf of a turn page, one CTA per leaf (grid-stride over blockIdx.x), after the
+// direction launch: along the leaf's direction (rows when horizontal, columns when vertical) its bands are node_profile's
+// maximal runs of non-white indices, and band k spans [lo_k, hi_k] across, the least and largest index of an ink bit of its
+// rows (columns) inside the leaf.  Its table entry is (n, E_lo, E_hi): n bands, E_lo = sum (lo_k - min lo) and
+// E_hi = sum (max hi - hi_k), all 0 without a band.  4096 indices at a time: each index's extent into shared memory (rows by a
+// warp's ffs / clz over its words, columns by per-bit atomicMin / atomicMax), then each band's by a max-scan of the keys
+// (w + 1) << 32 | value, w the last white index before it, which is constant along a band and grows from band to band.
+// Pages without a vote table, and pages with an error, return at once.
+__global__ void __launch_bounds__(kPageThreads) page_turn_kernel(mn_text_page* pages) {
+    mn_pdl_prologue();
+    __shared__ page_smem s;
+    __shared__ int s_hi[kChunk];
+    __shared__ unsigned long long s_key[32];
+    __shared__ long long s_sum[32];
+    const mn_text_page& p = pages[blockIdx.y];
+    if (!(p.dirs & MN_PAGE_DIRS_TURN) || p.res->error) return;
+    mn_page_turn* votes = turn_table(p);
+    const mn_page_node* list = p.list[p.src];
+    const int n = p.res->n_leaves;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+    constexpr int kPer = kChunk / kPageThreads;
+    constexpr int kFar = 32767;                         // lo is keyed as kFar - lo, so that the max-scan takes the least
+    for (int i = blockIdx.x; i < n; i += gridDim.x) {
+        const int st = p.leaves[i].st;
+        if (st & MN_PAGE_REJECTED) continue;
+        const mn_page_node nd = list[i];
+        const bool rows = !(st & MN_PAGE_VERTICAL);
+        node_profile(p, nd, rows, s);
+        const int lo = rows ? nd.y0 : nd.x0, L = (rows ? nd.y1 : nd.x1) - lo;
+        unsigned long long kl = 0, kh = 0;             // the keys carried from the chunks before
+        int white = -1, nb = 0, min_lo = kFar, max_hi = -1;
+        long long sum_lo = 0, sum_hi = 0;
+        for (int c0 = 0; c0 < L; c0 += kChunk) {
+            const int m = min(kChunk, L - c0);
+            __syncthreads();                            // the previous chunk's readers of s.cnt and s_hi are done
+            if (rows) {
+                const int wx0 = nd.x0 >> 5, wx1 = (nd.x1 - 1) >> 5;
+                for (int r = warp; r < m; r += n_warps) {
+                    const long long o = (long long)(lo + c0 + r) * p.wpitch;
+                    int f = 1 << 30, l = -1;
+                    for (int wd = wx0 + lane; wd <= wx1; wd += 32) {
+                        const unsigned v = p.bits[o + wd] & word_mask(wd, nd.x0, nd.x1);
+                        if (v) {
+                            f = min(f, 32 * wd + __ffs(v) - 1);
+                            l = max(l, 32 * wd + 31 - __clz(v));
+                        }
+                    }
+                    f = __reduce_min_sync(0xffffffffu, f);
+                    l = __reduce_max_sync(0xffffffffu, l);
+                    if (lane == 0) {
+                        s.cnt[r] = f - nd.x0;
+                        s_hi[r] = l - nd.x0;
+                    }
+                }
+            } else {
+                for (int j = threadIdx.x; j < m; j += blockDim.x) {
+                    s.cnt[j] = kFar;
+                    s_hi[j] = -1;
+                }
+                __syncthreads();
+                const int a = lo + c0, e = a + m, w0 = a >> 5, nwords = ((e - 1) >> 5) - w0 + 1;
+                const int total = nwords * (nd.y1 - nd.y0);
+                for (int k = threadIdx.x; k < total; k += blockDim.x) {
+                    const int y = nd.y0 + k / nwords, wd = w0 + k % nwords;
+                    for (unsigned v = p.bits[(long long)y * p.wpitch + wd] & word_mask(wd, a, e); v; v &= v - 1u) {
+                        const int c = (wd << 5) + __ffs(v) - 1 - a;
+                        atomicMin(&s.cnt[c], y - nd.y0);
+                        atomicMax(&s_hi[c], y - nd.y0);
+                    }
+                }
+            }
+            __syncthreads();
+            const int j0 = threadIdx.x * kPer, j1 = min(j0 + kPer, m);
+            auto inked = [&](int x) { return (s.nw[x >> 5] >> (x & 31)) & 1u; };
+            int my_white = -1;
+            unsigned long long my_kl = 0, my_kh = 0;
+            for (int j = j0; j < j1; ++j)
+                if (!inked(c0 + j)) my_white = c0 + j;
+            int w_total;
+            int w = max(white, cta_max_scan(my_white, s.scan, &w_total));
+            const int w_in = w;
+            for (int j = j0; j < j1; ++j) {
+                if (!inked(c0 + j)) {
+                    w = c0 + j;
+                    continue;
+                }
+                const unsigned long long key = (unsigned long long)(w + 1) << 32;
+                my_kl = max(my_kl, key | (unsigned)(kFar - s.cnt[j]));
+                my_kh = max(my_kh, key | (unsigned)s_hi[j]);
+            }
+            unsigned long long tl, th;
+            unsigned long long pl = max(kl, cta_max_scan64(my_kl, s_key, &tl));
+            unsigned long long ph = max(kh, cta_max_scan64(my_kh, s_key, &th));
+            w = w_in;
+            for (int j = j0; j < j1; ++j) {
+                const int x = c0 + j;
+                if (!inked(x)) {
+                    w = x;
+                    continue;
+                }
+                const unsigned long long key = (unsigned long long)(w + 1) << 32;
+                pl = max(pl, key | (unsigned)(kFar - s.cnt[j]));
+                ph = max(ph, key | (unsigned)s_hi[j]);
+                if (x + 1 == L || !inked(x + 1)) {      // the band ends here: its extent is complete
+                    const int blo = kFar - (int)(pl & 0xffffffffull), bhi = (int)(ph & 0xffffffffull);
+                    ++nb;
+                    sum_lo += blo;
+                    sum_hi += bhi;
+                    min_lo = min(min_lo, blo);
+                    max_hi = max(max_hi, bhi);
+                }
+            }
+            kl = max(kl, tl);
+            kh = max(kh, th);
+            white = max(white, w_total);
+        }
+        int n_bands, far_lo, top_hi;
+        cta_scan(nb, s.scan, &n_bands);
+        cta_max_scan(kFar - min_lo, s.scan, &far_lo);
+        cta_max_scan(max_hi, s.scan, &top_hi);
+        const long long s_lo = cta_sum64(sum_lo, s_sum), s_hi_sum = cta_sum64(sum_hi, s_sum);
+        if (threadIdx.x == 0) {
+            mn_page_turn r;
+            r.n_bands = n_bands;
+            r.pad = 0;
+            r.e_lo = n_bands ? s_lo - (long long)n_bands * (kFar - far_lo) : 0;
+            r.e_hi = n_bands ? (long long)n_bands * top_hi - s_hi_sum : 0;
+            votes[i] = r;
+        }
+    }
+}
+
 // ---- Skewed pages (DESIGN.md 7b, "Skewed pages") ----
 // The page's angle is searched by the skewed-block kernels on its mn_skew_block record; the XY-cut then runs unchanged on a
 // bitmap of frame cells, whose sides the page record takes.  A vertical page's bitmap is of the untransposed frame at the
@@ -2704,6 +2870,10 @@ int page_levels(mn_text_page* pages, int n, long long max_tiles, int flags, cuda
     MN_LAUNCH_CHECK();
     if (flags & MN_PAGE_DIRECTIONS) {
         MN_CUDA_CHECK((mn_launch(page_direction_kernel, grid, dim3(kPageThreads), 0, st, pages)));
+        MN_LAUNCH_CHECK();
+    }
+    if (flags & MN_PAGE_TURNS) {
+        MN_CUDA_CHECK((mn_launch(page_turn_kernel, grid, dim3(kPageThreads), 0, st, pages)));
         MN_LAUNCH_CHECK();
     }
     return MN_OK;

@@ -7,7 +7,6 @@ slices of a concatenation buffer).
 """
 import ctypes
 import functools
-import itertools
 import math
 from typing import NamedTuple
 
@@ -2108,6 +2107,7 @@ class PageItem(NamedTuple):
     panel_size: object = None
     seal_size: object = None
     seal_lines: bool = False
+    turns: bool = False
 
 
 def page_cap(w, h):
@@ -2144,13 +2144,15 @@ def _page_areas(L, M, cap, n_ang, stride, rules, figures, panels):
             plane if panels and not rules else 0]
 
 
-def page_bytes(w, h, vertical=False, cs=None, rules=False, figures=False, panels=False, seals=False, seal_lines=False):
+def page_bytes(w, h, vertical=False, cs=None, rules=False, figures=False, panels=False, seals=False, seal_lines=False,
+               turns=False):
     """Device bytes of one w x h page in find_blocks, with or without ``rules``, ``figures`` and ``panels``: its records,
     result and leaf table, a figure page's table of PAGE_MAX_FIGURES and a panel page's table of PAGE_MAX_PANELS page nodes,
     its work areas and 64 bytes for the call's 16-byte alignments.  ``cs``: None in a call without skewed pages, else the
     (c, s) table the page searches ([(1.0, 0.0)] for a page with skew None), which adds the search record, the table and 16
     bytes for its alignment; the page's bitmaps are then those of its largest frame.  ``seals``: with seal_bytes, and
-    ``seal_lines`` with seal_line_bytes."""
+    ``seal_lines`` with seal_line_bytes.  ``turns``: with its vote table of one mn_page_turn per leaf and 16 bytes for its
+    alignment."""
     n_ang = len(cs) if cs else 1
     L, M, stride = skew_page_frame(w, h, vertical, cs or [(1.0, 0.0)])
     cap = page_cap(M, L)
@@ -2158,7 +2160,7 @@ def page_bytes(w, h, vertical=False, cs=None, rules=False, figures=False, panels
     search = ctypes.sizeof(_lib.SkewBlock) + 16 * n_ang + 16 if cs else 0
     return (ctypes.sizeof(_lib.PageResult) + ctypes.sizeof(_lib.TextBlock) + ctypes.sizeof(_lib.TextPage) + tables + search
             + sum(_page_areas(L, M, cap, n_ang, stride, rules, figures, panels)) + 64 + (seal_bytes(w, h) if seals else 0)
-            + (seal_line_bytes() if seal_lines else 0))
+            + (seal_line_bytes() if seal_lines else 0) + (ctypes.sizeof(_lib.PageTurn) * cap + 16 if turns else 0))
 
 
 def seal_line_bytes():
@@ -2209,6 +2211,9 @@ def _check_page_options(page, what):
     v = page.seal_lines
     if not isinstance(v, bool) or (v and page.seal_size is None):
         raise ValueError(f"{what}: seal_lines {v!r} is not False, or True on a page with a seal_size")
+    v = page.turns
+    if not isinstance(v, bool) or (v and (page.skew is not None or page.seal_size is not None or not page.directions)):
+        raise ValueError(f"{what}: turns {v!r} is not False, or True on a page with directions, skew None and no seal_size")
 
 
 def find_blocks(pages, scores=False):
@@ -2248,6 +2253,10 @@ def find_blocks(pages, scores=False):
     and centre lines are found (mn_find_seal_lines_u8's 1 launch for all such pages of the call, after mn_find_seals_u8).  out
     then has, after the seal tables, each such page's mn_seal_line_table, in the order of the pages (seal_line_tables reads
     them back).
+    turns (DESIGN.md 7b, "Page turns"): False, or True on a page with directions (skew None, no seal_size): each kept leaf's
+    bands along its direction give its vote entry (n_bands, e_lo, e_hi) in the page's table of caps[i] _lib.PageTurn records
+    (1 more launch for all such pages of the call, after the direction launch).  The table lies in out at the first 16-byte
+    boundary after the page's leaf table (page_tables reads it back).
     A page without one of these options gets the tables of a call without it."""
     global LAUNCHES
     dev = _check_items(pages, "find_blocks", "page")
@@ -2265,7 +2274,7 @@ def find_blocks(pages, scores=False):
         opts = (p.rule_length is not None, p.figure_size is not None, p.panel_size is not None)   # rules, figures, panels
         L, M, stride = skew_page_frame(bw, bh, p.vertical, cs)
         need += page_bytes(bw, bh, p.vertical, cs if skewed else None, *opts, seals=p.seal_size is not None,
-                           seal_lines=p.seal_lines)
+                           seal_lines=p.seal_lines, turns=p.turns)
         if max(L, M) > 32767:
             raise ValueError(f"{what}: a frame side of {max(L, M)} exceeds 32767")
         if len(cs) > 1 and len(cs) * stride > SKEW_MAX_PROFILE:
@@ -2295,7 +2304,11 @@ def find_blocks(pages, scores=False):
     sk0 = out0 - n * ssz            # the skew records end where the results begin, the line tables where they begin and the
     lt0 = sk0 - ml * lsz            # seal tables where those begin
     st0 = lt0 - m * tsz
-    leaves = [pack.area(12 * d[4]) for d in dims]
+    leaves = []
+    for d, p in zip(dims, pages):                   # a turn page's vote table follows its leaves at the next 16-byte boundary
+        leaves.append(pack.area(12 * d[4]))
+        if p.turns:
+            pack.area(ctypes.sizeof(_lib.PageTurn) * d[4], 16)
     figs = [pack.area(12 * _lib.PAGE_MAX_FIGURES) if d[8][1] else None for d in dims]
     pans = [pack.area(12 * _lib.PAGE_MAX_PANELS) if d[8][2] else None for d in dims]
     out1 = pack.end
@@ -2325,7 +2338,8 @@ def find_blocks(pages, scores=False):
                                   counts + 8 * cap, base + out0 + i * rsz, -(-M // 32), cap, p.gap_x or 0, p.gap_y or 0,
                                   rbits=rbits if rules else pbits if panels else None, rule_length=p.rule_length or 0,
                                   fbits=fbits if figures else None, figs=base + f if figures else None,
-                                  figure_size=p.figure_size or 0, dirs=int(bool(p.directions)),
+                                  figure_size=p.figure_size or 0,
+                                  dirs=int(bool(p.directions)) | (_lib.PAGE_DIRS_TURN if p.turns else 0),
                                   pans=base + pn if panels else None, panel_size=p.panel_size or 0))
         views.append(pack.buf[wk[0]:wk[0] + 8 * n_ang].view(torch.int64) if n_ang > 1 else None)
         tiles = max(tiles, -(-bw // 32) * -(-bh // 32))
@@ -2341,40 +2355,56 @@ def find_blocks(pages, scores=False):
         LAUNCHES += 1
     ruled, figured, directed, paneled = (any(p.rule_length is not None for p in pages), any(f is not None for f in figs),
                                          any(p.directions for p in pages), any(pn is not None for pn in pans))
+    turned = any(p.turns for p in pages)
     flags = ((_lib.PAGE_RULES if ruled else 0) | (_lib.PAGE_FIGURES if figured else 0) | (_lib.PAGE_DIRECTIONS if directed else 0)
-             | (_lib.PAGE_PANELS if paneled else 0))
+             | (_lib.PAGE_PANELS if paneled else 0) | (_lib.PAGE_TURNS if turned else 0))
     entry, head = ("mn_find_blocks_skewed_u8", (base, base + sk0)) if skewed else ("mn_find_blocks_u8", (base,))
     w_bytes = (w_end if sealed else len(buf)) - out0
     _lib.check(getattr(_lib.load(), entry)(*head, base + pg, n, tiles, flags, base + out0, w_bytes, _stream()), entry)
-    LAUNCHES += (7 if skewed else 5) + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed + 2 * paneled
+    LAUNCHES += (7 if skewed else 5) + 6 * _lib.PAGE_LEVELS + 3 * ruled + figured + directed + 2 * paneled + turned
     res = buf[st0:out1], [d[4] for d in dims]
     return res + (views,) if scores else res
 
 
 def page_tables(host, pages, caps):
     """Per page of a find_blocks call, numpy views of its tables in ``host``, the uint8 host copy of the call's out:
-    (skew, res, leaves, figures, panels).  skew is its mn_skew_block record (None in a call without skewed pages), res its
-    mn_page_result record, and leaves, figures and panels its mn_page_node entries, as many as res counts; figures is None
-    unless the page has a figure_size, panels None unless it has a panel_size."""
-    sdt, rdt, ndt = skew_block_dtype(), page_result_dtype(), page_node_dtype()
+    (skew, res, leaves, figures, panels, turns).  skew is its mn_skew_block record (None in a call without skewed pages), res
+    its mn_page_result record, and leaves, figures and panels its mn_page_node entries, as many as res counts; figures is None
+    unless the page has a figure_size, panels None unless it has a panel_size.  turns is a turn page's mn_page_turn entries
+    (page_turn_dtype()), one per leaf, else None."""
+    sdt, rdt, ndt, tdt = skew_block_dtype(), page_result_dtype(), page_node_dtype(), page_turn_dtype()
     n = len(pages)
     host = host[ctypes.sizeof(_lib.SealTable) * sum(p.seal_size is not None for p in pages)
                 + ctypes.sizeof(_lib.SealLineTable) * sum(p.seal_lines for p in pages):]
     o = n * sdt.itemsize if any(p.skew is not None for p in pages) else 0
     skews = host[:o].view(sdt) if o else [None] * n
     res = host[o:o + n * rdt.itemsize].view(rdt)
-    nodes = host[o + n * rdt.itemsize:].view(ndt)       # every leaf table, then the figure pages' tables, then the panel pages'
-    f = sum(caps)
-    t = f + _lib.PAGE_MAX_FIGURES * sum(p.figure_size is not None for p in pages)
+    host = host[o:]                                     # from the results on, 16-byte aligned as in the device buffer
+    pos, tables = n * rdt.itemsize, []                  # every leaf table (and vote table), then the figure and panel tables
+    for p, cap in zip(pages, caps):
+        lv, pos, tv = pos, pos + 12 * cap, None
+        if p.turns:
+            t0 = -(-pos // 16) * 16
+            tv, pos = host[t0:t0 + tdt.itemsize * cap].view(tdt), t0 + tdt.itemsize * cap
+        tables.append((host[lv:lv + 12 * cap].view(ndt), tv))
+    nodes = host[pos:].view(ndt)
+    f = 0
+    t = _lib.PAGE_MAX_FIGURES * sum(p.figure_size is not None for p in pages)
     out = []
-    for p, sk, r, l0, cap in zip(pages, skews, res, itertools.accumulate(caps, initial=0), caps):
+    for p, sk, r, (lv, tv) in zip(pages, skews, res, tables):
         figs = pans = None
         if p.figure_size is not None:
             figs, f = nodes[f:f + _lib.PAGE_MAX_FIGURES][:int(r["n_figures"])], f + _lib.PAGE_MAX_FIGURES
         if p.panel_size is not None:
             pans, t = nodes[t:t + _lib.PAGE_MAX_PANELS][:int(r["n_panels"])], t + _lib.PAGE_MAX_PANELS
-        out.append((sk, r, nodes[l0:l0 + cap][:int(r["n_leaves"])], figs, pans))
+        out.append((sk, r, lv[:int(r["n_leaves"])], figs, pans, None if tv is None else tv[:int(r["n_leaves"])]))
     return out
+
+
+def page_turn_dtype():
+    """numpy view of an mn_page_turn record."""
+    import numpy as np
+    return np.dtype([("n_bands", "<i4"), ("pad", "<i4"), ("e_lo", "<i8"), ("e_hi", "<i8")])
 
 
 def seal_tables(host, pages):

@@ -2194,7 +2194,13 @@ class TextPage(NamedTuple):
     ``seal_lines`` (DESIGN.md 7b, "Seal centre lines"): None, or "auto" with seals="auto": each seal's turn is read off the gap
     of its arc text's outer bins, its arc band stops where the arc sectors thin out, and the horizontal lines of text across
     its centre (合同专用章 under a star, an invoice seal's number) are found in the stamp's frame and restored as rectangles or
-    OrientedRegions.  The arc, band and why then follow that definition."""
+    OrientedRegions.  The arc, band and why then follow that definition.
+    ``turn`` (DESIGN.md 7b, "Page turns"): None, 0, 90, 180, 270 or "auto", for a page scanned sideways or upside down.
+    turn = 90 k means the image shows the upright page turned k quarter turns counter-clockwise (the crop is
+    np.rot90(upright, k)).  A given turn is exactly TextPage(quad=turn_quad(rect or quad, turn), rect=None) with the page's
+    other fields (turn 0: the page without turn); "auto" votes on the device over the page's blocks, whose aligned line starts
+    and ragged line ends give the turn, and lays the page out again as the turn found.  ``direction`` stays the upright page's.
+    Only on level pages and quad pages: not with skew, curve or seals (flatten such a page with flatten_pages first)."""
     rect: object = None
     direction: str = "horizontal"
     polarity: str = "auto"
@@ -2214,6 +2220,43 @@ class TextPage(NamedTuple):
     seals: object = None
     seal_size: object = None
     seal_lines: object = None
+    turn: object = None
+
+
+TURNS = (0, 90, 180, 270)
+# The score a leaf's |D| = |E_hi - E_lo| adds to, by (page vertical, leaf vertical, D > 0): line starts are aligned and line
+# ends ragged, so an upright horizontal leaf has D > 0 (DESIGN.md 7b, "Page turns").
+_TURN_VOTE = {(False, False, True): 0, (False, False, False): 180, (False, True, True): 270, (False, True, False): 90,
+              (True, True, True): 0, (True, True, False): 180, (True, False, True): 90, (True, False, False): 270}
+
+
+def turn_quad(rect_or_quad, turn):
+    """The QuadRegion through which a page turned ``turn`` degrees (TextPage's turn) is read upright: the corners
+    (tl, tr, br, bl) of the integer rectangle (x0, y0, x1, y1) or of the QuadRegion, rotated right by turn / 90 places.  Its rectified crop is
+    np.rot90(crop, -turn // 90) for a rectangle."""
+    if turn not in TURNS or isinstance(turn, bool):
+        raise ValueError(f"turn must be one of {TURNS}, got {turn!r}")
+    if isinstance(rect_or_quad, QuadRegion):
+        pts = [(float(p[0]), float(p[1])) for p in rect_or_quad]
+    else:
+        x0, y0, x1, y1 = (float(v) for v in rect_or_quad)
+        pts = [(x0, y0), (x1, y0), (x1, y1), (x0, y1)]
+    k = turn // 90
+    return QuadRegion(*(pts[(m - k) % 4] for m in range(4)))
+
+
+def page_turn(votes):
+    """The turn (0, 90, 180 or 270) of the vote scores (V_0, V_90, V_180, V_270): the largest, ties to the least."""
+    return 90 * max(range(4), key=lambda k: (votes[k], -k))
+
+
+def _turned(pg, rect, shape=None):
+    """(TextPage, rect) of a page with a given turn (its quad known): TextPage(quad=turn_quad(...), rect=None, turn=None) and its
+    quad's pixel box, or the page without turn for turn 0."""
+    if pg.turn == 0:
+        return pg._replace(turn=None), rect
+    q = turn_quad(pg.quad if pg.quad is not None else rect, pg.turn)
+    return pg._replace(quad=q, rect=None, turn=None), _quad_box(q, shape)
 
 
 def _check_page(pg, H, W, name):
@@ -2250,6 +2293,21 @@ def _check_page(pg, H, W, name):
         raise ValueError(f"{name}: seal_lines must be None or 'auto', got {pg.seal_lines!r}")
     if pg.seal_lines is not None and pg.seals is None:
         raise ValueError(f"{name}: seal_lines is given, but seals is None, not 'auto'")
+    if pg.turn is not None:
+        if not (isinstance(pg.turn, str) and pg.turn == "auto") and (isinstance(pg.turn, bool) or pg.turn not in TURNS
+                                                                     or not isinstance(pg.turn, int)):
+            raise ValueError(f"{name}: turn must be None, 0, 90, 180, 270 or 'auto', got {pg.turn!r}")
+        for what in ("skew", "curve", "seals"):
+            if getattr(pg, what) is not None:
+                raise ValueError(f"{name}: turn and {what} are both given (a turned page is level and flat: flatten a tilted "
+                                 f"or curled page with flatten_pages first{', and turn it' if what == 'seals' else ''})")
+        if isinstance(pg.turn, int) and not isinstance(pg.quad, str):
+            base = _check_page(pg._replace(turn=None), H, W, name)
+            turned, _ = _turned(pg, base, (H, W))
+            rect = _check_page(turned, H, W, name)
+            if _page_bytes(pg, rect, False) > ops.PAGE_MAX_WORK:
+                raise ValueError(f"{name}: the page needs more than the {ops.PAGE_MAX_WORK} bytes of work memory a call may use")
+            return rect
     if pg.quad is not None:
         if pg.rect is not None:
             raise ValueError(f"{name}: rect and quad are both given (a page in perspective is its quad: give rect=None)")
@@ -2289,11 +2347,17 @@ def _page_table(pg):
 
 def _page_bytes(pg, rect, skewed):
     """Device bytes of a page in a find_blocks call with (``skewed``) or without skewed pages (ops.page_bytes): a quad page's
-    rectified crop and its page, or an auto page's corner search on the image ``rect``."""
+    rectified crop and its page, or an auto page's corner search on the image ``rect``.  A page with a given turn is its
+    turned quad page; one with turn "auto" counts its vote table and the rectified crop of a turned second pass."""
     from . import ops
     w, h = rect[2] - rect[0], rect[3] - rect[1]
+    if isinstance(pg.turn, int) and not isinstance(pg.quad, str):
+        return _page_bytes(*_turned(pg, rect), skewed)
+    if isinstance(pg.turn, str) and pg.quad is None:
+        table = ops.page_bytes(w, h, turns=True) - ops.page_bytes(w, h)
+        return 3 * w * h + _page_bytes(pg._replace(turn=None), rect, skewed) + table
     if isinstance(pg.quad, str):
-        return ops.quad_page_bytes(w, h)
+        return ops.quad_page_bytes(w, h) + (3 * w * h if isinstance(pg.turn, str) else 0)
     if pg.quad is not None:
         w_r, h_r = quad_maps(pg.quad, 1).size
         return 3 * w_r * h_r + _page_bytes(pg._replace(quad=None), (0, 0, w_r, h_r), skewed)
@@ -2353,12 +2417,39 @@ def _page_quads(dimg, items, spreads=()):
 
 def _find_pages(dimg, items, keys=()):
     """_page_quads, _rectify and _find_blocks over items (image index, TextPage, rect): per item the _find_blocks result or an
-    error message, and the rectified crops of every quad page and of ``keys`` (warped in one launch)."""
+    error message, and the rectified crops of every quad page and of ``keys`` (warped in one launch).  A page with a given
+    turn is laid out as its turned quad page (_turned), its dict gaining ``turn``; a page with turn "auto" votes in the same
+    layout, and the pages found turned are laid out once more as their turned quad pages (one more rectify launch and
+    layout for all of them), their dicts gaining ``turn`` and ``turn_votes``."""
     items = _page_quads(dimg, items)
+    given = {k: it[1].turn for k, it in enumerate(items) if not isinstance(it, str) and it[1].turn is not None}
+    for k, t in given.items():
+        if t == "auto":
+            continue
+        i, pg, rect = items[k]
+        items[k] = (i,) + _turned(pg, rect, dimg[i].shape[:2])
     ok = [it for it in items if not isinstance(it, str)]
     rq = _rectify(dimg, [_quad_key(i, pg.quad) for i, pg, _ in ok if pg.quad is not None] + list(keys))
     found = iter(_find_blocks(dimg, ok, rq) if ok else [])
-    return [it if isinstance(it, str) else next(found) for it in items], rq
+    res = [it if isinstance(it, str) else next(found) for it in items]
+    again = []                                          # "auto" pages found turned: (index, turned item)
+    for k, t in given.items():
+        if t != "auto" or isinstance(res[k], str):
+            continue
+        votes = res[k].pop("turn_votes")
+        turn = page_turn(votes)
+        res[k].update(turn=turn, turn_votes=votes)
+        if turn:
+            i, pg, rect = items[k]
+            again.append((k, (i,) + _turned(pg._replace(turn=turn), rect, dimg[i].shape[:2]), votes))
+    if again:
+        rq.update(_rectify(dimg, [_quad_key(i, pg.quad) for _, (i, pg, _), _ in again]))
+        for (k, _, votes), r in zip(again, _find_blocks(dimg, [it for _, it, _ in again], rq)):
+            res[k] = r if isinstance(r, str) else dict(r, turn=res[k]["turn"], turn_votes=votes)
+    for k, t in given.items():
+        if t != "auto" and not isinstance(res[k], str):
+            res[k]["turn"] = t
+    return res, rq
 
 
 def seal_size(w, h):
@@ -2440,6 +2531,20 @@ def _node_rects(nodes, x0=0, y0=0):
     return [(x0 + int(q["x0"]), y0 + int(q["y0"]), x0 + int(q["x1"]), y0 + int(q["y1"])) for q in nodes]
 
 
+def _turn_votes(vertical, leaves, table):
+    """The scores (V_0, V_90, V_180, V_270) of a turn page (DESIGN.md 7b, "Page turns") from its leaves and their mn_page_turn
+    entries: each kept leaf whose direction test was decided and which has at least 2 bands adds |D|, D = E_hi - E_lo, to the
+    score _TURN_VOTE names."""
+    from . import ops
+    lib, v = ops._lib, [0, 0, 0, 0]
+    for q, e in zip(leaves, table):
+        st, d = int(q["st"]), int(e["e_hi"]) - int(e["e_lo"])
+        if st & (lib.PAGE_REJECTED | lib.PAGE_UNDECIDED) or e["n_bands"] < 2 or d == 0:
+            continue
+        v[_TURN_VOTE[(vertical, bool(st & lib.PAGE_VERTICAL), d > 0)] // 90] += abs(d)
+    return tuple(v)
+
+
 def _find_blocks(dimg, items, rq=None):
     """ops.find_blocks over items (image index, TextPage, rect) of the uploaded images ``dimg``, its tables back through one
     pinned copy and one synchronisation; a quad page (its corners given) is a level page on all of its rectified crop in ``rq``
@@ -2461,10 +2566,10 @@ def _find_blocks(dimg, items, rq=None):
         return ops.PageItem(img, crop, pg.direction == "vertical", _INK[pg.polarity], pg.gap_x, pg.gap_y, pg.skew, pg.max_skew,
                             rule_length=rl,
                             figure_size=None if pg.figures is None else pg.figure_size or 0,
-                            directions=pg.block_direction is not None,
+                            directions=pg.block_direction is not None or pg.turn == "auto",
                             panel_size=None if pg.panels is None else pg.panel_size or 0,
                             seal_size=None if pg.seals is None else pg.seal_size or seal_size(crop[2] - crop[0], crop[3] - crop[1]),
-                            seal_lines=pg.seal_lines is not None)
+                            seal_lines=pg.seal_lines is not None, turns=pg.turn == "auto")
     pages = [page(*it) for it in items]
     res_t, caps = ops.find_blocks(pages)
     host = _to_host(res_t).numpy()
@@ -2472,8 +2577,8 @@ def _find_blocks(dimg, items, rq=None):
     limits = {lib.PAGE_ERR_BLOCKS: ("blocks", lib.PAGE_MAX_BLOCKS), lib.PAGE_ERR_FIGURES: ("figures", lib.PAGE_MAX_FIGURES),
               lib.PAGE_ERR_PANELS: ("panels", lib.PAGE_MAX_PANELS)}
     out = []
-    for (i, pg, rect), p, (sk, r, leaves, figs, pans), stab, ltab in zip(items, pages, ops.page_tables(host, pages, caps), stabs,
-                                                                        ltabs):
+    for (i, pg, rect), p, (sk, r, leaves, figs, pans, votes), stab, ltab in zip(items, pages, ops.page_tables(host, pages, caps),
+                                                                               stabs, ltabs):
         if stab is not None and stab["error"]:
             out.append(f"{int(stab['n_cand'])} seal candidates exceed the {lib.PAGE_MAX_SEALS} a text page may hold")
             continue
@@ -2521,6 +2626,8 @@ def _find_blocks(dimg, items, rq=None):
             res.update(block_direction=pg.block_direction, undecided=undecided)
         if pans is not None:                            # in image coordinates, or rectangles of R on a quad page
             res.update(panel_size=int(r["panel_size"]), panels=_node_rects(pans, X0, Y0))
+        if votes is not None:                           # _find_pages turns the scores into the page's turn
+            res["turn_votes"] = _turn_votes(vertical, leaves, votes)
         if pg.quad is not None:
             shape = dimg[i].shape[:2]
             res.update(blocks=[TextBlock.from_quad(pg.quad, shape, direction=d, polarity=pl, window=b)
@@ -2599,7 +2706,12 @@ def find_blocks(images, pages):
     per centre line top to bottom in the stamp's frame: box ((u0, v0, u1, v1), pixels from the seal box's centre in the
     stamp's frame), region (a rectangle when turn is 0, else an OrientedRegion; None when restore_regions rejects it) and, when
     region is None, why.  The seal's band, arc, region and why follow the centre-line definition: its turn and arc come from
-    the gap of the arc text's outer 4 bins, and its band stops where the arc sectors thin out."""
+    the gap of the arc text's outer 4 bins, and its band stops where the arc sectors thin out.
+    A page with a given ``turn`` (DESIGN.md 7b, "Page turns") is laid out as TextPage(quad=turn_quad(rect or quad, turn)) and
+    its dict gains ``turn``.  One with ``turn="auto"`` votes in its own layout (the direction launch if no page asked for it,
+    and 1 more launch for all such pages of the call), and the pages found turned are laid out once more as their turned
+    quads (one rectify launch and one layout for all of them, and one more synchronisation); its dict is that of its found
+    turn given, plus ``turn`` and ``turn_votes`` (V_0, V_90, V_180, V_270)."""
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
     items, names = [], []
@@ -2703,7 +2815,10 @@ class FlatPage(NamedTuple):
     ops.light_window of the frame, a heuristic: darker features wider than the window are lightened); the page's searches then
     run on the evened frame, and the flat page is evened with the same window and ink.  ``spread="auto"`` (DESIGN.md 7b, "Book
     spreads"; with quad="auto") takes the page for an open book: the spine is searched on the paper the corners are found on,
-    and the spread's two pages are each flattened as a FlatPage with its half of the quad given."""
+    and the spread's two pages are each flattened as a FlatPage with its half of the quad given.  ``turn`` (DESIGN.md 7b, "Page
+    turns"; rect and quad frames): a TextPage's.  A given turn is exactly FlatPage(quad=turn_quad(rect or quad, turn)) with
+    the page's other fields; "auto" votes on the page's frame (the crop, R, or the evened frame) and flattens the page as
+    with the turn found given.  Not with skew, curve or spread."""
     rect: object = None
     quad: object = None
     skew: object = None
@@ -2717,6 +2832,7 @@ class FlatPage(NamedTuple):
     light: object = None
     light_window: object = None
     spread: object = None
+    turn: object = None
 
 
 FLAT_MAX_WORK = 1 << 31     # bytes of device memory the flat pages of one flatten_pages call may use
@@ -2745,6 +2861,18 @@ def _check_flat(fp, H, W, name):
     for quad="auto"), validated under _check_page's, _check_quad's and _check_curve's rules, curve with quad allowed.  Raises
     ValueError naming ``name``."""
     from . import ops
+    if fp.turn is not None:
+        if not (isinstance(fp.turn, str) and fp.turn == "auto") and (isinstance(fp.turn, bool) or not isinstance(fp.turn, int)
+                                                                     or fp.turn not in TURNS):
+            raise ValueError(f"{name}: turn must be None, 0, 90, 180, 270 or 'auto', got {fp.turn!r}")
+        for what in ("skew", "curve", "spread"):
+            if getattr(fp, what) is not None:
+                raise ValueError(f"{name}: turn and {what} are both given (a turned page is a rect or quad frame: flatten a "
+                                 f"tilted, curled or spread page first, then turn it)")
+        rect = _check_flat(fp._replace(turn=None), H, W, name)
+        if isinstance(fp.turn, int) and not isinstance(fp.quad, str):
+            return _check_flat(_turned(fp, rect, (H, W))[0], H, W, name)
+        return rect
     if fp.spread is not None:
         if not (isinstance(fp.spread, str) and fp.spread == "auto"):
             raise ValueError(f"{name}: spread must be None or 'auto', got {fp.spread!r}")
@@ -2798,6 +2926,8 @@ def _flat_bytes(fp, size, crop):
     if fp.light is not None:
         frame = crop if fp.skew is not None else size
         n += ops.even_light_bytes(*max(size, frame, key=lambda s: s[0] * s[1]), frame)
+    if isinstance(fp.turn, str):                        # the turned flat page of a second pass
+        n += 3 * w * h
     return n
 
 
@@ -2813,8 +2943,8 @@ def _check_flat_work(items, names):
             raise ValueError(f"{name}: the call's flat pages up to this one need {total} bytes of work memory, over the "
                              f"{FLAT_MAX_WORK} a call may use (split the call)")
     from . import ops
-    searched = [(i, _flat_text_page(fp), rect) for i, fp, rect in items
-                if fp.curve is not None or isinstance(fp.skew, str) or isinstance(fp.quad, str)]
+    searched = [(i, _flat_text_page(fp, turn=fp.turn if isinstance(fp.turn, str) else None), rect) for i, fp, rect in items
+                if fp.curve is not None or isinstance(fp.skew, str) or isinstance(fp.quad, str) or isinstance(fp.turn, str)]
     if searched:
         _check_page_work(searched, sum(ops.spine_page_bytes(rect[2] - rect[0]) for _, fp, rect in items if fp.spread is not None))
 
@@ -2911,7 +3041,11 @@ def flatten_pages(images, pages, to_host=False):
     ops.even_light call (six launches), and its searches after the corners' read the evened frame; a skewed or curled light
     page is evened again after its warp or remap (four more launches for all of them).  Its dict gains ``light_window`` (the
     k used) and ``ink`` ("dark" or "light").  The ink comes back with the call's first synchronisation after the evening; a
-    call with no search and no ``to_host`` waits once for it, and only when an ink is "auto"."""
+    call with no search and no ``to_host`` waits once for it, and only when an ink is "auto".
+    A page with a given ``turn`` (DESIGN.md 7b, "Page turns") is exactly FlatPage(quad=turn_quad(rect or quad, turn)), its
+    dict kind "quad" plus ``turn``.  With ``turn="auto"`` the call is first flattened without those turns, the turns are
+    voted on the flat frames in one layout call, and the pages found turned are flattened again with their turn (and found
+    quad) given; the dict is that of the found turn given, plus ``turn_votes``."""
     from . import ops
     imgs = [_as_image(im, i) for i, im in enumerate(images)]
     pages = _per_image(pages, len(imgs), "pages (one list per image)")
@@ -2926,6 +3060,13 @@ def flatten_pages(images, pages, to_host=False):
     out = [[] for _ in imgs]
     if not items:
         return out
+    if any(isinstance(fp.turn, str) for _, fp, _ in items):
+        return _flatten_turned(imgs, pages, to_host)
+    turned = {k: fp.turn for k, (_, fp, _) in enumerate(items) if fp.turn is not None}
+    for k in turned:                    # a given turn is its turned quad page (a found quad's once it is found)
+        i, fp, rect = items[k]
+        if not isinstance(fp.quad, str):
+            items[k] = (i,) + _turned(fp, rect, imgs[i].shape[:2])
     dev = next((im.device for im in imgs if im.is_cuda), torch.device("cuda", torch.cuda.current_device()))
     with torch.cuda.device(dev):
         dimg = _device_images(sorted({i for i, _, _ in items}), imgs, dev)
@@ -2949,6 +3090,9 @@ def flatten_pages(images, pages, to_host=False):
                 continue
             if isinstance(fp.quad, str):
                 fp = fp._replace(quad=f[1].quad)
+                if fp.turn is not None:
+                    f = (i,) + _turned(fp, f[2], dimg[i].shape[:2])
+                    fp = f[1]
                 size = _flat_frame(fp, f[2])
                 if max(size) > 32767:
                     raise ValueError(f"{name}: a side of the page's flat frame reaches {max(size)} pixels, over 32767")
@@ -3066,8 +3210,42 @@ def flatten_pages(images, pages, to_host=False):
             for j, k in enumerate(light):
                 pol = items[k][1].polarity
                 res[k]["ink"] = pol if pol != "auto" else "dark" if int(ink_host[j, 2]) == ops._lib.INK_DARK else "light"
-    for (i, _, _), g in zip(given, groups):
+    for k, ((i, _, _), g) in enumerate(zip(given, groups)):
         out[i].append(res[g] if isinstance(g, int) else dict(g[0], pages=[dict(res[k], side=side) for k, side in g[1]]))
+        if k in turned:
+            out[i][-1]["turn"] = turned[k]
+    return out
+
+
+def _flatten_turned(imgs, pages, to_host):
+    """flatten_pages of a call with turn="auto" pages (DESIGN.md 7b, "Page turns"): the call without their turns, whose flat
+    pages are their frames; one _find_blocks vote on those frames; then the pages found turned flattened again with their turn
+    (and a found quad) given.  Each turn page's dict is that of its turn given, plus turn_votes."""
+    first = flatten_pages(imgs, [[fp._replace(turn=None) if isinstance(fp.turn, str) else fp for fp in pg or []]
+                                 for pg in pages])
+    auto = [(i, r) for i, pg in enumerate(pages) for r, fp in enumerate(pg or []) if isinstance(fp.turn, str)]
+    src = {(i, r): first[i][r]["image"] for i, r in auto}
+    vote = [((i, r), TextPage(None, pages[i][r].direction, pages[i][r].polarity, pages[i][r].gap_x, pages[i][r].gap_y,
+                              turn="auto"), (0, 0, src[(i, r)].shape[1], src[(i, r)].shape[0])) for i, r in auto]
+    with torch.cuda.device(src[auto[0]].device):
+        found = _find_blocks(src, vote)
+    turns, again, where = {}, [[] for _ in imgs], {}
+    for (i, r), v in zip(auto, found):
+        if isinstance(v, str):
+            raise ValueError(f"image {i}, page {r}: {v}")
+        turns[(i, r)] = page_turn(v["turn_votes"]), v["turn_votes"]
+        fp = pages[i][r]
+        if turns[(i, r)][0]:
+            where[(i, r)] = len(again[i])
+            quad = QuadRegion(*first[i][r]["quad"]) if isinstance(fp.quad, str) else fp.quad
+            again[i].append(fp._replace(quad=quad, turn=turns[(i, r)][0]))
+    second = flatten_pages(imgs, again) if where else None
+    out = [[dict(second[i][where[(i, r)]] if (i, r) in where else dict(d, turn=0), turn_votes=turns[(i, r)][1])
+            if (i, r) in turns else d for r, d in enumerate(row)] for i, row in enumerate(first)]
+    if to_host:
+        flat = [p for row in out for d in row for p in d.get("pages", [d])]
+        for d, v in zip(flat, _to_host_all([d["image"] for d in flat])):
+            d["image"] = v
     return out
 
 
